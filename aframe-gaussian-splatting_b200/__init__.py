@@ -1,4 +1,4 @@
-"""aframe-gaussian-splatting_b200 — B200-native sort + splat-raster path behind the reference component's API.
+"""aframe-gaussian-splatting_b200 — H100-native sort + splat-raster path behind the reference component's API.
 
 The directory name carries a hyphen, so import it with
     import importlib; gs = importlib.import_module("aframe-gaussian-splatting_b200")

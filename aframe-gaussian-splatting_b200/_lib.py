@@ -87,7 +87,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with __graft_entry__.build() "
-            "(nvcc, sm_100a).  There is no CPU fallback for the splat path.")
+            "(nvcc, sm_90a).  There is no CPU fallback for the splat path.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():
         fn = getattr(lib, name)  # AttributeError if the header and the library disagree

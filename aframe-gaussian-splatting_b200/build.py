@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA library (nvcc, sm_100a only).  `python -m` is not usable with the hyphenated
+"""In-tree build of the CUDA library (nvcc, sm_90a only).  `python -m` is not usable with the hyphenated
 package name; call build_library() or run this file directly."""
 from __future__ import annotations
 
@@ -13,7 +13,7 @@ SOURCES = ["gs_api.cu", "gs_sort.cu", "gs_slab.cu", "gs_pack.cu", "gs_project.cu
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "--fmad=false",  # no implicit FMA contraction: parity needs the written op order (DESIGN.md)
     "-Xcompiler", "-fPIC,-fvisibility=hidden",

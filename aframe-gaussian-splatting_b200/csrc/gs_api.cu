@@ -193,7 +193,7 @@ static void drop_graphs(gs_context *c) {
 // ---------------------------------------------------------------------------------------------
 extern "C" uint32_t gs_bin_size(void) { return (uint32_t)kBin; }
 
-extern "C" const char *gs_version(void) { return "gsplat_b200 0.1 (sm_100a; restates aframe-gaussian-splatting index.js @ b50238f)"; }
+extern "C" const char *gs_version(void) { return "gsplat_b200 0.1 (sm_90a; restates aframe-gaussian-splatting index.js @ b50238f)"; }
 
 extern "C" const char *gs_last_error(const gs_context *ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
@@ -215,8 +215,8 @@ extern "C" int gs_create(int device_ordinal, gs_context **out_ctx) {
     g_create_error = std::string("cudaGetDeviceProperties: ") + cudaGetErrorString(e);
     return GS_ERR_CUDA;
   }
-  if (prop.major != 10) {
-    g_create_error = "device is not sm_100 (Blackwell B200); kernels are built for sm_100a only";
+  if (prop.major != 9 || prop.minor != 0) {
+    g_create_error = "device is not sm_90 (Hopper H100); kernels are built for sm_90a only";
     return GS_ERR_CUDA;
   }
   gs_context *c = new (std::nothrow) gs_context();
@@ -276,7 +276,7 @@ extern "C" int gs_create(int device_ordinal, gs_context **out_ctx) {
   if (const char *e = getenv("GS_EMIT")) c->emit_by_entry = strcmp(e, "windows") != 0;
   if (const char *e = getenv("GS_SLAB_MIN")) c->slab_min = (uint32_t)strtoull(e, nullptr, 10);
   if (const char *e = getenv("GS_SLAB_FIRST")) c->slab_first = std::max<uint32_t>(1024u, (uint32_t)strtoull(e, nullptr, 10));
-  {  // pixel loop of the raster: packed fp32x2 (default) or scalar (GS_RASTER=scalar); both give identical frames
+  {  // pixel loop of the raster: two pixels per lane (default) or one (GS_RASTER=scalar); both give identical frames
     const char *rk = getenv("GS_RASTER");
     c->raster_base_flags = (rk && strcmp(rk, "scalar") == 0) ? 0u : 1u;
   }
@@ -675,8 +675,8 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
   return GS_OK;
 }
 
-// entries covered by the first k slabs: slab_first * (1 + 2 + 4 + ...) - each slab is twice the previous one (4x growth
-// was measured slower at 80 M splats: the few bins that stay open then force much larger slabs through sort + projection)
+// entries covered by the first k slabs: slab_first * (1 + 2 + 4 + ...) - each slab is twice the previous one (with faster
+// growth the few bins that stay open force much larger slabs through sort + projection)
 static uint64_t slab_cumulative(uint32_t first, int k) { return (uint64_t)first * ((1ull << k) - 1ull); }
 
 // Stage A of a slab frame (sort stream): depth + cull, keys + bucket histogram, slab plan, pixel-state reset.
@@ -856,7 +856,7 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
     fp.out = sl.out_user;
     sl.frame_src = nullptr;
   }
-  // raster instantiation: pixel loop (packed fp32x2 by default), depth test, statistics
+  // raster instantiation: pixel loop (two pixels per lane by default), depth test, statistics
   sl.raster_flags = c->raster_base_flags | (p->depth_in ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u);
   if (p->depth_in) {
     if (p->flags & GS_RENDER_DEPTH_DEVICE) {

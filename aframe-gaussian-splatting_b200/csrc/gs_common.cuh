@@ -1,4 +1,4 @@
-// gs_common.cuh — shared declarations of the B200 splat path (context, device counters, launch API).
+// gs_common.cuh — shared declarations of the H100 splat path (context, device counters, launch API).
 //
 // The whole library is compiled with --fmad=false: no implicit FMA contraction, so fp32/fp64
 // expressions execute in the order written (the reference's JS fp64 and GLSL fp32 semantics are
@@ -21,9 +21,8 @@ constexpr int kTile = 16;                 // 16x16 screen tiles (north_star): on
 // Binning granularity: splats are binned to square BINS of GS_BIN_TILES x GS_BIN_TILES tiles (96x96 pixels by default),
 // not to tiles.  A splat meets ~5x fewer bins than tiles, so the instance emission and the stable sort by bin id handle
 // ~5x fewer elements; each tile's raster CTA streams its bin's list and culls it against its own 16x16 pixels on the fly
-// (exact footprint test, one record per thread).  Measured at config 2 (1 M splats, 1080p): 64 px 3323, 96 px 3601,
-// 128 px 3626 frames/s, raster time unchanged; a 1920x1080 frame has 240 bins of 96 px, so the bin id is one byte and one
-// radix pass sorts the instances.  96 px keeps more bin columns for multi-GPU ownership and closes bins earlier (slab path).
+// (exact footprint test, one record per thread).  A 1920x1080 frame has 240 bins of 96 px, so the bin id is one byte and
+// one radix pass sorts the instances.  96 px keeps more bin columns for multi-GPU ownership and closes bins earlier (slab path).
 #ifndef GS_BIN_TILES
 #define GS_BIN_TILES 6
 #endif
@@ -134,7 +133,7 @@ struct SlabTable {
 
 struct gs_context {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;
   std::string err;
 
@@ -194,7 +193,7 @@ struct gs_context {
   bool have_last_sorted = false;
   uint32_t slab_first = 1u << 20;  // target entry count of the nearest slab (the following ones double)
   int last_mode = 0;               // 0 = one pass (three-stage pipeline), 1 = slab path
-  bool emit_by_entry = true;       // k_emit_entries + k_radix_hist<T1> (default; measured faster on every config) or, with
+  bool emit_by_entry = true;       // k_emit_entries + k_radix_hist<T1> (default) or, with
                                    // GS_EMIT=windows, the window-balanced k_emit of round 1 (one-pass path only)
   uint4 *tile_stats = nullptr;     // [tiles] per-tile counts of a GS_RENDER_STATS frame
   uint4 *tile_stats_host = nullptr;  // pinned copy
@@ -207,7 +206,7 @@ struct gs_context {
   // the host.  Three stages + the copy = four frames a caller can have outstanding; the GPU-side order of the stages is
   // kept by the buffer-set events below, a slot only holds a frame's parameters, counters, events and output staging.
   // (With three slots a caller that receives frames in host memory had to collect frame k-1's copy before it could
-  // submit frame k+2, and the sort stage idled for the length of the copy: 3 200 instead of 3 800 frames/s.) ----
+  // submit frame k+2, and the sort stage idled for the length of the copy.) ----
   static constexpr int kSlots = 4;
   struct Slot {
     gs::FrameCounters *ctr = nullptr;        // device
@@ -272,7 +271,7 @@ struct gs_context {
   cudaEvent_t ev_fork[2]{}, ev_join[2]{};
   bool use_graphs = true;
   bool use_pdl = false;                          // programmatic dependent launch inside the stage chains (GS_PDL=1 turns it on)
-  uint32_t raster_base_flags = 1;                // default pixel loop: 1 = packed fp32x2, 0 = scalar
+  uint32_t raster_base_flags = 1;                // default pixel loop: 1 = two pixels per lane, 0 = one
   // graph cache key: anything baked into the captured launches
   struct GraphKey { uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr; } gkey;
 
@@ -340,9 +339,9 @@ void launch_assemble(gs_context *c, const void *gathered, uint32_t tiles_per_ran
 // ---- programmatic dependent launch (PDL): the kernels of a stage form a chain of short dependent launches.  Launched
 // with the programmatic-stream-serialization attribute, kernel k+1 is set up (CTAs scheduled, arguments loaded) while
 // kernel k drains; it blocks in pdl_wait() until k has completed and its writes are visible.  Every kernel launched
-// this way calls pdl_trigger() + pdl_wait() before its first global access.  OFF by default (GS_PDL=1 enables): measured at
-// config 2 the isolated sort stage gains 8 % (0.094 -> 0.086 ms) but the pipelined frame rate drops 12 % (3784 -> 3335):
-// early-launched CTAs sit on SM resources while they wait, and those are the resources the co-running raster needs. ----
+// this way calls pdl_trigger() + pdl_wait() before its first global access.  OFF by default (GS_PDL=1 enables): it shortens
+// an isolated stage, but in the pipeline early-launched CTAs sit on SM resources while they wait, and those are the
+// resources the co-running raster needs. ----
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 #define GS_PDL_ENTRY() do { gs::pdl_trigger(); gs::pdl_wait(); } while (0)

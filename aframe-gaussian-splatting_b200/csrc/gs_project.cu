@@ -145,7 +145,7 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
 // (the slab's instances then carry j, not the splat index), and only the slab's splats are projected.
 // Index order, sparse frames (fewer than half of the resident splats passed the worker filter, e.g. a cutout box): the
 // survivors of every 1024-splat chunk are first compacted into shared memory, so the shader runs in full warps
-// instead of warps with a few live lanes each (20 M splats, 22 % kept: 0.41 ms -> see DESIGN.md 4).
+// instead of warps with a few live lanes each.
 template <bool BY_ENTRY>
 __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, const uint4 *__restrict__ cc,
                                                  const float *__restrict__ depth,

@@ -20,10 +20,10 @@
 //
 // Two pixel loops produce bit-identical frames:
 //   k_raster  <.., false>: 256 threads, one pixel per lane, scalar fp32;
-//   k_raster  <.., true> : 128 threads, two vertically adjacent pixels per lane, packed fp32x2 arithmetic
-//                          (FADD2 / FMUL2 / FFMA2: one issue slot per two lane-operations; the kernel is bound by
-//                          issue slots, not by the fp32 pipe itself).  The per-splat operands stay scalars in shared
-//                          memory: the packed instructions broadcast a scalar register operand (`Rn.F32`) themselves.
+//   k_raster  <.., true> : 128 threads, two vertically adjacent pixels per lane: the pair shares the shared-memory
+//                          loads of a record, dx and the two products with dx, and the loop overhead (the kernel is
+//                          bound by issue slots).  Hopper has no packed fp32x2 instructions, so the pair's arithmetic
+//                          is two scalar ops of the same rounding (add2 / mul2 / fma2 below).
 #include "gs_common.cuh"
 
 namespace gs {
@@ -60,6 +60,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
+}
+
+// one scalar op per pixel of a lane's pair, rounded to nearest like the one-pixel loop
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 __device__ __forceinline__ uint32_t to_u8(float v) {
@@ -292,26 +299,26 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
           // vPosition = (px, py) with the op order of the oracle (orc band_worker): d = sample - centre,
           // px = fma(dy, a2y, dx*a2x), py = fma(dy, a1y, dx*a1x), r2 = fma(py, py, px*px)
           const float dx = __fadd_rn(fx, q0.x);
-          const float2 dy2 = __fadd2_rn(fy2, make_float2(q1.x, q1.x));
+          const float2 dy2 = add2(fy2, make_float2(q1.x, q1.x));
           const float t = __fmul_rn(dx, q0.y), u = __fmul_rn(dx, q0.z);
-          const float2 px2 = __ffma2_rn(dy2, make_float2(q1.y, q1.y), make_float2(t, t));
-          const float2 py2 = __ffma2_rn(dy2, make_float2(q1.z, q1.z), make_float2(u, u));
-          const float2 r22 = __ffma2_rn(py2, py2, __fmul2_rn(px2, px2));
+          const float2 px2 = fma2(dy2, make_float2(q1.y, q1.y), make_float2(t, t));
+          const float2 py2 = fma2(dy2, make_float2(q1.z, q1.z), make_float2(u, u));
+          const float2 r22 = fma2(py2, py2, mul2(px2, px2));
           bool h0 = r22.x <= lim0, h1 = r22.y <= lim1;  // index.js:171-172: A = -r2; discard if A < -4
           if (DEPTH) { h0 = h0 && (q0.w <= d0); h1 = h1 && (q0.w <= d1); }
           if (STATS) { st_tests += (lim0 > 0.f ? 1u : 0u) + (lim1 > 0.f ? 1u : 0u); st_hits += (h0 ? 1u : 0u) + (h1 ? 1u : 0u); }
           if (h0 || h1) {
-            const float2 m2 = __fmul2_rn(r22, make_float2(kNegLog2e, kNegLog2e));
+            const float2 m2 = mul2(r22, make_float2(kNegLog2e, kNegLog2e));
             const float2 e2 = make_float2(ex2_approx(m2.x), ex2_approx(m2.y));
-            const float2 al2 = __fmul2_rn(e2, make_float2(q1.w, q1.w));  // index.js:173
-            float2 w2 = __fmul2_rn(al2, T2);
+            const float2 al2 = mul2(e2, make_float2(q1.w, q1.w));  // index.js:173
+            float2 w2 = mul2(al2, T2);
             w2.x = h0 ? w2.x : 0.0f;
             w2.y = h1 ? w2.y : 0.0f;
             const float4 q2 = s_cv[j * kCv + 2];
-            R2 = __ffma2_rn(make_float2(q2.x, q2.x), w2, R2);
-            G2 = __ffma2_rn(make_float2(q2.y, q2.y), w2, G2);
-            B2 = __ffma2_rn(make_float2(q2.z, q2.z), w2, B2);
-            T2 = __ffma2_rn(w2, make_float2(-1.0f, -1.0f), T2);  // T - w, one rounding
+            R2 = fma2(make_float2(q2.x, q2.x), w2, R2);
+            G2 = fma2(make_float2(q2.y, q2.y), w2, G2);
+            B2 = fma2(make_float2(q2.z, q2.z), w2, B2);
+            T2 = fma2(w2, make_float2(-1.0f, -1.0f), T2);  // T - w, one rounding
             lim0 = (T2.x >= kTStop) ? lim0 : -1.0f;
             lim1 = (T2.y >= kTStop) ? lim1 : -1.0f;
           }

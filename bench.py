@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — frames/sec of the splat hot path (sort + project + bin + raster) on B200.
+"""bench.py — frames/sec of the splat hot path (sort + project + bin + raster) on H100.
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA, through the C ABI)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle restatement)
@@ -18,6 +18,11 @@ frame by screen bin columns over the ranks and exchanges the finished tiles (str
            host memory, both copies inside the timed region.
 `parity` : the timed configuration's GPU frame against the CPU oracle's frame of the same inputs (max abs error on
            float RGBA, LSB histogram on RGBA8, exactness of the sort) — the run exits non-zero above 1e-3.
+
+`--dump-outputs DIR` writes the RGBA8 frame the last timed step of the headline configuration produced, as float32
+`DIR/frame.npy` (h, w, 4); the inputs are seeded, so two builds can be compared output for output.  A frame larger than
+64 MB is replaced by a fixed seeded sample of its pixels (`frame_sample.npy`, (k, 4)) and their row-major pixel indices
+(`frame_sample_index.npy`, float64).
 """
 from __future__ import annotations
 
@@ -46,6 +51,7 @@ METRICS = {
 }
 FRAME_TOL = 1e-3
 DTYPE = "f64 sort keys + f32 shading"
+DUMP_BYTES = 64_000_000  # all files of --dump-outputs together
 
 
 def load_peaks():
@@ -55,7 +61,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def algorithmic_bytes(st: dict) -> dict:
@@ -81,6 +87,20 @@ def algorithmic_bytes(st: dict) -> dict:
         "raster": 36 * D + 4 * P,             # K5: sorted values + 32 B record per instance + RGBA8 frame
         "total": 20 * N + 32 * V + 32 * V2 + 116 * D + 8 * T + 4 * P,
     }
+
+
+def dump_frame(d: str, frame: np.ndarray) -> None:
+    """frame (h, w, 4) -> DIR/frame.npy as float32, or a fixed seeded pixel sample when it exceeds DUMP_BYTES."""
+    os.makedirs(d, exist_ok=True)
+    f = frame.astype(np.float32)
+    if f.nbytes <= DUMP_BYTES:
+        np.save(os.path.join(d, "frame.npy"), f)
+        return
+    px = f.reshape(-1, f.shape[-1])
+    k = (DUMP_BYTES - 1024) // (px.shape[1] * 4 + 8)  # sampled pixels + their float64 indices (+ two .npy headers)
+    idx = np.sort(np.random.default_rng(0).choice(px.shape[0], k, replace=False))
+    np.save(os.path.join(d, "frame_sample.npy"), px[idx])
+    np.save(os.path.join(d, "frame_sample_index.npy"), idx.astype(np.float64))
 
 
 def parallel_mode(args) -> str:
@@ -111,7 +131,7 @@ def config_block(args, workload: str, n: int, w: int, h: int, orbit: bool) -> di
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,utilization.gpu,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -318,7 +338,7 @@ def run_ours(args):
     ctx = gs.SplatContext(local)
     stream = torch.cuda.ExternalStream(ctx._lib.gs_stream(ctx._h), device=dev)
     with torch.cuda.stream(stream):
-        flush = torch.empty(160 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+        flush = torch.empty(160 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
     stream.synchronize()
     os.environ.setdefault("GS_BENCH", "1")
     uuid = str(torch.cuda.get_device_properties(dev).uuid)
@@ -404,6 +424,16 @@ def run_ours(args):
             ctx.assemble_tiles(gath_bufs[i % 3].data_ptr(), tiles_per_rank, world, w, h, gs.GS_FORMAT_RGBA8, frames_dev[i % 3].data_ptr())
             return t
 
+        last_ticket = [None]
+
+        def last_frame(i):
+            """the RGBA8 frame submit_device(i) produced (i = the last step submitted, so its buffer is not reused yet)"""
+            if use_peer:
+                out = np.empty((h, w, 4), np.uint8)
+                ctx.memcpy_d2h(out, ctx.peer_frame(last_ticket[0]), out.nbytes)
+                return out
+            return frames_dev[i % (3 if sharded else 4)].cpu().numpy().reshape(h, w, 4)
+
         def run_pipeline(submit, k, collect=None, depth=3):
             """k frames, at most `depth` outstanding (3: sort(i) | bin(i-1) | raster(i-2); 4 when frames also cross PCIe:
             + copy(i-3)); one CUDA-event pair on the library's stream brackets everything (the L2 flushes between steps
@@ -416,6 +446,7 @@ def run_ours(args):
                 with torch.cuda.stream(stream):
                     flush.zero_()  # L2 flush between timed iterations
                 tickets.append(submit(i))
+                last_ticket[0] = tickets[-1]
                 if i >= depth - 1:
                     st = ctx.wait(tickets[i - (depth - 1)])
                     if collect is not None:
@@ -442,6 +473,8 @@ def run_ours(args):
         # ---- value: device-resident frames ----
         barrier()
         my_ms = run_pipeline(submit_device, steps, depth=3 if sharded else args.value_depth)
+        if headline and args.dump_outputs and rank == 0:
+            dump_frame(args.dump_outputs, last_frame(steps - 1))
         total_ms = allmax(my_ms)
         barrier()
         if world > 1:
@@ -540,15 +573,6 @@ def run_ours(args):
                 ms = stage_ms[nm]
                 ach = ab[nm] / (ms * 1e-3) / 1e9 if ms > 0 else 0.0
                 return {"bytes": ab[nm], "ms": ms, "achieved_gbs": ach, "frac": ach / peak}
-            # DRAM traffic is a MEASUREMENT of one profiled launch (ncu --set full): quoted only for the exact configuration
-            # profiles/traffic.json was captured on (N = 1, config 2), null everywhere else
-            traffic = None
-            tp = os.path.join(ROOT, "profiles", "traffic.json")
-            if world == 1 and name == "train_1m_1080p" and not args.splats and os.path.exists(tp):
-                try:
-                    traffic = json.load(open(tp)).get(dom)
-                except Exception:
-                    traffic = None
             r = roof(dom)
             slab_info = None
             if st["n_slabs"]:
@@ -572,7 +596,7 @@ def run_ours(args):
                 "gpu_launches": (int(st["kernel_launches"]) + (2 if use_peer else (1 if sharded else 0))) * steps * units,
                 "clocks": clocks,
                 "roofline": {"kernel": kernels[dom], "bound": "hbm", "achieved": r["achieved_gbs"], "peak": peak, "unit": "GB/s", "frac": r["frac"],
-                             "traffic": traffic, "peak_source": peak_src,
+                             "peak_source": peak_src,
                              "algorithmic_bytes_per_launch": ab[dom], "ms_per_launch": stage_ms[dom],
                              "note": "k_raster is FP32-pipe bound (one exp + ~16 fp32 ops per covered pixel-splat pair), reported against HBM as SURVEY.md 8d prescribes"},
                 "stages": {k: roof(k) for k in stage_ms},
@@ -601,7 +625,7 @@ def run_ours(args):
     alt = None
     if world > 1 and parallel_mode(args) == "tiles" and args.parallel == "auto":
         # the tile-sharded frame replicates the O(N) passes of the path on every rank; the same job dealt out as whole
-        # frames (every rank holds the scene: 2.9 GB of 180 GB at 80 M splats) is printed beside it
+        # frames (every rank holds the scene: 2.9 GB of 80 GB at 80 M splats) is printed beside it
         try:
             a = measure(args.workload, max(5, min(args.steps, 10)), False, mode="frames")
             if a is not None:
@@ -661,6 +685,8 @@ def main():
     ap.add_argument("--parallel", default="auto", choices=["auto", "frames", "tiles"],
                     help="N > 1: `frames` = every rank renders every N-th frame from its own replica (weak scaling, default); "
                          "`tiles` = one frame sharded by screen bin columns + tile exchange (strong scaling, default for the 80 M scene)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's frame as DIR/frame.npy (float32)")
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "nccl"],
                     help="multi-GPU frame exchange: fused raster + NVLink peer stores (default) or NCCL all-gather of tiles")
     args = ap.parse_args()

@@ -1,5 +1,5 @@
 /*
- * gsplat_b200.h — C ABI of the B200-native Gaussian-splat sort + raster path.
+ * gsplat_b200.h — C ABI of the H100-native Gaussian-splat sort + raster path.
  *
  * Drop-in boundary for the two hot loops of quadjr/aframe-gaussian-splatting `index.js`
  * (v0.0.22 @ b50238f).  Every entry point names the reference interface it replaces
@@ -17,7 +17,7 @@
  *   - every function returns 0 on success or a negative gs_status; no exception crosses the ABI.
  *   - a context is single-owner (not thread-safe), one context per GPU (index.js runs one
  *     worker + one GL context per component).
- *   - there is NO CPU fallback: gs_create fails with GS_ERR_CUDA when no sm_100 device exists.
+ *   - there is NO CPU fallback: gs_create fails with GS_ERR_CUDA when no sm_90 device exists.
  */
 #ifndef GSPLAT_B200_H
 #define GSPLAT_B200_H

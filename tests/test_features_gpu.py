@@ -1,5 +1,5 @@
 """GPU tests of the draw's optional features through the C ABI: depth interop (index.js:179-180), the two pixel loops
-of the raster (packed fp32x2 / scalar) producing identical frames, and the GS_RENDER_STATS counters."""
+of the raster (two pixels / one pixel per lane) producing identical frames, and the GS_RENDER_STATS counters."""
 import os
 
 import numpy as np
@@ -58,7 +58,7 @@ def test_depth_interop_parity(gs, orc, ctx, n, w, h):
 
 
 def test_packed_and_scalar_pixel_loops_agree(gs, orc):
-    """GS_RASTER=scalar selects the one-pixel-per-lane loop; the default is the packed fp32x2 loop.  Same operations in
+    """GS_RASTER=scalar selects the one-pixel-per-lane loop; the default is the two-pixels-per-lane loop.  Same operations in
     the same order per pixel -> bit-identical frames (float and RGBA8, with and without a depth buffer)."""
     rows, cs, cc, m, fr = scene_inputs(gs, orc, 150000, 4321, 1000, 562)
     order = orc.sort(m, fr.view)

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): every call goes through the C ABI (ctypes ->
+"""GPU parity tests (run with -m gpu on an H100): every call goes through the C ABI (ctypes ->
 libgsplat_b200.so) and is compared with the CPU oracle on the same seeded inputs.
 
 Tolerances (BASELINE.md "Parity gate"):
