@@ -11,7 +11,8 @@ LIB_PATH = os.path.join(HERE, "libgsplat_b200.so")
 GS_OK, GS_ERR_INVALID, GS_ERR_CUDA, GS_ERR_OOM, GS_ERR_CAPACITY, GS_ERR_EMPTY = 0, -1, -2, -3, -4, -5
 GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F = 0, 1
 GS_RENDER_OUT_DEVICE, GS_RENDER_REUSE_SORT, GS_RENDER_OUT_TILED, GS_RENDER_OUT_PEER = 1, 2, 4, 8
-GS_RENDER_STATS, GS_RENDER_DEPTH_DEVICE = 16, 32
+GS_RENDER_STATS, GS_RENDER_DEPTH_DEVICE, GS_RENDER_COLOR_DEVICE = 16, 32, 64
+GS_MAX_OBJECTS = 64
 
 
 class GsStats(C.Structure):
@@ -39,6 +40,14 @@ class GsRenderParams(C.Structure):
     ]
 
 
+class GsObject(C.Structure):
+    """gs_object: one entity of a scene frame."""
+    _fields_ = [
+        ("first", C.c_uint32), ("count", C.c_uint32), ("modelview", C.c_float * 16),
+        ("has_cutout", C.c_int32), ("cutout16", C.c_float * 16),
+    ]
+
+
 # every symbol include/gsplat_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -59,6 +68,10 @@ SYMBOLS = {
     "gs_wait": (C.c_int, [_P, C.c_uint64, C.POINTER(GsStats)]),
     "gs_render_stereo": (C.c_int, [_P, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(GsRenderParams), C.POINTER(_P),
                                    C.POINTER(GsStats)]),
+    "gs_render_scene_async": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.c_uint32, _P, _P,
+                                        C.POINTER(C.c_uint64)]),
+    "gs_render_scene": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.c_uint32, _P, _P, C.POINTER(GsStats)]),
+    "gs_sort_scene": (C.c_int, [_P, C.POINTER(GsObject), C.c_uint32, _P, C.POINTER(C.c_uint32)]),
     "gs_read_projected": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
     "gs_get_stats": (C.c_int, [_P, C.POINTER(GsStats)]),
     "gs_set_shard": (C.c_int, [_P, C.c_uint32, C.c_uint32]),

@@ -20,7 +20,7 @@ from typing import Callable, Optional
 import numpy as np
 
 from . import ply as _ply
-from .renderer import SplatContext
+from .renderer import SceneObject, SplatContext
 from .scenes import FrameInputs
 from .three_math import (Matrix4, Object3D, PerspectiveCamera, focal_length, get_model_view_matrix,
                          get_projection_matrix, world_to_cutout)
@@ -88,6 +88,7 @@ class GaussianSplattingComponent:
         self.instanceCount = 0
         self.pixelRatio = 1.0
         self._have_order = False
+        self.scene: Optional["SplatScene"] = None  # set by SplatScene.add: the entity shares that scene's context
 
     # ---- index.js:8-23 ----
     def init(self, camera: PerspectiveCamera, object3d: Object3D, renderer: Optional[SplatContext] = None):
@@ -104,14 +105,15 @@ class GaussianSplattingComponent:
         index.js:248-251); here the resident table is reserved for as many splats, so the pushes that follow never
         have to grow it (and never wait for frames in flight).  sortReady flips exactly as at index.js:220."""
         if numVertexes > 0 and self.renderer is not None:
-            self.renderer.reserve(int(numVertexes))
+            base = self.renderer.num_splats if self.scene is not None else 0  # a scene appends behind the other entities
+            self.renderer.reserve(base + int(numVertexes))
         self.sortReady = True
 
     # ---- index.js:222-327 ----
     def loadData(self, camera, object3d, renderer: SplatContext, src) -> None:
         self.camera, self.object, self.renderer = camera, object3d, renderer
         self.loadedVertexCount = 0
-        self.worker = SortWorker(renderer)
+        self.worker = SortWorker(renderer) if self.scene is None else _EntityWorker(self.scene, self)
         self.worker.onmessage = self._on_sorted
         self.worker.postMessage({"method": "clear"})
         if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)):
@@ -203,14 +205,134 @@ class GaussianSplattingComponent:
         return frames
 
     def render(self, width: int, height: int, camera=None, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
-               out: Optional[np.ndarray] = None, synchronous: bool = True) -> np.ndarray:
+               out: Optional[np.ndarray] = None, synchronous: bool = True, color_in: Optional[np.ndarray] = None) -> np.ndarray:
         """Draw the mesh into an RGBA frame (row 0 = bottom).  synchronous=True sorts with this frame's camera
         (the oracle's definition); synchronous=False draws with the order of the last tick(), which is what the
-        reference does while a sort is in flight (index.js:206,439-440)."""
+        reference does while a sort is in flight (index.js:206,439-440).
+        color_in: the colour buffer the mesh is blended into ((H, W, 4) of the output dtype, row 0 = bottom), i.e. the
+        rest of the scene drawn before it (index.js:177-181); None = the clear colour bg.  Such a frame, and any frame
+        of an entity that shares a SplatScene, sorts with this frame's camera."""
         fr = self.frame_inputs(width, height, camera)
-        reuse = (not synchronous) and self._have_order
-        return self.renderer.render(fr, bg=bg, fmt=fmt, out=out, reuse_sort=reuse)
+        if color_in is None and self.scene is None:
+            reuse = (not synchronous) and self._have_order
+            return self.renderer.render(fr, bg=bg, fmt=fmt, out=out, reuse_sort=reuse)
+        first, count = self.scene.range_of(self) if self.scene is not None else (0, self.renderer.num_splats)
+        obj = SceneObject(first, count, fr.modelview, fr.cutout)
+        return self.renderer.render_scene(fr, [obj], bg=bg, fmt=fmt, color_in=color_in, out=out)
 
     # ---- index.js:600-745 ----
     def processPlyBuffer(self, inputBuffer: bytes) -> bytes:
         return _ply.process_ply_buffer(inputBuffer)
+
+
+class _EntityWorker(SortWorker):
+    """The worker protocol of one entity of a SplatScene: `clear` drops only this entity's splats, `push` appends to its
+    range, `sort` replies with its own sortedIndexes (entity-local indices, as its own worker would)."""
+
+    def __init__(self, scene: "SplatScene", component: GaussianSplattingComponent):
+        super().__init__(scene.renderer)
+        self.scene, self.component = scene, component
+
+    def postMessage(self, data: dict, readback: bool = True):
+        method = data.get("method")
+        if method == "clear":
+            self.scene._clear_entity(self.component)
+            return None
+        if method == "push":
+            self.scene._push(self.component, np.frombuffer(memoryview(data["rows"]), dtype=np.uint8))
+            return None
+        if method == "sort":
+            first, count = self.scene.range_of(self.component)
+            if count == 0:
+                reply = {"sortedIndexes": np.zeros(1, np.uint32)}  # index.js:588-590 (quirk Q7)
+            else:
+                obj = SceneObject(first, count, np.zeros(16, np.float32), data.get("cutout"))
+                obj.modelview[[2, 6, 10, 14]] = np.asarray(data["view"], np.float32).reshape(4)
+                order = self.scene.renderer.sort_scene([obj]) - np.uint32(first)
+                self.scene.renderer.last_sort_count = len(order)
+                reply = {"sortedIndexes": order if readback else np.empty((0,), np.uint32)}
+            if self.onmessage is not None:
+                self.onmessage(reply)
+            return reply
+        return None
+
+
+class SplatScene:
+    """Several `gaussian_splatting` entities of one page drawn into one frame from one GPU context.
+
+    Each entity keeps its own worker semantics (index.js:229-236): its own sort with its own `view` row, cutout and
+    depth range (quirk Q5 repeats its own first splat); projection, viewport and focal are shared by the draw
+    (index.js:184-195).  render() draws the entities whole, in the order they were added (A-Frame 1.4 draws transparent
+    meshes in scene-graph order), over a caller-supplied colour and depth target: the opaque geometry already drawn.
+
+    Divergence: entities load one after another, each into its own contiguous range of the shared table; the reference
+    streams all of them at once, one worker each.  A component's clear() (loadData) drops only its own splats: the
+    other entities' rows are pushed again behind each other (the host keeps every entity's rows for that).
+    """
+
+    def __init__(self, renderer: Optional[SplatContext] = None, device: int = 0):
+        self.renderer = renderer or SplatContext(device)
+        self.entities: list = []   # components, in draw order
+        self._rows: dict = {}      # id(component) -> list of row chunks as pushed
+        self._range: dict = {}     # id(component) -> [first, count]
+
+    def add(self, component: GaussianSplattingComponent, camera, object3d) -> GaussianSplattingComponent:
+        """Attach `component` (drawn after the entities added before it) and load it: component.init() with this scene's
+        context."""
+        component.scene = self
+        self.entities.append(component)
+        self._rows[id(component)] = []
+        self._range[id(component)] = [self.renderer.num_splats, 0]
+        component.init(camera, object3d, self.renderer)
+        return component
+
+    def range_of(self, component: GaussianSplattingComponent):
+        first, count = self._range[id(component)]
+        return first, count
+
+    def _push(self, component, rows: np.ndarray) -> None:
+        rows = np.ascontiguousarray(rows, np.uint8).reshape(-1, 32)
+        first, count = self._range[id(component)]
+        if first + count != self.renderer.num_splats:  # another entity was loaded since: this one moves to the end
+            self._clear_entity(component, keep_rows=True)
+            first, count = self._range[id(component)]
+        self.renderer.push_splats(rows)
+        self._rows[id(component)].append(rows.copy())
+        self._range[id(component)][1] = count + rows.shape[0]
+
+    def _clear_entity(self, component, keep_rows: bool = False) -> None:
+        """Drop the entity's splats (keep_rows: move them to the end of the table instead) and repack the others."""
+        mine = self._rows[id(component)] if keep_rows else []
+        if not mine and not self._rows[id(component)]:  # nothing resident yet: the others stay where they are
+            self._range[id(component)] = [self.renderer.num_splats, 0]
+            return
+        self._rows[id(component)] = []
+        self.renderer.clear()
+        for e in self.entities:
+            if e is component:
+                continue
+            self._range[id(e)] = [self.renderer.num_splats, 0]
+            for r in self._rows[id(e)]:
+                self.renderer.push_splats(r)
+                self._range[id(e)][1] += r.shape[0]
+        self._range[id(component)] = [self.renderer.num_splats, 0]
+        for r in mine:
+            self.renderer.push_splats(r)
+            self._rows[id(component)].append(r)
+            self._range[id(component)][1] += r.shape[0]
+
+    def objects(self, width: int, height: int, camera=None):
+        """(shared FrameInputs of the draw, [SceneObject per entity in draw order]) for a width x height viewport."""
+        frames = [e.frame_inputs(width, height, camera) for e in self.entities]
+        objs = [SceneObject(*self.range_of(e), fr.modelview, fr.cutout) for e, fr in zip(self.entities, frames)]
+        return frames[0], objs
+
+    def render(self, width: int, height: int, camera=None, color_in: Optional[np.ndarray] = None,
+               depth_in: Optional[np.ndarray] = None, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
+               out: Optional[np.ndarray] = None) -> np.ndarray:
+        """One frame of every entity over the colour target `color_in` ((H, W, 4) of the output dtype; None = bg) and
+        the window-space depth `depth_in` ((H, W) f32; None = no depth test).  Row 0 = bottom."""
+        if not self.entities:
+            raise ValueError("SplatScene.render: no entity added")
+        frame, objs = self.objects(width, height, camera)
+        return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out)

@@ -106,6 +106,25 @@ static int ensure_scratch(gs_context *c) {
   return GS_OK;
 }
 
+// sort keys of scene frames, sized like the per-splat scratch; allocated by the first scene frame (the pipeline is idle)
+static int ensure_scene_bufs(gs_context *c) {
+  if (c->scene_cap >= c->cap && c->scene_key) return GS_OK;
+  dev_free(c->scene_key); dev_free(c->scene_pay); dev_free(c->scene_hi);
+  GS_CUDA(c, dev_alloc(&c->scene_key, (size_t)c->cap));
+  GS_CUDA(c, dev_alloc(&c->scene_pay, (size_t)c->cap));
+  GS_CUDA(c, dev_alloc(&c->scene_hi, (size_t)c->cap));
+  c->scene_cap = c->cap;
+  return GS_OK;
+}
+
+// a slot's scene table (device + pinned staging) and per-entity counters: fixed size, allocated once
+static int ensure_slot_scene(gs_context *c, gs_context::Slot &sl) {
+  if (!sl.scene_dev) GS_CUDA(c, cudaMalloc((void **)&sl.scene_dev, sizeof(SceneTable)));
+  if (!sl.scene_host) GS_CUDA(c, cudaHostAlloc((void **)&sl.scene_host, sizeof(SceneTable), cudaHostAllocDefault));
+  if (!sl.octr) GS_CUDA(c, dev_alloc(&sl.octr, (size_t)kMaxObjects));
+  return GS_OK;
+}
+
 static int ensure_instances(gs_context *c, uint64_t need) {
   if (need <= c->cap_inst && c->inst_rec[0]) return GS_OK;
   if (need >= (1ull << 30)) return fail(c, GS_ERR_CAPACITY, "more than 2^30 tile instances in one frame");
@@ -183,7 +202,7 @@ static void drop_graphs(gs_context *c) {
   auto kill = [](cudaGraphExec_t &g) { if (g) { cudaGraphExecDestroy(g); g = nullptr; } };
   for (auto &sl : c->slot)
     for (int i = 0; i < 2; ++i) {
-      kill(sl.graph_a[i][0]); kill(sl.graph_a[i][1]); kill(sl.graph_b[i]); kill(sl.graph_r[i]); kill(sl.graph_rp[i]);
+      kill(sl.graph_a[i][0]); kill(sl.graph_a[i][1]); kill(sl.graph_as[i]); kill(sl.graph_b[i]); kill(sl.graph_r[i]); kill(sl.graph_rp[i]);
       kill(sl.graph_sa[i]); kill(sl.graph_sl[i][0]); kill(sl.graph_sl[i][1]); kill(sl.graph_sl[i][2]);
     }
 }
@@ -223,6 +242,8 @@ extern "C" int gs_create(int device_ordinal, gs_context **out_ctx) {
   if (!c) return GS_ERR_OOM;
   c->device = device_ordinal;
   c->sm_count = prop.multiProcessorCount;
+  c->scene_tmp = new (std::nothrow) SceneTable();
+  if (!c->scene_tmp) { delete c; return GS_ERR_OOM; }
   auto bail = [&](const char *what, cudaError_t err) {
     g_create_error = std::string(what) + ": " + cudaGetErrorString(err);
     gs_destroy(c);
@@ -328,10 +349,15 @@ extern "C" int gs_destroy(gs_context *c) {
   dev_free(c->key32[0]); dev_free(c->key32[1]); dev_free(c->cidx); dev_free(c->ckey); dev_free(c->chunk_cnt[0]); dev_free(c->chunk_cnt[1]);
   dev_free(c->slab_tab[0]); dev_free(c->slab_tab[1]);
   dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open);
+  dev_free(c->scene_key); dev_free(c->scene_pay); dev_free(c->scene_hi);
+  delete c->scene_tmp;
   for (auto &sl : c->slot) {
     dev_free(sl.ctr); dev_free(sl.fp);
     if (sl.frame_dev) cudaFree(sl.frame_dev);
     if (sl.depth_dev) cudaFree(sl.depth_dev);
+    if (sl.color_dev) cudaFree(sl.color_dev);
+    dev_free(sl.scene_dev); dev_free(sl.octr);
+    if (sl.scene_host) cudaFreeHost(sl.scene_host);
     if (sl.ctr_host) cudaFreeHost(sl.ctr_host);
     if (sl.fp_host) cudaFreeHost(sl.fp_host);
     for (auto &ev : sl.ev) if (ev) cudaEventDestroy(ev);
@@ -464,6 +490,37 @@ static void fill_sort_consts(SortConsts &sc, const float view[4], const float *c
     for (int i = 0; i < 16; ++i) sc.cutout[i] = (double)cutout[i];
 }
 
+// Validates a scene's entity list and builds its table in t: non-empty entities sorted by their first splat, each with
+// its view row, cutout, modelview and draw rank.  Returns the table's byte count in *bytes.
+static int build_scene_table(gs_context *c, const gs_object *objs, uint32_t n_objs, SceneTable &t, size_t *bytes) {
+  if (!objs || n_objs == 0 || n_objs > (uint32_t)GS_MAX_OBJECTS)
+    return fail(c, GS_ERR_INVALID, "scene: between 1 and GS_MAX_OBJECTS entities");
+  std::vector<uint32_t> idx;
+  for (uint32_t k = 0; k < n_objs; ++k) {
+    if ((uint64_t)objs[k].first + objs[k].count > c->n)
+      return fail(c, GS_ERR_INVALID, "scene: an entity's range runs past the resident splats");
+    if (objs[k].count) idx.push_back(k);
+  }
+  std::sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return objs[a].first < objs[b].first; });
+  for (size_t j = 1; j < idx.size(); ++j)
+    if ((uint64_t)objs[idx[j - 1]].first + objs[idx[j - 1]].count > objs[idx[j]].first)
+      return fail(c, GS_ERR_INVALID, "scene: entity ranges overlap");
+  t.n = (uint32_t)idx.size();
+  for (size_t j = 0; j < idx.size(); ++j) {
+    const gs_object &g = objs[idx[j]];
+    SceneObject &o = t.obj[j];
+    const float view[4] = {g.modelview[2], g.modelview[6], g.modelview[10], g.modelview[14]};  // index.js:442
+    fill_sort_consts(o.sc, view, g.has_cutout ? g.cutout16 : nullptr);
+    memcpy(o.mv, g.modelview, sizeof(o.mv));
+    o.first = g.first;
+    o.end = g.first + g.count;
+    o.rank = idx[j];
+    o.pad = 0;
+  }
+  *bytes = offsetof(SceneTable, obj) + sizeof(SceneObject) * idx.size();
+  return GS_OK;
+}
+
 static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats);
 
 // finish whatever is in flight (before buffers are reallocated or the splat table changes)
@@ -582,6 +639,33 @@ static cudaError_t enqueue_sort_stage(gs_context *c, gs_context::Slot &sl, bool 
   return cudaGetLastError();
 }
 
+// Stage A of a scene frame: per-entity depth pass, keys and the (rank, key, index) sort; per-entity projection beside it.
+// The scene table was copied to sl.scene_dev ahead of the stage (submit).
+static cudaError_t enqueue_scene_sort_stage(gs_context *c, gs_context::Slot &sl, bool external_events) {
+  auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
+    return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
+  };
+  cudaStream_t m = c->stream, x = c->aux_stream;
+  const FrameBufs b = slot_bufs(c, sl);
+  cudaError_t e;
+  if ((e = cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, m))) return e;
+  if ((e = cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), m))) return e;
+  if ((e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, m))) return e;
+  if ((e = rec(sl.ev[0], m))) return e;
+  launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, m);
+  if ((e = cudaEventRecord(c->ev_fork[0], m))) return e;
+  if ((e = cudaStreamWaitEvent(x, c->ev_fork[0], 0))) return e;
+  if ((e = rec(sl.evp[0], x))) return e;
+  launch_project_scene(c, sl.fp, sl.scene_dev, sl.ctr, b, x);
+  if ((e = rec(sl.evp[1], x))) return e;
+  if ((e = cudaEventRecord(c->ev_join[0], x))) return e;
+  launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, m);
+  launch_scene_radix(c, sl.fp, sl.ctr, b, m);
+  if ((e = rec(sl.ev[1], m))) return e;
+  if ((e = cudaStreamWaitEvent(m, c->ev_join[0], 0))) return e;
+  return cudaGetLastError();
+}
+
 // Stage B (bin stream): tile instances in draw order, stable sort by tile, per-tile record lists and ranges.
 static cudaError_t enqueue_bin_stage(gs_context *c, gs_context::Slot &sl, uint32_t n_bins, bool external_events) {
   auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
@@ -646,6 +730,7 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
   // (re)capture when anything baked into the launches changed
   gs_context::GraphKey k;
   k.cap = c->cap; k.n_tiles = n_tiles; k.n_bins = n_bins; k.cap_inst = c->cap_inst; k.p0 = c->depth; k.p1 = c->inst_rec[0]; k.p2 = c->center_scale;
+  k.p3 = c->scene_key;
   if (memcmp(&k, &c->gkey, sizeof(k)) != 0) {
     drop_graphs(c);
     c->gkey = k;
@@ -653,7 +738,8 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
   const int set = sl.set;
   // A: order/proj_rec/rect[set] must no longer be read by the binning stage that used them last
   if (c->sort_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->sort_set_free[set], 0));
-  int rc = run_graph(c, sl.graph_a[set][reuse ? 1 : 0], c->stream, [&](bool ext) { return enqueue_sort_stage(c, sl, reuse, ext); });
+  int rc = sl.scene ? run_graph(c, sl.graph_as[set], c->stream, [&](bool ext) { return enqueue_scene_sort_stage(c, sl, ext); })
+                    : run_graph(c, sl.graph_a[set][reuse ? 1 : 0], c->stream, [&](bool ext) { return enqueue_sort_stage(c, sl, reuse, ext); });
   if (rc) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_sorted, c->stream));
   // B: needs A of this frame; inst_rec/bin_range[set] must no longer be read by the raster that used them last
@@ -671,7 +757,7 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
     // depth-tested / statistics frames use other instantiations of the raster: plain launches, no cached graph
     GS_CUDA(c, enqueue_raster_stage(c, sl, n_tiles, false));
   }
-  sl.launches = (reuse ? 0u : 7u) + 1u + (n_bins <= 256u ? 4u : 8u) + (c->emit_by_entry ? 1u : 0u) + 1u;
+  sl.launches = (sl.scene ? 11u : (reuse ? 0u : 7u)) + 1u + (n_bins <= 256u ? 4u : 8u) + (c->emit_by_entry ? 1u : 0u) + 1u;
   return GS_OK;
 }
 
@@ -735,6 +821,7 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
 static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
   gs_context::GraphKey k;
   k.cap = c->cap; k.n_tiles = n_tiles; k.n_bins = n_bins; k.cap_inst = c->cap_inst; k.p0 = c->depth; k.p1 = c->inst_rec[0]; k.p2 = c->center_scale;
+  k.p3 = c->scene_key;
   if (memcmp(&k, &c->gkey, sizeof(k)) != 0) {
     drop_graphs(c);
     c->gkey = k;
@@ -873,7 +960,24 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
       fp.depth_in = sl.depth_dev;
     }
   }
-  const bool reuse = (p->flags & GS_RENDER_REUSE_SORT) && c->have_order;
+  if (sl.color_in) {
+    if (sl.color_device) {
+      fp.color_in = sl.color_in;
+    } else {  // host colour target: staged per slot like a host depth_in
+      const size_t bytes = px_bytes * (size_t)p->width * p->height;
+      if (bytes > sl.color_bytes || !sl.color_dev) {
+        if (sl.color_dev) cudaFree(sl.color_dev);
+        sl.color_dev = nullptr;
+        GS_CUDA(c, cudaMalloc(&sl.color_dev, bytes));
+        sl.color_bytes = bytes;
+      }
+      GS_CUDA(c, cudaMemcpyAsync(sl.color_dev, sl.color_in, bytes, cudaMemcpyHostToDevice, c->stream));
+      fp.color_in = sl.color_dev;
+    }
+  }
+  // the scene table goes ahead of the sort stage on its stream (only the entities in use are copied)
+  if (sl.scene) GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, sl.scene_bytes, cudaMemcpyHostToDevice, c->stream));
+  const bool reuse = !sl.scene && (p->flags & GS_RENDER_REUSE_SORT) && c->have_order;
   // a frame normally takes the buffer set the previous frame did not; a frame that reuses the last sort must read
   // that sort's set, so it runs in it
   sl.set = reuse ? c->last_set : (c->last_set ^ 1);
@@ -885,7 +989,8 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   if ((rcode = enqueue_readback(c, sl))) return rcode;
   c->last_set = sl.set;
   sl.pending = true;
-  c->have_order = !sl.slab;  // a slab frame leaves no complete draw order behind (GS_RENDER_REUSE_SORT then sorts again)
+  // a slab frame leaves no complete draw order behind (GS_RENDER_REUSE_SORT then sorts again), nor does a scene frame
+  c->have_order = !sl.slab && !sl.scene;
   return GS_OK;
 }
 
@@ -982,9 +1087,10 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   return GS_OK;
 }
 
-extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *out_rgba, uint64_t *out_ticket) {
-  if (!c || !p || !out_rgba) return GS_ERR_INVALID;
-  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render before any push");
+// gs_render_async and scene frames.  scene: the table built by build_scene_table (nullptr = a plain frame);
+// color_in: the colour target or nullptr.
+static int render_async(gs_context *c, const gs_render_params *p, const SceneTable *scene, size_t scene_bytes,
+                        const void *color_in, void *out_rgba, uint64_t *out_ticket) {
   if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
   if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
@@ -1000,12 +1106,12 @@ extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *o
     gs_context::Slot &o = c->slot[(ticket - 3) % gs_context::kSlots];
     if (o.pending && o.ticket == ticket - 3 && (rcode = wait_slot(c, o, nullptr))) return rcode;
   }
-  if ((p->flags & GS_RENDER_REUSE_SORT) && c->have_order && (rcode = drain(c))) return rcode;  // runs in the last sort's buffers
+  if (!scene && (p->flags & GS_RENDER_REUSE_SORT) && c->have_order && (rcode = drain(c))) return rcode;  // runs in the last sort's buffers
   if ((p->flags & GS_RENDER_STATS) && (rcode = drain(c))) return rcode;  // the per-tile statistics buffer is not double-buffered
   // large scenes render front to back in depth slabs; the two paths share scratch buffers, so a change drains
   // (the criterion is the number of SORTED splats: the last frame's count when there is one, else the resident count)
   const uint32_t expect_sorted = c->have_last_sorted ? c->last_sorted : c->n;
-  const bool slab = expect_sorted >= c->slab_min && !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS));
+  const bool slab = !scene && expect_sorted >= c->slab_min && !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS));
   if ((int)slab != c->last_mode) {
     if ((rcode = drain(c))) return rcode;
     GS_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1014,7 +1120,8 @@ extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *o
     c->last_mode = (int)slab;
   }
   // growing any shared buffer needs an idle pipeline
-  const bool grow = (slab && (c->slab_cap < c->cap || !c->key32[0] || c->slab_tiles_cap < n_tiles || !c->slab_tab[1])) || !(c->scratch_cap >= c->cap && c->depth) || !(n_bins <= c->bins_cap && c->bin_range[0]) || !(n_tiles <= c->tile_stats_cap && c->tile_stats) || c->cap_inst == 0;
+  const bool grow = (slab && (c->slab_cap < c->cap || !c->key32[0] || c->slab_tiles_cap < n_tiles || !c->slab_tab[1])) || !(c->scratch_cap >= c->cap && c->depth) || !(n_bins <= c->bins_cap && c->bin_range[0]) || !(n_tiles <= c->tile_stats_cap && c->tile_stats) || c->cap_inst == 0 ||
+                    (scene && !(c->scene_cap >= c->cap && c->scene_key));
   if (grow) {
     if ((rcode = drain(c))) return rcode;
     GS_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1024,6 +1131,7 @@ extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *o
     if ((rcode = ensure_bins(c, n_bins))) return rcode;
     if ((rcode = ensure_tile_stats(c, n_tiles))) return rcode;
     if (slab && (rcode = ensure_slab(c, n_tiles, n_bins))) return rcode;
+    if (scene && (rcode = ensure_scene_bufs(c))) return rcode;
     if (c->cap_inst == 0) {
       // first frame: room for two bin instances per resident splat (a typical scene needs ~1); GS_INST_CAP overrides
       // the initial size (tests of the overflow / regrow path)
@@ -1037,9 +1145,98 @@ extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *o
   sl.ticket = ticket;
   sl.n_splats = c->n;
   sl.slab = slab;
+  sl.color_in = color_in;
+  sl.color_device = (p->flags & GS_RENDER_COLOR_DEVICE) != 0;
+  sl.scene = scene != nullptr;
+  if (scene) {
+    if ((rcode = ensure_slot_scene(c, sl))) return rcode;
+    memcpy(sl.scene_host, scene, scene_bytes);
+    sl.scene_bytes = scene_bytes;
+  }
   if ((rcode = submit(c, sl))) return rcode;
   c->next_ticket = ticket + 1;
   if (out_ticket) *out_ticket = ticket;
+  return GS_OK;
+}
+
+extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *out_rgba, uint64_t *out_ticket) {
+  if (!c || !p || !out_rgba) return GS_ERR_INVALID;
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render before any push");
+  return render_async(c, p, nullptr, 0, nullptr, out_rgba, out_ticket);
+}
+
+extern "C" int gs_render_scene_async(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                                     const void *color_in, void *out_rgba, uint64_t *out_ticket) {
+  if (!c || !frame || !out_rgba) return GS_ERR_INVALID;
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render_scene before any push");
+  if (frame->flags & GS_RENDER_REUSE_SORT) return fail(c, GS_ERR_INVALID, "scene frames always sort: GS_RENDER_REUSE_SORT is not accepted");
+  size_t bytes = 0;
+  int rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
+  if (rc) return rc;
+  if (n_objs == 1 && objs[0].first == 0 && objs[0].count == c->n) {
+    // one entity over the whole table: the plain frame with this entity's matrices, plus the colour target
+    gs_render_params p = *frame;
+    memcpy(p.modelview, objs[0].modelview, sizeof(p.modelview));
+    p.has_cutout = objs[0].has_cutout;
+    memcpy(p.cutout16, objs[0].cutout16, sizeof(p.cutout16));
+    return render_async(c, &p, nullptr, 0, color_in, out_rgba, out_ticket);
+  }
+  return render_async(c, frame, c->scene_tmp, bytes, color_in, out_rgba, out_ticket);
+}
+
+extern "C" int gs_render_scene(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                               const void *color_in, void *out_rgba, gs_stats *stats) {
+  uint64_t t = 0;
+  int rc = gs_render_scene_async(c, frame, objs, n_objs, color_in, out_rgba, &t);
+  if (rc) return rc;
+  return gs_wait(c, t, stats);
+}
+
+extern "C" int gs_sort_scene(gs_context *c, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx, uint32_t *out_count) {
+  if (!c) return GS_ERR_INVALID;
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_sort_scene before any push");
+  GS_CUDA(c, cudaSetDevice(c->device));
+  size_t bytes = 0;
+  int rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
+  if (rc) return rc;
+  if ((rc = drain(c))) return rc;
+  GS_CUDA(c, cudaStreamSynchronize(c->stream));
+  GS_CUDA(c, cudaStreamSynchronize(c->bstream));
+  GS_CUDA(c, cudaStreamSynchronize(c->rstream));
+  if ((rc = ensure_scratch(c))) return rc;
+  if ((rc = ensure_scene_bufs(c))) return rc;
+  gs_context::Slot &sl = c->slot[0];
+  if ((rc = ensure_slot_scene(c, sl))) return rc;
+  c->last_set = 0;
+  const FrameBufs bufs{c->order[0], c->proj_rec[0], c->rect[0], c->inst_rec[0], c->bin_range[0]};
+  memset(sl.fp_host, 0, sizeof(FrameParams));
+  sl.fp_host->n_splats = c->n;
+  memcpy(sl.scene_host, c->scene_tmp, bytes);
+  if (c->pushed) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->push_done, 0));
+  GS_CUDA(c, cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, c->stream));
+  GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, bytes, cudaMemcpyHostToDevice, c->stream));
+  GS_CUDA(c, cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), c->stream));
+  GS_CUDA(c, cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, c->stream));
+  GS_CUDA(c, cudaEventRecord(c->ev[0], c->stream));
+  launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
+  launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
+  launch_scene_radix(c, sl.fp, sl.ctr, bufs, c->stream);
+  GS_CUDA(c, cudaGetLastError());
+  GS_CUDA(c, cudaEventRecord(c->ev[1], c->stream));
+  GS_CUDA(c, cudaMemcpyAsync(sl.ctr_host, sl.ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, c->stream));
+  GS_CUDA(c, cudaStreamSynchronize(c->stream));
+  memset(&c->stats, 0, sizeof(c->stats));
+  stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
+  c->stats.kernel_launches = 11;
+  float ms = 0;
+  cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]);
+  c->stats.ms_sort = ms;
+  c->stats.ms_total = ms;
+  c->have_order = false;  // a concatenation of several entities' orders is no single-entity order
+  c->order_count = sl.ctr_host->sort.n_valid;
+  if (out_count) *out_count = c->order_count;
+  if (out_idx && c->order_count)
+    GS_CUDA(c, cudaMemcpy(out_idx, c->order[0], sizeof(uint32_t) * (size_t)c->order_count, cudaMemcpyDeviceToHost));
   return GS_OK;
 }
 

@@ -105,6 +105,8 @@ struct FrameParams {
   uint32_t n_splats;  // resident splats of THIS frame (the table may be growing behind it: progressive push)
   void *out;  // frame (or packed owned tiles) destination of the raster
   const void *depth_in;  // optional window-space depth of foreign geometry (f32, width*height, row 0 = bottom)
+  const void *color_in;  // optional colour of the geometry already drawn (output element type, width*height, row 0 =
+                         // bottom): the per-pixel destination of the blend in place of rc.bg
   // ---- fused raster + exchange over NVLink peer memory (GS_RENDER_OUT_PEER) ----
   uint32_t n_peer;                       // 0: plain output; else every finished tile is stored into all ranks' frames
   uint32_t peer_rank;
@@ -117,6 +119,37 @@ struct FrameParams {
   unsigned long long peer_need;          // slot may be overwritten once every rank released seq >= peer_need
 };
 
+// ---- scene frames (gs_render_scene / gs_sort_scene): several entities, each with its own camera-space matrix, cutout
+// and worker sort (index.js:229-236, 438-455), drawn whole one after another.  The table lives in a fixed-size per-slot
+// device buffer, so entity count, ranges and matrices change without re-capturing the stage graphs. ----
+constexpr int kMaxObjects = GS_MAX_OBJECTS;
+struct SceneObject {
+  SortConsts sc;         // the entity's view row (row 2 of its modelview, index.js:442) and cutout (index.js:443-448)
+  float mv[16];          // its gsModelViewMatrix (index.js:467-487)
+  uint32_t first, end;   // its splats: [first, end) of the resident table
+  uint32_t rank;         // draw position (index into the caller's list): the most significant part of the sort key
+  uint32_t pad;
+};
+struct SceneTable {
+  uint32_t n;            // non-empty entities, sorted by `first` (empty ones draw nothing and are left out)
+  uint32_t pad[3];
+  SceneObject obj[kMaxObjects];
+};
+// per-entity results of the depth pass (one worker's min / max / validCount, index.js:548-555)
+struct ObjCounters {
+  unsigned long long min_enc, max_enc;  // encodings as in SortHeader
+  uint32_t n_valid, pad;
+};
+
+// table index of the entity whose range holds splat i, or -1 (s_first ascending, ranges disjoint)
+__device__ __forceinline__ int scene_find(const uint32_t *s_first, const uint32_t *s_end, uint32_t n_obj, uint32_t i) {
+  uint32_t lo = 0, hi = n_obj;  // first k with s_first[k] > i
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (s_first[mid] <= i) lo = mid + 1; else hi = mid;
+  }
+  return (lo > 0 && i < s_end[lo - 1]) ? (int)lo - 1 : -1;
+}
 
 // ---- front-to-back slab path ----
 constexpr int kMaxSlabs = 12;          // geometric slab sizes: 1 M, 2 M, 4 M ... entries (nearest first)
@@ -198,6 +231,13 @@ struct gs_context {
   uint4 *tile_stats = nullptr;     // [tiles] per-tile counts of a GS_RENDER_STATS frame
   uint4 *tile_stats_host = nullptr;  // pinned copy
   uint32_t tile_stats_cap = 0;
+  // ---- scene frames: sort keys of the three-pass (entity, key, index) sort, allocated by the first scene frame ----
+  uint32_t scene_cap = 0;
+  uint32_t *scene_key = nullptr;   // [cap] (draw rank << 17 | 16-bit key, or 65536 for a quirk-Q5 drop), kNoKey if not sorted
+  uint32_t *scene_pay = nullptr;   // [cap] payload of pass 1 (splat index, or the entity's first splat for a Q5 drop);
+                                   //       reused as pass 2's index output
+  uint16_t *scene_hi = nullptr;    // [cap] key bits 8..23 carried from pass 1 to pass 2
+  gs::SceneTable *scene_tmp = nullptr;  // host: the table being validated before a slot is chosen
   double *quirk_table = nullptr;   // parseInt quirk thresholds (device)
   int quirk_n = 0;
   gs::SortHeader *sort_hdr = nullptr;  // device: counters header of the last sort (for GS_RENDER_REUSE_SORT)
@@ -217,6 +257,15 @@ struct gs_context {
     size_t frame_bytes = 0;
     void *depth_dev = nullptr;               // staging of a host depth_in
     size_t depth_bytes = 0;
+    const void *color_in = nullptr;          // caller's colour target (scene frames), host unless color_device
+    bool color_device = false;
+    void *color_dev = nullptr;               // staging of a host color_in
+    size_t color_bytes = 0;
+    bool scene = false;                      // multi-entity frame (gs_render_scene): scene table below
+    gs::SceneTable *scene_dev = nullptr;     // device copy, fixed size (captured graphs bake the pointer)
+    gs::SceneTable *scene_host = nullptr;    // pinned staging
+    size_t scene_bytes = 0;                  // bytes of the table in use (header + non-empty entities)
+    gs::ObjCounters *octr = nullptr;         // [kMaxObjects] per-entity depth-pass results
     uint32_t raster_flags = 0;               // k_raster instantiation of this frame (packed | depth | stats)
     uint32_t n_splats = 0;                   // resident splats when the frame was submitted
     bool slab = false;                       // rendered by the front-to-back slab path
@@ -227,6 +276,7 @@ struct gs_context {
     cudaEvent_t ev_done = nullptr, ev_copied = nullptr;
     // CUDA graphs of the three stages, one per buffer set this slot can be paired with
     cudaGraphExec_t graph_a[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // sort + project, [set][reuse_sort]
+    cudaGraphExec_t graph_as[2] = {nullptr, nullptr};                          // scene frames: sort + project, [set]
     cudaGraphExec_t graph_b[2] = {nullptr, nullptr};                           // binning, [set]
     cudaGraphExec_t graph_r[2] = {nullptr, nullptr};                           // raster, [set]
     cudaGraphExec_t graph_rp[2] = {nullptr, nullptr};                          // acquire + raster + signal/wait (fused exchange)
@@ -273,7 +323,7 @@ struct gs_context {
   bool use_pdl = false;                          // programmatic dependent launch inside the stage chains (GS_PDL=1 turns it on)
   uint32_t raster_base_flags = 1;                // default pixel loop: 1 = two pixels per lane, 0 = one
   // graph cache key: anything baked into the captured launches
-  struct GraphKey { uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr; } gkey;
+  struct GraphKey { uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr; } gkey;
 
   // ---- fused exchange: one shared allocation per rank = flag rows + a ring of 3 frames, opened by every peer ----
   void *peer_local = nullptr;            // our shared block
@@ -309,6 +359,14 @@ struct FrameBufs {
 // -- launchers (each .cu file owns its kernels); every per-frame input comes from device memory (fp, ctr) --
 void launch_depth_cull(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
 void launch_depth_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 6 launches -> b.order
+// scene frames: per-entity depth pass, per-entity keys, (rank, key, index) sort -> b.order, per-entity projection
+void launch_depth_cull_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, ObjCounters *octr, FrameCounters *ctr,
+                             cudaStream_t st);
+void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *scene, const ObjCounters *octr, FrameCounters *ctr,
+                       cudaStream_t st);
+void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 9 launches
+void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
+                          const FrameBufs &b, cudaStream_t st);
 void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_t n, cudaStream_t st);
 void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
 void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 2 launches

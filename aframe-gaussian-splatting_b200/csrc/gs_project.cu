@@ -2,7 +2,8 @@
 // ordered emission of bin instances (kBin x kBin-pixel bins = 6x6 raster tiles by default; "tile" below means bin).
 //
 //   k_project  : fp32 restatement of the vertex shader, op for op (no FMA contraction), producing a
-//                32 B projected record per splat + its packed tile rectangle.
+//                32 B projected record per splat + its packed tile rectangle (scene frames: with each splat's entity's
+//                gsModelViewMatrix).
 //   k_count    : per entry of the draw order (== reference sortedIndexes): instance offset inside its 256-entry slice;
 //                per slice: total; last CTA: prefix over the slices + frame total D.
 //                Sparse frames (fewer than half of the splats sorted): each chunk's survivors are compacted first.
@@ -39,12 +40,13 @@ __device__ __forceinline__ void unpack_int16(uint32_t value, float &lo, float &h
 // ---------------------------------------------------------------------------------------------
 // One splat through the vertex shader: returns its packed bin rectangle (kNoRect when nothing is drawn) and stores the
 // 32 B record at slot j.
-__device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const float4 *__restrict__ cs,
+// mv: the splat's gsModelViewMatrix (rc.mv, or its entity's in a scene frame).
+__device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const float *mv, const float4 *__restrict__ cs,
                                                 const uint4 *__restrict__ cc, uint32_t i, uint32_t j,
                                                 float4 *__restrict__ rec_out) {
   uint32_t rect = kNoRect;
   const float4 c = __ldg(cs + i);
-  const float *mv = rc.mv, *P = rc.proj;
+  const float *P = rc.proj;
   // index.js:106-108: camspace = MV * (center,1); pos2d = P * camspace  (sum x,y,z,w left to right)
   float cam[4], p[4];
 #pragma unroll
@@ -146,16 +148,39 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
 // Index order, sparse frames (fewer than half of the resident splats passed the worker filter, e.g. a cutout box): the
 // survivors of every 1024-splat chunk are first compacted into shared memory, so the shader runs in full warps
 // instead of warps with a few live lanes each.
-template <bool BY_ENTRY>
+// SCENE (scene frames, index order): every splat takes its entity's modelview, and the splat the Q5 tail may repeat is
+// each entity's first one.
+template <bool BY_ENTRY, bool SCENE = false>
 __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, const uint4 *__restrict__ cc,
                                                  const float *__restrict__ depth,
                                                  const FrameParams *__restrict__ fp, float4 *__restrict__ rec_out,
                                                  uint32_t *__restrict__ rect_out, const uint32_t *__restrict__ order,
-                                                 const FrameCounters *__restrict__ ctr) {
+                                                 const FrameCounters *__restrict__ ctr,
+                                                 const SceneTable *__restrict__ scene) {
   GS_PDL_ENTRY();
   const RenderConsts &rc = fp->rc;
   const uint32_t n = BY_ENTRY ? ctr->sort.n_valid : fp->n_splats;
   const uint32_t stride = gridDim.x * blockDim.x;
+  __shared__ uint32_t s_first[SCENE ? kMaxObjects : 1], s_end[SCENE ? kMaxObjects : 1];
+  uint32_t n_obj = 0;
+  if (SCENE) {
+    n_obj = scene->n;
+    for (uint32_t k = threadIdx.x; k < n_obj; k += blockDim.x) {
+      s_first[k] = scene->obj[k].first;
+      s_end[k] = scene->obj[k].end;
+    }
+    __syncthreads();
+  }
+  // splats projected although the worker filter rejected them: what the zero tail of quirk Q5 may draw
+  auto q5_head = [&](uint32_t i) -> bool {
+    if (!SCENE) return i == 0u;
+    const int k = scene_find(s_first, s_end, n_obj, i);
+    return k >= 0 && s_first[k] == i;
+  };
+  auto modelview = [&](uint32_t i) -> const float * {
+    if (!SCENE) return rc.mv;
+    return scene->obj[scene_find(s_first, s_end, n_obj, i)].mv;
+  };
   if (!BY_ENTRY && (unsigned long long)ctr->sort.n_valid * 2ull < n) {
     constexpr uint32_t kChunk = 1024;  // 4 splats per thread
     __shared__ uint32_t s_list[kChunk];
@@ -181,7 +206,7 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
       uint32_t m = 0;
 #pragma unroll
       for (uint32_t k = 0; k < 4; ++k) {
-        f[k] = (base + k < n) && ((d[k] != GS_DEPTH_REJECT) || (base + k == 0u));  // splat 0: quirk Q5's zero tail
+        f[k] = (base + k < n) && ((d[k] != GS_DEPTH_REJECT) || q5_head(base + k));  // quirk Q5's zero tail
         m += f[k] ? 1u : 0u;
       }
       uint32_t incl = m;
@@ -204,7 +229,7 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
       __syncthreads();
       for (uint32_t q = tid; q < total; q += blockDim.x) {
         const uint32_t i = s_list[q];
-        const uint32_t rect = project_one(rc, cs, cc, i, i, rec_out);
+        const uint32_t rect = project_one(rc, modelview(i), cs, cc, i, i, rec_out);
         if (rect != kNoRect) rect_out[i] = rect;
       }
       __syncthreads();
@@ -214,8 +239,8 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
   for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
     const uint32_t i = BY_ENTRY ? __ldg(order + j) : j;
     uint32_t rect = kNoRect;
-    const bool sorted = BY_ENTRY || (__ldg(depth + i) != GS_DEPTH_REJECT) || (i == 0);
-    if (sorted) rect = project_one(rc, cs, cc, i, j, rec_out);
+    const bool sorted = BY_ENTRY || (__ldg(depth + i) != GS_DEPTH_REJECT) || q5_head(i);
+    if (sorted) rect = project_one(rc, modelview(i), cs, cc, i, j, rec_out);
     rect_out[j] = rect;
   }
 }
@@ -674,7 +699,17 @@ void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *c
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   launch_chain(c, k_project<false>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
-               (const uint32_t *)nullptr, ctr);  // ctr: the sorted count picks the sparse-frame path
+               (const uint32_t *)nullptr, ctr, (const SceneTable *)nullptr);  // ctr: the sorted count picks the sparse-frame path
+}
+
+void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
+                          const FrameBufs &b, cudaStream_t stream) {
+  uint64_t blocks = ((uint64_t)c->cap + 255) / 256;
+  const uint64_t cap = (uint64_t)c->sm_count * 16;
+  if (blocks > cap) blocks = cap;
+  if (blocks < 1) blocks = 1;
+  launch_chain(c, k_project<false, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
+               (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene);
 }
 
 void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t stream) {
@@ -683,7 +718,7 @@ void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters 
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   launch_chain(c, k_project<true>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
-               (const uint32_t *)b.order, (const FrameCounters *)ctr);
+               (const uint32_t *)b.order, (const FrameCounters *)ctr, (const SceneTable *)nullptr);
 }
 
 static void launch_emit_impl(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st, bool slab);

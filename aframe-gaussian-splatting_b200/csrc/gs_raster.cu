@@ -13,6 +13,7 @@
 //
 //   back-to-front (reference):  C <- c*a + C*(1-a),  A <- a + A*(1-a)      (index.js:177-178)
 //   front-to-back (here):       C  = sum_i c_i a_i T_i + bg*T_end,  A = 1 - T_end + bg.a*T_end,
+//                               (bg: the clear colour, or the colour target's pixel when the frame has one)
 //                               T_i = prod_{j nearer than i} (1 - a_j)      (SURVEY.md A.5)
 // The two are algebraically identical.  A PIXEL stops accumulating at the first splat that finds its transmittance
 // below 3e-4 (the dropped contribution is <= 3e-4 per channel; the parity tolerance is 1e-3): the result does not
@@ -88,9 +89,24 @@ __device__ __forceinline__ void store_pixel(const FrameParams *fp, uint32_t tile
                                             uint32_t ly, uint32_t x, uint32_t y, bool inside, float T, float Cr, float Cg,
                                             float Cb) {
   const RenderConsts &rc = fp->rc;
-  // composite over the clear colour
-  const float oR = __fmaf_rn(rc.bg[0], T, Cr), oG = __fmaf_rn(rc.bg[1], T, Cg), oB = __fmaf_rn(rc.bg[2], T, Cb);
-  const float oA = __fmaf_rn(rc.bg[3], T, 1.0f - T);
+  // composite over the clear colour, or over the colour target's pixel (the geometry already drawn: the destination of
+  // the reference's blend, index.js:177-181); an RGBA8 target reads as float(byte) / 255.0 like the splat colours
+  float d0 = rc.bg[0], d1 = rc.bg[1], d2 = rc.bg[2], d3 = rc.bg[3];
+  if (fp->color_in && inside) {
+    const size_t p = (size_t)y * rc.width + x;
+    if (rc.out_format == GS_FORMAT_RGBA8) {
+      const uint32_t v = __ldg((const uint32_t *)fp->color_in + p);
+      d0 = __fdiv_rn((float)(v & 255u), 255.0f);
+      d1 = __fdiv_rn((float)((v >> 8) & 255u), 255.0f);
+      d2 = __fdiv_rn((float)((v >> 16) & 255u), 255.0f);
+      d3 = __fdiv_rn((float)(v >> 24), 255.0f);
+    } else {
+      const float4 v = __ldg((const float4 *)fp->color_in + p);
+      d0 = v.x; d1 = v.y; d2 = v.z; d3 = v.w;
+    }
+  }
+  const float oR = __fmaf_rn(d0, T, Cr), oG = __fmaf_rn(d1, T, Cg), oB = __fmaf_rn(d2, T, Cb);
+  const float oA = __fmaf_rn(d3, T, 1.0f - T);
   size_t pix;
   bool write;
   if (rc.out_tiled) {
@@ -477,7 +493,7 @@ void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr
     k_raster<true, false, false, true><<<n_tiles, RasterCfg<true>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
 }
 
-// slab path epilogue: pixel state -> frame (composite over the clear colour; plain / tiled / peer destinations)
+// slab path epilogue: pixel state -> frame (composite over the clear colour or colour target; plain / tiled / peer destinations)
 __global__ void __launch_bounds__(256) k_resolve(const float4 *__restrict__ state, const FrameParams *__restrict__ fp) {
   const RenderConsts &rc = fp->rc;
   const uint32_t tile = blockIdx.x;

@@ -10,6 +10,16 @@
 //   k_radix_{hist,scan,scatter}<S1>: first pass of a depth slab's sort (keys from the slab's compacted entries)
 //   k_tile_ranges : per-bin {start, end} in the final instance order (frames of more than 256 bins; otherwise pass T1 writes them)
 //
+// Scene frames (several entities, gs_render_scene): one worker per entity (index.js:229-236), each with its own view row,
+// cutout, min/max depth and 16-bit key space, drawn whole in the caller's order:
+//   k_depth_cull_scene : k_depth_cull with each splat's own entity (sorted range table in shared memory); min/max and
+//                        validCount per entity
+//   k_scene_keys       : 24-bit key = draw rank << 17 | the entity's 16-bit key, or | 65536 for a key outside
+//                        [0,65535] with payload = the entity's first splat (quirk Q5 per entity: the worker's dropped slots
+//                        stay 0, the entity-local splat 0, and come after all its in-range entries)
+//   k_radix_*<M1/M2/M3>: three stable 8-bit passes -> (rank, key, index) order = each entity's sortedIndexes + first,
+//                        concatenated in draw order
+//
 // Bit-exactness: JS evaluates in fp64 with IEEE rounding after every operation; the kernels use
 // __dmul_rn/__dadd_rn so nothing is contracted, and ToInt32 is restated exactly (js_to_int32).
 #include <type_traits>
@@ -22,6 +32,31 @@ namespace gs {
 // ---------------------------------------------------------------------------------------------
 // K1: depth + cull + min/max (index.js:517-555).  Reads 16 B + 4 B per splat, writes 4 B.
 // ---------------------------------------------------------------------------------------------
+// The worker's per-splat test (index.js:517-548): fp64 depth from the view row, cutout box, filter.  True = kept.
+__device__ __forceinline__ bool worker_keep(const SortConsts &sc, const float4 c, const float s, double &depth) {
+  const double x = c.x, y = c.y, z = c.z;
+  // index.js:519-523
+  depth = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(sc.view[0], x), __dmul_rn(sc.view[1], y)), __dmul_rn(sc.view[2], z)),
+                    sc.view[3]);
+  bool in_box = true;
+  if (sc.has_cutout) {
+    // index.js:533 -> mul(cutout, x, -y, z) of index.js:492-500 (Q12: centre only, y negated)
+    const double *e = sc.cutout;
+    const double ny = -y;
+    const double w = __ddiv_rn(
+        1.0, __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[3], x), __dmul_rn(e[7], ny)), __dmul_rn(e[11], z)), e[15]));
+    const double c0 = __dmul_rn(
+        __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[0], x), __dmul_rn(e[4], ny)), __dmul_rn(e[8], z)), e[12]), w);
+    const double c1 = __dmul_rn(
+        __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[1], x), __dmul_rn(e[5], ny)), __dmul_rn(e[9], z)), e[13]), w);
+    const double c2 = __dmul_rn(
+        __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[2], x), __dmul_rn(e[6], ny)), __dmul_rn(e[10], z)), e[14]), w);
+    if (c0 < -0.5 || c0 > 0.5 || c1 < -0.5 || c1 > 0.5 || c2 < -0.5 || c2 > 0.5) in_box = false;
+  }
+  // index.js:548
+  return (depth < 0.0) && ((double)s > __dmul_rn(-0.0001, depth)) && in_box;
+}
+
 __global__ void __launch_bounds__(256) k_depth_cull(const float4 *__restrict__ cs, const float *__restrict__ sa,
                                                     const FrameParams *__restrict__ fp,
                                                     float *__restrict__ depth_out, FrameCounters *ctr) {
@@ -32,28 +67,8 @@ __global__ void __launch_bounds__(256) k_depth_cull(const float4 *__restrict__ c
   uint32_t cnt = 0;
   const uint32_t stride = gridDim.x * blockDim.x;
   auto process = [&](uint32_t i, const float4 c, const float s) {
-    const double x = c.x, y = c.y, z = c.z;
-    // index.js:519-523
-    const double depth =
-        __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(sc.view[0], x), __dmul_rn(sc.view[1], y)), __dmul_rn(sc.view[2], z)),
-                  sc.view[3]);
-    bool in_box = true;
-    if (sc.has_cutout) {
-      // index.js:533 -> mul(cutout, x, -y, z) of index.js:492-500 (Q12: centre only, y negated)
-      const double *e = sc.cutout;
-      const double ny = -y;
-      const double w = __ddiv_rn(
-          1.0, __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[3], x), __dmul_rn(e[7], ny)), __dmul_rn(e[11], z)), e[15]));
-      const double c0 = __dmul_rn(
-          __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[0], x), __dmul_rn(e[4], ny)), __dmul_rn(e[8], z)), e[12]), w);
-      const double c1 = __dmul_rn(
-          __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[1], x), __dmul_rn(e[5], ny)), __dmul_rn(e[9], z)), e[13]), w);
-      const double c2 = __dmul_rn(
-          __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[2], x), __dmul_rn(e[6], ny)), __dmul_rn(e[10], z)), e[14]), w);
-      if (c0 < -0.5 || c0 > 0.5 || c1 < -0.5 || c1 > 0.5 || c2 < -0.5 || c2 > 0.5) in_box = false;
-    }
-    // index.js:548
-    const bool keep = (depth < 0.0) && ((double)s > __dmul_rn(-0.0001, depth)) && in_box;
+    double depth;
+    const bool keep = worker_keep(sc, c, s, depth);
     float out = GS_DEPTH_REJECT;
     if (keep) {
       out = (float)depth;  // Float32Array store (index.js:549)
@@ -106,6 +121,141 @@ __global__ void __launch_bounds__(256) k_depth_cull(const float4 *__restrict__ c
 }
 
 // ---------------------------------------------------------------------------------------------
+// Scene frames, K1: k_depth_cull with each splat's own entity; min/max/validCount per entity (and over the frame, for the
+// statistics).  Splats outside every entity's range are not sorted.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_depth_cull_scene(const float4 *__restrict__ cs, const float *__restrict__ sa,
+                                                          const FrameParams *__restrict__ fp, const SceneTable *__restrict__ scene,
+                                                          float *__restrict__ depth_out, FrameCounters *ctr, ObjCounters *octr) {
+  GS_PDL_ENTRY();
+  __shared__ uint32_t s_first[kMaxObjects], s_end[kMaxObjects], s_cnt[kMaxObjects];
+  __shared__ unsigned long long s_min[kMaxObjects], s_max[kMaxObjects];
+  const uint32_t n_obj = scene->n;
+  for (uint32_t k = threadIdx.x; k < n_obj; k += blockDim.x) {
+    s_first[k] = scene->obj[k].first;
+    s_end[k] = scene->obj[k].end;
+    s_cnt[k] = 0;
+    s_min[k] = 0;
+    s_max[k] = 0;
+  }
+  __syncthreads();
+  const uint32_t n = fp->n_splats;
+  const uint32_t stride = gridDim.x * blockDim.x;
+  // a thread's splats are `stride` apart and the ranges contiguous: it accumulates one entity at a time and flushes
+  // into shared memory when the entity changes
+  int cur = -1;
+  double dmin = INFINITY, dmax = -INFINITY;
+  uint32_t cnt = 0;
+  auto flush = [&]() {
+    if (cnt) {
+      atomicMax(&s_min[cur], ~enc_f64(dmin));
+      atomicMax(&s_max[cur], enc_f64(dmax));
+      atomicAdd(&s_cnt[cur], cnt);
+    }
+    dmin = INFINITY;
+    dmax = -INFINITY;
+    cnt = 0;
+  };
+  auto process = [&](uint32_t i, const float4 c, const float s) {
+    float out = GS_DEPTH_REJECT;
+    const int k = scene_find(s_first, s_end, n_obj, i);
+    double depth;
+    if (k >= 0 && worker_keep(scene->obj[k].sc, c, s, depth)) {
+      if (k != cur) {
+        flush();
+        cur = k;
+      }
+      out = (float)depth;  // Float32Array store (index.js:549)
+      ++cnt;
+      if (depth > dmax) dmax = depth;
+      if (depth < dmin) dmin = depth;
+    }
+    depth_out[i] = out;
+  };
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += 2 * stride) {
+    const uint32_t j = i + stride;
+    const bool two = j < n;
+    const float4 c0 = __ldg(cs + i);
+    const float s0 = __ldg(sa + i);
+    float4 c1 = c0;
+    float s1 = s0;
+    if (two) {
+      c1 = __ldg(cs + j);
+      s1 = __ldg(sa + j);
+    }
+    process(i, c0, s0);
+    if (two) process(j, c1, s1);
+  }
+  flush();
+  __syncthreads();
+  for (uint32_t k = threadIdx.x; k < n_obj; k += blockDim.x) {
+    if (!s_cnt[k]) continue;
+    atomicMax(&octr[k].min_enc, s_min[k]);
+    atomicMax(&octr[k].max_enc, s_max[k]);
+    atomicAdd(&octr[k].n_valid, s_cnt[k]);
+    atomicMax(&ctr->sort.min_enc, s_min[k]);
+    atomicMax(&ctr->sort.max_enc, s_max[k]);
+    atomicAdd(&ctr->sort.n_valid, s_cnt[k]);
+  }
+}
+
+// Scene frames: the 24-bit sort key of every splat (kNoKey = not sorted) and the payload of the first radix pass.
+__global__ void __launch_bounds__(256) k_scene_keys(const float *__restrict__ depth, const FrameParams *__restrict__ fp,
+                                                    const SceneTable *__restrict__ scene, const ObjCounters *__restrict__ octr,
+                                                    FrameCounters *ctr, uint32_t *__restrict__ key_out,
+                                                    uint32_t *__restrict__ pay_out) {
+  GS_PDL_ENTRY();
+  __shared__ uint32_t s_first[kMaxObjects], s_end[kMaxObjects], s_tag[kMaxObjects];
+  __shared__ double s_min[kMaxObjects], s_inv[kMaxObjects];
+  __shared__ uint32_t s_in, s_drop;
+  const uint32_t n_obj = scene->n;
+  for (uint32_t k = threadIdx.x; k < n_obj; k += blockDim.x) {
+    s_first[k] = scene->obj[k].first;
+    s_end[k] = scene->obj[k].end;
+    s_tag[k] = scene->obj[k].rank << 17;
+    // the entity's own range (index.js:552-558), as load_depth_range does for a single worker
+    const double mn = dec_f64(~octr[k].min_enc), mx = dec_f64(octr[k].max_enc);
+    s_min[k] = mn;
+    s_inv[k] = __ddiv_rn(65535.0, __dsub_rn(mx, mn));
+  }
+  if (threadIdx.x == 0) { s_in = 0; s_drop = 0; }
+  __syncthreads();
+  const uint32_t n = ctr->sort.n_valid ? fp->n_splats : 0u;
+  uint32_t in = 0, drop = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float d = __ldg(depth + i);
+    uint32_t key = kNoKey;
+    if (d != GS_DEPTH_REJECT) {
+      const int k = scene_find(s_first, s_end, n_obj, i);  // a sorted splat always lies in an entity's range
+      const int32_t q = depth_key(d, s_min[k], s_inv[k]);
+      if (q >= 0 && q <= 65535) {
+        key = s_tag[k] | (uint32_t)q;
+        pay_out[i] = i;
+        ++in;
+      } else {  // quirk Q5: the entity's slot stays 0 -> its first splat, after all its in-range entries
+        key = s_tag[k] | 65536u;
+        pay_out[i] = s_first[k];
+        ++drop;
+      }
+    }
+    key_out[i] = key;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    in += __shfl_xor_sync(0xffffffffu, in, o);
+    drop += __shfl_xor_sync(0xffffffffu, drop, o);
+  }
+  if ((threadIdx.x & 31u) == 0) {
+    if (in) atomicAdd(&s_in, in);
+    if (drop) atomicAdd(&s_drop, drop);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (s_in) atomicAdd(&ctr->sort.n_inrange, s_in);
+    if (s_drop) atomicAdd(&ctr->sort.n_dropped, s_drop);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Stable 8-bit radix pass = three fully parallel kernels (no inter-CTA spinning):
 //   k_radix_hist<PASS>   : per-chunk (4096 elements) digit histogram        -> table[digit][chunk]
 //   k_radix_scan<PASS>   : per-digit exclusive scan over the chunks (in place) + digit totals
@@ -113,7 +263,8 @@ __global__ void __launch_bounds__(256) k_depth_cull(const float4 *__restrict__ c
 // PASS_D1/D2: 16-bit depth key (index.js:557-567) low/high byte.  PASS_T1/T2: 16-bit tile id low/high byte;
 // T2's scatter gathers the 32 B projected record of each instance into its final per-tile slot.
 // ---------------------------------------------------------------------------------------------
-enum { PASS_D1 = 0, PASS_D2 = 1, PASS_T1 = 2, PASS_T2 = 3, PASS_S1 = 4 };  // S1: low key byte of a compacted slab (gs_slab.cu)
+enum { PASS_D1 = 0, PASS_D2 = 1, PASS_T1 = 2, PASS_T2 = 3, PASS_S1 = 4,  // S1: low key byte of a compacted slab (gs_slab.cu)
+       PASS_M1 = 5, PASS_M2 = 6, PASS_M3 = 7 };  // scene frames: bits 0-7, 8-15, 16-23 of the (rank, key) sort key
 
 struct RadixArgs {
   FrameCounters *ctr;
@@ -137,6 +288,10 @@ struct RadixArgs {
   // slab path: compacted (key, index) pairs of the current slab
   const uint16_t *ckey;
   const uint32_t *cidx;
+  // scene frames: M1 reads (skey, spay) and writes (idx_a, shi); M2 writes (spay, dig_a); M3 writes order
+  const uint32_t *skey;
+  uint32_t *spay;
+  uint16_t *shi;
   // frames of at most 256 bins: the bin id is one byte, pass T1 is the whole sort and gathers the records itself
   uint32_t t1_final;
   uint2 *bin_range;   // t1_final: the per-bin {start, end} fall out of the digit totals (no k_tile_ranges launch)
@@ -151,6 +306,8 @@ __device__ __forceinline__ uint32_t pass_n(const RadixArgs &a) {
   if (PASS == PASS_D1) return ctr->sort.n_valid ? a.fp->n_splats : 0u;
   if (PASS == PASS_D2) return ctr->sort.n_inrange;
   if (PASS == PASS_S1) return ctr->sort.n_valid;  // entries of the current slab (k_slab_begin)
+  if (PASS == PASS_M1) return ctr->sort.n_valid ? a.fp->n_splats : 0u;
+  if (PASS == PASS_M2 || PASS == PASS_M3) return ctr->sort.n_valid;  // every sorted entry, Q5 drops included
   if (PASS == PASS_T1) return ctr->overflow ? 0u : (uint32_t)ctr->n_inst;
   return ctr->overflow ? 0u : ctr->n_inst_kept;
 }
@@ -177,6 +334,17 @@ __device__ __forceinline__ void load_elem(const RadixArgs &a, uint32_t i, const 
   } else if (PASS == PASS_D2) {
     digit = a.dig_a[i];
     pay = a.idx_a[i];
+  } else if (PASS == PASS_M1) {
+    const uint32_t k = a.skey[i];
+    if (k != kNoKey) { digit = k & 255u; hi = k >> 8; pay = a.spay[i]; }
+  } else if (PASS == PASS_M2) {
+    const uint32_t h = a.shi[i];
+    digit = h & 255u;
+    hi = h >> 8;
+    pay = a.idx_a[i];
+  } else if (PASS == PASS_M3) {
+    digit = a.dig_a[i];
+    pay = a.spay[i];
   } else if (PASS == PASS_T1) {
     const uint16_t t = a.inst_tile[i];
     if (t != kNoTile) { digit = t & 255; hi = t; pay = a.inst_idx[i]; }
@@ -290,9 +458,10 @@ __global__ void __launch_bounds__(kScatThreads, 2) k_radix_scatter(RadixArgs a) 
   __shared__ uint32_t s_loc[256];     // slot of the digit's first element in the staged (locally sorted) chunk
   __shared__ uint32_t s_warp_tot[8];
   __shared__ uint32_t s_pay[kRadixTile];
-  // value carried to the next pass: D1 -> high key byte, T1/T2 -> the 16-bit tile id
-  using hi_t = typename std::conditional<(PASS == PASS_T1 || PASS == PASS_T2), uint16_t, uint8_t>::type;
-  __shared__ hi_t s_hi[(PASS == PASS_D2) ? 1 : kRadixTile];  // D1 / S1: high key byte
+  // value carried to the next pass: D1 -> high key byte, T1/T2 -> the 16-bit tile id, M1 -> key bits 8-23, M2 -> bits 16-23
+  using hi_t = typename std::conditional<(PASS == PASS_T1 || PASS == PASS_T2 || PASS == PASS_M1), uint16_t, uint8_t>::type;
+  constexpr bool kCarry = PASS != PASS_D2 && PASS != PASS_M3;  // the last pass of a sort carries nothing
+  __shared__ hi_t s_hi[kCarry ? kRadixTile : 1];  // D1 / S1: high key byte
   __shared__ uint8_t s_dig[kRadixTile];
   __shared__ uint32_t s_total;
   FrameCounters *ctr = a.ctr;
@@ -384,7 +553,7 @@ __global__ void __launch_bounds__(kScatThreads, 2) k_radix_scatter(RadixArgs a) 
       const uint32_t lp = s_loc[d] + wcnt[warp][d] + rank[s];
       s_pay[lp] = pay[s];
       s_dig[lp] = (uint8_t)d;
-      if (PASS != PASS_D2) s_hi[lp] = hi[s];
+      if (kCarry) s_hi[lp] = hi[s];
     }
     __syncthreads();
     // ---- write out: consecutive threads write consecutive slots of the same digit run (coalesced) ----
@@ -395,8 +564,14 @@ __global__ void __launch_bounds__(kScatThreads, 2) k_radix_scatter(RadixArgs a) 
       if (PASS == PASS_D1 || PASS == PASS_S1) {
         a.idx_a[pos] = p;
         a.dig_a[pos] = s_hi[i];
-      } else if (PASS == PASS_D2) {
+      } else if (PASS == PASS_D2 || PASS == PASS_M3) {
         a.order[pos] = p;
+      } else if (PASS == PASS_M1) {
+        a.idx_a[pos] = p;
+        a.shi[pos] = s_hi[i];
+      } else if (PASS == PASS_M2) {
+        a.spay[pos] = p;
+        a.dig_a[pos] = (uint8_t)s_hi[i];
       } else if (PASS == PASS_T1) {
         if (a.t1_final) {
           const float4 r0 = __ldg(a.proj_rec + 2 * (size_t)p);
@@ -446,6 +621,18 @@ void launch_depth_cull(gs_context *c, const FrameParams *fp, FrameCounters *ctr,
   launch_chain(c, k_depth_cull, grid, 256, st, c->center_scale, c->size_alpha, fp, c->depth, ctr);
 }
 
+void launch_depth_cull_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, ObjCounters *octr, FrameCounters *ctr,
+                             cudaStream_t st) {
+  const int grid = persistent_grid(c, c->cap, 256 * 4, 8);
+  launch_chain(c, k_depth_cull_scene, grid, 256, st, c->center_scale, c->size_alpha, fp, scene, c->depth, ctr, octr);
+}
+
+void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *scene, const ObjCounters *octr, FrameCounters *ctr,
+                       cudaStream_t st) {
+  const int grid = persistent_grid(c, c->cap, 256 * 4, 8);
+  launch_chain(c, k_scene_keys, grid, 256, st, (const float *)c->depth, fp, scene, octr, ctr, c->scene_key, c->scene_pay);
+}
+
 static RadixArgs make_args(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b) {
   RadixArgs a{};
   a.ctr = ctr;
@@ -480,6 +667,20 @@ void launch_depth_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr
   a.stride = c->table_n_stride;
   run_pass<PASS_D1>(c, a, c->cap, st);
   run_pass<PASS_D2>(c, a, c->cap, st);
+}
+
+// scene frames: (draw rank, key, index) as three stable 8-bit passes -> b.order (9 launches)
+void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
+  RadixArgs a = make_args(c, fp, ctr, b);
+  a.table = c->table_n;
+  a.totals = c->totals;
+  a.stride = c->table_n_stride;
+  a.skey = c->scene_key;
+  a.spay = c->scene_pay;
+  a.shi = c->scene_hi;
+  run_pass<PASS_M1>(c, a, c->cap, st);
+  run_pass<PASS_M2>(c, a, c->cap, st);
+  run_pass<PASS_M3>(c, a, c->cap, st);
 }
 
 void launch_tile_ranges(gs_context *c, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);

@@ -3,13 +3,14 @@ one GPU.  No computation happens here: numpy arrays are only the host buffers th
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional
+from dataclasses import dataclass
+from typing import Optional, Sequence
 
 import numpy as np
 
 from . import _lib
 from ._lib import (GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F, GS_RENDER_OUT_DEVICE, GS_RENDER_OUT_TILED,
-                   GS_RENDER_REUSE_SORT, GS_RENDER_STATS, GsRenderParams, GsStats)
+                   GS_RENDER_REUSE_SORT, GS_RENDER_STATS, GsObject, GsRenderParams, GsStats)
 from .scenes import FrameInputs
 
 
@@ -21,6 +22,28 @@ class GsError(RuntimeError):
 
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+@dataclass
+class SceneObject:
+    """One entity of a scene frame (gs_object): its splats [first, first+count) of the resident table, its
+    gsModelViewMatrix (16 f32, column-major; the sort uses row 2) and its worldToCutout or None."""
+    first: int
+    count: int
+    modelview: np.ndarray
+    cutout: Optional[np.ndarray] = None
+
+
+def make_objects(objects: Sequence[SceneObject]):
+    """ctypes array of gs_object, in draw order (objects[0] is drawn first, furthest back)."""
+    arr = (GsObject * max(1, len(objects)))()
+    for i, o in enumerate(objects):
+        arr[i].first, arr[i].count = int(o.first), int(o.count)
+        arr[i].modelview[:] = [float(x) for x in np.asarray(o.modelview, np.float32).reshape(16)]
+        if o.cutout is not None:
+            arr[i].has_cutout = 1
+            arr[i].cutout16[:] = [float(x) for x in np.asarray(o.cutout, np.float32).reshape(16)]
+    return arr
 
 
 class SplatContext:
@@ -141,6 +164,46 @@ class SplatContext:
         self._check(self._lib.gs_render(self._h, C.byref(p), _ptr(out), C.byref(st)))
         self.last_stats = st
         return out
+
+    def render_scene(self, frame: FrameInputs, objects: Sequence[SceneObject], bg=(0.0, 0.0, 0.0, 0.0),
+                     fmt: int = GS_FORMAT_RGBA8, color_in: Optional[np.ndarray] = None,
+                     depth_in: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None, stats: bool = False) -> np.ndarray:
+        """gs_render_scene: several entities in one frame, drawn whole in the order given, over `color_in` (the scene's
+        colour buffer, (H, W, 4) of the output dtype, row 0 = bottom; None = bg) and depth-tested against `depth_in`.
+        `frame` supplies projection, size and focal; its modelview and cutout are ignored."""
+        dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
+        if out is None:
+            out = np.empty((frame.height, frame.width, 4), dtype)
+        assert out.dtype == dtype and out.size == frame.height * frame.width * 4 and out.flags["C_CONTIGUOUS"]
+        col = None
+        if color_in is not None:
+            col = np.ascontiguousarray(color_in, dtype=dtype)
+            if col.size != frame.width * frame.height * 4:
+                raise ValueError("color_in must hold width*height RGBA pixels")
+        p = self.make_params(frame, bg, fmt, GS_RENDER_STATS if stats else 0, depth_in=depth_in)
+        objs = make_objects(objects)
+        st = GsStats()
+        self._check(self._lib.gs_render_scene(self._h, C.byref(p), objs, len(objects), _ptr(col), _ptr(out), C.byref(st)))
+        self.last_stats = st
+        return out
+
+    def render_scene_async(self, params: GsRenderParams, objects: Sequence[SceneObject], color_ptr: Optional[int],
+                           out_ptr: int) -> int:
+        """gs_render_scene_async: enqueue one scene frame (collected with wait()); color_ptr (host, or device with
+        GS_RENDER_COLOR_DEVICE in params.flags) and out_ptr must stay valid until the ticket is waited for."""
+        t = C.c_uint64()
+        self._check(self._lib.gs_render_scene_async(self._h, C.byref(params), make_objects(objects), len(objects),
+                                                    None if color_ptr is None else C.c_void_p(color_ptr),
+                                                    C.c_void_p(out_ptr), C.byref(t)))
+        return t.value
+
+    def sort_scene(self, objects: Sequence[SceneObject]) -> np.ndarray:
+        """gs_sort_scene: each entity's sortedIndexes (index.js:507-570 on its own range) + first, concatenated in
+        the order given."""
+        out = np.empty((max(1, self.num_splats),), np.uint32)
+        cnt = C.c_uint32()
+        self._check(self._lib.gs_sort_scene(self._h, make_objects(objects), len(objects), _ptr(out), C.byref(cnt)))
+        return out[:cnt.value].copy()
 
     def render_stereo(self, view: np.ndarray, eyes, cutout: Optional[np.ndarray] = None, bg=(0.0, 0.0, 0.0, 0.0),
                       fmt: int = GS_FORMAT_RGBA8):

@@ -2,6 +2,8 @@
 // addon a maintainer of the reference would add to bind include/gsplat_b200.h; see INTEGRATION.md.
 // bindings/node/gsplat_napi.cc  —  node-gyp: link -lgsplat_b200, include ../../include
 #include <napi.h>
+#include <cstring>
+#include <vector>
 #include "gsplat_b200.h"
 
 class Splats : public Napi::ObjectWrap<Splats> {
@@ -10,7 +12,8 @@ class Splats : public Napi::ObjectWrap<Splats> {
     exports.Set("Splats", DefineClass(env, "Splats", {
       InstanceMethod("clear", &Splats::Clear), InstanceMethod("push", &Splats::Push),
       InstanceMethod("reserve", &Splats::Reserve),
-      InstanceMethod("sort", &Splats::Sort),   InstanceMethod("render", &Splats::Render)}));
+      InstanceMethod("sort", &Splats::Sort),   InstanceMethod("render", &Splats::Render),
+      InstanceMethod("renderScene", &Splats::RenderScene)}));
     return exports;
   }
   explicit Splats(const Napi::CallbackInfo& i) : Napi::ObjectWrap<Splats>(i) {
@@ -54,6 +57,35 @@ class Splats : public Napi::ObjectWrap<Splats> {
     if (o.Has("depth")) p.depth_in = o.Get("depth").As<Napi::Float32Array>().Data();  // gl.readPixels(DEPTH) of the scene so far
     p.out_format = GS_FORMAT_RGBA8;
     Check(i.Env(), gs_render(ctx_, &p, i[1].As<Napi::Uint8Array>().Data(), nullptr));
+    return i.Env().Undefined();
+  }
+  // renderScene({proj, width, height, focal, depth?: Float32Array}, [{first, count, modelview, cutout?}, ...], Uint8Array color,
+  //             Uint8Array out)  <- the draws of every gaussian_splatting entity of the page, in DOM order (sortObjects false),
+  // over the opaque pass: color = gl.readPixels(RGBA, UNSIGNED_BYTE) and depth = the window-space depth buffer read back
+  // after the spheres and sky were drawn; each entity's {first, count} is its range of the shared table (pushed one
+  // entity after another), modelview its getModelViewMatrix(camera), cutout its worldToCutout.
+  Napi::Value RenderScene(const Napi::CallbackInfo& i) {
+    auto o = i[0].As<Napi::Object>();
+    gs_render_params p{};
+    memcpy(p.proj, o.Get("proj").As<Napi::Float32Array>().Data(), 64);
+    p.width = o.Get("width").As<Napi::Number>().Uint32Value();
+    p.height = o.Get("height").As<Napi::Number>().Uint32Value();
+    p.focal = o.Get("focal").As<Napi::Number>().FloatValue();
+    if (o.Has("depth")) p.depth_in = o.Get("depth").As<Napi::Float32Array>().Data();
+    p.out_format = GS_FORMAT_RGBA8;
+    auto list = i[1].As<Napi::Array>();
+    std::vector<gs_object> objs(list.Length());
+    for (uint32_t k = 0; k < list.Length(); ++k) {
+      auto e = list.Get(k).As<Napi::Object>();
+      gs_object& g = objs[k];
+      g = gs_object{};
+      g.first = e.Get("first").As<Napi::Number>().Uint32Value();
+      g.count = e.Get("count").As<Napi::Number>().Uint32Value();
+      memcpy(g.modelview, e.Get("modelview").As<Napi::Float32Array>().Data(), 64);
+      if (e.Has("cutout")) { g.has_cutout = 1; memcpy(g.cutout16, e.Get("cutout").As<Napi::Float32Array>().Data(), 64); }
+    }
+    const void* color = i[2].IsUndefined() ? nullptr : i[2].As<Napi::Uint8Array>().Data();
+    Check(i.Env(), gs_render_scene(ctx_, &p, objs.data(), (uint32_t)objs.size(), color, i[3].As<Napi::Uint8Array>().Data(), nullptr));
     return i.Env().Undefined();
   }
   gs_context* ctx_ = nullptr;

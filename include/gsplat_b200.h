@@ -67,7 +67,8 @@ enum {
   GS_RENDER_STATS = 1u << 4,      /* also fill the gs_stats fields marked (STATS): exact count of 16x16 tile
                                      instances and pixel-splat pair counters (a diagnostic frame: the raster
                                      keeps culling closed tiles' lists, so it is slower than a plain frame)  */
-  GS_RENDER_DEPTH_DEVICE = 1u << 5 /* gs_render_params.depth_in is a device pointer (default: host memory)  */
+  GS_RENDER_DEPTH_DEVICE = 1u << 5, /* gs_render_params.depth_in is a device pointer (default: host memory) */
+  GS_RENDER_COLOR_DEVICE = 1u << 6  /* gs_render_scene*: color_in is a device pointer (default: host memory)   */
 };
 
 /* Per-frame counters (SURVEY.md 8d symbols) and device timings of the last gs_sort/gs_render */
@@ -216,6 +217,53 @@ GS_API int gs_wait(gs_context *ctx, uint64_t ticket, gs_stats *stats);
  */
 GS_API int gs_render_stereo(gs_context *ctx, const float view[4], const float *cutout16_or_null,
                             const gs_render_params eyes[2], void *const out_rgba[2], gs_stats *stats2_or_null);
+
+/* ---- scenes: several gaussian_splatting entities in one frame, over the scene's colour + depth ------ */
+
+/*
+ * A page holds one mesh per entity, drawn into a target that already holds the rest of the scene (index.js:177-181:
+ * transparent, depthTest true, depthWrite false).  The reference's rules, restated:
+ *   - one worker per entity (index.js:229-236) with its own sort (tick(), index.js:438-455): its own `view` row, cutout
+ *     and min/max depth, hence its own 16-bit key space.  Quirk Q5 acts per entity: the dropped slots stay 0, i.e. the
+ *     entity-local splat 0 is drawn again - in a shared table, the entity's FIRST splat;
+ *   - projection, viewport and focal are shared by the draw (index.js:184-195); gsModelViewMatrix is per entity;
+ *   - each entity is drawn whole, back to front in its own order, over what the previous entities left: entities do
+ *     not interleave by depth and, writing no depth, never occlude each other; each depth-tests against depth_in;
+ *   - draw order: A-Frame 1.4's renderer system sets three.js sortObjects to false, so transparent meshes are drawn in
+ *     scene-graph (DOM) order (recalled from the three.js / A-Frame sources, not verifiable in this image; see SURVEY.md
+ *     A.1).  The library takes the order from the caller (objs[0] first, i.e. furthest back) and imposes none.
+ */
+#define GS_MAX_OBJECTS 64
+typedef struct gs_object {
+  uint32_t first, count;   /* the entity's splats: [first, first+count) of the resident table (count 0: still loading) */
+  float modelview[16];     /* its getModelViewMatrix() (index.js:467-487); view = row 2 (index.js:442)               */
+  int32_t has_cutout;
+  float cutout16[16];      /* its worldToCutout (index.js:443-448)                                                   */
+} gs_object;
+
+/*
+ * One frame of n_objs entities (1..GS_MAX_OBJECTS), collected with gs_wait like gs_render_async.
+ * frame: projection, size, focal, bg_rgba, out_format, flags and depth_in of the draw; its modelview / cutout are
+ * ignored.  Splats outside every range are not drawn.  Ranges must not overlap and must lie within the splats resident
+ * at submission; GS_RENDER_REUSE_SORT is not accepted (GS_ERR_INVALID).
+ * color_in: NULL (the blend starts from bg_rgba) or width*height pixels of the output's element type (u8 RGBA8 /
+ * f32 RGBA32F), row 0 = bottom: each pixel is the destination of the blend, C = sum c*a*T + dst*T_end,
+ * A = 1 - T_end + dst.a*T_end, an RGBA8 destination read as byte/255 in fp32.  Host memory unless
+ * GS_RENDER_COLOR_DEVICE; a host buffer is staged per frame and must stay valid until gs_wait.
+ * One entity spanning the whole table is exactly gs_render_async (same kernels, one-pass or slab path) plus color_in.
+ * Any other scene is rendered in one pass (no depth slabs) and leaves no single-entity order behind: a following
+ * GS_RENDER_REUSE_SORT frame sorts again.
+ */
+GS_API int gs_render_scene_async(gs_context *ctx, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                                 const void *color_in, void *out_rgba, uint64_t *out_ticket);
+GS_API int gs_render_scene(gs_context *ctx, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                           const void *color_in, void *out_rgba, gs_stats *stats);
+/*
+ * Draw order of such a frame: each entity's reference sortedIndexes (index.js:507-570 run on its own range, Q5 tail
+ * included), offset by `first` and concatenated in the order of objs.  out_idx: host, capacity gs_num_splats (or NULL);
+ * *out_count = its length.
+ */
+GS_API int gs_sort_scene(gs_context *ctx, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx, uint32_t *out_count);
 
 /* Per-splat projected record of the last gs_render (testing the vertex-shader restatement):
  * 8 floats per resident splat {cx, cy, a1x, a1y, a2x, a2y, rgba8-as-bits, tile-rect-as-bits};
