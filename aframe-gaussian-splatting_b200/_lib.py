@@ -58,6 +58,7 @@ SYMBOLS = {
     "gs_bin_size": (C.c_uint32, []),
     "gs_clear": (C.c_int, [_P]),
     "gs_push_splats": (C.c_int, [_P, _P, C.c_uint32]),
+    "gs_push_ply": (C.c_int, [_P, _P, C.c_size_t, _P, C.POINTER(C.c_uint32)]),
     "gs_reserve": (C.c_int, [_P, C.c_uint32]),
     "gs_push_packed": (C.c_int, [_P, _P, _P, _P, C.c_uint32]),
     "gs_num_splats": (C.c_int, [_P, C.POINTER(C.c_uint32)]),

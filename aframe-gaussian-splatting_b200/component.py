@@ -62,6 +62,10 @@ class SortWorker:
             return reply
         return None  # unknown methods are ignored, as in the reference
 
+    def push_ply(self, blob) -> int:
+        """processPlyBuffer + the push of its rows (index.js:315-324), both on the device (gs_push_ply)."""
+        return self.ctx.push_ply(blob)
+
 
 class GaussianSplattingComponent:
     """`gaussian_splatting` (index.js:1-746) for the sort + draw path."""
@@ -123,9 +127,14 @@ class GaussianSplattingComponent:
             with open(os.fspath(src), "rb") as f:
                 buf = np.frombuffer(f.read(), dtype=np.uint8)
         if is_ply:
-            # a .ply is converted first and sized afterwards, the reference's path when no Content-Length is known
-            # (index.js:315-323); sizing from the raw byte count (index.js:249-250) would over-reserve 248/32 x (Q11)
-            buf = np.frombuffer(self.processPlyBuffer(buf.tobytes()), dtype=np.uint8)  # index.js:315-317
+            # index.js:315-324: the whole file is converted (processPlyBuffer) and its rows pushed at once.  The device
+            # decodes, importance-sorts and packs it (gs_push_ply); the table is sized from the header's vertex count,
+            # not from the raw byte count (index.js:249-250 would over-reserve 248/32 x, Q11).
+            n = self.worker.push_ply(buf)
+            self.sortReady = True  # what initGL does (index.js:220)
+            self.loadedVertexCount += n
+            self._have_order = False
+            return
         self.initGL(len(buf) // self.rowLength)  # index.js:249-250 / 320-323
         # progressive push in chunks, whole rows only (index.js:279-298); a trailing partial row is dropped
         n_rows = len(buf) // self.rowLength
@@ -256,6 +265,9 @@ class _EntityWorker(SortWorker):
             return reply
         return None
 
+    def push_ply(self, blob) -> int:
+        return self.scene._push_ply(self.component, blob)
+
 
 class SplatScene:
     """Several `gaussian_splatting` entities of one page drawn into one frame from one GPU context.
@@ -299,6 +311,19 @@ class SplatScene:
         self.renderer.push_splats(rows)
         self._rows[id(component)].append(rows.copy())
         self._range[id(component)][1] = count + rows.shape[0]
+
+    def _push_ply(self, component, blob) -> int:
+        """A .ply entity: converted and pushed on the device; its rows come back (rows32_out) and are kept like pushed
+        rows, so that a later clear of another entity can push them again."""
+        first, count = self._range[id(component)]
+        if first + count != self.renderer.num_splats:
+            self._clear_entity(component, keep_rows=True)
+            first, count = self._range[id(component)]
+        n, rows = self.renderer.push_ply(blob, return_rows=True)
+        if n:
+            self._rows[id(component)].append(rows)
+        self._range[id(component)][1] = count + n
+        return n
 
     def _clear_entity(self, component, keep_rows: bool = False) -> None:
         """Drop the entity's splats (keep_rows: move them to the end of the table instead) and repack the others."""

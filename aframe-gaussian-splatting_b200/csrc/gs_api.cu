@@ -1,7 +1,7 @@
 // gs_api.cu — the C ABI of include/gsplat_b200.h: context lifetime, the worker protocol
 // (clear / push / sort, reference index.js:572-598) and the draw (index.js:184-207 + shaders).
 // Host code only orchestrates: every per-splat / per-pixel operation runs in the CUDA kernels of
-// gs_sort.cu, gs_pack.cu, gs_project.cu and gs_raster.cu.  There is no CPU fallback.
+// gs_sort.cu, gs_pack.cu, gs_ply.cu, gs_project.cu and gs_raster.cu.  There is no CPU fallback.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -339,6 +339,10 @@ extern "C" int gs_destroy(gs_context *c) {
     if (c->push_ev[i]) cudaEventDestroy(c->push_ev[i]);
   }
   if (c->push_done) cudaEventDestroy(c->push_done);
+  for (int i = 0; i < 2; ++i) {
+    if (c->ply_pinned[i]) cudaFreeHost(c->ply_pinned[i]);
+    if (c->ply_ev[i]) cudaEventDestroy(c->ply_ev[i]);
+  }
   if (c->push_stream) cudaStreamDestroy(c->push_stream);
   drop_graphs(c);
   for (uint32_t r = 0; r < c->peer_world; ++r)
@@ -450,6 +454,88 @@ extern "C" int gs_push_splats(gs_context *c, const void *rows32, uint32_t n) {
   c->n += n;
   c->pushed = true;
   c->have_order = false;
+  return GS_OK;
+}
+
+// pinned staging of the PLY path, created on first use
+static int ensure_ply_staging(gs_context *c) {
+  for (int i = 0; i < 2; ++i) {
+    if (!c->ply_pinned[i]) GS_CUDA(c, cudaHostAlloc(&c->ply_pinned[i], gs_context::kPlyChunkBytes, cudaHostAllocDefault));
+    if (!c->ply_ev[i]) GS_CUDA(c, cudaEventCreateWithFlags(&c->ply_ev[i], cudaEventDisableTiming));
+  }
+  return GS_OK;
+}
+
+// processPlyBuffer + one pushDataBuffer on the device (gs_ply.cu).  Same contract as gs_push_splats: frames in flight keep
+// drawing the old prefix, the caller's file is consumed on return, only a push that outgrows the table waits.
+extern "C" int gs_push_ply(gs_context *c, const void *ply, size_t bytes, void *rows32_out_or_null, uint32_t *out_n) {
+  if (!c || (!ply && bytes)) return GS_ERR_INVALID;
+  if (out_n) *out_n = 0;
+  PlyLayout L;
+  uint32_t n = 0;
+  size_t data_off = 0;
+  if (ply_parse((const uint8_t *)ply, bytes, L, n, data_off, c->err)) return GS_ERR_INVALID;  // nothing changed yet
+  if (!n) return GS_OK;
+  GS_CUDA(c, cudaSetDevice(c->device));
+  int rc;
+  if ((rc = ensure_table(c, (uint64_t)c->n + n))) return rc;  // the header gave the count: one growth, up front
+  if ((rc = ensure_ply_staging(c))) return rc;
+  cudaStream_t st = c->push_stream;
+  // temporaries, stream-ordered: decoded rows (32 B) + key per row, two permutations, radix tables, ordered rows
+  const uint32_t chunks = (n + kRadixTile - 1) / kRadixTile;
+  const size_t stride = L.stride, rows_per_chunk = gs_context::kPlyChunkBytes / stride;
+  uint8_t *rows_dev = nullptr, *out_dev = nullptr, *body[2] = {nullptr, nullptr};
+  uint32_t *key = nullptr, *perm_a = nullptr, *perm_b = nullptr, *table = nullptr, *totals = nullptr;
+  auto release = [&]() {
+    void *ps[] = {rows_dev, out_dev, body[0], body[1], key, perm_a, perm_b, table, totals};
+    for (void *p : ps)
+      if (p) cudaFreeAsync(p, st);
+  };
+  cudaError_t e = cudaSuccess;
+  const bool sort = L.has_scale && n > 1;  // without scale_0 every key is 0: the stable sort is the identity
+  e = cudaMallocAsync((void **)&rows_dev, (size_t)n * 32, st);
+  if (!e) e = cudaMallocAsync((void **)&key, (size_t)n * 4, st);
+  for (int i = 0; i < 2 && !e; ++i) e = cudaMallocAsync((void **)&body[i], rows_per_chunk * stride, st);
+  if (!e && sort) e = cudaMallocAsync((void **)&perm_a, (size_t)n * 4, st);
+  if (!e && sort) e = cudaMallocAsync((void **)&perm_b, (size_t)n * 4, st);
+  if (!e && sort) e = cudaMallocAsync((void **)&table, (size_t)256 * (chunks + 1) * 4, st);
+  if (!e && sort) e = cudaMallocAsync((void **)&totals, (size_t)256 * 4, st);
+  if (!e && rows32_out_or_null) e = cudaMallocAsync((void **)&out_dev, (size_t)n * 32, st);
+  if (e) {
+    release();
+    GS_CUDA(c, e);
+  }
+  // the body crosses in whole-row chunks through the two pinned buffers: the host copy of chunk k+1 overlaps the DMA and
+  // decode of chunk k, and no row straddles two chunks
+  const uint8_t *src = (const uint8_t *)ply + data_off;
+  for (uint32_t r0 = 0, k = 0; r0 < n && !e; r0 += (uint32_t)rows_per_chunk, ++k) {
+    const uint32_t m = (uint32_t)std::min<size_t>(rows_per_chunk, n - r0);
+    const int b = (int)(k & 1u);
+    if ((e = cudaEventSynchronize(c->ply_ev[b]))) break;  // this pinned buffer's previous chunk is on the device
+    memcpy(c->ply_pinned[b], src + (size_t)r0 * stride, (size_t)m * stride);
+    if ((e = cudaMemcpyAsync(body[b], c->ply_pinned[b], (size_t)m * stride, cudaMemcpyHostToDevice, st))) break;
+    if ((e = cudaEventRecord(c->ply_ev[b], st))) break;
+    launch_ply_decode(body[b], m, L, r0, rows_dev, key, st);
+    e = cudaGetLastError();
+  }
+  const uint32_t *perm = nullptr;
+  if (!e && sort) {
+    perm = launch_ply_sort(c, key, perm_a, perm_b, table, totals, n, st);
+    e = cudaGetLastError();
+  }
+  if (!e) {
+    launch_pack_perm(c, rows_dev, perm, c->n, n, out_dev, st);
+    e = cudaGetLastError();
+  }
+  if (!e && rows32_out_or_null) e = cudaMemcpyAsync(rows32_out_or_null, out_dev, (size_t)n * 32, cudaMemcpyDeviceToHost, st);
+  release();
+  if (!e && rows32_out_or_null) e = cudaStreamSynchronize(st);
+  GS_CUDA(c, e);
+  GS_CUDA(c, cudaEventRecord(c->push_done, st));
+  c->n += n;
+  c->pushed = true;
+  c->have_order = false;
+  if (out_n) *out_n = n;
   return GS_OK;
 }
 

@@ -151,8 +151,24 @@ __device__ __forceinline__ int scene_find(const uint32_t *s_first, const uint32_
   return (lo > 0 && i < s_end[lo - 1]) ? (int)lo - 1 : -1;
 }
 
+// ---- PLY ingest (gs_ply.cu, processPlyBuffer index.js:600-745): the header is parsed on the host; only the offset and
+// type of the fields the conversion reads go to the device ----
+enum { PK_F64 = 0, PK_I32, PK_U32, PK_F32, PK_I16, PK_U16, PK_U8, PK_I8, PK_ABSENT = -1 };  // index.js:613-621 TYPE_MAP
+enum { PF_X = 0, PF_Y, PF_Z, PF_S0, PF_S1, PF_S2, PF_R0, PF_R1, PF_R2, PF_R3, PF_OP, PF_DC0, PF_DC1, PF_DC2, PF_RED, PF_GREEN,
+       PF_BLUE, PF_COUNT };
+struct PlyField { int32_t off, kind; };
+struct PlyLayout {
+  uint32_t stride;                            // bytes per row: every property's size, summed (index.js:630)
+  uint32_t has_scale, has_fdc, has_opacity;   // types["scale_0"] / types["f_dc_0"] / types["opacity"] (index.js:660,722,733)
+  uint32_t all_f32;                           // every field read is a 4-byte-aligned float and the stride is a multiple of 4
+  PlyField f[PF_COUNT];                       // the LAST property of each name (offsets[name] is overwritten, index.js:628-629)
+};
+// Parses the header of a whole PLY file with the reference's rules.  Returns GS_OK, or GS_ERR_INVALID with `err` set to the
+// reference's message (header, missing property, short body).
+int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_t &data_off, std::string &err);
+
 // ---- front-to-back slab path ----
-constexpr int kMaxSlabs = 12;          // geometric slab sizes: 1 M, 2 M, 4 M ... entries (nearest first)
+constexpr int kMaxSlabs = 12;         // geometric slab sizes: 1 M, 2 M, 4 M ... entries (nearest first)
 constexpr int kSlabBuckets = 4096;     // slab boundaries are chosen on a 4096-bucket histogram of the 16-bit keys
 constexpr uint32_t kNoKey = 0xFFFFFFFFu;
 struct SlabTable {
@@ -317,6 +333,11 @@ struct gs_context {
   cudaEvent_t push_done = nullptr;                  // everything pushed so far is packed
   int push_buf = 0;
   bool pushed = false;
+  // ---- PLY push (gs_push_ply): the file body crosses in whole-row chunks through two pinned buffers, created on first
+  // use; every other buffer of a PLY push is allocated and freed stream-ordered on push_stream ----
+  static constexpr size_t kPlyChunkBytes = (size_t)16 << 20;
+  void *ply_pinned[2] = {nullptr, nullptr};
+  cudaEvent_t ply_ev[2] = {nullptr, nullptr};      // pinned buffer i has been copied to the device
   cudaStream_t aux_stream = nullptr;             // runs k_project beside the depth radix passes
   cudaEvent_t ev_fork[2]{}, ev_join[2]{};
   bool use_graphs = true;
@@ -368,6 +389,16 @@ void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr
 void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
                           const FrameBufs &b, cudaStream_t st);
 void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_t n, cudaStream_t st);
+// PLY push: k_pack reading row perm[j] (perm NULL: row j) into slot first + j; rows_out (or NULL) receives the ordered rows
+void launch_pack_perm(gs_context *c, const uint8_t *rows_dev, const uint32_t *perm, uint32_t first, uint32_t n,
+                      uint8_t *rows_out, cudaStream_t st);
+// PLY push: decode `rows` whole rows of a staged body chunk into .splat rows + importance keys at [first_row, ...)
+void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,
+                       uint32_t *key, cudaStream_t st);
+// PLY push: stable ascending sort of n 32-bit keys as four 8-bit passes (12 launches); returns the buffer holding the
+// permutation (perm_b).  table: 256 * (ceil(n / kRadixTile) + 1) words, totals: 256 words.
+uint32_t *launch_ply_sort(gs_context *c, const uint32_t *key, uint32_t *perm_a, uint32_t *perm_b, uint32_t *table,
+                          uint32_t *totals, uint32_t n, cudaStream_t st);
 void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
 void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 2 launches
 void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, bool hist_t1, cudaStream_t st);  // 2 .. 7 launches

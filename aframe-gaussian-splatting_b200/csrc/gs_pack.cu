@@ -1,4 +1,7 @@
 // gs_pack.cu — load-time pack on the device: the reference's `pushDataBuffer` loop (index.js:343-402).
+//   k_pack      : row i of a staged chunk -> table slot first + i (gs_push_splats)
+//   k_pack_perm : row perm[j] of the decoded PLY rows -> slot first + j, optionally also written out in that order
+//                 (gs_push_ply: the gather of processPlyBuffer's importance order fused with the pack)
 //
 // One thread per .splat row, all arithmetic in fp64 exactly as JavaScript evaluates it (Three.js r147
 // Matrix4.compose / transpose / scale / premultiply restated entry by entry, sums left to right, no FMA):
@@ -48,13 +51,10 @@ __device__ __forceinline__ int16_t parse_int_to_i16(double x, const double *__re
   return (int16_t)(uint16_t)((uint32_t)to_int32_wrap(r) & 0xFFFFu);
 }
 
-__global__ void __launch_bounds__(256) k_pack(const uint4 *__restrict__ rows, uint32_t first, uint32_t n,
-                                              float4 *__restrict__ cs, uint4 *__restrict__ cc,
-                                              float *__restrict__ sa, const double *__restrict__ tab, int nt) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint4 a = __ldg(rows + 2 * (size_t)i);      // pos.xyz, scale.x
-  const uint4 b = __ldg(rows + 2 * (size_t)i + 1);  // scale.yz, rgba, rot
+// one .splat row (a = pos.xyz, scale.x; b = scale.yz, rgba, rot) -> table slot o
+__device__ __forceinline__ void pack_row(const uint4 a, const uint4 b, const size_t o, float4 *__restrict__ cs,
+                                         uint4 *__restrict__ cc, float *__restrict__ sa, const double *__restrict__ tab,
+                                         int nt) {
   const double px = __uint_as_float(a.x), py = __uint_as_float(a.y), pz = __uint_as_float(a.z);
   const double sx = __uint_as_float(a.w), sy = __uint_as_float(b.x), sz = __uint_as_float(b.y);
   const uint32_t rgba = b.z, rot = b.w;
@@ -95,7 +95,6 @@ __global__ void __launch_bounds__(256) k_pack(const uint4 *__restrict__ rows, ui
   if (fabs(e6) > mx) mx = fabs(e6);
   if (fabs(e10) > mx) mx = fabs(e10);
   // index.js:378-382
-  const size_t o = (size_t)first + i;
   cs[o] = make_float4((float)px, (float)py, (float)(-pz), (float)__ddiv_rn(mx, 32767.0));
   // index.js:384-394
   const uint32_t c0 = (uint16_t)parse_int_to_i16(__ddiv_rn(__dmul_rn(e0, 32767.0), mx), tab, nt);
@@ -113,11 +112,47 @@ __global__ void __launch_bounds__(256) k_pack(const uint4 *__restrict__ rows, ui
   sa[o] = (float)__ddiv_rn(__dmul_rn(ms, (double)(rgba >> 24)), 255.0);
 }
 
+__global__ void __launch_bounds__(256) k_pack(const uint4 *__restrict__ rows, uint32_t first, uint32_t n,
+                                              float4 *__restrict__ cs, uint4 *__restrict__ cc,
+                                              float *__restrict__ sa, const double *__restrict__ tab, int nt) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint4 a = __ldg(rows + 2 * (size_t)i);      // pos.xyz, scale.x
+  const uint4 b = __ldg(rows + 2 * (size_t)i + 1);  // scale.yz, rgba, rot
+  pack_row(a, b, (size_t)first + i, cs, cc, sa, tab, nt);
+}
+
+// PLY push: the gather of processPlyBuffer's output order (index.js:680-681: row = sizeIndex[j]) fused with the pack.
+// Slot first + j takes row perm[j] (perm NULL: row j); rows_out, when given, receives that row as the j-th .splat row.
+__global__ void __launch_bounds__(256) k_pack_perm(const uint4 *__restrict__ rows, const uint32_t *__restrict__ perm,
+                                                   uint32_t first, uint32_t n, float4 *__restrict__ cs,
+                                                   uint4 *__restrict__ cc, float *__restrict__ sa,
+                                                   const double *__restrict__ tab, int nt, uint4 *__restrict__ rows_out) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint32_t r = perm ? __ldg(perm + j) : j;
+  const uint4 a = __ldg(rows + 2 * (size_t)r);
+  const uint4 b = __ldg(rows + 2 * (size_t)r + 1);
+  if (rows_out) {
+    rows_out[2 * (size_t)j] = a;
+    rows_out[2 * (size_t)j + 1] = b;
+  }
+  pack_row(a, b, (size_t)first + j, cs, cc, sa, tab, nt);
+}
+
 void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_t n, cudaStream_t st) {
   if (!n) return;
   const uint32_t grid = (n + 255) / 256;
   k_pack<<<grid, 256, 0, st>>>((const uint4 *)rows_dev, first, n, c->center_scale, c->cov_color, c->size_alpha,
                                       c->quirk_table, c->quirk_n);
+}
+
+void launch_pack_perm(gs_context *c, const uint8_t *rows_dev, const uint32_t *perm, uint32_t first, uint32_t n,
+                      uint8_t *rows_out, cudaStream_t st) {
+  if (!n) return;
+  const uint32_t grid = (n + 255) / 256;
+  k_pack_perm<<<grid, 256, 0, st>>>((const uint4 *)rows_dev, perm, first, n, c->center_scale, c->cov_color, c->size_alpha,
+                                    c->quirk_table, c->quirk_n, (uint4 *)rows_out);
 }
 
 }  // namespace gs

@@ -20,6 +20,10 @@
 //   k_radix_*<M1/M2/M3>: three stable 8-bit passes -> (rank, key, index) order = each entity's sortedIndexes + first,
 //                        concatenated in draw order
 //
+// PLY ingest (gs_push_ply): k_radix_*<P1..P4> sort the rows by a 32-bit importance key, four stable 8-bit passes (the
+// stable Array.prototype.sort of index.js:668).  Each pass reads the digit through the permutation (key[perm[i]]), so
+// nothing but the row index is carried.
+//
 // Bit-exactness: JS evaluates in fp64 with IEEE rounding after every operation; the kernels use
 // __dmul_rn/__dadd_rn so nothing is contracted, and ToInt32 is restated exactly (js_to_int32).
 #include <type_traits>
@@ -264,7 +268,8 @@ __global__ void __launch_bounds__(256) k_scene_keys(const float *__restrict__ de
 // T2's scatter gathers the 32 B projected record of each instance into its final per-tile slot.
 // ---------------------------------------------------------------------------------------------
 enum { PASS_D1 = 0, PASS_D2 = 1, PASS_T1 = 2, PASS_T2 = 3, PASS_S1 = 4,  // S1: low key byte of a compacted slab (gs_slab.cu)
-       PASS_M1 = 5, PASS_M2 = 6, PASS_M3 = 7 };  // scene frames: bits 0-7, 8-15, 16-23 of the (rank, key) sort key
+       PASS_M1 = 5, PASS_M2 = 6, PASS_M3 = 7,  // scene frames: bits 0-7, 8-15, 16-23 of the (rank, key) sort key
+       PASS_P1 = 8, PASS_P2 = 9, PASS_P3 = 10, PASS_P4 = 11 };  // PLY ingest: bits 0-7 .. 24-31 of the importance key
 
 struct RadixArgs {
   FrameCounters *ctr;
@@ -298,10 +303,16 @@ struct RadixArgs {
   uint32_t n_bins;
   uint32_t t1_chunk_cols;  // T1's histogram columns: 0 = one per 2048-instance window (produced by k_emit),
                            // 1 = one per 4096-element chunk (k_radix_hist<T1>, slab path)
+  // PLY ingest: pn keys, the permutation of the previous pass (P2..P4) and this pass's output
+  const uint32_t *pkey;
+  const uint32_t *pin;
+  uint32_t *pout;
+  uint32_t pn;
 };
 
 template <int PASS>
 __device__ __forceinline__ uint32_t pass_n(const RadixArgs &a) {
+  if (PASS >= PASS_P1) return a.pn;
   const FrameCounters *ctr = a.ctr;
   if (PASS == PASS_D1) return ctr->sort.n_valid ? a.fp->n_splats : 0u;
   if (PASS == PASS_D2) return ctr->sort.n_inrange;
@@ -345,6 +356,10 @@ __device__ __forceinline__ void load_elem(const RadixArgs &a, uint32_t i, const 
   } else if (PASS == PASS_M3) {
     digit = a.dig_a[i];
     pay = a.spay[i];
+  } else if (PASS >= PASS_P1) {
+    const uint32_t p = PASS == PASS_P1 ? i : a.pin[i];
+    digit = (__ldg(a.pkey + p) >> (8 * (PASS - PASS_P1))) & 255u;
+    pay = p;
   } else if (PASS == PASS_T1) {
     const uint16_t t = a.inst_tile[i];
     if (t != kNoTile) { digit = t & 255; hi = t; pay = a.inst_idx[i]; }
@@ -460,7 +475,7 @@ __global__ void __launch_bounds__(kScatThreads, 2) k_radix_scatter(RadixArgs a) 
   __shared__ uint32_t s_pay[kRadixTile];
   // value carried to the next pass: D1 -> high key byte, T1/T2 -> the 16-bit tile id, M1 -> key bits 8-23, M2 -> bits 16-23
   using hi_t = typename std::conditional<(PASS == PASS_T1 || PASS == PASS_T2 || PASS == PASS_M1), uint16_t, uint8_t>::type;
-  constexpr bool kCarry = PASS != PASS_D2 && PASS != PASS_M3;  // the last pass of a sort carries nothing
+  constexpr bool kCarry = PASS != PASS_D2 && PASS != PASS_M3 && PASS < PASS_P1;  // the last pass of a sort (and P) carries nothing
   __shared__ hi_t s_hi[kCarry ? kRadixTile : 1];  // D1 / S1: high key byte
   __shared__ uint8_t s_dig[kRadixTile];
   __shared__ uint32_t s_total;
@@ -572,6 +587,8 @@ __global__ void __launch_bounds__(kScatThreads, 2) k_radix_scatter(RadixArgs a) 
       } else if (PASS == PASS_M2) {
         a.spay[pos] = p;
         a.dig_a[pos] = (uint8_t)s_hi[i];
+      } else if (PASS >= PASS_P1) {
+        a.pout[pos] = p;
       } else if (PASS == PASS_T1) {
         if (a.t1_final) {
           const float4 r0 = __ldg(a.proj_rec + 2 * (size_t)p);
@@ -717,6 +734,26 @@ void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, 
   launch_chain(c, k_radix_scan<PASS_S1>, 256, 256, st, a);
   launch_chain(c, k_radix_scatter<PASS_S1>, grid, kScatThreads, st, a);
   run_pass<PASS_D2>(c, a, c->cap, st);
+}
+
+// PLY ingest: stable ascending sort of n 32-bit keys, four 8-bit passes (12 launches) on the caller's scratch -> perm_b
+uint32_t *launch_ply_sort(gs_context *c, const uint32_t *key, uint32_t *perm_a, uint32_t *perm_b, uint32_t *table,
+                          uint32_t *totals, uint32_t n, cudaStream_t st) {
+  RadixArgs a{};
+  a.table = table;
+  a.totals = totals;
+  a.stride = (n + kRadixTile - 1) / kRadixTile + 1;
+  a.pkey = key;
+  a.pn = n;
+  a.pout = perm_a;
+  run_pass<PASS_P1>(c, a, n, st);
+  a.pin = perm_a; a.pout = perm_b;
+  run_pass<PASS_P2>(c, a, n, st);
+  a.pin = perm_b; a.pout = perm_a;
+  run_pass<PASS_P3>(c, a, n, st);
+  a.pin = perm_a; a.pout = perm_b;
+  run_pass<PASS_P4>(c, a, n, st);
+  return perm_b;
 }
 
 void launch_tile_ranges(gs_context *c, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {

@@ -1,7 +1,7 @@
 """PLY ingest: host-side restatement of `processPlyBuffer` (reference index.js:600-745).
 
-Load-time, CPU-side work in the reference too (it runs on the main thread before the first push), so it
-stays on the host here: one vectorised numpy pass instead of a per-row DataView Proxy.  Semantics kept:
+Loads go through the device path (`gs_push_ply`, csrc/gs_ply.cu); this numpy pass is what the component's mirrored
+`processPlyBuffer` returns and the host reference the tests check the device rows against.  Semantics kept:
 10 KB ASCII header window, `element vertex N`, little-endian property table (unknown types read as 1-byte
 ints), importance = exp(s0)*exp(s1)*exp(s2)*sigmoid(opacity) stored as f32, rows emitted in descending
 importance (stable), Uint8ClampedArray stores (clamp, round half to even, NaN -> 0).

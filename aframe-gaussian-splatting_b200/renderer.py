@@ -3,6 +3,7 @@ one GPU.  No computation happens here: numpy arrays are only the host buffers th
 from __future__ import annotations
 
 import ctypes as C
+import re
 from dataclasses import dataclass
 from typing import Optional, Sequence
 
@@ -93,6 +94,23 @@ class SplatContext:
         """rows: (n, 32) uint8 raw .splat rows (pushDataBuffer, index.js:328)."""
         rows = np.ascontiguousarray(rows, dtype=np.uint8).reshape(-1, 32)
         self._check(self._lib.gs_push_splats(self._h, _ptr(rows), rows.shape[0]))
+
+    def push_ply(self, blob, return_rows: bool = False):
+        """gs_push_ply: processPlyBuffer + pushDataBuffer (index.js:315-324, 600-745) of a whole binary .ply file on the
+        device.  Returns the vertex count n, or (n, rows) with rows the (n, 32) uint8 .splat rows processPlyBuffer
+        returns.  A malformed file raises GsError (GS_ERR_INVALID) with the reference's message."""
+        buf = np.frombuffer(memoryview(blob), dtype=np.uint8)
+        rows = None
+        if return_rows:
+            # the header's `element vertex N` (index.js:608) sizes the output; a file the call refuses writes nothing, and
+            # every row takes at least one byte of the file, so a count above the file size is refused
+            m = re.search(rb"element vertex (\d+)\n", buf[:10240].tobytes())
+            rows = np.empty((min(int(m.group(1)), buf.size) if m else 0, 32), np.uint8)
+        n = C.c_uint32()
+        self._check(self._lib.gs_push_ply(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, _ptr(rows), C.byref(n)))
+        if return_rows:
+            return n.value, rows[:n.value]
+        return n.value
 
     def push_packed(self, center_scale: np.ndarray, cov_color: np.ndarray, size_alpha: np.ndarray) -> None:
         cs = np.ascontiguousarray(center_scale, dtype=np.float32).reshape(-1, 4)

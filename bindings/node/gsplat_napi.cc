@@ -11,7 +11,7 @@ class Splats : public Napi::ObjectWrap<Splats> {
   static Napi::Object Init(Napi::Env env, Napi::Object exports) {
     exports.Set("Splats", DefineClass(env, "Splats", {
       InstanceMethod("clear", &Splats::Clear), InstanceMethod("push", &Splats::Push),
-      InstanceMethod("reserve", &Splats::Reserve),
+      InstanceMethod("pushPly", &Splats::PushPly), InstanceMethod("reserve", &Splats::Reserve),
       InstanceMethod("sort", &Splats::Sort),   InstanceMethod("render", &Splats::Render),
       InstanceMethod("renderScene", &Splats::RenderScene)}));
     return exports;
@@ -34,6 +34,13 @@ class Splats : public Napi::ObjectWrap<Splats> {
     auto buf = i[0].As<Napi::ArrayBuffer>();
     Check(i.Env(), gs_push_splats(ctx_, buf.Data(), i[1].As<Napi::Number>().Uint32Value()));
     return i.Env().Undefined();
+  }
+  // pushPly(ArrayBuffer plyFile) -> vertexCount    <- processPlyBuffer + pushDataBuffer, index.js:315-324, 600-745
+  Napi::Value PushPly(const Napi::CallbackInfo& i) {
+    auto buf = i[0].As<Napi::ArrayBuffer>();
+    uint32_t n = 0;
+    Check(i.Env(), gs_push_ply(ctx_, buf.Data(), buf.ByteLength(), nullptr, &n));
+    return Napi::Number::New(i.Env(), n);
   }
   // sort(Float32Array view, Float32Array|undefined cutout) -> Uint32Array   <- worker "sort", index.js:587-596
   Napi::Value Sort(const Napi::CallbackInfo& i) {

@@ -1,4 +1,5 @@
-/* Plain-C use of the drop-in boundary (include/gsplat_b200.h): load a .splat file, render one frame, write a PPM.
+/* Plain-C use of the drop-in boundary (include/gsplat_b200.h): load a .splat (or, by extension, .ply) file, render one
+ * frame, write a PPM.
  *   gcc -std=c99 -O2 examples/render_frame.c -Iinclude -Laframe-gaussian-splatting_b200 -lgsplat_b200 -lm -o render_frame
  *   LD_LIBRARY_PATH=aframe-gaussian-splatting_b200 ./render_frame scene.splat out.ppm
  * The camera is A-Frame's default (fov 80, near 0.005, far 10000) at (0, 1.6, 0) with the entity at (0, 1.5, -2)
@@ -12,20 +13,25 @@
 #include "gsplat_b200.h"
 
 int main(int argc, char **argv) {
-  if (argc < 3) { fprintf(stderr, "usage: %s scene.splat out.ppm\n", argv[0]); return 2; }
+  if (argc < 3) { fprintf(stderr, "usage: %s scene.splat|scene.ply out.ppm\n", argv[0]); return 2; }
   FILE *f = fopen(argv[1], "rb");
   if (!f) { perror(argv[1]); return 1; }
   fseek(f, 0, SEEK_END);
   long bytes = ftell(f);
   fseek(f, 0, SEEK_SET);
+  const size_t len = strlen(argv[1]);
+  const int is_ply = len >= 4 && strcmp(argv[1] + len - 4, ".ply") == 0; /* index.js:257 */
+  /* a .splat file is read as whole 32-byte rows; a .ply file is read whole */
   uint32_t n = (uint32_t)(bytes / 32);
-  void *rows = malloc((size_t)n * 32);
-  if (fread(rows, 32, n, f) != n) { fprintf(stderr, "short read\n"); return 1; }
+  const size_t want = is_ply ? (size_t)bytes : (size_t)n * 32;
+  void *rows = malloc(want ? want : 1);
+  if (fread(rows, 1, want, f) != want) { fprintf(stderr, "short read\n"); return 1; }
   fclose(f);
 
   gs_context *ctx = NULL;
   if (gs_create(0, &ctx) != GS_OK) { fprintf(stderr, "gs_create: %s\n", gs_last_error(NULL)); return 1; }
-  if (gs_push_splats(ctx, rows, n) != GS_OK) { fprintf(stderr, "push: %s\n", gs_last_error(ctx)); return 1; }
+  const int rc = is_ply ? gs_push_ply(ctx, rows, want, NULL, &n) : gs_push_splats(ctx, rows, n);
+  if (rc != GS_OK) { fprintf(stderr, "push: %s\n", gs_last_error(ctx)); return 1; }
 
   const uint32_t W = 1920, H = 1080;
   gs_render_params p;

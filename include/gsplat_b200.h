@@ -125,6 +125,20 @@ GS_API int gs_clear(gs_context *ctx);
  */
 GS_API int gs_push_splats(gs_context *ctx, const void *rows32, uint32_t n);
 /*
+ * processPlyBuffer + one pushDataBuffer (index.js:315-324, 600-745): append the vertices of a whole binary PLY file.
+ * ply/bytes: the file in host memory.  rows32_out_or_null: optional host buffer (32 * vertex count bytes) that receives
+ * the .splat rows processPlyBuffer returns, in its order (descending importance, stable).  *out_n = vertices appended.
+ * The header is parsed on the host with the reference's rules; decode, importance sort and pack run on the device.
+ * Same contract as gs_push_splats (below): frames in flight are not waited for, the file is consumed on return (with
+ * rows32_out_or_null the call also waits for its rows), and only a push that outgrows the table waits for the pipeline.
+ * Malformed input returns GS_ERR_INVALID with the reference's message in gs_last_error and leaves the table unchanged:
+ * no "end_header\n" in the first 10 KB or no "element vertex N\n" ("Unable to read .ply file header"); a property the
+ * conversion reads is missing ("<name> not found": x/y/z; rot_*, scale_1/2 and opacity when scale_0 exists;
+ * f_dc_1/2 when f_dc_0 exists, else red/green/blue); a body shorter than N rows.  A header with a non-ASCII byte before
+ * end_header is also refused (the reference would read its body at a shifted offset).
+ */
+GS_API int gs_push_ply(gs_context *ctx, const void *ply, size_t bytes, void *rows32_out_or_null, uint32_t *out_n);
+/*
  * Progressive loading (index.js:259-298: rows are pushed as they arrive while the scene is already being drawn):
  * gs_push_splats / gs_push_packed do NOT wait for frames in flight.  A frame draws the splats that were resident when
  * it was submitted; the pushed rows are staged through page-locked buffers and packed on a separate stream behind it,
