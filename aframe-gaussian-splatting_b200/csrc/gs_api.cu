@@ -131,7 +131,7 @@ static int ensure_instances(gs_context *c, uint64_t need) {
   dev_free(c->inst_tile); dev_free(c->inst_idx); dev_free(c->inst_tile_b); dev_free(c->inst_tile_f); dev_free(c->inst_idx_b);
   dev_free(c->inst_rec[0]); dev_free(c->inst_rec[1]);
   dev_free(c->table_d);
-  c->table_d_stride = (uint32_t)((need + kRadixTile / 2 - 1) / (kRadixTile / 2) + 2);  // one column per 2048-instance window
+  c->table_d_stride = (uint32_t)((need + kRadixTile - 1) / kRadixTile + 1);
   GS_CUDA(c, dev_alloc(&c->table_d, (size_t)256 * c->table_d_stride));
   GS_CUDA(c, dev_alloc(&c->inst_tile, need));
   GS_CUDA(c, dev_alloc(&c->inst_idx, need));
@@ -294,7 +294,6 @@ extern "C" int gs_create(int device_ordinal, gs_context **out_ctx) {
   // frames expected to sort at least GS_SLAB_MIN splats (default 16 M) are rendered front to back in depth slabs (gs_slab.cu);
   // GS_SLAB_FIRST = target entry count of the nearest slab (default 1 M, the following ones double)
   if (const char *e = getenv("GS_PDL")) c->use_pdl = strcmp(e, "1") == 0;
-  if (const char *e = getenv("GS_EMIT")) c->emit_by_entry = strcmp(e, "windows") != 0;
   if (const char *e = getenv("GS_SLAB_MIN")) c->slab_min = (uint32_t)strtoull(e, nullptr, 10);
   if (const char *e = getenv("GS_SLAB_FIRST")) c->slab_first = std::max<uint32_t>(1024u, (uint32_t)strtoull(e, nullptr, 10));
   {  // pixel loop of the raster: two pixels per lane (default) or one (GS_RASTER=scalar); both give identical frames
@@ -762,8 +761,8 @@ static cudaError_t enqueue_bin_stage(gs_context *c, gs_context::Slot &sl, uint32
   cudaError_t e;
   if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, m))) return e;
   if ((e = rec(sl.ev[2], m))) return e;
-  launch_emit(c, sl.fp, sl.ctr, b, m);   // 2 launches (k_emit also histograms pass T1)
-  launch_tile_radix(c, sl.ctr, b, n_bins, c->emit_by_entry, m);    // (hist +) scan + scatter; above 256 bins also pass T2 + k_tile_ranges
+  launch_emit(c, sl.fp, sl.ctr, b, nullptr, m);
+  launch_tile_radix(c, sl.ctr, b, n_bins, m);    // pass T1; above 256 bins also pass T2 + k_tile_ranges
   if ((e = rec(sl.ev[3], m))) return e;
   return cudaGetLastError();
 }
@@ -843,7 +842,7 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
     // depth-tested / statistics frames use other instantiations of the raster: plain launches, no cached graph
     GS_CUDA(c, enqueue_raster_stage(c, sl, n_tiles, false));
   }
-  sl.launches = (sl.scene ? 11u : (reuse ? 0u : 7u)) + 1u + (n_bins <= 256u ? 4u : 8u) + (c->emit_by_entry ? 1u : 0u) + 1u;
+  sl.launches = (sl.scene ? 11u : (reuse ? 0u : 7u)) + 1u + (n_bins <= 256u ? 5u : 9u) + 1u;
   return GS_OK;
 }
 
@@ -886,8 +885,8 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
     launch_slab_sort(c, sl.fp, sl.ctr, b, st);            // draw order of the slab
     launch_project_entries(c, sl.fp, sl.ctr, b, st);      // vertex shader for the slab's entries
     if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, st))) return e;
-    launch_emit_slab(c, sl.fp, sl.ctr, b, st);
-    launch_tile_radix(c, sl.ctr, b, n_bins, true, st);  // k_emit_entries leaves T1's histogram to its own kernel
+    launch_emit(c, sl.fp, sl.ctr, b, c->bin_open, st);
+    launch_tile_radix(c, sl.ctr, b, n_bins, st);
     if ((e = rec(sl.slab_ev[s][0], st))) return e;
     launch_raster_slab(c, sl.fp, sl.ctr, n_tiles, b, (sl.raster_flags & 2u) != 0, st);
     if ((e = rec(sl.slab_ev[s][1], st))) return e;

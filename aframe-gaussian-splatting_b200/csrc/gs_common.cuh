@@ -242,8 +242,6 @@ struct gs_context {
   bool have_last_sorted = false;
   uint32_t slab_first = 1u << 20;  // target entry count of the nearest slab (the following ones double)
   int last_mode = 0;               // 0 = one pass (three-stage pipeline), 1 = slab path
-  bool emit_by_entry = true;       // k_emit_entries + k_radix_hist<T1> (default) or, with
-                                   // GS_EMIT=windows, the window-balanced k_emit of round 1 (one-pass path only)
   uint4 *tile_stats = nullptr;     // [tiles] per-tile counts of a GS_RENDER_STATS frame
   uint4 *tile_stats_host = nullptr;  // pinned copy
   uint32_t tile_stats_cap = 0;
@@ -400,9 +398,10 @@ void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, 
 uint32_t *launch_ply_sort(gs_context *c, const uint32_t *key, uint32_t *perm_a, uint32_t *perm_b, uint32_t *table,
                           uint32_t *totals, uint32_t n, cudaStream_t st);
 void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
-void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 2 launches
-void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, bool hist_t1, cudaStream_t st);  // 2 .. 7 launches
-void launch_tile_ranges(gs_context *c, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
+// bin instances in draw order (2 launches); bin_open: the slab path's open-bin table, NULL for one-pass frames
+void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,
+                 cudaStream_t st);
+void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, cudaStream_t st);  // 3 .. 7 launches
 void launch_raster(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags, cudaStream_t st);
 void launch_peer_acquire(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
 void launch_peer_signal_wait(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
@@ -417,7 +416,6 @@ void launch_compact_offsets(gs_context *c, const FrameParams *fp, int set, int n
 void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, int slab, cudaStream_t st);  // + compaction: 2 launches
 void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 6 launches
 void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
-void launch_emit_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
 void launch_slab_end(gs_context *c, FrameCounters *ctr, cudaStream_t st);
 void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, uint32_t n_tiles, const FrameBufs &b, bool depth,
                         cudaStream_t st);

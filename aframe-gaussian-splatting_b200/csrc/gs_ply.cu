@@ -7,7 +7,7 @@
 //                  32-bit sort key of its importance (index.js:653-664).  Row j of the reference's output depends only on
 //                  source row sizeIndex[j], so decoding in file order and gathering afterwards (k_pack_perm) is exact.
 //                  <true>: every field read is an aligned float (the INRIA layout); <false>: any TYPE_MAP type, byte loads.
-//   the stable sort of the keys is k_radix_*<P1..P4> (gs_sort.cu).
+//   the stable sort of the keys is k_radix_*<P<0>> .. <P<24>> (gs_sort.cu).
 //
 // Numerics: fp64 as JavaScript evaluates it, no contraction (the library is built with --fmad=false).  The importance
 // product runs left to right and is rounded to f32 (Float32Array store); the key is the complement of the order-preserving

@@ -7,11 +7,9 @@
 //   k_count    : per entry of the draw order (== reference sortedIndexes): instance offset inside its 256-entry slice;
 //                per slice: total; last CTA: prefix over the slices + frame total D.
 //                Sparse frames (fewer than half of the splats sorted): each chunk's survivors are compacted first.
-//   k_emit_entries (default): one thread per draw-order entry writes its (bin, splat) instances at the entry's offset,
+//   k_emit_entries: one thread per draw-order entry writes its (bin, splat) instances at the entry's offset,
 //                in draw order, so that a STABLE sort by bin id alone reproduces the reference's back-to-front order
 //                inside every bin; rectangles of more than 8 bins are finished by the whole warp.
-//   k_emit     (GS_EMIT=windows, round 1): one CTA per window of 2048 instance positions; also produces pass T1's
-//                per-window digit histograms (table[digit][window]).
 #include "gs_common.cuh"
 
 namespace gs {
@@ -246,9 +244,6 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
 }
 
 
-constexpr int kEmitPerThread = kRadixTile / 2 / kEmitThreads;  // 8: one emission window = half a radix chunk
-constexpr int kEmitWindow = kEmitThreads * kEmitPerThread;  // 2048 instances per CTA iteration
-
 // candidate tiles of a packed rectangle that this rank owns (all of them on one GPU)
 __device__ __forceinline__ uint32_t rect_count(uint32_t r, uint32_t rank, uint32_t world) {
   if (r == kNoRect) return 0u;
@@ -359,254 +354,11 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
 }
 
 // ---------------------------------------------------------------------------------------------
-// K3b: ordered instance emission, balanced by INSTANCES: CTA iteration = one window of 2048 consecutive
-// positions of the instance array (near splats own thousands of tiles, far ones a few: balancing by entries
-// would leave a few CTAs with most of the work).
-//   1. two warps locate the window's first / last draw-order entry with 32-ary searches (5 dependent loads);
-//   2. the entries of the window (and the footprint geometry of their splats) are staged in shared memory,
-//      coalesced, at most kEmitEnt at a time;
-//   3. thread t generates positions [8t, 8t+8) of the window: one binary search in shared memory, then an
-//      incremental walk over tiles / entries; every candidate tile of the bounding rectangle is tested exactly
-//      against the r<=2 footprint (closest point of the tile's pixel-centre box in the splat's (px,py) frame),
-//      rejected tiles become kNoTile and are dropped by the T1 pass;
-//   4. the window is written out coalesced.
-// Position = prefix(entry) + k, so the array is in draw order whatever the execution order.
-// ---------------------------------------------------------------------------------------------
-constexpr int kEmitEnt = 896;  // staged entries per pass (static shared memory stays under 48 KB)
-
-// largest i in [lo, hi) with key(i) <= p, keys non-decreasing, key(lo) <= p; all 32 lanes of a warp cooperate
-template <class F>
-__device__ __forceinline__ uint32_t warp_search_le(uint32_t lo, uint32_t hi, uint32_t p, F key) {
-  const uint32_t lane = threadIdx.x & 31;
-  while (hi - lo > 1) {
-    const uint32_t step = (hi - lo + 31) / 32;
-    const uint32_t i = lo + lane * step;
-    const bool ok = (i < hi) && (key(i) <= p);
-    const uint32_t c = __popc(__ballot_sync(0xffffffffu, ok));  // lanes 0..c-1 are ok (c >= 1)
-    const uint32_t nlo = lo + (c - 1) * step;
-    hi = min(hi, nlo + step);
-    lo = nlo;
-  }
-  return lo;
-}
-
-__global__ void __launch_bounds__(kEmitThreads, 4) k_emit(const uint2 *__restrict__ ent,
-                                                          const uint32_t *__restrict__ ent_off,
-                                                          const uint32_t *__restrict__ slice_prefix,
-                                                          const float4 *__restrict__ proj_rec,
-                                                          const FrameParams *__restrict__ fp, uint64_t cap_inst,
-                                                          uint16_t *__restrict__ inst_tile, uint32_t *__restrict__ inst_idx,
-                                                          uint32_t *__restrict__ table_t1, uint32_t table_stride,
-                                                          FrameCounters *ctr, const uint32_t *__restrict__ bin_open) {
-  GS_PDL_ENTRY();
-  const RenderConsts &rc = fp->rc;
-  __shared__ uint32_t s_wi[kEmitThreads * (kEmitPerThread + 1)];  // stride 9: conflict-free staging
-  __shared__ uint16_t s_wt[kEmitThreads * (kEmitPerThread + 1)];
-  __shared__ uint2 s_ent[kEmitEnt];         // {splat index, rect}
-  __shared__ uint32_t s_goff[kEmitEnt + 1];  // global instance offset of each staged entry
-  __shared__ float4 s_g0[kEmitEnt];         // cx, cy, a1x, a1y
-  __shared__ float2 s_g1[kEmitEnt];         // a2x, a2y
-  __shared__ uint32_t s_jfl[2];
-  __shared__ uint32_t s_cnt[kEmitThreads / 32];
-  __shared__ uint32_t s_hist[256];  // low tile-id byte of the kept instances of this window: pass T1's histogram column
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  s_hist[tid] = 0;
-  const uint32_t nv = ctr->sort.n_valid;
-  const uint32_t num_slices = (nv + kEmitTile - 1) / kEmitTile;
-  const unsigned long long d_all = ctr->n_inst;
-  if (d_all > cap_inst) {  // instance buffer too small: the host regrows it and re-runs the frame
-    if (blockIdx.x == 0 && tid == 0) ctr->overflow = 1u;
-    return;
-  }
-  const uint32_t total = (uint32_t)d_all;
-  const uint32_t num_windows = (total + kEmitWindow - 1) / kEmitWindow;
-  auto goff = [&](uint32_t j) -> uint32_t {  // global instance offset of entry j (j == nv: the total)
-    return j < nv ? __ldg(slice_prefix + (j >> 8)) + __ldg(ent_off + j) : total;
-  };
-  static_assert(kEmitTile == 256, "entry -> slice is j >> 8");
-  static_assert(kEmitThreads == 256 && kEmitWindow * 2 == kRadixTile, "one histogram column per window, two per radix chunk");
-
-  for (uint32_t win = blockIdx.x; win < num_windows; win += gridDim.x) {
-    const uint32_t wb = win * kEmitWindow, we = min(wb + (uint32_t)kEmitWindow, total);
-    // ---- 1. first / last entry of the window ----
-    if (warp < 2) {
-      const uint32_t p = warp == 0 ? wb : we - 1;
-      const uint32_t sl = warp_search_le(0u, num_slices, p, [&](uint32_t i) { return __ldg(slice_prefix + i); });
-      const uint32_t rel = p - __ldg(slice_prefix + sl);
-      const uint32_t a = sl * kEmitTile, b = min(a + (uint32_t)kEmitTile, nv);
-      const uint32_t j = warp_search_le(a, b, rel, [&](uint32_t i) { return __ldg(ent_off + i); });
-      if (lane == 0) s_jfl[warp] = j;
-    }
-    __syncthreads();
-    const uint32_t j_last = s_jfl[1];
-    uint32_t j0 = s_jfl[0], pos = wb;
-    while (pos < we) {
-      // ---- 2. stage the entries that own tiles, compacted in order, from source entries [j0, ...) ----
-      // (with the frame sharded over GPUs most entries own no tile of this rank: skipping them here keeps the
-      //  staged window dense); batches of 256 source entries until the staging arrays are full
-      uint32_t nE = 0, jn = j0;
-      while (jn <= j_last && nE + kEmitThreads <= (uint32_t)kEmitEnt) {
-        if ((jn & (uint32_t)(kEmitTile - 1)) == 0u) {
-          // at a slice boundary: skip runs of slices that own no instance at all (slab path after most bins have
-          // closed, or a rank that owns few of a region's bins) - 256 slices = 65536 entries per look
-          const uint32_t sl = (jn >> 8) + tid, sl_last = j_last >> 8;
-          const bool stop = (sl > sl_last) || (__ldg(slice_prefix + sl + 1) != __ldg(slice_prefix + sl));
-          const uint32_t bal0 = __ballot_sync(0xffffffffu, stop);
-          if (lane == 0) s_cnt[warp] = bal0 ? warp * 32u + (uint32_t)__ffs(bal0) - 1u : (uint32_t)kEmitThreads;
-          __syncthreads();
-          uint32_t skip = kEmitThreads;
-          for (uint32_t k2 = 0; k2 < kEmitThreads / 32; ++k2) skip = min(skip, s_cnt[k2]);
-          __syncthreads();  // s_cnt is reused by the batch below
-          jn += skip * (uint32_t)kEmitTile;
-          if (skip == (uint32_t)kEmitThreads) continue;
-          if (jn > j_last) break;
-        }
-        const uint32_t jend = (jn | (uint32_t)(kEmitTile - 1)) + 1u;  // batches end at slice boundaries
-        const uint32_t j = jn + tid;
-        uint2 en = make_uint2(0u, kNoRect);
-        if (j < jend && j <= j_last) en = __ldg(ent + j);
-        const bool nz = en.y != kNoRect;
-        const uint32_t bal = __ballot_sync(0xffffffffu, nz);
-        if (lane == 0) s_cnt[warp] = __popc(bal);
-        __syncthreads();
-        uint32_t base_w = nE, tot = 0;
-        for (uint32_t k2 = 0; k2 < kEmitThreads / 32; ++k2) {
-          if (k2 < warp) base_w += s_cnt[k2];
-          tot += s_cnt[k2];
-        }
-        if (nz) {
-          const uint32_t q = base_w + __popc(bal & ((1u << lane) - 1u));
-          s_ent[q] = en;
-          s_goff[q] = goff(j);
-          const uint32_t r = en.y;
-          const uint32_t wfull = ((r >> 8) & 255u) - (r & 255u) + 1u, hfull = (r >> 24) - ((r >> 16) & 255u) + 1u;
-          if (wfull * hfull > 1u) {  // footprint geometry for the exact tile test
-            s_g0[q] = __ldg(proj_rec + 2 * (size_t)en.x);
-            s_g1[q] = __ldg((const float2 *)(proj_rec + 2 * (size_t)en.x + 1));
-          }
-        }
-        nE += tot;
-        jn = jend;
-        __syncthreads();
-      }
-      const uint32_t jE = min(jn, j_last + 1);
-      if (tid == 0) s_goff[nE] = goff(jE);  // first position NOT covered by the staged entries
-      __syncthreads();
-      const uint32_t pe = min(we, s_goff[nE]);  // positions [pos, pe) belong to the staged entries
-      // ---- 3. generate ----
-      const uint32_t t0 = max(pos, wb + tid * kEmitPerThread), t1 = min(pe, wb + (tid + 1) * kEmitPerThread);
-      if (t0 < t1) {
-        uint32_t lo = 0, hi = nE;
-        while (hi - lo > 1) {
-          const uint32_t mid = (lo + hi) >> 1;
-          if (s_goff[mid] <= t0) lo = mid; else hi = mid;
-        }
-        uint32_t e = lo;                  // staged entry
-        uint32_t k = t0 - s_goff[lo];     // position inside it
-        uint32_t idx = 0, txf = 0, w = 1, step = 1, tx = 0, ty = 0, n_all = 0, n_own = 0;
-        float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f);
-        float2 r1 = make_float2(0.f, 0.f);
-        float cross = 0.f, inv_yy = 0.f, inv_xx = 0.f;
-        auto load_entry = [&](uint32_t ee, uint32_t kk) {
-          const uint2 en = s_ent[ee];
-          const uint32_t r = en.y;
-          n_own = 0;
-          if (r == kNoRect) return;
-          idx = en.x;
-          uint32_t tx0 = r & 255u;
-          const uint32_t ty0 = (r >> 16) & 255u, h = (r >> 24) - ty0 + 1u;
-          w = ((r >> 8) & 255u) - tx0 + 1u;
-          n_all = w * h;
-          step = 1u;
-          if (rc.shard_world > 1) {  // owned columns of the rectangle: first, first + world, ...
-            owned_span(tx0, (r >> 8) & 255u, rc.shard_rank, rc.shard_world, tx0, w);
-            step = rc.shard_world;
-          }
-          n_own = w * h;
-          if (n_own == 0) return;
-          txf = tx0;
-          // kk / w for kk < 65536, w <= 256: the float quotient of (kk + 0.5) is never within rounding of an integer
-          const uint32_t row = (uint32_t)__fdividef((float)kk + 0.5f, (float)w);
-          tx = tx0 + (kk - row * w) * step;
-          ty = ty0 + row;
-          if (n_all > 1) {
-            r0 = s_g0[ee];
-            r1 = s_g1[ee];
-            // q(d) = |(a2.d, a1.d)|^2 = M00 dx^2 + 2 M01 dx dy + M11 dy^2: edge minimisers need M01/M11, M01/M00
-            cross = r1.x * r1.y + r0.z * r0.w;
-            inv_yy = __fdividef(1.0f, r1.y * r1.y + r0.w * r0.w);
-            inv_xx = __fdividef(1.0f, r1.x * r1.x + r0.z * r0.z);
-          }
-        };
-        load_entry(e, k);
-#pragma unroll 1
-        for (uint32_t p = t0; p < t1; ++p) {
-          if (k >= n_own) {  // next staged entry (every staged entry owns tiles)
-            ++e;
-            load_entry(e, 0u);
-            k = 0;
-          }
-          bool keep = true;
-          if (n_all > 1) {
-            // pixel-centre box of the bin, relative to the splat centre
-            const float xa = (float)(tx * kBin) + 0.5f - r0.x, xb = xa + (float)(kBin - 1);
-            const float ya = (float)(ty * kBin) + 0.5f - r0.y, yb = ya + (float)(kBin - 1);
-            const bool in_x = (xa <= 0.0f) && (xb >= 0.0f), in_y = (ya <= 0.0f) && (yb >= 0.0f);
-            if (!(in_x && in_y)) {
-              float qmin = 3.0e38f;
-              if (!in_x) {  // nearest vertical edge, minimise over y on it; (px,py) evaluated at the found point
-                const float dx = (xa > 0.0f) ? xa : xb;
-                const float t = fminf(fmaxf(-dx * cross * inv_yy, ya), yb);
-                const float px = dx * r1.x + t * r1.y, py = dx * r0.z + t * r0.w;
-                qmin = px * px + py * py;
-              }
-              if (!in_y) {  // nearest horizontal edge, minimise over x on it
-                const float dy = (ya > 0.0f) ? ya : yb;
-                const float t = fminf(fmaxf(-dy * cross * inv_xx, xa), xb);
-                const float px = t * r1.x + dy * r1.y, py = t * r0.z + dy * r0.w;
-                qmin = fminf(qmin, px * px + py * py);
-              }
-              keep = !(qmin > 4.02f);  // r^2 <= 4 with slack for fp32 rounding of the closest-point search
-            }
-          }
-          uint32_t t = kNoTile;
-          if (keep && bin_open) keep = __ldg(bin_open + ty * rc.bins_x + tx) != 0u;  // slab path: closed bins take nothing
-          if (keep) {
-            t = ty * rc.bins_x + tx;
-            atomicAdd(&s_hist[t & 255u], 1u);
-          }
-          const uint32_t q = p - wb;  // window-relative position
-          const uint32_t si = (q / kEmitPerThread) * (kEmitPerThread + 1) + (q % kEmitPerThread);
-          s_wt[si] = (uint16_t)t;
-          s_wi[si] = idx;
-          // advance inside the rectangle (row-major over the owned columns)
-          ++k;
-          tx += step;
-          if (tx >= txf + w * step) { tx = txf; ++ty; }
-        }
-      }
-      __syncthreads();
-      pos = pe;
-      j0 = jE;
-    }
-    // ---- 4. write the window out ----
-    const uint32_t wn = we - wb;
-    for (uint32_t i = tid; i < wn; i += kEmitThreads) {
-      const uint32_t si = (i / kEmitPerThread) * (kEmitPerThread + 1) + (i % kEmitPerThread);
-      inst_tile[(size_t)wb + i] = s_wt[si];
-      inst_idx[(size_t)wb + i] = s_wi[si];
-    }
-    table_t1[(size_t)tid * table_stride + win] = s_hist[tid];  // kEmitThreads == 256 digits
-    s_hist[tid] = 0;
-    __syncthreads();
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// K3b', slab path: instance emission by ENTRY.  In a slab most entries own nothing any more (closed bins, other
-// ranks' bins), so the instance-window walk of k_emit would spend its time stepping over dead entries; here one thread
-// owns one live entry and writes its instances at the entry's own offset (position = prefix(entry) + k, so the array is
-// still in draw order).  Entries with large rectangles are finished by their whole warp, 32 candidates per step.
+// K3b: instance emission by ENTRY: one thread owns one live draw-order entry and writes its instances at the entry's
+// own offset (position = prefix(entry) + k, so the array is in draw order whatever the execution order).  Entries with
+// large rectangles are finished by their whole warp, 32 candidates per step.  Each candidate bin is tested exactly
+// against the r<=2 footprint; rejected bins (and, on the slab path, closed ones) become kNoTile and are dropped by the
+// bin sort.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void emit_candidate(const RenderConsts &rc, uint32_t bx, uint32_t by, bool multi, const float4 &r0,
                                                const float2 &r1, const uint32_t *__restrict__ bin_open, uint32_t payload,
@@ -721,36 +473,16 @@ void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters 
                (const uint32_t *)b.order, (const FrameCounters *)ctr, (const SceneTable *)nullptr);
 }
 
-static void launch_emit_impl(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st, bool slab);
-void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
-  launch_emit_impl(c, fp, ctr, b, st, false);
-}
-void launch_emit_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
-  launch_emit_impl(c, fp, ctr, b, st, true);
-}
-static void launch_emit_impl(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st, bool slab) {
+void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,
+                 cudaStream_t st) {
   uint64_t tiles = ((uint64_t)c->cap + kEmitTile - 1) / kEmitTile;
   const uint64_t cap = (uint64_t)c->sm_count * 8;
   if (tiles > cap) tiles = cap;
   if (tiles < 1) tiles = 1;
-  if (slab)
-    launch_chain(c, k_count<true>, (int)tiles, kEmitThreads, st, (const uint32_t *)b.order, (const uint32_t *)b.rect, c->ent, c->ent_off,
-                 c->slice_total, c->slice_prefix, ctr, fp, (const uint32_t *)c->bin_open);
-  else
-    launch_chain(c, k_count<false>, (int)tiles, kEmitThreads, st, (const uint32_t *)b.order, (const uint32_t *)b.rect, c->ent, c->ent_off,
-                 c->slice_total, c->slice_prefix, ctr, fp, (const uint32_t *)nullptr);
-  if (slab || c->emit_by_entry) {
-    launch_chain(c, k_emit_entries, (int)tiles, 256, st, (const uint2 *)c->ent, (const uint32_t *)c->ent_off, (const uint32_t *)c->slice_prefix,
-                 (const float4 *)b.proj_rec, fp, (uint64_t)c->cap_inst, c->inst_tile, c->inst_idx, ctr,
-                 (const uint32_t *)(slab ? c->bin_open : nullptr));
-    return;
-  }
-  uint64_t wins = (c->cap_inst + kEmitWindow - 1) / kEmitWindow;
-  if (wins > (uint64_t)c->sm_count * 4) wins = (uint64_t)c->sm_count * 4;
-  if (wins < 1) wins = 1;
-  k_emit<<<(int)wins, kEmitThreads, 0, st>>>(c->ent, c->ent_off, c->slice_prefix, b.proj_rec, fp, c->cap_inst,
-                                                    c->inst_tile, c->inst_idx, c->table_d, c->table_d_stride, ctr,
-                                                    slab ? c->bin_open : nullptr);
+  launch_chain(c, bin_open ? k_count<true> : k_count<false>, (int)tiles, kEmitThreads, st, (const uint32_t *)b.order,
+               (const uint32_t *)b.rect, c->ent, c->ent_off, c->slice_total, c->slice_prefix, ctr, fp, bin_open);
+  launch_chain(c, k_emit_entries, (int)tiles, 256, st, (const uint2 *)c->ent, (const uint32_t *)c->ent_off, (const uint32_t *)c->slice_prefix,
+               (const float4 *)b.proj_rec, fp, (uint64_t)c->cap_inst, c->inst_tile, c->inst_idx, ctr, bin_open);
 }
 
 }  // namespace gs

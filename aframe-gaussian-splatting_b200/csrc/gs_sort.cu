@@ -1,12 +1,11 @@
 // gs_sort.cu — device restatement of the Web-Worker `sortSplats` (reference index.js:507-570)
-// and the stable LSD radix passes shared by the depth sort and the tile binning.
+// and the stable LSD radix passes of every ordering in the library.
 //
 //   k_depth_cull  : index.js:517-555  depth (fp64, left to right), cutout box, filter, min/max
-//   k_radix_{hist,scan,scatter}<D1/D2>: index.js:557-567  16-bit key = ToInt32((f32 depth - min) * depthInv), stable
+//   k_radix_{hist,scan,scatter}<D1>, <D2>: index.js:557-567  16-bit key = ToInt32((f32 depth - min) * depthInv), stable
 //                   counting sort as two 8-bit passes
 //   k_radix_{hist,scan,scatter}<T1>, <T2>: stable sort of bin instances by 16-bit bin id; the final pass (T1 when a
-//                   frame has at most 256 bins, else T2) also gathers the 32 B records (with GS_EMIT=windows T1's
-//                   histograms come from k_emit instead of k_radix_hist<T1>)
+//                   frame has at most 256 bins, else T2) also gathers the 32 B records
 //   k_radix_{hist,scan,scatter}<S1>: first pass of a depth slab's sort (keys from the slab's compacted entries)
 //   k_tile_ranges : per-bin {start, end} in the final instance order (frames of more than 256 bins; otherwise pass T1 writes them)
 //
@@ -17,11 +16,11 @@
 //   k_scene_keys       : 24-bit key = draw rank << 17 | the entity's 16-bit key, or | 65536 for a key outside
 //                        [0,65535] with payload = the entity's first splat (quirk Q5 per entity: the worker's dropped slots
 //                        stay 0, the entity-local splat 0, and come after all its in-range entries)
-//   k_radix_*<M1/M2/M3>: three stable 8-bit passes -> (rank, key, index) order = each entity's sortedIndexes + first,
+//   k_radix_*<M1>, <M2>, <M3>: three stable 8-bit passes -> (rank, key, index) order = each entity's sortedIndexes + first,
 //                        concatenated in draw order
 //
-// PLY ingest (gs_push_ply): k_radix_*<P1..P4> sort the rows by a 32-bit importance key, four stable 8-bit passes (the
-// stable Array.prototype.sort of index.js:668).  Each pass reads the digit through the permutation (key[perm[i]]), so
+// PLY ingest (gs_push_ply): k_radix_*<P<0>> .. <P<24>> sort the rows by a 32-bit importance key, four stable 8-bit passes
+// (the stable Array.prototype.sort of index.js:668).  Each pass reads the digit through the permutation (key[perm[i]]), so
 // nothing but the row index is carried.
 //
 // Bit-exactness: JS evaluates in fp64 with IEEE rounding after every operation; the kernels use
@@ -259,371 +258,6 @@ __global__ void __launch_bounds__(256) k_scene_keys(const float *__restrict__ de
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// Stable 8-bit radix pass = three fully parallel kernels (no inter-CTA spinning):
-//   k_radix_hist<PASS>   : per-chunk (4096 elements) digit histogram        -> table[digit][chunk]
-//   k_radix_scan<PASS>   : per-digit exclusive scan over the chunks (in place) + digit totals
-//   k_radix_scatter<PASS>: per chunk: stable in-chunk ranks (warp match_any) + table offset -> scatter
-// PASS_D1/D2: 16-bit depth key (index.js:557-567) low/high byte.  PASS_T1/T2: 16-bit tile id low/high byte;
-// T2's scatter gathers the 32 B projected record of each instance into its final per-tile slot.
-// ---------------------------------------------------------------------------------------------
-enum { PASS_D1 = 0, PASS_D2 = 1, PASS_T1 = 2, PASS_T2 = 3, PASS_S1 = 4,  // S1: low key byte of a compacted slab (gs_slab.cu)
-       PASS_M1 = 5, PASS_M2 = 6, PASS_M3 = 7,  // scene frames: bits 0-7, 8-15, 16-23 of the (rank, key) sort key
-       PASS_P1 = 8, PASS_P2 = 9, PASS_P3 = 10, PASS_P4 = 11 };  // PLY ingest: bits 0-7 .. 24-31 of the importance key
-
-struct RadixArgs {
-  FrameCounters *ctr;
-  uint32_t *table;   // [256][stride]
-  uint32_t *totals;  // [256]
-  uint32_t stride;
-  const FrameParams *fp;  // D1: fp->n_splats = number of resident splats of this frame
-  // depth passes
-  const float *depth;
-  uint32_t *idx_a;
-  uint8_t *dig_a;
-  uint32_t *order;
-  // tile passes
-  const uint16_t *inst_tile;
-  const uint32_t *inst_idx;
-  uint16_t *inst_tile_b;  // T1 output / T2 input: full tile id
-  uint16_t *inst_tile_f;  // T2 output: tile id in final order
-  uint32_t *inst_idx_b;
-  const float4 *proj_rec;
-  float4 *inst_rec;
-  // slab path: compacted (key, index) pairs of the current slab
-  const uint16_t *ckey;
-  const uint32_t *cidx;
-  // scene frames: M1 reads (skey, spay) and writes (idx_a, shi); M2 writes (spay, dig_a); M3 writes order
-  const uint32_t *skey;
-  uint32_t *spay;
-  uint16_t *shi;
-  // frames of at most 256 bins: the bin id is one byte, pass T1 is the whole sort and gathers the records itself
-  uint32_t t1_final;
-  uint2 *bin_range;   // t1_final: the per-bin {start, end} fall out of the digit totals (no k_tile_ranges launch)
-  uint32_t n_bins;
-  uint32_t t1_chunk_cols;  // T1's histogram columns: 0 = one per 2048-instance window (produced by k_emit),
-                           // 1 = one per 4096-element chunk (k_radix_hist<T1>, slab path)
-  // PLY ingest: pn keys, the permutation of the previous pass (P2..P4) and this pass's output
-  const uint32_t *pkey;
-  const uint32_t *pin;
-  uint32_t *pout;
-  uint32_t pn;
-};
-
-template <int PASS>
-__device__ __forceinline__ uint32_t pass_n(const RadixArgs &a) {
-  if (PASS >= PASS_P1) return a.pn;
-  const FrameCounters *ctr = a.ctr;
-  if (PASS == PASS_D1) return ctr->sort.n_valid ? a.fp->n_splats : 0u;
-  if (PASS == PASS_D2) return ctr->sort.n_inrange;
-  if (PASS == PASS_S1) return ctr->sort.n_valid;  // entries of the current slab (k_slab_begin)
-  if (PASS == PASS_M1) return ctr->sort.n_valid ? a.fp->n_splats : 0u;
-  if (PASS == PASS_M2 || PASS == PASS_M3) return ctr->sort.n_valid;  // every sorted entry, Q5 drops included
-  if (PASS == PASS_T1) return ctr->overflow ? 0u : (uint32_t)ctr->n_inst;
-  return ctr->overflow ? 0u : ctr->n_inst_kept;
-}
-
-// digit (or kInvalidDigit), payload and next-pass digit of element i
-template <int PASS>
-__device__ __forceinline__ void load_elem(const RadixArgs &a, uint32_t i, const DepthRange &dr, uint32_t &digit,
-                                          uint32_t &pay, uint32_t &hi, uint32_t &dropped) {
-  digit = kInvalidDigit;
-  pay = 0;
-  hi = 0;
-  if (PASS == PASS_D1) {
-    const float d = __ldg(a.depth + i);
-    if (d != GS_DEPTH_REJECT) {
-      const int32_t key = depth_key(d, dr.min_depth, dr.depth_inv);
-      if (key >= 0 && key <= 65535) { digit = key & 255; hi = (uint32_t)key >> 8; pay = i; }
-      else ++dropped;  // typed-array write out of range: dropped (quirk Q5)
-    }
-  } else if (PASS == PASS_S1) {
-    const uint32_t k = a.ckey[i];
-    digit = k & 255u;
-    hi = k >> 8;
-    pay = a.cidx[i];
-  } else if (PASS == PASS_D2) {
-    digit = a.dig_a[i];
-    pay = a.idx_a[i];
-  } else if (PASS == PASS_M1) {
-    const uint32_t k = a.skey[i];
-    if (k != kNoKey) { digit = k & 255u; hi = k >> 8; pay = a.spay[i]; }
-  } else if (PASS == PASS_M2) {
-    const uint32_t h = a.shi[i];
-    digit = h & 255u;
-    hi = h >> 8;
-    pay = a.idx_a[i];
-  } else if (PASS == PASS_M3) {
-    digit = a.dig_a[i];
-    pay = a.spay[i];
-  } else if (PASS >= PASS_P1) {
-    const uint32_t p = PASS == PASS_P1 ? i : a.pin[i];
-    digit = (__ldg(a.pkey + p) >> (8 * (PASS - PASS_P1))) & 255u;
-    pay = p;
-  } else if (PASS == PASS_T1) {
-    const uint16_t t = a.inst_tile[i];
-    if (t != kNoTile) { digit = t & 255; hi = t; pay = a.inst_idx[i]; }
-  } else {
-    const uint16_t t = a.inst_tile_b[i];
-    digit = (uint32_t)t >> 8;
-    hi = t;
-    pay = a.inst_idx_b[i];
-  }
-}
-
-template <int PASS>
-__global__ void __launch_bounds__(kRadixThreads) k_radix_hist(RadixArgs a) {
-  GS_PDL_ENTRY();
-  __shared__ uint32_t h[256];
-  __shared__ uint32_t s_in, s_drop;
-  FrameCounters *ctr = a.ctr;
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t n = pass_n<PASS>(a);
-  const uint32_t num_chunks = (n + kRadixTile - 1) / kRadixTile;
-  DepthRange dr{0.0, 0.0};
-  if (PASS == PASS_D1 && n) dr = load_depth_range(ctr);
-  if (PASS == PASS_D2) {
-    // quirk Q5: the reference's output keeps length validCount; slots never written stay 0
-    const uint32_t nv = ctr->sort.n_valid;
-    for (uint32_t j = n + blockIdx.x * blockDim.x + tid; j < nv; j += gridDim.x * blockDim.x) a.order[j] = 0u;
-  }
-  if (tid == 0) { s_in = 0; s_drop = 0; }
-  uint32_t in = 0, drop = 0;
-  for (uint32_t c = blockIdx.x; c < num_chunks; c += gridDim.x) {
-    h[tid] = 0;
-    __syncthreads();
-    const uint32_t base = c * kRadixTile + warp * (32 * kRadixItems) + lane;
-#pragma unroll
-    for (int s = 0; s < kRadixItems; ++s) {
-      const uint32_t i = base + s * 32;
-      if (i < n) {
-        uint32_t digit, pay, hi;
-        load_elem<PASS>(a, i, dr, digit, pay, hi, drop);
-        if (digit != kInvalidDigit) { atomicAdd(&h[digit], 1u); ++in; }
-      }
-    }
-    __syncthreads();
-    a.table[(size_t)tid * a.stride + c] = h[tid];
-    __syncthreads();
-  }
-  if (PASS == PASS_D1) {
-    for (int o = 16; o > 0; o >>= 1) {
-      in += __shfl_xor_sync(0xffffffffu, in, o);
-      drop += __shfl_xor_sync(0xffffffffu, drop, o);
-    }
-    __syncthreads();
-    if (lane == 0) { if (in) atomicAdd(&s_in, in); if (drop) atomicAdd(&s_drop, drop); }
-    __syncthreads();
-    if (tid == 0) {
-      if (s_in) atomicAdd(&ctr->sort.n_inrange, s_in);
-      if (s_drop) atomicAdd(&ctr->sort.n_dropped, s_drop);
-    }
-  }
-}
-
-// grid = 256 CTAs (one per digit)
-template <int PASS>
-__global__ void __launch_bounds__(256) k_radix_scan(RadixArgs a) {
-  GS_PDL_ENTRY();
-  __shared__ uint32_t s_warp[8];
-  __shared__ uint32_t s_carry;
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t n = pass_n<PASS>(a);
-  // T1's histograms come from k_emit, one column per 2048-instance window (two per 4096-element chunk)
-  const uint32_t col_elems = (PASS == PASS_T1 && !a.t1_chunk_cols) ? (uint32_t)kRadixTile / 2 : (uint32_t)kRadixTile;
-  const uint32_t num_chunks = (n + col_elems - 1) / col_elems;
-  uint32_t *row = a.table + (size_t)blockIdx.x * a.stride;
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
-  for (uint32_t b = 0; b < num_chunks; b += 256) {
-    const uint32_t i = b + tid;
-    const uint32_t v = (i < num_chunks) ? row[i] : 0u;
-    uint32_t incl = v;
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= (uint32_t)o) incl += t;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    uint32_t wbase = 0;
-    for (uint32_t k = 0; k < warp; ++k) wbase += s_warp[k];
-    const uint32_t carry = s_carry;
-    if (i < num_chunks) row[i] = carry + wbase + incl - v;
-    __syncthreads();
-    if (tid == 255) s_carry = carry + wbase + incl;
-    __syncthreads();
-  }
-  if (tid == 0) {
-    a.totals[blockIdx.x] = s_carry;
-    if (PASS == PASS_T1 && s_carry) atomicAdd(&a.ctr->n_inst_kept, s_carry);
-  }
-}
-
-// 512 threads x 8 elements per chunk: 16 warps rank their 256-element slices independently (an 8-step
-// dependent chain each), then one scan over the 16 warp counters per digit orders the slices.
-constexpr int kScatThreads = 512;
-constexpr int kScatItems = kRadixTile / kScatThreads;  // 8
-constexpr int kScatWarps = kScatThreads / 32;          // 16
-
-template <int PASS>
-__global__ void __launch_bounds__(kScatThreads, 2) k_radix_scatter(RadixArgs a) {
-  GS_PDL_ENTRY();
-  __shared__ uint32_t wcnt[kScatWarps][256];
-  __shared__ uint32_t tile_off[256];  // global slot of the digit's first element MINUS its slot in the staged chunk
-  __shared__ uint32_t s_loc[256];     // slot of the digit's first element in the staged (locally sorted) chunk
-  __shared__ uint32_t s_warp_tot[8];
-  __shared__ uint32_t s_pay[kRadixTile];
-  // value carried to the next pass: D1 -> high key byte, T1/T2 -> the 16-bit tile id, M1 -> key bits 8-23, M2 -> bits 16-23
-  using hi_t = typename std::conditional<(PASS == PASS_T1 || PASS == PASS_T2 || PASS == PASS_M1), uint16_t, uint8_t>::type;
-  constexpr bool kCarry = PASS != PASS_D2 && PASS != PASS_M3 && PASS < PASS_P1;  // the last pass of a sort (and P) carries nothing
-  __shared__ hi_t s_hi[kCarry ? kRadixTile : 1];  // D1 / S1: high key byte
-  __shared__ uint8_t s_dig[kRadixTile];
-  __shared__ uint32_t s_total;
-  FrameCounters *ctr = a.ctr;
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t n = pass_n<PASS>(a);
-  const uint32_t num_chunks = (n + kRadixTile - 1) / kRadixTile;
-  if (blockIdx.x >= num_chunks) return;
-
-  // block-wide exclusive scan over the 256 digit slots (threads >= 256 contribute 0)
-  auto scan256 = [&](uint32_t v) -> uint32_t {
-    uint32_t incl = v;
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= (uint32_t)o) incl += t;
-    }
-    __syncthreads();  // previous users of s_warp_tot are done
-    if (lane == 31 && warp < 8) s_warp_tot[warp] = incl;
-    __syncthreads();
-    uint32_t wbase = 0;
-    for (uint32_t k = 0; k < warp && k < 8; ++k) wbase += s_warp_tot[k];
-    return wbase + incl - v;
-  };
-
-  // first output slot of each digit
-  const uint32_t dtot = tid < 256 ? a.totals[tid] : 0u;
-  const uint32_t dbase = scan256(dtot);
-  if (PASS == PASS_T1 && a.t1_final && blockIdx.x == 0 && tid < a.n_bins) a.bin_range[tid] = make_uint2(dbase, dbase + dtot);
-  DepthRange dr{0.0, 0.0};
-  if (PASS == PASS_D1) dr = load_depth_range(ctr);
-
-  for (uint32_t c = blockIdx.x; c < num_chunks; c += gridDim.x) {
-    // this chunk's per-digit offset: issued first so its latency hides behind the ranking
-    const uint32_t toff = tid < 256 ? __ldg(a.table + (size_t)tid * a.stride + ((PASS == PASS_T1 && !a.t1_chunk_cols) ? 2 * c : c)) : 0u;
-    for (uint32_t k = tid; k < kScatWarps * 256; k += kScatThreads) (&wcnt[0][0])[k] = 0u;
-    // ---- load (warp-striped: consecutive lanes read consecutive elements) ----
-    const uint32_t base = c * kRadixTile + warp * (32 * kScatItems) + lane;
-    uint32_t digit[kScatItems], pay[kScatItems], rank[kScatItems];
-    hi_t hi[kScatItems];
-    uint32_t dummy = 0;
-#pragma unroll
-    for (int s = 0; s < kScatItems; ++s) {
-      const uint32_t i = base + s * 32;
-      digit[s] = kInvalidDigit;
-      pay[s] = 0;
-      hi[s] = 0;
-      if (i < n) {
-        uint32_t h8;
-        load_elem<PASS>(a, i, dr, digit[s], pay[s], h8, dummy);
-        hi[s] = (hi_t)h8;
-      }
-    }
-    __syncthreads();
-    // ---- stable rank inside the warp (input order = lane order within a step, steps in order) ----
-#pragma unroll
-    for (int s = 0; s < kScatItems; ++s) {
-      const uint32_t d = digit[s];
-      const uint32_t peers = __match_any_sync(0xffffffffu, d);
-      const uint32_t lt = __popc(peers & ((1u << lane) - 1u));
-      uint32_t prior = 0;
-      if (d != kInvalidDigit) prior = wcnt[warp][d];
-      __syncwarp();
-      if (d != kInvalidDigit && lt == 0) wcnt[warp][d] = prior + __popc(peers);
-      __syncwarp();
-      rank[s] = prior + lt;
-    }
-    __syncthreads();
-    // ---- thread `tid` < 256 owns digit `tid`: exclusive scan over the warps, then over the digits ----
-    uint32_t total = 0;
-    if (tid < 256) {
-#pragma unroll
-      for (int w = 0; w < kScatWarps; ++w) {
-        const uint32_t cnt = wcnt[w][tid];
-        wcnt[w][tid] = total;
-        total += cnt;
-      }
-    }
-    const uint32_t loc = scan256(total);
-    if (tid < 256) {
-      s_loc[tid] = loc;
-      tile_off[tid] = dbase + toff - loc;
-      if (tid == 255) s_total = loc + total;
-    }
-    __syncthreads();
-    // ---- stage the chunk in shared memory in sorted order ----
-#pragma unroll
-    for (int s = 0; s < kScatItems; ++s) {
-      const uint32_t d = digit[s];
-      if (d == kInvalidDigit) continue;
-      const uint32_t lp = s_loc[d] + wcnt[warp][d] + rank[s];
-      s_pay[lp] = pay[s];
-      s_dig[lp] = (uint8_t)d;
-      if (kCarry) s_hi[lp] = hi[s];
-    }
-    __syncthreads();
-    // ---- write out: consecutive threads write consecutive slots of the same digit run (coalesced) ----
-    const uint32_t nvalid = s_total;
-    for (uint32_t i = tid; i < nvalid; i += kScatThreads) {
-      const uint32_t pos = tile_off[s_dig[i]] + i;
-      const uint32_t p = s_pay[i];
-      if (PASS == PASS_D1 || PASS == PASS_S1) {
-        a.idx_a[pos] = p;
-        a.dig_a[pos] = s_hi[i];
-      } else if (PASS == PASS_D2 || PASS == PASS_M3) {
-        a.order[pos] = p;
-      } else if (PASS == PASS_M1) {
-        a.idx_a[pos] = p;
-        a.shi[pos] = s_hi[i];
-      } else if (PASS == PASS_M2) {
-        a.spay[pos] = p;
-        a.dig_a[pos] = (uint8_t)s_hi[i];
-      } else if (PASS >= PASS_P1) {
-        a.pout[pos] = p;
-      } else if (PASS == PASS_T1) {
-        if (a.t1_final) {
-          const float4 r0 = __ldg(a.proj_rec + 2 * (size_t)p);
-          const float4 r1 = __ldg(a.proj_rec + 2 * (size_t)p + 1);
-          a.inst_rec[2 * (size_t)pos] = r0;
-          a.inst_rec[2 * (size_t)pos + 1] = r1;
-        } else {
-          a.inst_idx_b[pos] = p;
-          a.inst_tile_b[pos] = s_hi[i];
-        }
-      } else {
-        const float4 r0 = __ldg(a.proj_rec + 2 * (size_t)p);
-        const float4 r1 = __ldg(a.proj_rec + 2 * (size_t)p + 1);
-        a.inst_rec[2 * (size_t)pos] = r0;
-        a.inst_rec[2 * (size_t)pos + 1] = r1;
-        a.inst_tile_f[pos] = s_hi[i];
-      }
-    }
-    __syncthreads();
-  }
-}
-
-// {start, end} of every tile's run in the final (tile, draw order) instance array; tiles without instances keep
-// the {0, 0} the per-frame memset wrote.  One thread per instance, neighbours compared.
-__global__ void __launch_bounds__(256) k_tile_ranges(const uint16_t *__restrict__ tile_f, FrameCounters *ctr,
-                                                     uint2 *__restrict__ range) {
-  GS_PDL_ENTRY();
-  const uint32_t n = ctr->overflow ? 0u : ctr->n_inst_kept;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const uint32_t t = tile_f[i];
-    if (i == 0 || tile_f[i - 1] != t) range[t].x = i;
-    if (i == n - 1 || tile_f[i + 1] != t) range[t].y = i + 1;
-  }
-}
-
 static int persistent_grid(gs_context *c, uint64_t n_elems, int per_cta, int ctas_per_sm) {
   uint64_t tiles = (n_elems + per_cta - 1) / per_cta;
   uint64_t cap = (uint64_t)c->sm_count * ctas_per_sm;
@@ -650,115 +284,474 @@ void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *s
   launch_chain(c, k_scene_keys, grid, 256, st, (const float *)c->depth, fp, scene, octr, ctr, c->scene_key, c->scene_pay);
 }
 
-static RadixArgs make_args(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b) {
-  RadixArgs a{};
-  a.ctr = ctr;
-  a.fp = fp;
-  a.depth = c->depth;
-  a.idx_a = c->idx_a;
-  a.dig_a = c->dig_a;
-  a.order = b.order;
-  a.inst_tile = c->inst_tile;
-  a.inst_idx = c->inst_idx;
-  a.inst_tile_b = c->inst_tile_b;
-  a.inst_tile_f = c->inst_tile_f;
-  a.inst_idx_b = c->inst_idx_b;
-  a.proj_rec = b.proj_rec;
-  a.inst_rec = b.inst_rec;
-  return a;
+// ---------------------------------------------------------------------------------------------
+// Stable 8-bit radix pass = three fully parallel kernels (no inter-CTA spinning):
+//   k_radix_hist<Pass>   : per-chunk (4096 elements) digit histogram        -> table[digit][chunk]
+//   k_radix_scan<Pass>   : per-digit exclusive scan over the chunks (in place) + digit totals
+//   k_radix_scatter<Pass>: per chunk: stable in-chunk ranks (warp match_any) + table offset -> scatter
+// A pass type holds the pointers of its pass and states:
+//   count()                 its element count, read from the device counters
+//   load(i, pay, carry)     the digit of element i (kInvalidDigit: skipped), its payload and the bits for the next pass
+//   Carry                   the type those bits are staged in (void: the pass carries nothing)
+//   store(pos, pay, carry)  the write-out of output slot pos
+// and overrides the hooks of RadixPass it needs.
+// ---------------------------------------------------------------------------------------------
+struct RadixScratch {
+  uint32_t *table;   // [256][stride]: per-chunk digit counts, scanned in place into per-chunk offsets
+  uint32_t *totals;  // [256]: digit totals
+  uint32_t stride;
+};
+
+struct RadixPass {
+  using Carry = void;
+  __device__ void prepare(uint32_t n) {}                // start of k_radix_hist and k_radix_scatter
+  __device__ void hist_prologue(uint32_t n) const {}    // start of k_radix_hist
+  __device__ void hist_epilogue() {}                    // end of k_radix_hist, every thread
+  __device__ void scanned(uint32_t total) const {}      // k_radix_scan: one digit's total
+  __device__ void digit_range(uint32_t d, uint32_t start, uint32_t end) const {}  // k_radix_scatter: digit d's output slots
+};
+
+template <class Pass>
+__global__ void __launch_bounds__(kRadixThreads) k_radix_hist(Pass p, const RadixScratch s) {
+  GS_PDL_ENTRY();
+  __shared__ uint32_t h[256];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t n = p.count();
+  const uint32_t num_chunks = (n + kRadixTile - 1) / kRadixTile;
+  p.prepare(n);
+  p.hist_prologue(n);
+  for (uint32_t c = blockIdx.x; c < num_chunks; c += gridDim.x) {
+    h[tid] = 0;
+    __syncthreads();
+    const uint32_t base = c * kRadixTile + warp * (32 * kRadixItems) + lane;
+#pragma unroll
+    for (int k = 0; k < kRadixItems; ++k) {
+      const uint32_t i = base + k * 32;
+      if (i < n) {
+        uint32_t pay, carry;
+        const uint32_t digit = p.load(i, pay, carry);
+        if (digit != kInvalidDigit) atomicAdd(&h[digit], 1u);
+      }
+    }
+    __syncthreads();
+    s.table[(size_t)tid * s.stride + c] = h[tid];
+    __syncthreads();
+  }
+  p.hist_epilogue();
 }
 
-template <int PASS>
-static void run_pass(gs_context *c, RadixArgs &a, uint64_t n_max, cudaStream_t st) {
-  const int grid = persistent_grid(c, n_max, kRadixTile, 8);
-  if (PASS != PASS_T1) launch_chain(c, k_radix_hist<PASS>, grid, kRadixThreads, st, a);
-  launch_chain(c, k_radix_scan<PASS>, 256, 256, st, a);
-  launch_chain(c, k_radix_scatter<PASS>, grid, kScatThreads, st, a);
-}
-
-// index.js:557-567 as two stable 8-bit passes -> b.order (6 launches)
-void launch_depth_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
-  RadixArgs a = make_args(c, fp, ctr, b);
-  a.table = c->table_n;
-  a.totals = c->totals;
-  a.stride = c->table_n_stride;
-  run_pass<PASS_D1>(c, a, c->cap, st);
-  run_pass<PASS_D2>(c, a, c->cap, st);
-}
-
-// scene frames: (draw rank, key, index) as three stable 8-bit passes -> b.order (9 launches)
-void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
-  RadixArgs a = make_args(c, fp, ctr, b);
-  a.table = c->table_n;
-  a.totals = c->totals;
-  a.stride = c->table_n_stride;
-  a.skey = c->scene_key;
-  a.spay = c->scene_pay;
-  a.shi = c->scene_hi;
-  run_pass<PASS_M1>(c, a, c->cap, st);
-  run_pass<PASS_M2>(c, a, c->cap, st);
-  run_pass<PASS_M3>(c, a, c->cap, st);
-}
-
-void launch_tile_ranges(gs_context *c, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
-
-// stable sort of the tile instances by tile id (5 launches: T1's histogram is produced by k_emit);
-// T2 writes the per-tile record lists
-void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, bool hist_t1, cudaStream_t st) {
-  RadixArgs a = make_args(c, nullptr, ctr, b);
-  a.t1_chunk_cols = hist_t1 ? 1u : 0u;
-  a.table = c->table_d;
-  a.totals = c->totals + 256;
-  a.stride = c->table_d_stride;
-  a.t1_final = n_bins <= 256u ? 1u : 0u;  // one byte of bin id: T1 alone sorts, gathers the records and writes the ranges
-  a.bin_range = b.bin_range;
-  a.n_bins = n_bins;
-  if (hist_t1) launch_chain(c, k_radix_hist<PASS_T1>, persistent_grid(c, c->cap_inst, kRadixTile, 8), kRadixThreads, st, a);
-  run_pass<PASS_T1>(c, a, c->cap_inst, st);
-  if (!a.t1_final) {
-    run_pass<PASS_T2>(c, a, c->cap_inst, st);
-    launch_tile_ranges(c, ctr, b, st);
+// grid = 256 CTAs (one per digit)
+template <class Pass>
+__global__ void __launch_bounds__(256) k_radix_scan(const Pass p, const RadixScratch s) {
+  GS_PDL_ENTRY();
+  __shared__ uint32_t s_warp[8];
+  __shared__ uint32_t s_carry;
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t n = p.count();
+  const uint32_t num_chunks = (n + kRadixTile - 1) / kRadixTile;
+  uint32_t *row = s.table + (size_t)blockIdx.x * s.stride;
+  if (tid == 0) s_carry = 0;
+  __syncthreads();
+  for (uint32_t b = 0; b < num_chunks; b += 256) {
+    const uint32_t i = b + tid;
+    const uint32_t v = (i < num_chunks) ? row[i] : 0u;
+    uint32_t incl = v;
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= (uint32_t)o) incl += t;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    uint32_t wbase = 0;
+    for (uint32_t k = 0; k < warp; ++k) wbase += s_warp[k];
+    const uint32_t carry = s_carry;
+    if (i < num_chunks) row[i] = carry + wbase + incl - v;
+    __syncthreads();
+    if (tid == 255) s_carry = carry + wbase + incl;
+    __syncthreads();
+  }
+  if (tid == 0) {
+    s.totals[blockIdx.x] = s_carry;
+    p.scanned(s_carry);
   }
 }
 
-// slab path: stable sort of the compacted slab by its 16-bit key (6 launches) -> b.order = the slab's draw order
-void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
-  RadixArgs a = make_args(c, fp, ctr, b);
-  a.table = c->table_n;
-  a.totals = c->totals;
-  a.stride = c->table_n_stride;
-  a.ckey = c->ckey;
-  a.cidx = c->cidx;
-  const int grid = persistent_grid(c, c->cap, kRadixTile, 8);
-  launch_chain(c, k_radix_hist<PASS_S1>, grid, kRadixThreads, st, a);
-  launch_chain(c, k_radix_scan<PASS_S1>, 256, 256, st, a);
-  launch_chain(c, k_radix_scatter<PASS_S1>, grid, kScatThreads, st, a);
-  run_pass<PASS_D2>(c, a, c->cap, st);
+// 512 threads x 8 elements per chunk: 16 warps rank their 256-element slices independently (an 8-step
+// dependent chain each), then one scan over the 16 warp counters per digit orders the slices.
+constexpr int kScatThreads = 512;
+constexpr int kScatItems = kRadixTile / kScatThreads;  // 8
+constexpr int kScatWarps = kScatThreads / 32;          // 16
+
+template <class Pass>
+__global__ void __launch_bounds__(kScatThreads, 2) k_radix_scatter(Pass p, const RadixScratch s) {
+  GS_PDL_ENTRY();
+  constexpr bool kCarry = !std::is_void<typename Pass::Carry>::value;
+  using carry_t = typename std::conditional<kCarry, typename Pass::Carry, uint8_t>::type;
+  __shared__ uint32_t wcnt[kScatWarps][256];
+  __shared__ uint32_t tile_off[256];  // global slot of the digit's first element MINUS its slot in the staged chunk
+  __shared__ uint32_t s_loc[256];     // slot of the digit's first element in the staged (locally sorted) chunk
+  __shared__ uint32_t s_warp_tot[8];
+  __shared__ uint32_t s_pay[kRadixTile];
+  __shared__ carry_t s_carry[kCarry ? kRadixTile : 1];
+  __shared__ uint8_t s_dig[kRadixTile];
+  __shared__ uint32_t s_total;
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t n = p.count();
+  const uint32_t num_chunks = (n + kRadixTile - 1) / kRadixTile;
+  if (blockIdx.x >= num_chunks) return;
+
+  // block-wide exclusive scan over the 256 digit slots (threads >= 256 contribute 0)
+  auto scan256 = [&](uint32_t v) -> uint32_t {
+    uint32_t incl = v;
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= (uint32_t)o) incl += t;
+    }
+    __syncthreads();  // previous users of s_warp_tot are done
+    if (lane == 31 && warp < 8) s_warp_tot[warp] = incl;
+    __syncthreads();
+    uint32_t wbase = 0;
+    for (uint32_t k = 0; k < warp && k < 8; ++k) wbase += s_warp_tot[k];
+    return wbase + incl - v;
+  };
+
+  // first output slot of each digit
+  const uint32_t dtot = tid < 256 ? s.totals[tid] : 0u;
+  const uint32_t dbase = scan256(dtot);
+  if (blockIdx.x == 0 && tid < 256) p.digit_range(tid, dbase, dbase + dtot);
+  p.prepare(n);
+
+  for (uint32_t c = blockIdx.x; c < num_chunks; c += gridDim.x) {
+    // this chunk's per-digit offset: issued first so its latency hides behind the ranking
+    const uint32_t toff = tid < 256 ? __ldg(s.table + (size_t)tid * s.stride + c) : 0u;
+    for (uint32_t k = tid; k < kScatWarps * 256; k += kScatThreads) (&wcnt[0][0])[k] = 0u;
+    // ---- load (warp-striped: consecutive lanes read consecutive elements) ----
+    const uint32_t base = c * kRadixTile + warp * (32 * kScatItems) + lane;
+    uint32_t digit[kScatItems], pay[kScatItems], rank[kScatItems];
+    carry_t carry[kScatItems];
+#pragma unroll
+    for (int k = 0; k < kScatItems; ++k) {
+      const uint32_t i = base + k * 32;
+      uint32_t cv = 0;
+      digit[k] = kInvalidDigit;
+      pay[k] = 0;
+      if (i < n) digit[k] = p.load(i, pay[k], cv);
+      carry[k] = (carry_t)cv;
+    }
+    __syncthreads();
+    // ---- stable rank inside the warp (input order = lane order within a step, steps in order) ----
+#pragma unroll
+    for (int k = 0; k < kScatItems; ++k) {
+      const uint32_t d = digit[k];
+      const uint32_t peers = __match_any_sync(0xffffffffu, d);
+      const uint32_t lt = __popc(peers & ((1u << lane) - 1u));
+      uint32_t prior = 0;
+      if (d != kInvalidDigit) prior = wcnt[warp][d];
+      __syncwarp();
+      if (d != kInvalidDigit && lt == 0) wcnt[warp][d] = prior + __popc(peers);
+      __syncwarp();
+      rank[k] = prior + lt;
+    }
+    __syncthreads();
+    // ---- thread `tid` < 256 owns digit `tid`: exclusive scan over the warps, then over the digits ----
+    uint32_t total = 0;
+    if (tid < 256) {
+#pragma unroll
+      for (int w = 0; w < kScatWarps; ++w) {
+        const uint32_t cnt = wcnt[w][tid];
+        wcnt[w][tid] = total;
+        total += cnt;
+      }
+    }
+    const uint32_t loc = scan256(total);
+    if (tid < 256) {
+      s_loc[tid] = loc;
+      tile_off[tid] = dbase + toff - loc;
+      if (tid == 255) s_total = loc + total;
+    }
+    __syncthreads();
+    // ---- stage the chunk in shared memory in sorted order ----
+#pragma unroll
+    for (int k = 0; k < kScatItems; ++k) {
+      const uint32_t d = digit[k];
+      if (d == kInvalidDigit) continue;
+      const uint32_t lp = s_loc[d] + wcnt[warp][d] + rank[k];
+      s_pay[lp] = pay[k];
+      s_dig[lp] = (uint8_t)d;
+      if (kCarry) s_carry[lp] = carry[k];
+    }
+    __syncthreads();
+    // ---- write out: consecutive threads write consecutive slots of the same digit run (coalesced) ----
+    const uint32_t nvalid = s_total;
+    for (uint32_t i = tid; i < nvalid; i += kScatThreads)
+      p.store(tile_off[s_dig[i]] + i, s_pay[i], kCarry ? (uint32_t)s_carry[i] : 0u);
+    __syncthreads();
+  }
 }
 
-// PLY ingest: stable ascending sort of n 32-bit keys, four 8-bit passes (12 launches) on the caller's scratch -> perm_b
+template <class Pass>
+static void run_pass(gs_context *c, const Pass &p, const RadixScratch &s, uint64_t n_max, cudaStream_t st) {
+  const int grid = persistent_grid(c, n_max, kRadixTile, 8);
+  launch_chain(c, k_radix_hist<Pass>, grid, kRadixThreads, st, p, s);
+  launch_chain(c, k_radix_scan<Pass>, 256, 256, st, p, s);
+  launch_chain(c, k_radix_scatter<Pass>, grid, kScatThreads, st, p, s);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Depth sort: index.js:557-567 as two stable 8-bit passes over the 16-bit key -> b.order (6 launches)
+// ---------------------------------------------------------------------------------------------
+// D1: low key byte of every splat the worker filter kept.  Counts the entries in range and those the reference's
+// typed-array store drops (quirk Q5).
+struct D1 : RadixPass {
+  using Carry = uint8_t;  // high key byte
+  FrameCounters *ctr;
+  const FrameParams *fp;  // fp->n_splats: resident splats of this frame
+  const float *depth;
+  uint32_t *idx_out; uint8_t *hi_out;
+  DepthRange dr;            // per thread, from prepare()
+  uint32_t n_in, n_drop;    // per thread
+  __device__ uint32_t count() const { return ctr->sort.n_valid ? fp->n_splats : 0u; }
+  __device__ void prepare(uint32_t n) { if (n) dr = load_depth_range(ctr); }
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) {
+    const float d = __ldg(depth + i);
+    if (d == GS_DEPTH_REJECT) return kInvalidDigit;
+    const int32_t key = depth_key(d, dr.min_depth, dr.depth_inv);
+    if (key < 0 || key > 65535) { ++n_drop; return kInvalidDigit; }  // typed-array store out of range: dropped (quirk Q5)
+    ++n_in;
+    pay = i;
+    carry = (uint32_t)key >> 8;
+    return key & 255;
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const { idx_out[pos] = pay; hi_out[pos] = (uint8_t)carry; }
+  __device__ void hist_epilogue() {
+    __shared__ uint32_t s_in, s_drop;
+    uint32_t in = n_in, drop = n_drop;
+    for (int o = 16; o > 0; o >>= 1) {
+      in += __shfl_xor_sync(0xffffffffu, in, o);
+      drop += __shfl_xor_sync(0xffffffffu, drop, o);
+    }
+    if (threadIdx.x == 0) { s_in = 0; s_drop = 0; }
+    __syncthreads();
+    if ((threadIdx.x & 31u) == 0) { if (in) atomicAdd(&s_in, in); if (drop) atomicAdd(&s_drop, drop); }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      if (s_in) atomicAdd(&ctr->sort.n_inrange, s_in);
+      if (s_drop) atomicAdd(&ctr->sort.n_dropped, s_drop);
+    }
+  }
+};
+
+// D2: high key byte -> the draw order.  Quirk Q5: the reference's output keeps length validCount and the slots never
+// written stay 0, so the histogram kernel zeroes order[n_inrange, n_valid).
+struct D2 : RadixPass {
+  const FrameCounters *ctr;
+  const uint8_t *dig; const uint32_t *idx;
+  uint32_t *order;
+  __device__ uint32_t count() const { return ctr->sort.n_inrange; }
+  __device__ void hist_prologue(uint32_t n) const {
+    const uint32_t nv = ctr->sort.n_valid;
+    for (uint32_t j = n + blockIdx.x * blockDim.x + threadIdx.x; j < nv; j += gridDim.x * blockDim.x) order[j] = 0u;
+  }
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &) const { pay = idx[i]; return dig[i]; }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t) const { order[pos] = pay; }
+};
+
+void launch_depth_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
+  const RadixScratch s{c->table_n, c->totals, c->table_n_stride};
+  run_pass(c, D1{{}, ctr, fp, c->depth, c->idx_a, c->dig_a}, s, c->cap, st);
+  run_pass(c, D2{{}, ctr, c->dig_a, c->idx_a, b.order}, s, c->cap, st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Slab path: stable sort of the compacted slab by its 16-bit key -> b.order = the slab's draw order (6 launches)
+// ---------------------------------------------------------------------------------------------
+// S1: low key byte of the current slab's compacted (key, index) pairs (gs_slab.cu)
+struct S1 : RadixPass {
+  using Carry = uint8_t;  // high key byte
+  const FrameCounters *ctr;
+  const uint16_t *key; const uint32_t *idx;
+  uint32_t *idx_out; uint8_t *hi_out;
+  __device__ uint32_t count() const { return ctr->sort.n_valid; }  // entries of the current slab (k_slab_begin)
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) const {
+    const uint32_t k = key[i];
+    carry = k >> 8;
+    pay = idx[i];
+    return k & 255u;
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const { idx_out[pos] = pay; hi_out[pos] = (uint8_t)carry; }
+};
+
+// S1, then D2 as in the depth sort
+void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
+  const RadixScratch s{c->table_n, c->totals, c->table_n_stride};
+  run_pass(c, S1{{}, ctr, c->ckey, c->cidx, c->idx_a, c->dig_a}, s, c->cap, st);
+  run_pass(c, D2{{}, ctr, c->dig_a, c->idx_a, b.order}, s, c->cap, st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Scene frames: (draw rank, key, index) as three stable 8-bit passes over the 24-bit key of k_scene_keys -> b.order.
+// Every sorted entry takes part, Q5 drops included.  9 launches.
+// ---------------------------------------------------------------------------------------------
+// M1: key bits 0-7
+struct M1 : RadixPass {
+  using Carry = uint16_t;  // key bits 8-23
+  const FrameCounters *ctr;
+  const FrameParams *fp;
+  const uint32_t *key, *pay_in;
+  uint32_t *idx_out; uint16_t *hi_out;
+  __device__ uint32_t count() const { return ctr->sort.n_valid ? fp->n_splats : 0u; }
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) const {
+    const uint32_t k = key[i];
+    if (k == kNoKey) return kInvalidDigit;
+    carry = k >> 8;
+    pay = pay_in[i];
+    return k & 255u;
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const { idx_out[pos] = pay; hi_out[pos] = (uint16_t)carry; }
+};
+
+// M2: key bits 8-15
+struct M2 : RadixPass {
+  using Carry = uint8_t;  // key bits 16-23
+  const FrameCounters *ctr;
+  const uint16_t *hi; const uint32_t *idx;
+  uint32_t *idx_out; uint8_t *hi_out;
+  __device__ uint32_t count() const { return ctr->sort.n_valid; }
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) const {
+    const uint32_t h = hi[i];
+    carry = h >> 8;
+    pay = idx[i];
+    return h & 255u;
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const { idx_out[pos] = pay; hi_out[pos] = (uint8_t)carry; }
+};
+
+// M3: key bits 16-23 -> the draw order
+struct M3 : RadixPass {
+  const FrameCounters *ctr;
+  const uint8_t *dig; const uint32_t *idx;
+  uint32_t *order;
+  __device__ uint32_t count() const { return ctr->sort.n_valid; }
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &) const { pay = idx[i]; return dig[i]; }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t) const { order[pos] = pay; }
+};
+
+void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
+  const RadixScratch s{c->table_n, c->totals, c->table_n_stride};
+  run_pass(c, M1{{}, ctr, fp, c->scene_key, c->scene_pay, c->idx_a, c->scene_hi}, s, c->cap, st);
+  run_pass(c, M2{{}, ctr, c->scene_hi, c->idx_a, c->scene_pay, c->dig_a}, s, c->cap, st);
+  run_pass(c, M3{{}, ctr, c->dig_a, c->scene_pay, b.order}, s, c->cap, st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Bin sort: stable sort of the emitted instances by their 16-bit bin id (kNoTile: rejected by the footprint test,
+// dropped); the final pass gathers the 32 B projected record of every instance into its per-bin slot
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void gather_record(const float4 *rec, float4 *inst_rec, uint32_t splat, uint32_t pos) {
+  const float4 r0 = __ldg(rec + 2 * (size_t)splat);
+  const float4 r1 = __ldg(rec + 2 * (size_t)splat + 1);
+  inst_rec[2 * (size_t)pos] = r0;
+  inst_rec[2 * (size_t)pos + 1] = r1;
+}
+
+// T1: low byte of the bin id.  `last` (at most 256 bins: the id is one byte): T1 is the whole sort, gathers the records
+// and writes the per-bin {start, end}, which fall out of the digit totals (no k_tile_ranges launch).
+struct T1 : RadixPass {
+  using Carry = uint16_t;  // the whole bin id, for T2
+  FrameCounters *ctr;
+  const uint16_t *bin; const uint32_t *idx;  // emitted instances
+  uint16_t *bin_out; uint32_t *idx_out;      // not last: T2's input
+  const float4 *proj_rec; float4 *inst_rec; uint2 *bin_range;  // last
+  uint32_t n_bins;
+  bool last;
+  __device__ uint32_t count() const { return ctr->overflow ? 0u : (uint32_t)ctr->n_inst; }
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) const {
+    const uint16_t t = bin[i];
+    if (t == kNoTile) return kInvalidDigit;
+    carry = t;
+    pay = idx[i];
+    return t & 255;
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const {
+    if (last) gather_record(proj_rec, inst_rec, pay, pos);
+    else { idx_out[pos] = pay; bin_out[pos] = (uint16_t)carry; }
+  }
+  __device__ void scanned(uint32_t total) const { if (total) atomicAdd(&ctr->n_inst_kept, total); }
+  __device__ void digit_range(uint32_t d, uint32_t start, uint32_t end) const {
+    if (last && d < n_bins) bin_range[d] = make_uint2(start, end);
+  }
+};
+
+// T2: high byte of the bin id
+struct T2 : RadixPass {
+  using Carry = uint16_t;  // the bin id, for k_tile_ranges
+  const FrameCounters *ctr;
+  const uint16_t *bin; const uint32_t *idx;  // T1's output
+  const float4 *proj_rec; float4 *inst_rec; uint16_t *bin_out;
+  __device__ uint32_t count() const { return ctr->overflow ? 0u : ctr->n_inst_kept; }
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) const {
+    const uint16_t t = bin[i];
+    carry = t;
+    pay = idx[i];
+    return (uint32_t)t >> 8;
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const {
+    gather_record(proj_rec, inst_rec, pay, pos);
+    bin_out[pos] = (uint16_t)carry;
+  }
+};
+
+// {start, end} of every tile's run in the final (tile, draw order) instance array; tiles without instances keep
+// the {0, 0} the per-frame memset wrote.  One thread per instance, neighbours compared.
+__global__ void __launch_bounds__(256) k_tile_ranges(const uint16_t *__restrict__ tile_f, FrameCounters *ctr,
+                                                     uint2 *__restrict__ range) {
+  GS_PDL_ENTRY();
+  const uint32_t n = ctr->overflow ? 0u : ctr->n_inst_kept;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint32_t t = tile_f[i];
+    if (i == 0 || tile_f[i - 1] != t) range[t].x = i;
+    if (i == n - 1 || tile_f[i + 1] != t) range[t].y = i + 1;
+  }
+}
+
+// 3 launches up to 256 bins, else 7 (T2 and k_tile_ranges)
+void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, cudaStream_t st) {
+  const RadixScratch s{c->table_d, c->totals + 256, c->table_d_stride};
+  const bool last = n_bins <= 256u;
+  run_pass(c, T1{{}, ctr, c->inst_tile, c->inst_idx, c->inst_tile_b, c->inst_idx_b, b.proj_rec, b.inst_rec, b.bin_range, n_bins, last},
+           s, c->cap_inst, st);
+  if (last) return;
+  run_pass(c, T2{{}, ctr, c->inst_tile_b, c->inst_idx_b, b.proj_rec, b.inst_rec, c->inst_tile_f}, s, c->cap_inst, st);
+  launch_chain(c, k_tile_ranges, persistent_grid(c, c->cap_inst, 256 * 8, 8), 256, st, (const uint16_t *)c->inst_tile_f, ctr,
+               b.bin_range);
+}
+
+// ---------------------------------------------------------------------------------------------
+// PLY ingest: stable ascending sort of n 32-bit importance keys, four 8-bit passes on the caller's scratch (12 launches)
+// ---------------------------------------------------------------------------------------------
+// P<kShift>: key bits kShift .. kShift+7, read through the previous pass's permutation (P<0>: the identity)
+template <int kShift>
+struct P : RadixPass {
+  const uint32_t *key, *perm;
+  uint32_t *perm_out;
+  uint32_t n;
+  __device__ uint32_t count() const { return n; }
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &) const {
+    const uint32_t row = kShift == 0 ? i : perm[i];
+    pay = row;
+    return (__ldg(key + row) >> kShift) & 255u;
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t) const { perm_out[pos] = pay; }
+};
+
 uint32_t *launch_ply_sort(gs_context *c, const uint32_t *key, uint32_t *perm_a, uint32_t *perm_b, uint32_t *table,
                           uint32_t *totals, uint32_t n, cudaStream_t st) {
-  RadixArgs a{};
-  a.table = table;
-  a.totals = totals;
-  a.stride = (n + kRadixTile - 1) / kRadixTile + 1;
-  a.pkey = key;
-  a.pn = n;
-  a.pout = perm_a;
-  run_pass<PASS_P1>(c, a, n, st);
-  a.pin = perm_a; a.pout = perm_b;
-  run_pass<PASS_P2>(c, a, n, st);
-  a.pin = perm_b; a.pout = perm_a;
-  run_pass<PASS_P3>(c, a, n, st);
-  a.pin = perm_a; a.pout = perm_b;
-  run_pass<PASS_P4>(c, a, n, st);
+  const RadixScratch s{table, totals, (n + kRadixTile - 1) / kRadixTile + 1};
+  run_pass(c, P<0>{{}, key, nullptr, perm_a, n}, s, n, st);
+  run_pass(c, P<8>{{}, key, perm_a, perm_b, n}, s, n, st);
+  run_pass(c, P<16>{{}, key, perm_b, perm_a, n}, s, n, st);
+  run_pass(c, P<24>{{}, key, perm_a, perm_b, n}, s, n, st);
   return perm_b;
-}
-
-void launch_tile_ranges(gs_context *c, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
-  const int grid = persistent_grid(c, c->cap_inst, 256 * 8, 8);
-  launch_chain(c, k_tile_ranges, grid, 256, st, (const uint16_t *)c->inst_tile_f, ctr, b.bin_range);
 }
 
 }  // namespace gs

@@ -253,8 +253,7 @@ def test_render_async_pipeline(gs, orc, ctx):
             st = ctx.wait(tickets[i - 1])
             bs = ctx._lib.gs_bin_size()
             n_bins = -(-640 // bs) * -(-360 // bs)
-            by_entry = os.environ.get("GS_EMIT", "entries") != "windows"  # emission by entry adds k_radix_hist<T1>
-            assert st.n_sorted > 0 and st.kernel_launches == (13 if n_bins <= 256 else 17) + (1 if by_entry else 0)
+            assert st.n_sorted > 0 and st.kernel_launches == (14 if n_bins <= 256 else 18)
             assert np.array_equal(outs[i - 1], ref[i - 1])
     ctx.wait(tickets[-1])
     assert np.array_equal(outs[-1], ref[-1])

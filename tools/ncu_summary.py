@@ -96,7 +96,7 @@ def stage_traffic(src, key, pattern, dst_dir):
     mult = {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
     per = collections.OrderedDict()
     for r in rows[2:]:
-        name = r[ik].split("(RadixArgs")[0].split("(const")[0].strip()
+        name = r[ik].split("(")[0].strip()
         if not re.search(pattern, name):
             continue
         b = float(r[ir].replace(",", "")) * mult[units[ir]] + float(r[iw].replace(",", "")) * mult[units[iw]]
