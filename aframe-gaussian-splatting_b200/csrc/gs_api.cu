@@ -203,7 +203,10 @@ static void drop_graphs(gs_context *c) {
   for (auto &sl : c->slot)
     for (int i = 0; i < 2; ++i) {
       kill(sl.graph_a[i][0]); kill(sl.graph_a[i][1]); kill(sl.graph_as[i]); kill(sl.graph_b[i]); kill(sl.graph_r[i]); kill(sl.graph_rp[i]);
-      kill(sl.graph_sa[i]); kill(sl.graph_sl[i][0]); kill(sl.graph_sl[i][1]); kill(sl.graph_sl[i][2]);
+      for (int q = 0; q < 2; ++q) {
+        kill(sl.graph_sa[i][q]);
+        for (auto &g : sl.graph_sl[i][q]) kill(g);
+      }
     }
 }
 
@@ -591,6 +594,11 @@ static int build_scene_table(gs_context *c, const gs_object *objs, uint32_t n_ob
     if ((uint64_t)objs[idx[j - 1]].first + objs[idx[j - 1]].count > objs[idx[j]].first)
       return fail(c, GS_ERR_INVALID, "scene: entity ranges overlap");
   t.n = (uint32_t)idx.size();
+  // slab path: B = 4096 >> ceil(log2(n_objs)) buckets per draw rank (gs_common.cuh slab_bucket)
+  uint32_t rank_bits = 0;
+  while ((1u << rank_bits) < n_objs) ++rank_bits;
+  t.bucket_bits = 12u - rank_bits;
+  t.pad[0] = t.pad[1] = 0;
   for (size_t j = 0; j < idx.size(); ++j) {
     const gs_object &g = objs[idx[j]];
     SceneObject &o = t.obj[j];
@@ -850,20 +858,24 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
 // growth the few bins that stay open force much larger slabs through sort + projection)
 static uint64_t slab_cumulative(uint32_t first, int k) { return (uint64_t)first * ((1ull << k) - 1ull); }
 
-// Stage A of a slab frame (sort stream): depth + cull, keys + bucket histogram, slab plan, pixel-state reset.
+// Stage A of a slab frame (sort stream): depth + cull, keys + bucket histogram, slab plan, every slab's compaction offsets.
+// A scene frame takes the per-entity depth pass and 24-bit keys (the scene table was copied to sl.scene_dev ahead of it).
 static cudaError_t enqueue_slab_keys_stage(gs_context *c, gs_context::Slot &sl, bool external_events) {
   auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
     return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
   };
   cudaStream_t st = c->stream;
+  const SceneTable *scene = sl.scene ? sl.scene_dev : nullptr;
   cudaError_t e;
   if ((e = cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, st))) return e;
   if ((e = cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), st))) return e;
+  if (scene && (e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, st))) return e;
   if ((e = rec(sl.ev[0], st))) return e;
-  launch_depth_cull(c, sl.fp, sl.ctr, st);
-  launch_keys(c, sl.fp, sl.ctr, sl.set, st);
+  if (scene) launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, st);
+  else launch_depth_cull(c, sl.fp, sl.ctr, st);
+  launch_keys(c, sl.fp, sl.ctr, scene, sl.octr, sl.set, st);
   launch_slab_plan(c, sl.fp, sl.ctr, sl.set, c->slab_first, sl.n_slabs, st);
-  launch_compact_offsets(c, sl.fp, sl.set, sl.n_slabs, st);  // one pass over the keys for every slab's compaction offsets
+  launch_compact_offsets(c, sl.fp, scene, sl.set, sl.n_slabs, st);  // one pass over the keys for every slab's compaction offsets
   if ((e = rec(sl.ev[1], st))) return e;
   return cudaGetLastError();
 }
@@ -877,13 +889,14 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
   };
   cudaStream_t st = c->rstream;
   const FrameBufs b = slot_bufs(c, sl);
+  const SceneTable *scene = sl.scene ? sl.scene_dev : nullptr;
   cudaError_t e;
   launch_slab_init(c, sl.fp, sl.ctr, st);
   if ((e = rec(sl.ev[2], st))) return e;
   for (int s = 0; s < sl.n_slabs; ++s) {
-    launch_slab_begin(c, sl.fp, sl.ctr, sl.set, s, st);   // entry count (0 once every bin is closed) + compaction
-    launch_slab_sort(c, sl.fp, sl.ctr, b, st);            // draw order of the slab
-    launch_project_entries(c, sl.fp, sl.ctr, b, st);      // vertex shader for the slab's entries
+    launch_slab_begin(c, sl.fp, sl.ctr, scene, sl.set, s, st);   // entry count (0 once every bin is closed) + compaction
+    launch_slab_sort(c, sl.fp, sl.ctr, scene, b, st);            // draw order of the slab
+    launch_project_entries(c, sl.fp, sl.ctr, scene, b, st);      // vertex shader for the slab's entries
     if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, st))) return e;
     launch_emit(c, sl.fp, sl.ctr, b, c->bin_open, st);
     launch_tile_radix(c, sl.ctr, b, n_bins, st);
@@ -911,14 +924,15 @@ static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_ti
     drop_graphs(c);
     c->gkey = k;
   }
-  const int set = sl.set;
-  // slabs of slab_first, 2x, 4x ... entries: enough of them to cover every resident splat
+  const int set = sl.set, kind = sl.scene ? 1 : 0;  // plain and scene frames keep their own graphs
+  // slabs of slab_first, 2x, 4x ... entries: enough of them to cover every splat the sort considers
   int n_slabs = 1;
-  while (n_slabs < kMaxSlabs && slab_cumulative(c->slab_first, n_slabs) < sl.n_splats) ++n_slabs;
-  if (n_slabs != sl.graph_slabs[set]) {  // the captured loop bakes the slab count
+  while (n_slabs < kMaxSlabs && slab_cumulative(c->slab_first, n_slabs) < sl.n_sortable) ++n_slabs;
+  if (n_slabs != sl.graph_slabs[set][kind]) {  // the captured stages bake the slab count
     auto kill = [](cudaGraphExec_t &g) { if (g) { cudaGraphExecDestroy(g); g = nullptr; } };
-    kill(sl.graph_sa[set]); kill(sl.graph_sl[set][0]); kill(sl.graph_sl[set][1]); kill(sl.graph_sl[set][2]);
-    sl.graph_slabs[set] = n_slabs;
+    kill(sl.graph_sa[set][kind]);
+    for (auto &g : sl.graph_sl[set][kind]) kill(g);
+    sl.graph_slabs[set][kind] = n_slabs;
   }
   sl.n_slabs = n_slabs;
   for (int s = 0; s < n_slabs; ++s)
@@ -926,7 +940,7 @@ static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_ti
       if (!sl.slab_ev[s][q]) GS_CUDA(c, cudaEventCreate(&sl.slab_ev[s][q]));
   // A: the keys / slab table of this set must no longer be read by the loop that used them last
   if (c->sort_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->sort_set_free[set], 0));
-  int rc = run_graph(c, sl.graph_sa[set], c->stream, [&](bool ext) { return enqueue_slab_keys_stage(c, sl, ext); });
+  int rc = run_graph(c, sl.graph_sa[set][kind], c->stream, [&](bool ext) { return enqueue_slab_keys_stage(c, sl, ext); });
   if (rc) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_sorted, c->stream));
   // loop: needs A of this frame; consecutive loops are ordered by the stream itself
@@ -935,13 +949,14 @@ static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_ti
   const int variant = sl.peer ? 2 : ((sl.raster_flags & 2u) ? 1 : 0);
   if (sl.peer && (sl.raster_flags & 2u)) {  // depth-tested peer frames: rare, plain launches
     GS_CUDA(c, enqueue_slab_loop_stage(c, sl, n_tiles, n_bins, false));
-  } else if ((rc = run_graph(c, sl.graph_sl[set][variant], c->rstream,
+  } else if ((rc = run_graph(c, sl.graph_sl[set][kind][variant], c->rstream,
                              [&](bool ext) { return enqueue_slab_loop_stage(c, sl, n_tiles, n_bins, ext); }))) {
     return rc;
   }
   GS_CUDA(c, cudaEventRecord(sl.ev_binned, c->rstream));
   c->sort_set_free[set] = sl.ev_binned;
-  sl.launches = 6u + 1u + (uint32_t)n_slabs * (n_bins <= 256u ? 16u : 20u) + 2u;
+  // scene frames: three radix passes per slab instead of two
+  sl.launches = 6u + 1u + (uint32_t)n_slabs * ((n_bins <= 256u ? 16u : 20u) + (sl.scene ? 3u : 0u)) + 2u;
   return GS_OK;
 }
 
@@ -1193,10 +1208,16 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   }
   if (!scene && (p->flags & GS_RENDER_REUSE_SORT) && c->have_order && (rcode = drain(c))) return rcode;  // runs in the last sort's buffers
   if ((p->flags & GS_RENDER_STATS) && (rcode = drain(c))) return rcode;  // the per-tile statistics buffer is not double-buffered
-  // large scenes render front to back in depth slabs; the two paths share scratch buffers, so a change drains
-  // (the criterion is the number of SORTED splats: the last frame's count when there is one, else the resident count)
-  const uint32_t expect_sorted = c->have_last_sorted ? c->last_sorted : c->n;
-  const bool slab = !scene && expect_sorted >= c->slab_min && !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS));
+  // large scenes render front to back in depth slabs, plain and scene frames alike; the one-pass and slab paths share
+  // scratch buffers, so a change drains (the criterion is the number of SORTED splats: the last frame's count when there
+  // is one, else the splats the sort considers - the resident ones, or those in the scene's entity ranges)
+  uint32_t sortable = c->n;
+  if (scene) {
+    sortable = 0;
+    for (uint32_t k = 0; k < scene->n; ++k) sortable += scene->obj[k].end - scene->obj[k].first;
+  }
+  const uint32_t expect_sorted = c->have_last_sorted ? c->last_sorted : sortable;
+  const bool slab = expect_sorted >= c->slab_min && !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS));
   if ((int)slab != c->last_mode) {
     if ((rcode = drain(c))) return rcode;
     GS_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1229,6 +1250,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   sl.out_user = out_rgba;
   sl.ticket = ticket;
   sl.n_splats = c->n;
+  sl.n_sortable = sortable;
   sl.slab = slab;
   sl.color_in = color_in;
   sl.color_device = (p->flags & GS_RENDER_COLOR_DEVICE) != 0;

@@ -132,7 +132,8 @@ struct SceneObject {
 };
 struct SceneTable {
   uint32_t n;            // non-empty entities, sorted by `first` (empty ones draw nothing and are left out)
-  uint32_t pad[3];
+  uint32_t bucket_bits;  // slab path: log2 of the slab buckets per draw rank, 12 - ceil(log2(caller's entity count))
+  uint32_t pad[2];
   SceneObject obj[kMaxObjects];
 };
 // per-entity results of the depth pass (one worker's min / max / validCount, index.js:548-555)
@@ -169,8 +170,17 @@ int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_
 
 // ---- front-to-back slab path ----
 constexpr int kMaxSlabs = 12;         // geometric slab sizes: 1 M, 2 M, 4 M ... entries (nearest first)
-constexpr int kSlabBuckets = 4096;     // slab boundaries are chosen on a 4096-bucket histogram of the 16-bit keys
+constexpr int kSlabBuckets = 4096;     // slab boundaries are chosen on a 4096-bucket histogram of the sort keys
 constexpr uint32_t kNoKey = 0xFFFFFFFFu;
+// Slab bucket of a sort key (never kNoKey).  Plain frames: the 16-bit key's top 12 bits.  Scene frames, 24-bit key
+// rank << 17 | key17 (key17 = 16-bit key, or 65536 for a quirk-Q5 drop): draw rank r owns the B = 2^bits buckets
+// [r B, (r + 1) B) (SceneTable::bucket_bits), and key17 >> (16 - bits) picks one of them; a Q5 drop falls into the
+// entity's top bucket.  Either way the bucket order is the draw order, so slabs cut from the top are nearest first.
+template <bool SCENE>
+__device__ __forceinline__ uint32_t slab_bucket(uint32_t key, uint32_t bits) {
+  if (!SCENE) return key >> 4;
+  return ((key >> 17) << bits) | min((key & 0x1FFFFu) >> (16u - bits), (1u << bits) - 1u);
+}
 struct SlabTable {
   uint32_t hist[kSlabBuckets];  // entries per 16-key bucket
   uint32_t klo[kMaxSlabs];      // slab s holds the keys [klo[s], khi[s])
@@ -229,7 +239,7 @@ struct gs_context {
   uint32_t slab_cap = 0;           // splats the per-splat slab buffers are sized for
   uint32_t *key32[2] = {nullptr, nullptr};  // [cap] 16-bit depth key of every splat, kNoKey if not in the sort (one per set)
   uint32_t *cidx = nullptr;        // [cap] splat indices of the current slab, in index order
-  uint16_t *ckey = nullptr;        // [cap] their keys
+  uint16_t *ckey = nullptr;        // [cap] their keys (scene frames: 24-bit keys in scene_key)
   uint32_t *chunk_cnt[2] = {nullptr, nullptr};  // [kMaxSlabs][chunk_row] per-slab compaction offsets of every 2048-splat chunk (one per set)
   uint32_t chunk_row = 0;          // row stride of chunk_cnt: cap / 2048 + 4
   gs::SlabTable *slab_tab[2] = {nullptr, nullptr};
@@ -247,6 +257,7 @@ struct gs_context {
   uint32_t tile_stats_cap = 0;
   // ---- scene frames: sort keys of the three-pass (entity, key, index) sort, allocated by the first scene frame ----
   uint32_t scene_cap = 0;
+  // (scene slab frames: scene_key holds the current slab's compacted keys, the other two serve its sort as below)
   uint32_t *scene_key = nullptr;   // [cap] (draw rank << 17 | 16-bit key, or 65536 for a quirk-Q5 drop), kNoKey if not sorted
   uint32_t *scene_pay = nullptr;   // [cap] payload of pass 1 (splat index, or the entity's first splat for a Q5 drop);
                                    //       reused as pass 2's index output
@@ -282,6 +293,7 @@ struct gs_context {
     gs::ObjCounters *octr = nullptr;         // [kMaxObjects] per-entity depth-pass results
     uint32_t raster_flags = 0;               // k_raster instantiation of this frame (packed | depth | stats)
     uint32_t n_splats = 0;                   // resident splats when the frame was submitted
+    uint32_t n_sortable = 0;                 // splats the frame's sort considers (scene frames: in the entities' ranges)
     bool slab = false;                       // rendered by the front-to-back slab path
     int n_slabs = 0;
     cudaEvent_t slab_ev[gs::kMaxSlabs][2] = {};  // raster of each slab (timing)
@@ -294,9 +306,9 @@ struct gs_context {
     cudaGraphExec_t graph_b[2] = {nullptr, nullptr};                           // binning, [set]
     cudaGraphExec_t graph_r[2] = {nullptr, nullptr};                           // raster, [set]
     cudaGraphExec_t graph_rp[2] = {nullptr, nullptr};                          // acquire + raster + signal/wait (fused exchange)
-    cudaGraphExec_t graph_sa[2] = {nullptr, nullptr};                          // slab path: keys stage, [set]
-    cudaGraphExec_t graph_sl[2][3] = {{nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}};  // slab path: slab loop + resolve, [set][plain | depth | peer]
-    int graph_slabs[2] = {0, 0};                                               // slab count baked into graph_sl
+    cudaGraphExec_t graph_sa[2][2] = {};       // slab path: keys stage, [set][plain | scene frame]
+    cudaGraphExec_t graph_sl[2][2][3] = {};    // slab path: slab loop + resolve, [set][plain | scene frame][plain | depth | peer]
+    int graph_slabs[2][2] = {};                // slab count baked into graph_sa / graph_sl, [set][plain | scene frame]
     bool peer = false;
     uint64_t ticket = 0;
     int ring = 0;                            // slot of the shared frame ring (fused exchange)
@@ -409,13 +421,19 @@ struct PeerRows { unsigned long long *p[kMaxPeers]; };
 void launch_peer_release(gs_context *c, const PeerRows &rows, uint32_t world, uint32_t rank, unsigned long long seq,
                          cudaStream_t st);
 // ---- slab path launchers (gs_slab.cu / gs_raster.cu) ----
-void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, cudaStream_t st);  // keys + bucket histogram
+// scene: the slot's scene table (device) of a scene frame, NULL for a plain frame; octr: its per-entity depth ranges
+void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const ObjCounters *octr, int set,
+                 cudaStream_t st);  // keys + bucket histogram
 void launch_slab_plan(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, uint32_t first_target, int n_slabs, cudaStream_t st);
 void launch_slab_init(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
-void launch_compact_offsets(gs_context *c, const FrameParams *fp, int set, int n_slabs, cudaStream_t st);  // every slab's chunk offsets: 2 launches
-void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, int slab, cudaStream_t st);  // + compaction: 2 launches
-void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 6 launches
-void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
+void launch_compact_offsets(gs_context *c, const FrameParams *fp, const SceneTable *scene, int set, int n_slabs,
+                            cudaStream_t st);  // every slab's chunk offsets: 2 launches
+void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, int set, int slab,
+                       cudaStream_t st);  // + compaction: 2 launches
+void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
+                      cudaStream_t st);  // 6 launches (scene frames: 9)
+void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
+                            cudaStream_t st);
 void launch_slab_end(gs_context *c, FrameCounters *ctr, cudaStream_t st);
 void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, uint32_t n_tiles, const FrameBufs &b, bool depth,
                         cudaStream_t st);

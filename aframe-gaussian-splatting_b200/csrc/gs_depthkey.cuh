@@ -33,4 +33,34 @@ __device__ __forceinline__ DepthRange load_depth_range(const FrameCounters *ctr)
   return r;
 }
 
+// Scene frames: one worker per entity (index.js:229-236), each with its own depth range and 16-bit key space.  Held in
+// shared memory by the kernels that key a scene (k_scene_keys, k_keys<true>).
+struct SceneKeyTable {
+  uint32_t first[kMaxObjects], end[kMaxObjects], tag[kMaxObjects];
+  double min[kMaxObjects], inv[kMaxObjects];
+  uint32_t n;
+  // every thread of the CTA; a __syncthreads() must follow before the first key()
+  __device__ void load(const SceneTable *__restrict__ scene, const ObjCounters *__restrict__ octr) {
+    const uint32_t n_obj = scene->n;
+    if (threadIdx.x == 0) n = n_obj;
+    for (uint32_t k = threadIdx.x; k < n_obj; k += blockDim.x) {
+      first[k] = scene->obj[k].first;
+      end[k] = scene->obj[k].end;
+      tag[k] = scene->obj[k].rank << 17;
+      // the entity's own range (index.js:552-558), as load_depth_range does for a single worker
+      const double mn = dec_f64(~octr[k].min_enc), mx = dec_f64(octr[k].max_enc);
+      min[k] = mn;
+      inv[k] = __ddiv_rn(65535.0, __dsub_rn(mx, mn));
+    }
+  }
+  // 24-bit key of sorted splat i (f32 depth d): draw rank << 17 | the entity's 16-bit key, or | 65536 for a key outside
+  // [0, 65535] (quirk Q5: the worker's slot stays 0, the entity's first splat, after all its in-range entries).
+  // obj: the entity's table index.
+  __device__ uint32_t key(uint32_t i, float d, int &obj) const {
+    obj = scene_find(first, end, n, i);  // a sorted splat always lies in an entity's range
+    const int32_t q = depth_key(d, min[obj], inv[obj]);
+    return tag[obj] | ((q >= 0 && q <= 65535) ? (uint32_t)q : 65536u);
+  }
+};
+
 }  // namespace gs

@@ -146,8 +146,8 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
 // Index order, sparse frames (fewer than half of the resident splats passed the worker filter, e.g. a cutout box): the
 // survivors of every 1024-splat chunk are first compacted into shared memory, so the shader runs in full warps
 // instead of warps with a few live lanes each.
-// SCENE (scene frames, index order): every splat takes its entity's modelview, and the splat the Q5 tail may repeat is
-// each entity's first one.
+// SCENE (scene frames, by index or, on the slab path, by entry): every splat takes its entity's modelview; by index, the
+// splat the Q5 tail may repeat is each entity's first one.
 template <bool BY_ENTRY, bool SCENE = false>
 __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, const uint4 *__restrict__ cc,
                                                  const float *__restrict__ depth,
@@ -464,13 +464,16 @@ void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable
                (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene);
 }
 
-void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t stream) {
+// scene: the slot's scene table for a scene frame (every entry takes its entity's modelview), NULL for a plain frame
+void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
+                            cudaStream_t stream) {
   uint64_t blocks = ((uint64_t)c->cap + 255) / 256;
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  launch_chain(c, k_project<true>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
-               (const uint32_t *)b.order, (const FrameCounters *)ctr, (const SceneTable *)nullptr);
+  launch_chain(c, scene ? k_project<true, true> : k_project<true>, (int)blocks, 256, stream, (const float4 *)c->center_scale,
+               (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)b.order,
+               (const FrameCounters *)ctr, scene);
 }
 
 void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,

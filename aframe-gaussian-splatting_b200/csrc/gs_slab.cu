@@ -24,6 +24,15 @@
 // reference's (16-bit bucket, index) order.  Quirk Q5 (keys outside [0, 65535] are dropped and leave zeros at the END
 // of the reference's index array, i.e. extra draws of splat 0 in front of everything): slab 0 is given that many
 // extra entries for splat 0 behind its real ones.
+//
+// Scene frames (several entities, gs_render_scene) use the same machinery on the axis of their one-pass sort: the 24-bit
+// key rank << 17 | key17 of k_scene_keys, drawn in (rank, key17, index) order.  The 4096 buckets are split evenly
+// between the draw ranks (slab_bucket), so slabs are again contiguous and nearest first.  An entity's Q5 drops are real
+// entries with key17 = 65536 (its top bucket), compacted and sorted like the others; the pass SM1 turns each into a draw
+// of the entity's first splat.  The per-slab sort is SM1, M2, M3 over the compacted 24-bit keys, and the projection
+// takes each entry's entity modelview (k_project<true, true>).
+#include <type_traits>
+
 #include "gs_common.cuh"
 #include "gs_depthkey.cuh"
 
@@ -34,30 +43,46 @@ constexpr int kCompactItems = 8;
 constexpr int kCompactChunk = kCompactThreads * kCompactItems;  // 2048 splats per compaction chunk
 
 // ---------------------------------------------------------------------------------------------
-// keys of all splats + bucket histogram (index.js:557-563)
+// keys of all splats + bucket histogram (index.js:557-563).  Plain frames: the 16-bit key, kNoKey for a quirk-Q5 drop.
+// SCENE: the 24-bit key of k_scene_keys (each entity's own range); a Q5 drop is a real entry at the top of its entity.
 // ---------------------------------------------------------------------------------------------
+template <bool SCENE>
 __global__ void __launch_bounds__(256) k_keys(const float *__restrict__ depth, const FrameParams *__restrict__ fp,
-                                              FrameCounters *ctr, uint32_t *__restrict__ key32, SlabTable *tab) {
+                                              FrameCounters *ctr, uint32_t *__restrict__ key32, SlabTable *tab,
+                                              const SceneTable *__restrict__ scene, const ObjCounters *__restrict__ octr) {
   __shared__ uint32_t h[kSlabBuckets];
   __shared__ uint32_t s_in, s_drop;
+  __shared__ typename std::conditional<SCENE, SceneKeyTable, uint32_t>::type s_ent;
   const uint32_t tid = threadIdx.x;
   for (uint32_t i = tid; i < (uint32_t)kSlabBuckets; i += blockDim.x) h[i] = 0;
   if (tid == 0) { s_in = 0; s_drop = 0; }
+  DepthRange dr{0.0, 0.0};
+  uint32_t bits = 0;
+  if constexpr (SCENE) {
+    s_ent.load(scene, octr);
+    bits = scene->bucket_bits;
+  } else {
+    if (ctr->sort.n_valid) dr = load_depth_range(ctr);
+  }
   __syncthreads();
   const uint32_t n = fp->n_splats;
-  DepthRange dr{0.0, 0.0};
-  if (ctr->sort.n_valid) dr = load_depth_range(ctr);
   uint32_t in = 0, drop = 0;
-  auto key_of = [&](float d) -> uint32_t {
+  auto key_of = [&](uint32_t i, float d) -> uint32_t {
     if (d == GS_DEPTH_REJECT) return kNoKey;
-    const int32_t k = depth_key(d, dr.min_depth, dr.depth_inv);
-    if (k >= 0 && k <= 65535) {
-      atomicAdd(&h[(uint32_t)k >> 4], 1u);
-      ++in;
-      return (uint32_t)k;
+    uint32_t key;
+    bool dropped;  // typed-array write out of range (quirk Q5)
+    if constexpr (SCENE) {
+      int obj;
+      key = s_ent.key(i, d, obj);
+      dropped = (key & 65536u) != 0u;
+    } else {
+      const int32_t k = depth_key(d, dr.min_depth, dr.depth_inv);
+      dropped = k < 0 || k > 65535;
+      key = dropped ? kNoKey : (uint32_t)k;
     }
-    ++drop;  // typed-array write out of range: dropped (quirk Q5)
-    return kNoKey;
+    if (dropped) ++drop; else ++in;
+    if (key != kNoKey) atomicAdd(&h[slab_bucket<SCENE>(key, bits)], 1u);
+    return key;
   };
   // four splats per thread and step: the loads of a step are independent, so a thread keeps 16 B in flight instead
   // of 4 (one load per dependent iteration made this pass latency-bound: 20 % of the HBM peak at 80 M splats)
@@ -65,10 +90,10 @@ __global__ void __launch_bounds__(256) k_keys(const float *__restrict__ depth, c
   for (uint32_t i = (blockIdx.x * blockDim.x + tid) * 4u; i < n4; i += gridDim.x * blockDim.x * 4u) {
     const float4 d = __ldg((const float4 *)(depth + i));
     uint4 k;
-    k.x = key_of(d.x); k.y = key_of(d.y); k.z = key_of(d.z); k.w = key_of(d.w);
+    k.x = key_of(i, d.x); k.y = key_of(i + 1, d.y); k.z = key_of(i + 2, d.z); k.w = key_of(i + 3, d.w);
     *(uint4 *)(key32 + i) = k;
   }
-  if (blockIdx.x == 0 && tid < n - n4) key32[n4 + tid] = key_of(__ldg(depth + n4 + tid));
+  if (blockIdx.x == 0 && tid < n - n4) key32[n4 + tid] = key_of(n4 + tid, __ldg(depth + n4 + tid));
   for (int o = 16; o > 0; o >>= 1) {
     in += __shfl_xor_sync(0xffffffffu, in, o);
     drop += __shfl_xor_sync(0xffffffffu, drop, o);
@@ -170,14 +195,15 @@ __global__ void __launch_bounds__(256) k_slab_init(const FrameParams *__restrict
   if (mine) atomicAdd(&ctr->open_bins, mine);
 }
 
-// entry count of slab `slab` (0 when nothing is open); the sort / emit kernels read it from sort.n_valid / n_inrange
-__global__ void k_slab_begin(const SlabTable *__restrict__ tab, FrameCounters *ctr, int slab) {
+// entry count of slab `slab` (0 when nothing is open); the sort / emit kernels read it from sort.n_valid / n_inrange.
+// q5_tail: plain frames give slab 0 the quirk-Q5 repeats of splat 0 (scene frames count their drops as real entries).
+__global__ void k_slab_begin(const SlabTable *__restrict__ tab, FrameCounters *ctr, int slab, bool q5_tail) {
   if (threadIdx.x || blockIdx.x) return;
   ctr->n_inst_total += ctr->n_inst;  // close the previous slab's accounts
   ctr->n_kept_total += ctr->n_inst_kept;
   if (ctr->n_inst > ctr->n_inst_slab_max) ctr->n_inst_slab_max = ctr->n_inst;
   const uint32_t real = tab->count[slab];
-  const uint32_t extra = slab == 0 ? ctr->sort.n_dropped : 0u;  // quirk Q5: repeats of splat 0, in front of everything
+  const uint32_t extra = slab == 0 && q5_tail ? ctr->sort.n_dropped : 0u;  // quirk Q5: repeats of splat 0, in front of everything
   const bool active = ctr->open_bins > 0 && (real + extra) > 0 && !ctr->overflow;
   const uint32_t m = active ? real + extra : 0u;
   ctr->slab_real = active ? real : 0u;
@@ -216,12 +242,15 @@ __device__ __forceinline__ void load_keys8(const uint32_t *__restrict__ key32, u
 }
 
 // Chunk counts of EVERY scheduled slab in one pass over the keys (stage A, after the plan): slab boundaries are bucket
-// aligned, so a 4096-entry table maps a key to its slab; a thread tallies its 8 keys in 4-bit fields of one 64-bit
-// word (12 slabs x 4 bits, at most 8 per field), the warp adds each field with redux.  cnt[s * row + c] = entries of
-// slab s in chunk c.  (A pass per slab read the 4 B keys of all N splats once more for every slab that ran.)
+// aligned, so a 4096-entry table maps a key's bucket (slab_bucket) to its slab; a thread tallies its 8 keys in 4-bit
+// fields of one 64-bit word (12 slabs x 4 bits, at most 8 per field), the warp adds each field with redux.
+// cnt[s * row + c] = entries of slab s in chunk c.  (A pass per slab read the 4 B keys of all N splats once more for
+// every slab that ran.)
+template <bool SCENE>
 __global__ void __launch_bounds__(kCompactThreads) k_compact_count_all(const uint32_t *__restrict__ key32,
                                                                        const FrameParams *__restrict__ fp,
-                                                                       const SlabTable *__restrict__ tab, int n_slabs,
+                                                                       const SlabTable *__restrict__ tab,
+                                                                       const SceneTable *__restrict__ scene, int n_slabs,
                                                                        uint32_t *__restrict__ cnt, uint32_t row) {
   __shared__ uint8_t s_slab[kSlabBuckets];
   __shared__ uint32_t s_klo[kMaxSlabs];
@@ -234,6 +263,7 @@ __global__ void __launch_bounds__(kCompactThreads) k_compact_count_all(const uin
     for (int s = 0; s < n_slabs; ++s) sid += (b * 16u < s_klo[s]) ? 1u : 0u;
     s_slab[b] = (uint8_t)min(sid, (uint32_t)(kMaxSlabs - 1));
   }
+  const uint32_t bits = SCENE ? scene->bucket_bits : 0u;
   const uint32_t n = fp->n_splats;
   const uint32_t nchunks = (n + kCompactChunk - 1) / kCompactChunk;
   for (uint32_t c = blockIdx.x; c < nchunks; c += gridDim.x) {
@@ -244,7 +274,7 @@ __global__ void __launch_bounds__(kCompactThreads) k_compact_count_all(const uin
     unsigned long long m = 0ull;
 #pragma unroll
     for (int j = 0; j < 8; ++j)
-      if (k[j] < 65536u) m += 1ull << (4u * s_slab[k[j] >> 4]);
+      if (k[j] != kNoKey) m += 1ull << (4u * s_slab[slab_bucket<SCENE>(k[j], bits)]);
     for (int s = 0; s < n_slabs; ++s) {
       const uint32_t v = __reduce_add_sync(0xffffffffu, (uint32_t)(m >> (4 * s)) & 15u);
       if (lane == 0 && v) atomicAdd(&s_c[s], v);
@@ -295,16 +325,26 @@ __global__ void __launch_bounds__(1024) k_compact_scan_all(uint32_t *__restrict_
   }
 }
 
+// the slab's entries (buckets in [klo, khi) / 16) in index order: splat index and key (plain frames: the 16-bit key;
+// SCENE: the 24-bit key, whose quirk-Q5 entries pass SM1 the dropped splat's index)
+template <bool SCENE>
 __global__ void __launch_bounds__(kCompactThreads) k_compact_write(const uint32_t *__restrict__ key32,
                                                                    const FrameParams *__restrict__ fp,
                                                                    const FrameCounters *__restrict__ ctr,
-                                                                   const SlabTable *__restrict__ tab, int slab,
+                                                                   const SlabTable *__restrict__ tab,
+                                                                   const SceneTable *__restrict__ scene, int slab,
                                                                    const uint32_t *__restrict__ cnt, uint32_t *__restrict__ cidx,
-                                                                   uint16_t *__restrict__ ckey) {
+                                                                   typename std::conditional<SCENE, uint32_t, uint16_t>::type *__restrict__ ckey) {
   const uint32_t real = ctr->slab_real;
   if (!real) return;
   __shared__ uint32_t s_w[kCompactThreads / 32];
+  const uint32_t bits = SCENE ? scene->bucket_bits : 0u;
   const uint32_t n = fp->n_splats, lo = tab->klo[slab], hi = tab->khi[slab];
+  auto in_slab = [&](uint32_t k) {  // plain keys compare directly (bounds are bucket * 16); kNoKey maps past every bucket
+    if (!SCENE) return k >= lo && k < hi;
+    const uint32_t bk = slab_bucket<SCENE>(k, bits);
+    return bk >= (lo >> 4) && bk < (hi >> 4);
+  };
   const uint32_t nchunks = (n + kCompactChunk - 1) / kCompactChunk;
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   for (uint32_t c = blockIdx.x; c < nchunks; c += gridDim.x) {
@@ -312,7 +352,7 @@ __global__ void __launch_bounds__(kCompactThreads) k_compact_write(const uint32_
     uint32_t k[8], m = 0;
     load_keys8(key32, base, n, k);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) m += (k[j] >= lo && k[j] < hi) ? 1u : 0u;
+    for (int j = 0; j < 8; ++j) m += in_slab(k[j]) ? 1u : 0u;
     uint32_t incl = m;
     for (int o = 1; o < 32; o <<= 1) {
       const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
@@ -325,15 +365,16 @@ __global__ void __launch_bounds__(kCompactThreads) k_compact_write(const uint32_
     uint32_t pos = __ldg(cnt + c) + wb + incl - m;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      if (k[j] >= lo && k[j] < hi) {
+      if (in_slab(k[j])) {
         cidx[pos] = base + j;
-        ckey[pos] = (uint16_t)k[j];
+        ckey[pos] = k[j];
         ++pos;
       }
     }
     __syncthreads();
   }
-  // quirk Q5: the dropped entries' slots hold 0 at the END of the reference's array -> splat 0 again, drawn last
+  // quirk Q5: the dropped entries' slots hold 0 at the END of the reference's array -> splat 0 again, drawn last (plain
+  // frames, slab 0 only: k_slab_begin gives no other slab more entries than it holds)
   const uint32_t total = ctr->sort.n_valid;
   for (uint32_t e = real + blockIdx.x * blockDim.x + tid; e < total; e += gridDim.x * blockDim.x) {
     cidx[e] = 0u;
@@ -347,9 +388,11 @@ static int grid_for(gs_context *c, uint64_t n, int per_cta, int per_sm) {
   return (int)(t < cap ? t : cap);
 }
 
-void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, cudaStream_t st) {
+void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const ObjCounters *octr,
+                 int set, cudaStream_t st) {
   cudaMemsetAsync(c->slab_tab[set], 0, sizeof(SlabTable), st);
-  k_keys<<<grid_for(c, c->cap, 256 * 8, 8), 256, 0, st>>>(c->depth, fp, ctr, c->key32[set], c->slab_tab[set]);
+  (scene ? k_keys<true> : k_keys<false>)<<<grid_for(c, c->cap, 256 * 8, 8), 256, 0, st>>>(c->depth, fp, ctr, c->key32[set],
+                                                                                        c->slab_tab[set], scene, octr);
 }
 
 void launch_slab_plan(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, uint32_t first_target, int n_slabs,
@@ -364,17 +407,25 @@ void launch_slab_init(gs_context *c, const FrameParams *fp, FrameCounters *ctr, 
 }
 
 // stage A, after the plan: chunk offsets of every scheduled slab (the loop's k_compact_write reads row `slab`)
-void launch_compact_offsets(gs_context *c, const FrameParams *fp, int set, int n_slabs, cudaStream_t st) {
+void launch_compact_offsets(gs_context *c, const FrameParams *fp, const SceneTable *scene, int set, int n_slabs, cudaStream_t st) {
   const int grid = grid_for(c, c->cap, kCompactChunk, 8);
-  k_compact_count_all<<<grid, kCompactThreads, 0, st>>>(c->key32[set], fp, c->slab_tab[set], n_slabs, c->chunk_cnt[set], c->chunk_row);
+  (scene ? k_compact_count_all<true> : k_compact_count_all<false>)<<<grid, kCompactThreads, 0, st>>>(
+      c->key32[set], fp, c->slab_tab[set], scene, n_slabs, c->chunk_cnt[set], c->chunk_row);
   k_compact_scan_all<<<n_slabs, 1024, 0, st>>>(c->chunk_cnt[set], fp, c->chunk_row);
 }
 
-void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, int slab, cudaStream_t st) {
-  k_slab_begin<<<1, 32, 0, st>>>(c->slab_tab[set], ctr, slab);
+// scene frames compact into scene_key (24-bit keys), which the one-pass scene sort alone uses otherwise
+void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, int set, int slab,
+                       cudaStream_t st) {
+  k_slab_begin<<<1, 32, 0, st>>>(c->slab_tab[set], ctr, slab, scene == nullptr);
   const int grid = grid_for(c, c->cap, kCompactChunk, 8);
-  k_compact_write<<<grid, kCompactThreads, 0, st>>>(c->key32[set], fp, ctr, c->slab_tab[set], slab,
-                                                    c->chunk_cnt[set] + (size_t)slab * c->chunk_row, c->cidx, c->ckey);
+  const uint32_t *cnt = c->chunk_cnt[set] + (size_t)slab * c->chunk_row;
+  if (scene)
+    k_compact_write<true><<<grid, kCompactThreads, 0, st>>>(c->key32[set], fp, ctr, c->slab_tab[set], scene, slab, cnt, c->cidx,
+                                                            c->scene_key);
+  else
+    k_compact_write<false><<<grid, kCompactThreads, 0, st>>>(c->key32[set], fp, ctr, c->slab_tab[set], scene, slab, cnt, c->cidx,
+                                                             c->ckey);
 }
 
 void launch_slab_end(gs_context *c, FrameCounters *ctr, cudaStream_t st) { k_slab_end<<<1, 32, 0, st>>>(ctr); }

@@ -6,7 +6,8 @@
 //                   counting sort as two 8-bit passes
 //   k_radix_{hist,scan,scatter}<T1>, <T2>: stable sort of bin instances by 16-bit bin id; the final pass (T1 when a
 //                   frame has at most 256 bins, else T2) also gathers the 32 B records
-//   k_radix_{hist,scan,scatter}<S1>: first pass of a depth slab's sort (keys from the slab's compacted entries)
+//   k_radix_{hist,scan,scatter}<S1>, <SM1>: first pass of a depth slab's sort (keys from the slab's compacted entries;
+//                   SM1: the 24-bit keys of a scene frame, followed by M2 and M3)
 //   k_tile_ranges : per-bin {start, end} in the final instance order (frames of more than 256 bins; otherwise pass T1 writes them)
 //
 // Scene frames (several entities, gs_render_scene): one worker per entity (index.js:229-236), each with its own view row,
@@ -208,19 +209,9 @@ __global__ void __launch_bounds__(256) k_scene_keys(const float *__restrict__ de
                                                     FrameCounters *ctr, uint32_t *__restrict__ key_out,
                                                     uint32_t *__restrict__ pay_out) {
   GS_PDL_ENTRY();
-  __shared__ uint32_t s_first[kMaxObjects], s_end[kMaxObjects], s_tag[kMaxObjects];
-  __shared__ double s_min[kMaxObjects], s_inv[kMaxObjects];
+  __shared__ SceneKeyTable s_ent;
   __shared__ uint32_t s_in, s_drop;
-  const uint32_t n_obj = scene->n;
-  for (uint32_t k = threadIdx.x; k < n_obj; k += blockDim.x) {
-    s_first[k] = scene->obj[k].first;
-    s_end[k] = scene->obj[k].end;
-    s_tag[k] = scene->obj[k].rank << 17;
-    // the entity's own range (index.js:552-558), as load_depth_range does for a single worker
-    const double mn = dec_f64(~octr[k].min_enc), mx = dec_f64(octr[k].max_enc);
-    s_min[k] = mn;
-    s_inv[k] = __ddiv_rn(65535.0, __dsub_rn(mx, mn));
-  }
+  s_ent.load(scene, octr);
   if (threadIdx.x == 0) { s_in = 0; s_drop = 0; }
   __syncthreads();
   const uint32_t n = ctr->sort.n_valid ? fp->n_splats : 0u;
@@ -229,16 +220,14 @@ __global__ void __launch_bounds__(256) k_scene_keys(const float *__restrict__ de
     const float d = __ldg(depth + i);
     uint32_t key = kNoKey;
     if (d != GS_DEPTH_REJECT) {
-      const int k = scene_find(s_first, s_end, n_obj, i);  // a sorted splat always lies in an entity's range
-      const int32_t q = depth_key(d, s_min[k], s_inv[k]);
-      if (q >= 0 && q <= 65535) {
-        key = s_tag[k] | (uint32_t)q;
+      int k;
+      key = s_ent.key(i, d, k);
+      if (key & 65536u) {  // quirk Q5: the entity's first splat
+        pay_out[i] = s_ent.first[k];
+        ++drop;
+      } else {
         pay_out[i] = i;
         ++in;
-      } else {  // quirk Q5: the entity's slot stays 0 -> its first splat, after all its in-range entries
-        key = s_tag[k] | 65536u;
-        pay_out[i] = s_first[k];
-        ++drop;
       }
     }
     key_out[i] = key;
@@ -563,32 +552,6 @@ void launch_depth_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr
 }
 
 // ---------------------------------------------------------------------------------------------
-// Slab path: stable sort of the compacted slab by its 16-bit key -> b.order = the slab's draw order (6 launches)
-// ---------------------------------------------------------------------------------------------
-// S1: low key byte of the current slab's compacted (key, index) pairs (gs_slab.cu)
-struct S1 : RadixPass {
-  using Carry = uint8_t;  // high key byte
-  const FrameCounters *ctr;
-  const uint16_t *key; const uint32_t *idx;
-  uint32_t *idx_out; uint8_t *hi_out;
-  __device__ uint32_t count() const { return ctr->sort.n_valid; }  // entries of the current slab (k_slab_begin)
-  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) const {
-    const uint32_t k = key[i];
-    carry = k >> 8;
-    pay = idx[i];
-    return k & 255u;
-  }
-  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const { idx_out[pos] = pay; hi_out[pos] = (uint8_t)carry; }
-};
-
-// S1, then D2 as in the depth sort
-void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st) {
-  const RadixScratch s{c->table_n, c->totals, c->table_n_stride};
-  run_pass(c, S1{{}, ctr, c->ckey, c->cidx, c->idx_a, c->dig_a}, s, c->cap, st);
-  run_pass(c, D2{{}, ctr, c->dig_a, c->idx_a, b.order}, s, c->cap, st);
-}
-
-// ---------------------------------------------------------------------------------------------
 // Scene frames: (draw rank, key, index) as three stable 8-bit passes over the 24-bit key of k_scene_keys -> b.order.
 // Every sorted entry takes part, Q5 drops included.  9 launches.
 // ---------------------------------------------------------------------------------------------
@@ -641,6 +604,65 @@ void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr
   run_pass(c, M1{{}, ctr, fp, c->scene_key, c->scene_pay, c->idx_a, c->scene_hi}, s, c->cap, st);
   run_pass(c, M2{{}, ctr, c->scene_hi, c->idx_a, c->scene_pay, c->dig_a}, s, c->cap, st);
   run_pass(c, M3{{}, ctr, c->dig_a, c->scene_pay, b.order}, s, c->cap, st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Slab path: stable sort of the compacted slab by its key -> b.order = the draw order restricted to the slab
+// ---------------------------------------------------------------------------------------------
+// S1: low key byte of the current slab's compacted (key, index) pairs (gs_slab.cu)
+struct S1 : RadixPass {
+  using Carry = uint8_t;  // high key byte
+  const FrameCounters *ctr;
+  const uint16_t *key; const uint32_t *idx;
+  uint32_t *idx_out; uint8_t *hi_out;
+  __device__ uint32_t count() const { return ctr->sort.n_valid; }  // entries of the current slab (k_slab_begin)
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) const {
+    const uint32_t k = key[i];
+    carry = k >> 8;
+    pay = idx[i];
+    return k & 255u;
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const { idx_out[pos] = pay; hi_out[pos] = (uint8_t)carry; }
+};
+
+// SM1: key bits 0-7 of the current slab's compacted (24-bit scene key, index) pairs of a scene frame; the payload of a
+// quirk-Q5 entry is its entity's first splat, found from the dropped splat's own index.  M2 and M3 follow.
+struct SM1 : RadixPass {
+  using Carry = uint16_t;  // key bits 8-23
+  const FrameCounters *ctr;
+  const SceneTable *scene;
+  const uint32_t *key, *idx;
+  uint32_t *idx_out; uint16_t *hi_out;
+  __device__ uint32_t count() const { return ctr->sort.n_valid; }  // entries of the current slab (k_slab_begin)
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) const {
+    const uint32_t k = key[i];
+    carry = k >> 8;
+    pay = idx[i];
+    if (k & 65536u) {  // rare: the last entity whose range starts at or before the splat holds it
+      uint32_t lo = 0, hi = scene->n;
+      while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (scene->obj[mid].first <= pay) lo = mid; else hi = mid;
+      }
+      pay = scene->obj[lo].first;
+    }
+    return k & 255u;
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const { idx_out[pos] = pay; hi_out[pos] = (uint16_t)carry; }
+};
+
+// plain frames: S1, then D2 as in the depth sort (6 launches); scene frames: SM1, M2, M3 as in the scene sort (9 launches)
+void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
+                      cudaStream_t st) {
+  const RadixScratch s{c->table_n, c->totals, c->table_n_stride};
+  if (scene) {
+    run_pass(c, SM1{{}, ctr, scene, c->scene_key, c->cidx, c->idx_a, c->scene_hi}, s, c->cap, st);
+    run_pass(c, M2{{}, ctr, c->scene_hi, c->idx_a, c->scene_pay, c->dig_a}, s, c->cap, st);
+    run_pass(c, M3{{}, ctr, c->dig_a, c->scene_pay, b.order}, s, c->cap, st);
+    return;
+  }
+  run_pass(c, S1{{}, ctr, c->ckey, c->cidx, c->idx_a, c->dig_a}, s, c->cap, st);
+  run_pass(c, D2{{}, ctr, c->dig_a, c->idx_a, b.order}, s, c->cap, st);
 }
 
 // ---------------------------------------------------------------------------------------------

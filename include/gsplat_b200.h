@@ -265,7 +265,10 @@ typedef struct gs_object {
  * A = 1 - T_end + dst.a*T_end, an RGBA8 destination read as byte/255 in fp32.  Host memory unless
  * GS_RENDER_COLOR_DEVICE; a host buffer is staged per frame and must stay valid until gs_wait.
  * One entity spanning the whole table is exactly gs_render_async (same kernels, one-pass or slab path) plus color_in.
- * Any other scene is rendered in one pass (no depth slabs) and leaves no single-entity order behind: a following
+ * Any other scene takes the slab path by the rule of plain frames: when it is expected to sort at least GS_SLAB_MIN
+ * entries (the previous frame's sorted count, or before any frame the splats in its entities' ranges) and is no
+ * GS_RENDER_STATS frame, it is rendered front to back in depth slabs of its (draw position, key, index) order, with the
+ * same frame as the one-pass path.  A scene frame leaves no single-entity order behind: a following
  * GS_RENDER_REUSE_SORT frame sorts again.
  */
 GS_API int gs_render_scene_async(gs_context *ctx, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,

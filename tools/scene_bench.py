@@ -8,8 +8,10 @@ cutout box. They are placed so that they overlap on screen and drawn at 1920x108
 (the opaque geometry of the demo pages: RGBA8 noise and two opaque rectangles at 1.8 and 2.6 m). Scene frames and plain
 gs_render frames of the same table and camera are timed in three alternated rounds of K steps each. Three frames are in
 flight, the L2 is flushed between steps, and one CUDA-event pair brackets each round. The per-stage times come from
-un-overlapped scene frames. The algorithmic bytes are bench.py's one-pass formula plus the third radix pass (8 B per
-sorted entry) and the RGBA8 colour read (4 B per pixel). Parity compares the float frame against the chain of
+un-overlapped scene frames. The algorithmic bytes are bench.py's formula plus the third radix pass (8 B per sorted entry,
+or per slab entry when the frame took the slab path) and the RGBA8 colour read (4 B per pixel). A scene that sorts at
+least GS_SLAB_MIN (16 M) entries, e.g. --splats 40000000, is rendered front to back in depth slabs; the line's `slabs`
+block then reports the slabs scheduled and run and the entries they held. Parity compares the float frame against the chain of
 per-entity oracle draws (tests/scene_oracle.py); the run exits non-zero above 1e-3. Prints one JSON line.
 """
 from __future__ import annotations
@@ -127,7 +129,7 @@ def main():
         lat.append(ctx.wait(sub_scene(i)).as_dict())
     st = {k: float(np.mean([x[k] for x in lat])) for k in lat[0]}
     for k in ("n_splats", "n_sorted", "n_visible", "n_instances", "n_instances_kept", "n_tiles", "width", "height",
-              "kernel_launches", "n_dropped", "n_slabs"):
+              "kernel_launches", "n_dropped", "n_slabs", "n_slabs_run", "n_slab_entries"):
         st[k] = int(lat[0][k])
     p_stats = ctx.make_params(fr, fmt=gs.GS_FORMAT_RGBA8, flags=gs.GS_RENDER_OUT_DEVICE | gs.GS_RENDER_STATS)
     p_stats.depth_in = depth.ctypes.data
@@ -136,9 +138,12 @@ def main():
         st[k] = int(full[k])
     ab = bench.algorithmic_bytes(st)
     V, P = st["n_sorted"], st["width"] * st["height"]
-    ab["sort"] += 8 * V      # the third radix pass (draw rank) over the sorted entries
+    # the third radix pass (draw rank): over the sorted entries, or on the slab path over the entries of the slabs that ran
+    # (part of the slab loop, reported as the bin stage)
+    third = 8 * (st["n_slab_entries"] if st["n_slabs"] else V)
+    ab["bin" if st["n_slabs"] else "sort"] += third
     ab["raster"] += 4 * P    # the RGBA8 colour target, read once
-    ab["total"] += 8 * V + 4 * P
+    ab["total"] += third + 4 * P
     ms_s, ms_p = float(np.median(rounds["scene"])), float(np.median(rounds["plain"]))
     gpu = torch.cuda.get_device_properties(dev).name
     line = {"metric": "frames/sec @1920x1080 (scene frame: two entities of N/2 splats over a colour + depth target)",
@@ -149,7 +154,8 @@ def main():
             "counters": {k: st[k] for k in ("n_splats", "n_sorted", "n_visible", "n_instances", "n_instances_kept", "n_dropped",
                                             "kernel_launches")},
             "stages": {k: {"ms": st["ms_" + k], "bytes": ab[k]} for k in ("sort", "project", "bin", "raster")},
-            "frame": {"bytes": ab["total"], "ms_device": st["ms_total"]}}
+            "frame": {"bytes": ab["total"], "ms_device": st["ms_total"]},
+            "slabs": {k: st[k] for k in ("n_slabs", "n_slabs_run", "n_slab_entries")}}
     rc = 0
     if not args.no_cpu_baseline:
         from oracle import oracle as orc
