@@ -60,6 +60,9 @@ SYMBOLS = {
     "gs_push_splats": (C.c_int, [_P, _P, C.c_uint32]),
     "gs_push_ply": (C.c_int, [_P, _P, C.c_size_t, _P, C.POINTER(C.c_uint32)]),
     "gs_reserve": (C.c_int, [_P, C.c_uint32]),
+    "gs_insert_splats": (C.c_int, [_P, C.c_uint32, _P, C.c_uint32]),
+    "gs_insert_ply": (C.c_int, [_P, C.c_uint32, _P, C.c_size_t, _P, C.POINTER(C.c_uint32)]),
+    "gs_erase": (C.c_int, [_P, C.c_uint32, C.c_uint32]),
     "gs_push_packed": (C.c_int, [_P, _P, _P, _P, C.c_uint32]),
     "gs_num_splats": (C.c_int, [_P, C.POINTER(C.c_uint32)]),
     "gs_read_packed": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P]),

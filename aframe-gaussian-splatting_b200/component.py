@@ -107,10 +107,13 @@ class GaussianSplattingComponent:
     def initGL(self, numVertexes: int) -> None:
         """The reference sizes its two data textures from numVertexes (index.js:26-46, known from the Content-Length,
         index.js:248-251); here the resident table is reserved for as many splats, so the pushes that follow never
-        have to grow it (and never wait for frames in flight).  sortReady flips exactly as at index.js:220."""
+        have to grow it (and never wait for frames in flight).  In a SplatScene the table holds every entity: it is
+        reserved for all of their announced sizes.  sortReady flips exactly as at index.js:220."""
         if numVertexes > 0 and self.renderer is not None:
-            base = self.renderer.num_splats if self.scene is not None else 0  # a scene appends behind the other entities
-            self.renderer.reserve(base + int(numVertexes))
+            if self.scene is not None:
+                self.scene._reserve(self, int(numVertexes))
+            else:
+                self.renderer.reserve(int(numVertexes))
         self.sortReady = True
 
     # ---- index.js:222-327 ----
@@ -277,74 +280,83 @@ class SplatScene:
     (index.js:184-195).  render() draws the entities whole, in the order they were added (A-Frame 1.4 draws transparent
     meshes in scene-graph order), over a caller-supplied colour and depth target: the opaque geometry already drawn.
 
-    Divergence: entities load one after another, each into its own contiguous range of the shared table; the reference
-    streams all of them at once, one worker each.  A component's clear() (loadData) drops only its own splats: the
-    other entities' rows are pushed again behind each other (the host keeps every entity's rows for that).
+    Every entity owns one contiguous range of the shared table, in the order the entities were added.  Entities stream
+    in together, as the reference's one worker per entity does: a push inserts the rows at the end of the entity's own
+    range on the device (gs_insert_splats / gs_insert_ply), and the ranges behind it move up, so interleaved chunks of
+    several entities build the table that loading them one after another builds.  A component's clear() (loadData)
+    erases only its own range on the device (gs_erase); the emptied entity goes to the end of the table, where its next
+    rows append.  No row is kept on the host.
     """
 
     def __init__(self, renderer: Optional[SplatContext] = None, device: int = 0):
         self.renderer = renderer or SplatContext(device)
         self.entities: list = []   # components, in draw order
-        self._rows: dict = {}      # id(component) -> list of row chunks as pushed
+        self._order: list = []     # components, in table order (an empty range's place is its position here)
         self._range: dict = {}     # id(component) -> [first, count]
+        self._announced: dict = {}  # id(component) -> numVertexes of its last initGL
 
     def add(self, component: GaussianSplattingComponent, camera, object3d) -> GaussianSplattingComponent:
         """Attach `component` (drawn after the entities added before it) and load it: component.init() with this scene's
         context."""
         component.scene = self
         self.entities.append(component)
-        self._rows[id(component)] = []
+        self._order.append(component)
         self._range[id(component)] = [self.renderer.num_splats, 0]
         component.init(camera, object3d, self.renderer)
         return component
+
+    def remove(self, component: GaussianSplattingComponent) -> None:
+        """The entity leaves the page: its range is erased on the device and it is no longer drawn."""
+        self._erase(component)
+        self.entities.remove(component)
+        self._order.remove(component)
+        del self._range[id(component)]
+        self._announced.pop(id(component), None)
+        component.scene = None
 
     def range_of(self, component: GaussianSplattingComponent):
         first, count = self._range[id(component)]
         return first, count
 
+    def _reserve(self, component, num_vertexes: int) -> None:
+        """initGL of an entity: the table is reserved for every entity's announced size (or its count when larger)."""
+        self._announced[id(component)] = int(num_vertexes)
+        self.renderer.reserve(sum(max(self._announced.get(id(e), 0), self._range[id(e)][1]) for e in self._order))
+
+    def _shift_after(self, component, delta: int) -> None:
+        for e in self._order[self._order.index(component) + 1:]:
+            self._range[id(e)][0] += delta
+
     def _push(self, component, rows: np.ndarray) -> None:
         rows = np.ascontiguousarray(rows, np.uint8).reshape(-1, 32)
+        if not rows.shape[0]:
+            return
         first, count = self._range[id(component)]
-        if first + count != self.renderer.num_splats:  # another entity was loaded since: this one moves to the end
-            self._clear_entity(component, keep_rows=True)
-            first, count = self._range[id(component)]
-        self.renderer.push_splats(rows)
-        self._rows[id(component)].append(rows.copy())
+        self.renderer.insert_splats(first + count, rows)
         self._range[id(component)][1] = count + rows.shape[0]
+        self._shift_after(component, rows.shape[0])
 
     def _push_ply(self, component, blob) -> int:
-        """A .ply entity: converted and pushed on the device; its rows come back (rows32_out) and are kept like pushed
-        rows, so that a later clear of another entity can push them again."""
+        """A .ply entity: converted on the device and inserted at the end of its range."""
         first, count = self._range[id(component)]
-        if first + count != self.renderer.num_splats:
-            self._clear_entity(component, keep_rows=True)
-            first, count = self._range[id(component)]
-        n, rows = self.renderer.push_ply(blob, return_rows=True)
-        if n:
-            self._rows[id(component)].append(rows)
+        n = self.renderer.insert_ply(first + count, blob)
         self._range[id(component)][1] = count + n
+        self._shift_after(component, n)
         return n
 
-    def _clear_entity(self, component, keep_rows: bool = False) -> None:
-        """Drop the entity's splats (keep_rows: move them to the end of the table instead) and repack the others."""
-        mine = self._rows[id(component)] if keep_rows else []
-        if not mine and not self._rows[id(component)]:  # nothing resident yet: the others stay where they are
-            self._range[id(component)] = [self.renderer.num_splats, 0]
-            return
-        self._rows[id(component)] = []
-        self.renderer.clear()
-        for e in self.entities:
-            if e is component:
-                continue
-            self._range[id(e)] = [self.renderer.num_splats, 0]
-            for r in self._rows[id(e)]:
-                self.renderer.push_splats(r)
-                self._range[id(e)][1] += r.shape[0]
+    def _erase(self, component) -> None:
+        first, count = self._range[id(component)]
+        if count:
+            self.renderer.erase(first, count)
+            self._range[id(component)][1] = 0
+            self._shift_after(component, -count)
+
+    def _clear_entity(self, component) -> None:
+        """Erase the entity's splats; it moves to the end of the table, where its next rows append."""
+        self._erase(component)
+        self._order.remove(component)
+        self._order.append(component)
         self._range[id(component)] = [self.renderer.num_splats, 0]
-        for r in mine:
-            self.renderer.push_splats(r)
-            self._rows[id(component)].append(r)
-            self._range[id(component)][1] += r.shape[0]
 
     def objects(self, width: int, height: int, camera=None):
         """(shared FrameInputs of the draw, [SceneObject per entity in draw order]) for a width x height viewport."""

@@ -430,14 +430,39 @@ extern "C" int gs_reserve(gs_context *c, uint32_t n_total) {
   return ensure_table(c, n_total, /*exact=*/true);
 }
 
-extern "C" int gs_push_splats(gs_context *c, const void *rows32, uint32_t n) {
-  if (!c || (!rows32 && n)) return GS_ERR_INVALID;
-  if (!n) return GS_OK;
+// A table edit that moves resident rows (an insert below the end, any erase) first waits for the frames in flight: they
+// read the table in stage A and in every slab's projection, and wait_slot re-runs a frame whose instance buffer
+// overflowed, reading it again.  Its temporary (if the ranges overlap) is allocated here, stream-ordered on push_stream,
+// before anything moves; *tmp is freed by end_move.
+static int begin_move(gs_context *c, uint32_t from, uint32_t to, uint32_t len, void **tmp) {
+  *tmp = nullptr;
+  int rc = drain(c);
+  if (rc) return rc;
+  const size_t bytes = move_tmp_bytes(from, to, len);
+  const cudaError_t e = bytes ? cudaMallocAsync(tmp, bytes, c->push_stream) : cudaSuccess;
+  if (e) cudaGetLastError();  // an allocation failure is not sticky: do not leave it for the next launch check
+  GS_CUDA(c, e);
+  return GS_OK;
+}
+
+static int end_move(gs_context *c, uint32_t from, uint32_t to, uint32_t len, void *tmp) {
+  launch_move_rows(c, from, to, len, tmp, c->push_stream);
+  cudaError_t e = cudaGetLastError();
+  if (tmp) cudaFreeAsync(tmp, c->push_stream);
+  GS_CUDA(c, e);
+  return GS_OK;
+}
+
+// gs_push_splats (at == c->n) and gs_insert_splats; the caller checked 0 < n and at <= c->n
+static int insert_rows(gs_context *c, uint32_t at, const void *rows32, uint32_t n) {
   GS_CUDA(c, cudaSetDevice(c->device));
   int rc;
   if ((rc = ensure_table(c, (uint64_t)c->n + n))) return rc;
   if ((rc = ensure_push_staging(c))) return rc;
-  // Frames in flight keep rendering: they read rows [0, n_at_submit) only, the pack below writes rows >= c->n, on
+  const uint32_t tail = c->n - at;
+  void *tmp = nullptr;
+  if (tail && ((rc = begin_move(c, at, at + n, tail, &tmp)) || (rc = end_move(c, at, at + n, tail, tmp)))) return rc;
+  // An append does not wait: frames in flight read rows [0, n_at_submit) only, the pack below writes rows >= c->n, on
   // its own stream.  Chunks alternate between two pinned staging buffers, so the host copy of chunk k+1 overlaps the
   // DMA + pack of chunk k.  The caller's buffer is fully consumed when this returns.
   const uint8_t *src = (const uint8_t *)rows32;
@@ -448,12 +473,41 @@ extern "C" int gs_push_splats(gs_context *c, const void *rows32, uint32_t n) {
     GS_CUDA(c, cudaEventSynchronize(c->push_ev[b]));  // this staging pair's previous chunk has been packed
     memcpy(c->push_pinned[b], src + (size_t)off * 32, (size_t)m * 32);
     GS_CUDA(c, cudaMemcpyAsync(c->push_dev[b], c->push_pinned[b], (size_t)m * 32, cudaMemcpyHostToDevice, c->push_stream));
-    launch_pack(c, c->push_dev[b], c->n + off, m, c->push_stream);
+    launch_pack(c, c->push_dev[b], at + off, m, c->push_stream);
     GS_CUDA(c, cudaGetLastError());
     GS_CUDA(c, cudaEventRecord(c->push_ev[b], c->push_stream));
   }
   GS_CUDA(c, cudaEventRecord(c->push_done, c->push_stream));
   c->n += n;
+  c->pushed = true;
+  c->have_order = false;
+  return GS_OK;
+}
+
+extern "C" int gs_push_splats(gs_context *c, const void *rows32, uint32_t n) {
+  if (!c || (!rows32 && n)) return GS_ERR_INVALID;
+  if (!n) return GS_OK;
+  return insert_rows(c, c->n, rows32, n);
+}
+
+extern "C" int gs_insert_splats(gs_context *c, uint32_t at, const void *rows32, uint32_t n) {
+  if (!c) return GS_ERR_INVALID;
+  if (!rows32 || !n) return fail(c, GS_ERR_INVALID, "gs_insert_splats: no rows");
+  if (at > c->n) return fail(c, GS_ERR_INVALID, "gs_insert_splats: position past the resident splats");
+  return insert_rows(c, at, rows32, n);
+}
+
+extern "C" int gs_erase(gs_context *c, uint32_t first, uint32_t count) {
+  if (!c) return GS_ERR_INVALID;
+  if (!count || (uint64_t)first + count > c->n) return fail(c, GS_ERR_INVALID, "gs_erase: empty range or past the resident splats");
+  GS_CUDA(c, cudaSetDevice(c->device));
+  const uint32_t tail = c->n - first - count;
+  void *tmp = nullptr;
+  int rc;
+  // an erase at the end moves nothing, but still drains: the next push would overwrite rows a frame in flight reads
+  if ((rc = begin_move(c, first + count, first, tail, &tmp)) || (rc = end_move(c, first + count, first, tail, tmp))) return rc;
+  GS_CUDA(c, cudaEventRecord(c->push_done, c->push_stream));
+  c->n -= count;
   c->pushed = true;
   c->have_order = false;
   return GS_OK;
@@ -468,10 +522,10 @@ static int ensure_ply_staging(gs_context *c) {
   return GS_OK;
 }
 
-// processPlyBuffer + one pushDataBuffer on the device (gs_ply.cu).  Same contract as gs_push_splats: frames in flight keep
-// drawing the old prefix, the caller's file is consumed on return, only a push that outgrows the table waits.
-extern "C" int gs_push_ply(gs_context *c, const void *ply, size_t bytes, void *rows32_out_or_null, uint32_t *out_n) {
-  if (!c || (!ply && bytes)) return GS_ERR_INVALID;
+// processPlyBuffer + one pushDataBuffer on the device (gs_ply.cu), its rows packed into [at, at + n): gs_push_ply
+// (at == c->n) and gs_insert_ply.  Same contract as gs_push_splats: an append does not wait for frames in flight, the
+// caller's file is consumed on return, only a push that outgrows the table waits.
+static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes, void *rows32_out_or_null, uint32_t *out_n) {
   if (out_n) *out_n = 0;
   PlyLayout L;
   uint32_t n = 0;
@@ -482,6 +536,9 @@ extern "C" int gs_push_ply(gs_context *c, const void *ply, size_t bytes, void *r
   int rc;
   if ((rc = ensure_table(c, (uint64_t)c->n + n))) return rc;  // the header gave the count: one growth, up front
   if ((rc = ensure_ply_staging(c))) return rc;
+  const uint32_t tail = c->n - at;
+  void *move_tmp = nullptr;
+  if (tail && (rc = begin_move(c, at, at + n, tail, &move_tmp))) return rc;
   cudaStream_t st = c->push_stream;
   // temporaries, stream-ordered: decoded rows (32 B) + key per row, two permutations, radix tables, ordered rows
   const uint32_t chunks = (n + kRadixTile - 1) / kRadixTile;
@@ -489,7 +546,7 @@ extern "C" int gs_push_ply(gs_context *c, const void *ply, size_t bytes, void *r
   uint8_t *rows_dev = nullptr, *out_dev = nullptr, *body[2] = {nullptr, nullptr};
   uint32_t *key = nullptr, *perm_a = nullptr, *perm_b = nullptr, *table = nullptr, *totals = nullptr;
   auto release = [&]() {
-    void *ps[] = {rows_dev, out_dev, body[0], body[1], key, perm_a, perm_b, table, totals};
+    void *ps[] = {rows_dev, out_dev, body[0], body[1], key, perm_a, perm_b, table, totals, move_tmp};
     for (void *p : ps)
       if (p) cudaFreeAsync(p, st);
   };
@@ -526,7 +583,8 @@ extern "C" int gs_push_ply(gs_context *c, const void *ply, size_t bytes, void *r
     e = cudaGetLastError();
   }
   if (!e) {
-    launch_pack_perm(c, rows_dev, perm, c->n, n, out_dev, st);
+    launch_move_rows(c, at, at + n, tail, move_tmp, st);  // opens the gap for the rows (nothing to move for an append)
+    launch_pack_perm(c, rows_dev, perm, at, n, out_dev, st);
     e = cudaGetLastError();
   }
   if (!e && rows32_out_or_null) e = cudaMemcpyAsync(rows32_out_or_null, out_dev, (size_t)n * 32, cudaMemcpyDeviceToHost, st);
@@ -539,6 +597,19 @@ extern "C" int gs_push_ply(gs_context *c, const void *ply, size_t bytes, void *r
   c->have_order = false;
   if (out_n) *out_n = n;
   return GS_OK;
+}
+
+extern "C" int gs_push_ply(gs_context *c, const void *ply, size_t bytes, void *rows32_out_or_null, uint32_t *out_n) {
+  if (!c || (!ply && bytes)) return GS_ERR_INVALID;
+  return insert_ply(c, c->n, ply, bytes, rows32_out_or_null, out_n);
+}
+
+extern "C" int gs_insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes, void *rows32_out_or_null,
+                             uint32_t *out_n) {
+  if (!c || (!ply && bytes)) return GS_ERR_INVALID;
+  if (out_n) *out_n = 0;
+  if (at > c->n) return fail(c, GS_ERR_INVALID, "gs_insert_ply: position past the resident splats");
+  return insert_ply(c, at, ply, bytes, rows32_out_or_null, out_n);
 }
 
 extern "C" int gs_push_packed(gs_context *c, const float *center_scale4, const uint32_t *cov_color4,

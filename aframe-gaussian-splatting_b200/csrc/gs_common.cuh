@@ -402,6 +402,10 @@ void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_
 // PLY push: k_pack reading row perm[j] (perm NULL: row j) into slot first + j; rows_out (or NULL) receives the ordered rows
 void launch_pack_perm(gs_context *c, const uint8_t *rows_dev, const uint32_t *perm, uint32_t first, uint32_t n,
                       uint8_t *rows_out, cudaStream_t st);
+// table edits: bytes of the temporary a move of rows [from, from+len) to [to, to+len) needs (0: the ranges are disjoint)
+size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len);
+// k_move_rows: one launch for disjoint ranges, else two through tmp
+void launch_move_rows(gs_context *c, uint32_t from, uint32_t to, uint32_t len, void *tmp, cudaStream_t st);
 // PLY push: decode `rows` whole rows of a staged body chunk into .splat rows + importance keys at [first_row, ...)
 void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,
                        uint32_t *key, cudaStream_t st);

@@ -2,6 +2,7 @@
 //   k_pack      : row i of a staged chunk -> table slot first + i (gs_push_splats)
 //   k_pack_perm : row perm[j] of the decoded PLY rows -> slot first + j, optionally also written out in that order
 //                 (gs_push_ply: the gather of processPlyBuffer's importance order fused with the pack)
+//   k_move_rows : rows [from, from+len) of the table -> [to, to+len) (gs_insert_* / gs_erase open or close a gap)
 //
 // One thread per .splat row, all arithmetic in fp64 exactly as JavaScript evaluates it (Three.js r147
 // Matrix4.compose / transpose / scale / premultiply restated entry by entry, sums left to right, no FMA):
@@ -138,6 +139,69 @@ __global__ void __launch_bounds__(256) k_pack_perm(const uint4 *__restrict__ row
     rows_out[2 * (size_t)j + 1] = b;
   }
   pack_row(a, b, (size_t)first + j, cs, cc, sa, tab, nt);
+}
+
+// Table edit (gs_insert_*, gs_erase): copy n rows of the three table arrays from src to dst, one row per thread.  The two
+// ranges never overlap within one launch (an overlapping move goes through a temporary, launch_move_rows), so the
+// accesses are restrict.  The 16 B records are copied as they are; size_alpha goes as float4 when source and
+// destination share their alignment mod 16 B (sa_vec), with up to 3 scalar rows before the first aligned float4
+// (sa_head) and up to 3 after the last.
+struct RowSpan {
+  float4 *cs;
+  uint4 *cc;
+  float *sa;
+};
+
+__global__ void __launch_bounds__(256) k_move_rows(const RowSpan src, const RowSpan dst, uint32_t n, uint32_t sa_head,
+                                                   uint32_t sa_vec) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 *__restrict__ cs_s = src.cs;
+  const uint4 *__restrict__ cc_s = src.cc;
+  const float *__restrict__ sa_s = src.sa;
+  __stcs(dst.cs + i, __ldcs(cs_s + i));
+  __stcs(dst.cc + i, __ldcs(cc_s + i));
+  if (!sa_vec) {
+    __stcs(dst.sa + i, __ldcs(sa_s + i));
+    return;
+  }
+  const uint32_t nv = (n - sa_head) >> 2;  // aligned float4s; rows [sa_head + 4 nv, n) are the scalar tail
+  if (i < nv) {
+    __stcs((float4 *)(dst.sa + sa_head) + i, __ldcs((const float4 *)(sa_s + sa_head) + i));
+  } else {
+    const uint32_t k = i - nv;
+    const uint32_t j = k < sa_head ? k : 4 * nv + k;  // head rows, then the tail rows 4 nv + k for k >= sa_head
+    if (j < n) __stcs(dst.sa + j, __ldcs(sa_s + j));
+  }
+}
+
+static RowSpan table_span(gs_context *c, uint32_t row) {
+  return RowSpan{c->center_scale + row, c->cov_color + row, c->size_alpha + row};
+}
+
+static void launch_copy_rows(const RowSpan &src, const RowSpan &dst, uint32_t n, cudaStream_t st) {
+  const uintptr_t s = (uintptr_t)src.sa, d = (uintptr_t)dst.sa;
+  const uint32_t vec = ((s ^ d) & 15u) == 0, head = vec ? std::min<uint32_t>(n, (uint32_t)((16u - (d & 15u)) & 15u) / 4u) : 0;
+  k_move_rows<<<(n + 255) / 256, 256, 0, st>>>(src, dst, n, head, vec);
+}
+
+size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len) {
+  const uint32_t shift = from > to ? from - to : to - from;
+  return shift >= len ? 0 : (size_t)len * 36 + 16;  // cs | cc | 3 floats of alignment slack + sa
+}
+
+// Rows [from, from + len) of the table move to [to, to + len).  Disjoint ranges: one launch.  Overlapping ones: two,
+// through `tmp` (move_tmp_bytes(from, to, len) bytes, 16 B aligned), whose size_alpha starts at the source's alignment
+// so that the first copy is always vectorised.
+void launch_move_rows(gs_context *c, uint32_t from, uint32_t to, uint32_t len, void *tmp, cudaStream_t st) {
+  if (!len || from == to) return;
+  if (!move_tmp_bytes(from, to, len)) {
+    launch_copy_rows(table_span(c, from), table_span(c, to), len, st);
+    return;
+  }
+  const RowSpan t{(float4 *)tmp, (uint4 *)tmp + len, (float *)((uint4 *)tmp + 2 * (size_t)len) + (from & 3u)};
+  launch_copy_rows(table_span(c, from), t, len, st);
+  launch_copy_rows(t, table_span(c, to), len, st);
 }
 
 void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_t n, cudaStream_t st) {

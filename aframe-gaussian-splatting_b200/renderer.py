@@ -95,10 +95,19 @@ class SplatContext:
         rows = np.ascontiguousarray(rows, dtype=np.uint8).reshape(-1, 32)
         self._check(self._lib.gs_push_splats(self._h, _ptr(rows), rows.shape[0]))
 
+    def insert_splats(self, at: int, rows: np.ndarray) -> None:
+        """gs_insert_splats: rows ((n, 32) uint8 .splat rows) packed into [at, at+n); the splats from `at` on move up by n."""
+        rows = np.ascontiguousarray(rows, dtype=np.uint8).reshape(-1, 32)
+        self._check(self._lib.gs_insert_splats(self._h, int(at), _ptr(rows), rows.shape[0]))
+
     def push_ply(self, blob, return_rows: bool = False):
         """gs_push_ply: processPlyBuffer + pushDataBuffer (index.js:315-324, 600-745) of a whole binary .ply file on the
         device.  Returns the vertex count n, or (n, rows) with rows the (n, 32) uint8 .splat rows processPlyBuffer
         returns.  A malformed file raises GsError (GS_ERR_INVALID) with the reference's message."""
+        return self.insert_ply(None, blob, return_rows)
+
+    def insert_ply(self, at: Optional[int], blob, return_rows: bool = False):
+        """gs_insert_ply: push_ply with the file's rows packed into [at, at+n) (at None: gs_push_ply, at the end)."""
         buf = np.frombuffer(memoryview(blob), dtype=np.uint8)
         rows = None
         if return_rows:
@@ -107,10 +116,18 @@ class SplatContext:
             m = re.search(rb"element vertex (\d+)\n", buf[:10240].tobytes())
             rows = np.empty((min(int(m.group(1)), buf.size) if m else 0, 32), np.uint8)
         n = C.c_uint32()
-        self._check(self._lib.gs_push_ply(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, _ptr(rows), C.byref(n)))
+        src = buf.ctypes.data_as(C.c_void_p)
+        if at is None:
+            self._check(self._lib.gs_push_ply(self._h, src, buf.size, _ptr(rows), C.byref(n)))
+        else:
+            self._check(self._lib.gs_insert_ply(self._h, int(at), src, buf.size, _ptr(rows), C.byref(n)))
         if return_rows:
             return n.value, rows[:n.value]
         return n.value
+
+    def erase(self, first: int, count: int) -> None:
+        """gs_erase: remove splats [first, first+count); the splats behind them move down by count."""
+        self._check(self._lib.gs_erase(self._h, int(first), int(count)))
 
     def push_packed(self, center_scale: np.ndarray, cov_color: np.ndarray, size_alpha: np.ndarray) -> None:
         cs = np.ascontiguousarray(center_scale, dtype=np.float32).reshape(-1, 4)

@@ -13,7 +13,8 @@ class Splats : public Napi::ObjectWrap<Splats> {
       InstanceMethod("clear", &Splats::Clear), InstanceMethod("push", &Splats::Push),
       InstanceMethod("pushPly", &Splats::PushPly), InstanceMethod("reserve", &Splats::Reserve),
       InstanceMethod("sort", &Splats::Sort),   InstanceMethod("render", &Splats::Render),
-      InstanceMethod("renderScene", &Splats::RenderScene)}));
+      InstanceMethod("renderScene", &Splats::RenderScene), InstanceMethod("insert", &Splats::Insert),
+      InstanceMethod("insertPly", &Splats::InsertPly), InstanceMethod("erase", &Splats::Erase)}));
     return exports;
   }
   explicit Splats(const Napi::CallbackInfo& i) : Napi::ObjectWrap<Splats>(i) {
@@ -42,6 +43,26 @@ class Splats : public Napi::ObjectWrap<Splats> {
     Check(i.Env(), gs_push_ply(ctx_, buf.Data(), buf.ByteLength(), nullptr, &n));
     return Napi::Number::New(i.Env(), n);
   }
+  // insert(at, ArrayBuffer rows, vertexCount)     <- one entity's pushDataBuffer into the shared table, at the end of its
+  //                                                   own range: entities stream in together (index.js:259-298)
+  Napi::Value Insert(const Napi::CallbackInfo& i) {
+    auto buf = i[1].As<Napi::ArrayBuffer>();
+    Check(i.Env(), gs_insert_splats(ctx_, i[0].As<Napi::Number>().Uint32Value(), buf.Data(),
+                                    i[2].As<Napi::Number>().Uint32Value()));
+    return i.Env().Undefined();
+  }
+  // insertPly(at, ArrayBuffer plyFile) -> vertexCount   <- pushPly into one entity's range
+  Napi::Value InsertPly(const Napi::CallbackInfo& i) {
+    auto buf = i[1].As<Napi::ArrayBuffer>();
+    uint32_t n = 0;
+    Check(i.Env(), gs_insert_ply(ctx_, i[0].As<Napi::Number>().Uint32Value(), buf.Data(), buf.ByteLength(), nullptr, &n));
+    return Napi::Number::New(i.Env(), n);
+  }
+  // erase(first, count)                            <- one entity's worker "clear" (index.js:236,573-575) in a shared table
+  Napi::Value Erase(const Napi::CallbackInfo& i) {
+    Check(i.Env(), gs_erase(ctx_, i[0].As<Napi::Number>().Uint32Value(), i[1].As<Napi::Number>().Uint32Value()));
+    return i.Env().Undefined();
+  }
   // sort(Float32Array view, Float32Array|undefined cutout) -> Uint32Array   <- worker "sort", index.js:587-596
   Napi::Value Sort(const Napi::CallbackInfo& i) {
     auto view = i[0].As<Napi::Float32Array>();
@@ -69,8 +90,8 @@ class Splats : public Napi::ObjectWrap<Splats> {
   // renderScene({proj, width, height, focal, depth?: Float32Array}, [{first, count, modelview, cutout?}, ...], Uint8Array color,
   //             Uint8Array out)  <- the draws of every gaussian_splatting entity of the page, in DOM order (sortObjects false),
   // over the opaque pass: color = gl.readPixels(RGBA, UNSIGNED_BYTE) and depth = the window-space depth buffer read back
-  // after the spheres and sky were drawn; each entity's {first, count} is its range of the shared table (pushed one
-  // entity after another), modelview its getModelViewMatrix(camera), cutout its worldToCutout.
+  // after the spheres and sky were drawn; each entity's {first, count} is its range of the shared table (filled by
+  // insert / insertPly at the end of that range), modelview its getModelViewMatrix(camera), cutout its worldToCutout.
   Napi::Value RenderScene(const Napi::CallbackInfo& i) {
     auto o = i[0].As<Napi::Object>();
     gs_render_params p{};

@@ -151,6 +151,39 @@ GS_API int gs_push_ply(gs_context *ctx, const void *ply, size_t bytes, void *row
 GS_API int gs_reserve(gs_context *ctx, uint32_t n_total);
 
 /*
+ * Table edits: the entities of a page share one table, each in its own contiguous range, and stream in together (every
+ * entity's own fetch loop pushes at the end of its own range, index.js:259-298) or unload alone (the worker clear of one
+ * entity, index.js:236,573-586, which with a shared table would otherwise be a gs_clear plus a re-push of every other
+ * entity's rows).  The rows behind the edit move on the device (k_move_rows, one streaming pass); nothing is copied
+ * through the host.
+ *
+ * gs_insert_splats: insert n rows at position `at` (0 <= at <= gs_num_splats).  Splats [at, N) move to [at+n, N+n) on
+ *   the device; the new rows are packed into [at, at+n).  gs_push_splats(ctx, rows, n) == gs_insert_splats(ctx, N, rows, n).
+ * gs_insert_ply: gs_push_ply at position `at`: same header rules, messages, rows32_out and "malformed input leaves the
+ *   table unchanged" (the file is parsed and validated before anything moves).  A file with no vertex inserts nothing.
+ * gs_erase: remove splats [first, first+count): [first+count, N) moves down to [first, N-count) on the device.  Erasing
+ *   every splat leaves N = 0, and the next sort or render returns GS_ERR_EMPTY, as after gs_clear.
+ *
+ * Rules:
+ *   - at > N, first + count > N, n == 0 and count == 0 return GS_ERR_INVALID and change nothing.  A failed temporary
+ *     allocation returns GS_ERR_OOM with the table unchanged (it is allocated before the first kernel).
+ *   - An insert at N is an append and keeps the push contract above: it waits for frames in flight only when the table
+ *     grows.  An insert below N, and EVERY gs_erase, first waits for the frames in flight, because
+ *       . frames read the table in their depth sort and projection (k_depth_cull*, k_project), and on the slab path in
+ *         every slab's projection;
+ *       . gs_wait re-runs a frame whose tile-instance buffer overflowed, and that re-run reads the table again;
+ *       . an erase at the end moves nothing, but the next push would overwrite rows that a frame in flight may read.
+ *     Frames submitted after the edit see the new table.
+ *   - Overlapping source and destination ranges go through a stream-ordered temporary of 36 B per moved splat, freed
+ *     after the edit.
+ *   - After any edit the draw order is stale: a GS_RENDER_REUSE_SORT frame sorts again, as after a push.
+ */
+GS_API int gs_insert_splats(gs_context *ctx, uint32_t at, const void *rows32, uint32_t n);
+GS_API int gs_insert_ply(gs_context *ctx, uint32_t at, const void *ply, size_t bytes, void *rows32_out_or_null,
+                         uint32_t *out_n);
+GS_API int gs_erase(gs_context *ctx, uint32_t first, uint32_t count);
+
+/*
  * Append n already-packed splats: the two data-texture records the reference uploads
  * (centerAndScaleData float4, covAndColorData uint4, index.js:40-46,378-394) and the worker's
  * matrices[15] (max(scale)*alpha/255, index.js:397).  Host pointers.
