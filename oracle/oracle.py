@@ -51,6 +51,7 @@ def lib():
         L.orc_render_rows.restype = C.c_int
         L.orc_render_ex.restype = C.c_int
         L.orc_coverage_check.restype = C.c_int
+        L.orc_pairs.restype = C.c_int64
         L.orc_set_affinity.restype = None
         L.orc_ply_to_splat.restype = C.c_int64
         L.orc_ply_to_splat.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p]
@@ -180,6 +181,30 @@ def render(center_scale, cov_color, order, proj, mv, width, height, focal, bg=(0
                              C.c_uint32(r0), C.c_uint32(r1), _p(d))
     assert rc == 0
     return out, {"n_order": st.n_order, "n_visible": st.n_visible, "fragments": st.fragments}
+
+
+def pairs(center_scale, cov_color, order, proj, mv, width, height, focal, rows=None, depth_in=None) -> dict:
+    """Every (pixel, splat) pair render() blends (orc_pairs in gs_oracle.c), in draw order, then row-major:
+    {"pix": y * width + x (row 0 = bottom), "pos": draw position j, "r2": fp32 r^2, "tiles": distinct (draw position,
+    16x16 tile) pairs with at least one blended pixel}.  rows / depth_in as in render()."""
+    cs = np.ascontiguousarray(center_scale, np.float32).reshape(-1, 4)
+    cc = np.ascontiguousarray(cov_color, np.uint32).reshape(-1, 4)
+    o = np.ascontiguousarray(order, np.uint32)
+    d = None if depth_in is None else np.ascontiguousarray(depth_in, np.float32).reshape(height, width)
+    r0, r1 = (0, height) if rows is None else rows
+    P, M = np.ascontiguousarray(proj, np.float32), np.ascontiguousarray(mv, np.float32)
+    tiles = C.c_uint64()
+
+    def run(cap, pix, pos, r2):
+        return lib().orc_pairs(_p(cs), _p(cc), _p(o), C.c_uint32(o.shape[0]), _p(P), _p(M), C.c_uint32(width), C.c_uint32(height),
+                               C.c_float(focal), C.c_uint32(r0), C.c_uint32(r1), _p(d), C.c_uint64(cap), _p(pix), _p(pos), _p(r2),
+                               C.byref(tiles))
+
+    n = run(0, None, None, None)
+    assert n >= 0
+    pix, pos, r2 = np.zeros(max(n, 1), np.uint32), np.zeros(max(n, 1), np.uint32), np.zeros(max(n, 1), np.float32)
+    assert run(n, pix, pos, r2) == n
+    return {"pix": pix[:n], "pos": pos[:n], "r2": r2[:n], "tiles": int(tiles.value)}
 
 
 def coverage_check(center_scale, cov_color, order, proj, mv, width, height, focal, nthreads=None) -> dict:
