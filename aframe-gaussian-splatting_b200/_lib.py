@@ -76,6 +76,10 @@ SYMBOLS = {
                                         C.POINTER(C.c_uint64)]),
     "gs_render_scene": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.c_uint32, _P, _P, C.POINTER(GsStats)]),
     "gs_sort_scene": (C.c_int, [_P, C.POINTER(GsObject), C.c_uint32, _P, C.POINTER(C.c_uint32)]),
+    "gs_render_scene_stereo_async": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.POINTER(C.c_float),
+                                               C.c_uint32, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_uint64)]),
+    "gs_render_scene_stereo": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.POINTER(C.c_float), C.c_uint32,
+                                         C.POINTER(_P), C.POINTER(_P), C.POINTER(GsStats)]),
     "gs_read_projected": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
     "gs_get_stats": (C.c_int, [_P, C.POINTER(GsStats)]),
     "gs_set_shard": (C.c_int, [_P, C.c_uint32, C.c_uint32]),

@@ -373,3 +373,29 @@ class SplatScene:
             raise ValueError("SplatScene.render: no entity added")
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out)
+
+    def render_xr(self, eye_cameras, width: int, height: int, color_in=(None, None), depth_in=(None, None),
+                  bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8):
+        """WebXR presentation of every entity (index.js:13-15, 184-195, 438-455): one stereo frame
+        (gs_render_scene_stereo).  Each entity's sort comes from its getModelViewMatrix() of the scene camera - the head
+        pose its tick() uses - and each entity is drawn once per eye camera with that eye's matrices.
+        Eye viewport: the XR layer's native eye size (width x height) scaled by xrPixelRatio and floored, as
+        GaussianSplattingComponent.render_xr does.  The ratio is the FIRST entity's xrPixelRatio (1 when it is not
+        positive), by the rule of render(), whose shared viewport is the first entity's.
+        color_in[e] / depth_in[e]: eye e's colour ((h, w, 4) of the output dtype) and window-space depth ((h, w) f32) at
+        the scaled size, or None.  Returns [left, right] frames, row 0 = bottom."""
+        if not self.entities:
+            raise ValueError("SplatScene.render_xr: no entity added")
+        assert len(eye_cameras) == 2
+        ratio = float(self.entities[0].data.get("xrPixelRatio") or 0)
+        if ratio <= 0:
+            ratio = 1.0
+        w, h = int(math.floor(width * ratio)), int(math.floor(height * ratio))
+        objs = []
+        for e in self.entities:
+            head = e._frame_inputs_px(w, h)
+            objs.append(SceneObject(*self.range_of(e), head.modelview, head.cutout))
+        eye_frames = [[e._frame_inputs_px(w, h, cam) for e in self.entities] for cam in eye_cameras]
+        eyes = [frames[0] for frames in eye_frames]
+        eye_mvs = [[f.modelview for f in frames] for frames in eye_frames]
+        return self.renderer.render_scene_stereo(eyes, objs, eye_mvs, color_in=color_in, depth_in=depth_in, bg=bg, fmt=fmt)

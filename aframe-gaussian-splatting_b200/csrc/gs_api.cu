@@ -125,6 +125,26 @@ static int ensure_slot_scene(gs_context *c, gs_context::Slot &sl) {
   return GS_OK;
 }
 
+// the second eye's records and rectangles of stereo scene frames, sized like the per-splat scratch; allocated by the first
+// stereo frame (the pipeline is idle)
+static int ensure_stereo_bufs(gs_context *c) {
+  if (c->stereo_cap >= c->cap && c->proj_rec1[0]) return GS_OK;
+  for (int i = 0; i < 2; ++i) {
+    dev_free(c->proj_rec1[i]); dev_free(c->rect1[i]);
+    GS_CUDA(c, dev_alloc(&c->proj_rec1[i], 2 * (size_t)c->cap));
+    GS_CUDA(c, dev_alloc(&c->rect1[i], (size_t)c->cap));
+  }
+  c->stereo_cap = c->cap;
+  return GS_OK;
+}
+
+// a slot's stereo table (device + pinned staging): fixed size, allocated once
+static int ensure_slot_stereo(gs_context *c, gs_context::Slot &sl) {
+  if (!sl.stereo_dev) GS_CUDA(c, cudaMalloc((void **)&sl.stereo_dev, sizeof(StereoParams)));
+  if (!sl.stereo_host) GS_CUDA(c, cudaHostAlloc((void **)&sl.stereo_host, sizeof(StereoParams), cudaHostAllocDefault));
+  return GS_OK;
+}
+
 static int ensure_instances(gs_context *c, uint64_t need) {
   if (need <= c->cap_inst && c->inst_rec[0]) return GS_OK;
   if (need >= (1ull << 30)) return fail(c, GS_ERR_CAPACITY, "more than 2^30 tile instances in one frame");
@@ -144,8 +164,14 @@ static int ensure_instances(gs_context *c, uint64_t need) {
   return GS_OK;
 }
 
+static void drop_graphs(gs_context *c);
+static void drop_stereo_graphs(gs_context *c);
+
 static int ensure_bins(gs_context *c, uint32_t n_bins) {
   if (n_bins <= c->bins_cap && c->bin_range[0]) return GS_OK;
+  // the captured stages bake bin_range; a stereo frame grows it to both eyes' bins while a mono frame's key stays put
+  drop_graphs(c);
+  drop_stereo_graphs(c);
   dev_free(c->bin_range[0]); dev_free(c->bin_range[1]);
   GS_CUDA(c, dev_alloc(&c->bin_range[0], (size_t)n_bins + 1));
   GS_CUDA(c, dev_alloc(&c->bin_range[1], (size_t)n_bins + 1));
@@ -189,17 +215,22 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles, uint32_t n_bins) {
   return GS_OK;
 }
 
-static int ensure_frame(gs_context *c, gs_context::Slot &sl, size_t bytes) {
-  if (bytes <= sl.frame_bytes && sl.frame_dev) return GS_OK;
-  if (sl.frame_dev) cudaFree(sl.frame_dev);
-  sl.frame_dev = nullptr;
-  GS_CUDA(c, cudaMalloc(&sl.frame_dev, bytes));
-  sl.frame_bytes = bytes;
+// device buffer of `bytes` in *dev (capacity *cap), grown when too small
+static int ensure_dev(gs_context *c, void *&dev, size_t &cap, size_t bytes) {
+  if (bytes <= cap && dev) return GS_OK;
+  if (dev) cudaFree(dev);
+  dev = nullptr;
+  GS_CUDA(c, cudaMalloc(&dev, bytes));
+  cap = bytes;
   return GS_OK;
 }
 
+static void kill_graph(cudaGraphExec_t &g) {
+  if (g) { cudaGraphExecDestroy(g); g = nullptr; }
+}
+
 static void drop_graphs(gs_context *c) {
-  auto kill = [](cudaGraphExec_t &g) { if (g) { cudaGraphExecDestroy(g); g = nullptr; } };
+  auto kill = kill_graph;
   for (auto &sl : c->slot)
     for (int i = 0; i < 2; ++i) {
       kill(sl.graph_a[i][0]); kill(sl.graph_a[i][1]); kill(sl.graph_as[i]); kill(sl.graph_b[i]); kill(sl.graph_r[i]); kill(sl.graph_rp[i]);
@@ -208,6 +239,11 @@ static void drop_graphs(gs_context *c) {
         for (auto &g : sl.graph_sl[i][q]) kill(g);
       }
     }
+}
+
+static void drop_stereo_graphs(gs_context *c) {
+  for (auto &sl : c->slot)
+    for (int i = 0; i < 2; ++i) { kill_graph(sl.graph_xa[i]); kill_graph(sl.graph_xb[i]); kill_graph(sl.graph_xr[i]); }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -329,6 +365,7 @@ extern "C" int gs_destroy(gs_context *c) {
   dev_free(c->center_scale); dev_free(c->cov_color); dev_free(c->size_alpha);
   dev_free(c->depth); dev_free(c->idx_a); dev_free(c->dig_a);
   for (int i = 0; i < 2; ++i) { dev_free(c->order[i]); dev_free(c->proj_rec[i]); dev_free(c->rect[i]); }
+  for (int i = 0; i < 2; ++i) { dev_free(c->proj_rec1[i]); dev_free(c->rect1[i]); }
   dev_free(c->inst_tile); dev_free(c->inst_idx); dev_free(c->inst_tile_b); dev_free(c->inst_tile_f); dev_free(c->inst_idx_b);
   dev_free(c->inst_rec[0]); dev_free(c->inst_rec[1]);
   dev_free(c->bin_range[0]); dev_free(c->bin_range[1]); dev_free(c->quirk_table); dev_free(c->tile_stats);
@@ -347,6 +384,7 @@ extern "C" int gs_destroy(gs_context *c) {
   }
   if (c->push_stream) cudaStreamDestroy(c->push_stream);
   drop_graphs(c);
+  drop_stereo_graphs(c);
   for (uint32_t r = 0; r < c->peer_world; ++r)
     if (r != c->peer_rank && c->peer_base[r]) cudaIpcCloseMemHandle(c->peer_base[r]);
   if (c->peer_local) cudaFree(c->peer_local);
@@ -359,11 +397,14 @@ extern "C" int gs_destroy(gs_context *c) {
   delete c->scene_tmp;
   for (auto &sl : c->slot) {
     dev_free(sl.ctr); dev_free(sl.fp);
-    if (sl.frame_dev) cudaFree(sl.frame_dev);
-    if (sl.depth_dev) cudaFree(sl.depth_dev);
-    if (sl.color_dev) cudaFree(sl.color_dev);
-    dev_free(sl.scene_dev); dev_free(sl.octr);
+    for (int e = 0; e < 2; ++e) {
+      if (sl.frame_dev[e]) cudaFree(sl.frame_dev[e]);
+      if (sl.depth_dev[e]) cudaFree(sl.depth_dev[e]);
+      if (sl.color_dev[e]) cudaFree(sl.color_dev[e]);
+    }
+    dev_free(sl.scene_dev); dev_free(sl.octr); dev_free(sl.stereo_dev);
     if (sl.scene_host) cudaFreeHost(sl.scene_host);
+    if (sl.stereo_host) cudaFreeHost(sl.stereo_host);
     if (sl.ctr_host) cudaFreeHost(sl.ctr_host);
     if (sl.fp_host) cudaFreeHost(sl.fp_host);
     for (auto &ev : sl.ev) if (ev) cudaEventDestroy(ev);
@@ -767,8 +808,16 @@ extern "C" uint32_t gs_owned_tiles(uint32_t width, uint32_t height, uint32_t ran
 }
 
 static FrameBufs slot_bufs(gs_context *c, const gs_context::Slot &sl) {
-  return FrameBufs{c->order[sl.set], c->proj_rec[sl.set], c->rect[sl.set], c->inst_rec[sl.set], c->bin_range[sl.set]};
+  FrameBufs b{c->order[sl.set], c->proj_rec[sl.set], c->rect[sl.set], c->inst_rec[sl.set], c->bin_range[sl.set]};
+  if (sl.stereo) {
+    b.proj_rec1 = c->proj_rec1[sl.set];
+    b.rect1 = c->rect1[sl.set];
+  }
+  return b;
 }
+
+// per-frame parameters the kernels read: a stereo frame's pair (eye 1 at +1, for the raster), else the slot's own
+static const FrameParams *slot_fp(const gs_context::Slot &sl) { return sl.stereo ? &sl.stereo_dev->eye[0] : sl.fp; }
 
 // Stage A of a frame (sort stream): per-frame inputs to the device, depth sort, vertex shader.  All per-frame
 // inputs come from sl.fp (device memory), so each stage is captured once into a CUDA graph and replayed.
@@ -804,7 +853,8 @@ static cudaError_t enqueue_sort_stage(gs_context *c, gs_context::Slot &sl, bool 
 }
 
 // Stage A of a scene frame: per-entity depth pass, keys and the (rank, key, index) sort; per-entity projection beside it.
-// The scene table was copied to sl.scene_dev ahead of the stage (submit).
+// The scene table was copied to sl.scene_dev ahead of the stage (submit), and for a stereo frame the stereo table to
+// sl.stereo_dev: the sort is the head camera's, the projection covers both eyes.
 static cudaError_t enqueue_scene_sort_stage(gs_context *c, gs_context::Slot &sl, bool external_events) {
   auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
     return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
@@ -820,7 +870,8 @@ static cudaError_t enqueue_scene_sort_stage(gs_context *c, gs_context::Slot &sl,
   if ((e = cudaEventRecord(c->ev_fork[0], m))) return e;
   if ((e = cudaStreamWaitEvent(x, c->ev_fork[0], 0))) return e;
   if ((e = rec(sl.evp[0], x))) return e;
-  launch_project_scene(c, sl.fp, sl.scene_dev, sl.ctr, b, x);
+  if (sl.stereo) launch_project_stereo(c, sl.stereo_dev, sl.scene_dev, sl.ctr, b, x);
+  else launch_project_scene(c, sl.fp, sl.scene_dev, sl.ctr, b, x);
   if ((e = rec(sl.evp[1], x))) return e;
   if ((e = cudaEventRecord(c->ev_join[0], x))) return e;
   launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, m);
@@ -840,7 +891,7 @@ static cudaError_t enqueue_bin_stage(gs_context *c, gs_context::Slot &sl, uint32
   cudaError_t e;
   if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, m))) return e;
   if ((e = rec(sl.ev[2], m))) return e;
-  launch_emit(c, sl.fp, sl.ctr, b, nullptr, m);
+  launch_emit(c, slot_fp(sl), sl.ctr, b, nullptr, m);
   launch_tile_radix(c, sl.ctr, b, n_bins, m);    // pass T1; above 256 bins also pass T2 + k_tile_ranges
   if ((e = rec(sl.ev[3], m))) return e;
   return cudaGetLastError();
@@ -854,7 +905,8 @@ static cudaError_t enqueue_raster_stage(gs_context *c, gs_context::Slot &sl, uin
   cudaError_t e;
   if (sl.peer) launch_peer_acquire(c, sl.fp, sl.ctr, c->rstream);
   if ((e = rec(sl.ev_r0, c->rstream))) return e;
-  launch_raster(c, sl.fp, n_tiles, slot_bufs(c, sl), sl.raster_flags, c->rstream);
+  if (sl.stereo) launch_raster_stereo(c, slot_fp(sl), n_tiles, slot_bufs(c, sl), sl.raster_flags, c->rstream);
+  else launch_raster(c, sl.fp, n_tiles, slot_bufs(c, sl), sl.raster_flags, c->rstream);
   if ((e = rec(sl.ev[4], c->rstream))) return e;
   if (sl.peer) launch_peer_signal_wait(c, sl.fp, sl.ctr, c->rstream);
   return cudaGetLastError();
@@ -895,28 +947,33 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
   gs_context::GraphKey k;
   k.cap = c->cap; k.n_tiles = n_tiles; k.n_bins = n_bins; k.cap_inst = c->cap_inst; k.p0 = c->depth; k.p1 = c->inst_rec[0]; k.p2 = c->center_scale;
   k.p3 = c->scene_key;
-  if (memcmp(&k, &c->gkey, sizeof(k)) != 0) {
-    drop_graphs(c);
-    c->gkey = k;
+  // stereo frames keep their own graphs and key (n_bins: both eyes' bins), so neither kind re-captures the other's
+  gs_context::GraphKey &key = sl.stereo ? c->gkey_stereo : c->gkey;
+  if (memcmp(&k, &key, sizeof(k)) != 0) {
+    if (sl.stereo) drop_stereo_graphs(c);
+    else drop_graphs(c);
+    key = k;
   }
   const int set = sl.set;
   // A: order/proj_rec/rect[set] must no longer be read by the binning stage that used them last
   if (c->sort_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->sort_set_free[set], 0));
-  int rc = sl.scene ? run_graph(c, sl.graph_as[set], c->stream, [&](bool ext) { return enqueue_scene_sort_stage(c, sl, ext); })
+  cudaGraphExec_t &ga = sl.stereo ? sl.graph_xa[set] : sl.graph_as[set];
+  int rc = sl.scene ? run_graph(c, ga, c->stream, [&](bool ext) { return enqueue_scene_sort_stage(c, sl, ext); })
                     : run_graph(c, sl.graph_a[set][reuse ? 1 : 0], c->stream, [&](bool ext) { return enqueue_sort_stage(c, sl, reuse, ext); });
   if (rc) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_sorted, c->stream));
   // B: needs A of this frame; inst_rec/bin_range[set] must no longer be read by the raster that used them last
   GS_CUDA(c, cudaStreamWaitEvent(c->bstream, sl.ev_sorted, 0));
   if (c->bin_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->bstream, c->bin_set_free[set], 0));
-  if ((rc = run_graph(c, sl.graph_b[set], c->bstream, [&](bool ext) { return enqueue_bin_stage(c, sl, n_bins, ext); }))) return rc;
+  if ((rc = run_graph(c, sl.stereo ? sl.graph_xb[set] : sl.graph_b[set], c->bstream,
+                      [&](bool ext) { return enqueue_bin_stage(c, sl, n_bins, ext); }))) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_binned, c->bstream));
   c->sort_set_free[set] = sl.ev_binned;
   // C
   GS_CUDA(c, cudaStreamWaitEvent(c->rstream, sl.ev_binned, 0));
   if (sl.raster_flags == c->raster_base_flags) {
-    if ((rc = run_graph(c, sl.peer ? sl.graph_rp[set] : sl.graph_r[set], c->rstream,
-                        [&](bool ext) { return enqueue_raster_stage(c, sl, n_tiles, ext); }))) return rc;
+    cudaGraphExec_t &gr = sl.stereo ? sl.graph_xr[set] : (sl.peer ? sl.graph_rp[set] : sl.graph_r[set]);
+    if ((rc = run_graph(c, gr, c->rstream, [&](bool ext) { return enqueue_raster_stage(c, sl, n_tiles, ext); }))) return rc;
   } else {
     // depth-tested / statistics frames use other instantiations of the raster: plain launches, no cached graph
     GS_CUDA(c, enqueue_raster_stage(c, sl, n_tiles, false));
@@ -1039,7 +1096,8 @@ static int enqueue_readback(gs_context *c, gs_context::Slot &sl) {
   GS_CUDA(c, cudaStreamWaitEvent(c->copy_stream, sl.ev_done, 0));
   GS_CUDA(c, cudaMemcpyAsync(sl.ctr_host, sl.ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, c->copy_stream));
   if (sl.host_out)
-    GS_CUDA(c, cudaMemcpyAsync(sl.out_user, sl.frame_src, sl.out_bytes, cudaMemcpyDeviceToHost, c->copy_stream));
+    for (int e = 0; e < (sl.stereo ? 2 : 1); ++e)
+      GS_CUDA(c, cudaMemcpyAsync(sl.out_user[e], sl.frame_src[e], sl.out_bytes[e], cudaMemcpyDeviceToHost, c->copy_stream));
   if (sl.raster_flags & 4u)
     GS_CUDA(c, cudaMemcpyAsync(c->tile_stats_host, c->tile_stats, sizeof(uint4) * (size_t)sl.fp_host->rc.n_tiles,
                                cudaMemcpyDeviceToHost, c->copy_stream));
@@ -1047,13 +1105,8 @@ static int enqueue_readback(gs_context *c, gs_context::Slot &sl) {
   return GS_OK;
 }
 
-static int submit(gs_context *c, gs_context::Slot &sl) {
-  const gs_render_params *p = &sl.params;
-  FrameParams &fp = *sl.fp_host;
-  RenderConsts &rc = fp.rc;
-  memset(&fp, 0, sizeof(fp));
-  fp.n_splats = sl.n_splats;  // what was resident when the frame was submitted; later pushes append behind it
-  if (c->pushed) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->push_done, 0));
+// a frame's RenderConsts from its parameters
+static void fill_render_consts(gs_context *c, const gs_render_params *p, RenderConsts &rc) {
   memcpy(rc.proj, p->proj, sizeof(rc.proj));
   memcpy(rc.mv, p->modelview, sizeof(rc.mv));
   rc.width = p->width;
@@ -1073,6 +1126,58 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   rc.shard_world = c->shard_world;
   rc.out_format = p->out_format;
   rc.out_tiled = (p->flags & GS_RENDER_OUT_TILED) ? 1u : 0u;
+}
+
+// Output of eye e of the slot's frame (a plain or scene frame has eye 0 only): the caller's device buffer, or a per-slot
+// device frame that the readback copies to the caller's host buffer
+static int stage_out(gs_context *c, gs_context::Slot &sl, int e, FrameParams &fp) {
+  if (!sl.host_out) {
+    fp.out = sl.out_user[e];
+    sl.frame_src[e] = nullptr;
+    return GS_OK;
+  }
+  int rcode = ensure_dev(c, sl.frame_dev[e], sl.frame_bytes[e], sl.out_bytes[e]);
+  if (rcode) return rcode;
+  fp.out = sl.frame_dev[e];
+  sl.frame_src[e] = sl.frame_dev[e];
+  return GS_OK;
+}
+
+// Depth and colour targets of eye e: the caller's device buffers as they are, host buffers staged per slot and eye (copied
+// on the sort stream, which the raster stage is ordered after)
+static int stage_inputs(gs_context *c, gs_context::Slot &sl, int e, const gs_render_params *p, FrameParams &fp) {
+  int rcode;
+  const size_t px_bytes = p->out_format == GS_FORMAT_RGBA8 ? 4 : 16;
+  const size_t pixels = (size_t)p->width * p->height;
+  if (p->depth_in) {
+    if (p->flags & GS_RENDER_DEPTH_DEVICE) {
+      fp.depth_in = p->depth_in;
+    } else {  // host depth buffer
+      if ((rcode = ensure_dev(c, sl.depth_dev[e], sl.depth_bytes[e], sizeof(float) * pixels))) return rcode;
+      GS_CUDA(c, cudaMemcpyAsync(sl.depth_dev[e], p->depth_in, sizeof(float) * pixels, cudaMemcpyHostToDevice, c->stream));
+      fp.depth_in = sl.depth_dev[e];
+    }
+  }
+  if (sl.color_in[e]) {
+    if (sl.color_device) {
+      fp.color_in = sl.color_in[e];
+    } else {  // host colour target: staged like a host depth_in
+      if ((rcode = ensure_dev(c, sl.color_dev[e], sl.color_bytes[e], px_bytes * pixels))) return rcode;
+      GS_CUDA(c, cudaMemcpyAsync(sl.color_dev[e], sl.color_in[e], px_bytes * pixels, cudaMemcpyHostToDevice, c->stream));
+      fp.color_in = sl.color_dev[e];
+    }
+  }
+  return GS_OK;
+}
+
+static int submit(gs_context *c, gs_context::Slot &sl) {
+  const gs_render_params *p = &sl.params;
+  FrameParams &fp = *sl.fp_host;
+  RenderConsts &rc = fp.rc;
+  memset(&fp, 0, sizeof(fp));
+  fp.n_splats = sl.n_splats;  // what was resident when the frame was submitted; later pushes append behind it
+  if (c->pushed) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->push_done, 0));
+  fill_render_consts(c, p, rc);
   const float view[4] = {p->modelview[2], p->modelview[6], p->modelview[10], p->modelview[14]};  // index.js:442
   fill_sort_consts(fp.sc, view, p->has_cutout ? p->cutout16 : nullptr);
 
@@ -1080,14 +1185,14 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   const size_t px_bytes = p->out_format == GS_FORMAT_RGBA8 ? 4 : 16;
   size_t out_pixels = (size_t)p->width * p->height;
   if (rc.out_tiled) out_pixels = (size_t)gs_owned_tiles(p->width, p->height, c->shard_rank, c->shard_world) * 256;
-  sl.out_bytes = out_pixels * px_bytes;
+  sl.out_bytes[0] = out_pixels * px_bytes;
   sl.host_out = !(p->flags & GS_RENDER_OUT_DEVICE);
   sl.peer = (p->flags & GS_RENDER_OUT_PEER) != 0;
   if (sl.peer) {
     if (!c->peer_world || c->peer_world != c->shard_world || c->peer_rank != c->shard_rank)
       return fail(c, GS_ERR_INVALID, "GS_RENDER_OUT_PEER needs gs_peer_import with the rank/world of gs_set_shard");
     if (rc.out_tiled) return fail(c, GS_ERR_INVALID, "GS_RENDER_OUT_PEER writes row-major frames: do not combine with GS_RENDER_OUT_TILED");
-    if (sl.out_bytes > c->peer_frame_bytes) return fail(c, GS_ERR_INVALID, "frame larger than the exported peer frame size");
+    if (sl.out_bytes[0] > c->peer_frame_bytes) return fail(c, GS_ERR_INVALID, "frame larger than the exported peer frame size");
     // ring slot and sequence number come from the count of PEER frames, which every rank submits in the same order
     // (tickets also count each rank's private frames, e.g. warm-up)
     sl.ring = (int)(c->peer_count % 3);
@@ -1104,47 +1209,26 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
     fp.peer_seq = sl.peer_seq;
     fp.peer_need = c->peer_count >= 3 ? c->peer_count - 2 : 0;  // sequence number of this ring slot's previous frame
     fp.out = peer_frame(c->peer_local, c->peer_frame_bytes, sl.ring);
-    sl.frame_src = fp.out;
+    sl.frame_src[0] = fp.out;
     c->peer_count += 1;
-  } else if (sl.host_out) {
-    if ((rcode = ensure_frame(c, sl, sl.out_bytes))) return rcode;
-    fp.out = sl.frame_dev;
-    sl.frame_src = sl.frame_dev;
-  } else {
-    fp.out = sl.out_user;
-    sl.frame_src = nullptr;
+  } else if ((rcode = stage_out(c, sl, 0, fp))) {
+    return rcode;
   }
+  if ((rcode = stage_inputs(c, sl, 0, p, fp))) return rcode;
   // raster instantiation: pixel loop (two pixels per lane by default), depth test, statistics
   sl.raster_flags = c->raster_base_flags | (p->depth_in ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u);
-  if (p->depth_in) {
-    if (p->flags & GS_RENDER_DEPTH_DEVICE) {
-      fp.depth_in = p->depth_in;
-    } else {  // host depth buffer: staged per slot, copied on the sort stream (the raster stage is ordered after it)
-      const size_t bytes = sizeof(float) * (size_t)p->width * p->height;
-      if (bytes > sl.depth_bytes || !sl.depth_dev) {
-        if (sl.depth_dev) cudaFree(sl.depth_dev);
-        sl.depth_dev = nullptr;
-        GS_CUDA(c, cudaMalloc(&sl.depth_dev, bytes));
-        sl.depth_bytes = bytes;
-      }
-      GS_CUDA(c, cudaMemcpyAsync(sl.depth_dev, p->depth_in, bytes, cudaMemcpyHostToDevice, c->stream));
-      fp.depth_in = sl.depth_dev;
-    }
-  }
-  if (sl.color_in) {
-    if (sl.color_device) {
-      fp.color_in = sl.color_in;
-    } else {  // host colour target: staged per slot like a host depth_in
-      const size_t bytes = px_bytes * (size_t)p->width * p->height;
-      if (bytes > sl.color_bytes || !sl.color_dev) {
-        if (sl.color_dev) cudaFree(sl.color_dev);
-        sl.color_dev = nullptr;
-        GS_CUDA(c, cudaMalloc(&sl.color_dev, bytes));
-        sl.color_bytes = bytes;
-      }
-      GS_CUDA(c, cudaMemcpyAsync(sl.color_dev, sl.color_in, bytes, cudaMemcpyHostToDevice, c->stream));
-      fp.color_in = sl.color_dev;
-    }
+  if (sl.stereo) {
+    // the pair of eye frames the stereo kernels read: eye 0 as above, eye 1 from its own parameters (same size and flags)
+    StereoParams &st = *sl.stereo_host;
+    st.eye[0] = fp;
+    FrameParams &f1 = st.eye[1];
+    memset(&f1, 0, sizeof(f1));
+    f1.n_splats = sl.n_splats;
+    fill_render_consts(c, &sl.eye1, f1.rc);
+    sl.out_bytes[1] = (size_t)sl.eye1.width * sl.eye1.height * (sl.eye1.out_format == GS_FORMAT_RGBA8 ? 4 : 16);
+    if ((rcode = stage_out(c, sl, 1, f1)) || (rcode = stage_inputs(c, sl, 1, &sl.eye1, f1))) return rcode;
+    if (sl.eye1.depth_in) sl.raster_flags |= 2u;
+    GS_CUDA(c, cudaMemcpyAsync(sl.stereo_dev, sl.stereo_host, sl.stereo_bytes, cudaMemcpyHostToDevice, c->stream));
   }
   // the scene table goes ahead of the sort stage on its stream (only the entities in use are copied)
   if (sl.scene) GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, sl.scene_bytes, cudaMemcpyHostToDevice, c->stream));
@@ -1155,7 +1239,8 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   if (sl.slab) {
     if ((rcode = launch_frame_slabs(c, sl, rc.n_tiles, rc.n_bins))) return rcode;
   } else {
-    if ((rcode = launch_frame(c, sl, reuse, rc.n_tiles, rc.n_bins))) return rcode;
+    // a stereo frame bins both eyes (ids eye * n_bins + bin) and rasters both eyes' tiles in one grid
+    if ((rcode = launch_frame(c, sl, reuse, rc.n_tiles, sl.stereo ? 2 * rc.n_bins : rc.n_bins))) return rcode;
   }
   if ((rcode = enqueue_readback(c, sl))) return rcode;
   c->last_set = sl.set;
@@ -1213,7 +1298,7 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   memset(&c->stats, 0, sizeof(c->stats));
   stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
   c->stats.kernel_launches = sl.launches;
-  c->stats.n_tiles = sl.fp_host->rc.n_tiles;
+  c->stats.n_tiles = sl.fp_host->rc.n_tiles * (sl.stereo ? 2u : 1u);
   if (sl.raster_flags & 4u) {  // GS_RENDER_STATS: per-tile {records streamed, records kept, pair tests, pair hits}
     const RenderConsts &rc = sl.fp_host->rc;
     for (uint32_t t = 0; t < rc.n_tiles; ++t) {
@@ -1258,15 +1343,25 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   return GS_OK;
 }
 
-// gs_render_async and scene frames.  scene: the table built by build_scene_table (nullptr = a plain frame);
-// color_in: the colour target or nullptr.
+// the second eye of a stereo scene frame
+struct StereoInput {
+  const gs_render_params *eye1;
+  const void *color_in1;
+  void *out1;
+  const float (*mv)[2][16];  // per entity of the scene table, in its order: the modelview of each eye
+};
+
+// gs_render_async, scene and stereo scene frames.  scene: the table built by build_scene_table (nullptr = a plain frame);
+// color_in: the colour target or nullptr; stereo: the second eye of a stereo scene frame (nullptr otherwise; p is eye 0).
 static int render_async(gs_context *c, const gs_render_params *p, const SceneTable *scene, size_t scene_bytes,
-                        const void *color_in, void *out_rgba, uint64_t *out_ticket) {
+                        const void *color_in, void *out_rgba, uint64_t *out_ticket, const StereoInput *stereo = nullptr) {
   if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
   if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
   const uint32_t n_tiles = ((p->width + kTile - 1) / kTile) * ((p->height + kTile - 1) / kTile);
   const uint32_t n_bins = ((p->width + kBin - 1) / kBin) * ((p->height + kBin - 1) / kBin);  // <= 64*64: fits the 16-bit bin id
+  // a stereo frame's bin table holds both eyes' bins (2 * 43 * 43 at most, still a 16-bit id)
+  const uint32_t n_bins_all = stereo ? 2 * n_bins : n_bins;
   GS_CUDA(c, cudaSetDevice(c->device));
   const uint64_t ticket = c->next_ticket;
   gs_context::Slot &sl = c->slot[ticket % gs_context::kSlots];
@@ -1288,7 +1383,8 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     for (uint32_t k = 0; k < scene->n; ++k) sortable += scene->obj[k].end - scene->obj[k].first;
   }
   const uint32_t expect_sorted = c->have_last_sorted ? c->last_sorted : sortable;
-  const bool slab = expect_sorted >= c->slab_min && !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS));
+  // (a stereo frame always takes the one-pass path)
+  const bool slab = !stereo && expect_sorted >= c->slab_min && !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS));
   if ((int)slab != c->last_mode) {
     if ((rcode = drain(c))) return rcode;
     GS_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1297,18 +1393,19 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     c->last_mode = (int)slab;
   }
   // growing any shared buffer needs an idle pipeline
-  const bool grow = (slab && (c->slab_cap < c->cap || !c->key32[0] || c->slab_tiles_cap < n_tiles || !c->slab_tab[1])) || !(c->scratch_cap >= c->cap && c->depth) || !(n_bins <= c->bins_cap && c->bin_range[0]) || !(n_tiles <= c->tile_stats_cap && c->tile_stats) || c->cap_inst == 0 ||
-                    (scene && !(c->scene_cap >= c->cap && c->scene_key));
+  const bool grow = (slab && (c->slab_cap < c->cap || !c->key32[0] || c->slab_tiles_cap < n_tiles || !c->slab_tab[1])) || !(c->scratch_cap >= c->cap && c->depth) || !(n_bins_all <= c->bins_cap && c->bin_range[0]) || !(n_tiles <= c->tile_stats_cap && c->tile_stats) || c->cap_inst == 0 ||
+                    (scene && !(c->scene_cap >= c->cap && c->scene_key)) || (stereo && !(c->stereo_cap >= c->cap && c->proj_rec1[0]));
   if (grow) {
     if ((rcode = drain(c))) return rcode;
     GS_CUDA(c, cudaStreamSynchronize(c->stream));
     GS_CUDA(c, cudaStreamSynchronize(c->bstream));
     GS_CUDA(c, cudaStreamSynchronize(c->rstream));
     if ((rcode = ensure_scratch(c))) return rcode;
-    if ((rcode = ensure_bins(c, n_bins))) return rcode;
+    if ((rcode = ensure_bins(c, n_bins_all))) return rcode;
     if ((rcode = ensure_tile_stats(c, n_tiles))) return rcode;
     if (slab && (rcode = ensure_slab(c, n_tiles, n_bins))) return rcode;
     if (scene && (rcode = ensure_scene_bufs(c))) return rcode;
+    if (stereo && (rcode = ensure_stereo_bufs(c))) return rcode;
     if (c->cap_inst == 0) {
       // first frame: room for two bin instances per resident splat (a typical scene needs ~1); GS_INST_CAP overrides
       // the initial size (tests of the overflow / regrow path)
@@ -1318,18 +1415,27 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     }
   }
   sl.params = *p;
-  sl.out_user = out_rgba;
+  sl.out_user[0] = out_rgba;
   sl.ticket = ticket;
   sl.n_splats = c->n;
   sl.n_sortable = sortable;
   sl.slab = slab;
-  sl.color_in = color_in;
+  sl.color_in[0] = color_in;
   sl.color_device = (p->flags & GS_RENDER_COLOR_DEVICE) != 0;
   sl.scene = scene != nullptr;
   if (scene) {
     if ((rcode = ensure_slot_scene(c, sl))) return rcode;
     memcpy(sl.scene_host, scene, scene_bytes);
     sl.scene_bytes = scene_bytes;
+  }
+  sl.stereo = stereo != nullptr;
+  if (stereo) {
+    if ((rcode = ensure_slot_stereo(c, sl))) return rcode;
+    sl.eye1 = *stereo->eye1;
+    sl.out_user[1] = stereo->out1;
+    sl.color_in[1] = stereo->color_in1;
+    memcpy(sl.stereo_host->mv, stereo->mv, sizeof(float) * 32 * scene->n);
+    sl.stereo_bytes = offsetof(StereoParams, mv) + sizeof(float) * 32 * scene->n;
   }
   if ((rcode = submit(c, sl))) return rcode;
   c->next_ticket = ticket + 1;
@@ -1456,6 +1562,43 @@ extern "C" int gs_render_stereo(gs_context *c, const float view[4], const float 
     }
   }
   return GS_OK;
+}
+
+// XR over a multi-entity page: the one scene sort of the frame from the head camera (every entity's tick(), index.js:438-455),
+// each entity drawn once per eye with that eye's matrices (onBeforeRender per eye camera, index.js:184-195)
+extern "C" int gs_render_scene_stereo_async(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
+                                            const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
+                                            void *const out_rgba[2], uint64_t *out_ticket) {
+  if (!c) return GS_ERR_INVALID;
+  if (!eyes || !eye_modelviews || !out_rgba || !out_rgba[0] || !out_rgba[1])
+    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: missing eyes, eye modelviews or outputs");
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render_scene_stereo before any push");
+  if (eyes[0].width != eyes[1].width || eyes[0].height != eyes[1].height)
+    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: the eyes must have the same size");
+  if (eyes[0].flags != eyes[1].flags) return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: the eyes must have the same flags");
+  if (eyes[0].flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS | GS_RENDER_OUT_TILED | GS_RENDER_OUT_PEER))
+    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: GS_RENDER_REUSE_SORT, _STATS, _OUT_TILED and _OUT_PEER are not accepted");
+  if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: not on a sharded context");
+  if (eyes[1].out_format != GS_FORMAT_RGBA8 && eyes[1].out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+  size_t bytes = 0;
+  int rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
+  if (rc) return rc;
+  // each entity's per-eye modelviews, in the table's order (caller's entity k = its draw rank)
+  float mv[kMaxObjects][2][16];
+  const SceneTable &t = *c->scene_tmp;
+  for (uint32_t j = 0; j < t.n; ++j)
+    for (int e = 0; e < 2; ++e) memcpy(mv[j][e], eye_modelviews + ((size_t)e * n_objs + t.obj[j].rank) * 16, sizeof(mv[j][e]));
+  const StereoInput st{&eyes[1], color_in ? color_in[1] : nullptr, out_rgba[1], mv};
+  return render_async(c, &eyes[0], c->scene_tmp, bytes, color_in ? color_in[0] : nullptr, out_rgba[0], out_ticket, &st);
+}
+
+extern "C" int gs_render_scene_stereo(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
+                                      const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
+                                      void *const out_rgba[2], gs_stats *stats) {
+  uint64_t t = 0;
+  int rc = gs_render_scene_stereo_async(c, eyes, objs, eye_modelviews, n_objs, color_in, out_rgba, &t);
+  if (rc) return rc;
+  return gs_wait(c, t, stats);
 }
 
 extern "C" int gs_peer_export(gs_context *c, size_t frame_bytes, void *handle_out) {

@@ -136,6 +136,14 @@ struct SceneTable {
   uint32_t pad[2];
   SceneObject obj[kMaxObjects];
 };
+// ---- stereo scene frames (gs_render_scene_stereo): one head-camera sort, both eyes projected, binned and rasterised in
+// one pass each.  Bin ids of the pair are eye * n_bins + bin; eye e's raster CTAs are blocks [e * n_tiles, (e+1) * n_tiles).
+// Per slot, fixed size, allocated by the first stereo frame; only the entities in use are copied per frame. ----
+struct StereoParams {
+  FrameParams eye[2];              // each eye's frame (projection, viewport, output, colour / depth target); eye[0] also
+                                   // carries n_splats for the sort, as a slot's FrameParams does
+  float mv[kMaxObjects][2][16];    // entity k's (scene-table order) gsModelViewMatrix of eye e
+};
 // per-entity results of the depth pass (one worker's min / max / validCount, index.js:548-555)
 struct ObjCounters {
   unsigned long long min_enc, max_enc;  // encodings as in SortHeader
@@ -212,7 +220,11 @@ struct gs_context {
   uint32_t *order[2] = {nullptr, nullptr};    // draw order (== reference sortedIndexes)
   float4 *proj_rec[2] = {nullptr, nullptr};   // 2 x float4 per splat
   uint32_t *rect[2] = {nullptr, nullptr};     // packed tile rect per splat
-  uint32_t *table_n = nullptr;   // radix chunk histograms of the depth passes [256][table_n_stride]
+  // the second eye's proj_rec / rect of stereo scene frames, allocated by the first one
+  uint32_t stereo_cap = 0;
+  float4 *proj_rec1[2] = {nullptr, nullptr};
+  uint32_t *rect1[2] = {nullptr, nullptr};
+  uint32_t *table_n = nullptr;  // radix chunk histograms of the depth passes [256][table_n_stride]
   uint32_t table_n_stride = 0;
   uint32_t *totals = nullptr;    // [512]: digit totals of the depth / tile passes
   uint32_t *slice_total = nullptr;   // instances per 256-entry slice of the draw order
@@ -278,15 +290,21 @@ struct gs_context {
     gs::FrameCounters *ctr_host = nullptr;   // pinned
     gs::FrameParams *fp = nullptr;           // device
     gs::FrameParams *fp_host = nullptr;      // pinned staging
-    void *frame_dev = nullptr;               // used when the caller's buffer is host memory
-    size_t frame_bytes = 0;
-    void *depth_dev = nullptr;               // staging of a host depth_in
-    size_t depth_bytes = 0;
-    const void *color_in = nullptr;          // caller's colour target (scene frames), host unless color_device
+    // per eye ([1]: the second eye of a stereo scene frame)
+    void *frame_dev[2] = {};                 // used when the caller's buffer is host memory
+    size_t frame_bytes[2] = {};
+    void *depth_dev[2] = {};                 // staging of a host depth_in
+    size_t depth_bytes[2] = {};
+    const void *color_in[2] = {};            // caller's colour target (scene frames), host unless color_device
     bool color_device = false;
-    void *color_dev = nullptr;               // staging of a host color_in
-    size_t color_bytes = 0;
+    void *color_dev[2] = {};                 // staging of a host color_in
+    size_t color_bytes[2] = {};
     bool scene = false;                      // multi-entity frame (gs_render_scene): scene table below
+    bool stereo = false;                     // stereo scene frame (gs_render_scene_stereo): stereo table below
+    gs_render_params eye1{};                 // its second eye
+    gs::StereoParams *stereo_dev = nullptr;  // device copy, fixed size (captured graphs bake the pointer)
+    gs::StereoParams *stereo_host = nullptr; // pinned staging
+    size_t stereo_bytes = 0;                 // bytes in use (both eyes' frames + the entities in use)
     gs::SceneTable *scene_dev = nullptr;     // device copy, fixed size (captured graphs bake the pointer)
     gs::SceneTable *scene_host = nullptr;    // pinned staging
     size_t scene_bytes = 0;                  // bytes of the table in use (header + non-empty entities)
@@ -309,19 +327,20 @@ struct gs_context {
     cudaGraphExec_t graph_sa[2][2] = {};       // slab path: keys stage, [set][plain | scene frame]
     cudaGraphExec_t graph_sl[2][2][3] = {};    // slab path: slab loop + resolve, [set][plain | scene frame][plain | depth | peer]
     int graph_slabs[2][2] = {};                // slab count baked into graph_sa / graph_sl, [set][plain | scene frame]
+    cudaGraphExec_t graph_xa[2] = {}, graph_xb[2] = {}, graph_xr[2] = {};  // stereo scene frames: the three stages, [set]
     bool peer = false;
     uint64_t ticket = 0;
     int ring = 0;                            // slot of the shared frame ring (fused exchange)
     unsigned long long peer_seq = 0;
-    void *frame_src = nullptr;               // device buffer the host copy reads
+    void *frame_src[2] = {};                 // device buffer the host copy reads
     cudaEvent_t ev_sorted = nullptr;                // sort/project stage of this slot's frame finished
     cudaEvent_t ev_binned = nullptr;                // binning stage finished
     cudaEvent_t ev_r0 = nullptr;                    // raster start (timing)
     int index = 0;
     bool pending = false;
     bool host_out = false;
-    void *out_user = nullptr;
-    size_t out_bytes = 0;
+    void *out_user[2] = {};
+    size_t out_bytes[2] = {};
     gs_render_params params{};
     uint32_t launches = 0;
     int set = 0;                                    // which order/proj_rec/rect and inst_rec/bin_range copy it uses
@@ -355,6 +374,7 @@ struct gs_context {
   uint32_t raster_base_flags = 1;                // default pixel loop: 1 = two pixels per lane, 0 = one
   // graph cache key: anything baked into the captured launches
   struct GraphKey { uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr; } gkey;
+  GraphKey gkey_stereo;                          // ... of the stereo graphs (kept apart: a stereo frame re-captures only its own)
 
   // ---- fused exchange: one shared allocation per rank = flag rows + a ring of 3 frames, opened by every peer ----
   void *peer_local = nullptr;            // our shared block
@@ -384,7 +404,9 @@ struct FrameBufs {
   float4 *proj_rec;
   uint32_t *rect;
   float4 *inst_rec;
-  uint2 *bin_range;  // [n_bins] {start, end} of each bin's run in inst_rec
+  uint2 *bin_range;  // [n_bins] {start, end} of each bin's run in inst_rec (stereo frames: [2 * n_bins], eye-major)
+  float4 *proj_rec1 = nullptr;  // stereo scene frames: the second eye's records and rectangles (NULL otherwise)
+  uint32_t *rect1 = nullptr;
 };
 
 // -- launchers (each .cu file owns its kernels); every per-frame input comes from device memory (fp, ctr) --
@@ -398,6 +420,9 @@ void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *s
 void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 9 launches
 void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
                           const FrameBufs &b, cudaStream_t st);
+// stereo scene frames: both eyes' projection in one pass (fp = &stereo->eye[0]) -> b.proj_rec / rect, b.proj_rec1 / rect1
+void launch_project_stereo(gs_context *c, const StereoParams *stereo, const SceneTable *scene, const FrameCounters *ctr,
+                           const FrameBufs &b, cudaStream_t st);
 void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_t n, cudaStream_t st);
 // PLY push: k_pack reading row perm[j] (perm NULL: row j) into slot first + j; rows_out (or NULL) receives the ordered rows
 void launch_pack_perm(gs_context *c, const uint8_t *rows_dev, const uint32_t *perm, uint32_t first, uint32_t n,
@@ -414,11 +439,15 @@ void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, 
 uint32_t *launch_ply_sort(gs_context *c, const uint32_t *key, uint32_t *perm_a, uint32_t *perm_b, uint32_t *table,
                           uint32_t *totals, uint32_t n, cudaStream_t st);
 void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
-// bin instances in draw order (2 launches); bin_open: the slab path's open-bin table, NULL for one-pass frames
+// bin instances in draw order (2 launches); bin_open: the slab path's open-bin table, NULL for one-pass frames.
+// b.rect1 set (stereo frames): both eyes' instances, eye 1's bins numbered from fp->rc.n_bins on
 void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,
                  cudaStream_t st);
+// n_bins: bins of the frame (stereo frames: of both eyes, the record then gathered from b.proj_rec1 from n_bins / 2 on)
 void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, cudaStream_t st);  // 3 .. 7 launches
 void launch_raster(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags, cudaStream_t st);
+// stereo scene frames: one grid of 2 * n_tiles CTAs, eye e's frame at fp + e (flags: packed | depth)
+void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags, cudaStream_t st);
 void launch_peer_acquire(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
 void launch_peer_signal_wait(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
 struct PeerRows { unsigned long long *p[kMaxPeers]; };

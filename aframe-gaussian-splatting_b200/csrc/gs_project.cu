@@ -3,13 +3,14 @@
 //
 //   k_project  : fp32 restatement of the vertex shader, op for op (no FMA contraction), producing a
 //                32 B projected record per splat + its packed tile rectangle (scene frames: with each splat's entity's
-//                gsModelViewMatrix).
+//                gsModelViewMatrix; stereo scene frames: both eyes per splat, the table row loaded once).
 //   k_count    : per entry of the draw order (== reference sortedIndexes): instance offset inside its 256-entry slice;
 //                per slice: total; last CTA: prefix over the slices + frame total D.
 //                Sparse frames (fewer than half of the splats sorted): each chunk's survivors are compacted first.
 //   k_emit_entries: one thread per draw-order entry writes its (bin, splat) instances at the entry's offset,
 //                in draw order, so that a STABLE sort by bin id alone reproduces the reference's back-to-front order
-//                inside every bin; rectangles of more than 8 bins are finished by the whole warp.
+//                inside every bin; rectangles of more than 8 bins are finished by the whole warp.  Stereo scene frames:
+//                each entry emits eye 0's instances, then eye 1's, with bin ids eye * n_bins + bin.
 #include "gs_common.cuh"
 
 namespace gs {
@@ -38,12 +39,12 @@ __device__ __forceinline__ void unpack_int16(uint32_t value, float &lo, float &h
 // ---------------------------------------------------------------------------------------------
 // One splat through the vertex shader: returns its packed bin rectangle (kNoRect when nothing is drawn) and stores the
 // 32 B record at slot j.
-// mv: the splat's gsModelViewMatrix (rc.mv, or its entity's in a scene frame).
-__device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const float *mv, const float4 *__restrict__ cs,
+// mv: the splat's gsModelViewMatrix (rc.mv, or its entity's in a scene frame).  c: its center_scale row; q: its
+// cov_color row, loaded on the first call that needs it (have_q), so a stereo frame's two eyes load each row once.
+__device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const float *mv, const float4 c,
                                                 const uint4 *__restrict__ cc, uint32_t i, uint32_t j,
-                                                float4 *__restrict__ rec_out) {
+                                                float4 *__restrict__ rec_out, uint4 &q, bool &have_q) {
   uint32_t rect = kNoRect;
-  const float4 c = __ldg(cs + i);
   const float *P = rc.proj;
   // index.js:106-108: camspace = MV * (center,1); pos2d = P * camspace  (sum x,y,z,w left to right)
   float cam[4], p[4];
@@ -57,7 +58,10 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
   const float bounds = MUL(1.2f, p[3]);
   const bool culled = (p[2] < -p[3]) || (p[0] < -bounds) || (p[0] > bounds) || (p[1] < -bounds) || (p[1] > bounds);
   if (!culled) {
-    const uint4 q = __ldg(cc + i);
+    if (!have_q) {
+      q = __ldg(cc + i);
+      have_q = true;
+    }
     // index.js:117-125
     float c00, c01, c02, c11, c12, c22;
     unpack_int16(q.x, c00, c01);
@@ -148,13 +152,18 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
 // instead of warps with a few live lanes each.
 // SCENE (scene frames, by index or, on the slab path, by entry): every splat takes its entity's modelview; by index, the
 // splat the Q5 tail may repeat is each entity's first one.
-template <bool BY_ENTRY, bool SCENE = false>
+// STEREO (stereo scene frames, by index): fp = &stereo->eye[0]; every splat is projected for both eyes with each eye's
+// RenderConsts and its entity's per-eye modelview, eye 1 into rec_out1 / rect_out1.
+template <bool BY_ENTRY, bool SCENE = false, bool STEREO = false>
 __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, const uint4 *__restrict__ cc,
                                                  const float *__restrict__ depth,
                                                  const FrameParams *__restrict__ fp, float4 *__restrict__ rec_out,
                                                  uint32_t *__restrict__ rect_out, const uint32_t *__restrict__ order,
                                                  const FrameCounters *__restrict__ ctr,
-                                                 const SceneTable *__restrict__ scene) {
+                                                 const SceneTable *__restrict__ scene,
+                                                 const StereoParams *__restrict__ stereo, float4 *__restrict__ rec_out1,
+                                                 uint32_t *__restrict__ rect_out1) {
+  static_assert(!STEREO || (SCENE && !BY_ENTRY), "stereo frames are scene frames projected by index");
   GS_PDL_ENTRY();
   const RenderConsts &rc = fp->rc;
   const uint32_t n = BY_ENTRY ? ctr->sort.n_valid : fp->n_splats;
@@ -179,6 +188,20 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
     if (!SCENE) return rc.mv;
     return scene->obj[scene_find(s_first, s_end, n_obj, i)].mv;
   };
+  // splat i through the vertex shader (of each eye), record at slot j; returns eye 0's rectangle, eye 1's in *rect1
+  auto shade = [&](uint32_t i, uint32_t j, uint32_t *rect1) -> uint32_t {
+    uint4 q;
+    bool have_q = false;
+    if (!STEREO) {
+      const float *mv = modelview(i);
+      return project_one(rc, mv, __ldg(cs + i), cc, i, j, rec_out, q, have_q);
+    }
+    const float(*mv)[16] = stereo->mv[scene_find(s_first, s_end, n_obj, i)];
+    const float4 c = __ldg(cs + i);
+    const uint32_t r0 = project_one(rc, mv[0], c, cc, i, j, rec_out, q, have_q);
+    *rect1 = project_one(stereo->eye[1].rc, mv[1], c, cc, i, j, rec_out1, q, have_q);
+    return r0;
+  };
   if (!BY_ENTRY && (unsigned long long)ctr->sort.n_valid * 2ull < n) {
     constexpr uint32_t kChunk = 1024;  // 4 splats per thread
     __shared__ uint32_t s_list[kChunk];
@@ -193,11 +216,13 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
         d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
         // no rectangle unless a survivor stores one after the barrier below
         *(uint4 *)(rect_out + base) = make_uint4(kNoRect, kNoRect, kNoRect, kNoRect);
+        if (STEREO) *(uint4 *)(rect_out1 + base) = make_uint4(kNoRect, kNoRect, kNoRect, kNoRect);
       } else {
 #pragma unroll
         for (uint32_t k = 0; k < 4; ++k) {
           d[k] = (base + k < n) ? __ldg(depth + base + k) : GS_DEPTH_REJECT;
           if (base + k < n) rect_out[base + k] = kNoRect;
+          if (STEREO && base + k < n) rect_out1[base + k] = kNoRect;
         }
       }
       bool f[4];
@@ -227,8 +252,10 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
       __syncthreads();
       for (uint32_t q = tid; q < total; q += blockDim.x) {
         const uint32_t i = s_list[q];
-        const uint32_t rect = project_one(rc, modelview(i), cs, cc, i, i, rec_out);
+        uint32_t rect1 = kNoRect;
+        const uint32_t rect = shade(i, i, &rect1);
         if (rect != kNoRect) rect_out[i] = rect;
+        if (STEREO && rect1 != kNoRect) rect_out1[i] = rect1;
       }
       __syncthreads();
     }
@@ -236,10 +263,11 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
   }
   for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
     const uint32_t i = BY_ENTRY ? __ldg(order + j) : j;
-    uint32_t rect = kNoRect;
+    uint32_t rect = kNoRect, rect1 = kNoRect;
     const bool sorted = BY_ENTRY || (__ldg(depth + i) != GS_DEPTH_REJECT) || q5_head(i);
-    if (sorted) rect = project_one(rc, modelview(i), cs, cc, i, j, rec_out);
+    if (sorted) rect = shade(i, j, &rect1);
     rect_out[j] = rect;
+    if (STEREO) rect_out1[j] = rect1;
   }
 }
 
@@ -262,14 +290,17 @@ __device__ __forceinline__ uint32_t rect_count(uint32_t r, uint32_t rank, uint32
 // ---------------------------------------------------------------------------------------------
 // SLAB: rect is indexed by entry (k_project<true>), the entry's payload is j itself, and entries whose (small)
 // rectangle holds only closed bins own nothing any more.
-template <bool SLAB>
+// STEREO (stereo scene frames, one GPU): an entry owns its eye-0 instances, then its eye-1 instances (rect1); it stays
+// live when either eye sees it.
+template <bool SLAB, bool STEREO = false>
 __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restrict__ order,
                                                         const uint32_t *__restrict__ rect,
                                                         uint2 *__restrict__ ent, uint32_t *__restrict__ ent_off,
                                                         uint32_t *__restrict__ slice_total,
                                                         uint32_t *__restrict__ slice_prefix, FrameCounters *ctr,
                                                         const FrameParams *__restrict__ fp,
-                                                        const uint32_t *__restrict__ bin_open) {
+                                                        const uint32_t *__restrict__ bin_open,
+                                                        const uint32_t *__restrict__ rect1) {
   GS_PDL_ENTRY();
   const uint32_t shard_rank = fp->rc.shard_rank, shard_world = fp->rc.shard_world;
   __shared__ uint32_t s_warp[kEmitThreads / 32], s_vis[kEmitThreads / 32];
@@ -279,10 +310,11 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
   const uint32_t num_slices = (nv + kEmitTile - 1) / kEmitTile;
   for (uint32_t sl = blockIdx.x; sl < num_slices; sl += gridDim.x) {
     const uint32_t j = sl * kEmitTile + tid;
-    uint32_t idx = 0, r = kNoRect;
+    uint32_t idx = 0, r = kNoRect, r1 = kNoRect;
     if (j < nv) {
       idx = SLAB ? j : __ldg(order + j);
       r = __ldg(rect + idx);
+      if (STEREO) r1 = __ldg(rect1 + idx);
     }
     uint32_t cnt = rect_count(r, shard_rank, shard_world);
     if (SLAB && cnt) {
@@ -294,7 +326,8 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
         if (!any) cnt = 0;
       }
     }
-    uint32_t incl = cnt, vis = (r != kNoRect);
+    if (STEREO) cnt += rect_count(r1, 0u, 1u);
+    uint32_t incl = cnt, vis = (r != kNoRect) + (STEREO && r1 != kNoRect);
     for (int o = 1; o < 32; o <<= 1) {
       const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
       if (lane >= (uint32_t)o) incl += t;
@@ -360,25 +393,31 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
 // against the r<=2 footprint; rejected bins (and, on the slab path, closed ones) become kNoTile and are dropped by the
 // bin sort.
 // ---------------------------------------------------------------------------------------------
+// bin_base: first bin id of the eye (stereo frames: eye * n_bins; else 0)
 __device__ __forceinline__ void emit_candidate(const RenderConsts &rc, uint32_t bx, uint32_t by, bool multi, const float4 &r0,
                                                const float2 &r1, const uint32_t *__restrict__ bin_open, uint32_t payload,
-                                               size_t pos, uint16_t *__restrict__ inst_tile, uint32_t *__restrict__ inst_idx) {
+                                               size_t pos, uint16_t *__restrict__ inst_tile, uint32_t *__restrict__ inst_idx,
+                                               uint32_t bin_base) {
   bool keep = true;
   if (multi)
     keep = footprint_meets_box(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, (float)(bx * kBin) + 0.5f, (float)(by * kBin) + 0.5f,
                                (float)(kBin - 1));
-  const uint32_t t = by * rc.bins_x + bx;
+  const uint32_t t = bin_base + by * rc.bins_x + bx;
   if (keep && bin_open) keep = __ldg(bin_open + t) != 0u;
   inst_tile[pos] = keep ? (uint16_t)t : kNoTile;
   inst_idx[pos] = payload;
 }
 
+// STEREO: each entry writes its eye-0 instances, then its eye-1 instances (rectangle rect1, records proj_rec1, bin ids
+// from rc.n_bins on; the eyes share the viewport size, hence the bin grid)
+template <bool STEREO = false>
 __global__ void __launch_bounds__(256) k_emit_entries(const uint2 *__restrict__ ent, const uint32_t *__restrict__ ent_off,
                                                       const uint32_t *__restrict__ slice_prefix,
                                                       const float4 *__restrict__ proj_rec, const FrameParams *__restrict__ fp,
                                                       uint64_t cap_inst, uint16_t *__restrict__ inst_tile,
                                                       uint32_t *__restrict__ inst_idx, FrameCounters *ctr,
-                                                      const uint32_t *__restrict__ bin_open) {
+                                                      const uint32_t *__restrict__ bin_open,
+                                                      const float4 *__restrict__ proj_rec1, const uint32_t *__restrict__ rect1) {
   GS_PDL_ENTRY();
   const RenderConsts &rc = fp->rc;
   const uint32_t nv = ctr->sort.n_valid;
@@ -392,54 +431,62 @@ __global__ void __launch_bounds__(256) k_emit_entries(const uint2 *__restrict__ 
   for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < nv_pad; j += stride) {
     uint2 en = make_uint2(0u, kNoRect);
     if (j < nv) en = __ldg(ent + j);
-    const uint32_t r = en.y;
-    uint32_t bx0 = 0, by0 = 0, w = 0, h = 0, step = 1, n_own = 0;
-    size_t base = 0;
-    float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f);
-    float2 r1 = make_float2(0.f, 0.f);
-    bool multi = false;
-    if (r != kNoRect) {
-      bx0 = r & 255u;
-      by0 = (r >> 16) & 255u;
-      h = (r >> 24) - by0 + 1u;
-      w = ((r >> 8) & 255u) - bx0 + 1u;
-      multi = w * h > 1u;
-      if (rc.shard_world > 1) {  // owned columns of the rectangle: first, first + world, ...
-        owned_span(bx0, (r >> 8) & 255u, rc.shard_rank, rc.shard_world, bx0, w);
-        step = rc.shard_world;
+    uint32_t off = 0;  // instances of the entry's earlier eye
+#pragma unroll
+    for (uint32_t eye = 0; eye < (STEREO ? 2u : 1u); ++eye) {
+      const uint32_t r = eye == 0u ? en.y : (j < nv ? __ldg(rect1 + en.x) : kNoRect);
+      const float4 *rec = eye == 0u ? proj_rec : proj_rec1;
+      const uint32_t bin_base = eye * rc.n_bins;
+      uint32_t bx0 = 0, by0 = 0, w = 0, h = 0, step = 1, n_own = 0;
+      size_t base = 0;
+      float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f);
+      float2 r1 = make_float2(0.f, 0.f);
+      bool multi = false;
+      if (r != kNoRect) {
+        bx0 = r & 255u;
+        by0 = (r >> 16) & 255u;
+        h = (r >> 24) - by0 + 1u;
+        w = ((r >> 8) & 255u) - bx0 + 1u;
+        multi = w * h > 1u;
+        if (rc.shard_world > 1) {  // owned columns of the rectangle: first, first + world, ...
+          owned_span(bx0, (r >> 8) & 255u, rc.shard_rank, rc.shard_world, bx0, w);
+          step = rc.shard_world;
+        }
+        n_own = w * h;
+        base = (size_t)__ldg(slice_prefix + (j >> 8)) + __ldg(ent_off + j) + off;
+        if (multi) {
+          r0 = __ldg(rec + 2 * (size_t)en.x);
+          r1 = __ldg((const float2 *)(rec + 2 * (size_t)en.x + 1));
+        }
       }
-      n_own = w * h;
-      base = (size_t)__ldg(slice_prefix + (j >> 8)) + __ldg(ent_off + j);
-      if (multi) {
-        r0 = __ldg(proj_rec + 2 * (size_t)en.x);
-        r1 = __ldg((const float2 *)(proj_rec + 2 * (size_t)en.x + 1));
+      off += n_own;
+      const bool big = n_own > 8u;
+      if (!big) {
+        for (uint32_t k = 0; k < n_own; ++k) {
+          const uint32_t row = k / w;
+          emit_candidate(rc, bx0 + (k - row * w) * step, by0 + row, multi, r0, r1, bin_open, en.x, base + k, inst_tile, inst_idx,
+                         bin_base);
+        }
       }
-    }
-    const bool big = n_own > 8u;
-    if (!big) {
-      for (uint32_t k = 0; k < n_own; ++k) {
-        const uint32_t row = k / w;
-        emit_candidate(rc, bx0 + (k - row * w) * step, by0 + row, multi, r0, r1, bin_open, en.x, base + k, inst_tile, inst_idx);
-      }
-    }
-    // large rectangles: the warp finishes them together
-    uint32_t todo = __ballot_sync(0xffffffffu, big);
-    while (todo) {
-      const int src = __ffs(todo) - 1;
-      todo &= todo - 1;
-      const uint32_t s_bx0 = __shfl_sync(0xffffffffu, bx0, src), s_by0 = __shfl_sync(0xffffffffu, by0, src);
-      const uint32_t s_w = __shfl_sync(0xffffffffu, w, src), s_step = __shfl_sync(0xffffffffu, step, src);
-      const uint32_t s_n = __shfl_sync(0xffffffffu, n_own, src), s_pay = __shfl_sync(0xffffffffu, en.x, src);
-      const unsigned long long s_base = __shfl_sync(0xffffffffu, (unsigned long long)base, src);
-      float4 g0;
-      float2 g1;
-      g0.x = __shfl_sync(0xffffffffu, r0.x, src); g0.y = __shfl_sync(0xffffffffu, r0.y, src);
-      g0.z = __shfl_sync(0xffffffffu, r0.z, src); g0.w = __shfl_sync(0xffffffffu, r0.w, src);
-      g1.x = __shfl_sync(0xffffffffu, r1.x, src); g1.y = __shfl_sync(0xffffffffu, r1.y, src);
-      for (uint32_t k = lane; k < s_n; k += 32u) {
-        const uint32_t row = k / s_w;
-        emit_candidate(rc, s_bx0 + (k - row * s_w) * s_step, s_by0 + row, true, g0, g1, bin_open, s_pay, (size_t)s_base + k, inst_tile,
-                       inst_idx);
+      // large rectangles: the warp finishes them together
+      uint32_t todo = __ballot_sync(0xffffffffu, big);
+      while (todo) {
+        const int src = __ffs(todo) - 1;
+        todo &= todo - 1;
+        const uint32_t s_bx0 = __shfl_sync(0xffffffffu, bx0, src), s_by0 = __shfl_sync(0xffffffffu, by0, src);
+        const uint32_t s_w = __shfl_sync(0xffffffffu, w, src), s_step = __shfl_sync(0xffffffffu, step, src);
+        const uint32_t s_n = __shfl_sync(0xffffffffu, n_own, src), s_pay = __shfl_sync(0xffffffffu, en.x, src);
+        const unsigned long long s_base = __shfl_sync(0xffffffffu, (unsigned long long)base, src);
+        float4 g0;
+        float2 g1;
+        g0.x = __shfl_sync(0xffffffffu, r0.x, src); g0.y = __shfl_sync(0xffffffffu, r0.y, src);
+        g0.z = __shfl_sync(0xffffffffu, r0.z, src); g0.w = __shfl_sync(0xffffffffu, r0.w, src);
+        g1.x = __shfl_sync(0xffffffffu, r1.x, src); g1.y = __shfl_sync(0xffffffffu, r1.y, src);
+        for (uint32_t k = lane; k < s_n; k += 32u) {
+          const uint32_t row = k / s_w;
+          emit_candidate(rc, s_bx0 + (k - row * s_w) * s_step, s_by0 + row, true, g0, g1, bin_open, s_pay, (size_t)s_base + k,
+                         inst_tile, inst_idx, bin_base);
+        }
       }
     }
   }
@@ -451,7 +498,19 @@ void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *c
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   launch_chain(c, k_project<false>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
-               (const uint32_t *)nullptr, ctr, (const SceneTable *)nullptr);  // ctr: the sorted count picks the sparse-frame path
+               (const uint32_t *)nullptr, ctr, (const SceneTable *)nullptr,  // ctr: the sorted count picks the sparse-frame path
+               (const StereoParams *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr);
+}
+
+void launch_project_stereo(gs_context *c, const StereoParams *stereo, const SceneTable *scene, const FrameCounters *ctr,
+                           const FrameBufs &b, cudaStream_t stream) {
+  uint64_t blocks = ((uint64_t)c->cap + 255) / 256;
+  const uint64_t cap = (uint64_t)c->sm_count * 16;
+  if (blocks > cap) blocks = cap;
+  if (blocks < 1) blocks = 1;
+  launch_chain(c, k_project<false, true, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
+               (const float *)c->depth, &stereo->eye[0], b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, stereo,
+               b.proj_rec1, b.rect1);
 }
 
 void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
@@ -461,7 +520,8 @@ void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   launch_chain(c, k_project<false, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
-               (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene);
+               (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, (const StereoParams *)nullptr,
+               (float4 *)nullptr, (uint32_t *)nullptr);
 }
 
 // scene: the slot's scene table for a scene frame (every entry takes its entity's modelview), NULL for a plain frame
@@ -473,7 +533,7 @@ void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters 
   if (blocks < 1) blocks = 1;
   launch_chain(c, scene ? k_project<true, true> : k_project<true>, (int)blocks, 256, stream, (const float4 *)c->center_scale,
                (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)b.order,
-               (const FrameCounters *)ctr, scene);
+               (const FrameCounters *)ctr, scene, (const StereoParams *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr);
 }
 
 void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,
@@ -482,10 +542,13 @@ void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const
   const uint64_t cap = (uint64_t)c->sm_count * 8;
   if (tiles > cap) tiles = cap;
   if (tiles < 1) tiles = 1;
-  launch_chain(c, bin_open ? k_count<true> : k_count<false>, (int)tiles, kEmitThreads, st, (const uint32_t *)b.order,
-               (const uint32_t *)b.rect, c->ent, c->ent_off, c->slice_total, c->slice_prefix, ctr, fp, bin_open);
-  launch_chain(c, k_emit_entries, (int)tiles, 256, st, (const uint2 *)c->ent, (const uint32_t *)c->ent_off, (const uint32_t *)c->slice_prefix,
-               (const float4 *)b.proj_rec, fp, (uint64_t)c->cap_inst, c->inst_tile, c->inst_idx, ctr, bin_open);
+  const bool stereo = b.rect1 != nullptr;
+  launch_chain(c, bin_open ? k_count<true> : (stereo ? k_count<false, true> : k_count<false>), (int)tiles, kEmitThreads, st,
+               (const uint32_t *)b.order, (const uint32_t *)b.rect, c->ent, c->ent_off, c->slice_total, c->slice_prefix, ctr, fp, bin_open,
+               (const uint32_t *)b.rect1);
+  launch_chain(c, stereo ? k_emit_entries<true> : k_emit_entries<false>, (int)tiles, 256, st, (const uint2 *)c->ent, (const uint32_t *)c->ent_off,
+               (const uint32_t *)c->slice_prefix, (const float4 *)b.proj_rec, fp, (uint64_t)c->cap_inst, c->inst_tile, c->inst_idx, ctr,
+               bin_open, (const float4 *)b.proj_rec1, (const uint32_t *)b.rect1);
 }
 
 }  // namespace gs

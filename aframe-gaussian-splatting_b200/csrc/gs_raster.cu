@@ -167,14 +167,20 @@ struct SlabIO {
 // DEPTH: depth-test every fragment LEQUAL against fp->depth_in (index.js:179-180).  STATS: count what the tile does
 // (and keep culling the whole list after the tile has closed, so that the count of 16x16 tile instances is exact).
 // SLAB: one depth slab of a frame: start from / store back the pixel state, close saturated tiles; k_resolve writes the frame.
-template <bool PACKED, bool DEPTH, bool STATS, bool SLAB = false>
+// STEREO: both eyes of a stereo scene frame, 2 * n_tiles CTAs: CTA b draws tile b % n_tiles of eye b / n_tiles, with that
+// eye's frame fp[eye] (output, colour target, depth target: an eye without one keeps the depth 1, which passes every
+// fragment the projection keeps) and bins from eye * n_bins on.  The pixel loop is the one of the plain frame.
+template <bool PACKED, bool DEPTH, bool STATS, bool SLAB = false, bool STEREO = false>
 __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>::kMinBlocks) k_raster(const float4 *__restrict__ inst_rec,
                                                                         const uint2 *__restrict__ bin_range,
                                                                         const FrameParams *__restrict__ fp,
                                                                         uint4 *__restrict__ tile_stats, SlabIO slab) {
+  static_assert(!STEREO || (!STATS && !SLAB), "stereo frames take the one-pass path without statistics");
   using Cfg = RasterCfg<PACKED>;
   constexpr int kThreads = Cfg::kThreads, kChunk = Cfg::kChunk, kStages = Cfg::kStages, kCv = Cfg::kCv;
   constexpr int kWarps = kThreads / 32;
+  const uint32_t eye = STEREO ? (blockIdx.x >= fp->rc.n_tiles ? 1u : 0u) : 0u;
+  if (STEREO) fp += eye;
   const RenderConsts &rc = fp->rc;
   __shared__ __align__(128) float4 s_rec[kStages][kChunk * 2];
   __shared__ __align__(16) float4 s_cv[kChunk * kCv];
@@ -182,11 +188,11 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   __shared__ uint32_t s_wcnt[kWarps];
   __shared__ uint32_t s_stat[4];
 
-  const uint32_t tile = blockIdx.x;
+  const uint32_t tile = blockIdx.x - eye * rc.n_tiles;
   const uint32_t tx = tile % rc.tiles_x, ty = tile / rc.tiles_x;
   const uint32_t bcol = tx / kTilesPerBin;
   if (rc.shard_world > 1 && (bcol % rc.shard_world) != rc.shard_rank) return;
-  const uint32_t bin = (ty / kTilesPerBin) * rc.bins_x + bcol;
+  const uint32_t bin = eye * rc.n_bins + (ty / kTilesPerBin) * rc.bins_x + bcol;
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   // pixel ownership.  scalar: a warp owns a compact 8x4 block, tid = [ty2 tx1 | y2 x3].  packed: a warp owns an 8x8
@@ -208,8 +214,8 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   float d0 = 1.0f, d1 = 1.0f;  // window depth of the foreign geometry at the pixel(s)
   if (DEPTH) {
     const float *din = (const float *)fp->depth_in;
-    if (inside0) d0 = __ldg(din + (size_t)y * rc.width + x);
-    if (inside1) d1 = __ldg(din + (size_t)(y + 1) * rc.width + x);
+    if (inside0 && (!STEREO || din)) d0 = __ldg(din + (size_t)y * rc.width + x);
+    if (inside1 && (!STEREO || din)) d1 = __ldg(din + (size_t)(y + 1) * rc.width + x);
   }
 
   const uint2 range = bin_range[bin];
@@ -479,6 +485,19 @@ void launch_raster(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const
     GS_RASTER_CASE(5, true, false, true)
     GS_RASTER_CASE(6, false, true, true)
     GS_RASTER_CASE(7, true, true, true)
+#undef GS_RASTER_CASE
+  }
+}
+
+void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags,
+                          cudaStream_t st) {
+  switch (flags & 3u) {
+#define GS_RASTER_CASE(v, P, D) \
+  case v: k_raster<P, D, false, false, true><<<2 * n_tiles, RasterCfg<P>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{}); break;
+    GS_RASTER_CASE(0, false, false)
+    GS_RASTER_CASE(1, true, false)
+    GS_RASTER_CASE(2, false, true)
+    GS_RASTER_CASE(3, true, true)
 #undef GS_RASTER_CASE
   }
 }

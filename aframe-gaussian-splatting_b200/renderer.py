@@ -261,6 +261,57 @@ class SplatContext:
         self.last_stereo_stats = [stats[0], stats[1]]
         return outs
 
+    @staticmethod
+    def _stereo_args(eyes_params, objects: Sequence[SceneObject], eye_modelviews, color_ptrs, out_ptrs):
+        """ctypes arguments of gs_render_scene_stereo[_async]: eye_modelviews[e][k] is entity k's modelview of eye e."""
+        assert len(eyes_params) == 2 and len(out_ptrs) == 2
+        arr = (GsRenderParams * 2)()
+        for i in range(2):
+            C.memmove(C.addressof(arr[i]), C.addressof(eyes_params[i]), C.sizeof(GsRenderParams))
+        mv = np.ascontiguousarray(np.asarray(eye_modelviews, np.float32).reshape(2, len(objects), 16))
+        col = None
+        if color_ptrs is not None:
+            col = (C.c_void_p * 2)(*[None if p is None else C.c_void_p(p) for p in color_ptrs])
+        outs = (C.c_void_p * 2)(*[C.c_void_p(p) for p in out_ptrs])
+        return arr, make_objects(objects), mv, col, outs
+
+    def render_scene_stereo(self, eyes: Sequence[FrameInputs], objects: Sequence[SceneObject], eye_modelviews,
+                            color_in=(None, None), depth_in=(None, None), bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8):
+        """gs_render_scene_stereo: one WebXR frame of a multi-entity page.  `objects` carry each entity's range, HEAD
+        modelview (its sort) and cutout, in draw order; eyes[e] (FrameInputs) gives eye e's projection, size and focal;
+        eye_modelviews[e][k] is entity k's modelview of eye e.  color_in[e] / depth_in[e]: eye e's colour target ((H, W, 4)
+        of the output dtype) and window-space depth ((H, W) f32), or None.  Returns the two frames, row 0 = bottom."""
+        assert len(eyes) == 2
+        dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
+        outs = [np.empty((e.height, e.width, 4), dtype) for e in eyes]
+        cols = []
+        for e, c in zip(eyes, color_in):
+            if c is not None:
+                c = np.ascontiguousarray(c, dtype=dtype)
+                if c.size != e.width * e.height * 4:
+                    raise ValueError("color_in must hold width*height RGBA pixels")
+            cols.append(c)
+        params = [self.make_params(e, bg, fmt, 0, depth_in=d) for e, d in zip(eyes, depth_in)]
+        arr, objs, mv, col, ptrs = self._stereo_args(params, objects, eye_modelviews,
+                                                     [None if c is None else c.ctypes.data for c in cols],
+                                                     [o.ctypes.data for o in outs])
+        st = GsStats()
+        self._check(self._lib.gs_render_scene_stereo(self._h, arr, objs, mv.ctypes.data_as(C.POINTER(C.c_float)), len(objects),
+                                                     col, ptrs, C.byref(st)))
+        self.last_stats = st
+        return outs
+
+    def render_scene_stereo_async(self, eyes_params, objects: Sequence[SceneObject], eye_modelviews, color_ptrs,
+                                  out_ptrs) -> int:
+        """gs_render_scene_stereo_async: enqueue one stereo scene frame (collected with wait()).  eyes_params: two
+        GsRenderParams; color_ptrs: None or two pointers (each None, host, or device with GS_RENDER_COLOR_DEVICE);
+        out_ptrs: two pointers.  Every buffer must stay valid until the ticket is waited for."""
+        arr, objs, mv, col, ptrs = self._stereo_args(eyes_params, objects, eye_modelviews, color_ptrs, out_ptrs)
+        t = C.c_uint64()
+        self._check(self._lib.gs_render_scene_stereo_async(self._h, arr, objs, mv.ctypes.data_as(C.POINTER(C.c_float)),
+                                                           len(objects), col, ptrs, C.byref(t)))
+        return t.value
+
     def render_raw(self, params: GsRenderParams, out_ptr: int) -> GsStats:
         """gs_render with a caller-provided pointer (device pointer when GS_RENDER_OUT_DEVICE is set)."""
         st = GsStats()

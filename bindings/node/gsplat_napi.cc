@@ -14,7 +14,8 @@ class Splats : public Napi::ObjectWrap<Splats> {
       InstanceMethod("pushPly", &Splats::PushPly), InstanceMethod("reserve", &Splats::Reserve),
       InstanceMethod("sort", &Splats::Sort),   InstanceMethod("render", &Splats::Render),
       InstanceMethod("renderScene", &Splats::RenderScene), InstanceMethod("insert", &Splats::Insert),
-      InstanceMethod("insertPly", &Splats::InsertPly), InstanceMethod("erase", &Splats::Erase)}));
+      InstanceMethod("insertPly", &Splats::InsertPly), InstanceMethod("erase", &Splats::Erase),
+      InstanceMethod("renderSceneXR", &Splats::RenderSceneXR)}));
     return exports;
   }
   explicit Splats(const Napi::CallbackInfo& i) : Napi::ObjectWrap<Splats>(i) {
@@ -114,6 +115,49 @@ class Splats : public Napi::ObjectWrap<Splats> {
     }
     const void* color = i[2].IsUndefined() ? nullptr : i[2].As<Napi::Uint8Array>().Data();
     Check(i.Env(), gs_render_scene(ctx_, &p, objs.data(), (uint32_t)objs.size(), color, i[3].As<Napi::Uint8Array>().Data(), nullptr));
+    return i.Env().Undefined();
+  }
+  // renderSceneXR([eyeL, eyeR] {proj, width, height, focal, depth?: Float32Array}, [{first, count, modelview, cutout?,
+  //                eyeModelviews: [Float32Array, Float32Array]}, ...], [colorL, colorR] (Uint8Array or undefined),
+  //                [outL, outR] Uint8Array)  <- an XR frame of every entity of the page: each entity's tick() sort from the head
+  // camera (modelview = its getModelViewMatrix()), its draw once per eye with eyeModelviews[e] = getModelViewMatrix(eyeCamera
+  // e); both eyes share the XR layer's viewport size.  One gs_render_scene_stereo: one sort, both eyes in one pass.
+  Napi::Value RenderSceneXR(const Napi::CallbackInfo& i) {
+    auto eyes_in = i[0].As<Napi::Array>();
+    gs_render_params eyes[2] = {};
+    for (uint32_t e = 0; e < 2; ++e) {
+      auto o = eyes_in.Get(e).As<Napi::Object>();
+      memcpy(eyes[e].proj, o.Get("proj").As<Napi::Float32Array>().Data(), 64);
+      eyes[e].width = o.Get("width").As<Napi::Number>().Uint32Value();
+      eyes[e].height = o.Get("height").As<Napi::Number>().Uint32Value();
+      eyes[e].focal = o.Get("focal").As<Napi::Number>().FloatValue();
+      if (o.Has("depth")) eyes[e].depth_in = o.Get("depth").As<Napi::Float32Array>().Data();
+      eyes[e].out_format = GS_FORMAT_RGBA8;
+    }
+    auto list = i[1].As<Napi::Array>();
+    const uint32_t n = list.Length();
+    std::vector<gs_object> objs(n);
+    std::vector<float> eye_mv(2 * (size_t)n * 16);
+    for (uint32_t k = 0; k < n; ++k) {
+      auto e = list.Get(k).As<Napi::Object>();
+      gs_object& g = objs[k];
+      g = gs_object{};
+      g.first = e.Get("first").As<Napi::Number>().Uint32Value();
+      g.count = e.Get("count").As<Napi::Number>().Uint32Value();
+      memcpy(g.modelview, e.Get("modelview").As<Napi::Float32Array>().Data(), 64);
+      if (e.Has("cutout")) { g.has_cutout = 1; memcpy(g.cutout16, e.Get("cutout").As<Napi::Float32Array>().Data(), 64); }
+      auto mvs = e.Get("eyeModelviews").As<Napi::Array>();
+      for (uint32_t s = 0; s < 2; ++s) memcpy(&eye_mv[((size_t)s * n + k) * 16], mvs.Get(s).As<Napi::Float32Array>().Data(), 64);
+    }
+    auto cols = i[2].As<Napi::Array>();
+    auto outs = i[3].As<Napi::Array>();
+    const void* color[2];
+    void* out[2];
+    for (uint32_t s = 0; s < 2; ++s) {
+      color[s] = cols.Get(s).IsUndefined() ? nullptr : cols.Get(s).As<Napi::Uint8Array>().Data();
+      out[s] = outs.Get(s).As<Napi::Uint8Array>().Data();
+    }
+    Check(i.Env(), gs_render_scene_stereo(ctx_, eyes, objs.data(), eye_mv.data(), n, color, out, nullptr));
     return i.Env().Undefined();
   }
   gs_context* ctx_ = nullptr;

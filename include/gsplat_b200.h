@@ -315,6 +315,36 @@ GS_API int gs_render_scene(gs_context *ctx, const gs_render_params *frame, const
  */
 GS_API int gs_sort_scene(gs_context *ctx, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx, uint32_t *out_count);
 
+/*
+ * WebXR on a page of several entities: one scene sort per frame from the HEAD camera (each entity's tick(),
+ * index.js:438-455), then every entity drawn once per EYE with that eye's matrices (onBeforeRender per eye camera,
+ * index.js:184-195).  One pipelined frame covers both eyes: one sort, one projection and one binning pass for the pair,
+ * one raster grid over both eyes' tiles.
+ *   - objs[k]: entity k in draw order (objs[0] drawn first): its range, its HEAD getModelViewMatrix() - row 2 is the
+ *     view of its sort - and its cutout, which acts in the sort.  Ranges follow the rules of gs_render_scene.
+ *   - eye_modelviews: 2 * n_objs * 16 floats; entity k's getModelViewMatrix(eyeCamera) of eye e starts at
+ *     (e * n_objs + k) * 16.
+ *   - eyes[e]: eye e's projection, focal, bg_rgba, out_format and depth_in; its modelview and cutout are ignored.  Both
+ *     eyes have the same width x height (a WebXR projection layer gives both views one viewport size) and the same flags.
+ *   - color_in: NULL, or color_in[e] NULL or eye e's colour target, with the rules of gs_render_scene.
+ *   - out_rgba[e]: eye e's frame (as gs_render_scene's out_rgba).
+ * Each eye's frame is the chain of per-entity draws of gs_render_scene: every entity in its own head-sorted order (quirk
+ * Q5 included), drawn with the eye's matrices over what the previous entity left, depth-tested against the eye's
+ * depth_in.  Each eye's frame is byte-identical to the one-pass gs_render_scene frame of the same order and matrices.
+ * Returns GS_ERR_INVALID, changing nothing, for: unequal eye sizes or flags, GS_RENDER_REUSE_SORT, GS_RENDER_STATS,
+ * GS_RENDER_OUT_TILED or GS_RENDER_OUT_PEER, a sharded context (gs_set_shard world > 1), and what gs_render_scene refuses.
+ * One ticket per stereo frame, in the four pipeline slots shared with every other frame, collected with gs_wait.  Its
+ * gs_stats: n_sorted, n_dropped, min_depth and max_depth of the one sort; n_visible, n_instances, n_instances_kept and
+ * n_tiles summed over both eyes; width and height of one eye; kernel_launches as run.  A stereo frame always takes the
+ * one-pass path (also where gs_render_scene would take the slab path) and leaves no order for GS_RENDER_REUSE_SORT.
+ */
+GS_API int gs_render_scene_stereo_async(gs_context *ctx, const gs_render_params eyes[2], const gs_object *objs,
+                                        const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
+                                        void *const out_rgba[2], uint64_t *out_ticket);
+GS_API int gs_render_scene_stereo(gs_context *ctx, const gs_render_params eyes[2], const gs_object *objs,
+                                  const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
+                                  void *const out_rgba[2], gs_stats *stats);
+
 /* Per-splat projected record of the last gs_render (testing the vertex-shader restatement):
  * 8 floats per resident splat {cx, cy, a1x, a1y, a2x, a2y, rgba8-as-bits, tile-rect-as-bits};
  * rect == 0xFFFFFFFF marks a splat that was not projected/visible. */
