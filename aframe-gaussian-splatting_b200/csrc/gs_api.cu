@@ -191,7 +191,7 @@ static int ensure_tile_stats(gs_context *c, uint32_t n_tiles) {
 }
 
 // buffers of the front-to-back slab path (gs_slab.cu); the pipeline is idle when this runs
-static int ensure_slab(gs_context *c, uint32_t n_tiles, uint32_t n_bins) {
+static int ensure_slab(gs_context *c, uint32_t n_tiles) {
   if (c->slab_cap < c->cap || !c->key32[0]) {
     dev_free(c->key32[0]); dev_free(c->key32[1]); dev_free(c->cidx); dev_free(c->ckey); dev_free(c->chunk_cnt[0]); dev_free(c->chunk_cnt[1]);
     GS_CUDA(c, dev_alloc(&c->key32[0], (size_t)c->cap + 8));
@@ -209,7 +209,9 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles, uint32_t n_bins) {
     dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open);
     GS_CUDA(c, dev_alloc(&c->pix_state, (size_t)n_tiles * 256));
     GS_CUDA(c, dev_alloc(&c->tile_closed, (size_t)n_tiles));
-    GS_CUDA(c, dev_alloc(&c->bin_open, (size_t)n_bins));  // bins <= tiles
+    // sized by tiles, not by this frame's bins: bins never outnumber tiles, but a later frame of another shape can have
+    // more bins without more tiles (192x192: 144 tiles / 4 bins, then 97x289: 133 / 8), and only tiles trigger regrowth
+    GS_CUDA(c, dev_alloc(&c->bin_open, (size_t)n_tiles));
     c->slab_tiles_cap = n_tiles;
   }
   return GS_OK;
@@ -1403,7 +1405,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     if ((rcode = ensure_scratch(c))) return rcode;
     if ((rcode = ensure_bins(c, n_bins_all))) return rcode;
     if ((rcode = ensure_tile_stats(c, n_tiles))) return rcode;
-    if (slab && (rcode = ensure_slab(c, n_tiles, n_bins))) return rcode;
+    if (slab && (rcode = ensure_slab(c, n_tiles))) return rcode;
     if (scene && (rcode = ensure_scene_bufs(c))) return rcode;
     if (stereo && (rcode = ensure_stereo_bufs(c))) return rcode;
     if (c->cap_inst == 0) {
