@@ -190,7 +190,8 @@ static int ensure_tile_stats(gs_context *c, uint32_t n_tiles) {
   return GS_OK;
 }
 
-// buffers of the front-to-back slab path (gs_slab.cu); the pipeline is idle when this runs
+// buffers of the front-to-back slab path (gs_slab.cu); the pipeline is idle when this runs.  n_tiles: the frame's slab tiles
+// (a stereo frame's: both eyes')
 static int ensure_slab(gs_context *c, uint32_t n_tiles) {
   if (c->slab_cap < c->cap || !c->key32[0]) {
     dev_free(c->key32[0]); dev_free(c->key32[1]); dev_free(c->cidx); dev_free(c->ckey); dev_free(c->chunk_cnt[0]); dev_free(c->chunk_cnt[1]);
@@ -206,6 +207,10 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles) {
   for (int i = 0; i < 2; ++i)
     if (!c->slab_tab[i]) GS_CUDA(c, dev_alloc(&c->slab_tab[i], 1));
   if (c->slab_tiles_cap < n_tiles || !c->pix_state) {
+    // the captured slab loops bake these buffers, and a stereo frame grows them to both eyes' tiles while the mono frames'
+    // graph key stays put (and the other way round)
+    drop_graphs(c);
+    drop_stereo_graphs(c);
     dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open);
     GS_CUDA(c, dev_alloc(&c->pix_state, (size_t)n_tiles * 256));
     GS_CUDA(c, dev_alloc(&c->tile_closed, (size_t)n_tiles));
@@ -243,9 +248,14 @@ static void drop_graphs(gs_context *c) {
     }
 }
 
+// the stereo frames' graphs: the three one-pass stages and the slab path's (kind 2)
 static void drop_stereo_graphs(gs_context *c) {
   for (auto &sl : c->slot)
-    for (int i = 0; i < 2; ++i) { kill_graph(sl.graph_xa[i]); kill_graph(sl.graph_xb[i]); kill_graph(sl.graph_xr[i]); }
+    for (int i = 0; i < 2; ++i) {
+      kill_graph(sl.graph_xa[i]); kill_graph(sl.graph_xb[i]); kill_graph(sl.graph_xr[i]);
+      kill_graph(sl.graph_sa[i][2]);
+      for (auto &g : sl.graph_sl[i][2]) kill_graph(g);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -333,9 +343,12 @@ extern "C" int gs_create(int device_ordinal, gs_context **out_ctx) {
   if ((e = cudaMalloc((void **)&c->sort_hdr, sizeof(SortHeader))) != cudaSuccess) return bail("cudaMalloc", e);
   c->use_graphs = getenv("GS_NO_GRAPH") == nullptr;
   // frames expected to sort at least GS_SLAB_MIN splats (default 16 M) are rendered front to back in depth slabs (gs_slab.cu);
-  // GS_SLAB_FIRST = target entry count of the nearest slab (default 1 M, the following ones double)
+  // GS_SLAB_FIRST = target entry count of the nearest slab (default 1 M, the following ones double).  Stereo scene frames
+  // have their own threshold, GS_SLAB_MIN_XR: their one-pass frame already shares the sort between the eyes, while the
+  // projection, binning and raster run twice, so the crossover lies elsewhere
   if (const char *e = getenv("GS_PDL")) c->use_pdl = strcmp(e, "1") == 0;
   if (const char *e = getenv("GS_SLAB_MIN")) c->slab_min = (uint32_t)strtoull(e, nullptr, 10);
+  if (const char *e = getenv("GS_SLAB_MIN_XR")) c->slab_min_xr = (uint32_t)strtoull(e, nullptr, 10);
   if (const char *e = getenv("GS_SLAB_FIRST")) c->slab_first = std::max<uint32_t>(1024u, (uint32_t)strtoull(e, nullptr, 10));
   {  // pixel loop of the raster: two pixels per lane (default) or one (GS_RASTER=scalar); both give identical frames
     const char *rk = getenv("GS_RASTER");
@@ -1011,7 +1024,7 @@ static cudaError_t enqueue_slab_keys_stage(gs_context *c, gs_context::Slot &sl, 
 }
 
 // Stage B+C of a slab frame (raster stream): the slab loop and the resolve.  One chain: every slab depends on the tiles
-// the previous one closed.
+// the previous one closed.  A stereo frame runs it once for both eyes: n_tiles of one eye, n_bins of both.
 static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins,
                                            bool external_events) {
   auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
@@ -1020,25 +1033,27 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
   cudaStream_t st = c->rstream;
   const FrameBufs b = slot_bufs(c, sl);
   const SceneTable *scene = sl.scene ? sl.scene_dev : nullptr;
+  const StereoParams *stereo = sl.stereo ? sl.stereo_dev : nullptr;
+  const FrameParams *fp = slot_fp(sl);  // the frame's (a stereo frame's pair) for the projection, binning and raster
   cudaError_t e;
-  launch_slab_init(c, sl.fp, sl.ctr, st);
+  launch_slab_init(c, fp, sl.ctr, sl.stereo, st);
   if ((e = rec(sl.ev[2], st))) return e;
   for (int s = 0; s < sl.n_slabs; ++s) {
     launch_slab_begin(c, sl.fp, sl.ctr, scene, sl.set, s, st);   // entry count (0 once every bin is closed) + compaction
     launch_slab_sort(c, sl.fp, sl.ctr, scene, b, st);            // draw order of the slab
-    launch_project_entries(c, sl.fp, sl.ctr, scene, b, st);      // vertex shader for the slab's entries
+    launch_project_entries(c, sl.fp, sl.ctr, scene, stereo, b, st);  // vertex shader for the slab's entries (of each eye)
     if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, st))) return e;
-    launch_emit(c, sl.fp, sl.ctr, b, c->bin_open, st);
+    launch_emit(c, fp, sl.ctr, b, c->bin_open, st);
     launch_tile_radix(c, sl.ctr, b, n_bins, st);
     if ((e = rec(sl.slab_ev[s][0], st))) return e;
-    launch_raster_slab(c, sl.fp, sl.ctr, n_tiles, b, (sl.raster_flags & 2u) != 0, st);
+    launch_raster_slab(c, fp, sl.ctr, n_tiles, b, (sl.raster_flags & 2u) != 0, sl.stereo, st);
     if ((e = rec(sl.slab_ev[s][1], st))) return e;
   }
   launch_slab_end(c, sl.ctr, st);
   if ((e = rec(sl.ev[3], st))) return e;
   if (sl.peer) launch_peer_acquire(c, sl.fp, sl.ctr, st);
   if ((e = rec(sl.ev_r0, st))) return e;
-  launch_resolve(c, sl.fp, n_tiles, st);
+  launch_resolve(c, fp, n_tiles, sl.stereo, st);
   if ((e = rec(sl.ev[4], st))) return e;
   if (sl.peer) launch_peer_signal_wait(c, sl.fp, sl.ctr, st);
   return cudaGetLastError();
@@ -1046,15 +1061,18 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
 
 // Front-to-back slab path (gs_slab.cu).  Two stages: A (keys of every splat, O(N), sort stream) and the slab loop
 // (raster stream); stage A of frame k+1 runs under the loop of frame k (keys / slab table are double-buffered by set).
+// A stereo frame passes n_bins of both eyes and keeps its graphs under the stereo key, as on the one-pass path.
 static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
   gs_context::GraphKey k;
   k.cap = c->cap; k.n_tiles = n_tiles; k.n_bins = n_bins; k.cap_inst = c->cap_inst; k.p0 = c->depth; k.p1 = c->inst_rec[0]; k.p2 = c->center_scale;
   k.p3 = c->scene_key;
-  if (memcmp(&k, &c->gkey, sizeof(k)) != 0) {
-    drop_graphs(c);
-    c->gkey = k;
+  gs_context::GraphKey &key = sl.stereo ? c->gkey_stereo : c->gkey;
+  if (memcmp(&k, &key, sizeof(k)) != 0) {
+    if (sl.stereo) drop_stereo_graphs(c);
+    else drop_graphs(c);
+    key = k;
   }
-  const int set = sl.set, kind = sl.scene ? 1 : 0;  // plain and scene frames keep their own graphs
+  const int set = sl.set, kind = sl.stereo ? 2 : (sl.scene ? 1 : 0);  // plain, scene and stereo frames keep their own graphs
   // slabs of slab_first, 2x, 4x ... entries: enough of them to cover every splat the sort considers
   int n_slabs = 1;
   while (n_slabs < kMaxSlabs && slab_cumulative(c->slab_first, n_slabs) < sl.n_sortable) ++n_slabs;
@@ -1085,7 +1103,7 @@ static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_ti
   }
   GS_CUDA(c, cudaEventRecord(sl.ev_binned, c->rstream));
   c->sort_set_free[set] = sl.ev_binned;
-  // scene frames: three radix passes per slab instead of two
+  // scene frames: three radix passes per slab instead of two (stereo frames: the scene frame's launches, both eyes' bins)
   sl.launches = 6u + 1u + (uint32_t)n_slabs * ((n_bins <= 256u ? 16u : 20u) + (sl.scene ? 3u : 0u)) + 2u;
   return GS_OK;
 }
@@ -1238,11 +1256,12 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   // a frame normally takes the buffer set the previous frame did not; a frame that reuses the last sort must read
   // that sort's set, so it runs in it
   sl.set = reuse ? c->last_set : (c->last_set ^ 1);
+  // a stereo frame bins both eyes (ids eye * n_bins + bin) and rasters both eyes' tiles in one grid, on either path
+  const uint32_t n_bins_all = sl.stereo ? 2 * rc.n_bins : rc.n_bins;
   if (sl.slab) {
-    if ((rcode = launch_frame_slabs(c, sl, rc.n_tiles, rc.n_bins))) return rcode;
+    if ((rcode = launch_frame_slabs(c, sl, rc.n_tiles, n_bins_all))) return rcode;
   } else {
-    // a stereo frame bins both eyes (ids eye * n_bins + bin) and rasters both eyes' tiles in one grid
-    if ((rcode = launch_frame(c, sl, reuse, rc.n_tiles, sl.stereo ? 2 * rc.n_bins : rc.n_bins))) return rcode;
+    if ((rcode = launch_frame(c, sl, reuse, rc.n_tiles, n_bins_all))) return rcode;
   }
   if ((rcode = enqueue_readback(c, sl))) return rcode;
   c->last_set = sl.set;
@@ -1376,7 +1395,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   }
   if (!scene && (p->flags & GS_RENDER_REUSE_SORT) && c->have_order && (rcode = drain(c))) return rcode;  // runs in the last sort's buffers
   if ((p->flags & GS_RENDER_STATS) && (rcode = drain(c))) return rcode;  // the per-tile statistics buffer is not double-buffered
-  // large scenes render front to back in depth slabs, plain and scene frames alike; the one-pass and slab paths share
+  // large scenes render front to back in depth slabs, plain, scene and stereo frames alike; the one-pass and slab paths share
   // scratch buffers, so a change drains (the criterion is the number of SORTED splats: the last frame's count when there
   // is one, else the splats the sort considers - the resident ones, or those in the scene's entity ranges)
   uint32_t sortable = c->n;
@@ -1385,8 +1404,9 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     for (uint32_t k = 0; k < scene->n; ++k) sortable += scene->obj[k].end - scene->obj[k].first;
   }
   const uint32_t expect_sorted = c->have_last_sorted ? c->last_sorted : sortable;
-  // (a stereo frame always takes the one-pass path)
-  const bool slab = !stereo && expect_sorted >= c->slab_min && !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS));
+  // stereo frames by their own threshold (GS_SLAB_MIN_XR); they accept neither flag
+  const bool slab = expect_sorted >= (stereo ? c->slab_min_xr : c->slab_min) && !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS));
+  const uint32_t slab_tiles = stereo ? 2 * n_tiles : n_tiles;  // pixel state of both eyes
   if ((int)slab != c->last_mode) {
     if ((rcode = drain(c))) return rcode;
     GS_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1395,7 +1415,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     c->last_mode = (int)slab;
   }
   // growing any shared buffer needs an idle pipeline
-  const bool grow = (slab && (c->slab_cap < c->cap || !c->key32[0] || c->slab_tiles_cap < n_tiles || !c->slab_tab[1])) || !(c->scratch_cap >= c->cap && c->depth) || !(n_bins_all <= c->bins_cap && c->bin_range[0]) || !(n_tiles <= c->tile_stats_cap && c->tile_stats) || c->cap_inst == 0 ||
+  const bool grow = (slab && (c->slab_cap < c->cap || !c->key32[0] || c->slab_tiles_cap < slab_tiles || !c->slab_tab[1])) || !(c->scratch_cap >= c->cap && c->depth) || !(n_bins_all <= c->bins_cap && c->bin_range[0]) || !(n_tiles <= c->tile_stats_cap && c->tile_stats) || c->cap_inst == 0 ||
                     (scene && !(c->scene_cap >= c->cap && c->scene_key)) || (stereo && !(c->stereo_cap >= c->cap && c->proj_rec1[0]));
   if (grow) {
     if ((rcode = drain(c))) return rcode;
@@ -1405,7 +1425,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     if ((rcode = ensure_scratch(c))) return rcode;
     if ((rcode = ensure_bins(c, n_bins_all))) return rcode;
     if ((rcode = ensure_tile_stats(c, n_tiles))) return rcode;
-    if (slab && (rcode = ensure_slab(c, n_tiles))) return rcode;
+    if (slab && (rcode = ensure_slab(c, slab_tiles))) return rcode;
     if (scene && (rcode = ensure_scene_bufs(c))) return rcode;
     if (stereo && (rcode = ensure_stereo_bufs(c))) return rcode;
     if (c->cap_inst == 0) {

@@ -255,11 +255,13 @@ struct gs_context {
   uint32_t *chunk_cnt[2] = {nullptr, nullptr};  // [kMaxSlabs][chunk_row] per-slab compaction offsets of every 2048-splat chunk (one per set)
   uint32_t chunk_row = 0;          // row stride of chunk_cnt: cap / 2048 + 4
   gs::SlabTable *slab_tab[2] = {nullptr, nullptr};
-  float4 *pix_state = nullptr;     // [tiles * 256] {R, G, B, T} carried from slab to slab
+  float4 *pix_state = nullptr;     // [tiles * 256] {R, G, B, T} carried from slab to slab (stereo frames: both eyes' tiles)
   uint8_t *tile_closed = nullptr;  // [tiles]
   uint32_t *bin_open = nullptr;    // [bins] live tiles per bin (0 for bins of other ranks)
   uint32_t slab_tiles_cap = 0;
   uint32_t slab_min = 16u << 20;   // frames expected to SORT at least this many splats render front to back in slabs
+  uint32_t slab_min_xr = 8u << 20;  // ... stereo scene frames (their one-pass frame already shares its sort by the eyes;
+                                    // README, tools/xr_slab_bench.py: on an H100 the crossover lies between 4.9 and 9.7 M)
   uint32_t last_sorted = 0;        // V of the most recently completed frame (predicts the next frame's)
   bool have_last_sorted = false;
   uint32_t slab_first = 1u << 20;  // target entry count of the nearest slab (the following ones double)
@@ -324,9 +326,11 @@ struct gs_context {
     cudaGraphExec_t graph_b[2] = {nullptr, nullptr};                           // binning, [set]
     cudaGraphExec_t graph_r[2] = {nullptr, nullptr};                           // raster, [set]
     cudaGraphExec_t graph_rp[2] = {nullptr, nullptr};                          // acquire + raster + signal/wait (fused exchange)
-    cudaGraphExec_t graph_sa[2][2] = {};       // slab path: keys stage, [set][plain | scene frame]
-    cudaGraphExec_t graph_sl[2][2][3] = {};    // slab path: slab loop + resolve, [set][plain | scene frame][plain | depth | peer]
-    int graph_slabs[2][2] = {};                // slab count baked into graph_sa / graph_sl, [set][plain | scene frame]
+    // slab path, [set][plain | scene | stereo scene frame]: keys stage, slab loop + resolve ([plain | depth | peer]), and the
+    // slab count baked into both
+    cudaGraphExec_t graph_sa[2][3] = {};
+    cudaGraphExec_t graph_sl[2][3][3] = {};
+    int graph_slabs[2][3] = {};
     cudaGraphExec_t graph_xa[2] = {}, graph_xb[2] = {}, graph_xr[2] = {};  // stereo scene frames: the three stages, [set]
     bool peer = false;
     uint64_t ticket = 0;
@@ -458,19 +462,22 @@ void launch_peer_release(gs_context *c, const PeerRows &rows, uint32_t world, ui
 void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const ObjCounters *octr, int set,
                  cudaStream_t st);  // keys + bucket histogram
 void launch_slab_plan(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, uint32_t first_target, int n_slabs, cudaStream_t st);
-void launch_slab_init(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
+// stereo: both eyes' pixel state, closed flags and bins (fp = &stereo->eye[0])
+void launch_slab_init(gs_context *c, const FrameParams *fp, FrameCounters *ctr, bool stereo, cudaStream_t st);
 void launch_compact_offsets(gs_context *c, const FrameParams *fp, const SceneTable *scene, int set, int n_slabs,
                             cudaStream_t st);  // every slab's chunk offsets: 2 launches
 void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, int set, int slab,
                        cudaStream_t st);  // + compaction: 2 launches
 void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
                       cudaStream_t st);  // 6 launches (scene frames: 9)
-void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
-                            cudaStream_t st);
+// stereo: the slot's stereo table of a stereo scene frame (both eyes into b.proj_rec / rect and b.proj_rec1 / rect1)
+void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene,
+                            const StereoParams *stereo, const FrameBufs &b, cudaStream_t st);
 void launch_slab_end(gs_context *c, FrameCounters *ctr, cudaStream_t st);
+// stereo: one grid of 2 * n_tiles CTAs over both eyes (fp = &stereo->eye[0]); likewise the resolve
 void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, uint32_t n_tiles, const FrameBufs &b, bool depth,
-                        cudaStream_t st);
-void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, cudaStream_t st);
+                        bool stereo, cudaStream_t st);
+void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, bool stereo, cudaStream_t st);
 void launch_assemble(gs_context *c, const void *gathered, uint32_t tiles_per_rank, uint32_t world, uint32_t width,
                      uint32_t height, int32_t format, void *out_frame);
 

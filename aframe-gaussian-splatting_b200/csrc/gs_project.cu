@@ -10,7 +10,8 @@
 //   k_emit_entries: one thread per draw-order entry writes its (bin, splat) instances at the entry's offset,
 //                in draw order, so that a STABLE sort by bin id alone reproduces the reference's back-to-front order
 //                inside every bin; rectangles of more than 8 bins are finished by the whole warp.  Stereo scene frames:
-//                each entry emits eye 0's instances, then eye 1's, with bin ids eye * n_bins + bin.
+//                each entry emits eye 0's instances, then eye 1's, with bin ids eye * n_bins + bin (on the slab path too,
+//                each eye's closed bins skipped).
 #include "gs_common.cuh"
 
 namespace gs {
@@ -152,8 +153,8 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
 // instead of warps with a few live lanes each.
 // SCENE (scene frames, by index or, on the slab path, by entry): every splat takes its entity's modelview; by index, the
 // splat the Q5 tail may repeat is each entity's first one.
-// STEREO (stereo scene frames, by index): fp = &stereo->eye[0]; every splat is projected for both eyes with each eye's
-// RenderConsts and its entity's per-eye modelview, eye 1 into rec_out1 / rect_out1.
+// STEREO (stereo scene frames, by index or, on the slab path, by entry): fp = &stereo->eye[0]; every splat is projected
+// for both eyes with each eye's RenderConsts and its entity's per-eye modelview, eye 1 into rec_out1 / rect_out1.
 template <bool BY_ENTRY, bool SCENE = false, bool STEREO = false>
 __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, const uint4 *__restrict__ cc,
                                                  const float *__restrict__ depth,
@@ -163,7 +164,7 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
                                                  const SceneTable *__restrict__ scene,
                                                  const StereoParams *__restrict__ stereo, float4 *__restrict__ rec_out1,
                                                  uint32_t *__restrict__ rect_out1) {
-  static_assert(!STEREO || (SCENE && !BY_ENTRY), "stereo frames are scene frames projected by index");
+  static_assert(!STEREO || SCENE, "stereo frames are scene frames");
   GS_PDL_ENTRY();
   const RenderConsts &rc = fp->rc;
   const uint32_t n = BY_ENTRY ? ctr->sort.n_valid : fp->n_splats;
@@ -291,7 +292,8 @@ __device__ __forceinline__ uint32_t rect_count(uint32_t r, uint32_t rank, uint32
 // SLAB: rect is indexed by entry (k_project<true>), the entry's payload is j itself, and entries whose (small)
 // rectangle holds only closed bins own nothing any more.
 // STEREO (stereo scene frames, one GPU): an entry owns its eye-0 instances, then its eye-1 instances (rect1); it stays
-// live when either eye sees it.
+// live when either eye sees it.  On the slab path each eye's rectangle is tested against that eye's bins (eye 1's from
+// n_bins on); an eye whose rectangle lost its instances gives kNoRect to the emit walk (ent for eye 0, rect1 for eye 1).
 template <bool SLAB, bool STEREO = false>
 __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restrict__ order,
                                                         const uint32_t *__restrict__ rect,
@@ -300,7 +302,7 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
                                                         uint32_t *__restrict__ slice_prefix, FrameCounters *ctr,
                                                         const FrameParams *__restrict__ fp,
                                                         const uint32_t *__restrict__ bin_open,
-                                                        const uint32_t *__restrict__ rect1) {
+                                                        uint32_t *__restrict__ rect1) {
   GS_PDL_ENTRY();
   const uint32_t shard_rank = fp->rc.shard_rank, shard_world = fp->rc.shard_world;
   __shared__ uint32_t s_warp[kEmitThreads / 32], s_vis[kEmitThreads / 32];
@@ -314,19 +316,29 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
     if (j < nv) {
       idx = SLAB ? j : __ldg(order + j);
       r = __ldg(rect + idx);
-      if (STEREO) r1 = __ldg(rect1 + idx);
+      if (STEREO) r1 = SLAB ? rect1[idx] : __ldg(rect1 + idx);  // (the slab path may rewrite it below)
     }
+    // a small rectangle whose bins (from bin_base on) are all closed owns nothing; bins of other ranks count as closed
+    // (k_slab_init)
+    auto all_closed = [&](uint32_t rr, uint32_t bin_base) -> bool {
+      const uint32_t bx0 = rr & 255u, bx1 = (rr >> 8) & 255u, by0 = (rr >> 16) & 255u, by1 = rr >> 24;
+      if ((bx1 - bx0 + 1u) * (by1 - by0 + 1u) > 4u) return false;
+      bool any = false;
+      for (uint32_t by = by0; by <= by1; ++by)
+        for (uint32_t bx = bx0; bx <= bx1; ++bx) any = any || (__ldg(bin_open + bin_base + by * fp->rc.bins_x + bx) != 0u);
+      return !any;
+    };
     uint32_t cnt = rect_count(r, shard_rank, shard_world);
-    if (SLAB && cnt) {
-      const uint32_t bx0 = r & 255u, bx1 = (r >> 8) & 255u, by0 = (r >> 16) & 255u, by1 = r >> 24;
-      if ((bx1 - bx0 + 1u) * (by1 - by0 + 1u) <= 4u) {  // bins of other ranks count as closed (k_slab_init)
-        bool any = false;
-        for (uint32_t by = by0; by <= by1; ++by)
-          for (uint32_t bx = bx0; bx <= bx1; ++bx) any = any || (__ldg(bin_open + by * fp->rc.bins_x + bx) != 0u);
-        if (!any) cnt = 0;
+    if (SLAB && cnt && all_closed(r, 0u)) cnt = 0;
+    const uint32_t cnt0 = cnt;  // eye 0's instances
+    if (STEREO) {
+      uint32_t cnt1 = rect_count(r1, 0u, 1u);
+      if (SLAB && cnt1 && all_closed(r1, fp->rc.n_bins)) {
+        cnt1 = 0;
+        rect1[idx] = kNoRect;
       }
+      cnt += cnt1;
     }
-    if (STEREO) cnt += rect_count(r1, 0u, 1u);
     uint32_t incl = cnt, vis = (r != kNoRect) + (STEREO && r1 != kNoRect);
     for (int o = 1; o < 32; o <<= 1) {
       const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
@@ -343,7 +355,7 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
       v += s_vis[k];
     }
     if (j < nv) {
-      ent[j] = make_uint2(idx, cnt ? r : kNoRect);  // entries owning no tile are skipped by the emit walk
+      ent[j] = make_uint2(idx, (SLAB && STEREO ? cnt0 : cnt) ? r : kNoRect);  // entries owning no tile are skipped by the emit walk
       ent_off[j] = wbase + incl - cnt;
     }
     if (tid == 0) {
@@ -524,13 +536,20 @@ void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable
                (float4 *)nullptr, (uint32_t *)nullptr);
 }
 
-// scene: the slot's scene table for a scene frame (every entry takes its entity's modelview), NULL for a plain frame
-void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
-                            cudaStream_t stream) {
+// scene: the slot's scene table for a scene frame (every entry takes its entity's modelview), NULL for a plain frame;
+// stereo: the slot's stereo table of a stereo scene frame (both eyes, fp ignored), NULL otherwise
+void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene,
+                            const StereoParams *stereo, const FrameBufs &b, cudaStream_t stream) {
   uint64_t blocks = ((uint64_t)c->cap + 255) / 256;
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
+  if (stereo) {
+    launch_chain(c, k_project<true, true, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale,
+                 (const uint4 *)c->cov_color, (const float *)c->depth, &stereo->eye[0], b.proj_rec, b.rect,
+                 (const uint32_t *)b.order, (const FrameCounters *)ctr, scene, stereo, b.proj_rec1, b.rect1);
+    return;
+  }
   launch_chain(c, scene ? k_project<true, true> : k_project<true>, (int)blocks, 256, stream, (const float4 *)c->center_scale,
                (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)b.order,
                (const FrameCounters *)ctr, scene, (const StereoParams *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr);
@@ -543,9 +562,9 @@ void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const
   if (tiles > cap) tiles = cap;
   if (tiles < 1) tiles = 1;
   const bool stereo = b.rect1 != nullptr;
-  launch_chain(c, bin_open ? k_count<true> : (stereo ? k_count<false, true> : k_count<false>), (int)tiles, kEmitThreads, st,
-               (const uint32_t *)b.order, (const uint32_t *)b.rect, c->ent, c->ent_off, c->slice_total, c->slice_prefix, ctr, fp, bin_open,
-               (const uint32_t *)b.rect1);
+  auto count = bin_open ? (stereo ? k_count<true, true> : k_count<true>) : (stereo ? k_count<false, true> : k_count<false>);
+  launch_chain(c, count, (int)tiles, kEmitThreads, st, (const uint32_t *)b.order, (const uint32_t *)b.rect, c->ent, c->ent_off,
+               c->slice_total, c->slice_prefix, ctr, fp, bin_open, b.rect1);
   launch_chain(c, stereo ? k_emit_entries<true> : k_emit_entries<false>, (int)tiles, 256, st, (const uint2 *)c->ent, (const uint32_t *)c->ent_off,
                (const uint32_t *)c->slice_prefix, (const float4 *)b.proj_rec, fp, (uint64_t)c->cap_inst, c->inst_tile, c->inst_idx, ctr,
                bin_open, (const float4 *)b.proj_rec1, (const uint32_t *)b.rect1);

@@ -169,13 +169,14 @@ struct SlabIO {
 // SLAB: one depth slab of a frame: start from / store back the pixel state, close saturated tiles; k_resolve writes the frame.
 // STEREO: both eyes of a stereo scene frame, 2 * n_tiles CTAs: CTA b draws tile b % n_tiles of eye b / n_tiles, with that
 // eye's frame fp[eye] (output, colour target, depth target: an eye without one keeps the depth 1, which passes every
-// fragment the projection keeps) and bins from eye * n_bins on.  The pixel loop is the one of the plain frame.
+// fragment the projection keeps) and bins from eye * n_bins on.  The pixel loop is the one of the plain frame.  With SLAB,
+// the pixel state and closed flag of eye e's tile t are those of slab tile e * n_tiles + t (the CTA's index).
 template <bool PACKED, bool DEPTH, bool STATS, bool SLAB = false, bool STEREO = false>
 __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>::kMinBlocks) k_raster(const float4 *__restrict__ inst_rec,
                                                                         const uint2 *__restrict__ bin_range,
                                                                         const FrameParams *__restrict__ fp,
                                                                         uint4 *__restrict__ tile_stats, SlabIO slab) {
-  static_assert(!STEREO || (!STATS && !SLAB), "stereo frames take the one-pass path without statistics");
+  static_assert(!STEREO || !STATS, "stereo frames take no statistics");
   using Cfg = RasterCfg<PACKED>;
   constexpr int kThreads = Cfg::kThreads, kChunk = Cfg::kChunk, kStages = Cfg::kStages, kCv = Cfg::kCv;
   constexpr int kWarps = kThreads / 32;
@@ -189,6 +190,7 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   __shared__ uint32_t s_stat[4];
 
   const uint32_t tile = blockIdx.x - eye * rc.n_tiles;
+  const uint32_t stile = blockIdx.x;  // slab state index: the tile of a mono frame, eye * n_tiles + tile of a stereo one
   const uint32_t tx = tile % rc.tiles_x, ty = tile / rc.tiles_x;
   const uint32_t bcol = tx / kTilesPerBin;
   if (rc.shard_world > 1 && (bcol % rc.shard_world) != rc.shard_rank) return;
@@ -222,7 +224,7 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   const uint32_t start = range.x, end = range.y;
   const uint32_t count = end - start;
   const uint32_t n_chunks = (count + kChunk - 1) / kChunk;
-  if (SLAB && (count == 0 || slab.closed[tile])) return;  // nothing of this slab reaches the tile / the tile is saturated
+  if (SLAB && (count == 0 || slab.closed[stile])) return;  // nothing of this slab reaches the tile / the tile is saturated
 
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) mbar_init(&s_full[s], 1);
@@ -250,9 +252,9 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   float2 T2 = make_float2(1.0f, 1.0f), R2 = make_float2(0.f, 0.f), G2 = R2, B2 = R2;
   float lim0 = inside0 ? 4.0f : -1.0f, lim1 = inside1 ? 4.0f : -1.0f;
   if (SLAB) {  // continue where the nearer slabs left this tile
-    const float4 s0 = slab.state[(size_t)tile * 256 + ly * 16 + lx];
+    const float4 s0 = slab.state[(size_t)stile * 256 + ly * 16 + lx];
     if (PACKED) {
-      const float4 s1 = slab.state[(size_t)tile * 256 + (ly + 1) * 16 + lx];
+      const float4 s1 = slab.state[(size_t)stile * 256 + (ly + 1) * 16 + lx];
       R2 = make_float2(s0.x, s1.x); G2 = make_float2(s0.y, s1.y); B2 = make_float2(s0.z, s1.z); T2 = make_float2(s0.w, s1.w);
       lim0 = (inside0 && T2.x >= kTStop) ? 4.0f : -1.0f;
       lim1 = (inside1 && T2.y >= kTStop) ? 4.0f : -1.0f;
@@ -387,14 +389,14 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
 
   if (SLAB) {
     if (PACKED) {
-      slab.state[(size_t)tile * 256 + ly * 16 + lx] = make_float4(R2.x, G2.x, B2.x, T2.x);
-      slab.state[(size_t)tile * 256 + (ly + 1) * 16 + lx] = make_float4(R2.y, G2.y, B2.y, T2.y);
+      slab.state[(size_t)stile * 256 + ly * 16 + lx] = make_float4(R2.x, G2.x, B2.x, T2.x);
+      slab.state[(size_t)stile * 256 + (ly + 1) * 16 + lx] = make_float4(R2.y, G2.y, B2.y, T2.y);
     } else {
-      slab.state[(size_t)tile * 256 + ly * 16 + lx] = make_float4(R0, G0, B0, T0);
+      slab.state[(size_t)stile * 256 + ly * 16 + lx] = make_float4(R0, G0, B0, T0);
     }
     const int alive_end = __syncthreads_or((lim0 > 0.0f) || (lim1 > 0.0f));
     if (!alive_end && tid == 0) {  // saturated: later slabs skip the tile, and the bin once all its tiles are closed
-      slab.closed[tile] = 1;
+      slab.closed[stile] = 1;
       if (atomicSub(&slab.bin_open[bin], 1u) == 1u) atomicSub(&slab.ctr->open_bins, 1u);
     }
   } else if (PACKED) {
@@ -502,30 +504,40 @@ void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles
   }
 }
 
-// one slab of a frame (always the packed pixel loop)
+// one slab of a frame (always the packed pixel loop); stereo: both eyes' tiles in one grid, eye e's frame at fp + e
 void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, uint32_t n_tiles, const FrameBufs &b, bool depth,
-                        cudaStream_t st) {
+                        bool stereo, cudaStream_t st) {
   const SlabIO io{c->pix_state, c->tile_closed, c->bin_open, ctr};
-  if (depth)
-    k_raster<true, true, false, true><<<n_tiles, RasterCfg<true>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
+  constexpr int kT = RasterCfg<true>::kThreads;
+  if (stereo && depth)
+    k_raster<true, true, false, true, true><<<2 * n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
+  else if (stereo)
+    k_raster<true, false, false, true, true><<<2 * n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
+  else if (depth)
+    k_raster<true, true, false, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
   else
-    k_raster<true, false, false, true><<<n_tiles, RasterCfg<true>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
+    k_raster<true, false, false, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
 }
 
-// slab path epilogue: pixel state -> frame (composite over the clear colour or colour target; plain / tiled / peer destinations)
+// slab path epilogue: pixel state -> frame (composite over the clear colour or colour target; plain / tiled / peer destinations).
+// STEREO: 2 * n_tiles CTAs, CTA b resolves slab tile b into tile b % n_tiles of eye b / n_tiles, with that eye's frame fp[eye]
+template <bool STEREO>
 __global__ void __launch_bounds__(256) k_resolve(const float4 *__restrict__ state, const FrameParams *__restrict__ fp) {
+  const uint32_t eye = STEREO ? (blockIdx.x >= fp->rc.n_tiles ? 1u : 0u) : 0u;
+  if (STEREO) fp += eye;
   const RenderConsts &rc = fp->rc;
-  const uint32_t tile = blockIdx.x;
+  const uint32_t tile = blockIdx.x - eye * rc.n_tiles;
   const uint32_t tx = tile % rc.tiles_x, ty = tile / rc.tiles_x;
   if (rc.shard_world > 1 && ((tx / kTilesPerBin) % rc.shard_world) != rc.shard_rank) return;
   const uint32_t lx = threadIdx.x & 15u, ly = threadIdx.x >> 4;
   const uint32_t x = tx * kTile + lx, y = ty * kTile + ly;
-  const float4 s = state[(size_t)tile * 256 + threadIdx.x];
+  const float4 s = state[(size_t)blockIdx.x * 256 + threadIdx.x];
   store_pixel(fp, tile, tx, ty, lx, ly, x, y, (x < rc.width) && (y < rc.height), s.w, s.x, s.y, s.z);
 }
 
-void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, cudaStream_t st) {
-  k_resolve<<<n_tiles, 256, 0, st>>>(c->pix_state, fp);
+void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, bool stereo, cudaStream_t st) {
+  if (stereo) k_resolve<true><<<2 * n_tiles, 256, 0, st>>>(c->pix_state, fp);
+  else k_resolve<false><<<n_tiles, 256, 0, st>>>(c->pix_state, fp);
 }
 
 void launch_peer_acquire(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st) {

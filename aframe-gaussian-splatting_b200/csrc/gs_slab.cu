@@ -31,6 +31,12 @@
 // entries with key17 = 65536 (its top bucket), compacted and sorted like the others; the pass SM1 turns each into a draw
 // of the entity's first splat.  The per-slab sort is SM1, M2, M3 over the compacted 24-bit keys, and the projection
 // takes each entry's entity modelview (k_project<true, true>).
+//
+// Stereo scene frames (gs_render_scene_stereo) cut their slabs from the HEAD camera's scene order, which is both eyes'
+// draw order: stage A, the plan and the compaction offsets are those of the scene frame, shared by the eyes.  Per slab the
+// projection covers both eyes (k_project<true, true, true>), the bin instances of both eyes go into one id space (eye *
+// n_bins + bin, each eye's closed bins skipped) and one raster grid draws both eyes' tiles (eye * n_tiles + tile), each
+// continuing from its own pixel state; the loop stops when neither eye has an open bin.
 #include <type_traits>
 
 #include "gs_common.cuh"
@@ -175,17 +181,21 @@ __global__ void __launch_bounds__(1024) k_slab_plan(SlabTable *tab, FrameCounter
   }
 }
 
-// per-pixel state, closed flags, live tiles per bin
+// per-pixel state, closed flags, live tiles per bin.  STEREO (stereo scene frames, fp = &stereo->eye[0]): both eyes',
+// tiles eye * n_tiles + tile and bins eye * n_bins + bin (the eyes share the viewport size); open_bins counts both eyes
+template <bool STEREO>
 __global__ void __launch_bounds__(256) k_slab_init(const FrameParams *__restrict__ fp, FrameCounters *ctr,
                                                    float4 *__restrict__ pix_state, uint8_t *__restrict__ tile_closed,
                                                    uint32_t *__restrict__ bin_open) {
   const RenderConsts &rc = fp->rc;
+  const uint32_t eyes = STEREO ? 2u : 1u;
   const uint32_t stride = gridDim.x * blockDim.x, g = blockIdx.x * blockDim.x + threadIdx.x;
-  for (uint32_t i = g; i < rc.n_tiles * 256u; i += stride) pix_state[i] = make_float4(0.f, 0.f, 0.f, 1.f);
-  for (uint32_t i = g; i < rc.n_tiles; i += stride) tile_closed[i] = 0;
+  for (uint32_t i = g; i < eyes * rc.n_tiles * 256u; i += stride) pix_state[i] = make_float4(0.f, 0.f, 0.f, 1.f);
+  for (uint32_t i = g; i < eyes * rc.n_tiles; i += stride) tile_closed[i] = 0;
   uint32_t mine = 0;
-  for (uint32_t b = g; b < rc.n_bins; b += stride) {
-    const uint32_t bx = b % rc.bins_x, by = b / rc.bins_x;
+  for (uint32_t b = g; b < eyes * rc.n_bins; b += stride) {
+    const uint32_t eb = STEREO ? b % rc.n_bins : b;  // the bin inside its eye
+    const uint32_t bx = eb % rc.bins_x, by = eb / rc.bins_x;
     const bool owned = rc.shard_world <= 1 || (bx % rc.shard_world) == rc.shard_rank;
     const uint32_t tw = min((uint32_t)kTilesPerBin, rc.tiles_x - bx * kTilesPerBin);
     const uint32_t th = min((uint32_t)kTilesPerBin, rc.tiles_y - by * kTilesPerBin);
@@ -401,9 +411,9 @@ void launch_slab_plan(gs_context *c, const FrameParams *fp, FrameCounters *ctr, 
 }
 
 // pixel state / closed flags are shared by all frames: reset at the start of a frame's slab loop (raster stream)
-void launch_slab_init(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st) {
-  k_slab_init<<<grid_for(c, (uint64_t)c->slab_tiles_cap * 256, 256 * 4, 8), 256, 0, st>>>(fp, ctr, c->pix_state, c->tile_closed,
-                                                                                           c->bin_open);
+void launch_slab_init(gs_context *c, const FrameParams *fp, FrameCounters *ctr, bool stereo, cudaStream_t st) {
+  (stereo ? k_slab_init<true> : k_slab_init<false>)<<<grid_for(c, (uint64_t)c->slab_tiles_cap * 256, 256 * 4, 8), 256, 0, st>>>(
+      fp, ctr, c->pix_state, c->tile_closed, c->bin_open);
 }
 
 // stage A, after the plan: chunk offsets of every scheduled slab (the loop's k_compact_write reads row `slab`)

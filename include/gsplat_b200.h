@@ -335,8 +335,14 @@ GS_API int gs_sort_scene(gs_context *ctx, const gs_object *objs, uint32_t n_objs
  * GS_RENDER_OUT_TILED or GS_RENDER_OUT_PEER, a sharded context (gs_set_shard world > 1), and what gs_render_scene refuses.
  * One ticket per stereo frame, in the four pipeline slots shared with every other frame, collected with gs_wait.  Its
  * gs_stats: n_sorted, n_dropped, min_depth and max_depth of the one sort; n_visible, n_instances, n_instances_kept and
- * n_tiles summed over both eyes; width and height of one eye; kernel_launches as run.  A stereo frame always takes the
- * one-pass path (also where gs_render_scene would take the slab path) and leaves no order for GS_RENDER_REUSE_SORT.
+ * n_tiles summed over both eyes; width and height of one eye; kernel_launches as run.  A stereo frame expected to sort at
+ * least GS_SLAB_MIN_XR entries (default 8 M; the previous frame's sorted count, or before any frame the splats in its
+ * entities' ranges) is rendered front to back in depth slabs of the head sort's order, once for both eyes: each slab is
+ * projected, binned and rasterised for both eyes, each eye skipping its own saturated tiles, and the loop ends when neither
+ * eye has a tile left to draw.  Each eye's frame is byte-identical to the one-pass stereo frame; n_slabs, n_slabs_run and
+ * n_slab_entries then describe the one slab plan of the pair.  GS_SLAB_MIN_XR is its own threshold, apart from
+ * GS_SLAB_MIN: the one-pass stereo frame already shares its sort between the eyes.  A stereo frame leaves no order for
+ * GS_RENDER_REUSE_SORT.
  */
 GS_API int gs_render_scene_stereo_async(gs_context *ctx, const gs_render_params eyes[2], const gs_object *objs,
                                         const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
