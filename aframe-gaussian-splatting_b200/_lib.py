@@ -13,6 +13,7 @@ GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F = 0, 1
 GS_RENDER_OUT_DEVICE, GS_RENDER_REUSE_SORT, GS_RENDER_OUT_TILED, GS_RENDER_OUT_PEER = 1, 2, 4, 8
 GS_RENDER_STATS, GS_RENDER_DEPTH_DEVICE, GS_RENDER_COLOR_DEVICE = 16, 32, 64
 GS_MAX_OBJECTS = 64
+GS_TARGET_DEVICE = 1
 
 
 class GsStats(C.Structure):
@@ -48,6 +49,13 @@ class GsObject(C.Structure):
     ]
 
 
+class GsTarget(C.Structure):
+    """gs_target: the framebuffer a target frame is blended into in place (colour, optional depth, pitch x rows)."""
+    _fields_ = [
+        ("color", C.c_void_p), ("depth", C.c_void_p), ("pitch", C.c_uint32), ("rows", C.c_uint32), ("flags", C.c_uint32),
+    ]
+
+
 # every symbol include/gsplat_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -80,6 +88,15 @@ SYMBOLS = {
                                                C.c_uint32, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_uint64)]),
     "gs_render_scene_stereo": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.POINTER(C.c_float), C.c_uint32,
                                          C.POINTER(_P), C.POINTER(_P), C.POINTER(GsStats)]),
+    "gs_render_scene_target_async": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.c_uint32,
+                                               C.POINTER(GsTarget), C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64)]),
+    "gs_render_scene_target": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.c_uint32, C.POINTER(GsTarget),
+                                         C.c_uint32, C.c_uint32, C.POINTER(GsStats)]),
+    "gs_render_scene_stereo_target_async": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.POINTER(C.c_float),
+                                                      C.c_uint32, C.POINTER(GsTarget), C.POINTER(C.c_uint32),
+                                                      C.POINTER(C.c_uint64)]),
+    "gs_render_scene_stereo_target": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.POINTER(C.c_float),
+                                                C.c_uint32, C.POINTER(GsTarget), C.POINTER(C.c_uint32), C.POINTER(GsStats)]),
     "gs_read_projected": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
     "gs_get_stats": (C.c_int, [_P, C.POINTER(GsStats)]),
     "gs_set_shard": (C.c_int, [_P, C.c_uint32, C.c_uint32]),

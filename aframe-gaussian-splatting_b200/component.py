@@ -374,18 +374,25 @@ class SplatScene:
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out)
 
-    def render_xr(self, eye_cameras, width: int, height: int, color_in=(None, None), depth_in=(None, None),
-                  bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8):
-        """WebXR presentation of every entity (index.js:13-15, 184-195, 438-455): one stereo frame
-        (gs_render_scene_stereo).  Each entity's sort comes from its getModelViewMatrix() of the scene camera - the head
-        pose its tick() uses - and each entity is drawn once per eye camera with that eye's matrices.
-        Eye viewport: the XR layer's native eye size (width x height) scaled by xrPixelRatio and floored, as
-        GaussianSplattingComponent.render_xr does.  The ratio is the FIRST entity's xrPixelRatio (1 when it is not
-        positive), by the rule of render(), whose shared viewport is the first entity's.
-        color_in[e] / depth_in[e]: eye e's colour ((h, w, 4) of the output dtype) and window-space depth ((h, w) f32) at
-        the scaled size, or None.  Returns [left, right] frames, row 0 = bottom."""
+    def render_into(self, color: np.ndarray, depth: Optional[np.ndarray] = None, viewport=(0, 0), width: Optional[int] = None,
+                    height: Optional[int] = None, camera=None, fmt: int = GS_FORMAT_RGBA8) -> np.ndarray:
+        """Draw every entity IN PLACE into the caller's framebuffer at a viewport rectangle, as the reference's draw does
+        with the bound render target and renderer.setViewport (index.js:177-195).  color: (rows, pitch, 4) of the output
+        dtype, row 0 = bottom; depth: (rows, pitch) f32 window-space depth or None.  viewport = (x, y) or (x, y, w, h) in
+        CSS pixels: w x h (default: width x height, else the rest of the buffer) scaled by the first entity's pixelRatio
+        and floored, as render() sizes its frame.  Returns `color`."""
         if not self.entities:
-            raise ValueError("SplatScene.render_xr: no entity added")
+            raise ValueError("SplatScene.render_into: no entity added")
+        x, y = int(viewport[0]), int(viewport[1])
+        if len(viewport) == 4:
+            width, height = viewport[2], viewport[3]
+        width = color.shape[1] - x if width is None else width
+        height = color.shape[0] - y if height is None else height
+        frame, objs = self.objects(width, height, camera)
+        return self.renderer.render_scene_target(frame, objs, color, depth, viewport=(x, y), fmt=fmt)
+
+    def _xr_objects(self, eye_cameras, width: int, height: int):
+        """(eye size, objects with head matrices, eye FrameInputs, per-eye entity modelviews) of a WebXR frame."""
         assert len(eye_cameras) == 2
         ratio = float(self.entities[0].data.get("xrPixelRatio") or 0)
         if ratio <= 0:
@@ -398,4 +405,33 @@ class SplatScene:
         eye_frames = [[e._frame_inputs_px(w, h, cam) for e in self.entities] for cam in eye_cameras]
         eyes = [frames[0] for frames in eye_frames]
         eye_mvs = [[f.modelview for f in frames] for frames in eye_frames]
+        return (w, h), objs, eyes, eye_mvs
+
+    def render_xr_layer(self, eye_cameras, width: int, height: int, color: np.ndarray, depth: Optional[np.ndarray] = None,
+                        fmt: int = GS_FORMAT_RGBA8) -> np.ndarray:
+        """WebXR presentation into the XR layer's one framebuffer, IN PLACE: both eyes side by side over one depth buffer,
+        as three.js draws each eye camera of the session at its own viewport of the layer.  Eye size as render_xr (the
+        native eye size scaled by the first entity's xrPixelRatio, floored): the left eye at (0, 0), the right at (w, 0).
+        color: (rows, pitch, 4) of the output dtype with pitch >= 2w and rows >= h; depth: (rows, pitch) f32 or None.
+        Returns `color`."""
+        if not self.entities:
+            raise ValueError("SplatScene.render_xr_layer: no entity added")
+        (w, h), objs, eyes, eye_mvs = self._xr_objects(eye_cameras, width, height)
+        if color.shape[1] < 2 * w or color.shape[0] < h:
+            raise ValueError(f"render_xr_layer: the layer must hold two {w} x {h} eyes side by side")
+        return self.renderer.render_scene_stereo_target(eyes, objs, eye_mvs, color, depth, eye_xy=(0, 0, w, 0), fmt=fmt)
+
+    def render_xr(self, eye_cameras, width: int, height: int, color_in=(None, None), depth_in=(None, None),
+                  bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8):
+        """WebXR presentation of every entity (index.js:13-15, 184-195, 438-455): one stereo frame
+        (gs_render_scene_stereo).  Each entity's sort comes from its getModelViewMatrix() of the scene camera - the head
+        pose its tick() uses - and each entity is drawn once per eye camera with that eye's matrices.
+        Eye viewport: the XR layer's native eye size (width x height) scaled by xrPixelRatio and floored, as
+        GaussianSplattingComponent.render_xr does.  The ratio is the FIRST entity's xrPixelRatio (1 when it is not
+        positive), by the rule of render(), whose shared viewport is the first entity's.
+        color_in[e] / depth_in[e]: eye e's colour ((h, w, 4) of the output dtype) and window-space depth ((h, w) f32) at
+        the scaled size, or None.  Returns [left, right] frames, row 0 = bottom."""
+        if not self.entities:
+            raise ValueError("SplatScene.render_xr: no entity added")
+        _, objs, eyes, eye_mvs = self._xr_objects(eye_cameras, width, height)
         return self.renderer.render_scene_stereo(eyes, objs, eye_mvs, color_in=color_in, depth_in=depth_in, bg=bg, fmt=fmt)

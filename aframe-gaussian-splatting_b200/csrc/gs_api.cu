@@ -1116,8 +1116,16 @@ static int enqueue_readback(gs_context *c, gs_context::Slot &sl) {
   GS_CUDA(c, cudaStreamWaitEvent(c->copy_stream, sl.ev_done, 0));
   GS_CUDA(c, cudaMemcpyAsync(sl.ctr_host, sl.ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, c->copy_stream));
   if (sl.host_out)
-    for (int e = 0; e < (sl.stereo ? 2 : 1); ++e)
-      GS_CUDA(c, cudaMemcpyAsync(sl.out_user[e], sl.frame_src[e], sl.out_bytes[e], cudaMemcpyDeviceToHost, c->copy_stream));
+    for (int e = 0; e < (sl.stereo ? 2 : 1); ++e) {
+      if (sl.target) {  // a host gs_target: 2-D copies into the rectangles only
+        const size_t px_bytes = sl.params.out_format == GS_FORMAT_RGBA8 ? 4 : 16, row = px_bytes * sl.params.width;
+        char *dst = (char *)sl.tcolor + ((size_t)sl.torg[e][1] * sl.tpitch + sl.torg[e][0]) * px_bytes;
+        GS_CUDA(c, cudaMemcpy2DAsync(dst, px_bytes * sl.tpitch, sl.frame_src[e], row, row, sl.params.height,
+                                     cudaMemcpyDeviceToHost, c->copy_stream));
+      } else {
+        GS_CUDA(c, cudaMemcpyAsync(sl.out_user[e], sl.frame_src[e], sl.out_bytes[e], cudaMemcpyDeviceToHost, c->copy_stream));
+      }
+    }
   if (sl.raster_flags & 4u)
     GS_CUDA(c, cudaMemcpyAsync(c->tile_stats_host, c->tile_stats, sizeof(uint4) * (size_t)sl.fp_host->rc.n_tiles,
                                cudaMemcpyDeviceToHost, c->copy_stream));
@@ -1146,6 +1154,7 @@ static void fill_render_consts(gs_context *c, const gs_render_params *p, RenderC
   rc.shard_world = c->shard_world;
   rc.out_format = p->out_format;
   rc.out_tiled = (p->flags & GS_RENDER_OUT_TILED) ? 1u : 0u;
+  rc.pitch = p->width;  // tightly packed width x height buffers (stage_inputs gives a device target's frame its pitch)
 }
 
 // Output of eye e of the slot's frame (a plain or scene frame has eye 0 only): the caller's device buffer, or a per-slot
@@ -1169,6 +1178,35 @@ static int stage_inputs(gs_context *c, gs_context::Slot &sl, int e, const gs_ren
   int rcode;
   const size_t px_bytes = p->out_format == GS_FORMAT_RGBA8 ? 4 : 16;
   const size_t pixels = (size_t)p->width * p->height;
+  if (sl.target) {
+    // colour and depth of eye e's rectangle of a gs_target.  A run that overflows stores nothing (fp.overflow), and its
+    // re-run reuses the staged rectangles: the host buffers already hold the overflowed run's read-back by then
+    fp.overflow = &sl.ctr->overflow;
+    const uint32_t ox = sl.torg[e][0], oy = sl.torg[e][1];
+    if (sl.target_device) {  // in place: the buffers at the rectangle's origin, rows of the target's pitch
+      const size_t origin = (size_t)oy * sl.tpitch + ox;
+      fp.out = (char *)sl.tcolor + origin * px_bytes;
+      fp.color_in = fp.out;
+      fp.depth_in = sl.tdepth ? sl.tdepth + origin : nullptr;
+      fp.rc.pitch = sl.tpitch;
+      return GS_OK;
+    }
+    const size_t row = px_bytes * p->width;
+    if ((rcode = ensure_dev(c, sl.color_dev[e], sl.color_bytes[e], px_bytes * pixels))) return rcode;
+    if (sl.restage)
+      GS_CUDA(c, cudaMemcpy2DAsync(sl.color_dev[e], row, (const char *)sl.tcolor + ((size_t)oy * sl.tpitch + ox) * px_bytes,
+                                   px_bytes * sl.tpitch, row, p->height, cudaMemcpyHostToDevice, c->stream));
+    fp.color_in = sl.color_dev[e];
+    if (sl.tdepth) {
+      if ((rcode = ensure_dev(c, sl.depth_dev[e], sl.depth_bytes[e], sizeof(float) * pixels))) return rcode;
+      if (sl.restage)
+        GS_CUDA(c, cudaMemcpy2DAsync(sl.depth_dev[e], sizeof(float) * p->width, sl.tdepth + (size_t)oy * sl.tpitch + ox,
+                                     sizeof(float) * sl.tpitch, sizeof(float) * p->width, p->height, cudaMemcpyHostToDevice,
+                                     c->stream));
+      fp.depth_in = sl.depth_dev[e];
+    }
+    return GS_OK;
+  }
   if (p->depth_in) {
     if (p->flags & GS_RENDER_DEPTH_DEVICE) {
       fp.depth_in = p->depth_in;
@@ -1206,7 +1244,7 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   size_t out_pixels = (size_t)p->width * p->height;
   if (rc.out_tiled) out_pixels = (size_t)gs_owned_tiles(p->width, p->height, c->shard_rank, c->shard_world) * 256;
   sl.out_bytes[0] = out_pixels * px_bytes;
-  sl.host_out = !(p->flags & GS_RENDER_OUT_DEVICE);
+  sl.host_out = sl.target ? !sl.target_device : !(p->flags & GS_RENDER_OUT_DEVICE);
   sl.peer = (p->flags & GS_RENDER_OUT_PEER) != 0;
   if (sl.peer) {
     if (!c->peer_world || c->peer_world != c->shard_world || c->peer_rank != c->shard_rank)
@@ -1236,7 +1274,8 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   }
   if ((rcode = stage_inputs(c, sl, 0, p, fp))) return rcode;
   // raster instantiation: pixel loop (two pixels per lane by default), depth test, statistics
-  sl.raster_flags = c->raster_base_flags | (p->depth_in ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u);
+  const bool depth = p->depth_in || (sl.target && sl.tdepth);  // a target's depth is that of both eyes
+  sl.raster_flags = c->raster_base_flags | (depth ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u);
   if (sl.stereo) {
     // the pair of eye frames the stereo kernels read: eye 0 as above, eye 1 from its own parameters (same size and flags)
     StereoParams &st = *sl.stereo_host;
@@ -1314,6 +1353,7 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
       if (rcode) return rcode;
     }
     int rcode;
+    sl.restage = false;  // a target frame blends over the rectangles staged at its first submission
     if ((rcode = submit(c, sl))) return rcode;
   }
   memset(&c->stats, 0, sizeof(c->stats));
@@ -1372,10 +1412,47 @@ struct StereoInput {
   const float (*mv)[2][16];  // per entity of the scene table, in its order: the modelview of each eye
 };
 
+// a frame into a gs_target (validated by check_target): the target and the rectangle origin of each eye
+struct TargetInput {
+  const gs_target *t;
+  uint32_t xy[2][2];
+};
+
+// do the rectangles [ax, ax+aw) x [ay, ay+ah) and [bx, bx+bw) x [by, by+bh) share a pixel
+static bool rects_overlap(uint32_t ax, uint32_t ay, uint32_t aw, uint32_t ah, uint32_t bx, uint32_t by, uint32_t bw,
+                          uint32_t bh) {
+  return (uint64_t)ax < (uint64_t)bx + bw && (uint64_t)bx < (uint64_t)ax + aw && (uint64_t)ay < (uint64_t)by + bh &&
+         (uint64_t)by < (uint64_t)ay + ah;
+}
+
+// Successive frames into one target compose in submission order, like successive GL draws: a target frame first waits
+// (oldest first) for every pending target frame on the same colour buffer whose rectangles meet its own (w x h each).
+// Stream order alone is not enough: gs_wait may still re-run such a frame, and a host target's rectangle is read at
+// submission.
+static int wait_overlapping(gs_context *c, const TargetInput &t, uint32_t w, uint32_t h, int n_eyes) {
+  for (;;) {
+    gs_context::Slot *hit = nullptr;
+    for (auto &o : c->slot) {
+      if (!o.pending || !o.target || o.tcolor != t.t->color || (hit && o.ticket > hit->ticket)) continue;
+      bool meet = false;
+      for (int a = 0; a < n_eyes; ++a)
+        for (int b = 0; b < (o.stereo ? 2 : 1); ++b)
+          meet = meet || rects_overlap(t.xy[a][0], t.xy[a][1], w, h, o.torg[b][0], o.torg[b][1], o.params.width, o.params.height);
+      if (meet) hit = &o;
+    }
+    if (!hit) return GS_OK;
+    int rc = wait_slot(c, *hit, nullptr);
+    if (rc) return rc;
+  }
+}
+
 // gs_render_async, scene and stereo scene frames.  scene: the table built by build_scene_table (nullptr = a plain frame);
-// color_in: the colour target or nullptr; stereo: the second eye of a stereo scene frame (nullptr otherwise; p is eye 0).
+// color_in: the colour target or nullptr; stereo: the second eye of a stereo scene frame (nullptr otherwise; p is eye 0);
+// target: the gs_target the frame is drawn into in place (nullptr otherwise; color_in is then nullptr and out_rgba the
+// target's colour buffer).
 static int render_async(gs_context *c, const gs_render_params *p, const SceneTable *scene, size_t scene_bytes,
-                        const void *color_in, void *out_rgba, uint64_t *out_ticket, const StereoInput *stereo = nullptr) {
+                        const void *color_in, void *out_rgba, uint64_t *out_ticket, const StereoInput *stereo = nullptr,
+                        const TargetInput *target = nullptr) {
   if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
   if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
@@ -1388,6 +1465,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   gs_context::Slot &sl = c->slot[ticket % gs_context::kSlots];
   int rcode;
   if (sl.pending && (rcode = wait_slot(c, sl, nullptr))) return rcode;  // slot reuse: its previous frame must be done
+  if (target && (rcode = wait_overlapping(c, *target, p->width, p->height, stereo ? 2 : 1))) return rcode;
   if ((p->flags & GS_RENDER_OUT_PEER) && ticket >= 3) {
     // the shared frame ring of the fused exchange has three entries, released by gs_wait: at most three such frames
     gs_context::Slot &o = c->slot[(ticket - 3) % gs_context::kSlots];
@@ -1444,6 +1522,15 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   sl.slab = slab;
   sl.color_in[0] = color_in;
   sl.color_device = (p->flags & GS_RENDER_COLOR_DEVICE) != 0;
+  sl.target = target != nullptr;
+  sl.restage = true;
+  if (target) {
+    sl.target_device = (target->t->flags & GS_TARGET_DEVICE) != 0;
+    sl.tcolor = target->t->color;
+    sl.tdepth = target->t->depth;
+    sl.tpitch = target->t->pitch;
+    memcpy(sl.torg, target->xy, sizeof(sl.torg));
+  }
   sl.scene = scene != nullptr;
   if (scene) {
     if ((rcode = ensure_slot_scene(c, sl))) return rcode;
@@ -1471,9 +1558,9 @@ extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *o
   return render_async(c, p, nullptr, 0, nullptr, out_rgba, out_ticket);
 }
 
-extern "C" int gs_render_scene_async(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
-                                     const void *color_in, void *out_rgba, uint64_t *out_ticket) {
-  if (!c || !frame || !out_rgba) return GS_ERR_INVALID;
+// gs_render_scene_async, and gs_render_scene_target_async (target set: color_in is nullptr, out_rgba the target's colour)
+static int scene_async(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                       const void *color_in, void *out_rgba, uint64_t *out_ticket, const TargetInput *target) {
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render_scene before any push");
   if (frame->flags & GS_RENDER_REUSE_SORT) return fail(c, GS_ERR_INVALID, "scene frames always sort: GS_RENDER_REUSE_SORT is not accepted");
   size_t bytes = 0;
@@ -1485,9 +1572,52 @@ extern "C" int gs_render_scene_async(gs_context *c, const gs_render_params *fram
     memcpy(p.modelview, objs[0].modelview, sizeof(p.modelview));
     p.has_cutout = objs[0].has_cutout;
     memcpy(p.cutout16, objs[0].cutout16, sizeof(p.cutout16));
-    return render_async(c, &p, nullptr, 0, color_in, out_rgba, out_ticket);
+    return render_async(c, &p, nullptr, 0, color_in, out_rgba, out_ticket, nullptr, target);
   }
-  return render_async(c, frame, c->scene_tmp, bytes, color_in, out_rgba, out_ticket);
+  return render_async(c, frame, c->scene_tmp, bytes, color_in, out_rgba, out_ticket, nullptr, target);
+}
+
+extern "C" int gs_render_scene_async(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                                     const void *color_in, void *out_rgba, uint64_t *out_ticket) {
+  if (!c || !frame || !out_rgba) return GS_ERR_INVALID;
+  return scene_async(c, frame, objs, n_objs, color_in, out_rgba, out_ticket, nullptr);
+}
+
+// The rules of a frame into eye rectangle (x, y) of a gs_target that do not depend on the scene (those of gs_render_scene
+// and gs_render_scene_stereo are checked after these, also before anything is changed)
+static int check_target(gs_context *c, const gs_render_params *p, const gs_target *t, uint32_t x, uint32_t y) {
+  if (!t || !t->color) return fail(c, GS_ERR_INVALID, "target frame: no target or no colour buffer");
+  if (t->flags & ~(uint32_t)GS_TARGET_DEVICE) return fail(c, GS_ERR_INVALID, "target frame: unknown gs_target flags");
+  if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "target frame: not on a sharded context");
+  if (p->depth_in) return fail(c, GS_ERR_INVALID, "target frame: depth_in must be NULL (the depth is the target's)");
+  if (p->flags & (GS_RENDER_OUT_DEVICE | GS_RENDER_COLOR_DEVICE | GS_RENDER_DEPTH_DEVICE | GS_RENDER_OUT_TILED |
+                  GS_RENDER_OUT_PEER | GS_RENDER_REUSE_SORT))
+    return fail(c, GS_ERR_INVALID,
+                "target frame: GS_RENDER_OUT_DEVICE, _COLOR_DEVICE, _DEPTH_DEVICE (use GS_TARGET_DEVICE), _OUT_TILED, "
+                "_OUT_PEER and _REUSE_SORT are not accepted");
+  if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
+    return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
+  if ((uint64_t)x + p->width > t->pitch || (uint64_t)y + p->height > t->rows)
+    return fail(c, GS_ERR_INVALID, "target frame: the viewport rectangle is not inside the target");
+  return GS_OK;
+}
+
+extern "C" int gs_render_scene_target_async(gs_context *c, const gs_render_params *frame, const gs_object *objs,
+                                            uint32_t n_objs, const gs_target *target, uint32_t x, uint32_t y,
+                                            uint64_t *out_ticket) {
+  if (!c || !frame) return GS_ERR_INVALID;
+  int rc = check_target(c, frame, target, x, y);
+  if (rc) return rc;
+  const TargetInput t{target, {{x, y}, {0, 0}}};
+  return scene_async(c, frame, objs, n_objs, nullptr, target->color, out_ticket, &t);
+}
+
+extern "C" int gs_render_scene_target(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                                      const gs_target *target, uint32_t x, uint32_t y, gs_stats *stats) {
+  uint64_t t = 0;
+  int rc = gs_render_scene_target_async(c, frame, objs, n_objs, target, x, y, &t);
+  if (rc) return rc;
+  return gs_wait(c, t, stats);
 }
 
 extern "C" int gs_render_scene(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
@@ -1588,10 +1718,11 @@ extern "C" int gs_render_stereo(gs_context *c, const float view[4], const float 
 
 // XR over a multi-entity page: the one scene sort of the frame from the head camera (every entity's tick(), index.js:438-455),
 // each entity drawn once per eye with that eye's matrices (onBeforeRender per eye camera, index.js:184-195)
-extern "C" int gs_render_scene_stereo_async(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
-                                            const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
-                                            void *const out_rgba[2], uint64_t *out_ticket) {
-  if (!c) return GS_ERR_INVALID;
+// gs_render_scene_stereo_async, and gs_render_scene_stereo_target_async (target set: no color_in, out_rgba = the layer's
+// colour twice)
+static int scene_stereo_async(gs_context *c, const gs_render_params eyes[2], const gs_object *objs, const float *eye_modelviews,
+                              uint32_t n_objs, const void *const color_in[2], void *const out_rgba[2], uint64_t *out_ticket,
+                              const TargetInput *target) {
   if (!eyes || !eye_modelviews || !out_rgba || !out_rgba[0] || !out_rgba[1])
     return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: missing eyes, eye modelviews or outputs");
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render_scene_stereo before any push");
@@ -1611,7 +1742,43 @@ extern "C" int gs_render_scene_stereo_async(gs_context *c, const gs_render_param
   for (uint32_t j = 0; j < t.n; ++j)
     for (int e = 0; e < 2; ++e) memcpy(mv[j][e], eye_modelviews + ((size_t)e * n_objs + t.obj[j].rank) * 16, sizeof(mv[j][e]));
   const StereoInput st{&eyes[1], color_in ? color_in[1] : nullptr, out_rgba[1], mv};
-  return render_async(c, &eyes[0], c->scene_tmp, bytes, color_in ? color_in[0] : nullptr, out_rgba[0], out_ticket, &st);
+  return render_async(c, &eyes[0], c->scene_tmp, bytes, color_in ? color_in[0] : nullptr, out_rgba[0], out_ticket, &st, target);
+}
+
+extern "C" int gs_render_scene_stereo_async(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
+                                            const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
+                                            void *const out_rgba[2], uint64_t *out_ticket) {
+  if (!c) return GS_ERR_INVALID;
+  return scene_stereo_async(c, eyes, objs, eye_modelviews, n_objs, color_in, out_rgba, out_ticket, nullptr);
+}
+
+// WebXR into the layer's one framebuffer: each eye at its viewport rectangle (three.js renders each eye camera of the
+// ArrayCamera with its own viewport)
+extern "C" int gs_render_scene_stereo_target_async(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
+                                                   const float *eye_modelviews, uint32_t n_objs, const gs_target *layer,
+                                                   const uint32_t eye_xy[4], uint64_t *out_ticket) {
+  if (!c) return GS_ERR_INVALID;
+  if (!eyes || !eye_xy) return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo_target: missing eyes or eye rectangles");
+  int rc;
+  for (int e = 0; e < 2; ++e)
+    if ((rc = check_target(c, &eyes[e], layer, eye_xy[2 * e], eye_xy[2 * e + 1]))) return rc;
+  if (eyes[0].out_format != eyes[1].out_format)
+    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo_target: the eyes must have the layer's one format");
+  if (eyes[0].width == eyes[1].width && eyes[0].height == eyes[1].height &&
+      rects_overlap(eye_xy[0], eye_xy[1], eyes[0].width, eyes[0].height, eye_xy[2], eye_xy[3], eyes[1].width, eyes[1].height))
+    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo_target: the eye rectangles overlap");
+  const TargetInput t{layer, {{eye_xy[0], eye_xy[1]}, {eye_xy[2], eye_xy[3]}}};
+  void *const outs[2] = {layer->color, layer->color};
+  return scene_stereo_async(c, eyes, objs, eye_modelviews, n_objs, nullptr, outs, out_ticket, &t);
+}
+
+extern "C" int gs_render_scene_stereo_target(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
+                                             const float *eye_modelviews, uint32_t n_objs, const gs_target *layer,
+                                             const uint32_t eye_xy[4], gs_stats *stats) {
+  uint64_t t = 0;
+  int rc = gs_render_scene_stereo_target_async(c, eyes, objs, eye_modelviews, n_objs, layer, eye_xy, &t);
+  if (rc) return rc;
+  return gs_wait(c, t, stats);
 }
 
 extern "C" int gs_render_scene_stereo(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,

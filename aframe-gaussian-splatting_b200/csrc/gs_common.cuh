@@ -87,6 +87,10 @@ struct RenderConsts {
   uint32_t shard_rank, shard_world;
   int32_t out_format;
   uint32_t out_tiled;
+  // pixels per row of out, color_in and depth_in: pixel (x, y) of the frame is element y * pitch + x.  A frame into a device
+  // gs_target has the target's pitch and its buffers point at the rectangle's origin, so the frame reads and writes the
+  // rectangle in place while its pixel loop stays viewport-relative; every other frame has pitch = width
+  uint32_t pitch;
 };
 
 struct SortConsts {
@@ -107,6 +111,8 @@ struct FrameParams {
   const void *depth_in;  // optional window-space depth of foreign geometry (f32, width*height, row 0 = bottom)
   const void *color_in;  // optional colour of the geometry already drawn (output element type, width*height, row 0 =
                          // bottom): the per-pixel destination of the blend in place of rc.bg
+  const uint32_t *overflow;  // frames into a gs_target: the frame's FrameCounters::overflow.  A run that overflowed stores
+                             // nothing, so its re-run blends over the target as it was (NULL for every other frame)
   // ---- fused raster + exchange over NVLink peer memory (GS_RENDER_OUT_PEER) ----
   uint32_t n_peer;                       // 0: plain output; else every finished tile is stored into all ranks' frames
   uint32_t peer_rank;
@@ -311,6 +317,14 @@ struct gs_context {
     gs::SceneTable *scene_host = nullptr;    // pinned staging
     size_t scene_bytes = 0;                  // bytes of the table in use (header + non-empty entities)
     gs::ObjCounters *octr = nullptr;         // [kMaxObjects] per-entity depth-pass results
+    // frames into a gs_target (gs_render_scene*_target): each eye drawn in place at its rectangle of the caller's buffers
+    bool target = false;
+    bool target_device = false;              // GS_TARGET_DEVICE: read and written where they are; else staged per eye
+    void *tcolor = nullptr;
+    const float *tdepth = nullptr;
+    uint32_t tpitch = 0;
+    uint32_t torg[2][2] = {};                // rectangle origin (x, y) of each eye
+    bool restage = true;                     // false while gs_wait re-runs the frame: the staged rectangles are reused
     uint32_t raster_flags = 0;               // k_raster instantiation of this frame (packed | depth | stats)
     uint32_t n_splats = 0;                   // resident splats when the frame was submitted
     uint32_t n_sortable = 0;                 // splats the frame's sort considers (scene frames: in the entities' ranges)

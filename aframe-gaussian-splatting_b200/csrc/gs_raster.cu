@@ -89,11 +89,15 @@ __device__ __forceinline__ void store_pixel(const FrameParams *fp, uint32_t tile
                                             uint32_t ly, uint32_t x, uint32_t y, bool inside, float T, float Cr, float Cg,
                                             float Cb) {
   const RenderConsts &rc = fp->rc;
+  // a frame into a gs_target whose instance buffer overflowed is re-run over the target: this run leaves it as it was
+  if (fp->overflow && *fp->overflow) return;
+  // the pixel's place in out and color_in: rows of rc.pitch pixels (a device target's row pitch, else the width; the
+  // host points the buffers at the target rectangle's origin)
+  const size_t p = (size_t)y * rc.pitch + x;
   // composite over the clear colour, or over the colour target's pixel (the geometry already drawn: the destination of
   // the reference's blend, index.js:177-181); an RGBA8 target reads as float(byte) / 255.0 like the splat colours
   float d0 = rc.bg[0], d1 = rc.bg[1], d2 = rc.bg[2], d3 = rc.bg[3];
   if (fp->color_in && inside) {
-    const size_t p = (size_t)y * rc.width + x;
     if (rc.out_format == GS_FORMAT_RGBA8) {
       const uint32_t v = __ldg((const uint32_t *)fp->color_in + p);
       d0 = __fdiv_rn((float)(v & 255u), 255.0f);
@@ -114,7 +118,7 @@ __device__ __forceinline__ void store_pixel(const FrameParams *fp, uint32_t tile
     pix = (size_t)slot * 256 + ly * 16 + lx;
     write = true;
   } else {
-    pix = (size_t)y * rc.width + x;
+    pix = p;
     write = inside;
   }
   if (!write) return;
@@ -216,8 +220,8 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   float d0 = 1.0f, d1 = 1.0f;  // window depth of the foreign geometry at the pixel(s)
   if (DEPTH) {
     const float *din = (const float *)fp->depth_in;
-    if (inside0 && (!STEREO || din)) d0 = __ldg(din + (size_t)y * rc.width + x);
-    if (inside1 && (!STEREO || din)) d1 = __ldg(din + (size_t)(y + 1) * rc.width + x);
+    if (inside0 && (!STEREO || din)) d0 = __ldg(din + (size_t)y * rc.pitch + x);
+    if (inside1 && (!STEREO || din)) d1 = __ldg(din + (size_t)(y + 1) * rc.pitch + x);
   }
 
   const uint2 range = bin_range[bin];

@@ -11,7 +11,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F, GS_RENDER_OUT_DEVICE, GS_RENDER_OUT_TILED,
-                   GS_RENDER_REUSE_SORT, GS_RENDER_STATS, GsObject, GsRenderParams, GsStats)
+                   GS_RENDER_REUSE_SORT, GS_RENDER_STATS, GS_TARGET_DEVICE, GsObject, GsRenderParams, GsStats, GsTarget)
 from .scenes import FrameInputs
 
 
@@ -310,6 +310,83 @@ class SplatContext:
         t = C.c_uint64()
         self._check(self._lib.gs_render_scene_stereo_async(self._h, arr, objs, mv.ctypes.data_as(C.POINTER(C.c_float)),
                                                            len(objects), col, ptrs, C.byref(t)))
+        return t.value
+
+    # -- frames drawn into the caller's framebuffer in place (gs_render_scene*_target) --
+    @staticmethod
+    def make_target(color_ptr: int, depth_ptr: Optional[int], pitch: int, rows: int, device: bool = False) -> GsTarget:
+        """gs_target over caller-owned buffers: pitch x rows pixels of colour (and f32 depth, or None); device=True for
+        device memory on the context's GPU."""
+        t = GsTarget()
+        t.color, t.depth = color_ptr, depth_ptr
+        t.pitch, t.rows, t.flags = int(pitch), int(rows), GS_TARGET_DEVICE if device else 0
+        return t
+
+    @staticmethod
+    def _host_target(color: np.ndarray, depth: Optional[np.ndarray], fmt: int) -> GsTarget:
+        """gs_target over numpy buffers: color (rows, pitch, 4) of the format's dtype, depth (rows, pitch) f32 or None.
+        Both are written (colour) and read in place, so they must be C-contiguous already."""
+        dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
+        if color.dtype != dtype or color.ndim != 3 or color.shape[2] != 4 or not color.flags["C_CONTIGUOUS"]:
+            raise ValueError("color must be a C-contiguous (rows, pitch, 4) array of the output format's dtype")
+        rows, pitch = color.shape[:2]
+        if depth is not None and (depth.dtype != np.float32 or depth.shape != (rows, pitch) or not depth.flags["C_CONTIGUOUS"]):
+            raise ValueError("depth must be a C-contiguous (rows, pitch) float32 array")
+        return SplatContext.make_target(color.ctypes.data, None if depth is None else depth.ctypes.data, pitch, rows)
+
+    def render_scene_target(self, frame: FrameInputs, objects: Sequence[SceneObject], color: np.ndarray,
+                            depth: Optional[np.ndarray] = None, viewport=(0, 0), fmt: int = GS_FORMAT_RGBA8,
+                            stats: bool = False) -> np.ndarray:
+        """gs_render_scene_target: the scene frame blended IN PLACE into the rectangle of frame.width x frame.height at
+        viewport = (x, y) of `color` ((rows, pitch, 4), row 0 = bottom), depth-tested against `depth` ((rows, pitch) f32
+        window-space depth, or None).  Nothing outside the rectangle is read or written.  Returns `color`."""
+        t = self._host_target(color, depth, fmt)
+        p = self.make_params(frame, fmt=fmt, flags=GS_RENDER_STATS if stats else 0)
+        st = GsStats()
+        self._check(self._lib.gs_render_scene_target(self._h, C.byref(p), make_objects(objects), len(objects), C.byref(t),
+                                                     int(viewport[0]), int(viewport[1]), C.byref(st)))
+        self.last_stats = st
+        return color
+
+    def render_scene_target_async(self, params: GsRenderParams, objects: Sequence[SceneObject], target: GsTarget,
+                                  x: int, y: int) -> int:
+        """gs_render_scene_target_async: enqueue one scene frame into `target` (make_target) at (x, y); collected with
+        wait().  The target's buffers must stay valid until then."""
+        t = C.c_uint64()
+        self._check(self._lib.gs_render_scene_target_async(self._h, C.byref(params), make_objects(objects), len(objects),
+                                                           C.byref(target), int(x), int(y), C.byref(t)))
+        return t.value
+
+    def render_scene_stereo_target(self, eyes: Sequence[FrameInputs], objects: Sequence[SceneObject], eye_modelviews,
+                                   color: np.ndarray, depth: Optional[np.ndarray] = None, eye_xy=None,
+                                   fmt: int = GS_FORMAT_RGBA8) -> np.ndarray:
+        """gs_render_scene_stereo_target: one WebXR frame drawn IN PLACE into one layer ((rows, pitch, 4) colour, optional
+        (rows, pitch) f32 depth): eye e at (eye_xy[2e], eye_xy[2e+1]); eye_xy None = side by side, (0, 0, w, 0).
+        Arguments as render_scene_stereo.  Returns `color`."""
+        t = self._host_target(color, depth, fmt)
+        st = GsStats()
+        args = self._stereo_target_args(eyes, fmt, objects, eye_modelviews, eye_xy)
+        self._check(self._lib.gs_render_scene_stereo_target(self._h, args[0], args[1], args[2], len(objects), C.byref(t),
+                                                            args[3], C.byref(st)))
+        self.last_stats = st
+        return color
+
+    def _stereo_target_args(self, eyes, fmt, objects, eye_modelviews, eye_xy):
+        params = [e if isinstance(e, GsRenderParams) else self.make_params(e, fmt=fmt) for e in eyes]
+        arr, objs, mv, _, _ = self._stereo_args(params, objects, eye_modelviews, None, [0, 0])
+        if eye_xy is None:
+            eye_xy = (0, 0, params[0].width, 0)
+        xy = (C.c_uint32 * 4)(*[int(v) for v in eye_xy])
+        return arr, objs, mv.ctypes.data_as(C.POINTER(C.c_float)), xy, mv
+
+    def render_scene_stereo_target_async(self, eyes_params, objects: Sequence[SceneObject], eye_modelviews,
+                                         target: GsTarget, eye_xy) -> int:
+        """gs_render_scene_stereo_target_async: enqueue one stereo scene frame into `target` (make_target), eye e at
+        (eye_xy[2e], eye_xy[2e+1]); collected with wait().  The target's buffers must stay valid until then."""
+        args = self._stereo_target_args(eyes_params, None, objects, eye_modelviews, eye_xy)
+        t = C.c_uint64()
+        self._check(self._lib.gs_render_scene_stereo_target_async(self._h, args[0], args[1], args[2], len(objects),
+                                                                  C.byref(target), args[3], C.byref(t)))
         return t.value
 
     def render_raw(self, params: GsRenderParams, out_ptr: int) -> GsStats:

@@ -117,22 +117,26 @@ class Splats : public Napi::ObjectWrap<Splats> {
     Check(i.Env(), gs_render_scene(ctx_, &p, objs.data(), (uint32_t)objs.size(), color, i[3].As<Napi::Uint8Array>().Data(), nullptr));
     return i.Env().Undefined();
   }
-  // renderSceneXR([eyeL, eyeR] {proj, width, height, focal, depth?: Float32Array}, [{first, count, modelview, cutout?,
-  //                eyeModelviews: [Float32Array, Float32Array]}, ...], [colorL, colorR] (Uint8Array or undefined),
-  //                [outL, outR] Uint8Array)  <- an XR frame of every entity of the page: each entity's tick() sort from the head
-  // camera (modelview = its getModelViewMatrix()), its draw once per eye with eyeModelviews[e] = getModelViewMatrix(eyeCamera
-  // e); both eyes share the XR layer's viewport size.  One gs_render_scene_stereo: one sort, both eyes in one pass.
+  // renderSceneXR([eyeL, eyeR] {proj, width, height, focal, x, y}, [{first, count, modelview, cutout?,
+  //                eyeModelviews: [Float32Array, Float32Array]}, ...], layer {color: Uint8Array, depth?: Float32Array, pitch,
+  //                rows})  <- an XR frame of every entity of the page, drawn IN PLACE into the XR layer's one framebuffer:
+  // each entity's tick() sort from the head camera (modelview = its getModelViewMatrix()), its draw once per eye with
+  // eyeModelviews[e] = getModelViewMatrix(eyeCamera e) at that eye's viewport (x, y, width, height) = layer.getViewport(view
+  // e); both eyes share one viewport size and the layer's one depth buffer.  One gs_render_scene_stereo_target: one sort,
+  // both eyes in one pass, only the two eye rectangles read and written.
   Napi::Value RenderSceneXR(const Napi::CallbackInfo& i) {
     auto eyes_in = i[0].As<Napi::Array>();
     gs_render_params eyes[2] = {};
+    uint32_t eye_xy[4];
     for (uint32_t e = 0; e < 2; ++e) {
       auto o = eyes_in.Get(e).As<Napi::Object>();
       memcpy(eyes[e].proj, o.Get("proj").As<Napi::Float32Array>().Data(), 64);
       eyes[e].width = o.Get("width").As<Napi::Number>().Uint32Value();
       eyes[e].height = o.Get("height").As<Napi::Number>().Uint32Value();
       eyes[e].focal = o.Get("focal").As<Napi::Number>().FloatValue();
-      if (o.Has("depth")) eyes[e].depth_in = o.Get("depth").As<Napi::Float32Array>().Data();
       eyes[e].out_format = GS_FORMAT_RGBA8;
+      eye_xy[2 * e] = o.Get("x").As<Napi::Number>().Uint32Value();
+      eye_xy[2 * e + 1] = o.Get("y").As<Napi::Number>().Uint32Value();
     }
     auto list = i[1].As<Napi::Array>();
     const uint32_t n = list.Length();
@@ -149,15 +153,13 @@ class Splats : public Napi::ObjectWrap<Splats> {
       auto mvs = e.Get("eyeModelviews").As<Napi::Array>();
       for (uint32_t s = 0; s < 2; ++s) memcpy(&eye_mv[((size_t)s * n + k) * 16], mvs.Get(s).As<Napi::Float32Array>().Data(), 64);
     }
-    auto cols = i[2].As<Napi::Array>();
-    auto outs = i[3].As<Napi::Array>();
-    const void* color[2];
-    void* out[2];
-    for (uint32_t s = 0; s < 2; ++s) {
-      color[s] = cols.Get(s).IsUndefined() ? nullptr : cols.Get(s).As<Napi::Uint8Array>().Data();
-      out[s] = outs.Get(s).As<Napi::Uint8Array>().Data();
-    }
-    Check(i.Env(), gs_render_scene_stereo(ctx_, eyes, objs.data(), eye_mv.data(), n, color, out, nullptr));
+    auto l = i[2].As<Napi::Object>();
+    gs_target layer = {};
+    layer.color = l.Get("color").As<Napi::Uint8Array>().Data();
+    if (l.Has("depth")) layer.depth = l.Get("depth").As<Napi::Float32Array>().Data();
+    layer.pitch = l.Get("pitch").As<Napi::Number>().Uint32Value();
+    layer.rows = l.Get("rows").As<Napi::Number>().Uint32Value();
+    Check(i.Env(), gs_render_scene_stereo_target(ctx_, eyes, objs.data(), eye_mv.data(), n, &layer, eye_xy, nullptr));
     return i.Env().Undefined();
   }
   gs_context* ctx_ = nullptr;

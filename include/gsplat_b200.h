@@ -351,6 +351,66 @@ GS_API int gs_render_scene_stereo(gs_context *ctx, const gs_render_params eyes[2
                                   const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
                                   void *const out_rgba[2], gs_stats *stats);
 
+/*
+ * Drawing into the caller's framebuffer in place (index.js:177-195: the mesh is drawn into whatever framebuffer is bound, at
+ * the current viewport; in a WebXR session that is the XR layer's one framebuffer, both eyes side by side over one depth
+ * buffer, each eye camera drawn at its own viewport rectangle).
+ */
+enum { GS_TARGET_DEVICE = 1u << 0 /* color and depth are device memory on the context's GPU (default: host memory) */ };
+typedef struct gs_target {
+  void *color;         /* pitch * rows pixels of the frame's out_format (u8 RGBA8 / f32 RGBA32F), row 0 = bottom: the blend's
+                          destination, written in place                                                                  */
+  const float *depth;  /* NULL, or pitch * rows window-space depths in [0,1], row 0 = bottom (LEQUAL test, nothing written) */
+  uint32_t pitch;      /* pixels per row of both buffers                                                                  */
+  uint32_t rows;       /* rows of both buffers                                                                            */
+  uint32_t flags;      /* GS_TARGET_*                                                                                     */
+} gs_target;
+
+/*
+ * A scene frame (gs_render_scene) drawn into the viewport rectangle [x, x+w) x [y, y+h) of `target`, w x h = frame->width x
+ * frame->height (1..4096 per side).  Pixel (x+i, y+j) of the target becomes pixel (i, j) of the gs_render_scene frame whose
+ * color_in and depth_in are the rectangle's content, byte for byte, on every path (one-pass, slab, and the whole-table
+ * single-entity route of gs_render_scene).  The frame's pixel loop is viewport-relative: tiles start at the rectangle's
+ * origin, pixel centres are (i + 0.5, j + 0.5).
+ * Rules:
+ *   - the frame reads and writes its rectangle only: every other pixel of both buffers is neither read nor written;
+ *   - the blend's destination is the target's pixel, so frame->bg_rgba is ignored;
+ *   - frame->depth_in must be NULL (depth comes from the target); GS_RENDER_OUT_DEVICE, _COLOR_DEVICE and _DEPTH_DEVICE
+ *     are refused (GS_TARGET_DEVICE replaces them), and so are _OUT_TILED, _OUT_PEER and _REUSE_SORT; GS_RENDER_STATS is
+ *     accepted as by gs_render_scene;
+ *   - GS_ERR_INVALID, changing nothing, for: a sharded context, a NULL target or color, unknown target flags, a rectangle
+ *     outside pitch x rows, and whatever gs_render_scene refuses;
+ *   - device targets are read and written where they are, with no staging copy.  Host targets: the rectangle is read when
+ *     the frame is submitted (as a host color_in is) and written back into the rectangle by the frame's read-back; both
+ *     buffers must stay valid until gs_wait;
+ *   - frames in flight: a frame whose rectangle overlaps the rectangle of a still-pending target frame on the same `color`
+ *     first waits for that frame, so successive frames into one target compose in submission order, like successive GL
+ *     draws.  Frames into disjoint rectangles (split-screen viewports, or the next layer of a double-buffered target) stay
+ *     pipelined;
+ *   - a frame whose tile-instance buffer overflowed is re-run by gs_wait over the target's content as it was when the
+ *     frame started: the overflowed run stores nothing, and a host target's re-run reuses the copy taken at submission;
+ *   - gs_stats: those of the gs_render_scene frame.
+ */
+GS_API int gs_render_scene_target_async(gs_context *ctx, const gs_render_params *frame, const gs_object *objs,
+                                        uint32_t n_objs, const gs_target *target, uint32_t x, uint32_t y,
+                                        uint64_t *out_ticket);
+GS_API int gs_render_scene_target(gs_context *ctx, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                                  const gs_target *target, uint32_t x, uint32_t y, gs_stats *stats);
+/*
+ * A stereo scene frame (gs_render_scene_stereo) drawn into one layer: eye e into the rectangle at (eye_xy[2e],
+ * eye_xy[2e+1]) of eyes[e].width x eyes[e].height (a side-by-side WebXR layer: eye_xy = {0, 0, w, 0}).  Each eye's
+ * rectangle equals that eye's gs_render_scene_stereo frame over the rectangle's colour and depth, byte for byte, on the
+ * one-pass and the slab path.  The rules of gs_render_scene_target apply to each eye (both eyes take their depth from
+ * layer->depth, their destination from layer->color), plus those of gs_render_scene_stereo (equal eye sizes and flags; no
+ * GS_RENDER_STATS); overlapping eye rectangles are refused.
+ */
+GS_API int gs_render_scene_stereo_target_async(gs_context *ctx, const gs_render_params eyes[2], const gs_object *objs,
+                                               const float *eye_modelviews, uint32_t n_objs, const gs_target *layer,
+                                               const uint32_t eye_xy[4], uint64_t *out_ticket);
+GS_API int gs_render_scene_stereo_target(gs_context *ctx, const gs_render_params eyes[2], const gs_object *objs,
+                                         const float *eye_modelviews, uint32_t n_objs, const gs_target *layer,
+                                         const uint32_t eye_xy[4], gs_stats *stats);
+
 /* Per-splat projected record of the last gs_render (testing the vertex-shader restatement):
  * 8 floats per resident splat {cx, cy, a1x, a1y, a2x, a2y, rgba8-as-bits, tile-rect-as-bits};
  * rect == 0xFFFFFFFF marks a splat that was not projected/visible. */

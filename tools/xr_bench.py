@@ -11,6 +11,8 @@ xrPixelRatio 0.5) and 1832x1920.
 Arms, each timed with three frames in flight, the L2 flushed between steps and one CUDA-event pair per round, the arms
 alternated twice in the same run:
   stereo   one gs_render_scene_stereo_async per XR frame (one head sort, both eyes binned and rasterised together);
+  layer, stereo_copy  the stereo frame into one side-by-side device layer (RGBA8 colour plus f32 depth), in place
+           (gs_render_scene_stereo_target_async) or around six cudaMemcpy2DAsync copies (tools/xr_layer_arms.py);
   mono2    two gs_render_scene_async frames per XR frame, one per eye, each sorting itself - the only way to draw such a
            page for two eyes without the stereo entry point.  It is a cost comparison: its frames use each eye's own sort.
 For one entity spanning the whole table (the 3 M one), synchronous frames:
@@ -33,6 +35,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def card_power():
@@ -55,6 +58,7 @@ def main():
     args = ap.parse_args()
     gs = importlib.import_module("aframe-gaussian-splatting_b200")
     import poses
+    from xr_layer_arms import LayerArms
     sc = gs.scenes
     n_a, n_b = args.small, args.large
     # rows first: the generator forks worker processes, which must happen before this process owns a CUDA context
@@ -148,7 +152,10 @@ def main():
                 ts.append(t.value)
             return ts
 
-        rounds = timed({"stereo": sub_stereo, "mono2": sub_mono2}, args.steps)
+        la = LayerArms(gs, ctx, torch, dev, eyes, objs, eye_mvs, cols, deps, W, H)
+        rounds = timed({"stereo": sub_stereo, "mono2": sub_mono2, "layer": la.sub_layer, "stereo_copy": la.sub_stereo_copy},
+                       args.steps)
+        layer_sha = la.check()
         lat = [ctx.wait(sub_stereo(i)[0]).as_dict() for i in range(10)]
         st = {k: float(np.median([x[k] for x in lat])) for k in ("ms_sort", "ms_project", "ms_bin", "ms_raster", "ms_total")}
         cnt = {k: int(lat[0][k]) for k in ("n_sorted", "n_dropped", "n_visible", "n_instances", "n_instances_kept", "n_tiles",
@@ -180,7 +187,8 @@ def main():
         results.append({
             "eye": [W, H], "xr_frames_per_s": {a: 1000.0 / v for a, v in med.items()}, "ms_per_xr_frame": med,
             "rounds_ms": {**rounds, **rounds1},
-            "stereo_over_mono2": med["stereo"] / med["mono2"], "stereo1_over_render_stereo": med["stereo1"] / med["rstereo"],
+            "stereo_over_mono2": med["stereo"] / med["mono2"], "layer_over_stereo_copy": med["layer"] / med["stereo_copy"],
+            "layer_sha256": layer_sha, "stereo1_over_render_stereo": med["stereo1"] / med["rstereo"],
             "stereo_stages_ms": st, "stereo_counters": cnt, "mono_scene_frame_launches": int(mono["kernel_launches"]),
         })
     name, limit = card_power()

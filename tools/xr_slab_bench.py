@@ -13,7 +13,10 @@ round, the arms alternated twice in the same run):
   slab        one gs_render_scene_stereo_async per XR frame, on the slab path (GS_SLAB_MIN_XR=0);
   one_pass    the same frame on the one-pass path, in a context created with GS_SLAB_MIN_XR above N;
   mono2_slab  two gs_render_scene_async frames per XR frame, one per eye, each sorting itself and on the slab path, for
-              scale (its frames use each eye's own sort).
+              scale (its frames use each eye's own sort);
+  layer, stereo_copy  the slab stereo frame into one side-by-side device layer (RGBA8 colour plus f32 depth), in place
+              (gs_render_scene_stereo_target_async) or around six cudaMemcpy2DAsync copies (tools/xr_layer_arms.py); the
+              run also exits non-zero when the layer's eye rectangles differ from the stereo frame.
 Per workload the line also reports the slab counters (slabs scheduled and run, entries, instances of the eye pair), the
 stage times of un-overlapped frames and the SHA-256 of both eyes' frames per arm.  The run exits non-zero when the slab
 frame differs from the one-pass frame.  Prints one JSON line with the card name and power limit.
@@ -34,6 +37,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 from xr_bench import card_power  # noqa: E402
 
@@ -61,6 +65,7 @@ def main():
     sizes = [int(s) for s in args.splats.split(",")]
     gs = importlib.import_module("aframe-gaussian-splatting_b200")
     import poses
+    from xr_layer_arms import LayerArms
     sc = gs.scenes
     half = max(sizes) // 2
     # rows first: the generator forks worker processes, which must happen before this process owns a CUDA context
@@ -163,12 +168,17 @@ def main():
 
             arms = {"slab": ("slab", stereo_submit(ctx_s)), "one_pass": ("one_pass", stereo_submit(ctxs["one_pass"])),
                     "mono2_slab": ("slab", sub_mono2)}
-            rounds = {a: [] for a in arms}
-            for a, (cn, sub) in arms.items():
+            # the slab stereo frame into one side-by-side layer, in place or around the caller's six copies
+            la = LayerArms(gs, ctx_s, torch, dev, eyes, objs, eye_mvs, cols, deps, W, H)
+            timed_arms = dict(arms, layer=("slab", la.sub_layer), stereo_copy=("slab", la.sub_stereo_copy))
+            rounds = {a: [] for a in timed_arms}
+            for a, (cn, sub) in timed_arms.items():
                 pipe(ctxs[cn], streams[cn], sub, args.warmup + 3)
             for _ in range(2):  # alternated in the same run
-                for a, (cn, sub) in arms.items():
+                for a, (cn, sub) in timed_arms.items():
                     rounds[a].append(pipe(ctxs[cn], streams[cn], sub, args.steps))
+            layer_sha = la.check()
+            ok = ok and layer_sha["layer_equals_stereo"]
             med = {a: float(np.median(v)) for a, v in rounds.items()}
             # un-overlapped frames: stage times, counters and the frames themselves
             stages, counters, hashes = {}, {}, {}
@@ -192,6 +202,7 @@ def main():
                 "xr_frames_per_s": {a: 1000.0 / v for a, v in med.items()}, "ms_per_xr_frame": med, "rounds_ms": rounds,
                 "slab_over_one_pass": med["slab"] / med["one_pass"], "stages_ms": stages, "counters": counters,
                 "sha256": hashes, "slab_equals_one_pass": same,
+                "layer_over_stereo_copy": med["layer"] / med["stereo_copy"], "layer_sha256": layer_sha,
             })
             print(json.dumps({"progress": [n, W, H], "ms": med, "same": same}), file=sys.stderr, flush=True)
     name, limit = card_power()
@@ -202,7 +213,7 @@ def main():
     for c in ctxs.values():
         c.close()
     if not ok:
-        raise SystemExit("slab frames differ from one-pass frames")
+        raise SystemExit("slab frames differ from one-pass frames, or layer frames from stereo frames")
 
 
 if __name__ == "__main__":
