@@ -12,6 +12,7 @@ GS_OK, GS_ERR_INVALID, GS_ERR_CUDA, GS_ERR_OOM, GS_ERR_CAPACITY, GS_ERR_EMPTY = 
 GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F = 0, 1
 GS_RENDER_OUT_DEVICE, GS_RENDER_REUSE_SORT, GS_RENDER_OUT_TILED, GS_RENDER_OUT_PEER = 1, 2, 4, 8
 GS_RENDER_STATS, GS_RENDER_DEPTH_DEVICE, GS_RENDER_COLOR_DEVICE = 16, 32, 64
+GS_RENDER_BLEND_UNORM8 = 128
 GS_MAX_OBJECTS = 64
 GS_TARGET_DEVICE = 1
 

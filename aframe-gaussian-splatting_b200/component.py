@@ -366,21 +366,24 @@ class SplatScene:
 
     def render(self, width: int, height: int, camera=None, color_in: Optional[np.ndarray] = None,
                depth_in: Optional[np.ndarray] = None, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
-               out: Optional[np.ndarray] = None) -> np.ndarray:
+               out: Optional[np.ndarray] = None, blend_unorm8: bool = False) -> np.ndarray:
         """One frame of every entity over the colour target `color_in` ((H, W, 4) of the output dtype; None = bg) and
-        the window-space depth `depth_in` ((H, W) f32; None = no depth test).  Row 0 = bottom."""
+        the window-space depth `depth_in` ((H, W) f32; None = no depth test).  Row 0 = bottom.  blend_unorm8: the bytes
+        the page's RGBA8 target holds after the reference's blend, rounded after every fragment (GS_RENDER_BLEND_UNORM8)."""
         if not self.entities:
             raise ValueError("SplatScene.render: no entity added")
         frame, objs = self.objects(width, height, camera)
-        return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out)
+        return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out,
+                                          blend_unorm8=blend_unorm8)
 
     def render_into(self, color: np.ndarray, depth: Optional[np.ndarray] = None, viewport=(0, 0), width: Optional[int] = None,
-                    height: Optional[int] = None, camera=None, fmt: int = GS_FORMAT_RGBA8) -> np.ndarray:
+                    height: Optional[int] = None, camera=None, fmt: int = GS_FORMAT_RGBA8,
+                    blend_unorm8: bool = False) -> np.ndarray:
         """Draw every entity IN PLACE into the caller's framebuffer at a viewport rectangle, as the reference's draw does
         with the bound render target and renderer.setViewport (index.js:177-195).  color: (rows, pitch, 4) of the output
         dtype, row 0 = bottom; depth: (rows, pitch) f32 window-space depth or None.  viewport = (x, y) or (x, y, w, h) in
         CSS pixels: w x h (default: width x height, else the rest of the buffer) scaled by the first entity's pixelRatio
-        and floored, as render() sizes its frame.  Returns `color`."""
+        and floored, as render() sizes its frame.  blend_unorm8 as render().  Returns `color`."""
         if not self.entities:
             raise ValueError("SplatScene.render_into: no entity added")
         x, y = int(viewport[0]), int(viewport[1])
@@ -389,7 +392,8 @@ class SplatScene:
         width = color.shape[1] - x if width is None else width
         height = color.shape[0] - y if height is None else height
         frame, objs = self.objects(width, height, camera)
-        return self.renderer.render_scene_target(frame, objs, color, depth, viewport=(x, y), fmt=fmt)
+        return self.renderer.render_scene_target(frame, objs, color, depth, viewport=(x, y), fmt=fmt,
+                                                 blend_unorm8=blend_unorm8)
 
     def _xr_objects(self, eye_cameras, width: int, height: int):
         """(eye size, objects with head matrices, eye FrameInputs, per-eye entity modelviews) of a WebXR frame."""
@@ -408,21 +412,22 @@ class SplatScene:
         return (w, h), objs, eyes, eye_mvs
 
     def render_xr_layer(self, eye_cameras, width: int, height: int, color: np.ndarray, depth: Optional[np.ndarray] = None,
-                        fmt: int = GS_FORMAT_RGBA8) -> np.ndarray:
+                        fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False) -> np.ndarray:
         """WebXR presentation into the XR layer's one framebuffer, IN PLACE: both eyes side by side over one depth buffer,
         as three.js draws each eye camera of the session at its own viewport of the layer.  Eye size as render_xr (the
         native eye size scaled by the first entity's xrPixelRatio, floored): the left eye at (0, 0), the right at (w, 0).
         color: (rows, pitch, 4) of the output dtype with pitch >= 2w and rows >= h; depth: (rows, pitch) f32 or None.
-        Returns `color`."""
+        blend_unorm8 as render().  Returns `color`."""
         if not self.entities:
             raise ValueError("SplatScene.render_xr_layer: no entity added")
         (w, h), objs, eyes, eye_mvs = self._xr_objects(eye_cameras, width, height)
         if color.shape[1] < 2 * w or color.shape[0] < h:
             raise ValueError(f"render_xr_layer: the layer must hold two {w} x {h} eyes side by side")
-        return self.renderer.render_scene_stereo_target(eyes, objs, eye_mvs, color, depth, eye_xy=(0, 0, w, 0), fmt=fmt)
+        return self.renderer.render_scene_stereo_target(eyes, objs, eye_mvs, color, depth, eye_xy=(0, 0, w, 0), fmt=fmt,
+                                                        blend_unorm8=blend_unorm8)
 
     def render_xr(self, eye_cameras, width: int, height: int, color_in=(None, None), depth_in=(None, None),
-                  bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8):
+                  bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
         """WebXR presentation of every entity (index.js:13-15, 184-195, 438-455): one stereo frame
         (gs_render_scene_stereo).  Each entity's sort comes from its getModelViewMatrix() of the scene camera - the head
         pose its tick() uses - and each entity is drawn once per eye camera with that eye's matrices.
@@ -430,8 +435,9 @@ class SplatScene:
         GaussianSplattingComponent.render_xr does.  The ratio is the FIRST entity's xrPixelRatio (1 when it is not
         positive), by the rule of render(), whose shared viewport is the first entity's.
         color_in[e] / depth_in[e]: eye e's colour ((h, w, 4) of the output dtype) and window-space depth ((h, w) f32) at
-        the scaled size, or None.  Returns [left, right] frames, row 0 = bottom."""
+        the scaled size, or None.  blend_unorm8 as render().  Returns [left, right] frames, row 0 = bottom."""
         if not self.entities:
             raise ValueError("SplatScene.render_xr: no entity added")
         _, objs, eyes, eye_mvs = self._xr_objects(eye_cameras, width, height)
-        return self.renderer.render_scene_stereo(eyes, objs, eye_mvs, color_in=color_in, depth_in=depth_in, bg=bg, fmt=fmt)
+        return self.renderer.render_scene_stereo(eyes, objs, eye_mvs, color_in=color_in, depth_in=depth_in, bg=bg, fmt=fmt,
+                                                 blend_unorm8=blend_unorm8)

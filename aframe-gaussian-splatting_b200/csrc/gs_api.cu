@@ -990,7 +990,8 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
     cudaGraphExec_t &gr = sl.stereo ? sl.graph_xr[set] : (sl.peer ? sl.graph_rp[set] : sl.graph_r[set]);
     if ((rc = run_graph(c, gr, c->rstream, [&](bool ext) { return enqueue_raster_stage(c, sl, n_tiles, ext); }))) return rc;
   } else {
-    // depth-tested / statistics frames use other instantiations of the raster: plain launches, no cached graph
+    // depth-tested / statistics / GS_RENDER_BLEND_UNORM8 frames use other instantiations of the raster: plain launches, no
+    // cached graph (so a frame of one blend mode never replays a raster graph captured for the other)
     GS_CUDA(c, enqueue_raster_stage(c, sl, n_tiles, false));
   }
   sl.launches = (sl.scene ? 11u : (reuse ? 0u : 7u)) + 1u + (n_bins <= 256u ? 5u : 9u) + 1u;
@@ -1273,9 +1274,11 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
     return rcode;
   }
   if ((rcode = stage_inputs(c, sl, 0, p, fp))) return rcode;
-  // raster instantiation: pixel loop (two pixels per lane by default), depth test, statistics
+  // raster instantiation: pixel loop (two pixels per lane by default), depth test, statistics; GS_RENDER_BLEND_UNORM8
+  // frames always take the two-pixel loop of that mode (bit 3), whatever GS_RASTER says
   const bool depth = p->depth_in || (sl.target && sl.tdepth);  // a target's depth is that of both eyes
-  sl.raster_flags = c->raster_base_flags | (depth ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u);
+  const bool blend8 = (p->flags & GS_RENDER_BLEND_UNORM8) != 0;
+  sl.raster_flags = (blend8 ? 9u : c->raster_base_flags) | (depth ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u);
   if (sl.stereo) {
     // the pair of eye frames the stereo kernels read: eye 0 as above, eye 1 from its own parameters (same size and flags)
     StereoParams &st = *sl.stereo_host;
@@ -1446,6 +1449,15 @@ static int wait_overlapping(gs_context *c, const TargetInput &t, uint32_t w, uin
   }
 }
 
+// GS_RENDER_BLEND_UNORM8 stores RGBA8 bytes into a row-major frame: RGBA32F, tiled and peer output are refused
+static int check_blend8(gs_context *c, const gs_render_params *p) {
+  if (!(p->flags & GS_RENDER_BLEND_UNORM8)) return GS_OK;
+  if (p->out_format != GS_FORMAT_RGBA8) return fail(c, GS_ERR_INVALID, "GS_RENDER_BLEND_UNORM8 needs GS_FORMAT_RGBA8");
+  if (p->flags & (GS_RENDER_OUT_TILED | GS_RENDER_OUT_PEER))
+    return fail(c, GS_ERR_INVALID, "GS_RENDER_BLEND_UNORM8: GS_RENDER_OUT_TILED and _OUT_PEER are not accepted");
+  return GS_OK;
+}
+
 // gs_render_async, scene and stereo scene frames.  scene: the table built by build_scene_table (nullptr = a plain frame);
 // color_in: the colour target or nullptr; stereo: the second eye of a stereo scene frame (nullptr otherwise; p is eye 0);
 // target: the gs_target the frame is drawn into in place (nullptr otherwise; color_in is then nullptr and out_rgba the
@@ -1456,6 +1468,8 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
   if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+  int rcode;
+  if ((rcode = check_blend8(c, p))) return rcode;
   const uint32_t n_tiles = ((p->width + kTile - 1) / kTile) * ((p->height + kTile - 1) / kTile);
   const uint32_t n_bins = ((p->width + kBin - 1) / kBin) * ((p->height + kBin - 1) / kBin);  // <= 64*64: fits the 16-bit bin id
   // a stereo frame's bin table holds both eyes' bins (2 * 43 * 43 at most, still a 16-bit id)
@@ -1463,7 +1477,6 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   GS_CUDA(c, cudaSetDevice(c->device));
   const uint64_t ticket = c->next_ticket;
   gs_context::Slot &sl = c->slot[ticket % gs_context::kSlots];
-  int rcode;
   if (sl.pending && (rcode = wait_slot(c, sl, nullptr))) return rcode;  // slot reuse: its previous frame must be done
   if (target && (rcode = wait_overlapping(c, *target, p->width, p->height, stereo ? 2 : 1))) return rcode;
   if ((p->flags & GS_RENDER_OUT_PEER) && ticket >= 3) {
@@ -1482,8 +1495,10 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     for (uint32_t k = 0; k < scene->n; ++k) sortable += scene->obj[k].end - scene->obj[k].first;
   }
   const uint32_t expect_sorted = c->have_last_sorted ? c->last_sorted : sortable;
-  // stereo frames by their own threshold (GS_SLAB_MIN_XR); they accept neither flag
-  const bool slab = expect_sorted >= (stereo ? c->slab_min_xr : c->slab_min) && !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS));
+  // stereo frames by their own threshold (GS_SLAB_MIN_XR); they accept neither flag.  GS_RENDER_BLEND_UNORM8 frames are
+  // always one-pass: the slab path stops at front-to-back saturation, which rounding after every blend does not have
+  const bool slab = expect_sorted >= (stereo ? c->slab_min_xr : c->slab_min) &&
+                    !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS | GS_RENDER_BLEND_UNORM8));
   const uint32_t slab_tiles = stereo ? 2 * n_tiles : n_tiles;  // pixel state of both eyes
   if ((int)slab != c->last_mode) {
     if ((rcode = drain(c))) return rcode;
@@ -1700,7 +1715,10 @@ extern "C" int gs_render(gs_context *c, const gs_render_params *p, void *out_rgb
 extern "C" int gs_render_stereo(gs_context *c, const float view[4], const float *cutout16_or_null,
                                 const gs_render_params eyes[2], void *const out_rgba[2], gs_stats *stats2_or_null) {
   if (!c || !view || !eyes || !out_rgba || !out_rgba[0] || !out_rgba[1]) return GS_ERR_INVALID;
-  int rc = gs_sort(c, view, cutout16_or_null, nullptr, nullptr);
+  int rc;
+  for (int e = 0; e < 2; ++e)  // refused before the sort, so that a refusal changes nothing
+    if ((rc = check_blend8(c, &eyes[e]))) return rc;
+  rc = gs_sort(c, view, cutout16_or_null, nullptr, nullptr);
   if (rc) return rc;
   const float ms_sort = c->stats.ms_sort;
   for (int e = 0; e < 2; ++e) {
@@ -1733,8 +1751,10 @@ static int scene_stereo_async(gs_context *c, const gs_render_params eyes[2], con
     return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: GS_RENDER_REUSE_SORT, _STATS, _OUT_TILED and _OUT_PEER are not accepted");
   if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: not on a sharded context");
   if (eyes[1].out_format != GS_FORMAT_RGBA8 && eyes[1].out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+  int rc = check_blend8(c, &eyes[1]);
+  if (rc) return rc;
   size_t bytes = 0;
-  int rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
+  rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
   if (rc) return rc;
   // each entity's per-eye modelviews, in the table's order (caller's entity k = its draw rank)
   float mv[kMaxObjects][2][16];

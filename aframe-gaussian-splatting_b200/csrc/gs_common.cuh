@@ -572,6 +572,27 @@ __device__ __forceinline__ bool footprint_meets_box(float cx, float cy, float a1
   return !(qmin > 4.02f);  // NaN keeps
 }
 
+// expw(x) = exp(-x) for x = r^2 in [0, 4], as fixed IEEE fp32 operations in this order (GS_RENDER_BLEND_UNORM8 frames;
+// include/gsplat_b200.h states the same definition): k = rint(-x * log2(e)) in [-6, 0]; r = (-x - k * ln2_hi) - k * ln2_lo
+// (Cody-Waite: ln2_hi has 16 trailing zero bits, so k * ln2_hi is exact); p = Horner degree-7 Taylor polynomial of e^r,
+// |r| <= 0.35; result p * 2^k (exact).  Every op rounds to nearest on its own (no FMA, no ex2.approx), so a CPU restatement
+// gives the same bits; expw(0) = 1 exactly.  Over every fp32 x in [0, 4] it is within 1 ulp of exp(-x) (tests/test_blend8.py).
+__device__ __forceinline__ float expw(float x) {
+  const float t = -x;
+  const float k = rintf(__fmul_rn(t, 1.44269502e+00f));              // 0x3FB8AA3B
+  const float r = __fsub_rn(__fsub_rn(t, __fmul_rn(k, 6.93145752e-01f)),  // ln2_hi 0x3F317200
+                            __fmul_rn(k, 1.42860677e-06f));               // ln2_lo 0x35BFBE8E
+  float p = 1.98412701e-04f;                                           // 1/5040
+  p = __fadd_rn(__fmul_rn(p, r), 1.38888892e-03f);                     // 1/720
+  p = __fadd_rn(__fmul_rn(p, r), 8.33333377e-03f);                     // 1/120
+  p = __fadd_rn(__fmul_rn(p, r), 4.16666679e-02f);                     // 1/24
+  p = __fadd_rn(__fmul_rn(p, r), 1.66666672e-01f);                     // 1/6
+  p = __fadd_rn(__fmul_rn(p, r), 0.5f);
+  p = __fadd_rn(__fmul_rn(p, r), 1.0f);
+  p = __fadd_rn(__fmul_rn(p, r), 1.0f);
+  return __fmul_rn(p, __int_as_float((127 + (int)k) << 23));
+}
+
 // ---- multi-GPU ownership: rank r owns the BIN COLUMNS bx with bx % world == r (kBin-pixel wide vertical stripes,
 // interleaved), so the owned bins of any bin rectangle have a closed form; a tile belongs to the owner of its bin ----
 __host__ __device__ inline uint32_t owned_cols(uint32_t bins_x, uint32_t rank, uint32_t world) {

@@ -25,6 +25,8 @@
 //                          loads of a record, dx and the two products with dx, and the loop overhead (the kernel is
 //                          bound by issue slots).  Hopper has no packed fp32x2 instructions, so the pair's arithmetic
 //                          is two scalar ops of the same rounding (add2 / mul2 / fma2 below).
+// GS_RENDER_BLEND_UNORM8 frames (k_raster<true, .., B8 = true>) instead follow the reference's order: chunks farthest
+// first, kept records in draw order, every pair blended into the pixel's bytes and stored as UNORM8 (blend8 below).
 #include "gs_common.cuh"
 
 namespace gs {
@@ -141,6 +143,32 @@ __device__ __forceinline__ void store_pixel(const FrameParams *fp, uint32_t tile
   }
 }
 
+// GS_RENDER_BLEND_UNORM8: one pixel's RGBA8 destination d (each channel byte / 255, tab[b] = b / 255 correctly rounded)
+// after the reference's blend of one fragment of weight w and colour c (index.js:177-178), stored as UNORM8 like the
+// page's RGBA8 target does after every fragment: d <- q8(c * w + d * (1 - w)), a <- q8(w + a * (1 - w)), q8 = to_u8.
+// w = 0 leaves d unchanged (q8(b / 255) == b for every byte), so a pixel that does not take the fragment passes w = 0.
+__device__ __forceinline__ void blend8(float4 &d, float w, const float4 &c, const float *tab) {
+  const float om = __fsub_rn(1.0f, w);
+  d.x = tab[to_u8(__fadd_rn(__fmul_rn(c.x, w), __fmul_rn(d.x, om)))];
+  d.y = tab[to_u8(__fadd_rn(__fmul_rn(c.y, w), __fmul_rn(d.y, om)))];
+  d.z = tab[to_u8(__fadd_rn(__fmul_rn(c.z, w), __fmul_rn(d.z, om)))];
+  d.w = tab[to_u8(__fadd_rn(w, __fmul_rn(d.w, om)))];
+}
+
+// start state of a GS_RENDER_BLEND_UNORM8 pixel: the colour target's bytes, else the clear colour stored as bytes
+__device__ __forceinline__ float4 load_pixel8(const FrameParams *fp, uint32_t x, uint32_t y, bool inside, const float *tab) {
+  const RenderConsts &rc = fp->rc;
+  uint32_t v = to_u8(rc.bg[0]) | (to_u8(rc.bg[1]) << 8) | (to_u8(rc.bg[2]) << 16) | (to_u8(rc.bg[3]) << 24);
+  if (fp->color_in && inside) v = __ldg((const uint32_t *)fp->color_in + (size_t)y * rc.pitch + x);
+  return make_float4(tab[v & 255u], tab[(v >> 8) & 255u], tab[(v >> 16) & 255u], tab[v >> 24]);
+}
+
+// finished GS_RENDER_BLEND_UNORM8 pixel -> its bytes in out (row-major RGBA8 only: the flag refuses tiled and peer output)
+__device__ __forceinline__ void store_pixel8(const FrameParams *fp, uint32_t x, uint32_t y, bool inside, const float4 &d) {
+  if (!inside || (fp->overflow && *fp->overflow)) return;
+  ((uint32_t *)fp->out)[(size_t)y * fp->rc.pitch + x] = to_u8(d.x) | (to_u8(d.y) << 8) | (to_u8(d.z) << 16) | (to_u8(d.w) << 24);
+}
+
 #ifndef GS_RASTER_UNROLL
 #define GS_RASTER_UNROLL 2   // records per iteration of the packed pixel loop
 #endif
@@ -175,12 +203,16 @@ struct SlabIO {
 // eye's frame fp[eye] (output, colour target, depth target: an eye without one keeps the depth 1, which passes every
 // fragment the projection keeps) and bins from eye * n_bins on.  The pixel loop is the one of the plain frame.  With SLAB,
 // the pixel state and closed flag of eye e's tile t are those of slab tile e * n_tiles + t (the CTA's index).
-template <bool PACKED, bool DEPTH, bool STATS, bool SLAB = false, bool STEREO = false>
+// B8: GS_RENDER_BLEND_UNORM8 (packed loop, one pass): the reference's back-to-front blend with the RGBA8 store after every
+// fragment.  Chunks stream farthest first, the kept records are walked in draw order, every pair is blended (no stop rule:
+// rounding after each blend has no front-to-back form), and the pixel state is the destination's bytes (as byte / 255).
+template <bool PACKED, bool DEPTH, bool STATS, bool SLAB = false, bool STEREO = false, bool B8 = false>
 __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>::kMinBlocks) k_raster(const float4 *__restrict__ inst_rec,
                                                                         const uint2 *__restrict__ bin_range,
                                                                         const FrameParams *__restrict__ fp,
                                                                         uint4 *__restrict__ tile_stats, SlabIO slab) {
   static_assert(!STEREO || !STATS, "stereo frames take no statistics");
+  static_assert(!B8 || (PACKED && !SLAB), "blend8 frames take the packed one-pass loop");
   using Cfg = RasterCfg<PACKED>;
   constexpr int kThreads = Cfg::kThreads, kChunk = Cfg::kChunk, kStages = Cfg::kStages, kCv = Cfg::kCv;
   constexpr int kWarps = kThreads / 32;
@@ -192,6 +224,7 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   __shared__ __align__(8) uint64_t s_full[kStages];
   __shared__ uint32_t s_wcnt[kWarps];
   __shared__ uint32_t s_stat[4];
+  __shared__ float s_u8f[B8 ? 256 : 1];  // B8: byte -> byte / 255
 
   const uint32_t tile = blockIdx.x - eye * rc.n_tiles;
   const uint32_t stile = blockIdx.x;  // slab state index: the tile of a mono frame, eye * n_tiles + tile of a stereo one
@@ -235,12 +268,23 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     if (STATS) { s_stat[0] = 0; s_stat[1] = 0; s_stat[2] = 0; s_stat[3] = 0; }
   }
+  if (B8)
+    for (uint32_t i = tid; i < 256u; i += kThreads) s_u8f[i] = __fdiv_rn((float)i, 255.0f);
   __syncthreads();
 
-  // chunk k covers records [lo_k, hi_k) with hi_k = end - k*kChunk (nearest first)
+  // chunk k covers records [lo_k, hi_k) with hi_k = end - k*kChunk (nearest first); B8: lo_k = start + k*kChunk (farthest first)
+  auto chunk = [&](uint32_t k, uint32_t &lo, uint32_t &hi) {
+    if (B8) {
+      lo = start + k * kChunk;
+      hi = (end - lo > (uint32_t)kChunk) ? lo + kChunk : end;
+    } else {
+      hi = end - k * kChunk;
+      lo = (hi - start > (uint32_t)kChunk) ? hi - kChunk : start;
+    }
+  };
   auto issue = [&](uint32_t k) {
-    const uint32_t hi = end - k * kChunk;
-    const uint32_t lo = (hi - start > (uint32_t)kChunk) ? hi - kChunk : start;
+    uint32_t lo, hi;
+    chunk(k, lo, hi);
     const uint32_t bytes = (hi - lo) * 32u;
     uint64_t *bar = &s_full[k % kStages];
     mbar_expect_tx(bar, bytes);
@@ -267,6 +311,11 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
       lim0 = (inside0 && T0 >= kTStop) ? 4.0f : -1.0f;
     }
   }
+  float4 D0 = make_float4(0.f, 0.f, 0.f, 0.f), D1 = D0;  // B8: destination bytes / 255 of the pair
+  if (B8) {
+    D0 = load_pixel8(fp, x, y, inside0, s_u8f);
+    D1 = load_pixel8(fp, x, y + 1, inside1, s_u8f);
+  }
   const float2 fy2 = make_float2(fy, fy + 1.0f);
   uint32_t st_tests = 0, st_hits = 0, st_kept = 0;
   bool tile_alive = true;
@@ -275,8 +324,8 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   for (; k < n_chunks; ++k) {
     const uint32_t stage = k % kStages;
     mbar_wait(&s_full[stage], (k / kStages) & 1u);
-    const uint32_t hi = end - k * kChunk;
-    const uint32_t lo = (hi - start > (uint32_t)kChunk) ? hi - kChunk : start;
+    uint32_t lo, hi;
+    chunk(k, lo, hi);
     const uint32_t m = hi - lo;
     const float4 *rec = &s_rec[stage][0];
     // ---- 1. cull + convert: thread `tid` owns record `tid` of the chunk ----
@@ -318,8 +367,31 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
     }
     __syncthreads();
     if (STATS) st_kept += (tid == 0) ? kept : 0u;
-    // ---- 2. composite the kept records, nearest first ----
-    if (PACKED) {
+    // ---- 2. composite the kept records, nearest first (B8: blend them in draw order, farthest first) ----
+    if (B8) {
+      if (lim0 > 0.0f || lim1 > 0.0f) {
+        for (int j = 0; j < (int)kept; ++j) {
+          const float4 q0 = s_cv[j * kCv], q1 = s_cv[j * kCv + 1];
+          // r^2 exactly as the packed loop below
+          const float dx = __fadd_rn(fx, q0.x);
+          const float2 dy2 = add2(fy2, make_float2(q1.x, q1.x));
+          const float t = __fmul_rn(dx, q0.y), u = __fmul_rn(dx, q0.z);
+          const float2 px2 = fma2(dy2, make_float2(q1.y, q1.y), make_float2(t, t));
+          const float2 py2 = fma2(dy2, make_float2(q1.z, q1.z), make_float2(u, u));
+          const float2 r22 = fma2(py2, py2, mul2(px2, px2));
+          bool h0 = r22.x <= lim0, h1 = r22.y <= lim1;
+          if (DEPTH) { h0 = h0 && (q0.w <= d0); h1 = h1 && (q0.w <= d1); }
+          if (STATS) { st_tests += (lim0 > 0.f ? 1u : 0u) + (lim1 > 0.f ? 1u : 0u); st_hits += (h0 ? 1u : 0u) + (h1 ? 1u : 0u); }
+          if (h0 || h1) {
+            const float w0 = h0 ? __fmul_rn(expw(r22.x), q1.w) : 0.0f;  // index.js:173
+            const float w1 = h1 ? __fmul_rn(expw(r22.y), q1.w) : 0.0f;
+            const float4 q2 = s_cv[j * kCv + 2];
+            blend8(D0, w0, q2, s_u8f);
+            blend8(D1, w1, q2, s_u8f);
+          }
+        }
+      }
+    } else if (PACKED) {
       if (lim0 > 0.0f || lim1 > 0.0f) {
 #pragma unroll kPackedUnroll
         for (int j = (int)kept - 1; j >= 0; --j) {
@@ -403,6 +475,9 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
       slab.closed[stile] = 1;
       if (atomicSub(&slab.bin_open[bin], 1u) == 1u) atomicSub(&slab.ctr->open_bins, 1u);
     }
+  } else if (B8) {
+    store_pixel8(fp, x, y, inside0, D0);
+    store_pixel8(fp, x, y + 1, inside1, D1);
   } else if (PACKED) {
     store_pixel(fp, tile, tx, ty, lx, ly, x, y, inside0, T2.x, R2.x, G2.x, B2.x);
     store_pixel(fp, tile, tx, ty, lx, ly + 1, x, y + 1, inside1, T2.y, R2.y, G2.y, B2.y);
@@ -476,10 +551,24 @@ __global__ void __launch_bounds__(256) k_assemble(const void *__restrict__ gathe
   else ((float4 *)out)[dst] = ((const float4 *)gathered)[src];
 }
 
-// flags: bit 0 = packed pixel loop, bit 1 = depth test against fp->depth_in, bit 2 = per-tile statistics
+// flags: bit 0 = packed pixel loop, bit 1 = depth test against fp->depth_in, bit 2 = per-tile statistics,
+// bit 3 = GS_RENDER_BLEND_UNORM8 (always the packed loop)
 void launch_raster(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags,
                    cudaStream_t st) {
   uint4 *ts = c->tile_stats;
+  constexpr int kT = RasterCfg<true>::kThreads;
+  if (flags & 8u) {
+    switch ((flags >> 1) & 3u) {
+#define GS_RASTER_CASE(v, D, S) \
+  case v: k_raster<true, D, S, false, false, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, ts, SlabIO{}); break;
+      GS_RASTER_CASE(0, false, false)
+      GS_RASTER_CASE(1, true, false)
+      GS_RASTER_CASE(2, false, true)
+      GS_RASTER_CASE(3, true, true)
+#undef GS_RASTER_CASE
+    }
+    return;
+  }
   switch (flags & 7u) {
 #define GS_RASTER_CASE(v, P, D, S) \
   case v: k_raster<P, D, S><<<n_tiles, RasterCfg<P>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, ts, SlabIO{}); break;
@@ -497,6 +586,12 @@ void launch_raster(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const
 
 void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags,
                           cudaStream_t st) {
+  constexpr int kT = RasterCfg<true>::kThreads;
+  if (flags & 8u) {
+    if (flags & 2u) k_raster<true, true, false, false, true, true><<<2 * n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{});
+    else k_raster<true, false, false, false, true, true><<<2 * n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{});
+    return;
+  }
   switch (flags & 3u) {
 #define GS_RASTER_CASE(v, P, D) \
   case v: k_raster<P, D, false, false, true><<<2 * n_tiles, RasterCfg<P>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{}); break;

@@ -10,7 +10,7 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _lib
-from ._lib import (GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F, GS_RENDER_OUT_DEVICE, GS_RENDER_OUT_TILED,
+from ._lib import (GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F, GS_RENDER_BLEND_UNORM8, GS_RENDER_OUT_DEVICE, GS_RENDER_OUT_TILED,
                    GS_RENDER_REUSE_SORT, GS_RENDER_STATS, GS_TARGET_DEVICE, GsObject, GsRenderParams, GsStats, GsTarget)
 from .scenes import FrameInputs
 
@@ -23,6 +23,10 @@ class GsError(RuntimeError):
 
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _blend8(on: bool) -> int:
+    return GS_RENDER_BLEND_UNORM8 if on else 0
 
 
 @dataclass
@@ -187,14 +191,16 @@ class SplatContext:
         return p
 
     def render(self, frame: FrameInputs, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8, out: Optional[np.ndarray] = None,
-               reuse_sort: bool = False, depth_in: Optional[np.ndarray] = None, stats: bool = False) -> np.ndarray:
-        """One frame into host memory: (H, W, 4) uint8 or float32, row 0 = bottom (GL orientation)."""
+               reuse_sort: bool = False, depth_in: Optional[np.ndarray] = None, stats: bool = False,
+               blend_unorm8: bool = False) -> np.ndarray:
+        """One frame into host memory: (H, W, 4) uint8 or float32, row 0 = bottom (GL orientation).
+        blend_unorm8: GS_RENDER_BLEND_UNORM8, the RGBA8 target's blend rounded after every fragment (RGBA8 only)."""
         dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
         if out is None:
             out = np.empty((frame.height, frame.width, 4), dtype)
         assert out.dtype == dtype and out.size == frame.height * frame.width * 4 and out.flags["C_CONTIGUOUS"]
-        p = self.make_params(frame, bg, fmt, (GS_RENDER_REUSE_SORT if reuse_sort else 0) | (GS_RENDER_STATS if stats else 0),
-                             depth_in=depth_in)
+        p = self.make_params(frame, bg, fmt, (GS_RENDER_REUSE_SORT if reuse_sort else 0) | (GS_RENDER_STATS if stats else 0) |
+                             _blend8(blend_unorm8), depth_in=depth_in)
         st = GsStats()
         self._check(self._lib.gs_render(self._h, C.byref(p), _ptr(out), C.byref(st)))
         self.last_stats = st
@@ -202,10 +208,11 @@ class SplatContext:
 
     def render_scene(self, frame: FrameInputs, objects: Sequence[SceneObject], bg=(0.0, 0.0, 0.0, 0.0),
                      fmt: int = GS_FORMAT_RGBA8, color_in: Optional[np.ndarray] = None,
-                     depth_in: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None, stats: bool = False) -> np.ndarray:
+                     depth_in: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None, stats: bool = False,
+                     blend_unorm8: bool = False) -> np.ndarray:
         """gs_render_scene: several entities in one frame, drawn whole in the order given, over `color_in` (the scene's
         colour buffer, (H, W, 4) of the output dtype, row 0 = bottom; None = bg) and depth-tested against `depth_in`.
-        `frame` supplies projection, size and focal; its modelview and cutout are ignored."""
+        `frame` supplies projection, size and focal; its modelview and cutout are ignored.  blend_unorm8 as render()."""
         dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
         if out is None:
             out = np.empty((frame.height, frame.width, 4), dtype)
@@ -215,7 +222,7 @@ class SplatContext:
             col = np.ascontiguousarray(color_in, dtype=dtype)
             if col.size != frame.width * frame.height * 4:
                 raise ValueError("color_in must hold width*height RGBA pixels")
-        p = self.make_params(frame, bg, fmt, GS_RENDER_STATS if stats else 0, depth_in=depth_in)
+        p = self.make_params(frame, bg, fmt, (GS_RENDER_STATS if stats else 0) | _blend8(blend_unorm8), depth_in=depth_in)
         objs = make_objects(objects)
         st = GsStats()
         self._check(self._lib.gs_render_scene(self._h, C.byref(p), objs, len(objects), _ptr(col), _ptr(out), C.byref(st)))
@@ -241,14 +248,14 @@ class SplatContext:
         return out[:cnt.value].copy()
 
     def render_stereo(self, view: np.ndarray, eyes, cutout: Optional[np.ndarray] = None, bg=(0.0, 0.0, 0.0, 0.0),
-                      fmt: int = GS_FORMAT_RGBA8):
+                      fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
         """gs_render_stereo: one sort with the head camera's `view` (+ cutout), one draw per eye (two FrameInputs).
-        Returns the two frames, row 0 = bottom."""
+        Returns the two frames, row 0 = bottom.  blend_unorm8 as render()."""
         assert len(eyes) == 2
         dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
         outs = [np.empty((e.height, e.width, 4), dtype) for e in eyes]
         arr = (GsRenderParams * 2)()
-        keep = [self.make_params(e, bg, fmt, 0) for e in eyes]
+        keep = [self.make_params(e, bg, fmt, _blend8(blend_unorm8)) for e in eyes]
         for i in range(2):
             C.memmove(C.addressof(arr[i]), C.addressof(keep[i]), C.sizeof(GsRenderParams))
         ptrs = (C.c_void_p * 2)(outs[0].ctypes.data, outs[1].ctypes.data)
@@ -276,11 +283,13 @@ class SplatContext:
         return arr, make_objects(objects), mv, col, outs
 
     def render_scene_stereo(self, eyes: Sequence[FrameInputs], objects: Sequence[SceneObject], eye_modelviews,
-                            color_in=(None, None), depth_in=(None, None), bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8):
+                            color_in=(None, None), depth_in=(None, None), bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
+                            blend_unorm8: bool = False):
         """gs_render_scene_stereo: one WebXR frame of a multi-entity page.  `objects` carry each entity's range, HEAD
         modelview (its sort) and cutout, in draw order; eyes[e] (FrameInputs) gives eye e's projection, size and focal;
         eye_modelviews[e][k] is entity k's modelview of eye e.  color_in[e] / depth_in[e]: eye e's colour target ((H, W, 4)
-        of the output dtype) and window-space depth ((H, W) f32), or None.  Returns the two frames, row 0 = bottom."""
+        of the output dtype) and window-space depth ((H, W) f32), or None.  Returns the two frames, row 0 = bottom.
+        blend_unorm8 as render()."""
         assert len(eyes) == 2
         dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
         outs = [np.empty((e.height, e.width, 4), dtype) for e in eyes]
@@ -291,7 +300,7 @@ class SplatContext:
                 if c.size != e.width * e.height * 4:
                     raise ValueError("color_in must hold width*height RGBA pixels")
             cols.append(c)
-        params = [self.make_params(e, bg, fmt, 0, depth_in=d) for e, d in zip(eyes, depth_in)]
+        params = [self.make_params(e, bg, fmt, _blend8(blend_unorm8), depth_in=d) for e, d in zip(eyes, depth_in)]
         arr, objs, mv, col, ptrs = self._stereo_args(params, objects, eye_modelviews,
                                                      [None if c is None else c.ctypes.data for c in cols],
                                                      [o.ctypes.data for o in outs])
@@ -336,12 +345,13 @@ class SplatContext:
 
     def render_scene_target(self, frame: FrameInputs, objects: Sequence[SceneObject], color: np.ndarray,
                             depth: Optional[np.ndarray] = None, viewport=(0, 0), fmt: int = GS_FORMAT_RGBA8,
-                            stats: bool = False) -> np.ndarray:
+                            stats: bool = False, blend_unorm8: bool = False) -> np.ndarray:
         """gs_render_scene_target: the scene frame blended IN PLACE into the rectangle of frame.width x frame.height at
         viewport = (x, y) of `color` ((rows, pitch, 4), row 0 = bottom), depth-tested against `depth` ((rows, pitch) f32
-        window-space depth, or None).  Nothing outside the rectangle is read or written.  Returns `color`."""
+        window-space depth, or None).  Nothing outside the rectangle is read or written.  Returns `color`.
+        blend_unorm8 as render()."""
         t = self._host_target(color, depth, fmt)
-        p = self.make_params(frame, fmt=fmt, flags=GS_RENDER_STATS if stats else 0)
+        p = self.make_params(frame, fmt=fmt, flags=(GS_RENDER_STATS if stats else 0) | _blend8(blend_unorm8))
         st = GsStats()
         self._check(self._lib.gs_render_scene_target(self._h, C.byref(p), make_objects(objects), len(objects), C.byref(t),
                                                      int(viewport[0]), int(viewport[1]), C.byref(st)))
@@ -359,20 +369,20 @@ class SplatContext:
 
     def render_scene_stereo_target(self, eyes: Sequence[FrameInputs], objects: Sequence[SceneObject], eye_modelviews,
                                    color: np.ndarray, depth: Optional[np.ndarray] = None, eye_xy=None,
-                                   fmt: int = GS_FORMAT_RGBA8) -> np.ndarray:
+                                   fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False) -> np.ndarray:
         """gs_render_scene_stereo_target: one WebXR frame drawn IN PLACE into one layer ((rows, pitch, 4) colour, optional
         (rows, pitch) f32 depth): eye e at (eye_xy[2e], eye_xy[2e+1]); eye_xy None = side by side, (0, 0, w, 0).
         Arguments as render_scene_stereo.  Returns `color`."""
         t = self._host_target(color, depth, fmt)
         st = GsStats()
-        args = self._stereo_target_args(eyes, fmt, objects, eye_modelviews, eye_xy)
+        args = self._stereo_target_args(eyes, fmt, objects, eye_modelviews, eye_xy, _blend8(blend_unorm8))
         self._check(self._lib.gs_render_scene_stereo_target(self._h, args[0], args[1], args[2], len(objects), C.byref(t),
                                                             args[3], C.byref(st)))
         self.last_stats = st
         return color
 
-    def _stereo_target_args(self, eyes, fmt, objects, eye_modelviews, eye_xy):
-        params = [e if isinstance(e, GsRenderParams) else self.make_params(e, fmt=fmt) for e in eyes]
+    def _stereo_target_args(self, eyes, fmt, objects, eye_modelviews, eye_xy, flags: int = 0):
+        params = [e if isinstance(e, GsRenderParams) else self.make_params(e, fmt=fmt, flags=flags) for e in eyes]
         arr, objs, mv, _, _ = self._stereo_args(params, objects, eye_modelviews, None, [0, 0])
         if eye_xy is None:
             eye_xy = (0, 0, params[0].width, 0)

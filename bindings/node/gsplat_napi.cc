@@ -16,6 +16,8 @@ class Splats : public Napi::ObjectWrap<Splats> {
       InstanceMethod("renderScene", &Splats::RenderScene), InstanceMethod("insert", &Splats::Insert),
       InstanceMethod("insertPly", &Splats::InsertPly), InstanceMethod("erase", &Splats::Erase),
       InstanceMethod("renderSceneXR", &Splats::RenderSceneXR)}));
+    // the RGBA8 target's per-fragment rounding: frame objects take `blendUnorm8: true` (GS_RENDER_BLEND_UNORM8)
+    exports.Set("BLEND_UNORM8", Napi::Number::New(env, GS_RENDER_BLEND_UNORM8));
     return exports;
   }
   explicit Splats(const Napi::CallbackInfo& i) : Napi::ObjectWrap<Splats>(i) {
@@ -25,6 +27,10 @@ class Splats : public Napi::ObjectWrap<Splats> {
   ~Splats() { gs_destroy(ctx_); }
  private:
   void Check(Napi::Env e, int rc) { if (rc != GS_OK) Napi::Error::New(e, gs_last_error(ctx_)).ThrowAsJavaScriptException(); }
+  // {blendUnorm8: true}: the bytes the page's RGBA8 framebuffer holds after the reference's blend, rounded per fragment
+  static uint32_t Blend8(const Napi::Object& o) {
+    return (o.Has("blendUnorm8") && o.Get("blendUnorm8").ToBoolean().Value()) ? (uint32_t)GS_RENDER_BLEND_UNORM8 : 0u;
+  }
   Napi::Value Clear(const Napi::CallbackInfo& i) { Check(i.Env(), gs_clear(ctx_)); return i.Env().Undefined(); }
   // reserve(numVertexes)                           <- initGL(numVertexes), index.js:248-251
   Napi::Value Reserve(const Napi::CallbackInfo& i) {
@@ -73,7 +79,8 @@ class Splats : public Napi::ObjectWrap<Splats> {
     Check(i.Env(), gs_sort(ctx_, view.Data(), cut, out.Data(), &cnt));
     return Napi::Uint32Array::New(i.Env(), cnt, out.ArrayBuffer(), 0);
   }
-  // render({proj, modelview, width, height, focal, cutout?, bg?, depth?: Float32Array}, Uint8Array out)  <- onBeforeRender + draw
+  // render({proj, modelview, width, height, focal, cutout?, bg?, depth?: Float32Array, blendUnorm8?}, Uint8Array out)
+  //                                                <- onBeforeRender + draw
   Napi::Value Render(const Napi::CallbackInfo& i) {
     auto o = i[0].As<Napi::Object>();
     gs_render_params p{};
@@ -85,10 +92,11 @@ class Splats : public Napi::ObjectWrap<Splats> {
     if (o.Has("cutout")) { p.has_cutout = 1; memcpy(p.cutout16, o.Get("cutout").As<Napi::Float32Array>().Data(), 64); }
     if (o.Has("depth")) p.depth_in = o.Get("depth").As<Napi::Float32Array>().Data();  // gl.readPixels(DEPTH) of the scene so far
     p.out_format = GS_FORMAT_RGBA8;
+    p.flags = Blend8(o);
     Check(i.Env(), gs_render(ctx_, &p, i[1].As<Napi::Uint8Array>().Data(), nullptr));
     return i.Env().Undefined();
   }
-  // renderScene({proj, width, height, focal, depth?: Float32Array}, [{first, count, modelview, cutout?}, ...], Uint8Array color,
+  // renderScene({proj, width, height, focal, depth?: Float32Array, blendUnorm8?}, [{first, count, modelview, cutout?}, ...], Uint8Array color,
   //             Uint8Array out)  <- the draws of every gaussian_splatting entity of the page, in DOM order (sortObjects false),
   // over the opaque pass: color = gl.readPixels(RGBA, UNSIGNED_BYTE) and depth = the window-space depth buffer read back
   // after the spheres and sky were drawn; each entity's {first, count} is its range of the shared table (filled by
@@ -102,6 +110,7 @@ class Splats : public Napi::ObjectWrap<Splats> {
     p.focal = o.Get("focal").As<Napi::Number>().FloatValue();
     if (o.Has("depth")) p.depth_in = o.Get("depth").As<Napi::Float32Array>().Data();
     p.out_format = GS_FORMAT_RGBA8;
+    p.flags = Blend8(o);
     auto list = i[1].As<Napi::Array>();
     std::vector<gs_object> objs(list.Length());
     for (uint32_t k = 0; k < list.Length(); ++k) {
@@ -117,7 +126,7 @@ class Splats : public Napi::ObjectWrap<Splats> {
     Check(i.Env(), gs_render_scene(ctx_, &p, objs.data(), (uint32_t)objs.size(), color, i[3].As<Napi::Uint8Array>().Data(), nullptr));
     return i.Env().Undefined();
   }
-  // renderSceneXR([eyeL, eyeR] {proj, width, height, focal, x, y}, [{first, count, modelview, cutout?,
+  // renderSceneXR([eyeL, eyeR] {proj, width, height, focal, x, y, blendUnorm8?}, [{first, count, modelview, cutout?,
   //                eyeModelviews: [Float32Array, Float32Array]}, ...], layer {color: Uint8Array, depth?: Float32Array, pitch,
   //                rows})  <- an XR frame of every entity of the page, drawn IN PLACE into the XR layer's one framebuffer:
   // each entity's tick() sort from the head camera (modelview = its getModelViewMatrix()), its draw once per eye with
@@ -135,6 +144,7 @@ class Splats : public Napi::ObjectWrap<Splats> {
       eyes[e].height = o.Get("height").As<Napi::Number>().Uint32Value();
       eyes[e].focal = o.Get("focal").As<Napi::Number>().FloatValue();
       eyes[e].out_format = GS_FORMAT_RGBA8;
+      eyes[e].flags = Blend8(o);
       eye_xy[2 * e] = o.Get("x").As<Napi::Number>().Uint32Value();
       eye_xy[2 * e + 1] = o.Get("y").As<Napi::Number>().Uint32Value();
     }

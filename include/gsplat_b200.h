@@ -68,8 +68,34 @@ enum {
                                      instances and pixel-splat pair counters (a diagnostic frame: the raster
                                      keeps culling closed tiles' lists, so it is slower than a plain frame)  */
   GS_RENDER_DEPTH_DEVICE = 1u << 5, /* gs_render_params.depth_in is a device pointer (default: host memory) */
-  GS_RENDER_COLOR_DEVICE = 1u << 6  /* gs_render_scene*: color_in is a device pointer (default: host memory)   */
+  GS_RENDER_COLOR_DEVICE = 1u << 6, /* gs_render_scene*: color_in is a device pointer (default: host memory)   */
+  GS_RENDER_BLEND_UNORM8 = 1u << 7  /* RGBA8 frames whose bytes are those an RGBA8 framebuffer holds after the
+                                       reference's back-to-front blend, rounded after every fragment (below)    */
 };
+
+/*
+ * GS_RENDER_BLEND_UNORM8: the blend of the page's RGBA8 target.  The default raster composites front to back in fp32,
+ * stops a pixel once its transmittance falls below 3e-4 and rounds once at the end.  A WebGL RGBA8 framebuffer instead
+ * stores every fragment's blend (index.js:177-181) as 8 bits before the next one reads it.  With this flag:
+ *   - coverage, depth test and draw order are those of the default frame: a (pixel, splat) pair is blended iff the default
+ *     frame blends it (same fp32 r^2, r^2 <= 4, LEQUAL against depth_in or the target's depth);
+ *   - each pixel starts as bytes: the colour target's (color_in, gs_target), else q8(bg_rgba) (a clear of an RGBA8 target);
+ *   - every blended pair, in draw order (farthest first), with d = current byte / 255 (correctly rounded), a = the splat's
+ *     alpha byte / 255 and c its colour bytes / 255, each operation one fp32 rounding:
+ *       w = expw(r^2) * a;  om = 1 - w;  rgb' = q8(c * w + d * om);  a' = q8(w + d.a * om)
+ *   - q8(x) = floor(clamp(x, 0, 1) * 255 + 0.5), NaN -> 0: OpenGL ES 3.0's float-to-normalized conversion with its
+ *     preferred round-to-nearest (the mode models that rounding; it does not claim a particular browser or GPU does it);
+ *   - no stop rule: rounding after every blend has no exact front-to-back form, so every pair is blended;
+ *   - expw(x) = exp(-x) for x in [0, 4], fixed fp32 operations in this order (no FMA): k = rint(-x * 0x1.715476p+0);
+ *     r = (-x - k * 0x1.62e4p-1) - k * 0x1.7f7d1cp-20; p = Horner of 1 + r + r^2/2! + ... + r^7/7! from the r^7 term
+ *     (coefficients the fp32 values nearest 1/7! ... 1/2!, then 1, 1); expw = p * 2^k.  expw(0) = 1.
+ * Accepted by gs_render[_async], gs_render_stereo, gs_render_scene[_async], gs_render_scene_stereo[_async] and both
+ * *_target[_async] entry points, with GS_RENDER_REUSE_SORT and GS_RENDER_STATS where those accept them, depth and colour
+ * targets and host or device buffers.  Such a frame is always one-pass (never the slab path, whatever GS_SLAB_MIN /
+ * GS_SLAB_MIN_XR say: gs_stats.n_slabs is 0) and always uses the two-pixel raster loop (GS_RASTER=scalar does not apply).
+ * GS_RENDER_STATS counts this loop's pairs: n_pair_hits is every blended pair.  Refused with GS_ERR_INVALID, changing
+ * nothing: GS_FORMAT_RGBA32F, GS_RENDER_OUT_TILED and GS_RENDER_OUT_PEER.
+ */
 
 /* Per-frame counters (SURVEY.md 8d symbols) and device timings of the last gs_sort/gs_render */
 typedef struct gs_stats {
