@@ -14,6 +14,7 @@ GS_RENDER_OUT_DEVICE, GS_RENDER_REUSE_SORT, GS_RENDER_OUT_TILED, GS_RENDER_OUT_P
 GS_RENDER_STATS, GS_RENDER_DEPTH_DEVICE, GS_RENDER_COLOR_DEVICE = 16, 32, 64
 GS_RENDER_BLEND_UNORM8 = 128
 GS_MAX_OBJECTS = 64
+GS_MAX_VIEWS = 4
 GS_TARGET_DEVICE = 1
 
 
@@ -98,6 +99,17 @@ SYMBOLS = {
                                                       C.POINTER(C.c_uint64)]),
     "gs_render_scene_stereo_target": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.POINTER(C.c_float),
                                                 C.c_uint32, C.POINTER(GsTarget), C.POINTER(C.c_uint32), C.POINTER(GsStats)]),
+    "gs_render_scene_views_async": (C.c_int, [_P, C.POINTER(GsRenderParams), C.c_uint32, C.POINTER(GsObject),
+                                              C.POINTER(C.c_float), C.c_uint32, C.POINTER(_P), C.POINTER(_P),
+                                              C.POINTER(C.c_uint64)]),
+    "gs_render_scene_views": (C.c_int, [_P, C.POINTER(GsRenderParams), C.c_uint32, C.POINTER(GsObject), C.POINTER(C.c_float),
+                                        C.c_uint32, C.POINTER(_P), C.POINTER(_P), C.POINTER(GsStats)]),
+    "gs_render_scene_views_target_async": (C.c_int, [_P, C.POINTER(GsRenderParams), C.c_uint32, C.POINTER(GsObject),
+                                                     C.POINTER(C.c_float), C.c_uint32, C.POINTER(GsTarget),
+                                                     C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
+    "gs_render_scene_views_target": (C.c_int, [_P, C.POINTER(GsRenderParams), C.c_uint32, C.POINTER(GsObject),
+                                               C.POINTER(C.c_float), C.c_uint32, C.POINTER(GsTarget), C.POINTER(C.c_uint32),
+                                               C.POINTER(GsStats)]),
     "gs_read_projected": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
     "gs_get_stats": (C.c_int, [_P, C.POINTER(GsStats)]),
     "gs_set_shard": (C.c_int, [_P, C.c_uint32, C.c_uint32]),

@@ -29,6 +29,12 @@ from ._lib import GS_FORMAT_RGBA8
 ROW_LENGTH = 3 * 4 + 3 * 4 + 4 + 4  # index.js:227
 
 
+def xr_viewports(viewports, ratio: float):
+    """Native XR view rectangles (x, y, w, h), as XRWebGLLayer.getViewport(view) gives them, at the layer's scaled size:
+    every component times `ratio` (xrPixelRatio), floored - the rule render_xr applies to the eye size."""
+    return [tuple(int(math.floor(c * ratio)) for c in vp) for vp in viewports]
+
+
 class SortWorker:
     """The Web Worker's message protocol (index.js:572-598) served by the GPU context.
 
@@ -395,21 +401,53 @@ class SplatScene:
         return self.renderer.render_scene_target(frame, objs, color, depth, viewport=(x, y), fmt=fmt,
                                                  blend_unorm8=blend_unorm8)
 
+    def _xr_ratio(self) -> float:
+        """The first entity's xrPixelRatio, 1 when it is not positive (the rule of render_xr)."""
+        ratio = float(self.entities[0].data.get("xrPixelRatio") or 0)
+        return ratio if ratio > 0 else 1.0
+
     def _xr_objects(self, eye_cameras, width: int, height: int):
         """(eye size, objects with head matrices, eye FrameInputs, per-eye entity modelviews) of a WebXR frame."""
         assert len(eye_cameras) == 2
-        ratio = float(self.entities[0].data.get("xrPixelRatio") or 0)
-        if ratio <= 0:
-            ratio = 1.0
+        ratio = self._xr_ratio()
         w, h = int(math.floor(width * ratio)), int(math.floor(height * ratio))
+        objs, eyes, eye_mvs = self._xr_view_objects(eye_cameras, [(w, h), (w, h)])
+        return (w, h), objs, eyes, eye_mvs
+
+    def _xr_view_objects(self, view_cameras, sizes):
+        """(objects with head matrices, view FrameInputs, per-view entity modelviews) of a WebXR frame whose view v is
+        sizes[v] = (w, h) pixels; the head's matrices are taken at view 0's size."""
         objs = []
         for e in self.entities:
-            head = e._frame_inputs_px(w, h)
+            head = e._frame_inputs_px(*sizes[0])
             objs.append(SceneObject(*self.range_of(e), head.modelview, head.cutout))
-        eye_frames = [[e._frame_inputs_px(w, h, cam) for e in self.entities] for cam in eye_cameras]
-        eyes = [frames[0] for frames in eye_frames]
-        eye_mvs = [[f.modelview for f in frames] for frames in eye_frames]
-        return (w, h), objs, eyes, eye_mvs
+        view_frames = [[e._frame_inputs_px(w, h, cam) for e in self.entities] for cam, (w, h) in zip(view_cameras, sizes)]
+        views = [frames[0] for frames in view_frames]
+        view_mvs = [[f.modelview for f in frames] for frames in view_frames]
+        return objs, views, view_mvs
+
+    def render_xr_views(self, view_cameras, viewports, width: int, height: int, color: np.ndarray,
+                        depth: Optional[np.ndarray] = None, fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False) -> np.ndarray:
+        """WebXR presentation of every view of the viewer pose (1..4: two eyes plus an observer, or a quad-view device's
+        four) into the XR layer's one framebuffer, IN PLACE, from one head sort (gs_render_scene_views_target).
+        viewports[v] = (x, y, w, h): view v's native rectangle, as XRWebGLLayer.getViewport(view) gives it, in a layer of
+        width x height native pixels.  Every component is scaled by the first entity's xrPixelRatio and floored
+        (xr_viewports), as render_xr_layer sizes its eyes; two side-by-side viewports reproduce render_xr_layer.
+        color: (rows, pitch, 4) of the output dtype holding the scaled layer; depth: (rows, pitch) f32 or None.
+        blend_unorm8 as render().  Returns `color`."""
+        if not self.entities:
+            raise ValueError("SplatScene.render_xr_views: no entity added")
+        if len(view_cameras) != len(viewports):
+            raise ValueError("render_xr_views: one viewport per view camera")
+        ratio = self._xr_ratio()
+        rects = xr_viewports(viewports, ratio)
+        lw, lh = int(math.floor(width * ratio)), int(math.floor(height * ratio))
+        if color.shape[1] < lw or color.shape[0] < lh:
+            raise ValueError(f"render_xr_views: the layer must hold {lw} x {lh} pixels")
+        objs, views, view_mvs = self._xr_view_objects(view_cameras, [(w, h) for _, _, w, h in rects])
+        xy = [c for x, y, _, _ in rects for c in (x, y)]
+        return self.renderer.render_scene_views_target(views, objs, view_mvs, color, xy, depth, fmt=fmt,
+                                                       blend_unorm8=blend_unorm8)
 
     def render_xr_layer(self, eye_cameras, width: int, height: int, color: np.ndarray, depth: Optional[np.ndarray] = None,
                         fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False) -> np.ndarray:

@@ -125,23 +125,30 @@ static int ensure_slot_scene(gs_context *c, gs_context::Slot &sl) {
   return GS_OK;
 }
 
-// the second eye's records and rectangles of stereo scene frames, sized like the per-splat scratch; allocated by the first
-// stereo frame (the pipeline is idle)
-static int ensure_stereo_bufs(gs_context *c) {
-  if (c->stereo_cap >= c->cap && c->proj_rec1[0]) return GS_OK;
+// records and rectangles of views 1.. of views scene frames, each view's sized like the per-splat scratch (rounded up to
+// 4 splats: the projection clears 4 rectangles per store); allocated by the first views frame and grown to the largest
+// view count drawn since (the pipeline is idle)
+static bool stereo_bufs_ok(const gs_context *c, uint32_t n_views) {
+  return n_views <= 1 || (c->stereo_cap >= c->cap && c->stereo_views >= n_views - 1 && c->proj_recx[0]);
+}
+static int ensure_stereo_bufs(gs_context *c, uint32_t n_views) {
+  if (stereo_bufs_ok(c, n_views)) return GS_OK;
+  const uint32_t views = std::max(c->stereo_views, n_views - 1);
+  const size_t stride = ((size_t)c->cap + 3) & ~(size_t)3;
   for (int i = 0; i < 2; ++i) {
-    dev_free(c->proj_rec1[i]); dev_free(c->rect1[i]);
-    GS_CUDA(c, dev_alloc(&c->proj_rec1[i], 2 * (size_t)c->cap));
-    GS_CUDA(c, dev_alloc(&c->rect1[i], (size_t)c->cap));
+    dev_free(c->proj_recx[i]); dev_free(c->rectx[i]);
+    GS_CUDA(c, dev_alloc(&c->proj_recx[i], 2 * stride * views));
+    GS_CUDA(c, dev_alloc(&c->rectx[i], stride * views));
   }
-  c->stereo_cap = c->cap;
+  c->stereo_cap = (uint32_t)stride;
+  c->stereo_views = views;
   return GS_OK;
 }
 
-// a slot's stereo table (device + pinned staging): fixed size, allocated once
+// a slot's view table (device + pinned staging): fixed size, allocated once
 static int ensure_slot_stereo(gs_context *c, gs_context::Slot &sl) {
-  if (!sl.stereo_dev) GS_CUDA(c, cudaMalloc((void **)&sl.stereo_dev, sizeof(StereoParams)));
-  if (!sl.stereo_host) GS_CUDA(c, cudaHostAlloc((void **)&sl.stereo_host, sizeof(StereoParams), cudaHostAllocDefault));
+  if (!sl.stereo_dev) GS_CUDA(c, cudaMalloc((void **)&sl.stereo_dev, sizeof(ViewTable)));
+  if (!sl.stereo_host) GS_CUDA(c, cudaHostAlloc((void **)&sl.stereo_host, sizeof(ViewTable), cudaHostAllocDefault));
   return GS_OK;
 }
 
@@ -169,7 +176,7 @@ static void drop_stereo_graphs(gs_context *c);
 
 static int ensure_bins(gs_context *c, uint32_t n_bins) {
   if (n_bins <= c->bins_cap && c->bin_range[0]) return GS_OK;
-  // the captured stages bake bin_range; a stereo frame grows it to both eyes' bins while a mono frame's key stays put
+  // the captured stages bake bin_range; a views frame grows it to every view's bins while a mono frame's key stays put
   drop_graphs(c);
   drop_stereo_graphs(c);
   dev_free(c->bin_range[0]); dev_free(c->bin_range[1]);
@@ -191,7 +198,7 @@ static int ensure_tile_stats(gs_context *c, uint32_t n_tiles) {
 }
 
 // buffers of the front-to-back slab path (gs_slab.cu); the pipeline is idle when this runs.  n_tiles: the frame's slab tiles
-// (a stereo frame's: both eyes')
+// (a views frame's: every view's)
 static int ensure_slab(gs_context *c, uint32_t n_tiles) {
   if (c->slab_cap < c->cap || !c->key32[0]) {
     dev_free(c->key32[0]); dev_free(c->key32[1]); dev_free(c->cidx); dev_free(c->ckey); dev_free(c->chunk_cnt[0]); dev_free(c->chunk_cnt[1]);
@@ -207,7 +214,7 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles) {
   for (int i = 0; i < 2; ++i)
     if (!c->slab_tab[i]) GS_CUDA(c, dev_alloc(&c->slab_tab[i], 1));
   if (c->slab_tiles_cap < n_tiles || !c->pix_state) {
-    // the captured slab loops bake these buffers, and a stereo frame grows them to both eyes' tiles while the mono frames'
+    // the captured slab loops bake these buffers, and a views frame grows them to every view's tiles while the mono frames'
     // graph key stays put (and the other way round)
     drop_graphs(c);
     drop_stereo_graphs(c);
@@ -380,7 +387,7 @@ extern "C" int gs_destroy(gs_context *c) {
   dev_free(c->center_scale); dev_free(c->cov_color); dev_free(c->size_alpha);
   dev_free(c->depth); dev_free(c->idx_a); dev_free(c->dig_a);
   for (int i = 0; i < 2; ++i) { dev_free(c->order[i]); dev_free(c->proj_rec[i]); dev_free(c->rect[i]); }
-  for (int i = 0; i < 2; ++i) { dev_free(c->proj_rec1[i]); dev_free(c->rect1[i]); }
+  for (int i = 0; i < 2; ++i) { dev_free(c->proj_recx[i]); dev_free(c->rectx[i]); }
   dev_free(c->inst_tile); dev_free(c->inst_idx); dev_free(c->inst_tile_b); dev_free(c->inst_tile_f); dev_free(c->inst_idx_b);
   dev_free(c->inst_rec[0]); dev_free(c->inst_rec[1]);
   dev_free(c->bin_range[0]); dev_free(c->bin_range[1]); dev_free(c->quirk_table); dev_free(c->tile_stats);
@@ -412,7 +419,7 @@ extern "C" int gs_destroy(gs_context *c) {
   delete c->scene_tmp;
   for (auto &sl : c->slot) {
     dev_free(sl.ctr); dev_free(sl.fp);
-    for (int e = 0; e < 2; ++e) {
+    for (int e = 0; e < kMaxViews; ++e) {
       if (sl.frame_dev[e]) cudaFree(sl.frame_dev[e]);
       if (sl.depth_dev[e]) cudaFree(sl.depth_dev[e]);
       if (sl.color_dev[e]) cudaFree(sl.color_dev[e]);
@@ -825,14 +832,33 @@ extern "C" uint32_t gs_owned_tiles(uint32_t width, uint32_t height, uint32_t ran
 static FrameBufs slot_bufs(gs_context *c, const gs_context::Slot &sl) {
   FrameBufs b{c->order[sl.set], c->proj_rec[sl.set], c->rect[sl.set], c->inst_rec[sl.set], c->bin_range[sl.set]};
   if (sl.stereo) {
-    b.proj_rec1 = c->proj_rec1[sl.set];
-    b.rect1 = c->rect1[sl.set];
+    b.views = true;
+    if (sl.n_views > 1) {
+      b.proj_recx = c->proj_recx[sl.set];
+      b.rectx = c->rectx[sl.set];
+      b.x_stride = c->stereo_cap;
+    }
+    memcpy(b.bin_base, sl.stereo_host->bin_base, sizeof(b.bin_base));
   }
   return b;
 }
 
-// per-frame parameters the kernels read: a stereo frame's pair (eye 1 at +1, for the raster), else the slot's own
-static const FrameParams *slot_fp(const gs_context::Slot &sl) { return sl.stereo ? &sl.stereo_dev->eye[0] : sl.fp; }
+// per-frame parameters the kernels read: a views frame's views (view v at +v), else the slot's own
+static const FrameParams *slot_fp(const gs_context::Slot &sl) { return sl.stereo ? &sl.stereo_dev->view[0] : sl.fp; }
+
+// graph key of a frame: anything baked into its captured launches (views frames: also the view shape and the extra views'
+// buffers, which only their bin sort takes as kernel arguments)
+static gs_context::GraphKey graph_key(const gs_context *c, const gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
+  gs_context::GraphKey k;
+  k.cap = c->cap; k.n_tiles = n_tiles; k.n_bins = n_bins; k.cap_inst = c->cap_inst; k.p0 = c->depth; k.p1 = c->inst_rec[0]; k.p2 = c->center_scale;
+  k.p3 = c->scene_key;
+  if (sl.stereo) {
+    k.n_views = sl.n_views;
+    for (uint32_t v = 0; v < sl.n_views; ++v) k.view_size[v] = sl.view[v].width | sl.view[v].height << 16;
+    k.px = sl.n_views > 1 ? c->proj_recx[0] : nullptr;
+  }
+  return k;
+}
 
 // Stage A of a frame (sort stream): per-frame inputs to the device, depth sort, vertex shader.  All per-frame
 // inputs come from sl.fp (device memory), so each stage is captured once into a CUDA graph and replayed.
@@ -869,7 +895,7 @@ static cudaError_t enqueue_sort_stage(gs_context *c, gs_context::Slot &sl, bool 
 
 // Stage A of a scene frame: per-entity depth pass, keys and the (rank, key, index) sort; per-entity projection beside it.
 // The scene table was copied to sl.scene_dev ahead of the stage (submit), and for a stereo frame the stereo table to
-// sl.stereo_dev: the sort is the head camera's, the projection covers both eyes.
+// sl.stereo_dev: the sort is the head camera's, the projection covers every view.
 static cudaError_t enqueue_scene_sort_stage(gs_context *c, gs_context::Slot &sl, bool external_events) {
   auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
     return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
@@ -959,10 +985,8 @@ static int run_graph(gs_context *c, cudaGraphExec_t &ge, cudaStream_t stream, F 
 // long issue-bound raster's CTAs retire.  Stage hand-offs are events; buffers between stages are double-buffered.
 static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_t n_tiles, uint32_t n_bins) {
   // (re)capture when anything baked into the launches changed
-  gs_context::GraphKey k;
-  k.cap = c->cap; k.n_tiles = n_tiles; k.n_bins = n_bins; k.cap_inst = c->cap_inst; k.p0 = c->depth; k.p1 = c->inst_rec[0]; k.p2 = c->center_scale;
-  k.p3 = c->scene_key;
-  // stereo frames keep their own graphs and key (n_bins: both eyes' bins), so neither kind re-captures the other's
+  const gs_context::GraphKey k = graph_key(c, sl, n_tiles, n_bins);
+  // views frames keep their own graphs and key (n_tiles, n_bins: every view's), so neither kind re-captures the other's
   gs_context::GraphKey &key = sl.stereo ? c->gkey_stereo : c->gkey;
   if (memcmp(&k, &key, sizeof(k)) != 0) {
     if (sl.stereo) drop_stereo_graphs(c);
@@ -1025,7 +1049,7 @@ static cudaError_t enqueue_slab_keys_stage(gs_context *c, gs_context::Slot &sl, 
 }
 
 // Stage B+C of a slab frame (raster stream): the slab loop and the resolve.  One chain: every slab depends on the tiles
-// the previous one closed.  A stereo frame runs it once for both eyes: n_tiles of one eye, n_bins of both.
+// the previous one closed.  A views frame runs it once for every view: n_tiles and n_bins of every view.
 static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins,
                                            bool external_events) {
   auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
@@ -1034,7 +1058,7 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
   cudaStream_t st = c->rstream;
   const FrameBufs b = slot_bufs(c, sl);
   const SceneTable *scene = sl.scene ? sl.scene_dev : nullptr;
-  const StereoParams *stereo = sl.stereo ? sl.stereo_dev : nullptr;
+  const ViewTable *stereo = sl.stereo ? sl.stereo_dev : nullptr;
   const FrameParams *fp = slot_fp(sl);  // the frame's (a stereo frame's pair) for the projection, binning and raster
   cudaError_t e;
   launch_slab_init(c, fp, sl.ctr, sl.stereo, st);
@@ -1042,7 +1066,7 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
   for (int s = 0; s < sl.n_slabs; ++s) {
     launch_slab_begin(c, sl.fp, sl.ctr, scene, sl.set, s, st);   // entry count (0 once every bin is closed) + compaction
     launch_slab_sort(c, sl.fp, sl.ctr, scene, b, st);            // draw order of the slab
-    launch_project_entries(c, sl.fp, sl.ctr, scene, stereo, b, st);  // vertex shader for the slab's entries (of each eye)
+    launch_project_entries(c, sl.fp, sl.ctr, scene, stereo, b, st);  // vertex shader for the slab's entries (of each view)
     if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, st))) return e;
     launch_emit(c, fp, sl.ctr, b, c->bin_open, st);
     launch_tile_radix(c, sl.ctr, b, n_bins, st);
@@ -1062,11 +1086,9 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
 
 // Front-to-back slab path (gs_slab.cu).  Two stages: A (keys of every splat, O(N), sort stream) and the slab loop
 // (raster stream); stage A of frame k+1 runs under the loop of frame k (keys / slab table are double-buffered by set).
-// A stereo frame passes n_bins of both eyes and keeps its graphs under the stereo key, as on the one-pass path.
+// A views frame passes n_tiles and n_bins of every view and keeps its graphs under the views key, as on the one-pass path.
 static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
-  gs_context::GraphKey k;
-  k.cap = c->cap; k.n_tiles = n_tiles; k.n_bins = n_bins; k.cap_inst = c->cap_inst; k.p0 = c->depth; k.p1 = c->inst_rec[0]; k.p2 = c->center_scale;
-  k.p3 = c->scene_key;
+  const gs_context::GraphKey k = graph_key(c, sl, n_tiles, n_bins);
   gs_context::GraphKey &key = sl.stereo ? c->gkey_stereo : c->gkey;
   if (memcmp(&k, &key, sizeof(k)) != 0) {
     if (sl.stereo) drop_stereo_graphs(c);
@@ -1104,7 +1126,7 @@ static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_ti
   }
   GS_CUDA(c, cudaEventRecord(sl.ev_binned, c->rstream));
   c->sort_set_free[set] = sl.ev_binned;
-  // scene frames: three radix passes per slab instead of two (stereo frames: the scene frame's launches, both eyes' bins)
+  // scene frames: three radix passes per slab instead of two (views frames: the scene frame's launches, every view's bins)
   sl.launches = 6u + 1u + (uint32_t)n_slabs * ((n_bins <= 256u ? 16u : 20u) + (sl.scene ? 3u : 0u)) + 2u;
   return GS_OK;
 }
@@ -1117,11 +1139,12 @@ static int enqueue_readback(gs_context *c, gs_context::Slot &sl) {
   GS_CUDA(c, cudaStreamWaitEvent(c->copy_stream, sl.ev_done, 0));
   GS_CUDA(c, cudaMemcpyAsync(sl.ctr_host, sl.ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, c->copy_stream));
   if (sl.host_out)
-    for (int e = 0; e < (sl.stereo ? 2 : 1); ++e) {
+    for (uint32_t e = 0; e < sl.n_views; ++e) {
       if (sl.target) {  // a host gs_target: 2-D copies into the rectangles only
-        const size_t px_bytes = sl.params.out_format == GS_FORMAT_RGBA8 ? 4 : 16, row = px_bytes * sl.params.width;
+        const gs_render_params &vp = sl.view[e];
+        const size_t px_bytes = vp.out_format == GS_FORMAT_RGBA8 ? 4 : 16, row = px_bytes * vp.width;
         char *dst = (char *)sl.tcolor + ((size_t)sl.torg[e][1] * sl.tpitch + sl.torg[e][0]) * px_bytes;
-        GS_CUDA(c, cudaMemcpy2DAsync(dst, px_bytes * sl.tpitch, sl.frame_src[e], row, row, sl.params.height,
+        GS_CUDA(c, cudaMemcpy2DAsync(dst, px_bytes * sl.tpitch, sl.frame_src[e], row, row, vp.height,
                                      cudaMemcpyDeviceToHost, c->copy_stream));
       } else {
         GS_CUDA(c, cudaMemcpyAsync(sl.out_user[e], sl.frame_src[e], sl.out_bytes[e], cudaMemcpyDeviceToHost, c->copy_stream));
@@ -1158,7 +1181,7 @@ static void fill_render_consts(gs_context *c, const gs_render_params *p, RenderC
   rc.pitch = p->width;  // tightly packed width x height buffers (stage_inputs gives a device target's frame its pitch)
 }
 
-// Output of eye e of the slot's frame (a plain or scene frame has eye 0 only): the caller's device buffer, or a per-slot
+// Output of view e of the slot's frame (a plain or scene frame has view 0 only): the caller's device buffer, or a per-slot
 // device frame that the readback copies to the caller's host buffer
 static int stage_out(gs_context *c, gs_context::Slot &sl, int e, FrameParams &fp) {
   if (!sl.host_out) {
@@ -1173,14 +1196,14 @@ static int stage_out(gs_context *c, gs_context::Slot &sl, int e, FrameParams &fp
   return GS_OK;
 }
 
-// Depth and colour targets of eye e: the caller's device buffers as they are, host buffers staged per slot and eye (copied
+// Depth and colour targets of view e: the caller's device buffers as they are, host buffers staged per slot and view (copied
 // on the sort stream, which the raster stage is ordered after)
 static int stage_inputs(gs_context *c, gs_context::Slot &sl, int e, const gs_render_params *p, FrameParams &fp) {
   int rcode;
   const size_t px_bytes = p->out_format == GS_FORMAT_RGBA8 ? 4 : 16;
   const size_t pixels = (size_t)p->width * p->height;
   if (sl.target) {
-    // colour and depth of eye e's rectangle of a gs_target.  A run that overflows stores nothing (fp.overflow), and its
+    // colour and depth of view e's rectangle of a gs_target.  A run that overflows stores nothing (fp.overflow), and its
     // re-run reuses the staged rectangles: the host buffers already hold the overflowed run's read-back by then
     fp.overflow = &sl.ctr->overflow;
     const uint32_t ox = sl.torg[e][0], oy = sl.torg[e][1];
@@ -1276,20 +1299,34 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   if ((rcode = stage_inputs(c, sl, 0, p, fp))) return rcode;
   // raster instantiation: pixel loop (two pixels per lane by default), depth test, statistics; GS_RENDER_BLEND_UNORM8
   // frames always take the two-pixel loop of that mode (bit 3), whatever GS_RASTER says
-  const bool depth = p->depth_in || (sl.target && sl.tdepth);  // a target's depth is that of both eyes
+  const bool depth = p->depth_in || (sl.target && sl.tdepth);  // a target's depth is that of every view
   const bool blend8 = (p->flags & GS_RENDER_BLEND_UNORM8) != 0;
   sl.raster_flags = (blend8 ? 9u : c->raster_base_flags) | (depth ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u);
+  // a views frame bins every view (ids bin_base[v] + bin) and rasters every view's tiles in one grid, on either path
+  uint32_t n_tiles_all = rc.n_tiles, n_bins_all = rc.n_bins;
   if (sl.stereo) {
-    // the pair of eye frames the stereo kernels read: eye 0 as above, eye 1 from its own parameters (same size and flags)
-    StereoParams &st = *sl.stereo_host;
-    st.eye[0] = fp;
-    FrameParams &f1 = st.eye[1];
-    memset(&f1, 0, sizeof(f1));
-    f1.n_splats = sl.n_splats;
-    fill_render_consts(c, &sl.eye1, f1.rc);
-    sl.out_bytes[1] = (size_t)sl.eye1.width * sl.eye1.height * (sl.eye1.out_format == GS_FORMAT_RGBA8 ? 4 : 16);
-    if ((rcode = stage_out(c, sl, 1, f1)) || (rcode = stage_inputs(c, sl, 1, &sl.eye1, f1))) return rcode;
-    if (sl.eye1.depth_in) sl.raster_flags |= 2u;
+    // the view frames the views kernels read: view 0 as above, the others from their own parameters (same flags)
+    ViewTable &vt = *sl.stereo_host;
+    vt.n_views = sl.n_views;
+    vt.view[0] = fp;
+    n_tiles_all = n_bins_all = 0;
+    for (uint32_t v = 0; v < (uint32_t)kMaxViews; ++v) {
+      vt.tile_base[v] = v < sl.n_views ? n_tiles_all : 0xFFFFFFFFu;
+      vt.bin_base[v] = v < sl.n_views ? n_bins_all : 0xFFFFFFFFu;
+      if (v >= sl.n_views) continue;
+      FrameParams &fv = vt.view[v];
+      if (v > 0) {
+        const gs_render_params &pv = sl.view[v];
+        memset(&fv, 0, sizeof(fv));
+        fv.n_splats = sl.n_splats;
+        fill_render_consts(c, &pv, fv.rc);
+        sl.out_bytes[v] = (size_t)pv.width * pv.height * (pv.out_format == GS_FORMAT_RGBA8 ? 4 : 16);
+        if ((rcode = stage_out(c, sl, (int)v, fv)) || (rcode = stage_inputs(c, sl, (int)v, &pv, fv))) return rcode;
+        if (pv.depth_in) sl.raster_flags |= 2u;
+      }
+      n_tiles_all += fv.rc.n_tiles;
+      n_bins_all += fv.rc.n_bins;
+    }
     GS_CUDA(c, cudaMemcpyAsync(sl.stereo_dev, sl.stereo_host, sl.stereo_bytes, cudaMemcpyHostToDevice, c->stream));
   }
   // the scene table goes ahead of the sort stage on its stream (only the entities in use are copied)
@@ -1298,12 +1335,10 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   // a frame normally takes the buffer set the previous frame did not; a frame that reuses the last sort must read
   // that sort's set, so it runs in it
   sl.set = reuse ? c->last_set : (c->last_set ^ 1);
-  // a stereo frame bins both eyes (ids eye * n_bins + bin) and rasters both eyes' tiles in one grid, on either path
-  const uint32_t n_bins_all = sl.stereo ? 2 * rc.n_bins : rc.n_bins;
   if (sl.slab) {
-    if ((rcode = launch_frame_slabs(c, sl, rc.n_tiles, n_bins_all))) return rcode;
+    if ((rcode = launch_frame_slabs(c, sl, n_tiles_all, n_bins_all))) return rcode;
   } else {
-    if ((rcode = launch_frame(c, sl, reuse, rc.n_tiles, n_bins_all))) return rcode;
+    if ((rcode = launch_frame(c, sl, reuse, n_tiles_all, n_bins_all))) return rcode;
   }
   if ((rcode = enqueue_readback(c, sl))) return rcode;
   c->last_set = sl.set;
@@ -1362,7 +1397,11 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   memset(&c->stats, 0, sizeof(c->stats));
   stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
   c->stats.kernel_launches = sl.launches;
-  c->stats.n_tiles = sl.fp_host->rc.n_tiles * (sl.stereo ? 2u : 1u);
+  c->stats.n_tiles = sl.fp_host->rc.n_tiles;
+  if (sl.stereo) {  // every view's
+    const ViewTable &vt = *sl.stereo_host;
+    c->stats.n_tiles = vt.tile_base[vt.n_views - 1] + vt.view[vt.n_views - 1].rc.n_tiles;
+  }
   if (sl.raster_flags & 4u) {  // GS_RENDER_STATS: per-tile {records streamed, records kept, pair tests, pair hits}
     const RenderConsts &rc = sl.fp_host->rc;
     for (uint32_t t = 0; t < rc.n_tiles; ++t) {
@@ -1407,18 +1446,19 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   return GS_OK;
 }
 
-// the second eye of a stereo scene frame
-struct StereoInput {
-  const gs_render_params *eye1;
-  const void *color_in1;
-  void *out1;
-  const float (*mv)[2][16];  // per entity of the scene table, in its order: the modelview of each eye
+// the views of a views scene frame (views[0] is the frame's own parameters)
+struct ViewsInput {
+  uint32_t n;
+  const gs_render_params *views;
+  const void *const *color_in;  // NULL, or per view NULL or its colour target
+  void *const *out;
+  const float (*mv)[kMaxViews][16];  // per entity of the scene table, in its order: the modelview of each view
 };
 
-// a frame into a gs_target (validated by check_target): the target and the rectangle origin of each eye
+// a frame into a gs_target (validated by check_target): the target and the rectangle origin of each view
 struct TargetInput {
   const gs_target *t;
-  uint32_t xy[2][2];
+  uint32_t xy[kMaxViews][2];
 };
 
 // do the rectangles [ax, ax+aw) x [ay, ay+ah) and [bx, bx+bw) x [by, by+bh) share a pixel
@@ -1429,18 +1469,19 @@ static bool rects_overlap(uint32_t ax, uint32_t ay, uint32_t aw, uint32_t ah, ui
 }
 
 // Successive frames into one target compose in submission order, like successive GL draws: a target frame first waits
-// (oldest first) for every pending target frame on the same colour buffer whose rectangles meet its own (w x h each).
-// Stream order alone is not enough: gs_wait may still re-run such a frame, and a host target's rectangle is read at
-// submission.
-static int wait_overlapping(gs_context *c, const TargetInput &t, uint32_t w, uint32_t h, int n_eyes) {
+// (oldest first) for every pending target frame on the same colour buffer whose rectangles meet its own (view a's:
+// views[a].width x views[a].height).  Stream order alone is not enough: gs_wait may still re-run such a frame, and a host
+// target's rectangle is read at submission.
+static int wait_overlapping(gs_context *c, const TargetInput &t, const gs_render_params *views, uint32_t n_views) {
   for (;;) {
     gs_context::Slot *hit = nullptr;
     for (auto &o : c->slot) {
       if (!o.pending || !o.target || o.tcolor != t.t->color || (hit && o.ticket > hit->ticket)) continue;
       bool meet = false;
-      for (int a = 0; a < n_eyes; ++a)
-        for (int b = 0; b < (o.stereo ? 2 : 1); ++b)
-          meet = meet || rects_overlap(t.xy[a][0], t.xy[a][1], w, h, o.torg[b][0], o.torg[b][1], o.params.width, o.params.height);
+      for (uint32_t a = 0; a < n_views; ++a)
+        for (uint32_t b = 0; b < o.n_views; ++b)
+          meet = meet || rects_overlap(t.xy[a][0], t.xy[a][1], views[a].width, views[a].height, o.torg[b][0], o.torg[b][1],
+                                       o.view[b].width, o.view[b].height);
       if (meet) hit = &o;
     }
     if (!hit) return GS_OK;
@@ -1458,27 +1499,37 @@ static int check_blend8(gs_context *c, const gs_render_params *p) {
   return GS_OK;
 }
 
-// gs_render_async, scene and stereo scene frames.  scene: the table built by build_scene_table (nullptr = a plain frame);
-// color_in: the colour target or nullptr; stereo: the second eye of a stereo scene frame (nullptr otherwise; p is eye 0);
+// gs_render_async, scene and views scene frames.  scene: the table built by build_scene_table (nullptr = a plain frame);
+// color_in: the colour target or nullptr; stereo: the views of a views scene frame (nullptr otherwise; p is view 0);
 // target: the gs_target the frame is drawn into in place (nullptr otherwise; color_in is then nullptr and out_rgba the
 // target's colour buffer).
 static int render_async(gs_context *c, const gs_render_params *p, const SceneTable *scene, size_t scene_bytes,
-                        const void *color_in, void *out_rgba, uint64_t *out_ticket, const StereoInput *stereo = nullptr,
+                        const void *color_in, void *out_rgba, uint64_t *out_ticket, const ViewsInput *stereo = nullptr,
                         const TargetInput *target = nullptr) {
   if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
   if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
   int rcode;
   if ((rcode = check_blend8(c, p))) return rcode;
-  const uint32_t n_tiles = ((p->width + kTile - 1) / kTile) * ((p->height + kTile - 1) / kTile);
-  const uint32_t n_bins = ((p->width + kBin - 1) / kBin) * ((p->height + kBin - 1) / kBin);  // <= 64*64: fits the 16-bit bin id
-  // a stereo frame's bin table holds both eyes' bins (2 * 43 * 43 at most, still a 16-bit id)
-  const uint32_t n_bins_all = stereo ? 2 * n_bins : n_bins;
+  auto tiles_of = [](const gs_render_params &q) { return ((q.width + kTile - 1) / kTile) * ((q.height + kTile - 1) / kTile); };
+  auto bins_of = [](const gs_render_params &q) { return ((q.width + kBin - 1) / kBin) * ((q.height + kBin - 1) / kBin); };
+  const uint32_t n_tiles = tiles_of(*p);
+  const uint32_t n_bins = bins_of(*p);  // <= 64*64: fits the 16-bit bin id
+  // a views frame's bin table holds every view's bins (4 * 43 * 43 at most, still a 16-bit id), its slab state every
+  // view's tiles
+  uint32_t n_bins_all = n_bins, slab_tiles = n_tiles;
+  if (stereo) {
+    n_bins_all = slab_tiles = 0;
+    for (uint32_t v = 0; v < stereo->n; ++v) {
+      n_bins_all += bins_of(stereo->views[v]);
+      slab_tiles += tiles_of(stereo->views[v]);
+    }
+  }
   GS_CUDA(c, cudaSetDevice(c->device));
   const uint64_t ticket = c->next_ticket;
   gs_context::Slot &sl = c->slot[ticket % gs_context::kSlots];
   if (sl.pending && (rcode = wait_slot(c, sl, nullptr))) return rcode;  // slot reuse: its previous frame must be done
-  if (target && (rcode = wait_overlapping(c, *target, p->width, p->height, stereo ? 2 : 1))) return rcode;
+  if (target && (rcode = wait_overlapping(c, *target, stereo ? stereo->views : p, stereo ? stereo->n : 1u))) return rcode;
   if ((p->flags & GS_RENDER_OUT_PEER) && ticket >= 3) {
     // the shared frame ring of the fused exchange has three entries, released by gs_wait: at most three such frames
     gs_context::Slot &o = c->slot[(ticket - 3) % gs_context::kSlots];
@@ -1495,11 +1546,10 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     for (uint32_t k = 0; k < scene->n; ++k) sortable += scene->obj[k].end - scene->obj[k].first;
   }
   const uint32_t expect_sorted = c->have_last_sorted ? c->last_sorted : sortable;
-  // stereo frames by their own threshold (GS_SLAB_MIN_XR); they accept neither flag.  GS_RENDER_BLEND_UNORM8 frames are
+  // views frames by their own threshold (GS_SLAB_MIN_XR); they accept neither flag.  GS_RENDER_BLEND_UNORM8 frames are
   // always one-pass: the slab path stops at front-to-back saturation, which rounding after every blend does not have
   const bool slab = expect_sorted >= (stereo ? c->slab_min_xr : c->slab_min) &&
                     !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS | GS_RENDER_BLEND_UNORM8));
-  const uint32_t slab_tiles = stereo ? 2 * n_tiles : n_tiles;  // pixel state of both eyes
   if ((int)slab != c->last_mode) {
     if ((rcode = drain(c))) return rcode;
     GS_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1509,7 +1559,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   }
   // growing any shared buffer needs an idle pipeline
   const bool grow = (slab && (c->slab_cap < c->cap || !c->key32[0] || c->slab_tiles_cap < slab_tiles || !c->slab_tab[1])) || !(c->scratch_cap >= c->cap && c->depth) || !(n_bins_all <= c->bins_cap && c->bin_range[0]) || !(n_tiles <= c->tile_stats_cap && c->tile_stats) || c->cap_inst == 0 ||
-                    (scene && !(c->scene_cap >= c->cap && c->scene_key)) || (stereo && !(c->stereo_cap >= c->cap && c->proj_rec1[0]));
+                    (scene && !(c->scene_cap >= c->cap && c->scene_key)) || (stereo && !stereo_bufs_ok(c, stereo->n));
   if (grow) {
     if ((rcode = drain(c))) return rcode;
     GS_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1520,7 +1570,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     if ((rcode = ensure_tile_stats(c, n_tiles))) return rcode;
     if (slab && (rcode = ensure_slab(c, slab_tiles))) return rcode;
     if (scene && (rcode = ensure_scene_bufs(c))) return rcode;
-    if (stereo && (rcode = ensure_stereo_bufs(c))) return rcode;
+    if (stereo && (rcode = ensure_stereo_bufs(c, stereo->n))) return rcode;
     if (c->cap_inst == 0) {
       // first frame: room for two bin instances per resident splat (a typical scene needs ~1); GS_INST_CAP overrides
       // the initial size (tests of the overflow / regrow path)
@@ -1530,6 +1580,8 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     }
   }
   sl.params = *p;
+  sl.n_views = stereo ? stereo->n : 1u;
+  sl.view[0] = *p;
   sl.out_user[0] = out_rgba;
   sl.ticket = ticket;
   sl.n_splats = c->n;
@@ -1555,11 +1607,15 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   sl.stereo = stereo != nullptr;
   if (stereo) {
     if ((rcode = ensure_slot_stereo(c, sl))) return rcode;
-    sl.eye1 = *stereo->eye1;
-    sl.out_user[1] = stereo->out1;
-    sl.color_in[1] = stereo->color_in1;
-    memcpy(sl.stereo_host->mv, stereo->mv, sizeof(float) * 32 * scene->n);
-    sl.stereo_bytes = offsetof(StereoParams, mv) + sizeof(float) * 32 * scene->n;
+    for (uint32_t v = 1; v < stereo->n; ++v) {
+      sl.view[v] = stereo->views[v];
+      sl.out_user[v] = stereo->out[v];
+      sl.color_in[v] = stereo->color_in ? stereo->color_in[v] : nullptr;
+    }
+    memcpy(sl.stereo_host->mv, stereo->mv, sizeof(stereo->mv[0]) * scene->n);
+    // one copy: header, the frames, and the entities in use (up to the last view in use of the last one)
+    sl.stereo_bytes = offsetof(ViewTable, mv);
+    if (scene->n) sl.stereo_bytes += sizeof(stereo->mv[0]) * (scene->n - 1) + sizeof(float) * 16 * stereo->n;
   }
   if ((rcode = submit(c, sl))) return rcode;
   c->next_ticket = ticket + 1;
@@ -1598,7 +1654,7 @@ extern "C" int gs_render_scene_async(gs_context *c, const gs_render_params *fram
   return scene_async(c, frame, objs, n_objs, color_in, out_rgba, out_ticket, nullptr);
 }
 
-// The rules of a frame into eye rectangle (x, y) of a gs_target that do not depend on the scene (those of gs_render_scene
+// The rules of a frame into view rectangle (x, y) of a gs_target that do not depend on the scene (those of gs_render_scene
 // and gs_render_scene_stereo are checked after these, also before anything is changed)
 static int check_target(gs_context *c, const gs_render_params *p, const gs_target *t, uint32_t x, uint32_t y) {
   if (!t || !t->color) return fail(c, GS_ERR_INVALID, "target frame: no target or no colour buffer");
@@ -1735,45 +1791,98 @@ extern "C" int gs_render_stereo(gs_context *c, const float view[4], const float 
 }
 
 // XR over a multi-entity page: the one scene sort of the frame from the head camera (every entity's tick(), index.js:438-455),
-// each entity drawn once per eye with that eye's matrices (onBeforeRender per eye camera, index.js:184-195)
-// gs_render_scene_stereo_async, and gs_render_scene_stereo_target_async (target set: no color_in, out_rgba = the layer's
-// colour twice)
-static int scene_stereo_async(gs_context *c, const gs_render_params eyes[2], const gs_object *objs, const float *eye_modelviews,
-                              uint32_t n_objs, const void *const color_in[2], void *const out_rgba[2], uint64_t *out_ticket,
-                              const TargetInput *target) {
-  if (!eyes || !eye_modelviews || !out_rgba || !out_rgba[0] || !out_rgba[1])
-    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: missing eyes, eye modelviews or outputs");
-  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render_scene_stereo before any push");
-  if (eyes[0].width != eyes[1].width || eyes[0].height != eyes[1].height)
-    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: the eyes must have the same size");
-  if (eyes[0].flags != eyes[1].flags) return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: the eyes must have the same flags");
-  if (eyes[0].flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS | GS_RENDER_OUT_TILED | GS_RENDER_OUT_PEER))
-    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: GS_RENDER_REUSE_SORT, _STATS, _OUT_TILED and _OUT_PEER are not accepted");
-  if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: not on a sharded context");
-  if (eyes[1].out_format != GS_FORMAT_RGBA8 && eyes[1].out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
-  int rc = check_blend8(c, &eyes[1]);
-  if (rc) return rc;
+// each entity drawn once per view with that view's matrices and viewport (onBeforeRender per view camera, index.js:184-195).
+// gs_render_scene_views[_stereo]_async, and their _target variants (target set: no color_in, out_rgba = the layer's colour
+// per view)
+static int scene_views_async(gs_context *c, const gs_render_params *views, uint32_t n_views, const gs_object *objs,
+                             const float *view_modelviews, uint32_t n_objs, const void *const *color_in,
+                             void *const *out_rgba, uint64_t *out_ticket, const TargetInput *target) {
+  if (n_views == 0 || n_views > (uint32_t)kMaxViews) return fail(c, GS_ERR_INVALID, "views frame: between 1 and GS_MAX_VIEWS views");
+  if (!views || !view_modelviews || !out_rgba) return fail(c, GS_ERR_INVALID, "views frame: missing views, view modelviews or outputs");
+  for (uint32_t v = 0; v < n_views; ++v)
+    if (!out_rgba[v]) return fail(c, GS_ERR_INVALID, "views frame: missing output");
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "views frame before any push");
+  if (views[0].flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS | GS_RENDER_OUT_TILED | GS_RENDER_OUT_PEER))
+    return fail(c, GS_ERR_INVALID, "views frame: GS_RENDER_REUSE_SORT, _STATS, _OUT_TILED and _OUT_PEER are not accepted");
+  if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "views frame: not on a sharded context");
+  int rc;
+  for (uint32_t v = 1; v < n_views; ++v) {  // view 0 is checked by render_async
+    const gs_render_params &p = views[v];
+    if (p.flags != views[0].flags) return fail(c, GS_ERR_INVALID, "views frame: every view must have the same flags");
+    if (p.width == 0 || p.height == 0 || p.width > 4096 || p.height > 4096)
+      return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
+    if (p.out_format != GS_FORMAT_RGBA8 && p.out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+    if ((rc = check_blend8(c, &p))) return rc;
+  }
   size_t bytes = 0;
   rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
   if (rc) return rc;
-  // each entity's per-eye modelviews, in the table's order (caller's entity k = its draw rank)
-  float mv[kMaxObjects][2][16];
+  // each entity's per-view modelviews, in the table's order (caller's entity k = its draw rank)
+  float mv[kMaxObjects][kMaxViews][16];
   const SceneTable &t = *c->scene_tmp;
   for (uint32_t j = 0; j < t.n; ++j)
-    for (int e = 0; e < 2; ++e) memcpy(mv[j][e], eye_modelviews + ((size_t)e * n_objs + t.obj[j].rank) * 16, sizeof(mv[j][e]));
-  const StereoInput st{&eyes[1], color_in ? color_in[1] : nullptr, out_rgba[1], mv};
-  return render_async(c, &eyes[0], c->scene_tmp, bytes, color_in ? color_in[0] : nullptr, out_rgba[0], out_ticket, &st, target);
+    for (uint32_t v = 0; v < n_views; ++v)
+      memcpy(mv[j][v], view_modelviews + ((size_t)v * n_objs + t.obj[j].rank) * 16, sizeof(mv[j][v]));
+  const ViewsInput in{n_views, views, color_in, out_rgba, mv};
+  return render_async(c, &views[0], c->scene_tmp, bytes, color_in ? color_in[0] : nullptr, out_rgba[0], out_ticket, &in, target);
+}
+
+// the stereo calls are the two-view case, with equal eye sizes (a WebXR projection layer's two eyes)
+static int check_stereo_eyes(gs_context *c, const gs_render_params eyes[2]) {
+  if (!eyes) return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: missing eyes");
+  if (eyes[0].width != eyes[1].width || eyes[0].height != eyes[1].height)
+    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo: the eyes must have the same size");
+  return GS_OK;
 }
 
 extern "C" int gs_render_scene_stereo_async(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
                                             const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
                                             void *const out_rgba[2], uint64_t *out_ticket) {
   if (!c) return GS_ERR_INVALID;
-  return scene_stereo_async(c, eyes, objs, eye_modelviews, n_objs, color_in, out_rgba, out_ticket, nullptr);
+  int rc = check_stereo_eyes(c, eyes);
+  if (rc) return rc;
+  return scene_views_async(c, eyes, 2, objs, eye_modelviews, n_objs, color_in, out_rgba, out_ticket, nullptr);
 }
 
-// WebXR into the layer's one framebuffer: each eye at its viewport rectangle (three.js renders each eye camera of the
+extern "C" int gs_render_scene_views_async(gs_context *c, const gs_render_params *views, uint32_t n_views,
+                                           const gs_object *objs, const float *view_modelviews, uint32_t n_objs,
+                                           const void *const *color_in, void *const *out_rgba, uint64_t *out_ticket) {
+  if (!c) return GS_ERR_INVALID;
+  if (views)
+    for (uint32_t v = 1; v < n_views && v < (uint32_t)kMaxViews; ++v)
+      if (views[v].out_format != views[0].out_format)
+        return fail(c, GS_ERR_INVALID, "gs_render_scene_views: every view must have the same out_format");
+  return scene_views_async(c, views, n_views, objs, view_modelviews, n_objs, color_in, out_rgba, out_ticket, nullptr);
+}
+
+// WebXR into the layer's one framebuffer: each view at its viewport rectangle (three.js renders each view camera of the
 // ArrayCamera with its own viewport)
+static int scene_views_target_async(gs_context *c, const gs_render_params *views, uint32_t n_views, const gs_object *objs,
+                                    const float *view_modelviews, uint32_t n_objs, const gs_target *layer,
+                                    const uint32_t *view_xy, uint64_t *out_ticket) {
+  if (n_views == 0 || n_views > (uint32_t)kMaxViews) return fail(c, GS_ERR_INVALID, "views frame: between 1 and GS_MAX_VIEWS views");
+  if (!views || !view_xy) return fail(c, GS_ERR_INVALID, "views target frame: missing views or view rectangles");
+  int rc;
+  for (uint32_t v = 0; v < n_views; ++v)
+    if ((rc = check_target(c, &views[v], layer, view_xy[2 * v], view_xy[2 * v + 1]))) return rc;
+  for (uint32_t a = 0; a < n_views; ++a) {
+    if (views[a].out_format != views[0].out_format)
+      return fail(c, GS_ERR_INVALID, "views target frame: every view must have the layer's one format");
+    for (uint32_t b = 0; b < a; ++b)
+      if (rects_overlap(view_xy[2 * a], view_xy[2 * a + 1], views[a].width, views[a].height, view_xy[2 * b], view_xy[2 * b + 1],
+                        views[b].width, views[b].height))
+        return fail(c, GS_ERR_INVALID, "views target frame: the view rectangles overlap");
+  }
+  TargetInput t{layer, {}};
+  void *outs[kMaxViews];
+  for (uint32_t v = 0; v < n_views; ++v) {
+    t.xy[v][0] = view_xy[2 * v];
+    t.xy[v][1] = view_xy[2 * v + 1];
+    outs[v] = layer->color;
+  }
+  return scene_views_async(c, views, n_views, objs, view_modelviews, n_objs, nullptr, outs, out_ticket, &t);
+}
+
 extern "C" int gs_render_scene_stereo_target_async(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
                                                    const float *eye_modelviews, uint32_t n_objs, const gs_target *layer,
                                                    const uint32_t eye_xy[4], uint64_t *out_ticket) {
@@ -1782,14 +1891,15 @@ extern "C" int gs_render_scene_stereo_target_async(gs_context *c, const gs_rende
   int rc;
   for (int e = 0; e < 2; ++e)
     if ((rc = check_target(c, &eyes[e], layer, eye_xy[2 * e], eye_xy[2 * e + 1]))) return rc;
-  if (eyes[0].out_format != eyes[1].out_format)
-    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo_target: the eyes must have the layer's one format");
-  if (eyes[0].width == eyes[1].width && eyes[0].height == eyes[1].height &&
-      rects_overlap(eye_xy[0], eye_xy[1], eyes[0].width, eyes[0].height, eye_xy[2], eye_xy[3], eyes[1].width, eyes[1].height))
-    return fail(c, GS_ERR_INVALID, "gs_render_scene_stereo_target: the eye rectangles overlap");
-  const TargetInput t{layer, {{eye_xy[0], eye_xy[1]}, {eye_xy[2], eye_xy[3]}}};
-  void *const outs[2] = {layer->color, layer->color};
-  return scene_stereo_async(c, eyes, objs, eye_modelviews, n_objs, nullptr, outs, out_ticket, &t);
+  if ((rc = check_stereo_eyes(c, eyes))) return rc;
+  return scene_views_target_async(c, eyes, 2, objs, eye_modelviews, n_objs, layer, eye_xy, out_ticket);
+}
+
+extern "C" int gs_render_scene_views_target_async(gs_context *c, const gs_render_params *views, uint32_t n_views,
+                                                  const gs_object *objs, const float *view_modelviews, uint32_t n_objs,
+                                                  const gs_target *layer, const uint32_t *view_xy, uint64_t *out_ticket) {
+  if (!c) return GS_ERR_INVALID;
+  return scene_views_target_async(c, views, n_views, objs, view_modelviews, n_objs, layer, view_xy, out_ticket);
 }
 
 extern "C" int gs_render_scene_stereo_target(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
@@ -1801,11 +1911,29 @@ extern "C" int gs_render_scene_stereo_target(gs_context *c, const gs_render_para
   return gs_wait(c, t, stats);
 }
 
+extern "C" int gs_render_scene_views_target(gs_context *c, const gs_render_params *views, uint32_t n_views,
+                                            const gs_object *objs, const float *view_modelviews, uint32_t n_objs,
+                                            const gs_target *layer, const uint32_t *view_xy, gs_stats *stats) {
+  uint64_t t = 0;
+  int rc = gs_render_scene_views_target_async(c, views, n_views, objs, view_modelviews, n_objs, layer, view_xy, &t);
+  if (rc) return rc;
+  return gs_wait(c, t, stats);
+}
+
 extern "C" int gs_render_scene_stereo(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
                                       const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
                                       void *const out_rgba[2], gs_stats *stats) {
   uint64_t t = 0;
   int rc = gs_render_scene_stereo_async(c, eyes, objs, eye_modelviews, n_objs, color_in, out_rgba, &t);
+  if (rc) return rc;
+  return gs_wait(c, t, stats);
+}
+
+extern "C" int gs_render_scene_views(gs_context *c, const gs_render_params *views, uint32_t n_views, const gs_object *objs,
+                                     const float *view_modelviews, uint32_t n_objs, const void *const *color_in,
+                                     void *const *out_rgba, gs_stats *stats) {
+  uint64_t t = 0;
+  int rc = gs_render_scene_views_async(c, views, n_views, objs, view_modelviews, n_objs, color_in, out_rgba, &t);
   if (rc) return rc;
   return gs_wait(c, t, stats);
 }

@@ -142,14 +142,30 @@ struct SceneTable {
   uint32_t pad[2];
   SceneObject obj[kMaxObjects];
 };
-// ---- stereo scene frames (gs_render_scene_stereo): one head-camera sort, both eyes projected, binned and rasterised in
-// one pass each.  Bin ids of the pair are eye * n_bins + bin; eye e's raster CTAs are blocks [e * n_tiles, (e+1) * n_tiles).
-// Per slot, fixed size, allocated by the first stereo frame; only the entities in use are copied per frame. ----
-struct StereoParams {
-  FrameParams eye[2];              // each eye's frame (projection, viewport, output, colour / depth target); eye[0] also
+// ---- views scene frames (gs_render_scene_views, and gs_render_scene_stereo as its two-view case): one head-camera sort,
+// every view projected, binned and rasterised in one pass each.  Bin ids of view v are bin_base[v] + bin; view v's raster
+// CTAs (and slab tiles) are [tile_base[v], tile_base[v + 1]).  The kernels of a views frame receive fp = &views->view[0],
+// so fp + v is view v's frame, and reach the header through view_table(fp).
+// Per slot, fixed size (captured graphs bake its pointer), allocated by the first views frame; only the views and entities
+// in use are copied per frame. ----
+constexpr int kMaxViews = GS_MAX_VIEWS;
+struct ViewTable {
+  uint32_t n_views;
+  uint32_t tile_base[kMaxViews];   // first CTA of view v; 0xFFFFFFFF for the views not in use (never reached)
+  uint32_t bin_base[kMaxViews];    // first bin id of view v; likewise
+  uint32_t pad[3];
+  FrameParams view[kMaxViews];     // each view's frame (projection, viewport, output, colour / depth target); view[0] also
                                    // carries n_splats for the sort, as a slot's FrameParams does
-  float mv[kMaxObjects][2][16];    // entity k's (scene-table order) gsModelViewMatrix of eye e
+  float mv[kMaxObjects][kMaxViews][16];  // entity k's (scene-table order) gsModelViewMatrix of view v
 };
+__host__ __device__ inline const ViewTable *view_table(const FrameParams *fp) {
+  return (const ViewTable *)((const char *)fp - offsetof(ViewTable, view));
+}
+// the view whose CTAs (tile_base) or bins (bin_base) hold index i: at most three compares
+__device__ __forceinline__ uint32_t view_of(const uint32_t *base, uint32_t i) {
+  return (i >= base[1] ? 1u : 0u) + (i >= base[2] ? 1u : 0u) + (i >= base[3] ? 1u : 0u);
+}
+static_assert(kMaxViews == 4, "view_of compares against three bases");
 // per-entity results of the depth pass (one worker's min / max / validCount, index.js:548-555)
 struct ObjCounters {
   unsigned long long min_enc, max_enc;  // encodings as in SortHeader
@@ -226,10 +242,11 @@ struct gs_context {
   uint32_t *order[2] = {nullptr, nullptr};    // draw order (== reference sortedIndexes)
   float4 *proj_rec[2] = {nullptr, nullptr};   // 2 x float4 per splat
   uint32_t *rect[2] = {nullptr, nullptr};     // packed tile rect per splat
-  // the second eye's proj_rec / rect of stereo scene frames, allocated by the first one
-  uint32_t stereo_cap = 0;
-  float4 *proj_rec1[2] = {nullptr, nullptr};
-  uint32_t *rect1[2] = {nullptr, nullptr};
+  // proj_rec / rect of views 1.. of views frames, one buffer per set holding stereo_views views of stereo_cap splats each:
+  // view v's at (v - 1) * stereo_cap records / rectangles.  Allocated by the first views frame, grown with the view count
+  uint32_t stereo_cap = 0, stereo_views = 0;
+  float4 *proj_recx[2] = {nullptr, nullptr};
+  uint32_t *rectx[2] = {nullptr, nullptr};
   uint32_t *table_n = nullptr;  // radix chunk histograms of the depth passes [256][table_n_stride]
   uint32_t table_n_stride = 0;
   uint32_t *totals = nullptr;    // [512]: digit totals of the depth / tile passes
@@ -261,7 +278,7 @@ struct gs_context {
   uint32_t *chunk_cnt[2] = {nullptr, nullptr};  // [kMaxSlabs][chunk_row] per-slab compaction offsets of every 2048-splat chunk (one per set)
   uint32_t chunk_row = 0;          // row stride of chunk_cnt: cap / 2048 + 4
   gs::SlabTable *slab_tab[2] = {nullptr, nullptr};
-  float4 *pix_state = nullptr;     // [tiles * 256] {R, G, B, T} carried from slab to slab (stereo frames: both eyes' tiles)
+  float4 *pix_state = nullptr;     // [tiles * 256] {R, G, B, T} carried from slab to slab (views frames: every view's tiles)
   uint8_t *tile_closed = nullptr;  // [tiles]
   uint32_t *bin_open = nullptr;    // [bins] live tiles per bin (0 for bins of other ranks)
   uint32_t slab_tiles_cap = 0;
@@ -298,32 +315,33 @@ struct gs_context {
     gs::FrameCounters *ctr_host = nullptr;   // pinned
     gs::FrameParams *fp = nullptr;           // device
     gs::FrameParams *fp_host = nullptr;      // pinned staging
-    // per eye ([1]: the second eye of a stereo scene frame)
-    void *frame_dev[2] = {};                 // used when the caller's buffer is host memory
-    size_t frame_bytes[2] = {};
-    void *depth_dev[2] = {};                 // staging of a host depth_in
-    size_t depth_bytes[2] = {};
-    const void *color_in[2] = {};            // caller's colour target (scene frames), host unless color_device
+    // per view ([0] only, except in a views scene frame)
+    void *frame_dev[gs::kMaxViews] = {};     // used when the caller's buffer is host memory
+    size_t frame_bytes[gs::kMaxViews] = {};
+    void *depth_dev[gs::kMaxViews] = {};     // staging of a host depth_in
+    size_t depth_bytes[gs::kMaxViews] = {};
+    const void *color_in[gs::kMaxViews] = {};  // caller's colour target (scene frames), host unless color_device
     bool color_device = false;
-    void *color_dev[2] = {};                 // staging of a host color_in
-    size_t color_bytes[2] = {};
+    void *color_dev[gs::kMaxViews] = {};     // staging of a host color_in
+    size_t color_bytes[gs::kMaxViews] = {};
     bool scene = false;                      // multi-entity frame (gs_render_scene): scene table below
-    bool stereo = false;                     // stereo scene frame (gs_render_scene_stereo): stereo table below
-    gs_render_params eye1{};                 // its second eye
-    gs::StereoParams *stereo_dev = nullptr;  // device copy, fixed size (captured graphs bake the pointer)
-    gs::StereoParams *stereo_host = nullptr; // pinned staging
-    size_t stereo_bytes = 0;                 // bytes in use (both eyes' frames + the entities in use)
+    bool stereo = false;                     // views scene frame (gs_render_scene_views / _stereo): view table below
+    uint32_t n_views = 1;                    // its views (every other frame: 1)
+    gs_render_params view[gs::kMaxViews]{};  // each view's parameters ([0] = params)
+    gs::ViewTable *stereo_dev = nullptr;     // device copy, fixed size (captured graphs bake the pointer)
+    gs::ViewTable *stereo_host = nullptr;    // pinned staging
+    size_t stereo_bytes = 0;                 // bytes in use (header, frames, and the entities in use)
     gs::SceneTable *scene_dev = nullptr;     // device copy, fixed size (captured graphs bake the pointer)
     gs::SceneTable *scene_host = nullptr;    // pinned staging
     size_t scene_bytes = 0;                  // bytes of the table in use (header + non-empty entities)
     gs::ObjCounters *octr = nullptr;         // [kMaxObjects] per-entity depth-pass results
-    // frames into a gs_target (gs_render_scene*_target): each eye drawn in place at its rectangle of the caller's buffers
+    // frames into a gs_target (gs_render_scene*_target): each view drawn in place at its rectangle of the caller's buffers
     bool target = false;
-    bool target_device = false;              // GS_TARGET_DEVICE: read and written where they are; else staged per eye
+    bool target_device = false;              // GS_TARGET_DEVICE: read and written where they are; else staged per view
     void *tcolor = nullptr;
     const float *tdepth = nullptr;
     uint32_t tpitch = 0;
-    uint32_t torg[2][2] = {};                // rectangle origin (x, y) of each eye
+    uint32_t torg[gs::kMaxViews][2] = {};    // rectangle origin (x, y) of each view
     bool restage = true;                     // false while gs_wait re-runs the frame: the staged rectangles are reused
     uint32_t raster_flags = 0;               // k_raster instantiation of this frame (packed | depth | stats)
     uint32_t n_splats = 0;                   // resident splats when the frame was submitted
@@ -350,15 +368,15 @@ struct gs_context {
     uint64_t ticket = 0;
     int ring = 0;                            // slot of the shared frame ring (fused exchange)
     unsigned long long peer_seq = 0;
-    void *frame_src[2] = {};                 // device buffer the host copy reads
+    void *frame_src[gs::kMaxViews] = {};     // device buffer the host copy reads
     cudaEvent_t ev_sorted = nullptr;                // sort/project stage of this slot's frame finished
     cudaEvent_t ev_binned = nullptr;                // binning stage finished
     cudaEvent_t ev_r0 = nullptr;                    // raster start (timing)
     int index = 0;
     bool pending = false;
     bool host_out = false;
-    void *out_user[2] = {};
-    size_t out_bytes[2] = {};
+    void *out_user[gs::kMaxViews] = {};
+    size_t out_bytes[gs::kMaxViews] = {};
     gs_render_params params{};
     uint32_t launches = 0;
     int set = 0;                                    // which order/proj_rec/rect and inst_rec/bin_range copy it uses
@@ -391,8 +409,12 @@ struct gs_context {
   bool use_pdl = false;                          // programmatic dependent launch inside the stage chains (GS_PDL=1 turns it on)
   uint32_t raster_base_flags = 1;                // default pixel loop: 1 = two pixels per lane, 0 = one
   // graph cache key: anything baked into the captured launches
-  struct GraphKey { uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr; } gkey;
-  GraphKey gkey_stereo;                          // ... of the stereo graphs (kept apart: a stereo frame re-captures only its own)
+  // (views frames: n_views, each view's width | height << 16, and the extra views' buffers, baked into the bin sort)
+  struct GraphKey {
+    uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr;
+    uint32_t n_views = 0, view_size[gs::kMaxViews] = {}, pad2 = 0; const void *px = nullptr;
+  } gkey;
+  GraphKey gkey_stereo;                          // ... of the views graphs (kept apart: a views frame re-captures only its own)
 
   // ---- fused exchange: one shared allocation per rank = flag rows + a ring of 3 frames, opened by every peer ----
   void *peer_local = nullptr;            // our shared block
@@ -422,9 +444,14 @@ struct FrameBufs {
   float4 *proj_rec;
   uint32_t *rect;
   float4 *inst_rec;
-  uint2 *bin_range;  // [n_bins] {start, end} of each bin's run in inst_rec (stereo frames: [2 * n_bins], eye-major)
-  float4 *proj_rec1 = nullptr;  // stereo scene frames: the second eye's records and rectangles (NULL otherwise)
-  uint32_t *rect1 = nullptr;
+  uint2 *bin_range;  // [n_bins] {start, end} of each bin's run in inst_rec (views frames: every view's bins, view-major)
+  // views scene frames (NULL otherwise): records and rectangles of views 1.., view v's at (v - 1) * x_stride splats, and
+  // the first bin id of each view (0xFFFFFFFF past the views in use)
+  float4 *proj_recx = nullptr;
+  uint32_t *rectx = nullptr;
+  uint32_t x_stride = 0;
+  uint32_t bin_base[kMaxViews] = {};
+  bool views = false;
 };
 
 // -- launchers (each .cu file owns its kernels); every per-frame input comes from device memory (fp, ctr) --
@@ -438,8 +465,8 @@ void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *s
 void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 9 launches
 void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
                           const FrameBufs &b, cudaStream_t st);
-// stereo scene frames: both eyes' projection in one pass (fp = &stereo->eye[0]) -> b.proj_rec / rect, b.proj_rec1 / rect1
-void launch_project_stereo(gs_context *c, const StereoParams *stereo, const SceneTable *scene, const FrameCounters *ctr,
+// views scene frames: every view's projection in one pass -> b.proj_rec / rect (view 0), b.proj_recx / rectx (views 1..)
+void launch_project_stereo(gs_context *c, const ViewTable *views, const SceneTable *scene, const FrameCounters *ctr,
                            const FrameBufs &b, cudaStream_t st);
 void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_t n, cudaStream_t st);
 // PLY push: k_pack reading row perm[j] (perm NULL: row j) into slot first + j; rows_out (or NULL) receives the ordered rows
@@ -458,13 +485,13 @@ uint32_t *launch_ply_sort(gs_context *c, const uint32_t *key, uint32_t *perm_a, 
                           uint32_t *totals, uint32_t n, cudaStream_t st);
 void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);
 // bin instances in draw order (2 launches); bin_open: the slab path's open-bin table, NULL for one-pass frames.
-// b.rect1 set (stereo frames): both eyes' instances, eye 1's bins numbered from fp->rc.n_bins on
+// b.views (views frames, fp = &views->view[0]): every view's instances, view v's bins numbered from bin_base[v] on
 void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,
                  cudaStream_t st);
-// n_bins: bins of the frame (stereo frames: of both eyes, the record then gathered from b.proj_rec1 from n_bins / 2 on)
+// n_bins: bins of the frame (views frames: of every view, each record gathered from its view's projection)
 void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, cudaStream_t st);  // 3 .. 7 launches
 void launch_raster(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags, cudaStream_t st);
-// stereo scene frames: one grid of 2 * n_tiles CTAs, eye e's frame at fp + e (flags: packed | depth)
+// views scene frames: one grid over every view's tiles (n_tiles: their sum), view v's frame at fp + v (flags: packed | depth)
 void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags, cudaStream_t st);
 void launch_peer_acquire(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
 void launch_peer_signal_wait(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
@@ -476,7 +503,7 @@ void launch_peer_release(gs_context *c, const PeerRows &rows, uint32_t world, ui
 void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const ObjCounters *octr, int set,
                  cudaStream_t st);  // keys + bucket histogram
 void launch_slab_plan(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, uint32_t first_target, int n_slabs, cudaStream_t st);
-// stereo: both eyes' pixel state, closed flags and bins (fp = &stereo->eye[0])
+// stereo: every view's pixel state, closed flags and bins (fp = &views->view[0])
 void launch_slab_init(gs_context *c, const FrameParams *fp, FrameCounters *ctr, bool stereo, cudaStream_t st);
 void launch_compact_offsets(gs_context *c, const FrameParams *fp, const SceneTable *scene, int set, int n_slabs,
                             cudaStream_t st);  // every slab's chunk offsets: 2 launches
@@ -484,11 +511,11 @@ void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr,
                        cudaStream_t st);  // + compaction: 2 launches
 void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
                       cudaStream_t st);  // 6 launches (scene frames: 9)
-// stereo: the slot's stereo table of a stereo scene frame (both eyes into b.proj_rec / rect and b.proj_rec1 / rect1)
+// views: the slot's view table of a views scene frame (view 0 into b.proj_rec / rect, views 1.. into b.proj_recx / rectx)
 void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene,
-                            const StereoParams *stereo, const FrameBufs &b, cudaStream_t st);
+                            const ViewTable *views, const FrameBufs &b, cudaStream_t st);
 void launch_slab_end(gs_context *c, FrameCounters *ctr, cudaStream_t st);
-// stereo: one grid of 2 * n_tiles CTAs over both eyes (fp = &stereo->eye[0]); likewise the resolve
+// stereo: one grid over every view's tiles (n_tiles: their sum; fp = &views->view[0]); likewise the resolve
 void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, uint32_t n_tiles, const FrameBufs &b, bool depth,
                         bool stereo, cudaStream_t st);
 void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, bool stereo, cudaStream_t st);

@@ -3,15 +3,15 @@
 //
 //   k_project  : fp32 restatement of the vertex shader, op for op (no FMA contraction), producing a
 //                32 B projected record per splat + its packed tile rectangle (scene frames: with each splat's entity's
-//                gsModelViewMatrix; stereo scene frames: both eyes per splat, the table row loaded once).
+//                gsModelViewMatrix; views scene frames: every view per splat, the table row loaded once).
 //   k_count    : per entry of the draw order (== reference sortedIndexes): instance offset inside its 256-entry slice;
 //                per slice: total; last CTA: prefix over the slices + frame total D.
 //                Sparse frames (fewer than half of the splats sorted): each chunk's survivors are compacted first.
 //   k_emit_entries: one thread per draw-order entry writes its (bin, splat) instances at the entry's offset,
 //                in draw order, so that a STABLE sort by bin id alone reproduces the reference's back-to-front order
-//                inside every bin; rectangles of more than 8 bins are finished by the whole warp.  Stereo scene frames:
-//                each entry emits eye 0's instances, then eye 1's, with bin ids eye * n_bins + bin (on the slab path too,
-//                each eye's closed bins skipped).
+//                inside every bin; rectangles of more than 8 bins are finished by the whole warp.  Views scene frames:
+//                each entry emits view 0's instances, then those of views 1.., with bin ids bin_base[v] + bin (on the
+//                slab path too, each view's closed bins skipped).
 #include "gs_common.cuh"
 
 namespace gs {
@@ -41,7 +41,7 @@ __device__ __forceinline__ void unpack_int16(uint32_t value, float &lo, float &h
 // One splat through the vertex shader: returns its packed bin rectangle (kNoRect when nothing is drawn) and stores the
 // 32 B record at slot j.
 // mv: the splat's gsModelViewMatrix (rc.mv, or its entity's in a scene frame).  c: its center_scale row; q: its
-// cov_color row, loaded on the first call that needs it (have_q), so a stereo frame's two eyes load each row once.
+// cov_color row, loaded on the first call that needs it (have_q), so a views frame's views load each row once.
 __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const float *mv, const float4 c,
                                                 const uint4 *__restrict__ cc, uint32_t i, uint32_t j,
                                                 float4 *__restrict__ rec_out, uint4 &q, bool &have_q) {
@@ -153,8 +153,9 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
 // instead of warps with a few live lanes each.
 // SCENE (scene frames, by index or, on the slab path, by entry): every splat takes its entity's modelview; by index, the
 // splat the Q5 tail may repeat is each entity's first one.
-// STEREO (stereo scene frames, by index or, on the slab path, by entry): fp = &stereo->eye[0]; every splat is projected
-// for both eyes with each eye's RenderConsts and its entity's per-eye modelview, eye 1 into rec_out1 / rect_out1.
+// STEREO (views scene frames, by index or, on the slab path, by entry): fp = &views->view[0]; every splat is projected
+// for every view with the view's RenderConsts and its entity's per-view modelview, the table row loaded once; view v >= 1
+// into rec_x / rect_x at (v - 1) * x_stride.
 template <bool BY_ENTRY, bool SCENE = false, bool STEREO = false>
 __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, const uint4 *__restrict__ cc,
                                                  const float *__restrict__ depth,
@@ -162,9 +163,9 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
                                                  uint32_t *__restrict__ rect_out, const uint32_t *__restrict__ order,
                                                  const FrameCounters *__restrict__ ctr,
                                                  const SceneTable *__restrict__ scene,
-                                                 const StereoParams *__restrict__ stereo, float4 *__restrict__ rec_out1,
-                                                 uint32_t *__restrict__ rect_out1) {
-  static_assert(!STEREO || SCENE, "stereo frames are scene frames");
+                                                 const ViewTable *__restrict__ views, float4 *__restrict__ rec_x,
+                                                 uint32_t *__restrict__ rect_x, uint32_t x_stride) {
+  static_assert(!STEREO || SCENE, "views frames are scene frames");
   GS_PDL_ENTRY();
   const RenderConsts &rc = fp->rc;
   const uint32_t n = BY_ENTRY ? ctr->sort.n_valid : fp->n_splats;
@@ -189,19 +190,28 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
     if (!SCENE) return rc.mv;
     return scene->obj[scene_find(s_first, s_end, n_obj, i)].mv;
   };
-  // splat i through the vertex shader (of each eye), record at slot j; returns eye 0's rectangle, eye 1's in *rect1
-  auto shade = [&](uint32_t i, uint32_t j, uint32_t *rect1) -> uint32_t {
+  const uint32_t n_views = STEREO ? views->n_views : 1u;
+  // splat i through the vertex shader (of each view), record at slot j; returns view 0's rectangle and stores those of
+  // views 1.. at slot j of rect_x
+  auto shade = [&](uint32_t i, uint32_t j) -> uint32_t {
     uint4 q;
     bool have_q = false;
     if (!STEREO) {
       const float *mv = modelview(i);
       return project_one(rc, mv, __ldg(cs + i), cc, i, j, rec_out, q, have_q);
     }
-    const float(*mv)[16] = stereo->mv[scene_find(s_first, s_end, n_obj, i)];
+    const float(*mv)[16] = views->mv[scene_find(s_first, s_end, n_obj, i)];
     const float4 c = __ldg(cs + i);
     const uint32_t r0 = project_one(rc, mv[0], c, cc, i, j, rec_out, q, have_q);
-    *rect1 = project_one(stereo->eye[1].rc, mv[1], c, cc, i, j, rec_out1, q, have_q);
+    for (uint32_t v = 1; v < n_views; ++v) {
+      const size_t x = (size_t)(v - 1) * x_stride;
+      rect_x[x + j] = project_one(views->view[v].rc, mv[v], c, cc, i, j, rec_x + 2 * x, q, have_q);
+    }
     return r0;
+  };
+  // views 1..: no rectangle at slot i
+  auto clear_x = [&](uint32_t i) {
+    for (uint32_t v = 1; v < n_views; ++v) rect_x[(size_t)(v - 1) * x_stride + i] = kNoRect;
   };
   if (!BY_ENTRY && (unsigned long long)ctr->sort.n_valid * 2ull < n) {
     constexpr uint32_t kChunk = 1024;  // 4 splats per thread
@@ -217,13 +227,15 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
         d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
         // no rectangle unless a survivor stores one after the barrier below
         *(uint4 *)(rect_out + base) = make_uint4(kNoRect, kNoRect, kNoRect, kNoRect);
-        if (STEREO) *(uint4 *)(rect_out1 + base) = make_uint4(kNoRect, kNoRect, kNoRect, kNoRect);
+        if (STEREO)  // (x_stride is a multiple of 4)
+          for (uint32_t v = 1; v < n_views; ++v)
+            *(uint4 *)(rect_x + (size_t)(v - 1) * x_stride + base) = make_uint4(kNoRect, kNoRect, kNoRect, kNoRect);
       } else {
 #pragma unroll
         for (uint32_t k = 0; k < 4; ++k) {
           d[k] = (base + k < n) ? __ldg(depth + base + k) : GS_DEPTH_REJECT;
           if (base + k < n) rect_out[base + k] = kNoRect;
-          if (STEREO && base + k < n) rect_out1[base + k] = kNoRect;
+          if (STEREO && base + k < n) clear_x(base + k);
         }
       }
       bool f[4];
@@ -253,10 +265,8 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
       __syncthreads();
       for (uint32_t q = tid; q < total; q += blockDim.x) {
         const uint32_t i = s_list[q];
-        uint32_t rect1 = kNoRect;
-        const uint32_t rect = shade(i, i, &rect1);
+        const uint32_t rect = shade(i, i);
         if (rect != kNoRect) rect_out[i] = rect;
-        if (STEREO && rect1 != kNoRect) rect_out1[i] = rect1;
       }
       __syncthreads();
     }
@@ -264,11 +274,11 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
   }
   for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
     const uint32_t i = BY_ENTRY ? __ldg(order + j) : j;
-    uint32_t rect = kNoRect, rect1 = kNoRect;
+    uint32_t rect = kNoRect;
     const bool sorted = BY_ENTRY || (__ldg(depth + i) != GS_DEPTH_REJECT) || q5_head(i);
-    if (sorted) rect = shade(i, j, &rect1);
+    if (sorted) rect = shade(i, j);
+    else if (STEREO) clear_x(j);
     rect_out[j] = rect;
-    if (STEREO) rect_out1[j] = rect1;
   }
 }
 
@@ -291,9 +301,10 @@ __device__ __forceinline__ uint32_t rect_count(uint32_t r, uint32_t rank, uint32
 // ---------------------------------------------------------------------------------------------
 // SLAB: rect is indexed by entry (k_project<true>), the entry's payload is j itself, and entries whose (small)
 // rectangle holds only closed bins own nothing any more.
-// STEREO (stereo scene frames, one GPU): an entry owns its eye-0 instances, then its eye-1 instances (rect1); it stays
-// live when either eye sees it.  On the slab path each eye's rectangle is tested against that eye's bins (eye 1's from
-// n_bins on); an eye whose rectangle lost its instances gives kNoRect to the emit walk (ent for eye 0, rect1 for eye 1).
+// STEREO (views scene frames, one GPU; fp = &views->view[0]): an entry owns its view-0 instances, then those of views
+// 1.. (rect_x); it stays live when any view sees it.  On the slab path each view's rectangle is tested against that view's
+// bins (from bin_base[v] on); a view whose rectangle lost its instances gives kNoRect to the emit walk (ent for view 0,
+// rect_x for the others).
 template <bool SLAB, bool STEREO = false>
 __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restrict__ order,
                                                         const uint32_t *__restrict__ rect,
@@ -302,9 +313,10 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
                                                         uint32_t *__restrict__ slice_prefix, FrameCounters *ctr,
                                                         const FrameParams *__restrict__ fp,
                                                         const uint32_t *__restrict__ bin_open,
-                                                        uint32_t *__restrict__ rect1) {
+                                                        uint32_t *__restrict__ rect_x, uint32_t x_stride) {
   GS_PDL_ENTRY();
   const uint32_t shard_rank = fp->rc.shard_rank, shard_world = fp->rc.shard_world;
+  const uint32_t n_views = STEREO ? view_table(fp)->n_views : 1u;
   __shared__ uint32_t s_warp[kEmitThreads / 32], s_vis[kEmitThreads / 32];
   __shared__ uint32_t s_last;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -312,34 +324,39 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
   const uint32_t num_slices = (nv + kEmitTile - 1) / kEmitTile;
   for (uint32_t sl = blockIdx.x; sl < num_slices; sl += gridDim.x) {
     const uint32_t j = sl * kEmitTile + tid;
-    uint32_t idx = 0, r = kNoRect, r1 = kNoRect;
+    uint32_t idx = 0, r = kNoRect;
     if (j < nv) {
       idx = SLAB ? j : __ldg(order + j);
       r = __ldg(rect + idx);
-      if (STEREO) r1 = SLAB ? rect1[idx] : __ldg(rect1 + idx);  // (the slab path may rewrite it below)
     }
-    // a small rectangle whose bins (from bin_base on) are all closed owns nothing; bins of other ranks count as closed
-    // (k_slab_init)
-    auto all_closed = [&](uint32_t rr, uint32_t bin_base) -> bool {
+    // a small rectangle of view v whose bins (from bin_base on) are all closed owns nothing; bins of other ranks count as
+    // closed (k_slab_init)
+    auto all_closed = [&](uint32_t rr, uint32_t bin_base, uint32_t bins_x) -> bool {
       const uint32_t bx0 = rr & 255u, bx1 = (rr >> 8) & 255u, by0 = (rr >> 16) & 255u, by1 = rr >> 24;
       if ((bx1 - bx0 + 1u) * (by1 - by0 + 1u) > 4u) return false;
       bool any = false;
       for (uint32_t by = by0; by <= by1; ++by)
-        for (uint32_t bx = bx0; bx <= bx1; ++bx) any = any || (__ldg(bin_open + bin_base + by * fp->rc.bins_x + bx) != 0u);
+        for (uint32_t bx = bx0; bx <= bx1; ++bx) any = any || (__ldg(bin_open + bin_base + by * bins_x + bx) != 0u);
       return !any;
     };
     uint32_t cnt = rect_count(r, shard_rank, shard_world);
-    if (SLAB && cnt && all_closed(r, 0u)) cnt = 0;
-    const uint32_t cnt0 = cnt;  // eye 0's instances
-    if (STEREO) {
-      uint32_t cnt1 = rect_count(r1, 0u, 1u);
-      if (SLAB && cnt1 && all_closed(r1, fp->rc.n_bins)) {
-        cnt1 = 0;
-        rect1[idx] = kNoRect;
+    if (SLAB && cnt && all_closed(r, 0u, fp->rc.bins_x)) cnt = 0;
+    const uint32_t cnt0 = cnt;  // view 0's instances
+    uint32_t vis = r != kNoRect;
+    if (STEREO && j < nv) {
+      for (uint32_t v = 1; v < n_views; ++v) {
+        uint32_t *rv = rect_x + (size_t)(v - 1) * x_stride + idx;
+        const uint32_t rr = SLAB ? *rv : __ldg(rv);  // (the slab path may rewrite it below)
+        uint32_t cv = rect_count(rr, 0u, 1u);
+        if (SLAB && cv && all_closed(rr, view_table(fp)->bin_base[v], fp[v].rc.bins_x)) {
+          cv = 0;
+          *rv = kNoRect;
+        }
+        cnt += cv;
+        vis += rr != kNoRect;
       }
-      cnt += cnt1;
     }
-    uint32_t incl = cnt, vis = (r != kNoRect) + (STEREO && r1 != kNoRect);
+    uint32_t incl = cnt;
     for (int o = 1; o < 32; o <<= 1) {
       const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
       if (lane >= (uint32_t)o) incl += t;
@@ -405,7 +422,7 @@ __global__ void __launch_bounds__(kEmitThreads) k_count(const uint32_t *__restri
 // against the r<=2 footprint; rejected bins (and, on the slab path, closed ones) become kNoTile and are dropped by the
 // bin sort.
 // ---------------------------------------------------------------------------------------------
-// bin_base: first bin id of the eye (stereo frames: eye * n_bins; else 0)
+// bin_base: first bin id of the view (views frames: bin_base[v]; else 0)
 __device__ __forceinline__ void emit_candidate(const RenderConsts &rc, uint32_t bx, uint32_t by, bool multi, const float4 &r0,
                                                const float2 &r1, const uint32_t *__restrict__ bin_open, uint32_t payload,
                                                size_t pos, uint16_t *__restrict__ inst_tile, uint32_t *__restrict__ inst_idx,
@@ -420,8 +437,8 @@ __device__ __forceinline__ void emit_candidate(const RenderConsts &rc, uint32_t 
   inst_idx[pos] = payload;
 }
 
-// STEREO: each entry writes its eye-0 instances, then its eye-1 instances (rectangle rect1, records proj_rec1, bin ids
-// from rc.n_bins on; the eyes share the viewport size, hence the bin grid)
+// STEREO (fp = &views->view[0]): each entry writes its view-0 instances, then those of views 1.. (rectangles rect_x,
+// records proj_rec_x, view v's bin grid with ids from bin_base[v] on)
 template <bool STEREO = false>
 __global__ void __launch_bounds__(256) k_emit_entries(const uint2 *__restrict__ ent, const uint32_t *__restrict__ ent_off,
                                                       const uint32_t *__restrict__ slice_prefix,
@@ -429,9 +446,10 @@ __global__ void __launch_bounds__(256) k_emit_entries(const uint2 *__restrict__ 
                                                       uint64_t cap_inst, uint16_t *__restrict__ inst_tile,
                                                       uint32_t *__restrict__ inst_idx, FrameCounters *ctr,
                                                       const uint32_t *__restrict__ bin_open,
-                                                      const float4 *__restrict__ proj_rec1, const uint32_t *__restrict__ rect1) {
+                                                      const float4 *__restrict__ proj_rec_x, const uint32_t *__restrict__ rect_x,
+                                                      uint32_t x_stride) {
   GS_PDL_ENTRY();
-  const RenderConsts &rc = fp->rc;
+  const uint32_t n_views = STEREO ? view_table(fp)->n_views : 1u;
   const uint32_t nv = ctr->sort.n_valid;
   if (ctr->n_inst > cap_inst) {  // instance buffer too small: the host regrows it and re-runs the frame
     if (blockIdx.x == 0 && threadIdx.x == 0) ctr->overflow = 1u;
@@ -443,12 +461,13 @@ __global__ void __launch_bounds__(256) k_emit_entries(const uint2 *__restrict__ 
   for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < nv_pad; j += stride) {
     uint2 en = make_uint2(0u, kNoRect);
     if (j < nv) en = __ldg(ent + j);
-    uint32_t off = 0;  // instances of the entry's earlier eye
-#pragma unroll
-    for (uint32_t eye = 0; eye < (STEREO ? 2u : 1u); ++eye) {
-      const uint32_t r = eye == 0u ? en.y : (j < nv ? __ldg(rect1 + en.x) : kNoRect);
-      const float4 *rec = eye == 0u ? proj_rec : proj_rec1;
-      const uint32_t bin_base = eye * rc.n_bins;
+    uint32_t off = 0;  // instances of the entry's earlier views
+    for (uint32_t v = 0; v < n_views; ++v) {
+      const RenderConsts &rc = fp[v].rc;
+      const size_t x = v ? (size_t)(v - 1) * x_stride : 0;
+      const uint32_t r = v == 0u ? en.y : (j < nv ? __ldg(rect_x + x + en.x) : kNoRect);
+      const float4 *rec = v == 0u ? proj_rec : proj_rec_x + 2 * x;
+      const uint32_t bin_base = STEREO ? view_table(fp)->bin_base[v] : 0u;
       uint32_t bx0 = 0, by0 = 0, w = 0, h = 0, step = 1, n_own = 0;
       size_t base = 0;
       float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -511,18 +530,18 @@ void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *c
   if (blocks < 1) blocks = 1;
   launch_chain(c, k_project<false>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
                (const uint32_t *)nullptr, ctr, (const SceneTable *)nullptr,  // ctr: the sorted count picks the sparse-frame path
-               (const StereoParams *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr);
+               (const ViewTable *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr, 0u);
 }
 
-void launch_project_stereo(gs_context *c, const StereoParams *stereo, const SceneTable *scene, const FrameCounters *ctr,
+void launch_project_stereo(gs_context *c, const ViewTable *views, const SceneTable *scene, const FrameCounters *ctr,
                            const FrameBufs &b, cudaStream_t stream) {
   uint64_t blocks = ((uint64_t)c->cap + 255) / 256;
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   launch_chain(c, k_project<false, true, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
-               (const float *)c->depth, &stereo->eye[0], b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, stereo,
-               b.proj_rec1, b.rect1);
+               (const float *)c->depth, &views->view[0], b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, views,
+               b.proj_recx, b.rectx, b.x_stride);
 }
 
 void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
@@ -532,27 +551,27 @@ void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   launch_chain(c, k_project<false, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
-               (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, (const StereoParams *)nullptr,
-               (float4 *)nullptr, (uint32_t *)nullptr);
+               (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, (const ViewTable *)nullptr,
+               (float4 *)nullptr, (uint32_t *)nullptr, 0u);
 }
 
 // scene: the slot's scene table for a scene frame (every entry takes its entity's modelview), NULL for a plain frame;
-// stereo: the slot's stereo table of a stereo scene frame (both eyes, fp ignored), NULL otherwise
+// views: the slot's view table of a views scene frame (every view, fp ignored), NULL otherwise
 void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene,
-                            const StereoParams *stereo, const FrameBufs &b, cudaStream_t stream) {
+                            const ViewTable *views, const FrameBufs &b, cudaStream_t stream) {
   uint64_t blocks = ((uint64_t)c->cap + 255) / 256;
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  if (stereo) {
+  if (views) {
     launch_chain(c, k_project<true, true, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale,
-                 (const uint4 *)c->cov_color, (const float *)c->depth, &stereo->eye[0], b.proj_rec, b.rect,
-                 (const uint32_t *)b.order, (const FrameCounters *)ctr, scene, stereo, b.proj_rec1, b.rect1);
+                 (const uint4 *)c->cov_color, (const float *)c->depth, &views->view[0], b.proj_rec, b.rect,
+                 (const uint32_t *)b.order, (const FrameCounters *)ctr, scene, views, b.proj_recx, b.rectx, b.x_stride);
     return;
   }
   launch_chain(c, scene ? k_project<true, true> : k_project<true>, (int)blocks, 256, stream, (const float4 *)c->center_scale,
                (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)b.order,
-               (const FrameCounters *)ctr, scene, (const StereoParams *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr);
+               (const FrameCounters *)ctr, scene, (const ViewTable *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr, 0u);
 }
 
 void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,
@@ -561,13 +580,13 @@ void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const
   const uint64_t cap = (uint64_t)c->sm_count * 8;
   if (tiles > cap) tiles = cap;
   if (tiles < 1) tiles = 1;
-  const bool stereo = b.rect1 != nullptr;
+  const bool stereo = b.views;
   auto count = bin_open ? (stereo ? k_count<true, true> : k_count<true>) : (stereo ? k_count<false, true> : k_count<false>);
   launch_chain(c, count, (int)tiles, kEmitThreads, st, (const uint32_t *)b.order, (const uint32_t *)b.rect, c->ent, c->ent_off,
-               c->slice_total, c->slice_prefix, ctr, fp, bin_open, b.rect1);
+               c->slice_total, c->slice_prefix, ctr, fp, bin_open, b.rectx, b.x_stride);
   launch_chain(c, stereo ? k_emit_entries<true> : k_emit_entries<false>, (int)tiles, 256, st, (const uint2 *)c->ent, (const uint32_t *)c->ent_off,
                (const uint32_t *)c->slice_prefix, (const float4 *)b.proj_rec, fp, (uint64_t)c->cap_inst, c->inst_tile, c->inst_idx, ctr,
-               bin_open, (const float4 *)b.proj_rec1, (const uint32_t *)b.rect1);
+               bin_open, (const float4 *)b.proj_recx, (const uint32_t *)b.rectx, b.x_stride);
 }
 
 }  // namespace gs

@@ -199,10 +199,11 @@ struct SlabIO {
 // DEPTH: depth-test every fragment LEQUAL against fp->depth_in (index.js:179-180).  STATS: count what the tile does
 // (and keep culling the whole list after the tile has closed, so that the count of 16x16 tile instances is exact).
 // SLAB: one depth slab of a frame: start from / store back the pixel state, close saturated tiles; k_resolve writes the frame.
-// STEREO: both eyes of a stereo scene frame, 2 * n_tiles CTAs: CTA b draws tile b % n_tiles of eye b / n_tiles, with that
-// eye's frame fp[eye] (output, colour target, depth target: an eye without one keeps the depth 1, which passes every
-// fragment the projection keeps) and bins from eye * n_bins on.  The pixel loop is the one of the plain frame.  With SLAB,
-// the pixel state and closed flag of eye e's tile t are those of slab tile e * n_tiles + t (the CTA's index).
+// STEREO: every view of a views scene frame (fp = &views->view[0]), one CTA per tile of every view: CTA b draws tile
+// b - tile_base[v] of the view v whose CTAs hold b, with that view's frame fp[v] (output, colour target, depth target: a
+// view without one keeps the depth 1, which passes every fragment the projection keeps) and bins from bin_base[v] on.  The
+// pixel loop is the one of the plain frame.  With SLAB, the pixel state and closed flag of the tile are those of slab
+// tile b (the CTA's index).
 // B8: GS_RENDER_BLEND_UNORM8 (packed loop, one pass): the reference's back-to-front blend with the RGBA8 store after every
 // fragment.  Chunks stream farthest first, the kept records are walked in draw order, every pair is blended (no stop rule:
 // rounding after each blend has no front-to-back form), and the pixel state is the destination's bytes (as byte / 255).
@@ -216,8 +217,9 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   using Cfg = RasterCfg<PACKED>;
   constexpr int kThreads = Cfg::kThreads, kChunk = Cfg::kChunk, kStages = Cfg::kStages, kCv = Cfg::kCv;
   constexpr int kWarps = kThreads / 32;
-  const uint32_t eye = STEREO ? (blockIdx.x >= fp->rc.n_tiles ? 1u : 0u) : 0u;
-  if (STEREO) fp += eye;
+  const ViewTable *vt = STEREO ? view_table(fp) : nullptr;
+  const uint32_t view = STEREO ? view_of(vt->tile_base, blockIdx.x) : 0u;
+  if (STEREO) fp += view;
   const RenderConsts &rc = fp->rc;
   __shared__ __align__(128) float4 s_rec[kStages][kChunk * 2];
   __shared__ __align__(16) float4 s_cv[kChunk * kCv];
@@ -226,12 +228,12 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
   __shared__ uint32_t s_stat[4];
   __shared__ float s_u8f[B8 ? 256 : 1];  // B8: byte -> byte / 255
 
-  const uint32_t tile = blockIdx.x - eye * rc.n_tiles;
-  const uint32_t stile = blockIdx.x;  // slab state index: the tile of a mono frame, eye * n_tiles + tile of a stereo one
+  const uint32_t tile = blockIdx.x - (STEREO ? vt->tile_base[view] : 0u);
+  const uint32_t stile = blockIdx.x;  // slab state index: the tile of a mono frame, tile_base[view] + tile of a views one
   const uint32_t tx = tile % rc.tiles_x, ty = tile / rc.tiles_x;
   const uint32_t bcol = tx / kTilesPerBin;
   if (rc.shard_world > 1 && (bcol % rc.shard_world) != rc.shard_rank) return;
-  const uint32_t bin = eye * rc.n_bins + (ty / kTilesPerBin) * rc.bins_x + bcol;
+  const uint32_t bin = (STEREO ? vt->bin_base[view] : 0u) + (ty / kTilesPerBin) * rc.bins_x + bcol;
 
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   // pixel ownership.  scalar: a warp owns a compact 8x4 block, tid = [ty2 tx1 | y2 x3].  packed: a warp owns an 8x8
@@ -588,13 +590,13 @@ void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles
                           cudaStream_t st) {
   constexpr int kT = RasterCfg<true>::kThreads;
   if (flags & 8u) {
-    if (flags & 2u) k_raster<true, true, false, false, true, true><<<2 * n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{});
-    else k_raster<true, false, false, false, true, true><<<2 * n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{});
+    if (flags & 2u) k_raster<true, true, false, false, true, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{});
+    else k_raster<true, false, false, false, true, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{});
     return;
   }
   switch (flags & 3u) {
 #define GS_RASTER_CASE(v, P, D) \
-  case v: k_raster<P, D, false, false, true><<<2 * n_tiles, RasterCfg<P>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{}); break;
+  case v: k_raster<P, D, false, false, true><<<n_tiles, RasterCfg<P>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{}); break;
     GS_RASTER_CASE(0, false, false)
     GS_RASTER_CASE(1, true, false)
     GS_RASTER_CASE(2, false, true)
@@ -603,15 +605,16 @@ void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles
   }
 }
 
-// one slab of a frame (always the packed pixel loop); stereo: both eyes' tiles in one grid, eye e's frame at fp + e
+// one slab of a frame (always the packed pixel loop); stereo: every view's tiles in one grid (n_tiles: their sum), view v's
+// frame at fp + v
 void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, uint32_t n_tiles, const FrameBufs &b, bool depth,
                         bool stereo, cudaStream_t st) {
   const SlabIO io{c->pix_state, c->tile_closed, c->bin_open, ctr};
   constexpr int kT = RasterCfg<true>::kThreads;
   if (stereo && depth)
-    k_raster<true, true, false, true, true><<<2 * n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
+    k_raster<true, true, false, true, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
   else if (stereo)
-    k_raster<true, false, false, true, true><<<2 * n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
+    k_raster<true, false, false, true, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
   else if (depth)
     k_raster<true, true, false, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
   else
@@ -619,13 +622,14 @@ void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr
 }
 
 // slab path epilogue: pixel state -> frame (composite over the clear colour or colour target; plain / tiled / peer destinations).
-// STEREO: 2 * n_tiles CTAs, CTA b resolves slab tile b into tile b % n_tiles of eye b / n_tiles, with that eye's frame fp[eye]
+// STEREO: one CTA per tile of every view (fp = &views->view[0]): CTA b resolves slab tile b into tile b - tile_base[v] of
+// the view v whose CTAs hold b, with that view's frame fp[v]
 template <bool STEREO>
 __global__ void __launch_bounds__(256) k_resolve(const float4 *__restrict__ state, const FrameParams *__restrict__ fp) {
-  const uint32_t eye = STEREO ? (blockIdx.x >= fp->rc.n_tiles ? 1u : 0u) : 0u;
-  if (STEREO) fp += eye;
+  const uint32_t view = STEREO ? view_of(view_table(fp)->tile_base, blockIdx.x) : 0u;
+  const uint32_t tile = blockIdx.x - (STEREO ? view_table(fp)->tile_base[view] : 0u);
+  if (STEREO) fp += view;
   const RenderConsts &rc = fp->rc;
-  const uint32_t tile = blockIdx.x - eye * rc.n_tiles;
   const uint32_t tx = tile % rc.tiles_x, ty = tile / rc.tiles_x;
   if (rc.shard_world > 1 && ((tx / kTilesPerBin) % rc.shard_world) != rc.shard_rank) return;
   const uint32_t lx = threadIdx.x & 15u, ly = threadIdx.x >> 4;
@@ -635,7 +639,7 @@ __global__ void __launch_bounds__(256) k_resolve(const float4 *__restrict__ stat
 }
 
 void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, bool stereo, cudaStream_t st) {
-  if (stereo) k_resolve<true><<<2 * n_tiles, 256, 0, st>>>(c->pix_state, fp);
+  if (stereo) k_resolve<true><<<n_tiles, 256, 0, st>>>(c->pix_state, fp);
   else k_resolve<false><<<n_tiles, 256, 0, st>>>(c->pix_state, fp);
 }
 

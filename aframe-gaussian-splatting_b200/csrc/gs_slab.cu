@@ -32,11 +32,11 @@
 // of the entity's first splat.  The per-slab sort is SM1, M2, M3 over the compacted 24-bit keys, and the projection
 // takes each entry's entity modelview (k_project<true, true>).
 //
-// Stereo scene frames (gs_render_scene_stereo) cut their slabs from the HEAD camera's scene order, which is both eyes'
-// draw order: stage A, the plan and the compaction offsets are those of the scene frame, shared by the eyes.  Per slab the
-// projection covers both eyes (k_project<true, true, true>), the bin instances of both eyes go into one id space (eye *
-// n_bins + bin, each eye's closed bins skipped) and one raster grid draws both eyes' tiles (eye * n_tiles + tile), each
-// continuing from its own pixel state; the loop stops when neither eye has an open bin.
+// Views scene frames (gs_render_scene_views, gs_render_scene_stereo) cut their slabs from the HEAD camera's scene order,
+// which is every view's draw order: stage A, the plan and the compaction offsets are those of the scene frame, shared by
+// the views.  Per slab the projection covers every view (k_project<true, true, true>), the bin instances of every view go
+// into one id space (bin_base[v] + bin, each view's closed bins skipped) and one raster grid draws every view's tiles
+// (tile_base[v] + tile), each continuing from its own pixel state; the loop stops when no view has an open bin.
 #include <type_traits>
 
 #include "gs_common.cuh"
@@ -181,20 +181,24 @@ __global__ void __launch_bounds__(1024) k_slab_plan(SlabTable *tab, FrameCounter
   }
 }
 
-// per-pixel state, closed flags, live tiles per bin.  STEREO (stereo scene frames, fp = &stereo->eye[0]): both eyes',
-// tiles eye * n_tiles + tile and bins eye * n_bins + bin (the eyes share the viewport size); open_bins counts both eyes
+// per-pixel state, closed flags, live tiles per bin.  STEREO (views scene frames, fp = &views->view[0]): every view's,
+// tiles tile_base[v] + tile and bins bin_base[v] + bin; open_bins counts every view's
 template <bool STEREO>
 __global__ void __launch_bounds__(256) k_slab_init(const FrameParams *__restrict__ fp, FrameCounters *ctr,
                                                    float4 *__restrict__ pix_state, uint8_t *__restrict__ tile_closed,
                                                    uint32_t *__restrict__ bin_open) {
-  const RenderConsts &rc = fp->rc;
-  const uint32_t eyes = STEREO ? 2u : 1u;
+  const ViewTable *vt = STEREO ? view_table(fp) : nullptr;
+  const uint32_t last = STEREO ? vt->n_views - 1u : 0u;  // totals: the last view's base + its own count
+  const uint32_t n_tiles = (STEREO ? vt->tile_base[last] : 0u) + fp[last].rc.n_tiles;
+  const uint32_t n_bins = (STEREO ? vt->bin_base[last] : 0u) + fp[last].rc.n_bins;
   const uint32_t stride = gridDim.x * blockDim.x, g = blockIdx.x * blockDim.x + threadIdx.x;
-  for (uint32_t i = g; i < eyes * rc.n_tiles * 256u; i += stride) pix_state[i] = make_float4(0.f, 0.f, 0.f, 1.f);
-  for (uint32_t i = g; i < eyes * rc.n_tiles; i += stride) tile_closed[i] = 0;
+  for (uint32_t i = g; i < n_tiles * 256u; i += stride) pix_state[i] = make_float4(0.f, 0.f, 0.f, 1.f);
+  for (uint32_t i = g; i < n_tiles; i += stride) tile_closed[i] = 0;
   uint32_t mine = 0;
-  for (uint32_t b = g; b < eyes * rc.n_bins; b += stride) {
-    const uint32_t eb = STEREO ? b % rc.n_bins : b;  // the bin inside its eye
+  for (uint32_t b = g; b < n_bins; b += stride) {
+    const uint32_t v = STEREO ? view_of(vt->bin_base, b) : 0u;
+    const RenderConsts &rc = fp[v].rc;
+    const uint32_t eb = b - (STEREO ? vt->bin_base[v] : 0u);  // the bin inside its view
     const uint32_t bx = eb % rc.bins_x, by = eb / rc.bins_x;
     const bool owned = rc.shard_world <= 1 || (bx % rc.shard_world) == rc.shard_rank;
     const uint32_t tw = min((uint32_t)kTilesPerBin, rc.tiles_x - bx * kTilesPerBin);

@@ -5,8 +5,8 @@
 //   k_radix_{hist,scan,scatter}<D1>, <D2>: index.js:557-567  16-bit key = ToInt32((f32 depth - min) * depthInv), stable
 //                   counting sort as two 8-bit passes
 //   k_radix_{hist,scan,scatter}<T1>, <T2>: stable sort of bin instances by 16-bit bin id; the final pass (T1 when a
-//                   frame has at most 256 bins, else T2) also gathers the 32 B records (<T1S>, <T2S>: a stereo frame's
-//                   combined bins, each eye's record gathered from that eye's projection)
+//                   frame has at most 256 bins, else T2) also gathers the 32 B records (<T1S>, <T2S>: a views frame's
+//                   combined bins, each view's record gathered from that view's projection)
 //   k_radix_{hist,scan,scatter}<S1>, <SM1>: first pass of a depth slab's sort (keys from the slab's compacted entries;
 //                   SM1: the 24-bit keys of a scene frame, followed by M2 and M3)
 //   k_tile_ranges : per-bin {start, end} in the final instance order (frames of more than 256 bins; otherwise pass T1 writes them)
@@ -737,20 +737,28 @@ __global__ void __launch_bounds__(256) k_tile_ranges(const uint16_t *__restrict_
   }
 }
 
-// Stereo scene frames: the bin id of eye e's instance is e * eye_bins + bin, its record comes from that eye's projection
+// Views scene frames: the bin id of view v's instance is bin_base[v] + bin, its record comes from that view's projection
+// (view 0: proj_rec; view v >= 1: rec_x at (v - 1) * x_stride splats).  Bases past the views in use are 0xFFFFFFFF.
+struct ViewRecs {
+  const float4 *rec_x;
+  uint32_t x_stride;
+  uint32_t base1, base2, base3;
+  __device__ __forceinline__ const float4 *of(const float4 *rec0, uint32_t bin) const {
+    const uint32_t v = (bin >= base1 ? 1u : 0u) + (bin >= base2 ? 1u : 0u) + (bin >= base3 ? 1u : 0u);
+    return v ? rec_x + 2 * (size_t)(v - 1) * x_stride : rec0;
+  }
+};
 struct T1S : T1 {
-  const float4 *proj_rec1;
-  uint32_t eye_bins;
+  ViewRecs vr;
   __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const {
-    if (last) gather_record(carry >= eye_bins ? proj_rec1 : proj_rec, inst_rec, pay, pos);
+    if (last) gather_record(vr.of(proj_rec, carry), inst_rec, pay, pos);
     else { idx_out[pos] = pay; bin_out[pos] = (uint16_t)carry; }
   }
 };
 struct T2S : T2 {
-  const float4 *proj_rec1;
-  uint32_t eye_bins;
+  ViewRecs vr;
   __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const {
-    gather_record(carry >= eye_bins ? proj_rec1 : proj_rec, inst_rec, pay, pos);
+    gather_record(vr.of(proj_rec, carry), inst_rec, pay, pos);
     bin_out[pos] = (uint16_t)carry;
   }
 };
@@ -759,12 +767,14 @@ struct T2S : T2 {
 void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, cudaStream_t st) {
   const RadixScratch s{c->table_d, c->totals + 256, c->table_d_stride};
   const bool last = n_bins <= 256u;
-  if (b.proj_rec1) {  // stereo: both eyes' bins, n_bins / 2 each
+  if (b.views) {  // every view's bins
+    static_assert(kMaxViews == 4, "ViewRecs holds three bases");
+    const ViewRecs vr{b.proj_recx, b.x_stride, b.bin_base[1], b.bin_base[2], b.bin_base[3]};
     const T1 t1{{}, ctr, c->inst_tile, c->inst_idx, c->inst_tile_b, c->inst_idx_b, b.proj_rec, b.inst_rec, b.bin_range, n_bins, last};
-    run_pass(c, T1S{t1, b.proj_rec1, n_bins / 2}, s, c->cap_inst, st);
+    run_pass(c, T1S{t1, vr}, s, c->cap_inst, st);
     if (last) return;
     const T2 t2{{}, ctr, c->inst_tile_b, c->inst_idx_b, b.proj_rec, b.inst_rec, c->inst_tile_f};
-    run_pass(c, T2S{t2, b.proj_rec1, n_bins / 2}, s, c->cap_inst, st);
+    run_pass(c, T2S{t2, vr}, s, c->cap_inst, st);
     launch_chain(c, k_tile_ranges, persistent_grid(c, c->cap_inst, 256 * 8, 8), 256, st, (const uint16_t *)c->inst_tile_f, ctr,
                  b.bin_range);
     return;

@@ -272,14 +272,22 @@ class SplatContext:
     def _stereo_args(eyes_params, objects: Sequence[SceneObject], eye_modelviews, color_ptrs, out_ptrs):
         """ctypes arguments of gs_render_scene_stereo[_async]: eye_modelviews[e][k] is entity k's modelview of eye e."""
         assert len(eyes_params) == 2 and len(out_ptrs) == 2
-        arr = (GsRenderParams * 2)()
-        for i in range(2):
-            C.memmove(C.addressof(arr[i]), C.addressof(eyes_params[i]), C.sizeof(GsRenderParams))
-        mv = np.ascontiguousarray(np.asarray(eye_modelviews, np.float32).reshape(2, len(objects), 16))
+        return SplatContext._views_args(eyes_params, objects, eye_modelviews, color_ptrs, out_ptrs)
+
+    @staticmethod
+    def _views_args(views_params, objects: Sequence[SceneObject], view_modelviews, color_ptrs, out_ptrs):
+        """ctypes arguments of gs_render_scene_views[_async] (and the stereo calls): view_modelviews[v][k] is entity k's
+        modelview of view v."""
+        n = len(views_params)
+        assert len(out_ptrs) == n
+        arr = (GsRenderParams * max(n, 1))()
+        for i in range(n):
+            C.memmove(C.addressof(arr[i]), C.addressof(views_params[i]), C.sizeof(GsRenderParams))
+        mv = np.ascontiguousarray(np.asarray(view_modelviews, np.float32).reshape(n, len(objects), 16))
         col = None
         if color_ptrs is not None:
-            col = (C.c_void_p * 2)(*[None if p is None else C.c_void_p(p) for p in color_ptrs])
-        outs = (C.c_void_p * 2)(*[C.c_void_p(p) for p in out_ptrs])
+            col = (C.c_void_p * max(n, 1))(*[None if p is None else C.c_void_p(p) for p in color_ptrs])
+        outs = (C.c_void_p * max(n, 1))(*[C.c_void_p(p) for p in out_ptrs])
         return arr, make_objects(objects), mv, col, outs
 
     def render_scene_stereo(self, eyes: Sequence[FrameInputs], objects: Sequence[SceneObject], eye_modelviews,
@@ -319,6 +327,45 @@ class SplatContext:
         t = C.c_uint64()
         self._check(self._lib.gs_render_scene_stereo_async(self._h, arr, objs, mv.ctypes.data_as(C.POINTER(C.c_float)),
                                                            len(objects), col, ptrs, C.byref(t)))
+        return t.value
+
+    def render_scene_views(self, views: Sequence[FrameInputs], objects: Sequence[SceneObject], view_mvs,
+                           color_in=None, depth_in=None, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
+                           blend_unorm8: bool = False):
+        """gs_render_scene_views: every view of one WebXR frame (1..GS_MAX_VIEWS FrameInputs, each at its own size) from
+        one head sort.  view_mvs[v][k] is entity k's modelview of view v; color_in[v] / depth_in[v] as in
+        render_scene_stereo (None = none for every view).  Returns one frame per view, row 0 = bottom."""
+        n = len(views)
+        color_in = [None] * n if color_in is None else list(color_in)
+        depth_in = [None] * n if depth_in is None else list(depth_in)
+        dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
+        outs = [np.empty((v.height, v.width, 4), dtype) for v in views]
+        cols = []
+        for v, c in zip(views, color_in):
+            if c is not None:
+                c = np.ascontiguousarray(c, dtype=dtype)
+                if c.size != v.width * v.height * 4:
+                    raise ValueError("color_in must hold width*height RGBA pixels")
+            cols.append(c)
+        params = [self.make_params(v, bg, fmt, _blend8(blend_unorm8), depth_in=d) for v, d in zip(views, depth_in)]
+        arr, objs, mv, col, ptrs = self._views_args(params, objects, view_mvs,
+                                                    [None if c is None else c.ctypes.data for c in cols],
+                                                    [o.ctypes.data for o in outs])
+        st = GsStats()
+        self._check(self._lib.gs_render_scene_views(self._h, arr, n, objs, mv.ctypes.data_as(C.POINTER(C.c_float)),
+                                                    len(objects), col, ptrs, C.byref(st)))
+        self.last_stats = st
+        return outs
+
+    def render_scene_views_async(self, views_params, objects: Sequence[SceneObject], view_mvs, color_ptrs, out_ptrs) -> int:
+        """gs_render_scene_views_async: enqueue one views scene frame (collected with wait()).  views_params: one
+        GsRenderParams per view; color_ptrs: None or one pointer per view (each None, host, or device with
+        GS_RENDER_COLOR_DEVICE); out_ptrs: one pointer per view.  Every buffer must stay valid until the ticket is waited for."""
+        arr, objs, mv, col, ptrs = self._views_args(views_params, objects, view_mvs, color_ptrs, out_ptrs)
+        t = C.c_uint64()
+        self._check(self._lib.gs_render_scene_views_async(self._h, arr, len(views_params), objs,
+                                                          mv.ctypes.data_as(C.POINTER(C.c_float)), len(objects), col, ptrs,
+                                                          C.byref(t)))
         return t.value
 
     # -- frames drawn into the caller's framebuffer in place (gs_render_scene*_target) --
@@ -382,12 +429,40 @@ class SplatContext:
         return color
 
     def _stereo_target_args(self, eyes, fmt, objects, eye_modelviews, eye_xy, flags: int = 0):
-        params = [e if isinstance(e, GsRenderParams) else self.make_params(e, fmt=fmt, flags=flags) for e in eyes]
-        arr, objs, mv, _, _ = self._stereo_args(params, objects, eye_modelviews, None, [0, 0])
+        assert len(eyes) == 2
         if eye_xy is None:
-            eye_xy = (0, 0, params[0].width, 0)
-        xy = (C.c_uint32 * 4)(*[int(v) for v in eye_xy])
+            eye_xy = (0, 0, (eyes[0].width), 0)
+        return self._views_target_args(eyes, fmt, objects, eye_modelviews, eye_xy, flags)
+
+    def _views_target_args(self, views, fmt, objects, view_mvs, view_xy, flags: int = 0):
+        params = [v if isinstance(v, GsRenderParams) else self.make_params(v, fmt=fmt, flags=flags) for v in views]
+        arr, objs, mv, _, _ = self._views_args(params, objects, view_mvs, None, [0] * len(params))
+        xy = (C.c_uint32 * (2 * len(params)))(*[int(v) for v in view_xy])
         return arr, objs, mv.ctypes.data_as(C.POINTER(C.c_float)), xy, mv
+
+    def render_scene_views_target(self, views: Sequence[FrameInputs], objects: Sequence[SceneObject], view_mvs,
+                                  color: np.ndarray, view_xy, depth: Optional[np.ndarray] = None, fmt: int = GS_FORMAT_RGBA8,
+                                  blend_unorm8: bool = False) -> np.ndarray:
+        """gs_render_scene_views_target: one WebXR frame of every view drawn IN PLACE into one layer ((rows, pitch, 4)
+        colour, optional (rows, pitch) f32 depth): view v at (view_xy[2v], view_xy[2v+1]).  Arguments as
+        render_scene_views.  Returns `color`."""
+        t = self._host_target(color, depth, fmt)
+        st = GsStats()
+        args = self._views_target_args(views, fmt, objects, view_mvs, view_xy, _blend8(blend_unorm8))
+        self._check(self._lib.gs_render_scene_views_target(self._h, args[0], len(views), args[1], args[2], len(objects),
+                                                           C.byref(t), args[3], C.byref(st)))
+        self.last_stats = st
+        return color
+
+    def render_scene_views_target_async(self, views_params, objects: Sequence[SceneObject], view_mvs, target: GsTarget,
+                                        view_xy) -> int:
+        """gs_render_scene_views_target_async: enqueue one views scene frame into `target` (make_target), view v at
+        (view_xy[2v], view_xy[2v+1]); collected with wait().  The target's buffers must stay valid until then."""
+        args = self._views_target_args(views_params, None, objects, view_mvs, view_xy)
+        t = C.c_uint64()
+        self._check(self._lib.gs_render_scene_views_target_async(self._h, args[0], len(views_params), args[1], args[2],
+                                                                 len(objects), C.byref(target), args[3], C.byref(t)))
+        return t.value
 
     def render_scene_stereo_target_async(self, eyes_params, objects: Sequence[SceneObject], eye_modelviews,
                                          target: GsTarget, eye_xy) -> int:

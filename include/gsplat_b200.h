@@ -89,9 +89,9 @@ enum {
  *   - expw(x) = exp(-x) for x in [0, 4], fixed fp32 operations in this order (no FMA): k = rint(-x * 0x1.715476p+0);
  *     r = (-x - k * 0x1.62e4p-1) - k * 0x1.7f7d1cp-20; p = Horner of 1 + r + r^2/2! + ... + r^7/7! from the r^7 term
  *     (coefficients the fp32 values nearest 1/7! ... 1/2!, then 1, 1); expw = p * 2^k.  expw(0) = 1.
- * Accepted by gs_render[_async], gs_render_stereo, gs_render_scene[_async], gs_render_scene_stereo[_async] and both
- * *_target[_async] entry points, with GS_RENDER_REUSE_SORT and GS_RENDER_STATS where those accept them, depth and colour
- * targets and host or device buffers.  Such a frame is always one-pass (never the slab path, whatever GS_SLAB_MIN /
+ * Accepted by gs_render[_async], gs_render_stereo, gs_render_scene[_async], gs_render_scene_stereo[_async],
+ * gs_render_scene_views[_async] and every *_target[_async] entry point, with GS_RENDER_REUSE_SORT and GS_RENDER_STATS
+ * where those accept them, depth and colour targets and host or device buffers.  Such a frame is always one-pass (never the slab path, whatever GS_SLAB_MIN /
  * GS_SLAB_MIN_XR say: gs_stats.n_slabs is 0) and always uses the two-pixel raster loop (GS_RASTER=scalar does not apply).
  * GS_RENDER_STATS counts this loop's pairs: n_pair_hits is every blended pair.  Refused with GS_ERR_INVALID, changing
  * nothing: GS_FORMAT_RGBA32F, GS_RENDER_OUT_TILED and GS_RENDER_OUT_PEER.
@@ -436,6 +436,49 @@ GS_API int gs_render_scene_stereo_target_async(gs_context *ctx, const gs_render_
 GS_API int gs_render_scene_stereo_target(gs_context *ctx, const gs_render_params eyes[2], const gs_object *objs,
                                          const float *eye_modelviews, uint32_t n_objs, const gs_target *layer,
                                          const uint32_t eye_xy[4], gs_stats *stats);
+
+/*
+ * Every view of a WebXR frame, 1..GS_MAX_VIEWS of them, each at its own size (three.js draws one camera per XRView of the
+ * viewer pose, each at XRWebGLLayer.getViewport(view), and material.onBeforeRender reads that camera's viewport,
+ * index.js:184-195): two eyes plus a first-person-observer view, or the two context views and two focus insets of a
+ * quad-view device.  One head sort per frame (index.js:438-455) serves every view, as in gs_render_scene_stereo.
+ *   - objs[k]: as in gs_render_scene_stereo (range, HEAD getModelViewMatrix(), cutout).
+ *   - view_modelviews: n_views * n_objs * 16 floats; entity k's getModelViewMatrix(viewCamera) of view v starts at
+ *     (v * n_objs + k) * 16.
+ *   - views[v]: view v's projection, its own width x height (1..4096 per side), focal, bg_rgba, out_format and depth_in;
+ *     its modelview and cutout are ignored.  Every view has the same flags and out_format.
+ *   - color_in: NULL, or color_in[v] NULL or view v's colour target; out_rgba[v]: view v's frame.
+ * Each view's frame is the chain of per-entity draws of gs_render_scene in the head order, with the view's matrices and
+ * viewport: byte-identical to the frame gs_render_scene_stereo gives for that view paired with itself, on the one-pass and
+ * the slab path.  n_views = 2 with equal sizes is gs_render_scene_stereo.  One pipelined frame covers every view: one
+ * sort, one projection and one binning pass, one raster grid over every view's tiles; the kernel launches do not depend
+ * on n_views.  The path follows gs_render_scene_stereo's rule (GS_SLAB_MIN_XR).
+ * Returns GS_ERR_INVALID, changing nothing, for: n_views 0 or above GS_MAX_VIEWS, unequal flags or out_formats, and
+ * whatever gs_render_scene_stereo refuses except unequal sizes.  gs_stats: n_sorted, n_dropped, min_depth and max_depth
+ * of the one sort; n_visible, n_instances, n_instances_kept and n_tiles summed over the views; width and height of view 0.
+ * GS_MAX_VIEWS bounds the per-slot view table, which has a fixed size because captured graphs bake its address; four
+ * covers quad views and two eyes plus an observer.  Memory: each view beyond the first holds 36 B per resident splat in
+ * each of the two pipeline buffer sets, allocated up to the largest view count the context has drawn.
+ */
+#define GS_MAX_VIEWS 4
+GS_API int gs_render_scene_views_async(gs_context *ctx, const gs_render_params *views, uint32_t n_views,
+                                       const gs_object *objs, const float *view_modelviews, uint32_t n_objs,
+                                       const void *const *color_in, void *const *out_rgba, uint64_t *out_ticket);
+GS_API int gs_render_scene_views(gs_context *ctx, const gs_render_params *views, uint32_t n_views, const gs_object *objs,
+                                 const float *view_modelviews, uint32_t n_objs, const void *const *color_in,
+                                 void *const *out_rgba, gs_stats *stats);
+/*
+ * A views frame drawn into one layer: view v into the rectangle at (view_xy[2v], view_xy[2v+1]) of views[v].width x
+ * views[v].height.  Each view's rectangle equals that view's gs_render_scene_views frame over the rectangle's colour and
+ * depth, byte for byte, on either path.  The rules of gs_render_scene_target apply to each view, plus those of
+ * gs_render_scene_views; overlapping view rectangles are refused.
+ */
+GS_API int gs_render_scene_views_target_async(gs_context *ctx, const gs_render_params *views, uint32_t n_views,
+                                              const gs_object *objs, const float *view_modelviews, uint32_t n_objs,
+                                              const gs_target *layer, const uint32_t *view_xy, uint64_t *out_ticket);
+GS_API int gs_render_scene_views_target(gs_context *ctx, const gs_render_params *views, uint32_t n_views,
+                                        const gs_object *objs, const float *view_modelviews, uint32_t n_objs,
+                                        const gs_target *layer, const uint32_t *view_xy, gs_stats *stats);
 
 /* Per-splat projected record of the last gs_render (testing the vertex-shader restatement):
  * 8 floats per resident splat {cx, cy, a1x, a1y, a2x, a2y, rgba8-as-bits, tile-rect-as-bits};
