@@ -1348,6 +1348,22 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   return GS_OK;
 }
 
+// A frame into a host gs_target that is refused: its overflowed run stored nothing, but its read-back still copied the
+// frame buffer into the rectangles, so the colour staged at submission is copied back.  (A device target is drawn in
+// place, and an overflowed run leaves it untouched.)
+static int restore_host_target(gs_context *c, gs_context::Slot &sl) {
+  if (!sl.target || sl.target_device) return GS_OK;
+  for (uint32_t e = 0; e < sl.n_views; ++e) {
+    const gs_render_params &vp = sl.view[e];
+    const size_t px_bytes = vp.out_format == GS_FORMAT_RGBA8 ? 4 : 16, row = px_bytes * vp.width;
+    char *dst = (char *)sl.tcolor + ((size_t)sl.torg[e][1] * sl.tpitch + sl.torg[e][0]) * px_bytes;
+    GS_CUDA(c, cudaMemcpy2DAsync(dst, px_bytes * sl.tpitch, sl.color_dev[e], row, row, vp.height, cudaMemcpyDeviceToHost,
+                                 c->copy_stream));
+  }
+  GS_CUDA(c, cudaStreamSynchronize(c->copy_stream));
+  return GS_OK;
+}
+
 static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   if (!sl.pending) return fail(c, GS_ERR_INVALID, "gs_wait: no frame in flight for this ticket");
   for (int attempt = 0;; ++attempt) {
@@ -1367,7 +1383,11 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
       break;
     }
     if (!sl.ctr_host->overflow) break;
-    if (attempt == 7) return fail(c, GS_ERR_CAPACITY, "instance buffer kept overflowing");
+    if (attempt == 7) {
+      c->have_last_sorted = false;
+      int rcode = restore_host_target(c, sl);
+      return rcode ? rcode : fail(c, GS_ERR_CAPACITY, "instance buffer kept overflowing");
+    }
     // Instance buffer too small.  Frames submitted BEFORE this one that are still pending saw the same small
     // buffer: finish (and, if needed, re-run) them first so frames are always re-run in submission order and
     // last_set / have_order end up describing the most recently submitted frame.
@@ -1388,7 +1408,13 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
     if (demand > c->cap_inst) {
       const uint64_t need = std::max<uint64_t>(demand + demand / 8, c->cap_inst + c->cap_inst / 2);
       int rcode = ensure_instances(c, need);
-      if (rcode) return rcode;
+      if (rcode) {
+        // a refused frame leaves no sorted count behind: the next frame picks its path from the splats it may sort, as
+        // on a fresh context, not from the count of whatever frame completed before the refused one
+        c->have_last_sorted = false;
+        int rc_t = restore_host_target(c, sl);
+        return rc_t ? rc_t : rcode;
+      }
     }
     int rcode;
     sl.restage = false;  // a target frame blends over the rectangles staged at its first submission
