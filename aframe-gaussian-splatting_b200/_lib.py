@@ -76,6 +76,8 @@ SYMBOLS = {
     "gs_push_packed": (C.c_int, [_P, _P, _P, _P, C.c_uint32]),
     "gs_num_splats": (C.c_int, [_P, C.POINTER(C.c_uint32)]),
     "gs_read_packed": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P]),
+    "gs_set_sh_degree": (C.c_int, [_P, C.c_uint32]),
+    "gs_read_sh": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
     "gs_sort": (C.c_int, [_P, C.POINTER(C.c_float), C.POINTER(C.c_float), _P, C.POINTER(C.c_uint32)]),
     "gs_render": (C.c_int, [_P, C.POINTER(GsRenderParams), _P, C.POINTER(GsStats)]),
     "gs_render_async": (C.c_int, [_P, C.POINTER(GsRenderParams), _P, C.POINTER(C.c_uint64)]),

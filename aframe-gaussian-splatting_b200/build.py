@@ -16,7 +16,7 @@ NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "--fmad=false",  # no implicit FMA contraction: parity needs the written op order (DESIGN.md)
-    "-Xcompiler", "-fPIC,-fvisibility=hidden",
+    "-Xcompiler", "-fPIC,-fvisibility=hidden,-ffp-contract=off",  # host fp64 too (the SH camera position)
     "-shared",
 ]
 

@@ -294,8 +294,12 @@ class SplatScene:
     rows append.  No row is kept on the host.
     """
 
-    def __init__(self, renderer: Optional[SplatContext] = None, device: int = 0):
-        self.renderer = renderer or SplatContext(device)
+    def __init__(self, renderer: Optional[SplatContext] = None, device: int = 0, sh_degree: int = 0):
+        """sh_degree 1..3: .ply entities keep their spherical harmonics and draw their view-dependent colour (each view
+        from its own camera); 0 draws the reference's flat colour.  A given renderer takes the degree while it is empty."""
+        self.renderer = renderer or SplatContext(device, sh_degree=sh_degree)
+        if renderer is not None and sh_degree:
+            renderer.set_sh_degree(sh_degree)
         self.entities: list = []   # components, in draw order
         self._order: list = []     # components, in table order (an empty range's place is its position here)
         self._range: dict = {}     # id(component) -> [first, count]

@@ -62,21 +62,27 @@ static int ensure_table(gs_context *c, uint64_t need, bool exact = false) {
   float4 *cs = nullptr;
   uint4 *cc = nullptr;
   float *sa = nullptr;
+  uint4 *sh = nullptr;
   GS_CUDA(c, dev_alloc(&cs, ncap));
   GS_CUDA(c, dev_alloc(&cc, ncap));
   GS_CUDA(c, dev_alloc(&sa, ncap));
+  if (c->sh_vecs) GS_CUDA(c, dev_alloc(&sh, ncap * c->sh_vecs));  // SH contexts: the coefficients grow with the table
   if (c->n) {
     GS_CUDA(c, cudaMemcpyAsync(cs, c->center_scale, sizeof(float4) * c->n, cudaMemcpyDeviceToDevice, c->push_stream));
     GS_CUDA(c, cudaMemcpyAsync(cc, c->cov_color, sizeof(uint4) * c->n, cudaMemcpyDeviceToDevice, c->push_stream));
     GS_CUDA(c, cudaMemcpyAsync(sa, c->size_alpha, sizeof(float) * c->n, cudaMemcpyDeviceToDevice, c->push_stream));
+    if (sh)
+      GS_CUDA(c, cudaMemcpyAsync(sh, c->sh, sizeof(uint4) * c->sh_vecs * c->n, cudaMemcpyDeviceToDevice, c->push_stream));
   }
   GS_CUDA(c, cudaStreamSynchronize(c->push_stream));
   dev_free(c->center_scale);
   dev_free(c->cov_color);
   dev_free(c->size_alpha);
+  dev_free(c->sh);
   c->center_scale = cs;
   c->cov_color = cc;
   c->size_alpha = sa;
+  c->sh = sh;
   c->cap = (uint32_t)ncap;
   return GS_OK;
 }
@@ -384,7 +390,7 @@ extern "C" int gs_destroy(gs_context *c) {
   if (c->stream) cudaStreamSynchronize(c->stream);
   if (c->bstream) cudaStreamSynchronize(c->bstream);
   if (c->rstream) cudaStreamSynchronize(c->rstream);
-  dev_free(c->center_scale); dev_free(c->cov_color); dev_free(c->size_alpha);
+  dev_free(c->center_scale); dev_free(c->cov_color); dev_free(c->size_alpha); dev_free(c->sh);
   dev_free(c->depth); dev_free(c->idx_a); dev_free(c->dig_a);
   for (int i = 0; i < 2; ++i) { dev_free(c->order[i]); dev_free(c->proj_rec[i]); dev_free(c->rect[i]); }
   for (int i = 0; i < 2; ++i) { dev_free(c->proj_recx[i]); dev_free(c->rectx[i]); }
@@ -424,7 +430,8 @@ extern "C" int gs_destroy(gs_context *c) {
       if (sl.depth_dev[e]) cudaFree(sl.depth_dev[e]);
       if (sl.color_dev[e]) cudaFree(sl.color_dev[e]);
     }
-    dev_free(sl.scene_dev); dev_free(sl.octr); dev_free(sl.stereo_dev);
+    dev_free(sl.scene_dev); dev_free(sl.octr); dev_free(sl.stereo_dev); dev_free(sl.sh_cam_dev);
+    if (sl.sh_cam_host) cudaFreeHost(sl.sh_cam_host);
     if (sl.scene_host) cudaFreeHost(sl.scene_host);
     if (sl.stereo_host) cudaFreeHost(sl.stereo_host);
     if (sl.ctr_host) cudaFreeHost(sl.ctr_host);
@@ -470,6 +477,44 @@ extern "C" int gs_clear(gs_context *c) {
   return GS_OK;
 }
 
+extern "C" int gs_set_sh_degree(gs_context *c, uint32_t degree) {
+  if (!c) return GS_ERR_INVALID;
+  if (degree > 3) return fail(c, GS_ERR_INVALID, "gs_set_sh_degree: the degree is 0, 1, 2 or 3");
+  if (c->n) return fail(c, GS_ERR_INVALID, "gs_set_sh_degree: the table is not empty");
+  if (degree == c->sh_degree) return GS_OK;
+  GS_CUDA(c, cudaSetDevice(c->device));
+  int rc0 = drain(c);  // frames of an earlier table may still be in flight
+  if (rc0) return rc0;
+  GS_CUDA(c, cudaStreamSynchronize(c->push_stream));
+  uint4 *sh = nullptr;
+  if (degree) GS_CUDA(c, dev_alloc(&sh, (size_t)c->cap * sh_vecs(degree)));
+  dev_free(c->sh);
+  c->sh = sh;
+  c->sh_degree = degree;
+  c->sh_vecs = sh_vecs(degree);  // the graph key holds the degree and c->sh: the next frame captures its own graphs
+  return GS_OK;
+}
+
+extern "C" int gs_read_sh(gs_context *c, uint32_t first, uint32_t n, uint16_t *out) {
+  if (!c) return GS_ERR_INVALID;
+  if (!c->sh_degree) return fail(c, GS_ERR_INVALID, "gs_read_sh: the context keeps no SH (degree 0)");
+  if ((uint64_t)first + n > c->n || (n && !out)) return fail(c, GS_ERR_INVALID, "gs_read_sh: range past the resident splats");
+  if (!n) return GS_OK;
+  GS_CUDA(c, cudaSetDevice(c->device));
+  GS_CUDA(c, cudaStreamSynchronize(c->push_stream));  // pushes are asynchronous
+  const size_t row = 3 * sizeof(uint16_t) * sh_coeffs(c->sh_degree);
+  GS_CUDA(c, cudaMemcpy2D(out, row, c->sh + (size_t)first * c->sh_vecs, sizeof(uint4) * c->sh_vecs, row, n,
+                          cudaMemcpyDeviceToHost));
+  return GS_OK;
+}
+
+// SH contexts: rows [first, first + n) of the SH table become zeros (rows without coefficients: .splat and packed pushes)
+static int zero_sh(gs_context *c, uint32_t first, uint32_t n) {
+  if (c->sh)
+    GS_CUDA(c, cudaMemsetAsync(c->sh + (size_t)first * c->sh_vecs, 0, sizeof(uint4) * c->sh_vecs * n, c->push_stream));
+  return GS_OK;
+}
+
 extern "C" int gs_num_splats(const gs_context *c, uint32_t *out_n) {
   if (!c || !out_n) return GS_ERR_INVALID;
   *out_n = c->n;
@@ -501,7 +546,7 @@ static int begin_move(gs_context *c, uint32_t from, uint32_t to, uint32_t len, v
   *tmp = nullptr;
   int rc = drain(c);
   if (rc) return rc;
-  const size_t bytes = move_tmp_bytes(from, to, len);
+  const size_t bytes = move_tmp_bytes(from, to, len, c->sh ? c->sh_vecs : 0u);
   const cudaError_t e = bytes ? cudaMallocAsync(tmp, bytes, c->push_stream) : cudaSuccess;
   if (e) cudaGetLastError();  // an allocation failure is not sticky: do not leave it for the next launch check
   GS_CUDA(c, e);
@@ -540,6 +585,7 @@ static int insert_rows(gs_context *c, uint32_t at, const void *rows32, uint32_t 
     GS_CUDA(c, cudaGetLastError());
     GS_CUDA(c, cudaEventRecord(c->push_ev[b], c->push_stream));
   }
+  if ((rc = zero_sh(c, at, n))) return rc;
   GS_CUDA(c, cudaEventRecord(c->push_done, c->push_stream));
   c->n += n;
   c->pushed = true;
@@ -591,9 +637,13 @@ static int ensure_ply_staging(gs_context *c) {
 static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes, void *rows32_out_or_null, uint32_t *out_n) {
   if (out_n) *out_n = 0;
   PlyLayout L;
+  PlyShLayout S{};
+  S.ctx_k = sh_coeffs(c->sh_degree);
+  S.vecs = c->sh_vecs;
+  PlyShLayout *sh = c->sh_degree ? &S : nullptr;
   uint32_t n = 0;
   size_t data_off = 0;
-  if (ply_parse((const uint8_t *)ply, bytes, L, n, data_off, c->err)) return GS_ERR_INVALID;  // nothing changed yet
+  if (ply_parse((const uint8_t *)ply, bytes, L, n, data_off, c->err, sh)) return GS_ERR_INVALID;  // nothing changed yet
   if (!n) return GS_OK;
   GS_CUDA(c, cudaSetDevice(c->device));
   int rc;
@@ -608,8 +658,9 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   const size_t stride = L.stride, rows_per_chunk = gs_context::kPlyChunkBytes / stride;
   uint8_t *rows_dev = nullptr, *out_dev = nullptr, *body[2] = {nullptr, nullptr};
   uint32_t *key = nullptr, *perm_a = nullptr, *perm_b = nullptr, *table = nullptr, *totals = nullptr;
+  uint4 *sh_dev = nullptr;  // SH contexts: the decoded coefficients, in file order
   auto release = [&]() {
-    void *ps[] = {rows_dev, out_dev, body[0], body[1], key, perm_a, perm_b, table, totals, move_tmp};
+    void *ps[] = {rows_dev, out_dev, body[0], body[1], key, perm_a, perm_b, table, totals, move_tmp, sh_dev};
     for (void *p : ps)
       if (p) cudaFreeAsync(p, st);
   };
@@ -623,6 +674,7 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   if (!e && sort) e = cudaMallocAsync((void **)&table, (size_t)256 * (chunks + 1) * 4, st);
   if (!e && sort) e = cudaMallocAsync((void **)&totals, (size_t)256 * 4, st);
   if (!e && rows32_out_or_null) e = cudaMallocAsync((void **)&out_dev, (size_t)n * 32, st);
+  if (!e && sh) e = cudaMallocAsync((void **)&sh_dev, (size_t)n * sizeof(uint4) * S.vecs, st);
   if (e) {
     release();
     GS_CUDA(c, e);
@@ -637,7 +689,7 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
     memcpy(c->ply_pinned[b], src + (size_t)r0 * stride, (size_t)m * stride);
     if ((e = cudaMemcpyAsync(body[b], c->ply_pinned[b], (size_t)m * stride, cudaMemcpyHostToDevice, st))) break;
     if ((e = cudaEventRecord(c->ply_ev[b], st))) break;
-    launch_ply_decode(body[b], m, L, r0, rows_dev, key, st);
+    launch_ply_decode(body[b], m, L, r0, rows_dev, key, sh, sh_dev, st);
     e = cudaGetLastError();
   }
   const uint32_t *perm = nullptr;
@@ -647,7 +699,7 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   }
   if (!e) {
     launch_move_rows(c, at, at + n, tail, move_tmp, st);  // opens the gap for the rows (nothing to move for an append)
-    launch_pack_perm(c, rows_dev, perm, at, n, out_dev, st);
+    launch_pack_perm(c, rows_dev, perm, at, n, out_dev, sh_dev, st);
     e = cudaGetLastError();
   }
   if (!e && rows32_out_or_null) e = cudaMemcpyAsync(rows32_out_or_null, out_dev, (size_t)n * 32, cudaMemcpyDeviceToHost, st);
@@ -685,6 +737,7 @@ extern "C" int gs_push_packed(gs_context *c, const float *center_scale4, const u
   GS_CUDA(c, cudaMemcpyAsync(c->center_scale + c->n, center_scale4, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, c->push_stream));
   GS_CUDA(c, cudaMemcpyAsync(c->cov_color + c->n, cov_color4, sizeof(uint4) * (size_t)n, cudaMemcpyHostToDevice, c->push_stream));
   GS_CUDA(c, cudaMemcpyAsync(c->size_alpha + c->n, size_alpha, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, c->push_stream));
+  if ((rc = zero_sh(c, c->n, n))) return rc;
   GS_CUDA(c, cudaStreamSynchronize(c->push_stream));  // pageable sources: the caller may reuse them on return
   GS_CUDA(c, cudaEventRecord(c->push_done, c->push_stream));
   c->n += n;
@@ -831,6 +884,7 @@ extern "C" uint32_t gs_owned_tiles(uint32_t width, uint32_t height, uint32_t ran
 
 static FrameBufs slot_bufs(gs_context *c, const gs_context::Slot &sl) {
   FrameBufs b{c->order[sl.set], c->proj_rec[sl.set], c->rect[sl.set], c->inst_rec[sl.set], c->bin_range[sl.set]};
+  b.sh_cam = sl.sh_cam_dev;
   if (sl.stereo) {
     b.views = true;
     if (sl.n_views > 1) {
@@ -852,6 +906,8 @@ static gs_context::GraphKey graph_key(const gs_context *c, const gs_context::Slo
   gs_context::GraphKey k;
   k.cap = c->cap; k.n_tiles = n_tiles; k.n_bins = n_bins; k.cap_inst = c->cap_inst; k.p0 = c->depth; k.p1 = c->inst_rec[0]; k.p2 = c->center_scale;
   k.p3 = c->scene_key;
+  k.psh = c->sh;
+  k.sh_degree = c->sh_degree;
   if (sl.stereo) {
     k.n_views = sl.n_views;
     for (uint32_t v = 0; v < sl.n_views; ++v) k.view_size[v] = sl.view[v].width | sl.view[v].height << 16;
@@ -1157,6 +1213,27 @@ static int enqueue_readback(gs_context *c, gs_context::Slot &sl) {
   return GS_OK;
 }
 
+// SH contexts: the camera position of gsModelViewMatrix mv in the table's frame, cam = -A^-1 t (A: mv's upper 3x3, column
+// a, b, c; t: its translation), by Cramer's rule in fp64 in exactly this order, then rounded to f32 (DESIGN.md section 3;
+// tests/sh_oracle.c restates it).  With u = -t and det[p q r] = p . (q x r), dots left to right:
+//   bc = b x c, det = a . bc;  x = (u . bc) / det, y = (a . (u x c)) / det, z = (a . (b x u)) / det
+static void sh_camera(const float mv[16], float4 &cam) {
+  const double a[3] = {mv[0], mv[1], mv[2]}, b[3] = {mv[4], mv[5], mv[6]}, c[3] = {mv[8], mv[9], mv[10]};
+  const double u[3] = {-(double)mv[12], -(double)mv[13], -(double)mv[14]};
+  auto cross = [](const double *p, const double *q, double *r) {
+    r[0] = p[1] * q[2] - p[2] * q[1];
+    r[1] = p[2] * q[0] - p[0] * q[2];
+    r[2] = p[0] * q[1] - p[1] * q[0];
+  };
+  auto dot = [](const double *p, const double *q) { return (p[0] * q[0] + p[1] * q[1]) + p[2] * q[2]; };
+  double bc[3], uc[3], bu[3];
+  cross(b, c, bc);
+  cross(u, c, uc);
+  cross(b, u, bu);
+  const double det = dot(a, bc);
+  cam = make_float4((float)(dot(u, bc) / det), (float)(dot(a, uc) / det), (float)(dot(a, bu) / det), 0.0f);
+}
+
 // a frame's RenderConsts from its parameters
 static void fill_render_consts(gs_context *c, const gs_render_params *p, RenderConsts &rc) {
   memcpy(rc.proj, p->proj, sizeof(rc.proj));
@@ -1331,6 +1408,16 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   }
   // the scene table goes ahead of the sort stage on its stream (only the entities in use are copied)
   if (sl.scene) GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, sl.scene_bytes, cudaMemcpyHostToDevice, c->stream));
+  if (c->sh_degree) {
+    // SH contexts: the camera position of every modelview the projection uses, entity k's view v at k * kMaxViews + v
+    const uint32_t n_ent = sl.scene ? sl.scene_host->n : 1u;
+    for (uint32_t k = 0; k < n_ent; ++k)
+      for (uint32_t v = 0; v < sl.n_views; ++v)
+        sh_camera(sl.stereo ? sl.stereo_host->mv[k][v] : (sl.scene ? sl.scene_host->obj[k].mv : p->modelview),
+                  sl.sh_cam_host[k * kMaxViews + v]);
+    GS_CUDA(c, cudaMemcpyAsync(sl.sh_cam_dev, sl.sh_cam_host, sizeof(float4) * kMaxViews * std::max(n_ent, 1u),
+                               cudaMemcpyHostToDevice, c->stream));
+  }
   const bool reuse = !sl.scene && (p->flags & GS_RENDER_REUSE_SORT) && c->have_order;
   // a frame normally takes the buffer set the previous frame did not; a frame that reuses the last sort must read
   // that sort's set, so it runs in it
@@ -1623,6 +1710,10 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     sl.tdepth = target->t->depth;
     sl.tpitch = target->t->pitch;
     memcpy(sl.torg, target->xy, sizeof(sl.torg));
+  }
+  if (c->sh_degree && !sl.sh_cam_dev) {  // SH contexts: the slot's camera table, fixed size, allocated once
+    GS_CUDA(c, cudaMalloc((void **)&sl.sh_cam_dev, sizeof(float4) * kMaxObjects * kMaxViews));
+    GS_CUDA(c, cudaHostAlloc((void **)&sl.sh_cam_host, sizeof(float4) * kMaxObjects * kMaxViews, cudaHostAllocDefault));
   }
   sl.scene = scene != nullptr;
   if (scene) {

@@ -194,9 +194,22 @@ struct PlyLayout {
   uint32_t all_f32;                           // every field read is a 4-byte-aligned float and the stride is a multiple of 4
   PlyField f[PF_COUNT];                       // the LAST property of each name (offsets[name] is overwritten, index.js:628-629)
 };
+// ---- spherical harmonics (gs_set_sh_degree): per splat 3 K fp16 coefficients, K = (d + 1)^2 - 1, channel-major (R's K,
+// then G's, then B's: INRIA's f_rest order), padded to whole 16 B words ----
+constexpr int kMaxShCoeffs = 15;  // K of degree 3
+__host__ __device__ constexpr uint32_t sh_coeffs(uint32_t degree) { return (degree + 1) * (degree + 1) - 1; }
+__host__ __device__ constexpr uint32_t sh_vecs(uint32_t degree) { return (3 * sh_coeffs(degree) * 2 + 15) / 16; }  // 0, 2, 3, 6
+// f_rest_* fields of a PLY file (SH contexts): file_k = K of the file's degree (the largest d <= 3 whose 3 K f_rest_* all
+// exist), ctx_k = the context's K; coefficient k (1..ctx_k) of channel c is field f[c * file_k + k - 1] when k <= file_k, else 0
+struct PlyShLayout {
+  uint32_t file_k, ctx_k, vecs;
+  PlyField f[3 * kMaxShCoeffs];
+};
 // Parses the header of a whole PLY file with the reference's rules.  Returns GS_OK, or GS_ERR_INVALID with `err` set to the
-// reference's message (header, missing property, short body).
-int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_t &data_off, std::string &err);
+// reference's message (header, missing property, short body).  sh (SH contexts, sh->ctx_k set by the caller) also
+// receives the file's f_rest_* fields, and the fast all-f32 path then also requires them to be aligned floats.
+int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_t &data_off, std::string &err,
+              PlyShLayout *sh = nullptr);
 
 // ---- front-to-back slab path ----
 constexpr int kMaxSlabs = 12;         // geometric slab sizes: 1 M, 2 M, 4 M ... entries (nearest first)
@@ -231,6 +244,9 @@ struct gs_context {
   float4 *center_scale = nullptr;
   uint4 *cov_color = nullptr;
   float *size_alpha = nullptr;
+  // spherical-harmonic coefficients (gs_set_sh_degree; none at degree 0): sh_vecs 16 B words per splat, row i = splat i
+  uint32_t sh_degree = 0, sh_vecs = 0;
+  uint4 *sh = nullptr;
 
   // ---- per-splat scratch (sized to cap) ----
   uint32_t scratch_cap = 0;
@@ -335,6 +351,10 @@ struct gs_context {
     gs::SceneTable *scene_host = nullptr;    // pinned staging
     size_t scene_bytes = 0;                  // bytes of the table in use (header + non-empty entities)
     gs::ObjCounters *octr = nullptr;         // [kMaxObjects] per-entity depth-pass results
+    // SH contexts: camera position in the table's frame of every modelview the projection uses, entity k (scene-table
+    // order; 0 for a plain frame) and view v at k * kMaxViews + v.  Fixed size (captured graphs bake the pointer)
+    float4 *sh_cam_dev = nullptr;
+    float4 *sh_cam_host = nullptr;           // pinned staging
     // frames into a gs_target (gs_render_scene*_target): each view drawn in place at its rectangle of the caller's buffers
     bool target = false;
     bool target_device = false;              // GS_TARGET_DEVICE: read and written where they are; else staged per view
@@ -413,6 +433,7 @@ struct gs_context {
   struct GraphKey {
     uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr;
     uint32_t n_views = 0, view_size[gs::kMaxViews] = {}, pad2 = 0; const void *px = nullptr;
+    const void *psh = nullptr; uint32_t sh_degree = 0, pad3 = 0;  // the projection's instantiation and SH table
   } gkey;
   GraphKey gkey_stereo;                          // ... of the views graphs (kept apart: a views frame re-captures only its own)
 
@@ -452,6 +473,7 @@ struct FrameBufs {
   uint32_t x_stride = 0;
   uint32_t bin_base[kMaxViews] = {};
   bool views = false;
+  const float4 *sh_cam = nullptr;  // SH contexts: the slot's camera table (gs_context::Slot::sh_cam_dev)
 };
 
 // -- launchers (each .cu file owns its kernels); every per-frame input comes from device memory (fp, ctr) --
@@ -469,16 +491,19 @@ void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable
 void launch_project_stereo(gs_context *c, const ViewTable *views, const SceneTable *scene, const FrameCounters *ctr,
                            const FrameBufs &b, cudaStream_t st);
 void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_t n, cudaStream_t st);
-// PLY push: k_pack reading row perm[j] (perm NULL: row j) into slot first + j; rows_out (or NULL) receives the ordered rows
+// PLY push: k_pack reading row perm[j] (perm NULL: row j) into slot first + j; rows_out (or NULL) receives the ordered rows;
+// sh_rows (SH contexts): the decoded coefficients, gathered by the same permutation into the SH table
 void launch_pack_perm(gs_context *c, const uint8_t *rows_dev, const uint32_t *perm, uint32_t first, uint32_t n,
-                      uint8_t *rows_out, cudaStream_t st);
-// table edits: bytes of the temporary a move of rows [from, from+len) to [to, to+len) needs (0: the ranges are disjoint)
-size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len);
+                      uint8_t *rows_out, const uint4 *sh_rows, cudaStream_t st);
+// table edits: bytes of the temporary a move of rows [from, from+len) to [to, to+len) needs (0: the ranges are disjoint);
+// sh_vecs: the SH words per row that move with them
+size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len, uint32_t sh_vecs);
 // k_move_rows: one launch for disjoint ranges, else two through tmp
 void launch_move_rows(gs_context *c, uint32_t from, uint32_t to, uint32_t len, void *tmp, cudaStream_t st);
-// PLY push: decode `rows` whole rows of a staged body chunk into .splat rows + importance keys at [first_row, ...)
+// PLY push: decode `rows` whole rows of a staged body chunk into .splat rows + importance keys at [first_row, ...);
+// sh (SH contexts, else NULL): the rows' coefficients into sh_rows (sh->vecs words per row), in file order too
 void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,
-                       uint32_t *key, cudaStream_t st);
+                       uint32_t *key, const PlyShLayout *sh, uint4 *sh_rows, cudaStream_t st);
 // PLY push: stable ascending sort of n 32-bit keys as four 8-bit passes (12 launches); returns the buffer holding the
 // permutation (perm_b).  table: 256 * (ceil(n / kRadixTile) + 1) words, totals: 256 words.
 uint32_t *launch_ply_sort(gs_context *c, const uint32_t *key, uint32_t *perm_a, uint32_t *perm_b, uint32_t *table,

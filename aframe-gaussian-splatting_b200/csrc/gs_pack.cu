@@ -1,7 +1,8 @@
 // gs_pack.cu — load-time pack on the device: the reference's `pushDataBuffer` loop (index.js:343-402).
 //   k_pack      : row i of a staged chunk -> table slot first + i (gs_push_splats)
 //   k_pack_perm : row perm[j] of the decoded PLY rows -> slot first + j, optionally also written out in that order
-//                 (gs_push_ply: the gather of processPlyBuffer's importance order fused with the pack)
+//                 (gs_push_ply: the gather of processPlyBuffer's importance order fused with the pack; on an SH context
+//                 the row's coefficients are gathered with it)
 //   k_move_rows : rows [from, from+len) of the table -> [to, to+len) (gs_insert_* / gs_erase open or close a gap)
 //
 // One thread per .splat row, all arithmetic in fp64 exactly as JavaScript evaluates it (Three.js r147
@@ -128,10 +129,13 @@ __global__ void __launch_bounds__(256) k_pack(const uint4 *__restrict__ rows, ui
 __global__ void __launch_bounds__(256) k_pack_perm(const uint4 *__restrict__ rows, const uint32_t *__restrict__ perm,
                                                    uint32_t first, uint32_t n, float4 *__restrict__ cs,
                                                    uint4 *__restrict__ cc, float *__restrict__ sa,
-                                                   const double *__restrict__ tab, int nt, uint4 *__restrict__ rows_out) {
+                                                   const double *__restrict__ tab, int nt, uint4 *__restrict__ rows_out,
+                                                   const uint4 *__restrict__ sh_rows, uint4 *__restrict__ sh,
+                                                   uint32_t sh_vecs) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
   const uint32_t r = perm ? __ldg(perm + j) : j;
+  for (uint32_t v = 0; v < sh_vecs; ++v) sh[((size_t)first + j) * sh_vecs + v] = __ldg(sh_rows + (size_t)r * sh_vecs + v);
   const uint4 a = __ldg(rows + 2 * (size_t)r);
   const uint4 b = __ldg(rows + 2 * (size_t)r + 1);
   if (rows_out) {
@@ -141,19 +145,20 @@ __global__ void __launch_bounds__(256) k_pack_perm(const uint4 *__restrict__ row
   pack_row(a, b, (size_t)first + j, cs, cc, sa, tab, nt);
 }
 
-// Table edit (gs_insert_*, gs_erase): copy n rows of the three table arrays from src to dst, one row per thread.  The two
+// Table edit (gs_insert_*, gs_erase): copy n rows of the table arrays from src to dst, one row per thread.  The two
 // ranges never overlap within one launch (an overlapping move goes through a temporary, launch_move_rows), so the
-// accesses are restrict.  The 16 B records are copied as they are; size_alpha goes as float4 when source and
-// destination share their alignment mod 16 B (sa_vec), with up to 3 scalar rows before the first aligned float4
-// (sa_head) and up to 3 after the last.
+// accesses are restrict.  The 16 B records (and an SH context's sh_vecs words of coefficients) are copied as they are;
+// size_alpha goes as float4 when source and destination share their alignment mod 16 B (sa_vec), with up to 3 scalar
+// rows before the first aligned float4 (sa_head) and up to 3 after the last.
 struct RowSpan {
   float4 *cs;
   uint4 *cc;
   float *sa;
+  uint4 *sh;  // NULL on a degree-0 context
 };
 
 __global__ void __launch_bounds__(256) k_move_rows(const RowSpan src, const RowSpan dst, uint32_t n, uint32_t sa_head,
-                                                   uint32_t sa_vec) {
+                                                   uint32_t sa_vec, uint32_t sh_vecs) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float4 *__restrict__ cs_s = src.cs;
@@ -161,6 +166,7 @@ __global__ void __launch_bounds__(256) k_move_rows(const RowSpan src, const RowS
   const float *__restrict__ sa_s = src.sa;
   __stcs(dst.cs + i, __ldcs(cs_s + i));
   __stcs(dst.cc + i, __ldcs(cc_s + i));
+  for (uint32_t v = 0; v < sh_vecs; ++v) __stcs(dst.sh + (size_t)i * sh_vecs + v, __ldcs(src.sh + (size_t)i * sh_vecs + v));
   if (!sa_vec) {
     __stcs(dst.sa + i, __ldcs(sa_s + i));
     return;
@@ -176,32 +182,36 @@ __global__ void __launch_bounds__(256) k_move_rows(const RowSpan src, const RowS
 }
 
 static RowSpan table_span(gs_context *c, uint32_t row) {
-  return RowSpan{c->center_scale + row, c->cov_color + row, c->size_alpha + row};
+  return RowSpan{c->center_scale + row, c->cov_color + row, c->size_alpha + row,
+                 c->sh ? c->sh + (size_t)row * c->sh_vecs : nullptr};
 }
 
-static void launch_copy_rows(const RowSpan &src, const RowSpan &dst, uint32_t n, cudaStream_t st) {
+static void launch_copy_rows(const RowSpan &src, const RowSpan &dst, uint32_t n, uint32_t sh_vecs, cudaStream_t st) {
   const uintptr_t s = (uintptr_t)src.sa, d = (uintptr_t)dst.sa;
   const uint32_t vec = ((s ^ d) & 15u) == 0, head = vec ? std::min<uint32_t>(n, (uint32_t)((16u - (d & 15u)) & 15u) / 4u) : 0;
-  k_move_rows<<<(n + 255) / 256, 256, 0, st>>>(src, dst, n, head, vec);
+  k_move_rows<<<(n + 255) / 256, 256, 0, st>>>(src, dst, n, head, vec, sh_vecs);
 }
 
-size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len) {
+size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len, uint32_t sh_vecs) {
   const uint32_t shift = from > to ? from - to : to - from;
-  return shift >= len ? 0 : (size_t)len * 36 + 16;  // cs | cc | 3 floats of alignment slack + sa
+  // cs | cc | sh | 3 floats of alignment slack + sa
+  return shift >= len ? 0 : (size_t)len * (36 + 16 * (size_t)sh_vecs) + 16;
 }
 
 // Rows [from, from + len) of the table move to [to, to + len).  Disjoint ranges: one launch.  Overlapping ones: two,
-// through `tmp` (move_tmp_bytes(from, to, len) bytes, 16 B aligned), whose size_alpha starts at the source's alignment
-// so that the first copy is always vectorised.
+// through `tmp` (move_tmp_bytes(from, to, len, c->sh_vecs) bytes, 16 B aligned), whose size_alpha starts at the source's
+// alignment so that the first copy is always vectorised.
 void launch_move_rows(gs_context *c, uint32_t from, uint32_t to, uint32_t len, void *tmp, cudaStream_t st) {
   if (!len || from == to) return;
-  if (!move_tmp_bytes(from, to, len)) {
-    launch_copy_rows(table_span(c, from), table_span(c, to), len, st);
+  const uint32_t w = c->sh ? c->sh_vecs : 0u;
+  if (!move_tmp_bytes(from, to, len, w)) {
+    launch_copy_rows(table_span(c, from), table_span(c, to), len, w, st);
     return;
   }
-  const RowSpan t{(float4 *)tmp, (uint4 *)tmp + len, (float *)((uint4 *)tmp + 2 * (size_t)len) + (from & 3u)};
-  launch_copy_rows(table_span(c, from), t, len, st);
-  launch_copy_rows(t, table_span(c, to), len, st);
+  uint4 *sh_t = (uint4 *)tmp + 2 * (size_t)len;
+  const RowSpan t{(float4 *)tmp, (uint4 *)tmp + len, (float *)(sh_t + (size_t)w * len) + (from & 3u), w ? sh_t : nullptr};
+  launch_copy_rows(table_span(c, from), t, len, w, st);
+  launch_copy_rows(t, table_span(c, to), len, w, st);
 }
 
 void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_t n, cudaStream_t st) {
@@ -212,11 +222,12 @@ void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_
 }
 
 void launch_pack_perm(gs_context *c, const uint8_t *rows_dev, const uint32_t *perm, uint32_t first, uint32_t n,
-                      uint8_t *rows_out, cudaStream_t st) {
+                      uint8_t *rows_out, const uint4 *sh_rows, cudaStream_t st) {
   if (!n) return;
   const uint32_t grid = (n + 255) / 256;
   k_pack_perm<<<grid, 256, 0, st>>>((const uint4 *)rows_dev, perm, first, n, c->center_scale, c->cov_color, c->size_alpha,
-                                    c->quirk_table, c->quirk_n, (uint4 *)rows_out);
+                                    c->quirk_table, c->quirk_n, (uint4 *)rows_out, sh_rows, c->sh,
+                                    sh_rows ? c->sh_vecs : 0u);
 }
 
 }  // namespace gs

@@ -7,6 +7,7 @@
 //                  32-bit sort key of its importance (index.js:653-664).  Row j of the reference's output depends only on
 //                  source row sizeIndex[j], so decoding in file order and gathering afterwards (k_pack_perm) is exact.
 //                  <true>: every field read is an aligned float (the INRIA layout); <false>: any TYPE_MAP type, byte loads.
+//                  <., true> (SH contexts): also the row's f_rest_* coefficients as fp16, in file order like the rows.
 //   the stable sort of the keys is k_radix_*<P<0>> .. <P<24>> (gs_sort.cu).
 //
 // Numerics: fp64 as JavaScript evaluates it, no contraction (the library is built with --fmad=false).  The importance
@@ -15,6 +16,7 @@
 // last.  Uint8ClampedArray stores clamp, round half to even and map NaN to 0.  Device exp (fp64, <= 1 ulp) is not
 // bit-identical to V8's Math.exp or glibc's exp: an f32-rounded result can differ only when the exact value lies within
 // about one fp64 ulp of an f32 rounding midpoint (DESIGN.md section 3).
+#include <cuda_fp16.h>
 #include <string.h>
 
 #include "gs_common.cuh"
@@ -28,7 +30,8 @@ static const char *const kFieldName[PF_COUNT] = {"x",     "y",     "z",     "sca
                                                  "rot_0", "rot_1", "rot_2", "rot_3",   "opacity", "f_dc_0",
                                                  "f_dc_1", "f_dc_2", "red", "green",   "blue"};
 
-int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_t &data_off, std::string &err) {
+int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_t &data_off, std::string &err,
+              PlyShLayout *sh) {
   memset(&L, 0, sizeof(L));
   n = 0;
   data_off = 0;
@@ -53,6 +56,8 @@ int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_
   if (!found) { err = "Unable to read .ply file header"; return GS_ERR_INVALID; }
   // property table (index.js:613-631)
   for (int k = 0; k < PF_COUNT; ++k) L.f[k] = PlyField{0, PK_ABSENT};
+  if (sh)
+    for (int k = 0; k < 3 * kMaxShCoeffs; ++k) sh->f[k] = PlyField{0, PK_ABSENT};
   uint64_t row_offset = 0;
   size_t line = 0;
   while (line < header_end_index) {
@@ -79,6 +84,9 @@ int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_
     else if (type == "uchar") { kind = PK_U8; size = 1; }
     for (int k = 0; k < PF_COUNT; ++k)
       if (name == kFieldName[k]) L.f[k] = PlyField{(int32_t)row_offset, kind};  // the last one wins
+    if (sh && name.compare(0, 7, "f_rest_") == 0)
+      for (int k = 0; k < 3 * kMaxShCoeffs; ++k)
+        if (name == "f_rest_" + std::to_string(k)) sh->f[k] = PlyField{(int32_t)row_offset, kind};  // likewise
     row_offset += (uint64_t)size;
   }
   if (row_offset > 0x7FFFFFFFull) { err = "Unable to read .ply file header"; return GS_ERR_INVALID; }
@@ -113,6 +121,17 @@ int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_
     const bool read = (k <= PF_Z) || (k <= PF_OP && L.has_scale) || (k == PF_OP && L.has_opacity) ||
                       (k >= PF_DC0 && k <= PF_DC2 && L.has_fdc) || (k >= PF_RED && !L.has_fdc);
     if (read && (L.f[k].kind != PK_F32 || (L.f[k].off % 4) != 0)) f32 = false;
+  }
+  if (sh) {
+    // the file's degree: the largest d whose f_rest_0 .. f_rest_{3 K(d) - 1} all exist
+    sh->file_k = 0;
+    for (uint32_t d = 1; d <= 3; ++d) {
+      bool all = true;
+      for (uint32_t k = 0; k < 3 * sh_coeffs(d); ++k) all = all && sh->f[k].kind != PK_ABSENT;
+      if (all) sh->file_k = sh_coeffs(d);
+    }
+    for (uint32_t k = 0; k < 3 * sh->file_k; ++k)
+      if (sh->f[k].kind != PK_F32 || (sh->f[k].off % 4) != 0) f32 = false;
   }
   L.all_f32 = f32 ? 1u : 0u;
   return GS_OK;
@@ -155,13 +174,36 @@ __device__ __forceinline__ uint32_t js_store_u8_clamped(double v) {
   return (uint32_t)rint(v);
 }
 
+// coefficient h (channel-major, h < 3 ctx_k) of a row: the typed value rounded to f32, then to fp16 (round to nearest even)
 template <bool kF32>
+__device__ __forceinline__ uint32_t sh_half(const uint8_t *row, const PlyShLayout &S, uint32_t h) {
+  const uint32_t c = h / S.ctx_k, k = h - c * S.ctx_k;  // k: 0-based coefficient of channel c
+  if (k >= S.file_k) return 0u;
+  const float v = __double2float_rn(ply_get<kF32>(row, S.f[c * S.file_k + k]));
+  return (uint32_t)__half_as_ushort(__float2half_rn(v));
+}
+
+template <bool kF32, bool kSH>
 __global__ void __launch_bounds__(256) k_ply_decode(const uint8_t *__restrict__ chunk, uint32_t rows, PlyLayout L,
                                                     uint32_t first_row, uint4 *__restrict__ rows32,
-                                                    uint32_t *__restrict__ key_out) {
+                                                    uint32_t *__restrict__ key_out, const PlyShLayout S,
+                                                    uint4 *__restrict__ sh_rows) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= rows) return;
   const uint8_t *row = chunk + (size_t)i * L.stride;
+  if (kSH) {
+    const uint32_t nh = 3 * S.ctx_k;
+    uint4 *dst = sh_rows + (size_t)(first_row + i) * S.vecs;
+    for (uint32_t v = 0; v < S.vecs; ++v) {
+      uint32_t w[4];
+#pragma unroll
+      for (uint32_t q = 0; q < 4; ++q) {
+        const uint32_t h = v * 8 + q * 2;  // halves h (low) and h + 1 (high) of word q; the padding stays 0
+        w[q] = (h < nh ? sh_half<kF32>(row, S, h) : 0u) | ((h + 1 < nh ? sh_half<kF32>(row, S, h + 1) : 0u) << 16);
+      }
+      dst[v] = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+  }
   uint32_t scale[3], rot;
   uint32_t key = 0u;  // every key is 0 without scale_0: sizeList stays zero-filled (index.js:659-660)
   if (L.has_scale) {
@@ -221,13 +263,14 @@ __global__ void __launch_bounds__(256) k_ply_decode(const uint8_t *__restrict__ 
 }
 
 void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,
-                       uint32_t *key, cudaStream_t st) {
+                       uint32_t *key, const PlyShLayout *sh, uint4 *sh_rows, cudaStream_t st) {
   if (!rows) return;
   const uint32_t grid = (rows + 255) / 256;
-  if (L.all_f32)
-    k_ply_decode<true><<<grid, 256, 0, st>>>(chunk, rows, L, first_row, (uint4 *)rows32, key);
-  else
-    k_ply_decode<false><<<grid, 256, 0, st>>>(chunk, rows, L, first_row, (uint4 *)rows32, key);
+  PlyShLayout S{};
+  if (sh) S = *sh;
+  auto kernel = L.all_f32 ? (sh ? k_ply_decode<true, true> : k_ply_decode<true, false>)
+                          : (sh ? k_ply_decode<false, true> : k_ply_decode<false, false>);
+  kernel<<<grid, 256, 0, st>>>(chunk, rows, L, first_row, (uint4 *)rows32, key, S, sh_rows);
 }
 
 }  // namespace gs

@@ -4,6 +4,8 @@
 //   k_project  : fp32 restatement of the vertex shader, op for op (no FMA contraction), producing a
 //                32 B projected record per splat + its packed tile rectangle (scene frames: with each splat's entity's
 //                gsModelViewMatrix; views scene frames: every view per splat, the table row loaded once).
+//                <.., SH = 1..3> (contexts with gs_set_sh_degree > 0): each record's colour is the splat's view-dependent
+//                colour (sh_color below), its SH row loaded once with its cov_color row.
 //   k_count    : per entry of the draw order (== reference sortedIndexes): instance offset inside its 256-entry slice;
 //                per slice: total; last CTA: prefix over the slices + frame total D.
 //                Sparse frames (fewer than half of the splats sorted): each chunk's survivors are compacted first.
@@ -12,6 +14,8 @@
 //                inside every bin; rectangles of more than 8 bins are finished by the whole warp.  Views scene frames:
 //                each entry emits view 0's instances, then those of views 1.., with bin ids bin_base[v] + bin (on the
 //                slab path too, each view's closed bins skipped).
+#include <cuda_fp16.h>
+
 #include "gs_common.cuh"
 
 namespace gs {
@@ -34,6 +38,64 @@ __device__ __forceinline__ void unpack_int16(uint32_t value, float &lo, float &h
 #define DOT3(a0, b0, a1, b1, a2, b2) ADD(ADD(MUL(a0, b0), MUL(a1, b1)), MUL(a2, b2))
 
 // ---------------------------------------------------------------------------------------------
+// View-dependent colour of a record (SH contexts; DESIGN.md section 3, restated by tests/sh_oracle.c).  cam: the camera
+// position in the table's frame (the host's -A^-1 t of the modelview); sh: the splat's row, 3 K fp16 channel-major.
+//   d = centre - cam, in the PLY's frame (d.x, d.y, -d.z) (the pack negates z); len = sqrt((x x + y y) + z z); x, y, z /= len
+//   v_c = byte_c / 255, then INRIA eval_sh's terms of degrees 1..SH in its order and with its constants, each product
+//   left to right; byte'_c = q8(v_c) = floor(clamp(v_c, 0, 1) * 255 + 0.5), NaN -> 0.  Alpha is kept.
+// len == 0 has no higher terms, and q8(b / 255) == b for every byte, so zero coefficients give the flat colour exactly.
+// ---------------------------------------------------------------------------------------------
+template <int SH>
+__device__ __forceinline__ uint32_t sh_color(uint32_t rgba, const uint4 *sh, const float4 c, const float4 cam) {
+  constexpr int K = (int)sh_coeffs(SH);
+  const float dx = SUB(c.x, cam.x), dy = SUB(c.y, cam.y), dz = SUB(c.z, cam.z);
+  float x = dx, y = dy, z = -dz;
+  const float len = __fsqrt_rn(ADD(ADD(MUL(x, x), MUL(y, y)), MUL(z, z)));
+  if (len == 0.0f) return rgba;
+  x = DIV(x, len); y = DIV(y, len); z = DIV(z, len);
+  // b[k - 1]: the product of the term of coefficient k without the coefficient; the sign of the first three is in `sum`
+  float b[K];
+  b[0] = MUL(0.4886025119029199f, y);
+  b[1] = MUL(0.4886025119029199f, z);
+  b[2] = MUL(0.4886025119029199f, x);
+  if (SH > 1) {
+    const float xx = MUL(x, x), yy = MUL(y, y), zz = MUL(z, z);
+    const float xy = MUL(x, y), yz = MUL(y, z), xz = MUL(x, z);
+    b[3] = MUL(1.0925484305920792f, xy);
+    b[4] = MUL(-1.0925484305920792f, yz);
+    b[5] = MUL(0.31539156525252005f, SUB(SUB(MUL(2.0f, zz), xx), yy));
+    b[6] = MUL(-1.0925484305920792f, xz);
+    b[7] = MUL(0.5462742152960396f, SUB(xx, yy));
+    if (SH > 2) {
+      b[8] = MUL(MUL(-0.5900435899266435f, y), SUB(MUL(3.0f, xx), yy));
+      b[9] = MUL(MUL(2.890611442640554f, xy), z);
+      b[10] = MUL(MUL(-0.4570457994644658f, y), SUB(SUB(MUL(4.0f, zz), xx), yy));
+      b[11] = MUL(MUL(0.3731763325901154f, z), SUB(SUB(MUL(2.0f, zz), MUL(3.0f, xx)), MUL(3.0f, yy)));
+      b[12] = MUL(MUL(-0.4570457994644658f, x), SUB(SUB(MUL(4.0f, zz), xx), yy));
+      b[13] = MUL(MUL(1.445305721320277f, z), SUB(xx, yy));
+      b[14] = MUL(MUL(-0.5900435899266435f, x), SUB(xx, MUL(3.0f, yy)));
+    }
+  }
+  uint32_t out = rgba & 0xFF000000u;
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) {
+    float v = DIV((float)((rgba >> (8 * ch)) & 255u), 255.0f);
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+      const int h = ch * K + k;  // half h of the row: word h / 8, its 32-bit lane (h / 2) % 4, high half when h is odd
+      const uint4 w4 = sh[h / 8];
+      const uint32_t w = ((h / 2) % 4 == 0) ? w4.x : ((h / 2) % 4 == 1) ? w4.y : ((h / 2) % 4 == 2) ? w4.z : w4.w;
+      const float s = __half2float(__ushort_as_half((unsigned short)((h & 1) ? (w >> 16) : (w & 0xFFFFu))));
+      const float t = MUL(b[k], s);
+      v = (k == 0 || k == 2) ? SUB(v, t) : ADD(v, t);  // result - C1 y sh1 + C1 z sh2 - C1 x sh3 + ...
+    }
+    v = fminf(fmaxf(v, 0.0f), 1.0f);  // fmaxf(NaN, 0) = 0
+    out |= (uint32_t)ADD(MUL(v, 255.0f), 0.5f) << (8 * ch);
+  }
+  return out;
+}
+
+// ---------------------------------------------------------------------------------------------
 // K2: vertex shader restatement.  One thread per resident splat, index order (coalesced 16 B + 16 B
 // loads, 32 B + 4 B stores).  Splats rejected by the worker filter are skipped, except splat 0 which
 // the reference may draw through the zero tail of quirk Q5.
@@ -42,9 +104,13 @@ __device__ __forceinline__ void unpack_int16(uint32_t value, float &lo, float &h
 // 32 B record at slot j.
 // mv: the splat's gsModelViewMatrix (rc.mv, or its entity's in a scene frame).  c: its center_scale row; q: its
 // cov_color row, loaded on the first call that needs it (have_q), so a views frame's views load each row once.
+// SH > 0: shr receives the splat's SH row (sh) with q, and the record takes sh_color from eye, mv's camera position.
+template <int SH = 0>
 __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const float *mv, const float4 c,
                                                 const uint4 *__restrict__ cc, uint32_t i, uint32_t j,
-                                                float4 *__restrict__ rec_out, uint4 &q, bool &have_q) {
+                                                float4 *__restrict__ rec_out, uint4 &q, bool &have_q,
+                                                const uint4 *__restrict__ sh = nullptr, uint4 *shr = nullptr,
+                                                float4 eye = float4{}) {
   uint32_t rect = kNoRect;
   const float *P = rc.proj;
   // index.js:106-108: camspace = MV * (center,1); pos2d = P * camspace  (sum x,y,z,w left to right)
@@ -61,6 +127,11 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
   if (!culled) {
     if (!have_q) {
       q = __ldg(cc + i);
+      if constexpr (SH > 0) {
+        constexpr int kVecs = (int)sh_vecs(SH);
+#pragma unroll
+        for (int v = 0; v < kVecs; ++v) shr[v] = __ldg(sh + (size_t)i * kVecs + v);
+      }
       have_q = true;
     }
     // index.js:117-125
@@ -139,7 +210,9 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
         // rgba stay packed (converted to float(byte)/255.0, index.js:152-157, once per record in the raster);
         // the last slot carries gl_Position.z/w (index.js:163) for the depth test against foreign geometry
         rec_out[2 * (size_t)j] = make_float4(cx, cy, a1x, a1y);
-        rec_out[2 * (size_t)j + 1] = make_float4(a2x, a2y, __uint_as_float(q.w), zndc);
+        uint32_t rgba = q.w;
+        if constexpr (SH > 0) rgba = sh_color<SH>(q.w, shr, c, eye);
+        rec_out[2 * (size_t)j + 1] = make_float4(a2x, a2y, __uint_as_float(rgba), zndc);
       }
     }
   }
@@ -156,7 +229,9 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
 // STEREO (views scene frames, by index or, on the slab path, by entry): fp = &views->view[0]; every splat is projected
 // for every view with the view's RenderConsts and its entity's per-view modelview, the table row loaded once; view v >= 1
 // into rec_x / rect_x at (v - 1) * x_stride.
-template <bool BY_ENTRY, bool SCENE = false, bool STEREO = false>
+// SH (1..3, SH contexts): records take the view-dependent colour of degree SH: sh holds the table's SH rows, sh_cam the
+// camera position of entity k's view v at k * kMaxViews + v (plain frames: entry 0).
+template <bool BY_ENTRY, bool SCENE = false, bool STEREO = false, int SH = 0>
 __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, const uint4 *__restrict__ cc,
                                                  const float *__restrict__ depth,
                                                  const FrameParams *__restrict__ fp, float4 *__restrict__ rec_out,
@@ -164,7 +239,8 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
                                                  const FrameCounters *__restrict__ ctr,
                                                  const SceneTable *__restrict__ scene,
                                                  const ViewTable *__restrict__ views, float4 *__restrict__ rec_x,
-                                                 uint32_t *__restrict__ rect_x, uint32_t x_stride) {
+                                                 uint32_t *__restrict__ rect_x, uint32_t x_stride,
+                                                 const uint4 *__restrict__ sh, const float4 *__restrict__ sh_cam) {
   static_assert(!STEREO || SCENE, "views frames are scene frames");
   GS_PDL_ENTRY();
   const RenderConsts &rc = fp->rc;
@@ -196,6 +272,20 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
   auto shade = [&](uint32_t i, uint32_t j) -> uint32_t {
     uint4 q;
     bool have_q = false;
+    if constexpr (SH > 0) {
+      uint4 shr[sh_vecs(SH)];
+      const int k = SCENE ? scene_find(s_first, s_end, n_obj, i) : 0;
+      const float4 *cam = sh_cam + (size_t)k * kMaxViews;
+      const float4 c = __ldg(cs + i);
+      if (!STEREO) return project_one<SH>(rc, SCENE ? scene->obj[k].mv : rc.mv, c, cc, i, j, rec_out, q, have_q, sh, shr, cam[0]);
+      const float(*mv)[16] = views->mv[k];
+      const uint32_t r0 = project_one<SH>(rc, mv[0], c, cc, i, j, rec_out, q, have_q, sh, shr, cam[0]);
+      for (uint32_t v = 1; v < n_views; ++v) {
+        const size_t x = (size_t)(v - 1) * x_stride;
+        rect_x[x + j] = project_one<SH>(views->view[v].rc, mv[v], c, cc, i, j, rec_x + 2 * x, q, have_q, sh, shr, cam[v]);
+      }
+      return r0;
+    }
     if (!STEREO) {
       const float *mv = modelview(i);
       return project_one(rc, mv, __ldg(cs + i), cc, i, j, rec_out, q, have_q);
@@ -523,14 +613,25 @@ __global__ void __launch_bounds__(256) k_emit_entries(const uint2 *__restrict__ 
   }
 }
 
+// the instantiation of k_project<BY_ENTRY, SCENE, STEREO> for the context's SH degree (0: the flat colour)
+template <bool BY_ENTRY, bool SCENE = false, bool STEREO = false>
+static decltype(&k_project<BY_ENTRY, SCENE, STEREO>) project_kernel(uint32_t sh_degree) {
+  switch (sh_degree) {
+    case 1: return k_project<BY_ENTRY, SCENE, STEREO, 1>;
+    case 2: return k_project<BY_ENTRY, SCENE, STEREO, 2>;
+    case 3: return k_project<BY_ENTRY, SCENE, STEREO, 3>;
+    default: return k_project<BY_ENTRY, SCENE, STEREO>;
+  }
+}
+
 void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *ctr, const FrameBufs &b, cudaStream_t stream) {
   uint64_t blocks = ((uint64_t)c->cap + 255) / 256;
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  launch_chain(c, k_project<false>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
+  launch_chain(c, project_kernel<false>(c->sh_degree), (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
                (const uint32_t *)nullptr, ctr, (const SceneTable *)nullptr,  // ctr: the sorted count picks the sparse-frame path
-               (const ViewTable *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr, 0u);
+               (const ViewTable *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr, 0u, (const uint4 *)c->sh, b.sh_cam);
 }
 
 void launch_project_stereo(gs_context *c, const ViewTable *views, const SceneTable *scene, const FrameCounters *ctr,
@@ -539,9 +640,9 @@ void launch_project_stereo(gs_context *c, const ViewTable *views, const SceneTab
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  launch_chain(c, k_project<false, true, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
+  launch_chain(c, project_kernel<false, true, true>(c->sh_degree), (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
                (const float *)c->depth, &views->view[0], b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, views,
-               b.proj_recx, b.rectx, b.x_stride);
+               b.proj_recx, b.rectx, b.x_stride, (const uint4 *)c->sh, b.sh_cam);
 }
 
 void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
@@ -550,9 +651,9 @@ void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  launch_chain(c, k_project<false, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
+  launch_chain(c, project_kernel<false, true>(c->sh_degree), (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
                (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, (const ViewTable *)nullptr,
-               (float4 *)nullptr, (uint32_t *)nullptr, 0u);
+               (float4 *)nullptr, (uint32_t *)nullptr, 0u, (const uint4 *)c->sh, b.sh_cam);
 }
 
 // scene: the slot's scene table for a scene frame (every entry takes its entity's modelview), NULL for a plain frame;
@@ -564,14 +665,16 @@ void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters 
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   if (views) {
-    launch_chain(c, k_project<true, true, true>, (int)blocks, 256, stream, (const float4 *)c->center_scale,
+    launch_chain(c, project_kernel<true, true, true>(c->sh_degree), (int)blocks, 256, stream, (const float4 *)c->center_scale,
                  (const uint4 *)c->cov_color, (const float *)c->depth, &views->view[0], b.proj_rec, b.rect,
-                 (const uint32_t *)b.order, (const FrameCounters *)ctr, scene, views, b.proj_recx, b.rectx, b.x_stride);
+                 (const uint32_t *)b.order, (const FrameCounters *)ctr, scene, views, b.proj_recx, b.rectx, b.x_stride,
+                 (const uint4 *)c->sh, b.sh_cam);
     return;
   }
-  launch_chain(c, scene ? k_project<true, true> : k_project<true>, (int)blocks, 256, stream, (const float4 *)c->center_scale,
-               (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)b.order,
-               (const FrameCounters *)ctr, scene, (const ViewTable *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr, 0u);
+  launch_chain(c, scene ? project_kernel<true, true>(c->sh_degree) : project_kernel<true>(c->sh_degree), (int)blocks, 256, stream,
+               (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
+               (const uint32_t *)b.order, (const FrameCounters *)ctr, scene, (const ViewTable *)nullptr, (float4 *)nullptr,
+               (uint32_t *)nullptr, 0u, (const uint4 *)c->sh, b.sh_cam);
 }
 
 void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,

@@ -97,8 +97,51 @@ def process_ply_buffer(input_buffer: bytes) -> bytes:
     return out.tobytes()
 
 
-def write_inria_ply(path_or_none, xyz, f_dc, opacity, scale_log, rot, n_rest: int = 45) -> bytes:
-    """Write an INRIA-style 3DGS PLY (62 floats per vertex = 248 B) for tests / the config-3 generator."""
+def sh_coefficients(input_buffer: bytes, degree: int) -> np.ndarray:
+    """The spherical-harmonic coefficients a context of SH degree `degree` (1..3) keeps for this file, in table order (the
+    rows process_ply_buffer returns): (n, 3, K) float16, K = (degree+1)^2 - 1, channel-major.  The file's degree is the
+    largest d <= 3 whose f_rest_0 .. f_rest_{3 K(d) - 1} all exist; coefficient k of channel c is f_rest_{c K_f + k - 1}
+    (typed value -> f32 -> fp16, round to nearest even); coefficients above the file's degree are 0."""
+    ubuf = bytes(input_buffer)
+    header = ubuf[: 1024 * 10].decode("utf-8", errors="replace")
+    header_end_index = header.find("end_header\n")
+    m = re.search(r"element vertex (\d+)\n", header)
+    if header_end_index < 0 or m is None:
+        raise ValueError("Unable to read .ply file header")
+    n = int(m.group(1))
+    offsets, off = {}, 0
+    for line in header[:header_end_index].split("\n"):
+        if not line.startswith("property "):
+            continue
+        parts = line.split(" ")
+        typ = _TYPE_MAP.get(parts[1], "i1")
+        offsets[parts[2] if len(parts) > 2 else "undefined"] = (off, typ)  # the last property of a name wins
+        off += np.dtype(typ).itemsize
+    body = np.frombuffer(ubuf, np.uint8, count=n * off, offset=header_end_index + 11).reshape(n, off)
+
+    def field(name):
+        o, typ = offsets[name]
+        return np.ascontiguousarray(body[:, o:o + np.dtype(typ).itemsize]).view(typ).reshape(n).astype(np.float64)
+
+    k_file = 0
+    for d in (1, 2, 3):
+        if all(f"f_rest_{i}" in offsets for i in range(3 * ((d + 1) ** 2 - 1))):
+            k_file = (d + 1) ** 2 - 1
+    k = (int(degree) + 1) ** 2 - 1
+    out = np.zeros((n, 3, k), np.float16)
+    for c in range(3):
+        for j in range(min(k, k_file)):
+            out[:, c, j] = field(f"f_rest_{c * k_file + j}").astype(np.float32).astype(np.float16)
+    if "scale_0" in offsets:  # table order: descending importance, stable (process_ply_buffer)
+        size = np.exp(field("scale_0")) * np.exp(field("scale_1")) * np.exp(field("scale_2"))
+        imp = (size * (1.0 / (1.0 + np.exp(-field("opacity"))))).astype(np.float32)
+        out = out[np.argsort(-imp.astype(np.float64), kind="stable")]
+    return out
+
+
+def write_inria_ply(path_or_none, xyz, f_dc, opacity, scale_log, rot, n_rest: int = 45, f_rest=None) -> bytes:
+    """Write an INRIA-style 3DGS PLY (62 floats per vertex = 248 B) for tests / the config-3 generator.  f_rest:
+    (n, n_rest) values of f_rest_* (zeros when None)."""
     n = xyz.shape[0]
     names = ["x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2"] + [f"f_rest_{i}" for i in range(n_rest)] + \
             ["opacity", "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3"]
@@ -107,6 +150,8 @@ def write_inria_ply(path_or_none, xyz, f_dc, opacity, scale_log, rot, n_rest: in
     arr = np.zeros((n, len(names)), np.float32)
     arr[:, 0:3] = xyz
     arr[:, 6:9] = f_dc
+    if f_rest is not None:
+        arr[:, 9:9 + n_rest] = f_rest
     o = 9 + n_rest
     arr[:, o] = opacity
     arr[:, o + 1:o + 4] = scale_log

@@ -55,7 +55,9 @@ class SplatContext:
     """Owner of one gs_context.  Mirrors the worker protocol (clear / push / sort, index.js:572-598) and
     the draw (index.js:184-207)."""
 
-    def __init__(self, device: int = 0):
+    def __init__(self, device: int = 0, sh_degree: int = 0):
+        """sh_degree 1..3: keep the spherical-harmonic coefficients of .ply files and draw every splat in its
+        view-dependent colour (gs_set_sh_degree); 0 draws the reference's flat colour."""
         self._lib = _lib.load()
         h = C.c_void_p()
         rc = self._lib.gs_create(int(device), C.byref(h))
@@ -63,6 +65,9 @@ class SplatContext:
             raise GsError(rc, (self._lib.gs_last_error(None) or b"").decode())
         self._h = h
         self.device = int(device)
+        self.sh_degree = 0
+        if sh_degree:
+            self.set_sh_degree(sh_degree)
 
     # -- lifetime --
     def close(self) -> None:
@@ -154,6 +159,20 @@ class SplatContext:
         sa = np.empty((n,), np.float32)
         self._check(self._lib.gs_read_packed(self._h, first, n, _ptr(cs), _ptr(cc), _ptr(sa)))
         return cs, cc, sa
+
+    def set_sh_degree(self, degree: int) -> None:
+        """gs_set_sh_degree: 0 (flat colour) .. 3; only while the table is empty (after creation or clear())."""
+        self._check(self._lib.gs_set_sh_degree(self._h, int(degree)))
+        self.sh_degree = int(degree)
+
+    def read_sh(self, first: int = 0, n: Optional[int] = None) -> np.ndarray:
+        """gs_read_sh: the SH coefficients of splats [first, first+n) as (n, 3, K) float16, K = (degree+1)^2 - 1, in table
+        order (channel-major per splat, INRIA's f_rest order)."""
+        n = self.num_splats - first if n is None else n
+        k = (self.sh_degree + 1) ** 2 - 1
+        out = np.empty((n, 3, max(k, 1)), np.uint16)
+        self._check(self._lib.gs_read_sh(self._h, int(first), int(n), _ptr(out)))
+        return out.view(np.float16)
 
     def sort(self, view: np.ndarray, cutout: Optional[np.ndarray] = None, readback: bool = True) -> np.ndarray:
         """{method:'sort'} (index.js:587-596): returns the reference's sortedIndexes (uint32)."""

@@ -200,8 +200,8 @@ GS_API int gs_reserve(gs_context *ctx, uint32_t n_total);
  *       . gs_wait re-runs a frame whose tile-instance buffer overflowed, and that re-run reads the table again;
  *       . an erase at the end moves nothing, but the next push would overwrite rows that a frame in flight may read.
  *     Frames submitted after the edit see the new table.
- *   - Overlapping source and destination ranges go through a stream-ordered temporary of 36 B per moved splat, freed
- *     after the edit.
+ *   - Overlapping source and destination ranges go through a stream-ordered temporary of 36 B per moved splat (plus the
+ *     SH row of an SH context, 96 B at degree 3: gs_set_sh_degree), freed after the edit.
  *   - After any edit the draw order is stale: a GS_RENDER_REUSE_SORT frame sorts again, as after a push.
  */
 GS_API int gs_insert_splats(gs_context *ctx, uint32_t at, const void *rows32, uint32_t n);
@@ -222,6 +222,33 @@ GS_API int gs_num_splats(const gs_context *ctx, uint32_t *out_n);
 /* Read back the packed records of splats [first, first+n) (testing the device-side pack). */
 GS_API int gs_read_packed(gs_context *ctx, uint32_t first, uint32_t n, float *center_scale4, uint32_t *cov_color4,
                           float *size_alpha);
+
+/*
+ * View-dependent colour (spherical harmonics, SH) of INRIA 3DGS PLY files.
+ *
+ * gs_set_sh_degree: keep and draw SH coefficients of degree 1, 2 or 3; 0 (the default) keeps none and draws the flat
+ *   colour the reference draws.  Accepted only while the table is empty (after gs_create, gs_clear, or an erase of every
+ *   splat); a non-empty table or a degree above 3 returns GS_ERR_INVALID and changes nothing.
+ *   With degree d > 0 the context stores K = (d+1)^2 - 1 coefficients per channel and splat, as fp16, channel-major
+ *   (R's K, then G's, then B's: the f_rest_* order of INRIA files), 6 K bytes padded to 16 B per splat (96 B at degree 3),
+ *   beside the table, growing with it (gs_reserve sizes it) and moving with its rows (gs_insert_*, gs_erase).
+ *     - gs_push_ply / gs_insert_ply: the file's degree d_f is the largest of 0..3 whose f_rest_0 .. f_rest_{3 K_f - 1} all
+ *       exist (any TYPE_MAP type; the last property of a name wins).  Coefficient k (1..K) of channel c is
+ *       f_rest_{c K_f + k - 1}: its typed value rounded to f32, then to fp16 (round to nearest even).  A file above the
+ *       context's degree has its extra coefficients dropped, one below it has the missing ones 0.  The coefficients follow
+ *       their rows through the importance order.  Header rules, messages and rows32_out are unchanged.
+ *     - gs_push_splats / gs_insert_splats / gs_push_packed rows have zero coefficients.
+ *   Every frame of such a context (plain, stereo, scene, views, target, slab, sharded, GS_RENDER_BLEND_UNORM8, STATS) draws
+ *   each splat in its view-dependent colour, per view: with cam the camera position of the splat's gsModelViewMatrix in the
+ *   table's frame (-A^-1 t of its upper 3x3 A and translation t, fp64 by Cramer's rule, rounded to f32) and d = centre - cam
+ *   in f32, taken to the PLY's frame as (d.x, d.y, -d.z) and normalised, each colour channel is byte / 255 plus INRIA
+ *   eval_sh's terms of degrees 1..d (fp32, its order and constants), stored back as floor(clamp(x, 0, 1) * 255 + 0.5)
+ *   (NaN -> 0).  Alpha is unchanged.  All-zero coefficients draw exactly the degree-0 frame.
+ * gs_read_sh: splats [first, first+n) as 3 K fp16 bit patterns each, channel-major, in out (host, 6 K n bytes).  Returns
+ *   GS_ERR_INVALID on a degree-0 context or a range past the resident splats.
+ */
+GS_API int gs_set_sh_degree(gs_context *ctx, uint32_t degree);
+GS_API int gs_read_sh(gs_context *ctx, uint32_t first, uint32_t n, uint16_t *out);
 
 /*
  * {method:"sort", view, cutout} -> {sortedIndexes} (index.js:449-453, 507-570, 587-596).
