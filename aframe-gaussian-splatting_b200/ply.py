@@ -97,11 +97,21 @@ def process_ply_buffer(input_buffer: bytes) -> bytes:
     return out.tobytes()
 
 
+def sh_half(v: np.ndarray) -> np.ndarray:
+    """A stored coefficient: the typed value (fp64) -> f32 -> fp16, each rounded to nearest even, and every NaN the
+    canonical 0x7FFF (numpy would keep the sign and payload bits; the device conversion does not)."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        h = np.asarray(v, np.float64).astype(np.float32).astype(np.float16)
+    h.view(np.uint16)[np.isnan(h)] = 0x7FFF
+    return h
+
+
 def sh_coefficients(input_buffer: bytes, degree: int) -> np.ndarray:
     """The spherical-harmonic coefficients a context of SH degree `degree` (1..3) keeps for this file, in table order (the
     rows process_ply_buffer returns): (n, 3, K) float16, K = (degree+1)^2 - 1, channel-major.  The file's degree is the
     largest d <= 3 whose f_rest_0 .. f_rest_{3 K(d) - 1} all exist; coefficient k of channel c is f_rest_{c K_f + k - 1}
-    (typed value -> f32 -> fp16, round to nearest even); coefficients above the file's degree are 0."""
+    (typed value -> f32 -> fp16, round to nearest even; every NaN -> 0x7FFF, whatever its sign and payload);
+    coefficients above the file's degree are 0."""
     ubuf = bytes(input_buffer)
     header = ubuf[: 1024 * 10].decode("utf-8", errors="replace")
     header_end_index = header.find("end_header\n")
@@ -131,7 +141,7 @@ def sh_coefficients(input_buffer: bytes, degree: int) -> np.ndarray:
     out = np.zeros((n, 3, k), np.float16)
     for c in range(3):
         for j in range(min(k, k_file)):
-            out[:, c, j] = field(f"f_rest_{c * k_file + j}").astype(np.float32).astype(np.float16)
+            out[:, c, j] = sh_half(field(f"f_rest_{c * k_file + j}"))
     if "scale_0" in offsets:  # table order: descending importance, stable (process_ply_buffer)
         size = np.exp(field("scale_0")) * np.exp(field("scale_1")) * np.exp(field("scale_2"))
         imp = (size * (1.0 / (1.0 + np.exp(-field("opacity"))))).astype(np.float32)

@@ -234,7 +234,8 @@ GS_API int gs_read_packed(gs_context *ctx, uint32_t first, uint32_t n, float *ce
  *   beside the table, growing with it (gs_reserve sizes it) and moving with its rows (gs_insert_*, gs_erase).
  *     - gs_push_ply / gs_insert_ply: the file's degree d_f is the largest of 0..3 whose f_rest_0 .. f_rest_{3 K_f - 1} all
  *       exist (any TYPE_MAP type; the last property of a name wins).  Coefficient k (1..K) of channel c is
- *       f_rest_{c K_f + k - 1}: its typed value rounded to f32, then to fp16 (round to nearest even).  A file above the
+ *       f_rest_{c K_f + k - 1}: its typed value rounded to f32, then to fp16 (round to nearest even); every NaN is stored
+ *       as 0x7FFF, whatever its sign and payload.  A file above the
  *       context's degree has its extra coefficients dropped, one below it has the missing ones 0.  The coefficients follow
  *       their rows through the importance order.  Header rules, messages and rows32_out are unchanged.
  *     - gs_push_splats / gs_insert_splats / gs_push_packed rows have zero coefficients.

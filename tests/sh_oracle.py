@@ -171,10 +171,12 @@ def table_for(cs, cc, coef, ranges):
     return cc
 
 
-def decode_f_rest(blob: bytes, degree: int) -> np.ndarray:
+def decode_f_rest(blob: bytes, degree: int, mutant=None) -> np.ndarray:
     """(n, 3, K) float16 coefficients of a context of SH degree `degree`, in FILE order: the header read with the
     reference's rules (10 KB window, every property's offset accumulated, unknown types are 1-byte ints, the last
-    property of a name wins), coefficient k of channel c = f_rest_{c K_f + k - 1} with K_f the file's degree's K."""
+    property of a name wins), coefficient k of channel c = f_rest_{c K_f + k - 1} with K_f the file's degree's K, each
+    the typed value -> f32 -> fp16 (round to nearest even) and every NaN 0x7FFF.  mutant: "direct" (the value rounded
+    straight to fp16, skipping f32), "keep_nan" (NaN sign and payload bits kept, as numpy's casts keep them)."""
     head = bytes(blob[:10240]).decode("latin-1")
     end = head.index("end_header\n")
     n = int(re.search(r"element vertex (\d+)\n", head).group(1))
@@ -194,6 +196,10 @@ def decode_f_rest(blob: bytes, degree: int) -> np.ndarray:
         for k in range(min(K, k_file)):
             o, t = fields[f"f_rest_{c * k_file + k}"]
             v = np.ascontiguousarray(body[:, o:o + t.itemsize]).view(t).reshape(n)
-            out[:, c, k] = v.astype(np.float64).astype(F32).astype(np.float16)
+            with np.errstate(over="ignore", invalid="ignore"):
+                v = v.astype(np.float64)
+                out[:, c, k] = v.astype(np.float16) if mutant == "direct" else v.astype(F32).astype(np.float16)
+    if mutant != "keep_nan":
+        out.view(np.uint16)[np.isnan(out)] = 0x7FFF
     return out
 

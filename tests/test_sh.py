@@ -132,6 +132,53 @@ def test_f_rest_decode_matches_ply_module(n_rest, degree):
         assert np.array_equal(file_order[:, 2, used - 1].view(np.uint16), src.view(np.uint16))
 
 
+@pytest.mark.parametrize("degree", [1, 2, 3])
+def test_c_oracle_equals_numpy_restatement_on_every_half(degree):
+    """One coefficient slot per channel takes every fp16 bit pattern (subnormals, 65504, infinities, NaNs), seen from
+    random directions and along the file frame's axes (basis terms exactly 0, so inf * 0 = NaN)."""
+    rng = np.random.default_rng(300 + degree)
+    K = sho.n_coeffs(degree)
+    n = 65536
+    rgba, coef, cs = records(rng, n, degree)
+    every = np.arange(n, dtype=np.uint32).astype(np.uint16).view(np.float16)
+    for ch in range(3):
+        coef[:, ch, (ch * 5 + degree) % K] = np.roll(every, 9973 * ch)
+    cam = np.array([0.25, -0.5, 0.75], F32)
+    axis = np.arange(n) % 4 == 0  # a quarter of the records sit on a line through the camera along x, y or z
+    ax = (np.arange(n) // 4) % 3
+    off = np.where(np.arange(n) % 8 == 0, F32(1.5), F32(-2.0))
+    cs[axis, :3] = cam
+    cs[axis, ax[axis]] += off[axis]
+    with np.errstate(invalid="ignore", over="ignore"):
+        c = sho.color_c(rgba, coef, cs, cam[None])
+        npv = sho.color_np(rgba, coef, cs, cam)
+    assert np.array_equal(c, npv), int((c != npv).sum())
+    # the edges reach the bytes: NaN sums give 0, saturated ones 0 or 255, and inf * 0 gives NaN on the axes
+    bad = np.isnan(coef.astype(F32)).any((1, 2)) | np.isinf(coef.astype(F32)).any((1, 2))
+    assert bad.sum() > 1000 and (c[bad] & 0xFFFFFF != rgba[bad] & 0xFFFFFF).mean() > 0.9
+    assert np.array_equal(c >> 24, rgba >> 24)
+
+
+def test_f_rest_decode_of_the_fp16_edges():
+    """The edge file (tests/sh_edges.py): every typed value -> f32 -> fp16 as listed, every NaN 0x7FFF, in file and
+    table order; rounding the value straight to fp16, or keeping numpy's NaN bits, changes coefficients of this file."""
+    from sh_edges import edge_file, edge_values
+    blob, want = edge_file()
+    for t, v, bits in edge_values():  # the listed bits are the definition's, value by value
+        with np.errstate(over="ignore", invalid="ignore"):
+            assert int(gs.ply.sh_half(np.asarray([v], np.float64)).view(np.uint16)[0]) == bits, (t, v, hex(bits))
+    for degree in (1, 2, 3):
+        K = sho.n_coeffs(degree)
+        got = sho.decode_f_rest(blob, degree)
+        assert np.array_equal(got.view(np.uint16), want[:, :, :K]), degree
+        table = gs.ply.sh_coefficients(blob, degree)  # x holds the file row
+        assert np.array_equal(table.view(np.uint16), want[_file_rows(blob), :, :K]), degree
+    for mutant in ("direct", "keep_nan"):
+        bad = sho.decode_f_rest(blob, 3, mutant=mutant).view(np.uint16)
+        assert (bad != want).any(), mutant
+    assert (want == 0x7FFF).sum() > 100 and (want == 0x7C00).sum() > 100
+
+
 def test_f_rest_decode_of_mixed_types_and_duplicates():
     rng = np.random.default_rng(99)
     types = {f"f_rest_{k}": t for k, t in zip(range(45), ["double", "short", "uchar", "int", "float", "char"] * 8)}
