@@ -18,6 +18,7 @@ uint32_t owned_tiles_host(uint32_t width, uint32_t height, uint32_t rank, uint32
 using namespace gs;
 
 static int drain(gs_context *c);
+static int idle(gs_context *c);
 
 static thread_local std::string g_create_error;
 
@@ -87,8 +88,11 @@ static int ensure_table(gs_context *c, uint64_t need, bool exact = false) {
   return GS_OK;
 }
 
+// Each group of shared buffers has one readiness rule, X_ready.  It opens ensure_X, and through frame_bufs_ready it decides
+// whether the pipeline must be made idle before a frame: past its rule, ensure_X frees buffers that frames in flight read.
+static bool scratch_ready(const gs_context *c) { return c->scratch_cap >= c->cap && c->depth; }
 static int ensure_scratch(gs_context *c) {
-  if (c->scratch_cap >= c->cap && c->depth) return GS_OK;
+  if (scratch_ready(c)) return GS_OK;
   dev_free(c->depth); dev_free(c->idx_a); dev_free(c->dig_a); dev_free(c->table_n); dev_free(c->slice_total);
   for (int i = 0; i < 2; ++i) { dev_free(c->order[i]); dev_free(c->proj_rec[i]); dev_free(c->rect[i]); }
   dev_free(c->slice_prefix); dev_free(c->ent); dev_free(c->ent_off);
@@ -113,8 +117,9 @@ static int ensure_scratch(gs_context *c) {
 }
 
 // sort keys of scene frames, sized like the per-splat scratch; allocated by the first scene frame (the pipeline is idle)
+static bool scene_bufs_ready(const gs_context *c) { return c->scene_cap >= c->cap && c->scene_key; }
 static int ensure_scene_bufs(gs_context *c) {
-  if (c->scene_cap >= c->cap && c->scene_key) return GS_OK;
+  if (scene_bufs_ready(c)) return GS_OK;
   dev_free(c->scene_key); dev_free(c->scene_pay); dev_free(c->scene_hi);
   GS_CUDA(c, dev_alloc(&c->scene_key, (size_t)c->cap));
   GS_CUDA(c, dev_alloc(&c->scene_pay, (size_t)c->cap));
@@ -134,11 +139,11 @@ static int ensure_slot_scene(gs_context *c, gs_context::Slot &sl) {
 // records and rectangles of views 1.. of views scene frames, each view's sized like the per-splat scratch (rounded up to
 // 4 splats: the projection clears 4 rectangles per store); allocated by the first views frame and grown to the largest
 // view count drawn since (the pipeline is idle)
-static bool stereo_bufs_ok(const gs_context *c, uint32_t n_views) {
+static bool stereo_bufs_ready(const gs_context *c, uint32_t n_views) {
   return n_views <= 1 || (c->stereo_cap >= c->cap && c->stereo_views >= n_views - 1 && c->proj_recx[0]);
 }
 static int ensure_stereo_bufs(gs_context *c, uint32_t n_views) {
-  if (stereo_bufs_ok(c, n_views)) return GS_OK;
+  if (stereo_bufs_ready(c, n_views)) return GS_OK;
   const uint32_t views = std::max(c->stereo_views, n_views - 1);
   const size_t stride = ((size_t)c->cap + 3) & ~(size_t)3;
   for (int i = 0; i < 2; ++i) {
@@ -177,14 +182,24 @@ static int ensure_instances(gs_context *c, uint64_t need) {
   return GS_OK;
 }
 
-static void drop_graphs(gs_context *c);
-static void drop_stereo_graphs(gs_context *c);
+static void kill_graph(cudaGraphExec_t &g) {
+  if (g) { cudaGraphExecDestroy(g); g = nullptr; }
+}
 
+// every cached graph of one domain (GraphId: the mono ids come first)
+static void drop_graphs(gs_context *c, GraphDomain domain) {
+  const int first = domain == kGraphsViews ? kGraphViewsFirst : 0, end = domain == kGraphsViews ? kGraphCount : kGraphViewsFirst;
+  for (auto &sl : c->slot)
+    for (auto &set : sl.graph)
+      for (int id = first; id < end; ++id) kill_graph(set[id]);
+}
+
+static bool bins_ready(const gs_context *c, uint32_t n_bins) { return n_bins <= c->bins_cap && c->bin_range[0]; }
 static int ensure_bins(gs_context *c, uint32_t n_bins) {
-  if (n_bins <= c->bins_cap && c->bin_range[0]) return GS_OK;
+  if (bins_ready(c, n_bins)) return GS_OK;
   // the captured stages bake bin_range; a views frame grows it to every view's bins while a mono frame's key stays put
-  drop_graphs(c);
-  drop_stereo_graphs(c);
+  drop_graphs(c, kGraphsMono);
+  drop_graphs(c, kGraphsViews);
   dev_free(c->bin_range[0]); dev_free(c->bin_range[1]);
   GS_CUDA(c, dev_alloc(&c->bin_range[0], (size_t)n_bins + 1));
   GS_CUDA(c, dev_alloc(&c->bin_range[1], (size_t)n_bins + 1));
@@ -192,8 +207,9 @@ static int ensure_bins(gs_context *c, uint32_t n_bins) {
   return GS_OK;
 }
 
+static bool tile_stats_ready(const gs_context *c, uint32_t n_tiles) { return n_tiles <= c->tile_stats_cap && c->tile_stats; }
 static int ensure_tile_stats(gs_context *c, uint32_t n_tiles) {
-  if (n_tiles <= c->tile_stats_cap && c->tile_stats) return GS_OK;
+  if (tile_stats_ready(c, n_tiles)) return GS_OK;
   dev_free(c->tile_stats);
   if (c->tile_stats_host) cudaFreeHost(c->tile_stats_host);
   c->tile_stats_host = nullptr;
@@ -205,8 +221,14 @@ static int ensure_tile_stats(gs_context *c, uint32_t n_tiles) {
 
 // buffers of the front-to-back slab path (gs_slab.cu); the pipeline is idle when this runs.  n_tiles: the frame's slab tiles
 // (a views frame's: every view's)
+static bool slab_keys_ready(const gs_context *c) { return c->slab_cap >= c->cap && c->key32[0]; }
+static bool slab_tiles_ready(const gs_context *c, uint32_t n_tiles) { return c->slab_tiles_cap >= n_tiles && c->pix_state; }
+static bool slab_ready(const gs_context *c, uint32_t n_tiles) {
+  return slab_keys_ready(c) && c->slab_tab[0] && c->slab_tab[1] && slab_tiles_ready(c, n_tiles);
+}
 static int ensure_slab(gs_context *c, uint32_t n_tiles) {
-  if (c->slab_cap < c->cap || !c->key32[0]) {
+  if (slab_ready(c, n_tiles)) return GS_OK;
+  if (!slab_keys_ready(c)) {
     dev_free(c->key32[0]); dev_free(c->key32[1]); dev_free(c->cidx); dev_free(c->ckey); dev_free(c->chunk_cnt[0]); dev_free(c->chunk_cnt[1]);
     GS_CUDA(c, dev_alloc(&c->key32[0], (size_t)c->cap + 8));
     GS_CUDA(c, dev_alloc(&c->key32[1], (size_t)c->cap + 8));
@@ -219,11 +241,11 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles) {
   }
   for (int i = 0; i < 2; ++i)
     if (!c->slab_tab[i]) GS_CUDA(c, dev_alloc(&c->slab_tab[i], 1));
-  if (c->slab_tiles_cap < n_tiles || !c->pix_state) {
+  if (!slab_tiles_ready(c, n_tiles)) {
     // the captured slab loops bake these buffers, and a views frame grows them to every view's tiles while the mono frames'
     // graph key stays put (and the other way round)
-    drop_graphs(c);
-    drop_stereo_graphs(c);
+    drop_graphs(c, kGraphsMono);
+    drop_graphs(c, kGraphsViews);
     dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open);
     GS_CUDA(c, dev_alloc(&c->pix_state, (size_t)n_tiles * 256));
     GS_CUDA(c, dev_alloc(&c->tile_closed, (size_t)n_tiles));
@@ -231,6 +253,34 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles) {
     // more bins without more tiles (192x192: 144 tiles / 4 bins, then 97x289: 133 / 8), and only tiles trigger regrowth
     GS_CUDA(c, dev_alloc(&c->bin_open, (size_t)n_tiles));
     c->slab_tiles_cap = n_tiles;
+  }
+  return GS_OK;
+}
+
+// The shared buffers one frame needs: is every group big enough, and the allocation of those that are not (the pipeline
+// is idle).  A views frame (n_views views; every other frame: 1) bins every view's bins and keeps slab state for every
+// view's tiles; the tile statistics are view 0's.
+struct FrameNeeds {
+  bool slab, scene;
+  uint32_t n_views, n_bins_all, n_tiles, n_tiles_all;
+};
+static bool frame_bufs_ready(const gs_context *c, const FrameNeeds &f) {
+  return scratch_ready(c) && bins_ready(c, f.n_bins_all) && tile_stats_ready(c, f.n_tiles) &&
+         (!f.slab || slab_ready(c, f.n_tiles_all)) && (!f.scene || scene_bufs_ready(c)) && stereo_bufs_ready(c, f.n_views) &&
+         c->cap_inst != 0;
+}
+static int ensure_frame_bufs(gs_context *c, const FrameNeeds &f) {
+  int rc;
+  if ((rc = ensure_scratch(c)) || (rc = ensure_bins(c, f.n_bins_all)) || (rc = ensure_tile_stats(c, f.n_tiles))) return rc;
+  if (f.slab && (rc = ensure_slab(c, f.n_tiles_all))) return rc;
+  if (f.scene && (rc = ensure_scene_bufs(c))) return rc;
+  if ((rc = ensure_stereo_bufs(c, f.n_views))) return rc;
+  if (c->cap_inst == 0) {
+    // first frame: room for two bin instances per resident splat (a typical scene needs ~1); GS_INST_CAP overrides
+    // the initial size (tests of the overflow / regrow path)
+    uint64_t first = std::max<uint64_t>(1u << 20, f.slab ? (uint64_t)c->n : (uint64_t)c->n * 2);
+    if (const char *e = getenv("GS_INST_CAP")) first = std::max<uint64_t>(1024, strtoull(e, nullptr, 10));
+    if ((rc = ensure_instances(c, first))) return rc;
   }
   return GS_OK;
 }
@@ -243,32 +293,6 @@ static int ensure_dev(gs_context *c, void *&dev, size_t &cap, size_t bytes) {
   GS_CUDA(c, cudaMalloc(&dev, bytes));
   cap = bytes;
   return GS_OK;
-}
-
-static void kill_graph(cudaGraphExec_t &g) {
-  if (g) { cudaGraphExecDestroy(g); g = nullptr; }
-}
-
-static void drop_graphs(gs_context *c) {
-  auto kill = kill_graph;
-  for (auto &sl : c->slot)
-    for (int i = 0; i < 2; ++i) {
-      kill(sl.graph_a[i][0]); kill(sl.graph_a[i][1]); kill(sl.graph_as[i]); kill(sl.graph_b[i]); kill(sl.graph_r[i]); kill(sl.graph_rp[i]);
-      for (int q = 0; q < 2; ++q) {
-        kill(sl.graph_sa[i][q]);
-        for (auto &g : sl.graph_sl[i][q]) kill(g);
-      }
-    }
-}
-
-// the stereo frames' graphs: the three one-pass stages and the slab path's (kind 2)
-static void drop_stereo_graphs(gs_context *c) {
-  for (auto &sl : c->slot)
-    for (int i = 0; i < 2; ++i) {
-      kill_graph(sl.graph_xa[i]); kill_graph(sl.graph_xb[i]); kill_graph(sl.graph_xr[i]);
-      kill_graph(sl.graph_sa[i][2]);
-      for (auto &g : sl.graph_sl[i][2]) kill_graph(g);
-    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -411,8 +435,8 @@ extern "C" int gs_destroy(gs_context *c) {
     if (c->ply_ev[i]) cudaEventDestroy(c->ply_ev[i]);
   }
   if (c->push_stream) cudaStreamDestroy(c->push_stream);
-  drop_graphs(c);
-  drop_stereo_graphs(c);
+  drop_graphs(c, kGraphsMono);
+  drop_graphs(c, kGraphsViews);
   for (uint32_t r = 0; r < c->peer_world; ++r)
     if (r != c->peer_rank && c->peer_base[r]) cudaIpcCloseMemHandle(c->peer_base[r]);
   if (c->peer_local) cudaFree(c->peer_local);
@@ -813,6 +837,20 @@ static int drain(gs_context *c) {
   return GS_OK;
 }
 
+// the three stage streams have run dry (frames not yet collected may still be on the copy stream)
+static int sync_streams(gs_context *c) {
+  GS_CUDA(c, cudaStreamSynchronize(c->stream));
+  GS_CUDA(c, cudaStreamSynchronize(c->bstream));
+  GS_CUDA(c, cudaStreamSynchronize(c->rstream));
+  return GS_OK;
+}
+
+// nothing in flight and nothing queued: the state in which shared buffers may be replaced
+static int idle(gs_context *c) {
+  int rc = drain(c);
+  return rc ? rc : sync_streams(c);
+}
+
 static void stats_from_counters(gs_context *c, const FrameCounters &h, uint32_t n_splats) {
   gs_stats &s = c->stats;
   s.n_splats = n_splats;
@@ -825,46 +863,62 @@ static void stats_from_counters(gs_context *c, const FrameCounters &h, uint32_t 
   s.max_depth = h.sort.n_valid ? dec_f64(h.sort.max_enc) : -INFINITY;
 }
 
+// gs_sort and gs_sort_scene: one sort in slot 0 and buffer set 0 of an idle pipeline, its counters and order read back.
+// scene: the validated table of gs_sort_scene (nullptr: the one-entity sort of gs_sort, by view and cutout)
+static int sort_only(gs_context *c, const float *view, const float *cutout, const SceneTable *scene, size_t scene_bytes,
+                     uint32_t *out_idx, uint32_t *out_count) {
+  int rc = idle(c);
+  if (rc) return rc;
+  if ((rc = ensure_scratch(c))) return rc;
+  gs_context::Slot &sl = c->slot[0];
+  if (scene && ((rc = ensure_scene_bufs(c)) || (rc = ensure_slot_scene(c, sl)))) return rc;
+  c->last_set = 0;
+  const FrameBufs bufs{c->order[0], c->proj_rec[0], c->rect[0], c->inst_rec[0], c->bin_range[0]};
+  memset(sl.fp_host, 0, sizeof(FrameParams));
+  if (scene) memcpy(sl.scene_host, scene, scene_bytes);  // every entity's view row and cutout are in the table
+  else fill_sort_consts(sl.fp_host->sc, view, cutout);
+  sl.fp_host->n_splats = c->n;
+  if (c->pushed) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->push_done, 0));
+  GS_CUDA(c, cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, c->stream));
+  if (scene) GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, scene_bytes, cudaMemcpyHostToDevice, c->stream));
+  GS_CUDA(c, cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), c->stream));
+  if (scene) GS_CUDA(c, cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, c->stream));
+  GS_CUDA(c, cudaEventRecord(c->ev[0], c->stream));
+  if (scene) {
+    launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
+    launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
+    launch_scene_radix(c, sl.fp, sl.ctr, bufs, c->stream);
+  } else {
+    launch_depth_cull(c, sl.fp, sl.ctr, c->stream);
+    launch_depth_radix(c, sl.fp, sl.ctr, bufs, c->stream);
+  }
+  GS_CUDA(c, cudaGetLastError());
+  GS_CUDA(c, cudaEventRecord(c->ev[1], c->stream));
+  // the counters a GS_RENDER_REUSE_SORT frame starts from
+  if (!scene) GS_CUDA(c, cudaMemcpyAsync(c->sort_hdr, sl.ctr, sizeof(SortHeader), cudaMemcpyDeviceToDevice, c->stream));
+  GS_CUDA(c, cudaMemcpyAsync(sl.ctr_host, sl.ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, c->stream));
+  GS_CUDA(c, cudaStreamSynchronize(c->stream));
+  memset(&c->stats, 0, sizeof(c->stats));
+  stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
+  c->stats.kernel_launches = scene ? 11 : 7;
+  float ms = 0;
+  cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]);
+  c->stats.ms_sort = ms;
+  c->stats.ms_total = ms;
+  c->have_order = !scene;  // a concatenation of several entities' orders is no single-entity order
+  c->order_count = sl.ctr_host->sort.n_valid;
+  if (out_count) *out_count = c->order_count;
+  if (out_idx && c->order_count)
+    GS_CUDA(c, cudaMemcpy(out_idx, c->order[0], sizeof(uint32_t) * (size_t)c->order_count, cudaMemcpyDeviceToHost));
+  return GS_OK;
+}
+
 extern "C" int gs_sort(gs_context *c, const float view[4], const float *cutout16_or_null, uint32_t *out_idx,
                        uint32_t *out_count) {
   if (!c || !view) return GS_ERR_INVALID;
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_sort before any push");
   GS_CUDA(c, cudaSetDevice(c->device));
-  int rc = drain(c);
-  if (rc) return rc;
-  if ((rc = ensure_scratch(c))) return rc;
-  GS_CUDA(c, cudaStreamSynchronize(c->bstream));
-  GS_CUDA(c, cudaStreamSynchronize(c->rstream));
-  gs_context::Slot &sl = c->slot[0];
-  c->last_set = 0;
-  const FrameBufs bufs{c->order[0], c->proj_rec[0], c->rect[0], c->inst_rec[0], c->bin_range[0]};
-  memset(sl.fp_host, 0, sizeof(FrameParams));
-  fill_sort_consts(sl.fp_host->sc, view, cutout16_or_null);
-  sl.fp_host->n_splats = c->n;
-  if (c->pushed) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->push_done, 0));
-  GS_CUDA(c, cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, c->stream));
-  GS_CUDA(c, cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), c->stream));
-  GS_CUDA(c, cudaEventRecord(c->ev[0], c->stream));
-  launch_depth_cull(c, sl.fp, sl.ctr, c->stream);
-  launch_depth_radix(c, sl.fp, sl.ctr, bufs, c->stream);
-  GS_CUDA(c, cudaGetLastError());
-  GS_CUDA(c, cudaEventRecord(c->ev[1], c->stream));
-  GS_CUDA(c, cudaMemcpyAsync(c->sort_hdr, sl.ctr, sizeof(SortHeader), cudaMemcpyDeviceToDevice, c->stream));
-  GS_CUDA(c, cudaMemcpyAsync(sl.ctr_host, sl.ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, c->stream));
-  GS_CUDA(c, cudaStreamSynchronize(c->stream));
-  memset(&c->stats, 0, sizeof(c->stats));
-  stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
-  c->stats.kernel_launches = 7;
-  float ms = 0;
-  cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]);
-  c->stats.ms_sort = ms;
-  c->stats.ms_total = ms;
-  c->have_order = true;
-  c->order_count = sl.ctr_host->sort.n_valid;
-  if (out_count) *out_count = c->order_count;
-  if (out_idx && c->order_count)
-    GS_CUDA(c, cudaMemcpy(out_idx, c->order[c->last_set], sizeof(uint32_t) * (size_t)c->order_count, cudaMemcpyDeviceToHost));
-  return GS_OK;
+  return sort_only(c, view, cutout16_or_null, nullptr, 0, out_idx, out_count);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -916,19 +970,27 @@ static gs_context::GraphKey graph_key(const gs_context *c, const gs_context::Slo
   return k;
 }
 
+// the events inside a stage (timing): under capture they are recorded as external events, so that replays record them too
+static cudaError_t record(cudaEvent_t ev, cudaStream_t st, bool external) {
+  return external ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
+}
+
 // Stage A of a frame (sort stream): per-frame inputs to the device, depth sort, vertex shader.  All per-frame
 // inputs come from sl.fp (device memory), so each stage is captured once into a CUDA graph and replayed.
+// A scene frame takes the per-entity depth pass, keys and the (rank, key, index) sort, with the per-entity projection
+// beside it.  Its scene table was copied to sl.scene_dev ahead of the stage (submit), and for a views frame the view table
+// to sl.stereo_dev: the sort is the head camera's, the projection covers every view.
 static cudaError_t enqueue_sort_stage(gs_context *c, gs_context::Slot &sl, bool reuse, bool external_events) {
-  auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
-    return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
-  };
   cudaStream_t m = c->stream, x = c->aux_stream;
   const FrameBufs b = slot_bufs(c, sl);
   cudaError_t e;
   if ((e = cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, m))) return e;
   if ((e = cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), m))) return e;
-  if ((e = rec(sl.ev[0], m))) return e;
-  if (reuse) {
+  if (sl.scene && (e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, m))) return e;
+  if ((e = record(sl.ev[0], m, external_events))) return e;
+  if (sl.scene) {
+    launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, m);
+  } else if (reuse) {
     if ((e = cudaMemcpyAsync(sl.ctr, c->sort_hdr, sizeof(SortHeader), cudaMemcpyDeviceToDevice, m))) return e;
   } else {
     launch_depth_cull(c, sl.fp, sl.ctr, m);
@@ -936,75 +998,45 @@ static cudaError_t enqueue_sort_stage(gs_context *c, gs_context::Slot &sl, bool 
   // fork: the vertex-shader kernel only needs the cull result, so it runs beside the depth radix passes
   if ((e = cudaEventRecord(c->ev_fork[0], m))) return e;
   if ((e = cudaStreamWaitEvent(x, c->ev_fork[0], 0))) return e;
-  if ((e = rec(sl.evp[0], x))) return e;
-  launch_project(c, sl.fp, sl.ctr, b, x);
-  if ((e = rec(sl.evp[1], x))) return e;
+  if ((e = record(sl.evp[0], x, external_events))) return e;
+  if (sl.stereo) launch_project_stereo(c, sl.stereo_dev, sl.scene_dev, sl.ctr, b, x);
+  else if (sl.scene) launch_project_scene(c, sl.fp, sl.scene_dev, sl.ctr, b, x);
+  else launch_project(c, sl.fp, sl.ctr, b, x);
+  if ((e = record(sl.evp[1], x, external_events))) return e;
   if ((e = cudaEventRecord(c->ev_join[0], x))) return e;
-  if (!reuse) {
+  if (sl.scene) {
+    launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, m);
+    launch_scene_radix(c, sl.fp, sl.ctr, b, m);
+  } else if (!reuse) {
     launch_depth_radix(c, sl.fp, sl.ctr, b, m);
     if ((e = cudaMemcpyAsync(c->sort_hdr, sl.ctr, sizeof(SortHeader), cudaMemcpyDeviceToDevice, m))) return e;
   }
-  if ((e = rec(sl.ev[1], m))) return e;
-  if ((e = cudaStreamWaitEvent(m, c->ev_join[0], 0))) return e;
-  return cudaGetLastError();
-}
-
-// Stage A of a scene frame: per-entity depth pass, keys and the (rank, key, index) sort; per-entity projection beside it.
-// The scene table was copied to sl.scene_dev ahead of the stage (submit), and for a stereo frame the stereo table to
-// sl.stereo_dev: the sort is the head camera's, the projection covers every view.
-static cudaError_t enqueue_scene_sort_stage(gs_context *c, gs_context::Slot &sl, bool external_events) {
-  auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
-    return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
-  };
-  cudaStream_t m = c->stream, x = c->aux_stream;
-  const FrameBufs b = slot_bufs(c, sl);
-  cudaError_t e;
-  if ((e = cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, m))) return e;
-  if ((e = cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), m))) return e;
-  if ((e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, m))) return e;
-  if ((e = rec(sl.ev[0], m))) return e;
-  launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, m);
-  if ((e = cudaEventRecord(c->ev_fork[0], m))) return e;
-  if ((e = cudaStreamWaitEvent(x, c->ev_fork[0], 0))) return e;
-  if ((e = rec(sl.evp[0], x))) return e;
-  if (sl.stereo) launch_project_stereo(c, sl.stereo_dev, sl.scene_dev, sl.ctr, b, x);
-  else launch_project_scene(c, sl.fp, sl.scene_dev, sl.ctr, b, x);
-  if ((e = rec(sl.evp[1], x))) return e;
-  if ((e = cudaEventRecord(c->ev_join[0], x))) return e;
-  launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, m);
-  launch_scene_radix(c, sl.fp, sl.ctr, b, m);
-  if ((e = rec(sl.ev[1], m))) return e;
+  if ((e = record(sl.ev[1], m, external_events))) return e;
   if ((e = cudaStreamWaitEvent(m, c->ev_join[0], 0))) return e;
   return cudaGetLastError();
 }
 
 // Stage B (bin stream): tile instances in draw order, stable sort by tile, per-tile record lists and ranges.
 static cudaError_t enqueue_bin_stage(gs_context *c, gs_context::Slot &sl, uint32_t n_bins, bool external_events) {
-  auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
-    return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
-  };
   cudaStream_t m = c->bstream;
   const FrameBufs b = slot_bufs(c, sl);
   cudaError_t e;
   if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, m))) return e;
-  if ((e = rec(sl.ev[2], m))) return e;
+  if ((e = record(sl.ev[2], m, external_events))) return e;
   launch_emit(c, slot_fp(sl), sl.ctr, b, nullptr, m);
   launch_tile_radix(c, sl.ctr, b, n_bins, m);    // pass T1; above 256 bins also pass T2 + k_tile_ranges
-  if ((e = rec(sl.ev[3], m))) return e;
+  if ((e = record(sl.ev[3], m, external_events))) return e;
   return cudaGetLastError();
 }
 
 // Stage C (raster stream, low priority): reads only this frame's inst_rec / bin_range copy.
 static cudaError_t enqueue_raster_stage(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, bool external_events) {
-  auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
-    return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
-  };
   cudaError_t e;
   if (sl.peer) launch_peer_acquire(c, sl.fp, sl.ctr, c->rstream);
-  if ((e = rec(sl.ev_r0, c->rstream))) return e;
+  if ((e = record(sl.ev_r0, c->rstream, external_events))) return e;
   if (sl.stereo) launch_raster_stereo(c, slot_fp(sl), n_tiles, slot_bufs(c, sl), sl.raster_flags, c->rstream);
   else launch_raster(c, sl.fp, n_tiles, slot_bufs(c, sl), sl.raster_flags, c->rstream);
-  if ((e = rec(sl.ev[4], c->rstream))) return e;
+  if ((e = record(sl.ev[4], c->rstream, external_events))) return e;
   if (sl.peer) launch_peer_signal_wait(c, sl.fp, sl.ctr, c->rstream);
   return cudaGetLastError();
 }
@@ -1036,39 +1068,61 @@ static int run_graph(gs_context *c, cudaGraphExec_t &ge, cudaStream_t stream, F 
   return GS_OK;
 }
 
+// The cached graph of one stage of the slot's frame in its buffer set (GraphId).  A slab frame has two stages: its keys
+// stage is kSortStage, its slab loop kRasterStage.  Plain and scene frames differ in their sort stage only.
+enum FrameStage { kSortStage, kBinStage, kRasterStage };
+static int slab_graph_base(const gs_context::Slot &sl) {
+  return sl.stereo ? kGraphSlabViews : (sl.scene ? kGraphSlabScene : kGraphSlabPlain);
+}
+static cudaGraphExec_t &stage_graph(gs_context::Slot &sl, FrameStage stage, bool reuse) {
+  int id;
+  if (sl.slab) {
+    id = slab_graph_base(sl);
+    if (stage != kSortStage) id += sl.peer ? 3 : ((sl.raster_flags & 2u) ? 2 : 1);  // loop: plain, depth-tested, fused peer exchange
+  } else if (sl.stereo) {
+    id = kGraphViewsSort + (int)stage;
+  } else if (stage == kSortStage) {
+    id = sl.scene ? kGraphSortScene : (reuse ? kGraphSortReuse : kGraphSort);
+  } else {
+    id = stage == kBinStage ? kGraphBin : (sl.peer ? kGraphRasterPeer : kGraphRaster);
+  }
+  return sl.graph[sl.set][id];
+}
+
+// (re)capture when anything baked into the launches changed.  Views frames keep their own graphs and key (n_tiles, n_bins:
+// every view's), so neither kind re-captures the other's
+static void sync_graph_key(gs_context *c, const gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
+  const gs_context::GraphKey k = graph_key(c, sl, n_tiles, n_bins);
+  const GraphDomain domain = sl.stereo ? kGraphsViews : kGraphsMono;
+  if (memcmp(&k, &c->gkey[domain], sizeof(k)) != 0) {
+    drop_graphs(c, domain);
+    c->gkey[domain] = k;
+  }
+}
+
 // Three frames overlap: while frame k is rasterised (stream C), frame k+1 is binned (stream B) and frame k+2 is
 // sorted / projected (stream A).  A and B are high priority: their short latency-bound kernels slot in as the
 // long issue-bound raster's CTAs retire.  Stage hand-offs are events; buffers between stages are double-buffered.
 static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_t n_tiles, uint32_t n_bins) {
-  // (re)capture when anything baked into the launches changed
-  const gs_context::GraphKey k = graph_key(c, sl, n_tiles, n_bins);
-  // views frames keep their own graphs and key (n_tiles, n_bins: every view's), so neither kind re-captures the other's
-  gs_context::GraphKey &key = sl.stereo ? c->gkey_stereo : c->gkey;
-  if (memcmp(&k, &key, sizeof(k)) != 0) {
-    if (sl.stereo) drop_stereo_graphs(c);
-    else drop_graphs(c);
-    key = k;
-  }
+  sync_graph_key(c, sl, n_tiles, n_bins);
   const int set = sl.set;
   // A: order/proj_rec/rect[set] must no longer be read by the binning stage that used them last
   if (c->sort_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->sort_set_free[set], 0));
-  cudaGraphExec_t &ga = sl.stereo ? sl.graph_xa[set] : sl.graph_as[set];
-  int rc = sl.scene ? run_graph(c, ga, c->stream, [&](bool ext) { return enqueue_scene_sort_stage(c, sl, ext); })
-                    : run_graph(c, sl.graph_a[set][reuse ? 1 : 0], c->stream, [&](bool ext) { return enqueue_sort_stage(c, sl, reuse, ext); });
+  int rc = run_graph(c, stage_graph(sl, kSortStage, reuse), c->stream, [&](bool ext) { return enqueue_sort_stage(c, sl, reuse, ext); });
   if (rc) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_sorted, c->stream));
   // B: needs A of this frame; inst_rec/bin_range[set] must no longer be read by the raster that used them last
   GS_CUDA(c, cudaStreamWaitEvent(c->bstream, sl.ev_sorted, 0));
   if (c->bin_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->bstream, c->bin_set_free[set], 0));
-  if ((rc = run_graph(c, sl.stereo ? sl.graph_xb[set] : sl.graph_b[set], c->bstream,
+  if ((rc = run_graph(c, stage_graph(sl, kBinStage, reuse), c->bstream,
                       [&](bool ext) { return enqueue_bin_stage(c, sl, n_bins, ext); }))) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_binned, c->bstream));
   c->sort_set_free[set] = sl.ev_binned;
   // C
   GS_CUDA(c, cudaStreamWaitEvent(c->rstream, sl.ev_binned, 0));
   if (sl.raster_flags == c->raster_base_flags) {
-    cudaGraphExec_t &gr = sl.stereo ? sl.graph_xr[set] : (sl.peer ? sl.graph_rp[set] : sl.graph_r[set]);
-    if ((rc = run_graph(c, gr, c->rstream, [&](bool ext) { return enqueue_raster_stage(c, sl, n_tiles, ext); }))) return rc;
+    if ((rc = run_graph(c, stage_graph(sl, kRasterStage, reuse), c->rstream,
+                        [&](bool ext) { return enqueue_raster_stage(c, sl, n_tiles, ext); }))) return rc;
   } else {
     // depth-tested / statistics / GS_RENDER_BLEND_UNORM8 frames use other instantiations of the raster: plain launches, no
     // cached graph (so a frame of one blend mode never replays a raster graph captured for the other)
@@ -1085,22 +1139,19 @@ static uint64_t slab_cumulative(uint32_t first, int k) { return (uint64_t)first 
 // Stage A of a slab frame (sort stream): depth + cull, keys + bucket histogram, slab plan, every slab's compaction offsets.
 // A scene frame takes the per-entity depth pass and 24-bit keys (the scene table was copied to sl.scene_dev ahead of it).
 static cudaError_t enqueue_slab_keys_stage(gs_context *c, gs_context::Slot &sl, bool external_events) {
-  auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
-    return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
-  };
   cudaStream_t st = c->stream;
   const SceneTable *scene = sl.scene ? sl.scene_dev : nullptr;
   cudaError_t e;
   if ((e = cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, st))) return e;
   if ((e = cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), st))) return e;
   if (scene && (e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, st))) return e;
-  if ((e = rec(sl.ev[0], st))) return e;
+  if ((e = record(sl.ev[0], st, external_events))) return e;
   if (scene) launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, st);
   else launch_depth_cull(c, sl.fp, sl.ctr, st);
   launch_keys(c, sl.fp, sl.ctr, scene, sl.octr, sl.set, st);
   launch_slab_plan(c, sl.fp, sl.ctr, sl.set, c->slab_first, sl.n_slabs, st);
   launch_compact_offsets(c, sl.fp, scene, sl.set, sl.n_slabs, st);  // one pass over the keys for every slab's compaction offsets
-  if ((e = rec(sl.ev[1], st))) return e;
+  if ((e = record(sl.ev[1], st, external_events))) return e;
   return cudaGetLastError();
 }
 
@@ -1108,9 +1159,6 @@ static cudaError_t enqueue_slab_keys_stage(gs_context *c, gs_context::Slot &sl, 
 // the previous one closed.  A views frame runs it once for every view: n_tiles and n_bins of every view.
 static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins,
                                            bool external_events) {
-  auto rec = [&](cudaEvent_t ev, cudaStream_t st) {
-    return external_events ? cudaEventRecordWithFlags(ev, st, cudaEventRecordExternal) : cudaEventRecord(ev, st);
-  };
   cudaStream_t st = c->rstream;
   const FrameBufs b = slot_bufs(c, sl);
   const SceneTable *scene = sl.scene ? sl.scene_dev : nullptr;
@@ -1118,7 +1166,7 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
   const FrameParams *fp = slot_fp(sl);  // the frame's (a stereo frame's pair) for the projection, binning and raster
   cudaError_t e;
   launch_slab_init(c, fp, sl.ctr, sl.stereo, st);
-  if ((e = rec(sl.ev[2], st))) return e;
+  if ((e = record(sl.ev[2], st, external_events))) return e;
   for (int s = 0; s < sl.n_slabs; ++s) {
     launch_slab_begin(c, sl.fp, sl.ctr, scene, sl.set, s, st);   // entry count (0 once every bin is closed) + compaction
     launch_slab_sort(c, sl.fp, sl.ctr, scene, b, st);            // draw order of the slab
@@ -1126,16 +1174,16 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
     if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, st))) return e;
     launch_emit(c, fp, sl.ctr, b, c->bin_open, st);
     launch_tile_radix(c, sl.ctr, b, n_bins, st);
-    if ((e = rec(sl.slab_ev[s][0], st))) return e;
+    if ((e = record(sl.slab_ev[s][0], st, external_events))) return e;
     launch_raster_slab(c, fp, sl.ctr, n_tiles, b, (sl.raster_flags & 2u) != 0, sl.stereo, st);
-    if ((e = rec(sl.slab_ev[s][1], st))) return e;
+    if ((e = record(sl.slab_ev[s][1], st, external_events))) return e;
   }
   launch_slab_end(c, sl.ctr, st);
-  if ((e = rec(sl.ev[3], st))) return e;
+  if ((e = record(sl.ev[3], st, external_events))) return e;
   if (sl.peer) launch_peer_acquire(c, sl.fp, sl.ctr, st);
-  if ((e = rec(sl.ev_r0, st))) return e;
+  if ((e = record(sl.ev_r0, st, external_events))) return e;
   launch_resolve(c, fp, n_tiles, sl.stereo, st);
-  if ((e = rec(sl.ev[4], st))) return e;
+  if ((e = record(sl.ev[4], st, external_events))) return e;
   if (sl.peer) launch_peer_signal_wait(c, sl.fp, sl.ctr, st);
   return cudaGetLastError();
 }
@@ -1144,21 +1192,14 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
 // (raster stream); stage A of frame k+1 runs under the loop of frame k (keys / slab table are double-buffered by set).
 // A views frame passes n_tiles and n_bins of every view and keeps its graphs under the views key, as on the one-pass path.
 static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
-  const gs_context::GraphKey k = graph_key(c, sl, n_tiles, n_bins);
-  gs_context::GraphKey &key = sl.stereo ? c->gkey_stereo : c->gkey;
-  if (memcmp(&k, &key, sizeof(k)) != 0) {
-    if (sl.stereo) drop_stereo_graphs(c);
-    else drop_graphs(c);
-    key = k;
-  }
-  const int set = sl.set, kind = sl.stereo ? 2 : (sl.scene ? 1 : 0);  // plain, scene and stereo frames keep their own graphs
+  sync_graph_key(c, sl, n_tiles, n_bins);
+  const int set = sl.set, kind = sl.stereo ? 2 : (sl.scene ? 1 : 0);  // plain, scene and views frames keep their own graphs
   // slabs of slab_first, 2x, 4x ... entries: enough of them to cover every splat the sort considers
   int n_slabs = 1;
   while (n_slabs < kMaxSlabs && slab_cumulative(c->slab_first, n_slabs) < sl.n_sortable) ++n_slabs;
   if (n_slabs != sl.graph_slabs[set][kind]) {  // the captured stages bake the slab count
-    auto kill = [](cudaGraphExec_t &g) { if (g) { cudaGraphExecDestroy(g); g = nullptr; } };
-    kill(sl.graph_sa[set][kind]);
-    for (auto &g : sl.graph_sl[set][kind]) kill(g);
+    const int base = slab_graph_base(sl), n_ids = sl.stereo ? 3 : 4;  // this set's and kind's keys graph and loop graphs
+    for (int id = base; id < base + n_ids; ++id) kill_graph(sl.graph[set][id]);
     sl.graph_slabs[set][kind] = n_slabs;
   }
   sl.n_slabs = n_slabs;
@@ -1167,16 +1208,14 @@ static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_ti
       if (!sl.slab_ev[s][q]) GS_CUDA(c, cudaEventCreate(&sl.slab_ev[s][q]));
   // A: the keys / slab table of this set must no longer be read by the loop that used them last
   if (c->sort_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->sort_set_free[set], 0));
-  int rc = run_graph(c, sl.graph_sa[set][kind], c->stream, [&](bool ext) { return enqueue_slab_keys_stage(c, sl, ext); });
+  int rc = run_graph(c, stage_graph(sl, kSortStage, false), c->stream, [&](bool ext) { return enqueue_slab_keys_stage(c, sl, ext); });
   if (rc) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_sorted, c->stream));
   // loop: needs A of this frame; consecutive loops are ordered by the stream itself
   GS_CUDA(c, cudaStreamWaitEvent(c->rstream, sl.ev_sorted, 0));
-  // graph variants of the loop: [plain, depth-tested, fused peer exchange]
-  const int variant = sl.peer ? 2 : ((sl.raster_flags & 2u) ? 1 : 0);
   if (sl.peer && (sl.raster_flags & 2u)) {  // depth-tested peer frames: rare, plain launches
     GS_CUDA(c, enqueue_slab_loop_stage(c, sl, n_tiles, n_bins, false));
-  } else if ((rc = run_graph(c, sl.graph_sl[set][kind][variant], c->rstream,
+  } else if ((rc = run_graph(c, stage_graph(sl, kRasterStage, false), c->rstream,
                              [&](bool ext) { return enqueue_slab_loop_stage(c, sl, n_tiles, n_bins, ext); }))) {
     return rc;
   }
@@ -1234,6 +1273,16 @@ static void sh_camera(const float mv[16], float4 &cam) {
   cam = make_float4((float)(dot(u, bc) / det), (float)(dot(a, uc) / det), (float)(dot(a, bu) / det), 0.0f);
 }
 
+// the tile and bin grid of a width x height frame (n_bins <= 64 * 64: fits the 16-bit bin id)
+static void fill_grid(uint32_t width, uint32_t height, RenderConsts &rc) {
+  rc.tiles_x = (width + kTile - 1) / kTile;
+  rc.tiles_y = (height + kTile - 1) / kTile;
+  rc.n_tiles = rc.tiles_x * rc.tiles_y;
+  rc.bins_x = (width + kBin - 1) / kBin;
+  rc.bins_y = (height + kBin - 1) / kBin;
+  rc.n_bins = rc.bins_x * rc.bins_y;
+}
+
 // a frame's RenderConsts from its parameters
 static void fill_render_consts(gs_context *c, const gs_render_params *p, RenderConsts &rc) {
   memcpy(rc.proj, p->proj, sizeof(rc.proj));
@@ -1244,12 +1293,7 @@ static void fill_render_consts(gs_context *c, const gs_render_params *p, RenderC
   rc.vh = (float)p->height;
   // index.js:191: focal = (viewport.w / 2.0) * Math.abs(projectionMatrix.elements[5]), fp64 then f32 uniform
   rc.focal = p->focal > 0.0f ? p->focal : (float)(((double)p->height / 2.0) * fabs((double)p->proj[5]));
-  rc.tiles_x = (p->width + kTile - 1) / kTile;
-  rc.tiles_y = (p->height + kTile - 1) / kTile;
-  rc.n_tiles = rc.tiles_x * rc.tiles_y;
-  rc.bins_x = (p->width + kBin - 1) / kBin;
-  rc.bins_y = (p->height + kBin - 1) / kBin;
-  rc.n_bins = rc.bins_x * rc.bins_y;
+  fill_grid(p->width, p->height, rc);
   memcpy(rc.bg, p->bg_rgba, sizeof(rc.bg));
   rc.shard_rank = c->shard_rank;
   rc.shard_world = c->shard_world;
@@ -1458,7 +1502,6 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
     sl.pending = false;
     if (sl.peer) {
       // the frame has been published to (and consumed by) the other ranks: it cannot be silently re-run
-      const bool bad = sl.ctr_host->overflow || sl.ctr_host->peer_timeout;
       PeerRows rows{};
       for (uint32_t r = 0; r < c->peer_world; ++r) rows.p[r] = peer_released_row(c->peer_base[r], sl.ring);
       launch_peer_release(c, rows, c->peer_world, c->peer_rank, sl.peer_seq, c->copy_stream);
@@ -1466,7 +1509,6 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
       if (sl.ctr_host->peer_timeout) return fail(c, GS_ERR_CUDA, "fused exchange: a peer did not signal in time");
       if (sl.ctr_host->overflow)
         return fail(c, GS_ERR_CAPACITY, "instance buffer overflow in a GS_RENDER_OUT_PEER frame: size the buffers with one plain frame first");
-      (void)bad;
       break;
     }
     if (!sl.ctr_host->overflow) break;
@@ -1486,15 +1528,14 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
       int rc_old = wait_slot(c, *older, nullptr);
       if (rc_old) return rc_old;
     }
-    GS_CUDA(c, cudaStreamSynchronize(c->stream));  // the other slots' frames may still be using the buffers
-    GS_CUDA(c, cudaStreamSynchronize(c->bstream));
-    GS_CUDA(c, cudaStreamSynchronize(c->rstream));
+    int rcode = sync_streams(c);  // the other slots' frames may still be using the buffers
+    if (rcode) return rcode;
     // grow once to the measured demand (+12.5 %); a frame whose overflow flag is stale (an earlier frame's regrow
     // already made room) is simply run again
     const uint64_t demand = sl.slab ? sl.ctr_host->n_inst_slab_max : sl.ctr_host->n_inst;
     if (demand > c->cap_inst) {
       const uint64_t need = std::max<uint64_t>(demand + demand / 8, c->cap_inst + c->cap_inst / 2);
-      int rcode = ensure_instances(c, need);
+      rcode = ensure_instances(c, need);
       if (rcode) {
         // a refused frame leaves no sorted count behind: the next frame picks its path from the splats it may sort, as
         // on a fresh context, not from the count of whatever frame completed before the refused one
@@ -1503,7 +1544,6 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
         return rc_t ? rc_t : rcode;
       }
     }
-    int rcode;
     sl.restage = false;  // a target frame blends over the rectangles staged at its first submission
     if ((rcode = submit(c, sl))) return rcode;
   }
@@ -1624,25 +1664,24 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
   int rcode;
   if ((rcode = check_blend8(c, p))) return rcode;
-  auto tiles_of = [](const gs_render_params &q) { return ((q.width + kTile - 1) / kTile) * ((q.height + kTile - 1) / kTile); };
-  auto bins_of = [](const gs_render_params &q) { return ((q.width + kBin - 1) / kBin) * ((q.height + kBin - 1) / kBin); };
-  const uint32_t n_tiles = tiles_of(*p);
-  const uint32_t n_bins = bins_of(*p);  // <= 64*64: fits the 16-bit bin id
   // a views frame's bin table holds every view's bins (4 * 43 * 43 at most, still a 16-bit id), its slab state every
   // view's tiles
-  uint32_t n_bins_all = n_bins, slab_tiles = n_tiles;
-  if (stereo) {
-    n_bins_all = slab_tiles = 0;
-    for (uint32_t v = 0; v < stereo->n; ++v) {
-      n_bins_all += bins_of(stereo->views[v]);
-      slab_tiles += tiles_of(stereo->views[v]);
-    }
+  FrameNeeds need{};
+  need.scene = scene != nullptr;
+  need.n_views = stereo ? stereo->n : 1u;
+  for (uint32_t v = 0; v < need.n_views; ++v) {
+    const gs_render_params &q = stereo ? stereo->views[v] : *p;
+    RenderConsts grid;
+    fill_grid(q.width, q.height, grid);
+    if (v == 0) need.n_tiles = grid.n_tiles;
+    need.n_bins_all += grid.n_bins;
+    need.n_tiles_all += grid.n_tiles;
   }
   GS_CUDA(c, cudaSetDevice(c->device));
   const uint64_t ticket = c->next_ticket;
   gs_context::Slot &sl = c->slot[ticket % gs_context::kSlots];
   if (sl.pending && (rcode = wait_slot(c, sl, nullptr))) return rcode;  // slot reuse: its previous frame must be done
-  if (target && (rcode = wait_overlapping(c, *target, stereo ? stereo->views : p, stereo ? stereo->n : 1u))) return rcode;
+  if (target && (rcode = wait_overlapping(c, *target, stereo ? stereo->views : p, need.n_views))) return rcode;
   if ((p->flags & GS_RENDER_OUT_PEER) && ticket >= 3) {
     // the shared frame ring of the fused exchange has three entries, released by gs_wait: at most three such frames
     gs_context::Slot &o = c->slot[(ticket - 3) % gs_context::kSlots];
@@ -1663,37 +1702,15 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   // always one-pass: the slab path stops at front-to-back saturation, which rounding after every blend does not have
   const bool slab = expect_sorted >= (stereo ? c->slab_min_xr : c->slab_min) &&
                     !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS | GS_RENDER_BLEND_UNORM8));
+  need.slab = slab;
   if ((int)slab != c->last_mode) {
-    if ((rcode = drain(c))) return rcode;
-    GS_CUDA(c, cudaStreamSynchronize(c->stream));
-    GS_CUDA(c, cudaStreamSynchronize(c->bstream));
-    GS_CUDA(c, cudaStreamSynchronize(c->rstream));
+    if ((rcode = idle(c))) return rcode;
     c->last_mode = (int)slab;
   }
   // growing any shared buffer needs an idle pipeline
-  const bool grow = (slab && (c->slab_cap < c->cap || !c->key32[0] || c->slab_tiles_cap < slab_tiles || !c->slab_tab[1])) || !(c->scratch_cap >= c->cap && c->depth) || !(n_bins_all <= c->bins_cap && c->bin_range[0]) || !(n_tiles <= c->tile_stats_cap && c->tile_stats) || c->cap_inst == 0 ||
-                    (scene && !(c->scene_cap >= c->cap && c->scene_key)) || (stereo && !stereo_bufs_ok(c, stereo->n));
-  if (grow) {
-    if ((rcode = drain(c))) return rcode;
-    GS_CUDA(c, cudaStreamSynchronize(c->stream));
-    GS_CUDA(c, cudaStreamSynchronize(c->bstream));
-    GS_CUDA(c, cudaStreamSynchronize(c->rstream));
-    if ((rcode = ensure_scratch(c))) return rcode;
-    if ((rcode = ensure_bins(c, n_bins_all))) return rcode;
-    if ((rcode = ensure_tile_stats(c, n_tiles))) return rcode;
-    if (slab && (rcode = ensure_slab(c, slab_tiles))) return rcode;
-    if (scene && (rcode = ensure_scene_bufs(c))) return rcode;
-    if (stereo && (rcode = ensure_stereo_bufs(c, stereo->n))) return rcode;
-    if (c->cap_inst == 0) {
-      // first frame: room for two bin instances per resident splat (a typical scene needs ~1); GS_INST_CAP overrides
-      // the initial size (tests of the overflow / regrow path)
-      uint64_t first = std::max<uint64_t>(1u << 20, slab ? (uint64_t)c->n : (uint64_t)c->n * 2);
-      if (const char *e = getenv("GS_INST_CAP")) first = std::max<uint64_t>(1024, strtoull(e, nullptr, 10));
-      if ((rcode = ensure_instances(c, first))) return rcode;
-    }
-  }
+  if (!frame_bufs_ready(c, need) && ((rcode = idle(c)) || (rcode = ensure_frame_bufs(c, need)))) return rcode;
   sl.params = *p;
-  sl.n_views = stereo ? stereo->n : 1u;
+  sl.n_views = need.n_views;
   sl.view[0] = *p;
   sl.out_user[0] = out_rgba;
   sl.ticket = ticket;
@@ -1823,45 +1840,7 @@ extern "C" int gs_sort_scene(gs_context *c, const gs_object *objs, uint32_t n_ob
   size_t bytes = 0;
   int rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
   if (rc) return rc;
-  if ((rc = drain(c))) return rc;
-  GS_CUDA(c, cudaStreamSynchronize(c->stream));
-  GS_CUDA(c, cudaStreamSynchronize(c->bstream));
-  GS_CUDA(c, cudaStreamSynchronize(c->rstream));
-  if ((rc = ensure_scratch(c))) return rc;
-  if ((rc = ensure_scene_bufs(c))) return rc;
-  gs_context::Slot &sl = c->slot[0];
-  if ((rc = ensure_slot_scene(c, sl))) return rc;
-  c->last_set = 0;
-  const FrameBufs bufs{c->order[0], c->proj_rec[0], c->rect[0], c->inst_rec[0], c->bin_range[0]};
-  memset(sl.fp_host, 0, sizeof(FrameParams));
-  sl.fp_host->n_splats = c->n;
-  memcpy(sl.scene_host, c->scene_tmp, bytes);
-  if (c->pushed) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->push_done, 0));
-  GS_CUDA(c, cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, c->stream));
-  GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, bytes, cudaMemcpyHostToDevice, c->stream));
-  GS_CUDA(c, cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), c->stream));
-  GS_CUDA(c, cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, c->stream));
-  GS_CUDA(c, cudaEventRecord(c->ev[0], c->stream));
-  launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
-  launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
-  launch_scene_radix(c, sl.fp, sl.ctr, bufs, c->stream);
-  GS_CUDA(c, cudaGetLastError());
-  GS_CUDA(c, cudaEventRecord(c->ev[1], c->stream));
-  GS_CUDA(c, cudaMemcpyAsync(sl.ctr_host, sl.ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, c->stream));
-  GS_CUDA(c, cudaStreamSynchronize(c->stream));
-  memset(&c->stats, 0, sizeof(c->stats));
-  stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
-  c->stats.kernel_launches = 11;
-  float ms = 0;
-  cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]);
-  c->stats.ms_sort = ms;
-  c->stats.ms_total = ms;
-  c->have_order = false;  // a concatenation of several entities' orders is no single-entity order
-  c->order_count = sl.ctr_host->sort.n_valid;
-  if (out_count) *out_count = c->order_count;
-  if (out_idx && c->order_count)
-    GS_CUDA(c, cudaMemcpy(out_idx, c->order[0], sizeof(uint32_t) * (size_t)c->order_count, cudaMemcpyDeviceToHost));
-  return GS_OK;
+  return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count);
 }
 
 extern "C" int gs_wait(gs_context *c, uint64_t ticket, gs_stats *stats) {
@@ -2166,8 +2145,5 @@ extern "C" void *gs_stream(gs_context *c) { return c ? (void *)c->rstream : null
 extern "C" int gs_synchronize(gs_context *c) {
   if (!c) return GS_ERR_INVALID;
   GS_CUDA(c, cudaSetDevice(c->device));
-  GS_CUDA(c, cudaStreamSynchronize(c->stream));
-  GS_CUDA(c, cudaStreamSynchronize(c->bstream));
-  GS_CUDA(c, cudaStreamSynchronize(c->rstream));
-  return GS_OK;
+  return sync_streams(c);
 }

@@ -231,6 +231,23 @@ struct SlabTable {
   uint32_t count[kMaxSlabs];    // entries of slab s
 };
 
+// ---- the stage graphs a slot caches per buffer set (gs_context::Slot::graph).  Two domains, each dropped as a whole when
+// its own gs_context::GraphKey changes: mono (plain and scene frames, which share their bin and raster graphs) and views.
+// The four (views: three) ids of a slab kind are its keys stage and its slab loop without depth test, depth-tested and with
+// the fused peer exchange (views frames are never peer frames).
+// Invariant: an id stands for exactly one captured launch sequence.  A frame captures its stage's id only when that id is
+// empty - after a drop of its domain (key change, or the bin table / slab state both domains share regrown) or, for a slab
+// kind, a change of its slab count - and replays it otherwise: a scene frame captures no bin graph of its own, and a views
+// frame invalidates no mono graph except through those shared buffers ----
+enum GraphId : int {
+  kGraphSort, kGraphSortReuse, kGraphSortScene, kGraphBin, kGraphRaster, kGraphRasterPeer,
+  kGraphSlabPlain, kGraphSlabScene = kGraphSlabPlain + 4,
+  kGraphViewsFirst = kGraphSlabScene + 4,  // mono ids end, views ids begin
+  kGraphViewsSort = kGraphViewsFirst, kGraphViewsBin, kGraphViewsRaster, kGraphSlabViews,
+  kGraphCount = kGraphSlabViews + 3
+};
+enum GraphDomain : int { kGraphsMono, kGraphsViews };
+
 }  // namespace gs
 
 struct gs_context {
@@ -372,18 +389,10 @@ struct gs_context {
     cudaEvent_t ev[5]{};                     // stage boundaries (timing)
     cudaEvent_t evp[2]{};                    // k_project on the aux stream (timing)
     cudaEvent_t ev_done = nullptr, ev_copied = nullptr;
-    // CUDA graphs of the three stages, one per buffer set this slot can be paired with
-    cudaGraphExec_t graph_a[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // sort + project, [set][reuse_sort]
-    cudaGraphExec_t graph_as[2] = {nullptr, nullptr};                          // scene frames: sort + project, [set]
-    cudaGraphExec_t graph_b[2] = {nullptr, nullptr};                           // binning, [set]
-    cudaGraphExec_t graph_r[2] = {nullptr, nullptr};                           // raster, [set]
-    cudaGraphExec_t graph_rp[2] = {nullptr, nullptr};                          // acquire + raster + signal/wait (fused exchange)
-    // slab path, [set][plain | scene | stereo scene frame]: keys stage, slab loop + resolve ([plain | depth | peer]), and the
-    // slab count baked into both
-    cudaGraphExec_t graph_sa[2][3] = {};
-    cudaGraphExec_t graph_sl[2][3][3] = {};
+    // CUDA graphs of the stages, one per buffer set this slot can be paired with: [set][GraphId]; and the slab count
+    // baked into the keys and loop graphs of each slab kind: [set][plain | scene | views]
+    cudaGraphExec_t graph[2][gs::kGraphCount] = {};
     int graph_slabs[2][3] = {};
-    cudaGraphExec_t graph_xa[2] = {}, graph_xb[2] = {}, graph_xr[2] = {};  // stereo scene frames: the three stages, [set]
     bool peer = false;
     uint64_t ticket = 0;
     int ring = 0;                            // slot of the shared frame ring (fused exchange)
@@ -434,8 +443,7 @@ struct gs_context {
     uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr;
     uint32_t n_views = 0, view_size[gs::kMaxViews] = {}, pad2 = 0; const void *px = nullptr;
     const void *psh = nullptr; uint32_t sh_degree = 0, pad3 = 0;  // the projection's instantiation and SH table
-  } gkey;
-  GraphKey gkey_stereo;                          // ... of the views graphs (kept apart: a views frame re-captures only its own)
+  } gkey[2];                                     // [GraphDomain] (kept apart: a views frame re-captures only its own graphs)
 
   // ---- fused exchange: one shared allocation per rank = flag rows + a ring of 3 frames, opened by every peer ----
   void *peer_local = nullptr;            // our shared block
