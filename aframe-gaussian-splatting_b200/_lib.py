@@ -51,6 +51,15 @@ class GsObject(C.Structure):
     ]
 
 
+GS_PICK_NONE = 0xFFFFFFFF
+GS_MAX_PICKS = 4096
+
+
+class GsPick(C.Structure):
+    """gs_pick: the splat, entity, window depth and alpha where a pixel of a scene frame turns half opaque."""
+    _fields_ = [("splat", C.c_uint32), ("object", C.c_int32), ("depth", C.c_float), ("alpha", C.c_float)]
+
+
 class GsTarget(C.Structure):
     """gs_target: the framebuffer a target frame is blended into in place (colour, optional depth, pitch x rows)."""
     _fields_ = [
@@ -112,6 +121,8 @@ SYMBOLS = {
     "gs_render_scene_views_target": (C.c_int, [_P, C.POINTER(GsRenderParams), C.c_uint32, C.POINTER(GsObject),
                                                C.POINTER(C.c_float), C.c_uint32, C.POINTER(GsTarget), C.POINTER(C.c_uint32),
                                                C.POINTER(GsStats)]),
+    "gs_pick_scene": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.c_uint32, C.POINTER(C.c_uint32),
+                                C.c_uint32, C.POINTER(GsPick)]),
     "gs_read_projected": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
     "gs_get_stats": (C.c_int, [_P, C.POINTER(GsStats)]),
     "gs_set_shard": (C.c_int, [_P, C.c_uint32, C.c_uint32]),

@@ -35,6 +35,42 @@ def xr_viewports(viewports, ratio: float):
     return [tuple(int(math.floor(c * ratio)) for c in vp) for vp in viewports]
 
 
+def _unproject(frame: FrameInputs, modelview, object3d: Object3D, xy, depth: float) -> np.ndarray:
+    """World position (fp64) of pixel centre xy (row 0 = bottom) at window depth `depth` of an entity drawn with `frame`'s
+    projection and its gsModelViewMatrix: inverse(P * MV) takes the window point to the table's frame; the table's frame
+    is the entity's local frame with y negated (getModelViewMatrix conjugates by diag(1, -1, 1, 1), index.js:467-487), so
+    object3D.matrixWorld * diag(1, -1, 1, 1) takes it to the world."""
+    P = np.asarray(frame.proj, np.float64).reshape(4, 4).T  # column-major elements
+    MV = np.asarray(modelview, np.float64).reshape(4, 4).T
+    ndc = np.array([(xy[0] + 0.5) / frame.width * 2.0 - 1.0, (xy[1] + 0.5) / frame.height * 2.0 - 1.0, depth * 2.0 - 1.0, 1.0])
+    q = np.linalg.solve(P @ MV, ndc)
+    local = np.array([q[0] / q[3], -q[1] / q[3], q[2] / q[3], 1.0])
+    W = np.asarray(object3d.matrixWorld.elements, np.float64).reshape(4, 4).T
+    return (W @ local)[:3]
+
+
+def _look_quaternion(d: np.ndarray):
+    """Quaternion (x, y, z, w) turning a camera's -Z axis onto the unit vector d (up stays as close to +Y as it can)."""
+    up = np.array([0.0, 1.0, 0.0]) if abs(d[1]) < 0.999 else np.array([0.0, 0.0, 1.0])
+    z = -d
+    x = np.cross(up, z)
+    x /= np.linalg.norm(x)
+    y = np.cross(z, x)
+    m = np.stack([x, y, z], axis=1)  # columns: the camera's axes in the world
+    t = m[0, 0] + m[1, 1] + m[2, 2]
+    if t > 0:
+        s = 0.5 / math.sqrt(t + 1.0)
+        return ((m[2, 1] - m[1, 2]) * s, (m[0, 2] - m[2, 0]) * s, (m[1, 0] - m[0, 1]) * s, 0.25 / s)
+    i = int(np.argmax([m[0, 0], m[1, 1], m[2, 2]]))
+    j, k = (i + 1) % 3, (i + 2) % 3
+    s = 2.0 * math.sqrt(1.0 + m[i, i] - m[j, j] - m[k, k])
+    q = [0.0, 0.0, 0.0]
+    q[i] = 0.25 * s
+    q[j] = (m[j, i] + m[i, j]) / s
+    q[k] = (m[k, i] + m[i, k]) / s
+    return (q[0], q[1], q[2], (m[k, j] - m[j, k]) / s)
+
+
 class SortWorker:
     """The Web Worker's message protocol (index.js:572-598) served by the GPU context.
 
@@ -385,6 +421,45 @@ class SplatScene:
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out,
                                           blend_unorm8=blend_unorm8)
+
+    def pick(self, points, width: int, height: int, camera=None, depth_in: Optional[np.ndarray] = None):
+        """What lies under pixels of the frame render() draws with these arguments (gs_pick_scene): for each (x, y) of
+        `points` (frame pixels, row 0 = bottom) the splat where the pixel turns half opaque.  Returns one dict per point,
+        None where no splat is hit: `component` (the visible entity: later entities cover earlier ones), `index` (the
+        splat's row in that entity's range), `depth` (window depth of its quad), `alpha` (the pixel's final alpha) and
+        `point` (the world position, fp64: the pixel centre at that depth unprojected through the entity's
+        gsProjectionMatrix * gsModelViewMatrix to the table's frame, then taken by object3D.matrixWorld * diag(1, -1, 1, 1),
+        the frame the reference's cutout test uses, index.js:532-533)."""
+        if not self.entities:
+            raise ValueError("SplatScene.pick: no entity added")
+        frame, objs = self.objects(width, height, camera)
+        xy = np.ascontiguousarray(points, dtype=np.uint32).reshape(-1, 2)
+        splat, obj, depth, alpha = self.renderer.pick_scene(frame, objs, xy, depth_in=depth_in)
+        out = []
+        for (x, y), s, k, d, a in zip(xy, splat, obj, depth, alpha):
+            if k < 0:
+                out.append(None)
+                continue
+            comp, o = self.entities[k], objs[k]
+            out.append({"component": comp, "index": int(s) - int(o.first), "depth": float(d), "alpha": float(a),
+                        "point": _unproject(frame, o.modelview, comp.object, (int(x), int(y)), float(d))})
+        return out
+
+    def raycast(self, origin, direction, camera, size: int = 1):
+        """A gaze cursor's or controller laser's ray from `origin` along `direction` (world frame): the pick of the centre
+        pixel of a size x size view (size odd, so the pixel centre lies on the ray) looking down the ray with `camera`'s
+        projection.  Returns the pick's dict plus `distance` along the ray (fp64), or None."""
+        if size % 2 != 1:
+            raise ValueError("SplatScene.raycast: size must be odd")
+        o = np.asarray(origin, np.float64)
+        dvec = np.asarray(direction, np.float64)
+        dvec = dvec / np.linalg.norm(dvec)
+        eye = PerspectiveCamera(fov=camera.fov, aspect=1.0, near=camera.near, far=camera.far, position=tuple(o),
+                                quaternion=_look_quaternion(dvec))
+        hit = self.pick([(size // 2, size // 2)], size, size, camera=eye)[0]
+        if hit is not None:
+            hit["distance"] = float(np.dot(np.asarray(hit["point"]) - o, dvec))
+        return hit
 
     def render_into(self, color: np.ndarray, depth: Optional[np.ndarray] = None, viewport=(0, 0), width: Optional[int] = None,
                     height: Optional[int] = None, camera=None, fmt: int = GS_FORMAT_RGBA8,

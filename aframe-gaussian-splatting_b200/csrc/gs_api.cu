@@ -186,9 +186,10 @@ static void kill_graph(cudaGraphExec_t &g) {
   if (g) { cudaGraphExecDestroy(g); g = nullptr; }
 }
 
-// every cached graph of one domain (GraphId: the mono ids come first)
+// every cached graph of one domain (GraphId: the mono ids come first, then the views ids, then the pick ids)
 static void drop_graphs(gs_context *c, GraphDomain domain) {
-  const int first = domain == kGraphsViews ? kGraphViewsFirst : 0, end = domain == kGraphsViews ? kGraphCount : kGraphViewsFirst;
+  static const int kFirst[kGraphDomains + 1] = {0, kGraphViewsFirst, kGraphPickFirst, kGraphCount};
+  const int first = kFirst[domain], end = kFirst[domain + 1];
   for (auto &sl : c->slot)
     for (auto &set : sl.graph)
       for (int id = first; id < end; ++id) kill_graph(set[id]);
@@ -200,6 +201,7 @@ static int ensure_bins(gs_context *c, uint32_t n_bins) {
   // the captured stages bake bin_range; a views frame grows it to every view's bins while a mono frame's key stays put
   drop_graphs(c, kGraphsMono);
   drop_graphs(c, kGraphsViews);
+  drop_graphs(c, kGraphsPick);
   dev_free(c->bin_range[0]); dev_free(c->bin_range[1]);
   GS_CUDA(c, dev_alloc(&c->bin_range[0], (size_t)n_bins + 1));
   GS_CUDA(c, dev_alloc(&c->bin_range[1], (size_t)n_bins + 1));
@@ -282,6 +284,22 @@ static int ensure_frame_bufs(gs_context *c, const FrameNeeds &f) {
     if (const char *e = getenv("GS_INST_CAP")) first = std::max<uint64_t>(1024, strtoull(e, nullptr, 10));
     if ((rc = ensure_instances(c, first))) return rc;
   }
+  return GS_OK;
+}
+
+// picks: the query points and results (fixed size, allocated by the first pick) and the per-instance payloads, which follow
+// the instance buffers.  Only a pick reads these and one pick is in flight at a time, so they are replaced without draining
+// the frames in flight; the pick graphs that bake them go with them.
+static int ensure_pick_bufs(gs_context *c) {
+  if (!c->pick_in) GS_CUDA(c, cudaMalloc((void **)&c->pick_in, sizeof(PickInput)));
+  if (!c->pick_in_host) GS_CUDA(c, cudaHostAlloc((void **)&c->pick_in_host, sizeof(PickInput), cudaHostAllocDefault));
+  if (!c->pick_out) GS_CUDA(c, dev_alloc(&c->pick_out, (size_t)GS_MAX_PICKS));
+  if (!c->pick_out_host) GS_CUDA(c, cudaHostAlloc((void **)&c->pick_out_host, sizeof(gs_pick) * GS_MAX_PICKS, cudaHostAllocDefault));
+  if (c->pick_cap >= c->cap_inst && c->pick_pay) return GS_OK;
+  drop_graphs(c, kGraphsPick);
+  dev_free(c->pick_pay);
+  GS_CUDA(c, dev_alloc(&c->pick_pay, (size_t)c->cap_inst));
+  c->pick_cap = c->cap_inst;
   return GS_OK;
 }
 
@@ -437,6 +455,7 @@ extern "C" int gs_destroy(gs_context *c) {
   if (c->push_stream) cudaStreamDestroy(c->push_stream);
   drop_graphs(c, kGraphsMono);
   drop_graphs(c, kGraphsViews);
+  drop_graphs(c, kGraphsPick);
   for (uint32_t r = 0; r < c->peer_world; ++r)
     if (r != c->peer_rank && c->peer_base[r]) cudaIpcCloseMemHandle(c->peer_base[r]);
   if (c->peer_local) cudaFree(c->peer_local);
@@ -446,6 +465,9 @@ extern "C" int gs_destroy(gs_context *c) {
   dev_free(c->slab_tab[0]); dev_free(c->slab_tab[1]);
   dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open);
   dev_free(c->scene_key); dev_free(c->scene_pay); dev_free(c->scene_hi);
+  dev_free(c->pick_pay); dev_free(c->pick_in); dev_free(c->pick_out);
+  if (c->pick_in_host) cudaFreeHost(c->pick_in_host);
+  if (c->pick_out_host) cudaFreeHost(c->pick_out_host);
   delete c->scene_tmp;
   for (auto &sl : c->slot) {
     dev_free(sl.ctr); dev_free(sl.fp);
@@ -1029,6 +1051,29 @@ static cudaError_t enqueue_bin_stage(gs_context *c, gs_context::Slot &sl, uint32
   return cudaGetLastError();
 }
 
+// Stage B of a pick (bin stream): the one-pass emission with only the bins of the query points open, and the bin sort
+// whose final pass also keeps every instance's splat index (pick_pay).
+static cudaError_t enqueue_pick_bin_stage(gs_context *c, gs_context::Slot &sl, uint32_t n_bins, bool external_events) {
+  cudaStream_t m = c->bstream;
+  const FrameBufs b = slot_bufs(c, sl);
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, m))) return e;
+  if ((e = record(sl.ev[2], m, external_events))) return e;
+  launch_emit_pick(c, sl.fp, sl.ctr, b, c->pick_in->open, m);
+  launch_tile_radix_pick(c, sl.ctr, b, n_bins, c->pick_pay, m);
+  if ((e = record(sl.ev[3], m, external_events))) return e;
+  return cudaGetLastError();
+}
+
+// Stage C of a pick (raster stream): k_pick over the query points
+static cudaError_t enqueue_pick_stage(gs_context *c, gs_context::Slot &sl, bool external_events) {
+  cudaError_t e;
+  if ((e = record(sl.ev_r0, c->rstream, external_events))) return e;
+  launch_pick(c, sl.fp, sl.scene_dev, slot_bufs(c, sl), c->pick_pay, c->pick_in, c->pick_out, c->rstream);
+  if ((e = record(sl.ev[4], c->rstream, external_events))) return e;
+  return cudaGetLastError();
+}
+
 // Stage C (raster stream, low priority): reads only this frame's inst_rec / bin_range copy.
 static cudaError_t enqueue_raster_stage(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, bool external_events) {
   cudaError_t e;
@@ -1076,7 +1121,10 @@ static int slab_graph_base(const gs_context::Slot &sl) {
 }
 static cudaGraphExec_t &stage_graph(gs_context::Slot &sl, FrameStage stage, bool reuse) {
   int id;
-  if (sl.slab) {
+  if (sl.pick) {
+    id = stage == kSortStage ? (sl.scene ? kGraphPickSortScene : kGraphPickSortPlain)
+                             : (stage == kBinStage ? kGraphPickBin : kGraphPick);
+  } else if (sl.slab) {
     id = slab_graph_base(sl);
     if (stage != kSortStage) id += sl.peer ? 3 : ((sl.raster_flags & 2u) ? 2 : 1);  // loop: plain, depth-tested, fused peer exchange
   } else if (sl.stereo) {
@@ -1093,7 +1141,7 @@ static cudaGraphExec_t &stage_graph(gs_context::Slot &sl, FrameStage stage, bool
 // every view's), so neither kind re-captures the other's
 static void sync_graph_key(gs_context *c, const gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
   const gs_context::GraphKey k = graph_key(c, sl, n_tiles, n_bins);
-  const GraphDomain domain = sl.stereo ? kGraphsViews : kGraphsMono;
+  const GraphDomain domain = sl.pick ? kGraphsPick : (sl.stereo ? kGraphsViews : kGraphsMono);
   if (memcmp(&k, &c->gkey[domain], sizeof(k)) != 0) {
     drop_graphs(c, domain);
     c->gkey[domain] = k;
@@ -1114,13 +1162,17 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
   // B: needs A of this frame; inst_rec/bin_range[set] must no longer be read by the raster that used them last
   GS_CUDA(c, cudaStreamWaitEvent(c->bstream, sl.ev_sorted, 0));
   if (c->bin_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->bstream, c->bin_set_free[set], 0));
-  if ((rc = run_graph(c, stage_graph(sl, kBinStage, reuse), c->bstream,
-                      [&](bool ext) { return enqueue_bin_stage(c, sl, n_bins, ext); }))) return rc;
+  if ((rc = run_graph(c, stage_graph(sl, kBinStage, reuse), c->bstream, [&](bool ext) {
+         return sl.pick ? enqueue_pick_bin_stage(c, sl, n_bins, ext) : enqueue_bin_stage(c, sl, n_bins, ext);
+       }))) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_binned, c->bstream));
   c->sort_set_free[set] = sl.ev_binned;
   // C
   GS_CUDA(c, cudaStreamWaitEvent(c->rstream, sl.ev_binned, 0));
-  if (sl.raster_flags == c->raster_base_flags) {
+  if (sl.pick) {
+    if ((rc = run_graph(c, stage_graph(sl, kRasterStage, reuse), c->rstream,
+                        [&](bool ext) { return enqueue_pick_stage(c, sl, ext); }))) return rc;
+  } else if (sl.raster_flags == c->raster_base_flags) {
     if ((rc = run_graph(c, stage_graph(sl, kRasterStage, reuse), c->rstream,
                         [&](bool ext) { return enqueue_raster_stage(c, sl, n_tiles, ext); }))) return rc;
   } else {
@@ -1233,6 +1285,9 @@ static int enqueue_readback(gs_context *c, gs_context::Slot &sl) {
   c->bin_set_free[sl.set] = sl.ev_done;
   GS_CUDA(c, cudaStreamWaitEvent(c->copy_stream, sl.ev_done, 0));
   GS_CUDA(c, cudaMemcpyAsync(sl.ctr_host, sl.ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, c->copy_stream));
+  if (sl.pick)
+    GS_CUDA(c, cudaMemcpyAsync(c->pick_out_host, c->pick_out, sizeof(gs_pick) * c->pick_in_host->n, cudaMemcpyDeviceToHost,
+                               c->copy_stream));
   if (sl.host_out)
     for (uint32_t e = 0; e < sl.n_views; ++e) {
       if (sl.target) {  // a host gs_target: 2-D copies into the rectangles only
@@ -1391,7 +1446,10 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   sl.out_bytes[0] = out_pixels * px_bytes;
   sl.host_out = sl.target ? !sl.target_device : !(p->flags & GS_RENDER_OUT_DEVICE);
   sl.peer = (p->flags & GS_RENDER_OUT_PEER) != 0;
-  if (sl.peer) {
+  if (sl.pick) {  // no frame: the results go to pick_out (a re-run after an overflow may have grown pick_pay's demand)
+    sl.host_out = false;
+    if ((rcode = ensure_pick_bufs(c))) return rcode;
+  } else if (sl.peer) {
     if (!c->peer_world || c->peer_world != c->shard_world || c->peer_rank != c->shard_rank)
       return fail(c, GS_ERR_INVALID, "GS_RENDER_OUT_PEER needs gs_peer_import with the rank/world of gs_set_shard");
     if (rc.out_tiled) return fail(c, GS_ERR_INVALID, "GS_RENDER_OUT_PEER writes row-major frames: do not combine with GS_RENDER_OUT_TILED");
@@ -1450,8 +1508,9 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
     }
     GS_CUDA(c, cudaMemcpyAsync(sl.stereo_dev, sl.stereo_host, sl.stereo_bytes, cudaMemcpyHostToDevice, c->stream));
   }
-  // the scene table goes ahead of the sort stage on its stream (only the entities in use are copied)
-  if (sl.scene) GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, sl.scene_bytes, cudaMemcpyHostToDevice, c->stream));
+  // the scene table goes ahead of the sort stage on its stream (only the entities in use are copied; a pick on the plain
+  // path also maps its hits through it)
+  if (sl.scene || sl.pick) GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, sl.scene_bytes, cudaMemcpyHostToDevice, c->stream));
   if (c->sh_degree) {
     // SH contexts: the camera position of every modelview the projection uses, entity k's view v at k * kMaxViews + v
     const uint32_t n_ent = sl.scene ? sl.scene_host->n : 1u;
@@ -1474,8 +1533,9 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   if ((rcode = enqueue_readback(c, sl))) return rcode;
   c->last_set = sl.set;
   sl.pending = true;
-  // a slab frame leaves no complete draw order behind (GS_RENDER_REUSE_SORT then sorts again), nor does a scene frame
-  c->have_order = !sl.slab && !sl.scene;
+  // a slab frame leaves no complete draw order behind (GS_RENDER_REUSE_SORT then sorts again), nor does a scene frame or a
+  // pick
+  c->have_order = !sl.slab && !sl.scene && !sl.pick;
   return GS_OK;
 }
 
@@ -1547,6 +1607,7 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
     sl.restage = false;  // a target frame blends over the rectangles staged at its first submission
     if ((rcode = submit(c, sl))) return rcode;
   }
+  if (sl.pick) return GS_OK;  // a pick leaves the statistics and the sorted count of the frames as they were
   memset(&c->stats, 0, sizeof(c->stats));
   stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
   c->stats.kernel_launches = sl.launches;
@@ -1717,6 +1778,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   sl.n_splats = c->n;
   sl.n_sortable = sortable;
   sl.slab = slab;
+  sl.pick = false;
   sl.color_in[0] = color_in;
   sl.color_device = (p->flags & GS_RENDER_COLOR_DEVICE) != 0;
   sl.target = target != nullptr;
@@ -1831,6 +1893,90 @@ extern "C" int gs_render_scene(gs_context *c, const gs_render_params *frame, con
   int rc = gs_render_scene_async(c, frame, objs, n_objs, color_in, out_rgba, &t);
   if (rc) return rc;
   return gs_wait(c, t, stats);
+}
+
+// gs_pick_scene: the scene frame's sort and projection stage, then a bin stage that bins only the bins of the query points
+// and keeps each instance's splat index, then k_pick.  It takes a slot and a buffer set like a frame and is waited for at once.
+extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                             const uint32_t *xy, uint32_t n_points, gs_pick *out) {
+  if (!c || !frame || !xy || !out) return GS_ERR_INVALID;
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_pick_scene before any push");
+  if (n_points == 0 || n_points > GS_MAX_PICKS) return fail(c, GS_ERR_INVALID, "gs_pick_scene: between 1 and GS_MAX_PICKS points");
+  if (frame->flags & ~(uint32_t)GS_RENDER_DEPTH_DEVICE)
+    return fail(c, GS_ERR_INVALID, "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE is accepted");
+  if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "gs_pick_scene: not on a sharded context");
+  if (frame->width == 0 || frame->height == 0 || frame->width > 4096 || frame->height > 4096)
+    return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
+  if (frame->out_format != GS_FORMAT_RGBA8 && frame->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+  for (uint32_t i = 0; i < n_points; ++i)
+    if (xy[2 * i] >= frame->width || xy[2 * i + 1] >= frame->height)
+      return fail(c, GS_ERR_INVALID, "gs_pick_scene: a point lies outside the frame");
+  size_t bytes = 0;
+  int rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
+  if (rc) return rc;
+  // the frame gs_render_scene draws: one entity over the whole table takes the plain path with its matrices
+  gs_render_params p = *frame;
+  const bool plain = n_objs == 1 && objs[0].first == 0 && objs[0].count == c->n;
+  if (plain) {
+    memcpy(p.modelview, objs[0].modelview, sizeof(p.modelview));
+    p.has_cutout = objs[0].has_cutout;
+    memcpy(p.cutout16, objs[0].cutout16, sizeof(p.cutout16));
+  }
+  GS_CUDA(c, cudaSetDevice(c->device));
+  const uint64_t ticket = c->next_ticket;
+  gs_context::Slot &sl = c->slot[ticket % gs_context::kSlots];
+  if (sl.pending && (rc = wait_slot(c, sl, nullptr))) return rc;
+  if (c->last_mode != 0) {  // always one-pass: the one-pass and slab paths share scratch buffers
+    if ((rc = idle(c))) return rc;
+    c->last_mode = 0;
+  }
+  FrameNeeds need{};
+  need.scene = !plain;
+  need.n_views = 1;
+  {
+    RenderConsts grid;
+    fill_grid(p.width, p.height, grid);
+    need.n_tiles = need.n_tiles_all = grid.n_tiles;
+    need.n_bins_all = grid.n_bins;
+  }
+  if (!frame_bufs_ready(c, need) && ((rc = idle(c)) || (rc = ensure_frame_bufs(c, need)))) return rc;
+  if ((rc = ensure_pick_bufs(c)) || (rc = ensure_slot_scene(c, sl))) return rc;
+  // the points and their bins, ahead of the frame's stages on the sort stream
+  PickInput &in = *c->pick_in_host;
+  in.n = n_points;
+  memset(in.open, 0, sizeof(in.open));
+  const uint32_t bins_x = (p.width + kBin - 1) / kBin;
+  for (uint32_t i = 0; i < n_points; ++i) {
+    in.xy[i] = make_uint2(xy[2 * i], xy[2 * i + 1]);
+    in.open[(xy[2 * i + 1] / kBin) * bins_x + xy[2 * i] / kBin] = 1u;
+  }
+  GS_CUDA(c, cudaMemcpyAsync(c->pick_in, c->pick_in_host, sizeof(PickInput), cudaMemcpyHostToDevice, c->stream));
+  sl.params = p;
+  sl.n_views = 1;
+  sl.view[0] = p;
+  sl.out_user[0] = nullptr;
+  sl.ticket = ticket;
+  sl.n_splats = c->n;
+  sl.n_sortable = c->n;
+  sl.slab = false;
+  sl.pick = true;
+  sl.color_in[0] = nullptr;
+  sl.color_device = false;
+  sl.target = false;
+  sl.restage = true;
+  if (c->sh_degree && !sl.sh_cam_dev) {
+    GS_CUDA(c, cudaMalloc((void **)&sl.sh_cam_dev, sizeof(float4) * kMaxObjects * kMaxViews));
+    GS_CUDA(c, cudaHostAlloc((void **)&sl.sh_cam_host, sizeof(float4) * kMaxObjects * kMaxViews, cudaHostAllocDefault));
+  }
+  sl.scene = !plain;
+  memcpy(sl.scene_host, c->scene_tmp, bytes);
+  sl.scene_bytes = bytes;
+  sl.stereo = false;
+  if ((rc = submit(c, sl))) return rc;
+  c->next_ticket = ticket + 1;
+  if ((rc = wait_slot(c, sl, nullptr))) return rc;
+  memcpy(out, c->pick_out_host, sizeof(gs_pick) * n_points);
+  return GS_OK;
 }
 
 extern "C" int gs_sort_scene(gs_context *c, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx, uint32_t *out_count) {

@@ -224,6 +224,15 @@ __device__ __forceinline__ uint32_t slab_bucket(uint32_t key, uint32_t bits) {
   if (!SCENE) return key >> 4;
   return ((key >> 17) << bits) | min((key & 0x1FFFFu) >> (16u - bits), (1u << bits) - 1u);
 }
+// ---- picks (gs_pick_scene, gs_pick.cu): the query points and the bins that hold them, one host -> device copy per pick.
+// Fixed size (captured graphs bake the pointer); one pick is in flight at a time, since gs_pick_scene waits for it ----
+constexpr uint32_t kMaxPickBins = ((4096 + kBin - 1) / kBin) * ((4096 + kBin - 1) / kBin);
+struct PickInput {
+  uint32_t n, pad[3];
+  uint2 xy[GS_MAX_PICKS];      // pixel of each point, row 0 = bottom
+  uint32_t open[kMaxPickBins]; // 1: the bin holds a point and is binned; 0: its instances are dropped
+};
+
 struct SlabTable {
   uint32_t hist[kSlabBuckets];  // entries per 16-key bucket
   uint32_t klo[kMaxSlabs];      // slab s holds the keys [klo[s], khi[s])
@@ -239,14 +248,19 @@ struct SlabTable {
 // empty - after a drop of its domain (key change, or the bin table / slab state both domains share regrown) or, for a slab
 // kind, a change of its slab count - and replays it otherwise: a scene frame captures no bin graph of its own, and a views
 // frame invalidates no mono graph except through those shared buffers ----
+// Picks (gs_pick_scene) are a third domain with its own key: a pick of another size than the page's frames (a raycast's small
+// view) re-captures only the pick graphs, and the frames keep theirs.  Its sort stages (plain and scene) capture the same
+// launches as the frames' ----
 enum GraphId : int {
   kGraphSort, kGraphSortReuse, kGraphSortScene, kGraphBin, kGraphRaster, kGraphRasterPeer,
   kGraphSlabPlain, kGraphSlabScene = kGraphSlabPlain + 4,
   kGraphViewsFirst = kGraphSlabScene + 4,  // mono ids end, views ids begin
   kGraphViewsSort = kGraphViewsFirst, kGraphViewsBin, kGraphViewsRaster, kGraphSlabViews,
-  kGraphCount = kGraphSlabViews + 3
+  kGraphPickFirst = kGraphSlabViews + 3,  // views ids end, pick ids begin
+  kGraphPickSortPlain = kGraphPickFirst, kGraphPickSortScene, kGraphPickBin, kGraphPick,
+  kGraphCount
 };
-enum GraphDomain : int { kGraphsMono, kGraphsViews };
+enum GraphDomain : int { kGraphsMono, kGraphsViews, kGraphsPick, kGraphDomains };
 
 }  // namespace gs
 
@@ -336,6 +350,13 @@ struct gs_context {
   double *quirk_table = nullptr;   // parseInt quirk thresholds (device)
   int quirk_n = 0;
   gs::SortHeader *sort_hdr = nullptr;  // device: counters header of the last sort (for GS_RENDER_REUSE_SORT)
+  // ---- picks (gs_pick_scene), allocated by the first pick ----
+  uint64_t pick_cap = 0;               // instances pick_pay holds (follows cap_inst)
+  uint32_t *pick_pay = nullptr;        // [pick_cap] splat index of every binned instance, beside inst_rec
+  gs::PickInput *pick_in = nullptr;    // device
+  gs::PickInput *pick_in_host = nullptr;  // pinned staging
+  gs_pick *pick_out = nullptr;         // device [GS_MAX_PICKS]
+  gs_pick *pick_out_host = nullptr;    // pinned [GS_MAX_PICKS]
 
   // ---- pipeline slots (ticket % kSlots): frame k is rasterised while k+1 is binned, k+2 is sorted and k-1 is copied to
   // the host.  Three stages + the copy = four frames a caller can have outstanding; the GPU-side order of the stages is
@@ -384,6 +405,7 @@ struct gs_context {
     uint32_t n_splats = 0;                   // resident splats when the frame was submitted
     uint32_t n_sortable = 0;                 // splats the frame's sort considers (scene frames: in the entities' ranges)
     bool slab = false;                       // rendered by the front-to-back slab path
+    bool pick = false;                       // a pick (gs_pick_scene): bin and pick stages instead of binning and raster
     int n_slabs = 0;
     cudaEvent_t slab_ev[gs::kMaxSlabs][2] = {};  // raster of each slab (timing)
     cudaEvent_t ev[5]{};                     // stage boundaries (timing)
@@ -443,7 +465,7 @@ struct gs_context {
     uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr;
     uint32_t n_views = 0, view_size[gs::kMaxViews] = {}, pad2 = 0; const void *px = nullptr;
     const void *psh = nullptr; uint32_t sh_degree = 0, pad3 = 0;  // the projection's instantiation and SH table
-  } gkey[2];                                     // [GraphDomain] (kept apart: a views frame re-captures only its own graphs)
+  } gkey[gs::kGraphDomains];                     // [GraphDomain] (kept apart: a views frame or a pick re-captures only its own graphs)
 
   // ---- fused exchange: one shared allocation per rank = flag rows + a ring of 3 frames, opened by every peer ----
   void *peer_local = nullptr;            // our shared block
@@ -524,6 +546,16 @@ void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const
 // n_bins: bins of the frame (views frames: of every view, each record gathered from its view's projection)
 void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, cudaStream_t st);  // 3 .. 7 launches
 void launch_raster(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags, cudaStream_t st);
+// ---- picks (gs_pick_scene) ----
+// one-pass emission (records and payloads by splat) keeping only the instances of open bins (2 launches)
+void launch_emit_pick(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,
+                      cudaStream_t st);
+// launch_tile_radix whose final pass also stores every instance's splat index into pay (3 .. 7 launches)
+void launch_tile_radix_pick(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, uint32_t *pay, cudaStream_t st);
+// k_pick: one warp per point (scene: the slot's scene table, also filled when the pick takes the plain path of one entity
+// over the whole table)
+void launch_pick(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameBufs &b, const uint32_t *pay,
+                 const PickInput *in, gs_pick *out, cudaStream_t st);
 // views scene frames: one grid over every view's tiles (n_tiles: their sum), view v's frame at fp + v (flags: packed | depth)
 void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags, cudaStream_t st);
 void launch_peer_acquire(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);

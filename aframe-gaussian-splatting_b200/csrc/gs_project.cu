@@ -692,4 +692,20 @@ void launch_emit(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const
                bin_open, (const float4 *)b.proj_recx, (const uint32_t *)b.rectx, b.x_stride);
 }
 
+// Picks: the one-pass count (entries' records and payloads by splat) and emission, with bin_open dropping every instance of
+// a bin that holds no query point (emit_candidate).  k_count<false> reads no bin table, so the open bins act in the emission
+// only: the candidates are counted and written as in a frame, and the bin sort drops the closed ones.
+void launch_emit_pick(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, const uint32_t *bin_open,
+                      cudaStream_t st) {
+  uint64_t tiles = ((uint64_t)c->cap + kEmitTile - 1) / kEmitTile;
+  const uint64_t cap = (uint64_t)c->sm_count * 8;
+  if (tiles > cap) tiles = cap;
+  if (tiles < 1) tiles = 1;
+  launch_chain(c, k_count<false>, (int)tiles, kEmitThreads, st, (const uint32_t *)b.order, (const uint32_t *)b.rect, c->ent,
+               c->ent_off, c->slice_total, c->slice_prefix, ctr, fp, (const uint32_t *)nullptr, (uint32_t *)nullptr, 0u);
+  launch_chain(c, k_emit_entries<false>, (int)tiles, 256, st, (const uint2 *)c->ent, (const uint32_t *)c->ent_off,
+               (const uint32_t *)c->slice_prefix, (const float4 *)b.proj_rec, fp, (uint64_t)c->cap_inst, c->inst_tile, c->inst_idx,
+               ctr, bin_open, (const float4 *)nullptr, (const uint32_t *)nullptr, 0u);
+}
+
 }  // namespace gs

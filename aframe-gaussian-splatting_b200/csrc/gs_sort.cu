@@ -763,6 +763,36 @@ struct T2S : T2 {
   }
 };
 
+// Picks (gs_pick_scene): the final pass also keeps each instance's payload - the splat index of a one-pass frame, whose
+// records are indexed by splat - in pay, beside inst_rec.  Pick-only pass types, so T1 / T2 keep their code.
+struct T1P : T1 {
+  uint32_t *pay_out;
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const {
+    if (last) { gather_record(proj_rec, inst_rec, pay, pos); pay_out[pos] = pay; }
+    else { idx_out[pos] = pay; bin_out[pos] = (uint16_t)carry; }
+  }
+};
+struct T2P : T2 {
+  uint32_t *pay_out;
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const {
+    gather_record(proj_rec, inst_rec, pay, pos);
+    pay_out[pos] = pay;
+    bin_out[pos] = (uint16_t)carry;
+  }
+};
+
+void launch_tile_radix_pick(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, uint32_t *pay, cudaStream_t st) {
+  const RadixScratch s{c->table_d, c->totals + 256, c->table_d_stride};
+  const bool last = n_bins <= 256u;
+  const T1 t1{{}, ctr, c->inst_tile, c->inst_idx, c->inst_tile_b, c->inst_idx_b, b.proj_rec, b.inst_rec, b.bin_range, n_bins, last};
+  run_pass(c, T1P{t1, pay}, s, c->cap_inst, st);
+  if (last) return;
+  const T2 t2{{}, ctr, c->inst_tile_b, c->inst_idx_b, b.proj_rec, b.inst_rec, c->inst_tile_f};
+  run_pass(c, T2P{t2, pay}, s, c->cap_inst, st);
+  launch_chain(c, k_tile_ranges, persistent_grid(c, c->cap_inst, 256 * 8, 8), 256, st, (const uint16_t *)c->inst_tile_f, ctr,
+               b.bin_range);
+}
+
 // 3 launches up to 256 bins, else 7 (T2 and k_tile_ranges)
 void launch_tile_radix(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, cudaStream_t st) {
   const RadixScratch s{c->table_d, c->totals + 256, c->table_d_stride};

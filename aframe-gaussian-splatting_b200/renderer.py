@@ -258,6 +258,24 @@ class SplatContext:
                                                     C.c_void_p(out_ptr), C.byref(t)))
         return t.value
 
+    def pick_scene(self, frame: FrameInputs, objects: Sequence[SceneObject], points, depth_in: Optional[np.ndarray] = None,
+                   depth_device: bool = False):
+        """gs_pick_scene: for each pixel (x, y) of `points` ((n, 2), row 0 = bottom) of the scene frame render_scene draws
+        with these arguments, the splat where the pixel turns half opaque.  Returns (splat u32, object i32, depth f32,
+        alpha f32) arrays of n entries: GS_PICK_NONE / -1 / 1 where the pixel never does.  depth_in as render_scene, or a
+        device pointer (int) with depth_device=True."""
+        xy = np.ascontiguousarray(points, dtype=np.uint32).reshape(-1, 2)
+        p = self.make_params(frame, depth_in=None if depth_device else depth_in)
+        if depth_device:
+            p.depth_in = int(depth_in)
+            p.flags |= _lib.GS_RENDER_DEPTH_DEVICE
+        out = (_lib.GsPick * max(1, len(xy)))()
+        self._check(self._lib.gs_pick_scene(self._h, C.byref(p), make_objects(objects), len(objects),
+                                            xy.ctypes.data_as(C.POINTER(C.c_uint32)), len(xy), out))
+        res = np.ctypeslib.as_array(out)[: len(xy)]
+        return (res["splat"].astype(np.uint32), res["object"].astype(np.int32), res["depth"].astype(np.float32),
+                res["alpha"].astype(np.float32))
+
     def sort_scene(self, objects: Sequence[SceneObject]) -> np.ndarray:
         """gs_sort_scene: each entity's sortedIndexes (index.js:507-570 on its own range) + first, concatenated in
         the order given."""

@@ -15,7 +15,7 @@ class Splats : public Napi::ObjectWrap<Splats> {
       InstanceMethod("sort", &Splats::Sort),   InstanceMethod("render", &Splats::Render),
       InstanceMethod("renderScene", &Splats::RenderScene), InstanceMethod("insert", &Splats::Insert),
       InstanceMethod("insertPly", &Splats::InsertPly), InstanceMethod("erase", &Splats::Erase),
-      InstanceMethod("renderSceneXR", &Splats::RenderSceneXR)}));
+      InstanceMethod("renderSceneXR", &Splats::RenderSceneXR), InstanceMethod("pickScene", &Splats::PickScene)}));
     // the RGBA8 target's per-fragment rounding: frame objects take `blendUnorm8: true` (GS_RENDER_BLEND_UNORM8)
     exports.Set("BLEND_UNORM8", Napi::Number::New(env, GS_RENDER_BLEND_UNORM8));
     return exports;
@@ -125,6 +125,55 @@ class Splats : public Napi::ObjectWrap<Splats> {
     const void* color = i[2].IsUndefined() ? nullptr : i[2].As<Napi::Uint8Array>().Data();
     Check(i.Env(), gs_render_scene(ctx_, &p, objs.data(), (uint32_t)objs.size(), color, i[3].As<Napi::Uint8Array>().Data(), nullptr));
     return i.Env().Undefined();
+  }
+  // pickScene({proj, width, height, focal, depth?: Float32Array}, [{first, count, modelview, cutout?}, ...], Uint32Array xy)
+  //   -> {splat: Uint32Array, object: Int32Array, depth: Float32Array, alpha: Float32Array}   <- what a cursor, gaze or
+  // controller ray meets on a splat entity (A-Frame's raycaster only sees each entity's dummy quad): for each (x, y) pixel of
+  // xy (row 0 = bottom) of the frame renderScene draws with these arguments, the splat where the pixel turns half opaque
+  // (splat 0xFFFFFFFF = GS_PICK_NONE and object -1 where none does), its entity's index in the list, its window depth and
+  // the pixel's alpha.  At most GS_MAX_PICKS points per call; synchronous, like renderScene.
+  Napi::Value PickScene(const Napi::CallbackInfo& i) {
+    auto o = i[0].As<Napi::Object>();
+    gs_render_params p{};
+    memcpy(p.proj, o.Get("proj").As<Napi::Float32Array>().Data(), 64);
+    p.width = o.Get("width").As<Napi::Number>().Uint32Value();
+    p.height = o.Get("height").As<Napi::Number>().Uint32Value();
+    p.focal = o.Get("focal").As<Napi::Number>().FloatValue();
+    if (o.Has("depth")) p.depth_in = o.Get("depth").As<Napi::Float32Array>().Data();
+    p.out_format = GS_FORMAT_RGBA8;
+    auto list = i[1].As<Napi::Array>();
+    std::vector<gs_object> objs(list.Length());
+    for (uint32_t k = 0; k < list.Length(); ++k) {
+      auto e = list.Get(k).As<Napi::Object>();
+      gs_object& g = objs[k];
+      g = gs_object{};
+      g.first = e.Get("first").As<Napi::Number>().Uint32Value();
+      g.count = e.Get("count").As<Napi::Number>().Uint32Value();
+      memcpy(g.modelview, e.Get("modelview").As<Napi::Float32Array>().Data(), 64);
+      if (e.Has("cutout")) { g.has_cutout = 1; memcpy(g.cutout16, e.Get("cutout").As<Napi::Float32Array>().Data(), 64); }
+    }
+    auto xy = i[2].As<Napi::Uint32Array>();
+    const uint32_t n = (uint32_t)(xy.ElementLength() / 2);
+    std::vector<gs_pick> hits(n ? n : 1);
+    Napi::Env env = i.Env();
+    Check(env, gs_pick_scene(ctx_, &p, objs.data(), (uint32_t)objs.size(), xy.Data(), n, hits.data()));
+    if (env.IsExceptionPending()) return env.Undefined();
+    auto splat = Napi::Uint32Array::New(env, n);
+    auto object = Napi::Int32Array::New(env, n);
+    auto depth = Napi::Float32Array::New(env, n);
+    auto alpha = Napi::Float32Array::New(env, n);
+    for (uint32_t k = 0; k < n; ++k) {
+      splat[k] = hits[k].splat;
+      object[k] = hits[k].object;
+      depth[k] = hits[k].depth;
+      alpha[k] = hits[k].alpha;
+    }
+    auto r = Napi::Object::New(env);
+    r.Set("splat", splat);
+    r.Set("object", object);
+    r.Set("depth", depth);
+    r.Set("alpha", alpha);
+    return r;
   }
   // renderSceneXR([eyeL, eyeR] {proj, width, height, focal, x, y, blendUnorm8?}, [{first, count, modelview, cutout?,
   //                eyeModelviews: [Float32Array, Float32Array]}, ...], layer {color: Uint8Array, depth?: Float32Array, pitch,

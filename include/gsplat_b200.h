@@ -508,6 +508,47 @@ GS_API int gs_render_scene_views_target(gs_context *ctx, const gs_render_params 
                                         const gs_object *objs, const float *view_modelviews, uint32_t n_objs,
                                         const gs_target *layer, const uint32_t *view_xy, gs_stats *stats);
 
+/*
+ * Picking: which splat a pointer, gaze cursor or controller ray meets.  A splat entity's mesh is one dummy quad
+ * (index.js:52-66, 197-198), so A-Frame's raycaster never hits splats; the answer has to come from the same sort,
+ * projection, binning and blend that drew the pixel.
+ *
+ * A pick of pixel (x, y) (row 0 = bottom) of a scene frame takes the arguments of gs_render_scene and walks that pixel's
+ * blended pairs nearest first, exactly as the default raster does: the same fp32 r^2, r^2 <= 4, the LEQUAL depth test
+ * against depth_in, w = ex2(r^2 * -log2 e) * a * T, T = fma(w, -1, T), and the stop once T < 3e-4.  It returns
+ *   splat: the table index of the first pair after whose blend T falls below 0.5 (the pixel's median surface), or
+ *          GS_PICK_NONE when T never does.  A hit on a quirk-Q5 repeat reports what is drawn there: the entity's first splat;
+ *   object: the index into objs of that splat's entity, or -1;
+ *   depth: the window depth z/w * 0.5 + 0.5 of the hit splat's quad, as the depth test compares it; 1 with no hit;
+ *   alpha: 1 - T where the walk ends: bit-equal to the A channel of the GS_FORMAT_RGBA32F gs_render_scene frame of the same
+ *          arguments with bg_rgba alpha 0 and no colour target.
+ * Entities are drawn whole in objs order and never interleave by depth (see the scene rules above): a later entity covers
+ * an earlier one whatever their depths, so the pick reports the entity that is visible, not the nearer one.
+ *
+ * gs_pick_scene: n_points (x, y) pairs in xy (host), results in out (host, n_points entries), in the order of xy.
+ *   - From frame it reads projection, width, height, focal, depth_in and GS_RENDER_DEPTH_DEVICE; objs as gs_render_scene.
+ *   - Synchronous: it runs in the four pipeline slots like a scene frame, waits only for the frame whose slot it takes (as
+ *     a fifth gs_render_scene_async would) and returns when out is filled.  It is always one-pass, whatever GS_SLAB_MIN
+ *     says (the slab path draws the same bytes), and leaves no order for GS_RENDER_REUSE_SORT.  Frames submitted before or
+ *     after it are unchanged by it.  An instance-buffer overflow is re-run as a frame's is.
+ *   - Only the instances of the bins holding a query point are sorted and gathered; the bin-instance candidates of the
+ *     whole frame are counted, so a pick needs the instance buffers of the one-pass frame (82 B per candidate), also on
+ *     a context whose frames take the slab path, and returns GS_ERR_CAPACITY where that frame would.
+ *   - GS_ERR_INVALID, changing nothing, for: n_points 0 or above GS_MAX_PICKS, a point outside the frame, any flag other than
+ *     GS_RENDER_DEPTH_DEVICE, a sharded context (gs_set_shard world > 1), and whatever gs_render_scene refuses.  An empty
+ *     table returns GS_ERR_EMPTY.
+ */
+typedef struct gs_pick {
+  uint32_t splat;  /* table index of the hit splat, or GS_PICK_NONE */
+  int32_t object;  /* index into objs of its entity, or -1          */
+  float depth;     /* window depth of the hit splat's quad, or 1    */
+  float alpha;     /* 1 - T at the end of the pixel's walk          */
+} gs_pick;
+#define GS_PICK_NONE 0xFFFFFFFFu
+#define GS_MAX_PICKS 4096
+GS_API int gs_pick_scene(gs_context *ctx, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
+                         const uint32_t *xy, uint32_t n_points, gs_pick *out);
+
 /* Per-splat projected record of the last gs_render (testing the vertex-shader restatement):
  * 8 floats per resident splat {cx, cy, a1x, a1y, a2x, a2y, rgba8-as-bits, tile-rect-as-bits};
  * rect == 0xFFFFFFFF marks a splat that was not projected/visible. */
