@@ -16,6 +16,7 @@ GS_RENDER_BLEND_UNORM8 = 128
 GS_MAX_OBJECTS = 64
 GS_MAX_VIEWS = 4
 GS_TARGET_DEVICE = 1
+GS_TARGET_DEPTH_WRITE = 2
 
 
 class GsStats(C.Structure):

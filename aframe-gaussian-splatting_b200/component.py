@@ -463,14 +463,19 @@ class SplatScene:
 
     def render_into(self, color: np.ndarray, depth: Optional[np.ndarray] = None, viewport=(0, 0), width: Optional[int] = None,
                     height: Optional[int] = None, camera=None, fmt: int = GS_FORMAT_RGBA8,
-                    blend_unorm8: bool = False) -> np.ndarray:
+                    blend_unorm8: bool = False, write_depth: bool = False) -> np.ndarray:
         """Draw every entity IN PLACE into the caller's framebuffer at a viewport rectangle, as the reference's draw does
         with the bound render target and renderer.setViewport (index.js:177-195).  color: (rows, pitch, 4) of the output
         dtype, row 0 = bottom; depth: (rows, pitch) f32 window-space depth or None.  viewport = (x, y) or (x, y, w, h) in
         CSS pixels: w x h (default: width x height, else the rest of the buffer) scaled by the first entity's pixelRatio
-        and floored, as render() sizes its frame.  blend_unorm8 as render().  Returns `color`."""
+        and floored, as render() sizes its frame.  blend_unorm8 as render().  numpy buffers are host memory, torch CUDA
+        tensors on the context's GPU device memory (the draw first waits for the caller's current torch stream, and is
+        finished when it returns).  write_depth: each pixel that turns half opaque also leaves its splat depth (the median surface)
+        in `depth`, for what the page draws after the splats.  Returns `color`."""
         if not self.entities:
             raise ValueError("SplatScene.render_into: no entity added")
+        if write_depth and depth is None:
+            raise ValueError("SplatScene.render_into: write_depth needs a depth buffer")
         x, y = int(viewport[0]), int(viewport[1])
         if len(viewport) == 4:
             width, height = viewport[2], viewport[3]
@@ -478,7 +483,7 @@ class SplatScene:
         height = color.shape[0] - y if height is None else height
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene_target(frame, objs, color, depth, viewport=(x, y), fmt=fmt,
-                                                 blend_unorm8=blend_unorm8)
+                                                 blend_unorm8=blend_unorm8, write_depth=write_depth)
 
     def _xr_ratio(self) -> float:
         """The first entity's xrPixelRatio, 1 when it is not positive (the rule of render_xr)."""
@@ -506,16 +511,20 @@ class SplatScene:
         return objs, views, view_mvs
 
     def render_xr_views(self, view_cameras, viewports, width: int, height: int, color: np.ndarray,
-                        depth: Optional[np.ndarray] = None, fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False) -> np.ndarray:
+                        depth: Optional[np.ndarray] = None, fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False,
+                        write_depth: bool = False) -> np.ndarray:
         """WebXR presentation of every view of the viewer pose (1..4: two eyes plus an observer, or a quad-view device's
         four) into the XR layer's one framebuffer, IN PLACE, from one head sort (gs_render_scene_views_target).
         viewports[v] = (x, y, w, h): view v's native rectangle, as XRWebGLLayer.getViewport(view) gives it, in a layer of
         width x height native pixels.  Every component is scaled by the first entity's xrPixelRatio and floored
         (xr_viewports), as render_xr_layer sizes its eyes; two side-by-side viewports reproduce render_xr_layer.
         color: (rows, pitch, 4) of the output dtype holding the scaled layer; depth: (rows, pitch) f32 or None.
-        blend_unorm8 as render().  Returns `color`."""
+        blend_unorm8, write_depth and the buffers as render_into (write_depth: the layer depth the compositor receives
+        holds the splats).  Returns `color`."""
         if not self.entities:
             raise ValueError("SplatScene.render_xr_views: no entity added")
+        if write_depth and depth is None:
+            raise ValueError("SplatScene.render_xr_views: write_depth needs a depth buffer")
         if len(view_cameras) != len(viewports):
             raise ValueError("render_xr_views: one viewport per view camera")
         ratio = self._xr_ratio()
@@ -526,22 +535,24 @@ class SplatScene:
         objs, views, view_mvs = self._xr_view_objects(view_cameras, [(w, h) for _, _, w, h in rects])
         xy = [c for x, y, _, _ in rects for c in (x, y)]
         return self.renderer.render_scene_views_target(views, objs, view_mvs, color, xy, depth, fmt=fmt,
-                                                       blend_unorm8=blend_unorm8)
+                                                       blend_unorm8=blend_unorm8, write_depth=write_depth)
 
     def render_xr_layer(self, eye_cameras, width: int, height: int, color: np.ndarray, depth: Optional[np.ndarray] = None,
-                        fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False) -> np.ndarray:
+                        fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False, write_depth: bool = False) -> np.ndarray:
         """WebXR presentation into the XR layer's one framebuffer, IN PLACE: both eyes side by side over one depth buffer,
         as three.js draws each eye camera of the session at its own viewport of the layer.  Eye size as render_xr (the
         native eye size scaled by the first entity's xrPixelRatio, floored): the left eye at (0, 0), the right at (w, 0).
         color: (rows, pitch, 4) of the output dtype with pitch >= 2w and rows >= h; depth: (rows, pitch) f32 or None.
-        blend_unorm8 as render().  Returns `color`."""
+        blend_unorm8, write_depth and the buffers as render_into.  Returns `color`."""
         if not self.entities:
             raise ValueError("SplatScene.render_xr_layer: no entity added")
+        if write_depth and depth is None:
+            raise ValueError("SplatScene.render_xr_layer: write_depth needs a depth buffer")
         (w, h), objs, eyes, eye_mvs = self._xr_objects(eye_cameras, width, height)
         if color.shape[1] < 2 * w or color.shape[0] < h:
             raise ValueError(f"render_xr_layer: the layer must hold two {w} x {h} eyes side by side")
         return self.renderer.render_scene_stereo_target(eyes, objs, eye_mvs, color, depth, eye_xy=(0, 0, w, 0), fmt=fmt,
-                                                        blend_unorm8=blend_unorm8)
+                                                        blend_unorm8=blend_unorm8, write_depth=write_depth)
 
     def render_xr(self, eye_cameras, width: int, height: int, color_in=(None, None), depth_in=(None, None),
                   bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):

@@ -248,7 +248,7 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles) {
     // graph key stays put (and the other way round)
     drop_graphs(c, kGraphsMono);
     drop_graphs(c, kGraphsViews);
-    dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open);
+    dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open); dev_free(c->pix_depth);
     GS_CUDA(c, dev_alloc(&c->pix_state, (size_t)n_tiles * 256));
     GS_CUDA(c, dev_alloc(&c->tile_closed, (size_t)n_tiles));
     // sized by tiles, not by this frame's bins: bins never outnumber tiles, but a later frame of another shape can have
@@ -263,18 +263,21 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles) {
 // is idle).  A views frame (n_views views; every other frame: 1) bins every view's bins and keeps slab state for every
 // view's tiles; the tile statistics are view 0's.
 struct FrameNeeds {
-  bool slab, scene;
+  bool slab, scene, depth_write;
   uint32_t n_views, n_bins_all, n_tiles, n_tiles_all;
 };
 static bool frame_bufs_ready(const gs_context *c, const FrameNeeds &f) {
   return scratch_ready(c) && bins_ready(c, f.n_bins_all) && tile_stats_ready(c, f.n_tiles) &&
-         (!f.slab || slab_ready(c, f.n_tiles_all)) && (!f.scene || scene_bufs_ready(c)) && stereo_bufs_ready(c, f.n_views) &&
-         c->cap_inst != 0;
+         (!f.slab || slab_ready(c, f.n_tiles_all)) && (!f.slab || !f.depth_write || c->pix_depth) &&
+         (!f.scene || scene_bufs_ready(c)) && stereo_bufs_ready(c, f.n_views) && c->cap_inst != 0;
 }
 static int ensure_frame_bufs(gs_context *c, const FrameNeeds &f) {
   int rc;
   if ((rc = ensure_scratch(c)) || (rc = ensure_bins(c, f.n_bins_all)) || (rc = ensure_tile_stats(c, f.n_tiles))) return rc;
   if (f.slab && (rc = ensure_slab(c, f.n_tiles_all))) return rc;
+  // the slab loop of a GS_TARGET_DEPTH_WRITE frame carries each pixel's crossing depth beside pix_state (no graph can bake it
+  // before it exists, and ensure_slab frees it only together with pix_state, dropping the graphs)
+  if (f.slab && f.depth_write && !c->pix_depth) GS_CUDA(c, dev_alloc(&c->pix_depth, (size_t)c->slab_tiles_cap * 256));
   if (f.scene && (rc = ensure_scene_bufs(c))) return rc;
   if ((rc = ensure_stereo_bufs(c, f.n_views))) return rc;
   if (c->cap_inst == 0) {
@@ -463,7 +466,7 @@ extern "C" int gs_destroy(gs_context *c) {
   dev_free(c->slice_prefix); dev_free(c->ent); dev_free(c->ent_off);
   dev_free(c->key32[0]); dev_free(c->key32[1]); dev_free(c->cidx); dev_free(c->ckey); dev_free(c->chunk_cnt[0]); dev_free(c->chunk_cnt[1]);
   dev_free(c->slab_tab[0]); dev_free(c->slab_tab[1]);
-  dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open);
+  dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open); dev_free(c->pix_depth);
   dev_free(c->scene_key); dev_free(c->scene_pay); dev_free(c->scene_hi);
   dev_free(c->pick_pay); dev_free(c->pick_in); dev_free(c->pick_out);
   if (c->pick_in_host) cudaFreeHost(c->pick_in_host);
@@ -1126,7 +1129,8 @@ static cudaGraphExec_t &stage_graph(gs_context::Slot &sl, FrameStage stage, bool
                              : (stage == kBinStage ? kGraphPickBin : kGraphPick);
   } else if (sl.slab) {
     id = slab_graph_base(sl);
-    if (stage != kSortStage) id += sl.peer ? 3 : ((sl.raster_flags & 2u) ? 2 : 1);  // loop: plain, depth-tested, fused peer exchange
+    // loop: plain, depth-tested, fused peer exchange, depth-tested with depth write (views: no peer id, depth write at 3)
+    if (stage != kSortStage) id += sl.depth_write ? (sl.stereo ? 3 : 4) : (sl.peer ? 3 : ((sl.raster_flags & 2u) ? 2 : 1));
   } else if (sl.stereo) {
     id = kGraphViewsSort + (int)stage;
   } else if (stage == kSortStage) {
@@ -1227,14 +1231,14 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
     launch_emit(c, fp, sl.ctr, b, c->bin_open, st);
     launch_tile_radix(c, sl.ctr, b, n_bins, st);
     if ((e = record(sl.slab_ev[s][0], st, external_events))) return e;
-    launch_raster_slab(c, fp, sl.ctr, n_tiles, b, (sl.raster_flags & 2u) != 0, sl.stereo, st);
+    launch_raster_slab(c, fp, sl.ctr, n_tiles, b, (sl.raster_flags & 2u) != 0, sl.stereo, sl.depth_write, st);
     if ((e = record(sl.slab_ev[s][1], st, external_events))) return e;
   }
   launch_slab_end(c, sl.ctr, st);
   if ((e = record(sl.ev[3], st, external_events))) return e;
   if (sl.peer) launch_peer_acquire(c, sl.fp, sl.ctr, st);
   if ((e = record(sl.ev_r0, st, external_events))) return e;
-  launch_resolve(c, fp, n_tiles, sl.stereo, st);
+  launch_resolve(c, fp, n_tiles, sl.stereo, sl.depth_write, st);
   if ((e = record(sl.ev[4], st, external_events))) return e;
   if (sl.peer) launch_peer_signal_wait(c, sl.fp, sl.ctr, st);
   return cudaGetLastError();
@@ -1250,7 +1254,7 @@ static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_ti
   int n_slabs = 1;
   while (n_slabs < kMaxSlabs && slab_cumulative(c->slab_first, n_slabs) < sl.n_sortable) ++n_slabs;
   if (n_slabs != sl.graph_slabs[set][kind]) {  // the captured stages bake the slab count
-    const int base = slab_graph_base(sl), n_ids = sl.stereo ? 3 : 4;  // this set's and kind's keys graph and loop graphs
+    const int base = slab_graph_base(sl), n_ids = sl.stereo ? 4 : 5;  // this set's and kind's keys graph and loop graphs
     for (int id = base; id < base + n_ids; ++id) kill_graph(sl.graph[set][id]);
     sl.graph_slabs[set][kind] = n_slabs;
   }
@@ -1296,6 +1300,11 @@ static int enqueue_readback(gs_context *c, gs_context::Slot &sl) {
         char *dst = (char *)sl.tcolor + ((size_t)sl.torg[e][1] * sl.tpitch + sl.torg[e][0]) * px_bytes;
         GS_CUDA(c, cudaMemcpy2DAsync(dst, px_bytes * sl.tpitch, sl.frame_src[e], row, row, vp.height,
                                      cudaMemcpyDeviceToHost, c->copy_stream));
+        if (sl.depth_write) {  // and the depth the frame wrote into its staged rectangle
+          float *ddst = const_cast<float *>(sl.tdepth) + (size_t)sl.torg[e][1] * sl.tpitch + sl.torg[e][0];
+          GS_CUDA(c, cudaMemcpy2DAsync(ddst, sizeof(float) * sl.tpitch, sl.depth_dev[e], sizeof(float) * vp.width,
+                                       sizeof(float) * vp.width, vp.height, cudaMemcpyDeviceToHost, c->copy_stream));
+        }
       } else {
         GS_CUDA(c, cudaMemcpyAsync(sl.out_user[e], sl.frame_src[e], sl.out_bytes[e], cudaMemcpyDeviceToHost, c->copy_stream));
       }
@@ -1388,6 +1397,9 @@ static int stage_inputs(gs_context *c, gs_context::Slot &sl, int e, const gs_ren
       fp.out = (char *)sl.tcolor + origin * px_bytes;
       fp.color_in = fp.out;
       fp.depth_in = sl.tdepth ? sl.tdepth + origin : nullptr;
+      // GS_TARGET_DEPTH_WRITE: the depth is written where it is read (gs_target::depth is const for the frames that only
+      // test against it)
+      if (sl.depth_write) fp.depth_out = const_cast<float *>(sl.tdepth) + origin;
       fp.rc.pitch = sl.tpitch;
       return GS_OK;
     }
@@ -1404,6 +1416,7 @@ static int stage_inputs(gs_context *c, gs_context::Slot &sl, int e, const gs_ren
                                      sizeof(float) * sl.tpitch, sizeof(float) * p->width, p->height, cudaMemcpyHostToDevice,
                                      c->stream));
       fp.depth_in = sl.depth_dev[e];
+      if (sl.depth_write) fp.depth_out = (float *)sl.depth_dev[e];  // written in the staging copy, read back with the colour
     }
     return GS_OK;
   }
@@ -1480,7 +1493,8 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   // frames always take the two-pixel loop of that mode (bit 3), whatever GS_RASTER says
   const bool depth = p->depth_in || (sl.target && sl.tdepth);  // a target's depth is that of every view
   const bool blend8 = (p->flags & GS_RENDER_BLEND_UNORM8) != 0;
-  sl.raster_flags = (blend8 ? 9u : c->raster_base_flags) | (depth ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u);
+  sl.raster_flags = (blend8 ? 9u : c->raster_base_flags) | (depth ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u) |
+                    (sl.depth_write ? 16u : 0u);
   // a views frame bins every view (ids bin_base[v] + bin) and rasters every view's tiles in one grid, on either path
   uint32_t n_tiles_all = rc.n_tiles, n_bins_all = rc.n_bins;
   if (sl.stereo) {
@@ -1684,13 +1698,16 @@ static bool rects_overlap(uint32_t ax, uint32_t ay, uint32_t aw, uint32_t ah, ui
 
 // Successive frames into one target compose in submission order, like successive GL draws: a target frame first waits
 // (oldest first) for every pending target frame on the same colour buffer whose rectangles meet its own (view a's:
-// views[a].width x views[a].height).  Stream order alone is not enough: gs_wait may still re-run such a frame, and a host
-// target's rectangle is read at submission.
+// views[a].width x views[a].height), and, when either frame writes depth (GS_TARGET_DEPTH_WRITE), for one on the same
+// depth buffer.  Stream order alone is not enough: gs_wait may still re-run such a frame, and a host target's rectangle is
+// read at submission.
 static int wait_overlapping(gs_context *c, const TargetInput &t, const gs_render_params *views, uint32_t n_views) {
+  const bool dw = (t.t->flags & GS_TARGET_DEPTH_WRITE) != 0;
   for (;;) {
     gs_context::Slot *hit = nullptr;
     for (auto &o : c->slot) {
-      if (!o.pending || !o.target || o.tcolor != t.t->color || (hit && o.ticket > hit->ticket)) continue;
+      const bool shared = o.tcolor == t.t->color || ((dw || o.depth_write) && t.t->depth && o.tdepth == t.t->depth);
+      if (!o.pending || !o.target || !shared || (hit && o.ticket > hit->ticket)) continue;
       bool meet = false;
       for (uint32_t a = 0; a < n_views; ++a)
         for (uint32_t b = 0; b < o.n_views; ++b)
@@ -1730,6 +1747,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   FrameNeeds need{};
   need.scene = scene != nullptr;
   need.n_views = stereo ? stereo->n : 1u;
+  need.depth_write = target && (target->t->flags & GS_TARGET_DEPTH_WRITE);
   for (uint32_t v = 0; v < need.n_views; ++v) {
     const gs_render_params &q = stereo ? stereo->views[v] : *p;
     RenderConsts grid;
@@ -1782,6 +1800,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   sl.color_in[0] = color_in;
   sl.color_device = (p->flags & GS_RENDER_COLOR_DEVICE) != 0;
   sl.target = target != nullptr;
+  sl.depth_write = need.depth_write;
   sl.restage = true;
   if (target) {
     sl.target_device = (target->t->flags & GS_TARGET_DEVICE) != 0;
@@ -1854,7 +1873,12 @@ extern "C" int gs_render_scene_async(gs_context *c, const gs_render_params *fram
 // and gs_render_scene_stereo are checked after these, also before anything is changed)
 static int check_target(gs_context *c, const gs_render_params *p, const gs_target *t, uint32_t x, uint32_t y) {
   if (!t || !t->color) return fail(c, GS_ERR_INVALID, "target frame: no target or no colour buffer");
-  if (t->flags & ~(uint32_t)GS_TARGET_DEVICE) return fail(c, GS_ERR_INVALID, "target frame: unknown gs_target flags");
+  if (t->flags & ~(uint32_t)(GS_TARGET_DEVICE | GS_TARGET_DEPTH_WRITE))
+    return fail(c, GS_ERR_INVALID, "target frame: unknown gs_target flags");
+  if ((t->flags & GS_TARGET_DEPTH_WRITE) && !t->depth)
+    return fail(c, GS_ERR_INVALID, "target frame: GS_TARGET_DEPTH_WRITE needs a depth buffer");
+  if ((t->flags & GS_TARGET_DEPTH_WRITE) && (p->flags & GS_RENDER_BLEND_UNORM8))
+    return fail(c, GS_ERR_INVALID, "target frame: GS_TARGET_DEPTH_WRITE is not accepted with GS_RENDER_BLEND_UNORM8");
   if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "target frame: not on a sharded context");
   if (p->depth_in) return fail(c, GS_ERR_INVALID, "target frame: depth_in must be NULL (the depth is the target's)");
   if (p->flags & (GS_RENDER_OUT_DEVICE | GS_RENDER_COLOR_DEVICE | GS_RENDER_DEPTH_DEVICE | GS_RENDER_OUT_TILED |
@@ -1963,6 +1987,7 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   sl.color_in[0] = nullptr;
   sl.color_device = false;
   sl.target = false;
+  sl.depth_write = false;
   sl.restage = true;
   if (c->sh_degree && !sl.sh_cam_dev) {
     GS_CUDA(c, cudaMalloc((void **)&sl.sh_cam_dev, sizeof(float4) * kMaxObjects * kMaxViews));

@@ -116,7 +116,13 @@ struct FrameParams {
   // ---- fused raster + exchange over NVLink peer memory (GS_RENDER_OUT_PEER) ----
   uint32_t n_peer;                       // 0: plain output; else every finished tile is stored into all ranks' frames
   uint32_t peer_rank;
-  void *peer_out[kMaxPeers];             // this frame's slot in every rank's shared frame ring (own rank included)
+  union {
+    void *peer_out[kMaxPeers];           // this frame's slot in every rank's shared frame ring (own rank included)
+    // GS_TARGET_DEPTH_WRITE frames (rows of rc.pitch, like depth_in; NULL otherwise): where each pixel that turns half
+    // opaque stores the window depth of the pair that made it so.  Such a frame is a target frame, which never exchanges
+    // (targets refuse sharded contexts), so it shares peer_out's room and FrameParams keeps its size and layout
+    float *depth_out;
+  };
   unsigned long long *peer_done[kMaxPeers];      // rank r's done[slot][*] flag row (we write [.][peer_rank])
   unsigned long long *peer_released[kMaxPeers];  // rank r's released[slot][*] flag row
   unsigned long long *local_done;        // our done[slot][*]
@@ -242,8 +248,8 @@ struct SlabTable {
 
 // ---- the stage graphs a slot caches per buffer set (gs_context::Slot::graph).  Two domains, each dropped as a whole when
 // its own gs_context::GraphKey changes: mono (plain and scene frames, which share their bin and raster graphs) and views.
-// The four (views: three) ids of a slab kind are its keys stage and its slab loop without depth test, depth-tested and with
-// the fused peer exchange (views frames are never peer frames).
+// The five (views: four) ids of a slab kind are its keys stage and its slab loop without depth test, depth-tested, with
+// the fused peer exchange (views frames are never peer frames) and depth-tested with GS_TARGET_DEPTH_WRITE.
 // Invariant: an id stands for exactly one captured launch sequence.  A frame captures its stage's id only when that id is
 // empty - after a drop of its domain (key change, or the bin table / slab state both domains share regrown) or, for a slab
 // kind, a change of its slab count - and replays it otherwise: a scene frame captures no bin graph of its own, and a views
@@ -253,10 +259,10 @@ struct SlabTable {
 // launches as the frames' ----
 enum GraphId : int {
   kGraphSort, kGraphSortReuse, kGraphSortScene, kGraphBin, kGraphRaster, kGraphRasterPeer,
-  kGraphSlabPlain, kGraphSlabScene = kGraphSlabPlain + 4,
-  kGraphViewsFirst = kGraphSlabScene + 4,  // mono ids end, views ids begin
+  kGraphSlabPlain, kGraphSlabScene = kGraphSlabPlain + 5,
+  kGraphViewsFirst = kGraphSlabScene + 5,  // mono ids end, views ids begin
   kGraphViewsSort = kGraphViewsFirst, kGraphViewsBin, kGraphViewsRaster, kGraphSlabViews,
-  kGraphPickFirst = kGraphSlabViews + 3,  // views ids end, pick ids begin
+  kGraphPickFirst = kGraphSlabViews + 4,  // views ids end, pick ids begin
   kGraphPickSortPlain = kGraphPickFirst, kGraphPickSortScene, kGraphPickBin, kGraphPick,
   kGraphCount
 };
@@ -326,6 +332,8 @@ struct gs_context {
   uint32_t chunk_row = 0;          // row stride of chunk_cnt: cap / 2048 + 4
   gs::SlabTable *slab_tab[2] = {nullptr, nullptr};
   float4 *pix_state = nullptr;     // [tiles * 256] {R, G, B, T} carried from slab to slab (views frames: every view's tiles)
+  float *pix_depth = nullptr;      // [slab_tiles_cap * 256] GS_TARGET_DEPTH_WRITE frames: window depth of the pair after which
+                                   // the pixel's T fell below 0.5, layout of pix_state (allocated by the first such slab frame)
   uint8_t *tile_closed = nullptr;  // [tiles]
   uint32_t *bin_open = nullptr;    // [bins] live tiles per bin (0 for bins of other ranks)
   uint32_t slab_tiles_cap = 0;
@@ -401,7 +409,8 @@ struct gs_context {
     uint32_t tpitch = 0;
     uint32_t torg[gs::kMaxViews][2] = {};    // rectangle origin (x, y) of each view
     bool restage = true;                     // false while gs_wait re-runs the frame: the staged rectangles are reused
-    uint32_t raster_flags = 0;               // k_raster instantiation of this frame (packed | depth | stats)
+    bool depth_write = false;                // GS_TARGET_DEPTH_WRITE: the frame also stores the target's depth
+    uint32_t raster_flags = 0;               // k_raster instantiation of this frame (packed | depth | stats | blend8 | depth write)
     uint32_t n_splats = 0;                   // resident splats when the frame was submitted
     uint32_t n_sortable = 0;                 // splats the frame's sort considers (scene frames: in the entities' ranges)
     bool slab = false;                       // rendered by the front-to-back slab path
@@ -556,7 +565,8 @@ void launch_tile_radix_pick(gs_context *c, FrameCounters *ctr, const FrameBufs &
 // over the whole table)
 void launch_pick(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameBufs &b, const uint32_t *pay,
                  const PickInput *in, gs_pick *out, cudaStream_t st);
-// views scene frames: one grid over every view's tiles (n_tiles: their sum), view v's frame at fp + v (flags: packed | depth)
+// views scene frames: one grid over every view's tiles (n_tiles: their sum), view v's frame at fp + v (flags: packed | depth,
+// and bit 4, depth write, with the depth test)
 void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags, cudaStream_t st);
 void launch_peer_acquire(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
 void launch_peer_signal_wait(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
@@ -581,9 +591,11 @@ void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters 
                             const ViewTable *views, const FrameBufs &b, cudaStream_t st);
 void launch_slab_end(gs_context *c, FrameCounters *ctr, cudaStream_t st);
 // stereo: one grid over every view's tiles (n_tiles: their sum; fp = &views->view[0]); likewise the resolve
+// depth_write (GS_TARGET_DEPTH_WRITE, depth-tested frames only): the slabs carry each pixel's crossing depth in pix_depth and
+// the resolve stores it into fp->depth_out
 void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, uint32_t n_tiles, const FrameBufs &b, bool depth,
-                        bool stereo, cudaStream_t st);
-void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, bool stereo, cudaStream_t st);
+                        bool stereo, bool depth_write, cudaStream_t st);
+void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, bool stereo, bool depth_write, cudaStream_t st);
 void launch_assemble(gs_context *c, const void *gathered, uint32_t tiles_per_rank, uint32_t world, uint32_t width,
                      uint32_t height, int32_t format, void *out_frame);
 

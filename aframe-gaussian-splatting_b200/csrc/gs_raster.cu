@@ -32,6 +32,7 @@
 namespace gs {
 
 constexpr float kTStop = 3e-4f;
+constexpr float kTHalf = 0.5f;  // GS_TARGET_DEPTH_WRITE: a pixel's depth is that of the pair after which T < kTHalf (gs_pick's)
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -86,13 +87,19 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 constexpr float kNegLog2e = -1.4426950216293334961f;  // the constant __expf multiplies by (0xBFB8AA3B)
 
-// Finished pixel -> frame (or packed owned tile, or every rank's frame over NVLink peer stores)
+// Finished pixel -> frame (or packed owned tile, or every rank's frame over NVLink peer stores).  DW (GS_TARGET_DEPTH_WRITE):
+// a pixel whose T ended below kTHalf also stores zc, the window depth of the pair that took it there, into fp->depth_out
+__device__ __forceinline__ void store_pixel_dw(const FrameParams *fp, uint32_t x, uint32_t y, bool inside, float T, float zc) {
+  if (inside && T < kTHalf) fp->depth_out[(size_t)y * fp->rc.pitch + x] = zc;
+}
+template <bool DW = false>
 __device__ __forceinline__ void store_pixel(const FrameParams *fp, uint32_t tile, uint32_t tx, uint32_t ty, uint32_t lx,
                                             uint32_t ly, uint32_t x, uint32_t y, bool inside, float T, float Cr, float Cg,
-                                            float Cb) {
+                                            float Cb, float zc = 1.0f) {
   const RenderConsts &rc = fp->rc;
   // a frame into a gs_target whose instance buffer overflowed is re-run over the target: this run leaves it as it was
   if (fp->overflow && *fp->overflow) return;
+  if (DW) store_pixel_dw(fp, x, y, inside, T, zc);  // a target frame: row-major, no peers
   // the pixel's place in out and color_in: rows of rc.pitch pixels (a device target's row pitch, else the width; the
   // host points the buffers at the target rectangle's origin)
   const size_t p = (size_t)y * rc.pitch + x;
@@ -194,6 +201,8 @@ struct SlabIO {
   uint8_t *closed;       // [tiles] every pixel of the tile is dead
   uint32_t *bin_open;    // [bins] live tiles per bin
   FrameCounters *ctr;    // open_bins
+  float *depth;          // [tiles * 256] DW: window depth of the pair after which the pixel's T fell below kTHalf, tile-major;
+                         // written by the slab in which that happened, read by k_resolve
 };
 
 // DEPTH: depth-test every fragment LEQUAL against fp->depth_in (index.js:179-180).  STATS: count what the tile does
@@ -207,13 +216,18 @@ struct SlabIO {
 // B8: GS_RENDER_BLEND_UNORM8 (packed loop, one pass): the reference's back-to-front blend with the RGBA8 store after every
 // fragment.  Chunks stream farthest first, the kept records are walked in draw order, every pair is blended (no stop rule:
 // rounding after each blend has no front-to-back form), and the pixel state is the destination's bytes (as byte / 255).
-template <bool PACKED, bool DEPTH, bool STATS, bool SLAB = false, bool STEREO = false, bool B8 = false>
+// DW: GS_TARGET_DEPTH_WRITE (depth-tested front-to-back frames): every pixel keeps the window depth of the last pair it
+// blended while its T was still >= kTHalf.  Once T has fallen below kTHalf that is the pair after which it did (the pick's
+// pair, gs_pick.cu), and the pixel stores it into fp->depth_out next to its colour; with SLAB the slab in which T crossed
+// kTHalf hands it to k_resolve through slab.depth instead, since later slabs still depth-test against depth_in.
+template <bool PACKED, bool DEPTH, bool STATS, bool SLAB = false, bool STEREO = false, bool B8 = false, bool DW = false>
 __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>::kMinBlocks) k_raster(const float4 *__restrict__ inst_rec,
                                                                         const uint2 *__restrict__ bin_range,
                                                                         const FrameParams *__restrict__ fp,
                                                                         uint4 *__restrict__ tile_stats, SlabIO slab) {
   static_assert(!STEREO || !STATS, "stereo frames take no statistics");
   static_assert(!B8 || (PACKED && !SLAB), "blend8 frames take the packed one-pass loop");
+  static_assert(!DW || (DEPTH && !B8), "depth-writing frames are depth-tested front-to-back frames");
   using Cfg = RasterCfg<PACKED>;
   constexpr int kThreads = Cfg::kThreads, kChunk = Cfg::kChunk, kStages = Cfg::kStages, kCv = Cfg::kCv;
   constexpr int kWarps = kThreads / 32;
@@ -313,6 +327,8 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
       lim0 = (inside0 && T0 >= kTStop) ? 4.0f : -1.0f;
     }
   }
+  float z0 = 1.0f, z1 = 1.0f;  // DW: depth of the last pair blended while T >= kTHalf
+  const float tb0 = PACKED ? T2.x : T0, tb1 = T2.y;  // DW with SLAB: T where this slab starts
   float4 D0 = make_float4(0.f, 0.f, 0.f, 0.f), D1 = D0;  // B8: destination bytes / 255 of the pair
   if (B8) {
     D0 = load_pixel8(fp, x, y, inside0, s_u8f);
@@ -420,6 +436,10 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
             R2 = fma2(make_float2(q2.x, q2.x), w2, R2);
             G2 = fma2(make_float2(q2.y, q2.y), w2, G2);
             B2 = fma2(make_float2(q2.z, q2.z), w2, B2);
+            if (DW) {
+              z0 = (T2.x >= kTHalf) ? q0.w : z0;
+              z1 = (T2.y >= kTHalf) ? q0.w : z1;
+            }
             T2 = fma2(w2, make_float2(-1.0f, -1.0f), T2);  // T - w, one rounding
             lim0 = (T2.x >= kTStop) ? lim0 : -1.0f;
             lim1 = (T2.y >= kTStop) ? lim1 : -1.0f;
@@ -446,6 +466,7 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
             R0 = __fmaf_rn(col.x, w, R0);
             G0 = __fmaf_rn(col.y, w, G0);
             B0 = __fmaf_rn(col.z, w, B0);
+            if (DW) z0 = (T0 >= kTHalf) ? q1.z : z0;
             T0 = __fmaf_rn(w, -1.0f, T0);
             lim0 = (T0 >= kTStop) ? lim0 : -1.0f;
           }
@@ -472,6 +493,11 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
     } else {
       slab.state[(size_t)stile * 256 + ly * 16 + lx] = make_float4(R0, G0, B0, T0);
     }
+    if (DW) {  // T crossed kTHalf in this slab: the crossing pair's depth for k_resolve
+      const float te0 = PACKED ? T2.x : T0;
+      if (tb0 >= kTHalf && te0 < kTHalf) slab.depth[(size_t)stile * 256 + ly * 16 + lx] = z0;
+      if (PACKED && tb1 >= kTHalf && T2.y < kTHalf) slab.depth[(size_t)stile * 256 + (ly + 1) * 16 + lx] = z1;
+    }
     const int alive_end = __syncthreads_or((lim0 > 0.0f) || (lim1 > 0.0f));
     if (!alive_end && tid == 0) {  // saturated: later slabs skip the tile, and the bin once all its tiles are closed
       slab.closed[stile] = 1;
@@ -481,10 +507,10 @@ __global__ void __launch_bounds__(RasterCfg<PACKED>::kThreads, RasterCfg<PACKED>
     store_pixel8(fp, x, y, inside0, D0);
     store_pixel8(fp, x, y + 1, inside1, D1);
   } else if (PACKED) {
-    store_pixel(fp, tile, tx, ty, lx, ly, x, y, inside0, T2.x, R2.x, G2.x, B2.x);
-    store_pixel(fp, tile, tx, ty, lx, ly + 1, x, y + 1, inside1, T2.y, R2.y, G2.y, B2.y);
+    store_pixel<DW>(fp, tile, tx, ty, lx, ly, x, y, inside0, T2.x, R2.x, G2.x, B2.x, z0);
+    store_pixel<DW>(fp, tile, tx, ty, lx, ly + 1, x, y + 1, inside1, T2.y, R2.y, G2.y, B2.y, z1);
   } else {
-    store_pixel(fp, tile, tx, ty, lx, ly, x, y, inside0, T0, R0, G0, B0);
+    store_pixel<DW>(fp, tile, tx, ty, lx, ly, x, y, inside0, T0, R0, G0, B0, z0);
   }
   if (STATS) {
     for (int o = 16; o > 0; o >>= 1) {
@@ -554,11 +580,23 @@ __global__ void __launch_bounds__(256) k_assemble(const void *__restrict__ gathe
 }
 
 // flags: bit 0 = packed pixel loop, bit 1 = depth test against fp->depth_in, bit 2 = per-tile statistics,
-// bit 3 = GS_RENDER_BLEND_UNORM8 (always the packed loop)
+// bit 3 = GS_RENDER_BLEND_UNORM8 (always the packed loop), bit 4 = GS_TARGET_DEPTH_WRITE (with bit 1, never with bit 3)
 void launch_raster(gs_context *c, const FrameParams *fp, uint32_t n_tiles, const FrameBufs &b, uint32_t flags,
                    cudaStream_t st) {
   uint4 *ts = c->tile_stats;
   constexpr int kT = RasterCfg<true>::kThreads;
+  if (flags & 16u) {
+    switch (flags & 5u) {
+#define GS_RASTER_CASE(v, P, S) \
+  case v: k_raster<P, true, S, false, false, false, true><<<n_tiles, RasterCfg<P>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, ts, SlabIO{}); break;
+      GS_RASTER_CASE(0, false, false)
+      GS_RASTER_CASE(1, true, false)
+      GS_RASTER_CASE(4, false, true)
+      GS_RASTER_CASE(5, true, true)
+#undef GS_RASTER_CASE
+    }
+    return;
+  }
   if (flags & 8u) {
     switch ((flags >> 1) & 3u) {
 #define GS_RASTER_CASE(v, D, S) \
@@ -594,6 +632,11 @@ void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles
     else k_raster<true, false, false, false, true, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{});
     return;
   }
+  if (flags & 16u) {
+    if (flags & 1u) k_raster<true, true, false, false, true, false, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{});
+    else k_raster<false, true, false, false, true, false, true><<<n_tiles, RasterCfg<false>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{});
+    return;
+  }
   switch (flags & 3u) {
 #define GS_RASTER_CASE(v, P, D) \
   case v: k_raster<P, D, false, false, true><<<n_tiles, RasterCfg<P>::kThreads, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, SlabIO{}); break;
@@ -608,10 +651,14 @@ void launch_raster_stereo(gs_context *c, const FrameParams *fp, uint32_t n_tiles
 // one slab of a frame (always the packed pixel loop); stereo: every view's tiles in one grid (n_tiles: their sum), view v's
 // frame at fp + v
 void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr, uint32_t n_tiles, const FrameBufs &b, bool depth,
-                        bool stereo, cudaStream_t st) {
-  const SlabIO io{c->pix_state, c->tile_closed, c->bin_open, ctr};
+                        bool stereo, bool depth_write, cudaStream_t st) {
+  const SlabIO io{c->pix_state, c->tile_closed, c->bin_open, ctr, c->pix_depth};
   constexpr int kT = RasterCfg<true>::kThreads;
-  if (stereo && depth)
+  if (depth_write && stereo)
+    k_raster<true, true, false, true, true, false, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
+  else if (depth_write)
+    k_raster<true, true, false, true, false, false, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
+  else if (stereo && depth)
     k_raster<true, true, false, true, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
   else if (stereo)
     k_raster<true, false, false, true, true><<<n_tiles, kT, 0, st>>>(b.inst_rec, b.bin_range, fp, nullptr, io);
@@ -623,9 +670,11 @@ void launch_raster_slab(gs_context *c, const FrameParams *fp, FrameCounters *ctr
 
 // slab path epilogue: pixel state -> frame (composite over the clear colour or colour target; plain / tiled / peer destinations).
 // STEREO: one CTA per tile of every view (fp = &views->view[0]): CTA b resolves slab tile b into tile b - tile_base[v] of
-// the view v whose CTAs hold b, with that view's frame fp[v]
-template <bool STEREO>
-__global__ void __launch_bounds__(256) k_resolve(const float4 *__restrict__ state, const FrameParams *__restrict__ fp) {
+// the view v whose CTAs hold b, with that view's frame fp[v].  DW: a pixel whose T ended below kTHalf also stores the depth
+// its crossing slab left in `depth` into fp->depth_out
+template <bool STEREO, bool DW = false>
+__global__ void __launch_bounds__(256) k_resolve(const float4 *__restrict__ state, const FrameParams *__restrict__ fp,
+                                                 const float *__restrict__ depth) {
   const uint32_t view = STEREO ? view_of(view_table(fp)->tile_base, blockIdx.x) : 0u;
   const uint32_t tile = blockIdx.x - (STEREO ? view_table(fp)->tile_base[view] : 0u);
   if (STEREO) fp += view;
@@ -635,12 +684,15 @@ __global__ void __launch_bounds__(256) k_resolve(const float4 *__restrict__ stat
   const uint32_t lx = threadIdx.x & 15u, ly = threadIdx.x >> 4;
   const uint32_t x = tx * kTile + lx, y = ty * kTile + ly;
   const float4 s = state[(size_t)blockIdx.x * 256 + threadIdx.x];
-  store_pixel(fp, tile, tx, ty, lx, ly, x, y, (x < rc.width) && (y < rc.height), s.w, s.x, s.y, s.z);
+  const float z = (DW && s.w < kTHalf) ? depth[(size_t)blockIdx.x * 256 + threadIdx.x] : 1.0f;
+  store_pixel<DW>(fp, tile, tx, ty, lx, ly, x, y, (x < rc.width) && (y < rc.height), s.w, s.x, s.y, s.z, z);
 }
 
-void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, bool stereo, cudaStream_t st) {
-  if (stereo) k_resolve<true><<<n_tiles, 256, 0, st>>>(c->pix_state, fp);
-  else k_resolve<false><<<n_tiles, 256, 0, st>>>(c->pix_state, fp);
+void launch_resolve(gs_context *c, const FrameParams *fp, uint32_t n_tiles, bool stereo, bool depth_write, cudaStream_t st) {
+  if (depth_write && stereo) k_resolve<true, true><<<n_tiles, 256, 0, st>>>(c->pix_state, fp, c->pix_depth);
+  else if (depth_write) k_resolve<false, true><<<n_tiles, 256, 0, st>>>(c->pix_state, fp, c->pix_depth);
+  else if (stereo) k_resolve<true><<<n_tiles, 256, 0, st>>>(c->pix_state, fp, nullptr);
+  else k_resolve<false><<<n_tiles, 256, 0, st>>>(c->pix_state, fp, nullptr);
 }
 
 void launch_peer_acquire(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st) {

@@ -11,7 +11,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F, GS_RENDER_BLEND_UNORM8, GS_RENDER_OUT_DEVICE, GS_RENDER_OUT_TILED,
-                   GS_RENDER_REUSE_SORT, GS_RENDER_STATS, GS_TARGET_DEVICE, GsObject, GsRenderParams, GsStats, GsTarget)
+                   GS_RENDER_REUSE_SORT, GS_RENDER_STATS, GS_TARGET_DEPTH_WRITE, GS_TARGET_DEVICE, GsObject, GsRenderParams, GsStats, GsTarget)
 from .scenes import FrameInputs
 
 
@@ -407,34 +407,62 @@ class SplatContext:
 
     # -- frames drawn into the caller's framebuffer in place (gs_render_scene*_target) --
     @staticmethod
-    def make_target(color_ptr: int, depth_ptr: Optional[int], pitch: int, rows: int, device: bool = False) -> GsTarget:
+    def make_target(color_ptr: int, depth_ptr: Optional[int], pitch: int, rows: int, device: bool = False,
+                    write_depth: bool = False) -> GsTarget:
         """gs_target over caller-owned buffers: pitch x rows pixels of colour (and f32 depth, or None); device=True for
-        device memory on the context's GPU."""
+        device memory on the context's GPU; write_depth=True (GS_TARGET_DEPTH_WRITE, needs depth): every pixel that turns
+        half opaque also leaves its splat depth in the depth buffer."""
         t = GsTarget()
         t.color, t.depth = color_ptr, depth_ptr
-        t.pitch, t.rows, t.flags = int(pitch), int(rows), GS_TARGET_DEVICE if device else 0
+        t.pitch, t.rows = int(pitch), int(rows)
+        t.flags = (GS_TARGET_DEVICE if device else 0) | (GS_TARGET_DEPTH_WRITE if write_depth else 0)
         return t
 
-    @staticmethod
-    def _host_target(color: np.ndarray, depth: Optional[np.ndarray], fmt: int) -> GsTarget:
-        """gs_target over numpy buffers: color (rows, pitch, 4) of the format's dtype, depth (rows, pitch) f32 or None.
-        Both are written (colour) and read in place, so they must be C-contiguous already."""
+    def _array_target(self, color, depth, fmt: int, write_depth: bool = False) -> GsTarget:
+        """gs_target of a synchronous target frame over numpy buffers (host) or torch CUDA tensors on the context's GPU
+        (device): color (rows, pitch, 4) of the format's dtype, depth (rows, pitch) f32 or None.  Both are written and read
+        in place, so they must be C-contiguous already.  write_depth (GS_TARGET_DEPTH_WRITE) needs depth.
+        The library's streams do not wait for torch's, so for tensors this first waits for the caller's current stream on
+        their device: the frame reads what torch wrote there, and the synchronous call returns only once the frame is done,
+        so later torch work sees what the frame wrote."""
+        if write_depth and depth is None:
+            raise ValueError("write_depth needs a depth buffer")
         dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
+        if hasattr(color, "data_ptr"):  # torch tensors on the GPU
+            import torch
+            tdtype = torch.uint8 if fmt == GS_FORMAT_RGBA8 else torch.float32
+            if (not color.is_cuda or color.dtype != tdtype or color.dim() != 3 or color.shape[2] != 4
+                    or not color.is_contiguous()):
+                raise ValueError("color must be a contiguous (rows, pitch, 4) CUDA tensor of the output format's dtype")
+            rows, pitch = color.shape[:2]
+            if depth is not None and (not hasattr(depth, "data_ptr") or not depth.is_cuda or depth.dtype != torch.float32
+                                      or tuple(depth.shape) != (rows, pitch) or not depth.is_contiguous()):
+                raise ValueError("depth must be a contiguous (rows, pitch) float32 CUDA tensor")
+            for t in (color, depth):
+                if t is not None and t.device.index != self.device:
+                    raise ValueError(f"target tensors must be on the context's GPU (cuda:{self.device}), not {t.device}")
+            torch.cuda.current_stream(color.device).synchronize()
+            return SplatContext.make_target(color.data_ptr(), None if depth is None else depth.data_ptr(), pitch, rows,
+                                            device=True, write_depth=write_depth)
         if color.dtype != dtype or color.ndim != 3 or color.shape[2] != 4 or not color.flags["C_CONTIGUOUS"]:
             raise ValueError("color must be a C-contiguous (rows, pitch, 4) array of the output format's dtype")
         rows, pitch = color.shape[:2]
-        if depth is not None and (depth.dtype != np.float32 or depth.shape != (rows, pitch) or not depth.flags["C_CONTIGUOUS"]):
+        if depth is not None and (not isinstance(depth, np.ndarray) or depth.dtype != np.float32
+                                  or depth.shape != (rows, pitch) or not depth.flags["C_CONTIGUOUS"]):
             raise ValueError("depth must be a C-contiguous (rows, pitch) float32 array")
-        return SplatContext.make_target(color.ctypes.data, None if depth is None else depth.ctypes.data, pitch, rows)
+        return SplatContext.make_target(color.ctypes.data, None if depth is None else depth.ctypes.data, pitch, rows,
+                                        write_depth=write_depth)
 
     def render_scene_target(self, frame: FrameInputs, objects: Sequence[SceneObject], color: np.ndarray,
                             depth: Optional[np.ndarray] = None, viewport=(0, 0), fmt: int = GS_FORMAT_RGBA8,
-                            stats: bool = False, blend_unorm8: bool = False) -> np.ndarray:
+                            stats: bool = False, blend_unorm8: bool = False, write_depth: bool = False) -> np.ndarray:
         """gs_render_scene_target: the scene frame blended IN PLACE into the rectangle of frame.width x frame.height at
         viewport = (x, y) of `color` ((rows, pitch, 4), row 0 = bottom), depth-tested against `depth` ((rows, pitch) f32
         window-space depth, or None).  Nothing outside the rectangle is read or written.  Returns `color`.
-        blend_unorm8 as render()."""
-        t = self._host_target(color, depth, fmt)
+        numpy buffers are host targets, CUDA tensors on the context's GPU device targets (the frame waits for the
+        caller's current torch stream and is finished when this returns).  blend_unorm8 as render(); write_depth
+        (GS_TARGET_DEPTH_WRITE): each pixel that turns half opaque also leaves its splat depth in `depth`."""
+        t = self._array_target(color, depth, fmt, write_depth)
         p = self.make_params(frame, fmt=fmt, flags=(GS_RENDER_STATS if stats else 0) | _blend8(blend_unorm8))
         st = GsStats()
         self._check(self._lib.gs_render_scene_target(self._h, C.byref(p), make_objects(objects), len(objects), C.byref(t),
@@ -453,11 +481,12 @@ class SplatContext:
 
     def render_scene_stereo_target(self, eyes: Sequence[FrameInputs], objects: Sequence[SceneObject], eye_modelviews,
                                    color: np.ndarray, depth: Optional[np.ndarray] = None, eye_xy=None,
-                                   fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False) -> np.ndarray:
+                                   fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False,
+                                   write_depth: bool = False) -> np.ndarray:
         """gs_render_scene_stereo_target: one WebXR frame drawn IN PLACE into one layer ((rows, pitch, 4) colour, optional
         (rows, pitch) f32 depth): eye e at (eye_xy[2e], eye_xy[2e+1]); eye_xy None = side by side, (0, 0, w, 0).
-        Arguments as render_scene_stereo.  Returns `color`."""
-        t = self._host_target(color, depth, fmt)
+        Arguments as render_scene_stereo; buffers and write_depth as render_scene_target.  Returns `color`."""
+        t = self._array_target(color, depth, fmt, write_depth)
         st = GsStats()
         args = self._stereo_target_args(eyes, fmt, objects, eye_modelviews, eye_xy, _blend8(blend_unorm8))
         self._check(self._lib.gs_render_scene_stereo_target(self._h, args[0], args[1], args[2], len(objects), C.byref(t),
@@ -479,11 +508,11 @@ class SplatContext:
 
     def render_scene_views_target(self, views: Sequence[FrameInputs], objects: Sequence[SceneObject], view_mvs,
                                   color: np.ndarray, view_xy, depth: Optional[np.ndarray] = None, fmt: int = GS_FORMAT_RGBA8,
-                                  blend_unorm8: bool = False) -> np.ndarray:
+                                  blend_unorm8: bool = False, write_depth: bool = False) -> np.ndarray:
         """gs_render_scene_views_target: one WebXR frame of every view drawn IN PLACE into one layer ((rows, pitch, 4)
         colour, optional (rows, pitch) f32 depth): view v at (view_xy[2v], view_xy[2v+1]).  Arguments as
-        render_scene_views.  Returns `color`."""
-        t = self._host_target(color, depth, fmt)
+        render_scene_views; buffers and write_depth as render_scene_target.  Returns `color`."""
+        t = self._array_target(color, depth, fmt, write_depth)
         st = GsStats()
         args = self._views_target_args(views, fmt, objects, view_mvs, view_xy, _blend8(blend_unorm8))
         self._check(self._lib.gs_render_scene_views_target(self._h, args[0], len(views), args[1], args[2], len(objects),

@@ -410,11 +410,15 @@ GS_API int gs_render_scene_stereo(gs_context *ctx, const gs_render_params eyes[2
  * the current viewport; in a WebXR session that is the XR layer's one framebuffer, both eyes side by side over one depth
  * buffer, each eye camera drawn at its own viewport rectangle).
  */
-enum { GS_TARGET_DEVICE = 1u << 0 /* color and depth are device memory on the context's GPU (default: host memory) */ };
+enum {
+  GS_TARGET_DEVICE = 1u << 0,      /* color and depth are device memory on the context's GPU (default: host memory)       */
+  GS_TARGET_DEPTH_WRITE = 1u << 1  /* the frame also writes depth: see "Depth write" below                                */
+};
 typedef struct gs_target {
   void *color;         /* pitch * rows pixels of the frame's out_format (u8 RGBA8 / f32 RGBA32F), row 0 = bottom: the blend's
                           destination, written in place                                                                  */
-  const float *depth;  /* NULL, or pitch * rows window-space depths in [0,1], row 0 = bottom (LEQUAL test, nothing written) */
+  const float *depth;  /* NULL, or pitch * rows window-space depths in [0,1], row 0 = bottom (LEQUAL test; written only with
+                          GS_TARGET_DEPTH_WRITE)                                                                          */
   uint32_t pitch;      /* pixels per row of both buffers                                                                  */
   uint32_t rows;       /* rows of both buffers                                                                            */
   uint32_t flags;      /* GS_TARGET_*                                                                                     */
@@ -444,6 +448,20 @@ typedef struct gs_target {
  *   - a frame whose tile-instance buffer overflowed is re-run by gs_wait over the target's content as it was when the
  *     frame started: the overflowed run stores nothing, and a host target's re-run reuses the copy taken at submission;
  *   - gs_stats: those of the gs_render_scene frame.
+ * Depth write (GS_TARGET_DEPTH_WRITE, accepted by every *_target[_async] entry point, on every path): after the frame, each
+ * pixel of each view's rectangle whose transmittance T fell below 0.5 holds the window depth z/w * 0.5 + 0.5 of the first
+ * pair, in the raster's nearest-first walk of the blended pairs (same pairs, same fp32 T = fma(w, -1, T), same stop rule),
+ * after whose blend T < 0.5: the pixel's median surface.  A mono frame's value is bit for bit gs_pick_scene(...).depth at
+ * that pixel with depth_in the rectangle's depth before the frame; stereo and views frames walk each view's pairs in the
+ * head-sorted draw order.  A pixel whose T stays >= 0.5 keeps its depth.  Every written value passed the LEQUAL test, so
+ * depth never increases.  The colour is byte-identical to the frame without the flag.
+ *   - device targets: the depth is written in place; host targets: the rectangle staged at submission is written back by
+ *     the frame's read-back, next to the colour;
+ *   - an overflowed run stores no depth either, and its re-run starts from the depth as it was;
+ *   - frames in flight: when either frame writes depth, a pending target frame whose rectangle overlaps on the same `depth`
+ *     buffer is waited for as one on the same `color` is, so depth-writing frames compose in submission order;
+ *   - GS_ERR_INVALID, changing nothing, for the flag on a target without depth, or with GS_RENDER_BLEND_UNORM8 (whose
+ *     back-to-front byte blend has no front-to-back T).
  */
 GS_API int gs_render_scene_target_async(gs_context *ctx, const gs_render_params *frame, const gs_object *objs,
                                         uint32_t n_objs, const gs_target *target, uint32_t x, uint32_t y,
