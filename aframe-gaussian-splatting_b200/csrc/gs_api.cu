@@ -681,18 +681,23 @@ static int ensure_ply_staging(gs_context *c) {
 }
 
 // processPlyBuffer + one pushDataBuffer on the device (gs_ply.cu), its rows packed into [at, at + n): gs_push_ply
-// (at == c->n) and gs_insert_ply.  Same contract as gs_push_splats: an append does not wait for frames in flight, the
-// caller's file is consumed on return, only a push that outgrows the table waits.
+// (at == c->n) and gs_insert_ply; a compressed PLY gives the rows of its float restatement (ply.decompress_ply).
+// Same contract as gs_push_splats: an append does not wait for frames in flight, the caller's file is consumed on
+// return, only a push that outgrows the table waits.
 static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes, void *rows32_out_or_null, uint32_t *out_n) {
   if (out_n) *out_n = 0;
-  PlyLayout L;
+  PlyLayout L{};
+  PlyCompressedLayout Z{};  // a compressed PLY (ply_is_compressed): decoded by k_ply_decode_compressed
   PlyShLayout S{};
   S.ctx_k = sh_coeffs(c->sh_degree);
   S.vecs = c->sh_vecs;
   PlyShLayout *sh = c->sh_degree ? &S : nullptr;
   uint32_t n = 0;
   size_t data_off = 0;
-  if (ply_parse((const uint8_t *)ply, bytes, L, n, data_off, c->err, sh)) return GS_ERR_INVALID;  // nothing changed yet
+  const bool compressed = ply_is_compressed((const uint8_t *)ply, bytes);
+  if (compressed ? ply_parse_compressed((const uint8_t *)ply, bytes, Z, n, c->err)
+                 : ply_parse((const uint8_t *)ply, bytes, L, n, data_off, c->err, sh))
+    return GS_ERR_INVALID;  // nothing changed yet
   if (!n) return GS_OK;
   GS_CUDA(c, cudaSetDevice(c->device));
   int rc;
@@ -704,7 +709,11 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   cudaStream_t st = c->push_stream;
   // temporaries, stream-ordered: decoded rows (32 B) + key per row, two permutations, radix tables, ordered rows
   const uint32_t chunks = (n + kRadixTile - 1) / kRadixTile;
-  const size_t stride = L.stride, rows_per_chunk = gs_context::kPlyChunkBytes / stride;
+  // a compressed piece: whole chunks of rows (ply_stage_compressed); sh_k: its SH bytes per splat / 3
+  const uint32_t sh_k = sh ? Z.file_k : 0u;
+  const size_t stride = L.stride;
+  const size_t rows_per_chunk = compressed ? ply_compressed_piece_rows(sh_k) : gs_context::kPlyChunkBytes / stride;
+  const size_t body_bytes = compressed ? gs_context::kPlyChunkBytes : rows_per_chunk * stride;
   uint8_t *rows_dev = nullptr, *out_dev = nullptr, *body[2] = {nullptr, nullptr};
   uint32_t *key = nullptr, *perm_a = nullptr, *perm_b = nullptr, *table = nullptr, *totals = nullptr;
   uint4 *sh_dev = nullptr;  // SH contexts: the decoded coefficients, in file order
@@ -714,10 +723,10 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
       if (p) cudaFreeAsync(p, st);
   };
   cudaError_t e = cudaSuccess;
-  const bool sort = L.has_scale && n > 1;  // without scale_0 every key is 0: the stable sort is the identity
+  const bool sort = (compressed || L.has_scale) && n > 1;  // without scale_0 every key is 0: the stable sort is the identity
   e = cudaMallocAsync((void **)&rows_dev, (size_t)n * 32, st);
   if (!e) e = cudaMallocAsync((void **)&key, (size_t)n * 4, st);
-  for (int i = 0; i < 2 && !e; ++i) e = cudaMallocAsync((void **)&body[i], rows_per_chunk * stride, st);
+  for (int i = 0; i < 2 && !e; ++i) e = cudaMallocAsync((void **)&body[i], body_bytes, st);
   if (!e && sort) e = cudaMallocAsync((void **)&perm_a, (size_t)n * 4, st);
   if (!e && sort) e = cudaMallocAsync((void **)&perm_b, (size_t)n * 4, st);
   if (!e && sort) e = cudaMallocAsync((void **)&table, (size_t)256 * (chunks + 1) * 4, st);
@@ -734,11 +743,18 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   for (uint32_t r0 = 0, k = 0; r0 < n && !e; r0 += (uint32_t)rows_per_chunk, ++k) {
     const uint32_t m = (uint32_t)std::min<size_t>(rows_per_chunk, n - r0);
     const int b = (int)(k & 1u);
+    const size_t piece = compressed ? ply_compressed_piece_bytes(m, sh_k) : (size_t)m * stride;
     if ((e = cudaEventSynchronize(c->ply_ev[b]))) break;  // this pinned buffer's previous chunk is on the device
-    memcpy(c->ply_pinned[b], src + (size_t)r0 * stride, (size_t)m * stride);
-    if ((e = cudaMemcpyAsync(body[b], c->ply_pinned[b], (size_t)m * stride, cudaMemcpyHostToDevice, st))) break;
+    if (compressed)
+      ply_stage_compressed((const uint8_t *)ply, Z, sh_k, r0, m, (uint8_t *)c->ply_pinned[b]);
+    else
+      memcpy(c->ply_pinned[b], src + (size_t)r0 * stride, piece);
+    if ((e = cudaMemcpyAsync(body[b], c->ply_pinned[b], piece, cudaMemcpyHostToDevice, st))) break;
     if ((e = cudaEventRecord(c->ply_ev[b], st))) break;
-    launch_ply_decode(body[b], m, L, r0, rows_dev, key, sh, sh_dev, st);
+    if (compressed)
+      launch_ply_decode_compressed(body[b], m, Z, r0, rows_dev, key, sh, sh_dev, st);
+    else
+      launch_ply_decode(body[b], m, L, r0, rows_dev, key, sh, sh_dev, st);
     e = cudaGetLastError();
   }
   const uint32_t *perm = nullptr;

@@ -216,6 +216,30 @@ struct PlyShLayout {
 // receives the file's f_rest_* fields, and the fast all-f32 path then also requires them to be aligned floats.
 int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_t &data_off, std::string &err,
               PlyShLayout *sh = nullptr);
+// ---- compressed PLY (SuperSplat's export): element `chunk` (one row of f32 bounds per 256 splats), element `vertex`
+// (uint packed_position / _rotation / _scale / _color), optional element `sh` (uchar f_rest_*).  A piece of the body is
+// staged as [chunk rows, 18 f32 each, padded to 16 B | 16 B of packed words per splat | 3 file_k SH bytes per splat, padded
+// to 16 B] for a run of rows that starts on a chunk boundary ----
+constexpr int kPlyBounds = 18;  // min_x .. max_z, min_scale_x .. max_scale_z, min_r .. max_b
+struct PlyCompressedLayout {
+  uint64_t body[3];               // file offsets of the chunk, vertex and sh element bodies
+  uint32_t stride[3];             // their row sizes
+  int32_t bound[kPlyBounds];      // offset of each bound in a chunk row (the colour ones -1 without colour bounds)
+  int32_t word[4];                // offset of packed_position, _rotation, _scale, _color in a vertex row
+  int32_t rest[3 * kMaxShCoeffs];  // offset of f_rest_k in an sh row, k < 3 file_k
+  uint32_t has_color, file_k;     // colour bounds present; K of the sh element's degree (0 without one)
+};
+// Whether the header declares a compressed PLY: element chunk and element vertex, the vertex element's uint packed_position,
+// packed_rotation, packed_scale and packed_color, and no property named x (which every file ply_parse accepts has).
+bool ply_is_compressed(const uint8_t *ply, size_t bytes);
+// Parses a header ply_is_compressed accepted.  Returns GS_OK with the layout and vertex count, or GS_ERR_INVALID with `err`.
+int ply_parse_compressed(const uint8_t *ply, size_t bytes, PlyCompressedLayout &Z, uint32_t &n, std::string &err);
+// Rows per staged piece (a multiple of 256) and the bytes of a piece of m rows; sh_k: SH bytes per splat / 3 (0 = none)
+uint32_t ply_compressed_piece_rows(uint32_t sh_k);
+size_t ply_compressed_piece_bytes(uint32_t m, uint32_t sh_k);
+// Stages rows [r0, r0 + m) of the file (r0 a multiple of 256) as one piece at dst
+void ply_stage_compressed(const uint8_t *ply, const PlyCompressedLayout &Z, uint32_t sh_k, uint32_t r0, uint32_t m,
+                          uint8_t *dst);
 
 // ---- front-to-back slab path ----
 constexpr int kMaxSlabs = 12;         // geometric slab sizes: 1 M, 2 M, 4 M ... entries (nearest first)
@@ -543,6 +567,9 @@ void launch_move_rows(gs_context *c, uint32_t from, uint32_t to, uint32_t len, v
 // sh (SH contexts, else NULL): the rows' coefficients into sh_rows (sh->vecs words per row), in file order too
 void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,
                        uint32_t *key, const PlyShLayout *sh, uint4 *sh_rows, cudaStream_t st);
+// compressed PLY push: the same for a staged piece of `rows` rows (ply_stage_compressed with sh_k = sh ? file_k : 0)
+void launch_ply_decode_compressed(const uint8_t *piece, uint32_t rows, const PlyCompressedLayout &Z, uint32_t first_row,
+                                  uint8_t *rows32, uint32_t *key, const PlyShLayout *sh, uint4 *sh_rows, cudaStream_t st);
 // PLY push: stable ascending sort of n 32-bit keys as four 8-bit passes (12 launches); returns the buffer holding the
 // permutation (perm_b).  table: 256 * (ceil(n / kRadixTile) + 1) words, totals: 256 words.
 uint32_t *launch_ply_sort(gs_context *c, const uint32_t *key, uint32_t *perm_a, uint32_t *perm_b, uint32_t *table,

@@ -9,6 +9,10 @@
 //                  <true>: every field read is an aligned float (the INRIA layout); <false>: any TYPE_MAP type, byte loads.
 //                  <., true> (SH contexts): also the row's f_rest_* coefficients as fp16, in file order like the rows.
 //   the stable sort of the keys is k_radix_*<P<0>> .. <P<24>> (gs_sort.cu).
+//   compressed PLY (SuperSplat's export; ply_is_compressed): ply_parse_compressed reads an element-aware header,
+//   ply_stage_compressed stages whole chunks of rows as [chunk bounds | 16 B packed words | SH bytes], and
+//   k_ply_decode_compressed<kSH> (one CTA of 256 threads per chunk) forms each property in fp64, rounds it once to f32
+//   and runs the row conversion k_ply_decode runs (ply_convert_row): the rows of the file's float restatement.
 //
 // Numerics: fp64 as JavaScript evaluates it, no contraction (the library is built with --fmad=false).  The importance
 // product runs left to right and is rounded to f32 (Float32Array store); the key is the complement of the order-preserving
@@ -18,6 +22,8 @@
 // about one fp64 ulp of an f32 rounding midpoint (DESIGN.md section 3).
 #include <cuda_fp16.h>
 #include <string.h>
+
+#include <vector>
 
 #include "gs_common.cuh"
 
@@ -137,6 +143,212 @@ int ply_parse(const uint8_t *ply, size_t bytes, PlyLayout &L, uint32_t &n, size_
   return GS_OK;
 }
 
+// ---- compressed PLY header: element-aware, so offsets restart in every element ----
+namespace {
+struct PlyProp {
+  std::string name, type;
+  int off, size;  // size 0: a list or unknown type
+};
+struct PlyElement {
+  std::string name;
+  uint64_t count = 0;
+  uint32_t stride = 0;
+  bool counted = false;  // `element <name> <digits>`
+  std::vector<PlyProp> props;
+  const PlyProp *find(const std::string &n) const {  // the last property of a name
+    for (size_t i = props.size(); i-- > 0;)
+      if (props[i].name == n) return &props[i];
+    return nullptr;
+  }
+};
+int ply_type_size(const std::string &t) {
+  if (t == "double") return 8;
+  if (t == "int" || t == "uint" || t == "float") return 4;
+  if (t == "short" || t == "ushort") return 2;
+  if (t == "uchar") return 1;
+  return 0;
+}
+const char *const kBoundName[kPlyBounds] = {"min_x",       "min_y",       "min_z",       "max_x",       "max_y",
+                                            "max_z",       "min_scale_x", "min_scale_y", "min_scale_z", "max_scale_x",
+                                            "max_scale_y", "max_scale_z", "min_r",       "min_g",       "min_b",
+                                            "max_r",       "max_g",       "max_b"};
+const char *const kWordName[4] = {"packed_position", "packed_rotation", "packed_scale", "packed_color"};
+// The header's lines split by single spaces, as the reference splits them.  Returns false without "end_header\n" in the
+// 10 KB window or with a non-ASCII byte before it (ply_parse's rules, which then refuse the file).
+bool ply_header_lines(const uint8_t *ply, size_t bytes, std::vector<std::vector<std::string>> &lines, size_t &data_off) {
+  const std::string head((const char *)ply, bytes < 10240 ? bytes : 10240);
+  const size_t end = head.find("end_header\n");
+  if (end == std::string::npos) return false;
+  for (size_t i = 0; i < end; ++i)
+    if ((uint8_t)head[i] >= 0x80) return false;
+  for (size_t line = 0; line < end;) {
+    size_t eol = head.find('\n', line);
+    if (eol == std::string::npos || eol > end) eol = end;
+    std::vector<std::string> tok;
+    for (size_t p = line;;) {
+      const size_t q = head.find(' ', p);
+      if (q == std::string::npos || q >= eol) { tok.push_back(head.substr(p, eol - p)); break; }
+      tok.push_back(head.substr(p, q - p));
+      p = q + 1;
+    }
+    lines.push_back(tok);
+    line = eol + 1;
+  }
+  data_off = end + 11;
+  return true;
+}
+// Elements in declaration order; false on a property before any element
+bool ply_elements(const std::vector<std::vector<std::string>> &lines, std::vector<PlyElement> &els) {
+  for (const auto &t : lines) {
+    if (t[0] == "element") {
+      PlyElement e;
+      e.name = t.size() > 1 ? t[1] : "";
+      const std::string cnt = t.size() > 2 ? t[2] : "";
+      e.counted = t.size() == 3 && !cnt.empty() && cnt.size() <= 10;
+      for (char ch : cnt) e.counted = e.counted && ch >= '0' && ch <= '9';
+      if (e.counted) e.count = std::stoull(cnt);
+      els.push_back(e);
+    } else if (t[0] == "property") {
+      if (els.empty()) return false;
+      PlyElement &e = els.back();
+      const std::string type = t.size() > 1 ? t[1] : "";
+      const int size = ply_type_size(type);
+      e.props.push_back({t.size() > 2 ? t[2] : "undefined", type, (int)e.stride, size});
+      e.stride += (uint32_t)size;
+    }
+  }
+  return true;
+}
+const PlyElement *ply_element(const std::vector<PlyElement> &els, const char *name) {
+  for (const auto &e : els)
+    if (e.name == name) return &e;
+  return nullptr;
+}
+}  // namespace
+
+bool ply_is_compressed(const uint8_t *ply, size_t bytes) {
+  std::vector<std::vector<std::string>> lines;
+  size_t data_off;
+  if (!ply_header_lines(ply, bytes, lines, data_off)) return false;
+  bool chunk = false, vertex = false, in_vertex = false, word_uint[4] = {false, false, false, false};
+  for (const auto &t : lines) {
+    if (t[0] == "element") {
+      in_vertex = t.size() > 1 && t[1] == "vertex";
+      chunk = chunk || (t.size() > 1 && t[1] == "chunk");
+      vertex = vertex || in_vertex;
+    } else if (t[0] == "property" && t.size() > 2) {
+      if (t[2] == "x") return false;  // by the reference's rule: the name is the third word
+      for (int k = 0; k < 4; ++k)
+        if (in_vertex && t[2] == kWordName[k]) word_uint[k] = t[1] == "uint";  // the last one wins
+    }
+  }
+  return chunk && vertex && word_uint[0] && word_uint[1] && word_uint[2] && word_uint[3];
+}
+
+int ply_parse_compressed(const uint8_t *ply, size_t bytes, PlyCompressedLayout &Z, uint32_t &n, std::string &err) {
+  memset(&Z, 0, sizeof(Z));
+  n = 0;
+  std::vector<std::vector<std::string>> lines;
+  std::vector<PlyElement> els;
+  size_t data_off = 0;
+  auto refuse = [&](const std::string &m) { err = "compressed .ply: " + m; return GS_ERR_INVALID; };
+  if (!ply_header_lines(ply, bytes, lines, data_off)) return refuse("unreadable header");
+  bool format = false;
+  for (const auto &t : lines) format = format || (t.size() == 3 && t[0] == "format" && t[1] == "binary_little_endian" && t[2] == "1.0");
+  if (!format) return refuse("the format must be binary_little_endian 1.0");
+  if (!ply_elements(lines, els)) return refuse("property before any element");
+  uint64_t body = data_off;
+  for (size_t i = 0; i < els.size(); ++i) {
+    const PlyElement &e = els[i];
+    if (!e.counted || e.count > 0xFFFFFFFFull) return refuse("element " + e.name + " needs a count below 2^32");
+    for (size_t j = 0; j < i; ++j)
+      if (els[j].name == e.name) return refuse("element " + e.name + " declared twice");
+    for (const auto &p : e.props)
+      if (!p.size) return refuse("element " + e.name + " has a list or unknown property type");
+    const int k = e.name == "chunk" ? 0 : e.name == "vertex" ? 1 : e.name == "sh" ? 2 : -1;
+    if (k >= 0) {
+      Z.body[k] = body;
+      Z.stride[k] = e.stride;
+    }
+    body += e.count * e.stride;  // < 2^32 * 2^17: no overflow
+  }
+  const PlyElement &C = *ply_element(els, "chunk"), &V = *ply_element(els, "vertex"), *S = ply_element(els, "sh");
+  if (C.count != (V.count + 255) / 256) return refuse("chunk count is not ceil(vertex count / 256)");
+  int colour = 0, colour_float = 0;
+  for (int b = 0; b < kPlyBounds; ++b) {
+    const PlyProp *p = C.find(kBoundName[b]);
+    const bool is_float = p && p->type == "float";
+    if (b < 12 && !is_float) return refuse(std::string("chunk needs float ") + kBoundName[b]);
+    if (b >= 12) {
+      colour += p ? 1 : 0;
+      colour_float += is_float ? 1 : 0;
+    }
+    Z.bound[b] = is_float ? p->off : -1;
+  }
+  if (colour && colour_float != 6) return refuse("chunk colour bounds need all six of min_r .. max_b as float");
+  Z.has_color = colour ? 1u : 0u;
+  for (int w = 0; w < 4; ++w) Z.word[w] = V.find(kWordName[w])->off;
+  if (S) {
+    if (S->count != V.count) return refuse("sh count is not the vertex count");
+    for (const auto &p : S->props)
+      if (p.name.compare(0, 7, "f_rest_") == 0 && p.type != "uchar") return refuse("sh property " + p.name + " is not uchar");
+    for (uint32_t d = 1; d <= 3; ++d) {
+      bool all = true;
+      for (uint32_t k = 0; k < 3 * sh_coeffs(d); ++k) all = all && S->find("f_rest_" + std::to_string(k));
+      if (all) Z.file_k = sh_coeffs(d);
+    }
+    for (uint32_t k = 0; k < 3 * Z.file_k; ++k) Z.rest[k] = S->find("f_rest_" + std::to_string(k))->off;
+  }
+  if (body > bytes) return refuse("body shorter than its elements");
+  n = (uint32_t)V.count;
+  return GS_OK;
+}
+
+uint32_t ply_compressed_piece_rows(uint32_t sh_k) {
+  // per 256 rows: one chunk row, 256 packed words, 256 * 3 sh_k SH bytes; 32 B for the two 16 B paddings
+  const size_t per_chunk = kPlyBounds * 4 + 256 * 16 + 256 * 3 * (size_t)sh_k;
+  return (uint32_t)((gs_context::kPlyChunkBytes - 32) / per_chunk) * 256u;
+}
+
+size_t ply_compressed_piece_bytes(uint32_t m, uint32_t sh_k) {
+  const size_t nch = (m + 255) / 256;
+  return ((nch * kPlyBounds * 4 + 15) & ~(size_t)15) + (size_t)m * 16 + (((size_t)m * 3 * sh_k + 15) & ~(size_t)15);
+}
+
+void ply_stage_compressed(const uint8_t *ply, const PlyCompressedLayout &Z, uint32_t sh_k, uint32_t r0, uint32_t m,
+                          uint8_t *dst) {
+  const uint32_t c0 = r0 / 256, nch = (m + 255) / 256;
+  float *bound = (float *)dst;
+  for (uint32_t c = 0; c < nch; ++c) {
+    const uint8_t *row = ply + Z.body[0] + (size_t)(c0 + c) * Z.stride[0];
+    for (int b = 0; b < kPlyBounds; ++b) {
+      float v = 0.0f;  // colour bounds of a file without them are never read
+      if (Z.bound[b] >= 0) memcpy(&v, row + Z.bound[b], 4);
+      bound[(size_t)c * kPlyBounds + b] = v;
+    }
+  }
+  uint8_t *words = dst + (((size_t)nch * kPlyBounds * 4 + 15) & ~(size_t)15);
+  const uint8_t *vsrc = ply + Z.body[1] + (size_t)r0 * Z.stride[1];
+  if (Z.stride[1] == 16 && Z.word[0] == 0 && Z.word[1] == 4 && Z.word[2] == 8 && Z.word[3] == 12) {
+    memcpy(words, vsrc, (size_t)m * 16);  // SuperSplat's layout
+  } else {
+    for (uint32_t i = 0; i < m; ++i)
+      for (int w = 0; w < 4; ++w) memcpy(words + (size_t)i * 16 + 4 * w, vsrc + (size_t)i * Z.stride[1] + Z.word[w], 4);
+  }
+  if (!sh_k) return;
+  uint8_t *sh = words + (size_t)m * 16;
+  const uint32_t nb = 3 * sh_k;
+  const uint8_t *ssrc = ply + Z.body[2] + (size_t)r0 * Z.stride[2];
+  bool plain = Z.stride[2] == nb;
+  for (uint32_t k = 0; k < nb; ++k) plain = plain && Z.rest[k] == (int32_t)k;
+  if (plain) {
+    memcpy(sh, ssrc, (size_t)m * nb);
+  } else {
+    for (uint32_t i = 0; i < m; ++i)
+      for (uint32_t k = 0; k < nb; ++k) sh[(size_t)i * nb + k] = ssrc[(size_t)i * Z.stride[2] + Z.rest[k]];
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // decode (device)
 // ---------------------------------------------------------------------------------------------
@@ -162,6 +374,8 @@ __device__ __forceinline__ double ply_get(const uint8_t *row, const PlyField f) 
   }
 }
 
+constexpr double kShC0 = 0.28209479177387814;  // index.js:728
+
 // Float32Array store (round to nearest even; NaN as the host's quiet NaN)
 __device__ __forceinline__ uint32_t f32_bits(double v) {
   return isnan(v) ? 0x7FC00000u : __float_as_uint(__double2float_rn(v));
@@ -183,36 +397,38 @@ __device__ __forceinline__ uint32_t sh_half(const uint8_t *row, const PlyShLayou
   return (uint32_t)__half_as_ushort(__float2half_rn(v));
 }
 
-template <bool kF32, bool kSH>
-__global__ void __launch_bounds__(256) k_ply_decode(const uint8_t *__restrict__ chunk, uint32_t rows, PlyLayout L,
-                                                    uint32_t first_row, uint4 *__restrict__ rows32,
-                                                    uint32_t *__restrict__ key_out, const PlyShLayout S,
-                                                    uint4 *__restrict__ sh_rows) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= rows) return;
-  const uint8_t *row = chunk + (size_t)i * L.stride;
-  if (kSH) {
-    const uint32_t nh = 3 * S.ctx_k;
-    uint4 *dst = sh_rows + (size_t)(first_row + i) * S.vecs;
-    for (uint32_t v = 0; v < S.vecs; ++v) {
-      uint32_t w[4];
+// The SH words of table row o: coefficient h (channel-major, h < 3 ctx_k) is half(h) as fp16 bits; the padding stays 0
+template <class Half>
+__device__ __forceinline__ void ply_store_sh(const Half &half, const PlyShLayout &S, uint32_t o, uint4 *__restrict__ sh_rows) {
+  const uint32_t nh = 3 * S.ctx_k;
+  uint4 *dst = sh_rows + (size_t)o * S.vecs;
+  for (uint32_t v = 0; v < S.vecs; ++v) {
+    uint32_t w[4];
 #pragma unroll
-      for (uint32_t q = 0; q < 4; ++q) {
-        const uint32_t h = v * 8 + q * 2;  // halves h (low) and h + 1 (high) of word q; the padding stays 0
-        w[q] = (h < nh ? sh_half<kF32>(row, S, h) : 0u) | ((h + 1 < nh ? sh_half<kF32>(row, S, h + 1) : 0u) << 16);
-      }
-      dst[v] = make_uint4(w[0], w[1], w[2], w[3]);
+    for (uint32_t q = 0; q < 4; ++q) {
+      const uint32_t h = v * 8 + q * 2;  // halves h (low) and h + 1 (high) of word q
+      w[q] = (h < nh ? half(h) : 0u) | ((h + 1 < nh ? half(h + 1) : 0u) << 16);
     }
+    dst[v] = make_uint4(w[0], w[1], w[2], w[3]);
   }
+}
+
+// processPlyBuffer's conversion of one row (index.js:653-742) into table row o's 32-byte .splat row and importance key.
+// get(PF_*): a property the row has, as a JS number; px, py, pz: the f32 bits of x, y, z; has_*: whether the file has
+// scale_0 / f_dc_0 / opacity.
+template <class Get>
+__device__ __forceinline__ void ply_convert_row(const Get &get, uint32_t px, uint32_t py, uint32_t pz, bool has_scale, bool has_fdc,
+                                                bool has_opacity, uint32_t o, uint4 *__restrict__ rows32,
+                                                uint32_t *__restrict__ key_out) {
   uint32_t scale[3], rot;
   uint32_t key = 0u;  // every key is 0 without scale_0: sizeList stays zero-filled (index.js:659-660)
-  if (L.has_scale) {
-    const double e0 = exp(ply_get<kF32>(row, L.f[PF_S0]));
-    const double e1 = exp(ply_get<kF32>(row, L.f[PF_S1]));
-    const double e2 = exp(ply_get<kF32>(row, L.f[PF_S2]));
+  if (has_scale) {
+    const double e0 = exp(get(PF_S0));
+    const double e1 = exp(get(PF_S1));
+    const double e2 = exp(get(PF_S2));
     // index.js:661-665: importance, stored as f32
     const double size = e0 * e1 * e2;
-    const double opacity = 1.0 / (1.0 + exp(-ply_get<kF32>(row, L.f[PF_OP])));
+    const double opacity = 1.0 / (1.0 + exp(-get(PF_OP)));
     const double imp = size * opacity;
     if (isnan(imp)) {
       key = 0xFFFFFFFFu;  // after every number
@@ -223,8 +439,8 @@ __global__ void __launch_bounds__(256) k_ply_decode(const uint8_t *__restrict__ 
       key = ~asc;                                                        // ascending with -value
     }
     // index.js:697-709
-    const double r0 = ply_get<kF32>(row, L.f[PF_R0]), r1 = ply_get<kF32>(row, L.f[PF_R1]);
-    const double r2 = ply_get<kF32>(row, L.f[PF_R2]), r3 = ply_get<kF32>(row, L.f[PF_R3]);
+    const double r0 = get(PF_R0), r1 = get(PF_R1);
+    const double r2 = get(PF_R2), r3 = get(PF_R3);
     const double qlen = sqrt(r0 * r0 + r1 * r1 + r2 * r2 + r3 * r3);
     rot = js_store_u8_clamped((r0 / qlen) * 128.0 + 128.0) | (js_store_u8_clamped((r1 / qlen) * 128.0 + 128.0) << 8) |
           (js_store_u8_clamped((r2 / qlen) * 128.0 + 128.0) << 16) | (js_store_u8_clamped((r3 / qlen) * 128.0 + 128.0) << 24);
@@ -236,6 +452,32 @@ __global__ void __launch_bounds__(256) k_ply_decode(const uint8_t *__restrict__ 
     scale[0] = scale[1] = scale[2] = __float_as_uint(0.01f);
     rot = 255u;
   }
+  // index.js:725-737
+  uint32_t rgba;
+  if (has_fdc) {
+    rgba = js_store_u8_clamped((0.5 + kShC0 * get(PF_DC0)) * 255.0) |
+           (js_store_u8_clamped((0.5 + kShC0 * get(PF_DC1)) * 255.0) << 8) |
+           (js_store_u8_clamped((0.5 + kShC0 * get(PF_DC2)) * 255.0) << 16);
+  } else {
+    rgba = js_store_u8_clamped(get(PF_RED)) | (js_store_u8_clamped(get(PF_GREEN)) << 8) |
+           (js_store_u8_clamped(get(PF_BLUE)) << 16);
+  }
+  const uint32_t alpha = has_opacity ? js_store_u8_clamped((1.0 / (1.0 + exp(-get(PF_OP)))) * 255.0) : 255u;
+  rgba |= alpha << 24;
+  rows32[2 * (size_t)o] = make_uint4(px, py, pz, scale[0]);
+  rows32[2 * (size_t)o + 1] = make_uint4(scale[1], scale[2], rgba, rot);
+  key_out[o] = key;
+}
+
+template <bool kF32, bool kSH>
+__global__ void __launch_bounds__(256) k_ply_decode(const uint8_t *__restrict__ chunk, uint32_t rows, PlyLayout L,
+                                                    uint32_t first_row, uint4 *__restrict__ rows32,
+                                                    uint32_t *__restrict__ key_out, const PlyShLayout S,
+                                                    uint4 *__restrict__ sh_rows) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows) return;
+  const uint8_t *row = chunk + (size_t)i * L.stride;
+  if (kSH) ply_store_sh([&](uint32_t h) { return sh_half<kF32>(row, S, h); }, S, first_row + i, sh_rows);
   // index.js:721-723: a float property is stored bit for bit
   uint32_t pos[3];
   for (int k = 0; k < 3; ++k) {
@@ -243,23 +485,78 @@ __global__ void __launch_bounds__(256) k_ply_decode(const uint8_t *__restrict__ 
     pos[k] = kF32 ? __ldg((const uint32_t *)(row + f.off))
                   : (f.kind == PK_F32 ? ld_u32(row + f.off) : f32_bits(ply_get<false>(row, f)));
   }
-  // index.js:725-737
-  uint32_t rgba;
-  if (L.has_fdc) {
-    const double SH_C0 = 0.28209479177387814;
-    rgba = js_store_u8_clamped((0.5 + SH_C0 * ply_get<kF32>(row, L.f[PF_DC0])) * 255.0) |
-           (js_store_u8_clamped((0.5 + SH_C0 * ply_get<kF32>(row, L.f[PF_DC1])) * 255.0) << 8) |
-           (js_store_u8_clamped((0.5 + SH_C0 * ply_get<kF32>(row, L.f[PF_DC2])) * 255.0) << 16);
-  } else {
-    rgba = js_store_u8_clamped(ply_get<kF32>(row, L.f[PF_RED])) | (js_store_u8_clamped(ply_get<kF32>(row, L.f[PF_GREEN])) << 8) |
-           (js_store_u8_clamped(ply_get<kF32>(row, L.f[PF_BLUE])) << 16);
+  ply_convert_row([&](int k) { return ply_get<kF32>(row, L.f[k]); }, pos[0], pos[1], pos[2], L.has_scale, L.has_fdc, L.has_opacity,
+                  first_row + i, rows32, key_out);
+}
+
+// ---- compressed PLY: each property in fp64, rounded once to f32, then the conversion above (DESIGN.md section 3) ----
+// An sh byte u is the centre of the exporter's bucket trunc((f / 8 + 0.5) * 256) clamped to [0, 255]: a multiple of 1/64 in
+// [-4, 4), exact in f32 and fp16.  This decode is the project's definition; ply.py's sh_byte_value states it for the host.
+__device__ __forceinline__ double ply_sh_byte(uint32_t u) { return ((u + 0.5) / 256.0 - 0.5) * 8.0; }
+__device__ __forceinline__ double ply_lerp(float a, float b, double t) { return (double)a + ((double)b - (double)a) * t; }
+__device__ __forceinline__ double ply_f32(double v) { return (double)__double2float_rn(v); }
+
+template <bool kSH>
+__global__ void __launch_bounds__(256) k_ply_decode_compressed(const uint8_t *__restrict__ piece, uint32_t rows,
+                                                               uint32_t has_color, uint32_t file_k, uint32_t first_row,
+                                                               uint4 *__restrict__ rows32, uint32_t *__restrict__ key_out,
+                                                               const PlyShLayout S, uint4 *__restrict__ sh_rows) {
+  __shared__ float s_bound[kPlyBounds];
+  __shared__ uint4 s_sh[kSH ? 256 * 3 * kMaxShCoeffs / 16 : 1];
+  const uint32_t nch = (rows + 255) / 256, base = blockIdx.x * 256, i = base + threadIdx.x;
+  const size_t words_off = ((size_t)nch * kPlyBounds * 4 + 15) & ~(size_t)15;
+  if (threadIdx.x < kPlyBounds) s_bound[threadIdx.x] = ((const float *)piece)[(size_t)blockIdx.x * kPlyBounds + threadIdx.x];
+  if (kSH) {  // this chunk's SH bytes, coalesced 16 B loads (the piece pads its end to 16 B)
+    const uint32_t nb = 3 * file_k, nvec = (min(256u, rows - base) * nb + 15) / 16;
+    const uint4 *src = (const uint4 *)(piece + words_off + (size_t)rows * 16 + (size_t)base * nb);
+    for (uint32_t v = threadIdx.x; v < nvec; v += 256) s_sh[v] = src[v];
   }
-  const uint32_t alpha = L.has_opacity ? js_store_u8_clamped((1.0 / (1.0 + exp(-ply_get<kF32>(row, L.f[PF_OP])))) * 255.0) : 255u;
-  rgba |= alpha << 24;
-  const uint32_t o = first_row + i;
-  rows32[2 * (size_t)o] = make_uint4(pos[0], pos[1], pos[2], scale[0]);
-  rows32[2 * (size_t)o + 1] = make_uint4(scale[1], scale[2], rgba, rot);
-  key_out[o] = key;
+  __syncthreads();
+  if (i >= rows) return;
+  const uint4 w = ((const uint4 *)(piece + words_off))[i];
+  const float *b = s_bound;
+  if (kSH) {
+    const uint8_t *u = (const uint8_t *)s_sh + (size_t)threadIdx.x * 3 * file_k;
+    ply_store_sh([&](uint32_t h) {
+      const uint32_t c = h / S.ctx_k, k = h - c * S.ctx_k;
+      if (k >= file_k) return 0u;
+      return (uint32_t)__half_as_ushort(__float2half_rn(__double2float_rn(ply_sh_byte(u[c * file_k + k]))));
+    }, S, first_row + i, sh_rows);
+  }
+  double v[PF_COUNT];
+  // packed_position / packed_scale: 11, 10, 11 bits of (x, y, z) between the chunk's min and max
+  uint32_t pos[3];
+  pos[0] = f32_bits(ply_lerp(b[0], b[3], (double)(w.x >> 21) / 2047.0));
+  pos[1] = f32_bits(ply_lerp(b[1], b[4], (double)((w.x >> 11) & 1023u) / 1023.0));
+  pos[2] = f32_bits(ply_lerp(b[2], b[5], (double)(w.x & 2047u) / 2047.0));
+  v[PF_S0] = ply_f32(ply_lerp(b[6], b[9], (double)(w.z >> 21) / 2047.0));
+  v[PF_S1] = ply_f32(ply_lerp(b[7], b[10], (double)((w.z >> 11) & 1023u) / 1023.0));
+  v[PF_S2] = ply_f32(ply_lerp(b[8], b[11], (double)(w.z & 2047u) / 2047.0));
+  // packed_rotation: the three smallest components in 10 bits each, the largest (index v >> 30) from the unit norm
+  const double norm = 1.0 / (sqrt(2.0) * 0.5);
+  const double qa = ((double)((w.y >> 20) & 1023u) / 1023.0 - 0.5) * norm;
+  const double qb = ((double)((w.y >> 10) & 1023u) / 1023.0 - 0.5) * norm;
+  const double qc = ((double)(w.y & 1023u) / 1023.0 - 0.5) * norm;
+  const double qm = sqrt(1.0 - (qa * qa + qb * qb + qc * qc));  // NaN above a unit sum: rot bytes 0, as processPlyBuffer
+  const uint32_t big = w.y >> 30;
+  const double qx = big == 0 ? qm : qa, qy = big == 0 ? qa : big == 1 ? qm : qb;
+  const double qz = big <= 1 ? qb : big == 2 ? qm : qc, qw = big == 3 ? qm : qc;
+  v[PF_R0] = ply_f32(qw);
+  v[PF_R1] = ply_f32(qx);
+  v[PF_R2] = ply_f32(qy);
+  v[PF_R3] = ply_f32(qz);
+  // packed_color: 8-bit r, g, b (between the chunk's colour bounds when it has them) and alpha
+  double cr = (double)(w.w >> 24) / 255.0, cg = (double)((w.w >> 16) & 255u) / 255.0, cb = (double)((w.w >> 8) & 255u) / 255.0;
+  if (has_color) {
+    cr = ply_lerp(b[12], b[15], cr);
+    cg = ply_lerp(b[13], b[16], cg);
+    cb = ply_lerp(b[14], b[17], cb);
+  }
+  v[PF_DC0] = ply_f32((cr - 0.5) / kShC0);
+  v[PF_DC1] = ply_f32((cg - 0.5) / kShC0);
+  v[PF_DC2] = ply_f32((cb - 0.5) / kShC0);
+  v[PF_OP] = ply_f32(-log(1.0 / ((double)(w.w & 255u) / 255.0) - 1.0));
+  ply_convert_row([&](int k) { return v[k]; }, pos[0], pos[1], pos[2], true, true, true, first_row + i, rows32, key_out);
 }
 
 void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,
@@ -271,6 +568,18 @@ void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, 
   auto kernel = L.all_f32 ? (sh ? k_ply_decode<true, true> : k_ply_decode<true, false>)
                           : (sh ? k_ply_decode<false, true> : k_ply_decode<false, false>);
   kernel<<<grid, 256, 0, st>>>(chunk, rows, L, first_row, (uint4 *)rows32, key, S, sh_rows);
+}
+
+void launch_ply_decode_compressed(const uint8_t *piece, uint32_t rows, const PlyCompressedLayout &Z, uint32_t first_row,
+                                  uint8_t *rows32, uint32_t *key, const PlyShLayout *sh, uint4 *sh_rows, cudaStream_t st) {
+  if (!rows) return;
+  const uint32_t grid = (rows + 255) / 256;  // one CTA per chunk row
+  if (sh)
+    k_ply_decode_compressed<true><<<grid, 256, 0, st>>>(piece, rows, Z.has_color, Z.file_k, first_row, (uint4 *)rows32,
+                                                         key, *sh, sh_rows);
+  else
+    k_ply_decode_compressed<false><<<grid, 256, 0, st>>>(piece, rows, Z.has_color, 0u, first_row, (uint4 *)rows32, key,
+                                                          PlyShLayout{}, nullptr);
 }
 
 }  // namespace gs

@@ -8,6 +8,7 @@ importance (stable), Uint8ClampedArray stores (clamp, round half to even, NaN ->
 """
 from __future__ import annotations
 
+import math
 import re
 
 import numpy as np
@@ -147,6 +148,182 @@ def sh_coefficients(input_buffer: bytes, degree: int) -> np.ndarray:
         imp = (size * (1.0 / (1.0 + np.exp(-field("opacity"))))).astype(np.float32)
         out = out[np.argsort(-imp.astype(np.float64), kind="stable")]
     return out
+
+
+_BOUNDS = ("min_x", "min_y", "min_z", "max_x", "max_y", "max_z", "min_scale_x", "min_scale_y", "min_scale_z",
+           "max_scale_x", "max_scale_y", "max_scale_z", "min_r", "min_g", "min_b", "max_r", "max_g", "max_b")
+_WORDS = ("packed_position", "packed_rotation", "packed_scale", "packed_color")
+_SIZES = {"double": 8, "int": 4, "uint": 4, "float": 4, "short": 2, "ushort": 2, "uchar": 1}
+
+
+def sh_byte_value(u):
+    """The f_rest value of a compressed PLY's sh byte u: the centre of the exporter's bucket
+    trunc((f / 8 + 0.5) * 256) clamped to [0, 255], a multiple of 1/64 in [-4, 4).  This is the project's definition
+    (gs_ply.cu's ply_sh_byte states it for the device)."""
+    return ((np.asarray(u, np.float64) + 0.5) / 256.0 - 0.5) * 8.0
+
+
+def _header_lines(blob: bytes):
+    """The header's lines split by single spaces and the body's offset, or None without "end_header\\n" in the 10 KB
+    window or with a non-ASCII byte before it (process_ply_buffer's rules, which then refuse the file)."""
+    head = bytes(blob[:1024 * 10])
+    end = head.find(b"end_header\n")
+    if end < 0 or any(b >= 0x80 for b in head[:end]):
+        return None
+    return [line.split(" ") for line in head[:end].decode("ascii").split("\n")], end + 11
+
+
+def is_compressed_ply(blob) -> bool:
+    """Whether gs_push_ply decodes `blob` as a compressed PLY (SuperSplat's export): the header declares element chunk
+    and element vertex, the vertex element has uint packed_position, packed_rotation, packed_scale and packed_color, and
+    no property is named x (every file process_ply_buffer accepts has one)."""
+    parsed = _header_lines(blob)
+    if parsed is None:
+        return False
+    chunk = vertex = in_vertex = False
+    word_uint = {}
+    for t in parsed[0]:
+        if t[0] == "element":
+            in_vertex = len(t) > 1 and t[1] == "vertex"
+            chunk = chunk or (len(t) > 1 and t[1] == "chunk")
+            vertex = vertex or in_vertex
+        elif t[0] == "property" and len(t) > 2:
+            if t[2] == "x":
+                return False
+            if in_vertex and t[2] in _WORDS:
+                word_uint[t[2]] = t[1] == "uint"  # the last one wins
+    return chunk and vertex and all(word_uint.get(w, False) for w in _WORDS)
+
+
+def _parse_compressed(blob: bytes):
+    """The header of a compressed PLY -> {element: (body offset, count, {name: (offset, type)}, stride)}, file_k; the
+    rules and messages of gs_push_ply (ValueError)."""
+    def refuse(m):
+        raise ValueError("compressed .ply: " + m)
+
+    lines, data_off = _header_lines(blob)
+    if not any(t == ["format", "binary_little_endian", "1.0"] for t in lines):
+        refuse("the format must be binary_little_endian 1.0")
+    els = []  # [name, count or None, [(name, type, offset, size)], stride]
+    for t in lines:
+        if t[0] == "element":
+            cnt = t[2] if len(t) > 2 else ""
+            ok = len(t) == 3 and 0 < len(cnt) <= 10 and all("0" <= ch <= "9" for ch in cnt)
+            els.append([t[1] if len(t) > 1 else "", int(cnt) if ok else None, [], 0])
+        elif t[0] == "property":
+            if not els:
+                refuse("property before any element")
+            e = els[-1]
+            typ = t[1] if len(t) > 1 else ""
+            size = _SIZES.get(typ, 0)
+            e[2].append((t[2] if len(t) > 2 else "undefined", typ, e[3], size))
+            e[3] += size
+    out, body = {}, data_off
+    for i, (name, count, props, stride) in enumerate(els):
+        if count is None or count > 0xFFFFFFFF:
+            refuse(f"element {name} needs a count below 2^32")
+        if any(els[j][0] == name for j in range(i)):
+            refuse(f"element {name} declared twice")
+        if any(p[3] == 0 for p in props):
+            refuse(f"element {name} has a list or unknown property type")
+        out[name] = (body, count, {p[0]: (p[2], p[1]) for p in props}, stride)  # the last property of a name wins
+        body += count * stride
+    n = out["vertex"][1]
+    chunk = out["chunk"]
+    if chunk[1] != (n + 255) // 256:
+        refuse("chunk count is not ceil(vertex count / 256)")
+    for b in _BOUNDS[:12]:
+        if chunk[2].get(b, (0, ""))[1] != "float":
+            refuse("chunk needs float " + b)
+    colour = [chunk[2].get(b, (0, None))[1] for b in _BOUNDS[12:]]
+    if any(t is not None for t in colour) and not all(t == "float" for t in colour):
+        refuse("chunk colour bounds need all six of min_r .. max_b as float")
+    file_k = 0
+    if "sh" in out:
+        sh = out["sh"]
+        if sh[1] != n:
+            refuse("sh count is not the vertex count")
+        for p in next(e for e in els if e[0] == "sh")[2]:
+            if p[0].startswith("f_rest_") and p[1] != "uchar":
+                refuse(f"sh property {p[0]} is not uchar")
+        for d in (1, 2, 3):
+            k = (d + 1) ** 2 - 1
+            if all(f"f_rest_{i}" in sh[2] for i in range(3 * k)):
+                file_k = k
+    if body > len(blob):
+        refuse("body shorter than its elements")
+    return out, file_k
+
+
+def _column(blob, el, name, typ):
+    body, count, props, stride = el
+    off = props[name][0]
+    raw = np.frombuffer(blob, np.uint8, count=count * stride, offset=body).reshape(count, stride)
+    return np.ascontiguousarray(raw[:, off:off + np.dtype(typ).itemsize]).view(typ).reshape(count)
+
+
+def _f32(v: np.ndarray) -> np.ndarray:
+    """fp64 -> f32, rounded once; every NaN the device's 0x7FC00000."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        out = np.asarray(v, np.float64).astype(np.float32)
+    out.view(np.uint32)[np.isnan(out)] = 0x7FC00000
+    return out
+
+
+def decompress_ply(blob) -> bytes:
+    """A compressed PLY (is_compressed_ply) -> the INRIA float PLY gs_push_ply decodes it to: x y z, f_dc_*, f_rest_*
+    when the file has an sh element of degree >= 1, opacity, scale_*, rot_*, each computed in fp64 and rounded once to
+    f32 (NaN as 0x7FC00000).  Splat i uses chunk row i // 256 and lerp(a, b, t) = a + (b - a) * t of its f32 bounds:
+    packed_position / packed_scale hold 11, 10, 11 bits of x, y, z (scale_* are log scales); packed_rotation the three
+    smallest quaternion components in 10 bits each, ((q / 1023) - 0.5) / (sqrt(2) * 0.5), and in its top 2 bits the
+    place of the largest, sqrt(1 - a^2 - b^2 - c^2); packed_color r, g, b, alpha in 8 bits each (r, g, b between the
+    chunk's colour bounds when it has them), f_dc = (c - 0.5) / SH_C0, opacity = -log(1 / alpha - 1); an sh byte u is
+    sh_byte_value(u).  Raises ValueError with gs_push_ply's message for a malformed file."""
+    blob = bytes(blob)
+    if not is_compressed_ply(blob):
+        raise ValueError("not a compressed .ply")
+    els, file_k = _parse_compressed(blob)
+    n = els["vertex"][1]
+    chunk, vert = els["chunk"], els["vertex"]
+    bnd = np.stack([_column(blob, chunk, b, "<f4") if b in chunk[2] else np.zeros(chunk[1], np.float32)
+                    for b in _BOUNDS], axis=1).astype(np.float64)[np.arange(n) // 256]
+    has_color = "min_r" in chunk[2]
+    w = {k: _column(blob, vert, k, "<u4").astype(np.uint64) for k in _WORDS}
+
+    def lerp(j, t):  # inf / NaN bounds give inf / NaN
+        with np.errstate(invalid="ignore"):
+            return bnd[:, j] + (bnd[:, j + 3] - bnd[:, j]) * t
+
+    def unpack111011(v, j):
+        return [lerp(j, (v >> 21).astype(np.float64) / 2047.0), lerp(j + 1, ((v >> 11) & 1023).astype(np.float64) / 1023.0),
+                lerp(j + 2, (v & 2047).astype(np.float64) / 2047.0)]
+
+    xyz = np.stack([_f32(c) for c in unpack111011(w["packed_position"], 0)], axis=1)
+    scale = np.stack([_f32(c) for c in unpack111011(w["packed_scale"], 6)], axis=1)
+    r = w["packed_rotation"]
+    norm = 1.0 / (math.sqrt(2.0) * 0.5)
+    a, b, c = [((r >> s & 1023).astype(np.float64) / 1023.0 - 0.5) * norm for s in (20, 10, 0)]
+    with np.errstate(invalid="ignore"):
+        m = np.sqrt(1.0 - (a * a + b * b + c * c))
+    big = (r >> 30).astype(np.int64)
+    qx = np.where(big == 0, m, a)
+    qy = np.where(big == 0, a, np.where(big == 1, m, b))
+    qz = np.where(big <= 1, b, np.where(big == 2, m, c))
+    qw = np.where(big == 3, m, c)
+    rot = np.stack([_f32(qw), _f32(qx), _f32(qy), _f32(qz)], axis=1)
+    col = w["packed_color"]
+    rgb = [((col >> s) & 255).astype(np.float64) / 255.0 for s in (24, 16, 8)]
+    if has_color:
+        rgb = [lerp(12 + k, rgb[k]) for k in range(3)]
+    f_dc = np.stack([_f32((v - 0.5) / SH_C0) for v in rgb], axis=1)
+    alpha = (col & 255).astype(np.float64) / 255.0
+    with np.errstate(divide="ignore"):
+        opacity = _f32(-np.log(1.0 / alpha - 1.0))
+    f_rest = None
+    if file_k:
+        f_rest = np.stack([_f32(sh_byte_value(_column(blob, els["sh"], f"f_rest_{k}", "u1")))
+                           for k in range(3 * file_k)], axis=1)
+    return write_inria_ply(None, xyz, f_dc, opacity, scale, rot, n_rest=3 * file_k, f_rest=f_rest)
 
 
 def write_inria_ply(path_or_none, xyz, f_dc, opacity, scale_log, rot, n_rest: int = 45, f_rest=None) -> bytes:

@@ -162,6 +162,37 @@ GS_API int gs_push_splats(gs_context *ctx, const void *rows32, uint32_t n);
  * conversion reads is missing ("<name> not found": x/y/z; rot_*, scale_1/2 and opacity when scale_0 exists;
  * f_dc_1/2 when f_dc_0 exists, else red/green/blue); a body shorter than N rows.  A header with a non-ASCII byte before
  * end_header is also refused (the reference would read its body at a shifted offset).
+ *
+ * Compressed PLY files (SuperSplat's export, e.g. scene.compressed.ply) take their own path, chosen from the header in
+ * the same 10 KB window: a header that declares `element chunk C` and `element vertex N`, whose vertex element has the
+ * uint properties packed_position, packed_rotation, packed_scale and packed_color, and that declares no property named x
+ * anywhere.  The reference refuses every such file (x is required), so every file it reads decodes as before.
+ *   Header rules (offsets restart in every element; a violation returns GS_ERR_INVALID, the message in quotes, prefixed
+ *   "compressed .ply: ", and leaves the table unchanged):
+ *     - a line `format binary_little_endian 1.0` ("the format must be binary_little_endian 1.0");
+ *     - no property before the first element ("property before any element"); every element has a count below 2^32
+ *       ("element <name> needs a count below 2^32") and a name used once ("element <name> declared twice");
+ *     - element bodies follow one another in declaration order, count x stride each; any element may carry extra scalar
+ *       properties of the TYPE_MAP types, counted in its stride and otherwise ignored; a list or unknown type is refused
+ *       ("element <name> has a list or unknown property type");
+ *     - chunk: C == ceil(N / 256) ("chunk count is not ceil(vertex count / 256)"); float min_x min_y min_z max_x max_y
+ *       max_z min_scale_x .. min_scale_z max_scale_x .. max_scale_z ("chunk needs float <name>"); optional float
+ *       min_r min_g min_b max_r max_g max_b, all six or none ("chunk colour bounds need all six of min_r .. max_b as float");
+ *     - sh (optional): count N ("sh count is not the vertex count"), f_rest_* all uchar ("sh property <name> is not
+ *       uchar"); its degree is the largest d whose f_rest_0 .. f_rest_{3 K(d) - 1} exist;
+ *     - a body shorter than the elements declare ("body shorter than its elements").  N == 0 inserts nothing.
+ *   Decode: the rows, table and SH coefficients are exactly those of the INRIA float PLY that this writes, each property
+ *   computed in fp64 and rounded once to f32 (ply.decompress_ply writes that file).  Splat i uses chunk row i >> 8 and
+ *   lerp(a, b, t) = a + (b - a) t of the chunk's f32 bounds:
+ *     - packed_position v: x = lerp(min_x, max_x, (v >> 21) / 2047), y = lerp(min_y, max_y, ((v >> 11) & 1023) / 1023),
+ *       z = lerp(min_z, max_z, (v & 2047) / 2047); packed_scale likewise gives scale_0..2 (log scales);
+ *     - packed_rotation v: a, b, c = (((v >> 20, >> 10, >> 0) & 1023) / 1023 - 0.5) / (sqrt(2) 0.5), m = sqrt(1 - (a a +
+ *       b b + c c)) (NaN above a unit sum: rot bytes 0); v >> 30 = 0, 1, 2, 3 gives (x, y, z, w) = (m,a,b,c), (a,m,b,c),
+ *       (a,b,m,c), (a,b,c,m); rot_0 = w, rot_1 = x, rot_2 = y, rot_3 = z;
+ *     - packed_color v: r, g, b, alpha = bytes 3, 2, 1, 0 of v over 255; with colour bounds r = lerp(min_r, max_r, r)
+ *       and likewise g, b (never alpha); f_dc_k = (c_k - 0.5) / SH_C0; opacity = -log(1 / alpha - 1) (+-inf at 1 and 0);
+ *     - sh byte u: f_rest = ((u + 0.5) / 256 - 0.5) 8, the centre of the exporter's bucket trunc((f / 8 + 0.5) 256)
+ *       clamped to [0, 255].  No published file pins this rule down; it is this library's definition.
  */
 GS_API int gs_push_ply(gs_context *ctx, const void *ply, size_t bytes, void *rows32_out_or_null, uint32_t *out_n);
 /*
@@ -237,7 +268,9 @@ GS_API int gs_read_packed(gs_context *ctx, uint32_t first, uint32_t n, float *ce
  *       f_rest_{c K_f + k - 1}: its typed value rounded to f32, then to fp16 (round to nearest even); every NaN is stored
  *       as 0x7FFF, whatever its sign and payload.  A file above the
  *       context's degree has its extra coefficients dropped, one below it has the missing ones 0.  The coefficients follow
- *       their rows through the importance order.  Header rules, messages and rows32_out are unchanged.
+ *       their rows through the importance order.  Header rules, messages and rows32_out are unchanged.  A compressed PLY's
+ *       coefficients are those of its float restatement (gs_push_ply): its sh element's bytes decoded to multiples of
+ *       1/64 in [-4, 4), exact in fp16.
  *     - gs_push_splats / gs_insert_splats / gs_push_packed rows have zero coefficients.
  *   Every frame of such a context (plain, stereo, scene, views, target, slab, sharded, GS_RENDER_BLEND_UNORM8, STATS) draws
  *   each splat in its view-dependent colour, per view: with cam the camera position of the splat's gsModelViewMatrix in the
