@@ -328,11 +328,18 @@ class SplatScene:
     several entities build the table that loading them one after another builds.  A component's clear() (loadData)
     erases only its own range on the device (gs_erase); the emptied entity goes to the end of the table, where its next
     rows append.  No row is kept on the host.
+
+    interleave=True (GS_RENDER_SCENE_INTERLEAVE) draws every entity's splats in one back-to-front order instead, so an
+    object placed inside or behind another splat entity blends with it by depth; picks then report the nearer entity.
+    It applies to render, render_into, render_xr, render_xr_layer, render_xr_views, pick and raycast.
     """
 
-    def __init__(self, renderer: Optional[SplatContext] = None, device: int = 0, sh_degree: int = 0):
+    def __init__(self, renderer: Optional[SplatContext] = None, device: int = 0, sh_degree: int = 0,
+                 interleave: bool = False):
         """sh_degree 1..3: .ply entities keep their spherical harmonics and draw their view-dependent colour (each view
-        from its own camera); 0 draws the reference's flat colour.  A given renderer takes the degree while it is empty."""
+        from its own camera); 0 draws the reference's flat colour.  A given renderer takes the degree while it is empty.
+        interleave: one depth order over every entity (see the class)."""
+        self.interleave = bool(interleave)
         self.renderer = renderer or SplatContext(device, sh_degree=sh_degree)
         if renderer is not None and sh_degree:
             renderer.set_sh_degree(sh_degree)
@@ -420,12 +427,13 @@ class SplatScene:
             raise ValueError("SplatScene.render: no entity added")
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out,
-                                          blend_unorm8=blend_unorm8)
+                                          blend_unorm8=blend_unorm8, interleave=self.interleave)
 
     def pick(self, points, width: int, height: int, camera=None, depth_in: Optional[np.ndarray] = None):
         """What lies under pixels of the frame render() draws with these arguments (gs_pick_scene): for each (x, y) of
         `points` (frame pixels, row 0 = bottom) the splat where the pixel turns half opaque.  Returns one dict per point,
-        None where no splat is hit: `component` (the visible entity: later entities cover earlier ones), `index` (the
+        None where no splat is hit: `component` (the visible entity: later entities cover earlier ones, or with
+        interleave the entity of the splat where the merged order turns the pixel half opaque), `index` (the
         splat's row in that entity's range), `depth` (window depth of its quad), `alpha` (the pixel's final alpha) and
         `point` (the world position, fp64: the pixel centre at that depth unprojected through the entity's
         gsProjectionMatrix * gsModelViewMatrix to the table's frame, then taken by object3D.matrixWorld * diag(1, -1, 1, 1),
@@ -434,7 +442,7 @@ class SplatScene:
             raise ValueError("SplatScene.pick: no entity added")
         frame, objs = self.objects(width, height, camera)
         xy = np.ascontiguousarray(points, dtype=np.uint32).reshape(-1, 2)
-        splat, obj, depth, alpha = self.renderer.pick_scene(frame, objs, xy, depth_in=depth_in)
+        splat, obj, depth, alpha = self.renderer.pick_scene(frame, objs, xy, depth_in=depth_in, interleave=self.interleave)
         out = []
         for (x, y), s, k, d, a in zip(xy, splat, obj, depth, alpha):
             if k < 0:
@@ -483,7 +491,8 @@ class SplatScene:
         height = color.shape[0] - y if height is None else height
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene_target(frame, objs, color, depth, viewport=(x, y), fmt=fmt,
-                                                 blend_unorm8=blend_unorm8, write_depth=write_depth)
+                                                 blend_unorm8=blend_unorm8, write_depth=write_depth,
+                                                 interleave=self.interleave)
 
     def _xr_ratio(self) -> float:
         """The first entity's xrPixelRatio, 1 when it is not positive (the rule of render_xr)."""
@@ -535,7 +544,8 @@ class SplatScene:
         objs, views, view_mvs = self._xr_view_objects(view_cameras, [(w, h) for _, _, w, h in rects])
         xy = [c for x, y, _, _ in rects for c in (x, y)]
         return self.renderer.render_scene_views_target(views, objs, view_mvs, color, xy, depth, fmt=fmt,
-                                                       blend_unorm8=blend_unorm8, write_depth=write_depth)
+                                                       blend_unorm8=blend_unorm8, write_depth=write_depth,
+                                                       interleave=self.interleave)
 
     def render_xr_layer(self, eye_cameras, width: int, height: int, color: np.ndarray, depth: Optional[np.ndarray] = None,
                         fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False, write_depth: bool = False) -> np.ndarray:
@@ -552,7 +562,8 @@ class SplatScene:
         if color.shape[1] < 2 * w or color.shape[0] < h:
             raise ValueError(f"render_xr_layer: the layer must hold two {w} x {h} eyes side by side")
         return self.renderer.render_scene_stereo_target(eyes, objs, eye_mvs, color, depth, eye_xy=(0, 0, w, 0), fmt=fmt,
-                                                        blend_unorm8=blend_unorm8, write_depth=write_depth)
+                                                        blend_unorm8=blend_unorm8, write_depth=write_depth,
+                                                        interleave=self.interleave)
 
     def render_xr(self, eye_cameras, width: int, height: int, color_in=(None, None), depth_in=(None, None),
                   bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
@@ -568,4 +579,4 @@ class SplatScene:
             raise ValueError("SplatScene.render_xr: no entity added")
         _, objs, eyes, eye_mvs = self._xr_objects(eye_cameras, width, height)
         return self.renderer.render_scene_stereo(eyes, objs, eye_mvs, color_in=color_in, depth_in=depth_in, bg=bg, fmt=fmt,
-                                                 blend_unorm8=blend_unorm8)
+                                                 blend_unorm8=blend_unorm8, interleave=self.interleave)

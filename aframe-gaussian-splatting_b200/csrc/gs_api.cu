@@ -831,8 +831,10 @@ static void fill_sort_consts(SortConsts &sc, const float view[4], const float *c
 }
 
 // Validates a scene's entity list and builds its table in t: non-empty entities sorted by their first splat, each with
-// its view row, cutout, modelview and draw rank.  Returns the table's byte count in *bytes.
-static int build_scene_table(gs_context *c, const gs_object *objs, uint32_t n_objs, SceneTable &t, size_t *bytes) {
+// its view row, cutout, modelview and draw rank, and the order's mode (GS_RENDER_SCENE_INTERLEAVE).  Returns the table's
+// byte count in *bytes.
+static int build_scene_table(gs_context *c, const gs_object *objs, uint32_t n_objs, bool interleave, SceneTable &t,
+                             size_t *bytes) {
   if (!objs || n_objs == 0 || n_objs > (uint32_t)GS_MAX_OBJECTS)
     return fail(c, GS_ERR_INVALID, "scene: between 1 and GS_MAX_OBJECTS entities");
   std::vector<uint32_t> idx;
@@ -850,7 +852,8 @@ static int build_scene_table(gs_context *c, const gs_object *objs, uint32_t n_ob
   uint32_t rank_bits = 0;
   while ((1u << rank_bits) < n_objs) ++rank_bits;
   t.bucket_bits = 12u - rank_bits;
-  t.pad[0] = t.pad[1] = 0;
+  t.interleave = interleave ? 1u : 0u;
+  t.pad = 0;
   for (size_t j = 0; j < idx.size(); ++j) {
     const gs_object &g = objs[idx[j]];
     SceneObject &o = t.obj[j];
@@ -927,7 +930,7 @@ static int sort_only(gs_context *c, const float *view, const float *cutout, cons
   GS_CUDA(c, cudaEventRecord(c->ev[0], c->stream));
   if (scene) {
     launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
-    launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
+    launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, scene->interleave != 0, c->stream);
     launch_scene_radix(c, sl.fp, sl.ctr, bufs, c->stream);
   } else {
     launch_depth_cull(c, sl.fp, sl.ctr, c->stream);
@@ -995,6 +998,9 @@ static FrameBufs slot_bufs(gs_context *c, const gs_context::Slot &sl) {
 // per-frame parameters the kernels read: a views frame's views (view v at +v), else the slot's own
 static const FrameParams *slot_fp(const gs_context::Slot &sl) { return sl.stereo ? &sl.stereo_dev->view[0] : sl.fp; }
 
+// a scene frame (or pick) of GS_RENDER_SCENE_INTERLEAVE: its scene keys and slab passes are the interleaved instantiations
+static bool interleaved(const gs_context::Slot &sl) { return sl.scene && sl.scene_host->interleave; }
+
 // graph key of a frame: anything baked into its captured launches (views frames: also the view shape and the extra views'
 // buffers, which only their bin sort takes as kernel arguments)
 static gs_context::GraphKey graph_key(const gs_context *c, const gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
@@ -1003,6 +1009,7 @@ static gs_context::GraphKey graph_key(const gs_context *c, const gs_context::Slo
   k.p3 = c->scene_key;
   k.psh = c->sh;
   k.sh_degree = c->sh_degree;
+  k.interleave = interleaved(sl) ? 1u : 0u;
   if (sl.stereo) {
     k.n_views = sl.n_views;
     for (uint32_t v = 0; v < sl.n_views; ++v) k.view_size[v] = sl.view[v].width | sl.view[v].height << 16;
@@ -1046,7 +1053,7 @@ static cudaError_t enqueue_sort_stage(gs_context *c, gs_context::Slot &sl, bool 
   if ((e = record(sl.evp[1], x, external_events))) return e;
   if ((e = cudaEventRecord(c->ev_join[0], x))) return e;
   if (sl.scene) {
-    launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, m);
+    launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, interleaved(sl), m);
     launch_scene_radix(c, sl.fp, sl.ctr, b, m);
   } else if (!reuse) {
     launch_depth_radix(c, sl.fp, sl.ctr, b, m);
@@ -1220,9 +1227,9 @@ static cudaError_t enqueue_slab_keys_stage(gs_context *c, gs_context::Slot &sl, 
   if ((e = record(sl.ev[0], st, external_events))) return e;
   if (scene) launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, st);
   else launch_depth_cull(c, sl.fp, sl.ctr, st);
-  launch_keys(c, sl.fp, sl.ctr, scene, sl.octr, sl.set, st);
+  launch_keys(c, sl.fp, sl.ctr, scene, interleaved(sl), sl.octr, sl.set, st);
   launch_slab_plan(c, sl.fp, sl.ctr, sl.set, c->slab_first, sl.n_slabs, st);
-  launch_compact_offsets(c, sl.fp, scene, sl.set, sl.n_slabs, st);  // one pass over the keys for every slab's compaction offsets
+  launch_compact_offsets(c, sl.fp, scene, interleaved(sl), sl.set, sl.n_slabs, st);  // one pass over the keys for every slab's compaction offsets
   if ((e = record(sl.ev[1], st, external_events))) return e;
   return cudaGetLastError();
 }
@@ -1240,8 +1247,8 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
   launch_slab_init(c, fp, sl.ctr, sl.stereo, st);
   if ((e = record(sl.ev[2], st, external_events))) return e;
   for (int s = 0; s < sl.n_slabs; ++s) {
-    launch_slab_begin(c, sl.fp, sl.ctr, scene, sl.set, s, st);   // entry count (0 once every bin is closed) + compaction
-    launch_slab_sort(c, sl.fp, sl.ctr, scene, b, st);            // draw order of the slab
+    launch_slab_begin(c, sl.fp, sl.ctr, scene, interleaved(sl), sl.set, s, st);  // entry count (0 once every bin is closed) + compaction
+    launch_slab_sort(c, sl.fp, sl.ctr, scene, interleaved(sl), b, st);           // draw order of the slab
     launch_project_entries(c, sl.fp, sl.ctr, scene, stereo, b, st);  // vertex shader for the slab's entries (of each view)
     if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, st))) return e;
     launch_emit(c, fp, sl.ctr, b, c->bin_open, st);
@@ -1856,6 +1863,8 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
 
 extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *out_rgba, uint64_t *out_ticket) {
   if (!c || !p || !out_rgba) return GS_ERR_INVALID;
+  if (p->flags & GS_RENDER_SCENE_INTERLEAVE)
+    return fail(c, GS_ERR_INVALID, "GS_RENDER_SCENE_INTERLEAVE is a scene frame flag: gs_render has no entities");
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render before any push");
   return render_async(c, p, nullptr, 0, nullptr, out_rgba, out_ticket);
 }
@@ -1866,10 +1875,12 @@ static int scene_async(gs_context *c, const gs_render_params *frame, const gs_ob
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render_scene before any push");
   if (frame->flags & GS_RENDER_REUSE_SORT) return fail(c, GS_ERR_INVALID, "scene frames always sort: GS_RENDER_REUSE_SORT is not accepted");
   size_t bytes = 0;
-  int rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
+  const bool interleave = (frame->flags & GS_RENDER_SCENE_INTERLEAVE) != 0;
+  int rc = build_scene_table(c, objs, n_objs, interleave, *c->scene_tmp, &bytes);
   if (rc) return rc;
-  if (n_objs == 1 && objs[0].first == 0 && objs[0].count == c->n) {
-    // one entity over the whole table: the plain frame with this entity's matrices, plus the colour target
+  if (!interleave && n_objs == 1 && objs[0].first == 0 && objs[0].count == c->n) {
+    // one entity over the whole table: the plain frame with this entity's matrices, plus the colour target (an interleaved
+    // frame keeps the scene path, whose keys clamp where the plain sort drops)
     gs_render_params p = *frame;
     memcpy(p.modelview, objs[0].modelview, sizeof(p.modelview));
     p.has_cutout = objs[0].has_cutout;
@@ -1942,8 +1953,8 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   if (!c || !frame || !xy || !out) return GS_ERR_INVALID;
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_pick_scene before any push");
   if (n_points == 0 || n_points > GS_MAX_PICKS) return fail(c, GS_ERR_INVALID, "gs_pick_scene: between 1 and GS_MAX_PICKS points");
-  if (frame->flags & ~(uint32_t)GS_RENDER_DEPTH_DEVICE)
-    return fail(c, GS_ERR_INVALID, "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE is accepted");
+  if (frame->flags & ~(uint32_t)(GS_RENDER_DEPTH_DEVICE | GS_RENDER_SCENE_INTERLEAVE))
+    return fail(c, GS_ERR_INVALID, "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE and GS_RENDER_SCENE_INTERLEAVE is accepted");
   if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "gs_pick_scene: not on a sharded context");
   if (frame->width == 0 || frame->height == 0 || frame->width > 4096 || frame->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
@@ -1952,11 +1963,13 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
     if (xy[2 * i] >= frame->width || xy[2 * i + 1] >= frame->height)
       return fail(c, GS_ERR_INVALID, "gs_pick_scene: a point lies outside the frame");
   size_t bytes = 0;
-  int rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
+  const bool interleave = (frame->flags & GS_RENDER_SCENE_INTERLEAVE) != 0;
+  int rc = build_scene_table(c, objs, n_objs, interleave, *c->scene_tmp, &bytes);
   if (rc) return rc;
-  // the frame gs_render_scene draws: one entity over the whole table takes the plain path with its matrices
+  // the frame gs_render_scene draws: one entity over the whole table takes the plain path with its matrices (not when
+  // interleaved)
   gs_render_params p = *frame;
-  const bool plain = n_objs == 1 && objs[0].first == 0 && objs[0].count == c->n;
+  const bool plain = !interleave && n_objs == 1 && objs[0].first == 0 && objs[0].count == c->n;
   if (plain) {
     memcpy(p.modelview, objs[0].modelview, sizeof(p.modelview));
     p.has_cutout = objs[0].has_cutout;
@@ -2025,7 +2038,18 @@ extern "C" int gs_sort_scene(gs_context *c, const gs_object *objs, uint32_t n_ob
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_sort_scene before any push");
   GS_CUDA(c, cudaSetDevice(c->device));
   size_t bytes = 0;
-  int rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
+  int rc = build_scene_table(c, objs, n_objs, false, *c->scene_tmp, &bytes);
+  if (rc) return rc;
+  return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count);
+}
+
+extern "C" int gs_sort_scene_interleaved(gs_context *c, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx,
+                                         uint32_t *out_count) {
+  if (!c) return GS_ERR_INVALID;
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_sort_scene_interleaved before any push");
+  GS_CUDA(c, cudaSetDevice(c->device));
+  size_t bytes = 0;
+  int rc = build_scene_table(c, objs, n_objs, true, *c->scene_tmp, &bytes);
   if (rc) return rc;
   return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count);
 }
@@ -2055,8 +2079,11 @@ extern "C" int gs_render_stereo(gs_context *c, const float view[4], const float 
                                 const gs_render_params eyes[2], void *const out_rgba[2], gs_stats *stats2_or_null) {
   if (!c || !view || !eyes || !out_rgba || !out_rgba[0] || !out_rgba[1]) return GS_ERR_INVALID;
   int rc;
-  for (int e = 0; e < 2; ++e)  // refused before the sort, so that a refusal changes nothing
+  for (int e = 0; e < 2; ++e) {  // refused before the sort, so that a refusal changes nothing
+    if (eyes[e].flags & GS_RENDER_SCENE_INTERLEAVE)
+      return fail(c, GS_ERR_INVALID, "GS_RENDER_SCENE_INTERLEAVE is a scene frame flag: gs_render_stereo has no entities");
     if ((rc = check_blend8(c, &eyes[e]))) return rc;
+  }
   rc = gs_sort(c, view, cutout16_or_null, nullptr, nullptr);
   if (rc) return rc;
   const float ms_sort = c->stats.ms_sort;
@@ -2098,7 +2125,7 @@ static int scene_views_async(gs_context *c, const gs_render_params *views, uint3
     if ((rc = check_blend8(c, &p))) return rc;
   }
   size_t bytes = 0;
-  rc = build_scene_table(c, objs, n_objs, *c->scene_tmp, &bytes);
+  rc = build_scene_table(c, objs, n_objs, (views[0].flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes);
   if (rc) return rc;
   // each entity's per-view modelviews, in the table's order (caller's entity k = its draw rank)
   float mv[kMaxObjects][kMaxViews][16];

@@ -145,7 +145,9 @@ struct SceneObject {
 struct SceneTable {
   uint32_t n;            // non-empty entities, sorted by `first` (empty ones draw nothing and are left out)
   uint32_t bucket_bits;  // slab path: log2 of the slab buckets per draw rank, 12 - ceil(log2(caller's entity count))
-  uint32_t pad[2];
+  uint32_t interleave;   // GS_RENDER_SCENE_INTERLEAVE: one depth order over all entities (read by the host, which picks
+                         // the kernels' instantiation)
+  uint32_t pad;
   SceneObject obj[kMaxObjects];
 };
 // ---- views scene frames (gs_render_scene_views, and gs_render_scene_stereo as its two-view case): one head-camera sort,
@@ -248,10 +250,13 @@ constexpr uint32_t kNoKey = 0xFFFFFFFFu;
 // Slab bucket of a sort key (never kNoKey).  Plain frames: the 16-bit key's top 12 bits.  Scene frames, 24-bit key
 // rank << 17 | key17 (key17 = 16-bit key, or 65536 for a quirk-Q5 drop): draw rank r owns the B = 2^bits buckets
 // [r B, (r + 1) B) (SceneTable::bucket_bits), and key17 >> (16 - bits) picks one of them; a Q5 drop falls into the
-// entity's top bucket.  Either way the bucket order is the draw order, so slabs cut from the top are nearest first.
-template <bool SCENE>
+// entity's top bucket.  Interleaved scene frames (IL), 22-bit key key16 << 6 | rank: key >> 10 = key16 >> 4, the plain
+// frame's bucket, shared by every entity (bits does not apply).  Either way the bucket order is the draw order, so slabs
+// cut from the top are nearest first.
+template <bool SCENE, bool IL = false>
 __device__ __forceinline__ uint32_t slab_bucket(uint32_t key, uint32_t bits) {
   if (!SCENE) return key >> 4;
+  if (IL) return key >> 10;
   return ((key >> 17) << bits) | min((key & 0x1FFFFu) >> (16u - bits), (1u << bits) - 1u);
 }
 // ---- picks (gs_pick_scene, gs_pick.cu): the query points and the bins that hold them, one host -> device copy per pick.
@@ -497,7 +502,8 @@ struct gs_context {
   struct GraphKey {
     uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr;
     uint32_t n_views = 0, view_size[gs::kMaxViews] = {}, pad2 = 0; const void *px = nullptr;
-    const void *psh = nullptr; uint32_t sh_degree = 0, pad3 = 0;  // the projection's instantiation and SH table
+    const void *psh = nullptr; uint32_t sh_degree = 0;  // the projection's instantiation and SH table
+    uint32_t interleave = 0;  // scene keys and slab passes of GS_RENDER_SCENE_INTERLEAVE frames
   } gkey[gs::kGraphDomains];                     // [GraphDomain] (kept apart: a views frame or a pick re-captures only its own graphs)
 
   // ---- fused exchange: one shared allocation per rank = flag rows + a ring of 3 frames, opened by every peer ----
@@ -545,8 +551,9 @@ void launch_depth_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr
 // scene frames: per-entity depth pass, per-entity keys, (rank, key, index) sort -> b.order, per-entity projection
 void launch_depth_cull_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, ObjCounters *octr, FrameCounters *ctr,
                              cudaStream_t st);
+// interleave (GS_RENDER_SCENE_INTERLEAVE): one key space over every entity, in the same launches
 void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *scene, const ObjCounters *octr, FrameCounters *ctr,
-                       cudaStream_t st);
+                       bool interleave, cudaStream_t st);
 void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 9 launches
 void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
                           const FrameBufs &b, cudaStream_t st);
@@ -601,18 +608,19 @@ struct PeerRows { unsigned long long *p[kMaxPeers]; };
 void launch_peer_release(gs_context *c, const PeerRows &rows, uint32_t world, uint32_t rank, unsigned long long seq,
                          cudaStream_t st);
 // ---- slab path launchers (gs_slab.cu / gs_raster.cu) ----
-// scene: the slot's scene table (device) of a scene frame, NULL for a plain frame; octr: its per-entity depth ranges
-void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const ObjCounters *octr, int set,
-                 cudaStream_t st);  // keys + bucket histogram
+// scene: the slot's scene table (device) of a scene frame, NULL for a plain frame; octr: its per-entity depth ranges;
+// interleave: the scene is keyed and cut as one interleaved order (GS_RENDER_SCENE_INTERLEAVE)
+void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
+                 const ObjCounters *octr, int set, cudaStream_t st);  // keys + bucket histogram
 void launch_slab_plan(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, uint32_t first_target, int n_slabs, cudaStream_t st);
 // stereo: every view's pixel state, closed flags and bins (fp = &views->view[0])
 void launch_slab_init(gs_context *c, const FrameParams *fp, FrameCounters *ctr, bool stereo, cudaStream_t st);
-void launch_compact_offsets(gs_context *c, const FrameParams *fp, const SceneTable *scene, int set, int n_slabs,
+void launch_compact_offsets(gs_context *c, const FrameParams *fp, const SceneTable *scene, bool interleave, int set, int n_slabs,
                             cudaStream_t st);  // every slab's chunk offsets: 2 launches
-void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, int set, int slab,
-                       cudaStream_t st);  // + compaction: 2 launches
-void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
-                      cudaStream_t st);  // 6 launches (scene frames: 9)
+void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave, int set,
+                       int slab, cudaStream_t st);  // + compaction: 2 launches
+void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
+                      const FrameBufs &b, cudaStream_t st);  // 6 launches (scene frames: 9)
 // views: the slot's view table of a views scene frame (view 0 into b.proj_rec / rect, views 1.. into b.proj_recx / rectx)
 void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene,
                             const ViewTable *views, const FrameBufs &b, cudaStream_t st);

@@ -31,6 +31,9 @@
 // entries with key17 = 65536 (its top bucket), compacted and sorted like the others; the pass SM1 turns each into a draw
 // of the entity's first splat.  The per-slab sort is SM1, M2, M3 over the compacted 24-bit keys, and the projection
 // takes each entry's entity modelview (k_project<true, true>).
+// Interleaved scene frames (GS_RENDER_SCENE_INTERLEAVE, the IL instantiations) cut the axis of their 22-bit key
+// key16 << 6 | rank: the buckets are depth buckets shared by every entity, no entry is a Q5 drop, and the per-slab sort
+// is SM1I, M2, M3.
 //
 // Views scene frames (gs_render_scene_views, gs_render_scene_stereo) cut their slabs from the HEAD camera's scene order,
 // which is every view's draw order: stage A, the plan and the compaction offsets are those of the scene frame, shared by
@@ -51,8 +54,9 @@ constexpr int kCompactChunk = kCompactThreads * kCompactItems;  // 2048 splats p
 // ---------------------------------------------------------------------------------------------
 // keys of all splats + bucket histogram (index.js:557-563).  Plain frames: the 16-bit key, kNoKey for a quirk-Q5 drop.
 // SCENE: the 24-bit key of k_scene_keys (each entity's own range); a Q5 drop is a real entry at the top of its entity.
+// IL: the interleaved key of k_scene_keys<true> (the frame's one range), never dropped.
 // ---------------------------------------------------------------------------------------------
-template <bool SCENE>
+template <bool SCENE, bool IL = false>
 __global__ void __launch_bounds__(256) k_keys(const float *__restrict__ depth, const FrameParams *__restrict__ fp,
                                               FrameCounters *ctr, uint32_t *__restrict__ key32, SlabTable *tab,
                                               const SceneTable *__restrict__ scene, const ObjCounters *__restrict__ octr) {
@@ -65,7 +69,7 @@ __global__ void __launch_bounds__(256) k_keys(const float *__restrict__ depth, c
   DepthRange dr{0.0, 0.0};
   uint32_t bits = 0;
   if constexpr (SCENE) {
-    s_ent.load(scene, octr);
+    s_ent.template load<IL>(scene, octr, ctr);
     bits = scene->bucket_bits;
   } else {
     if (ctr->sort.n_valid) dr = load_depth_range(ctr);
@@ -79,15 +83,15 @@ __global__ void __launch_bounds__(256) k_keys(const float *__restrict__ depth, c
     bool dropped;  // typed-array write out of range (quirk Q5)
     if constexpr (SCENE) {
       int obj;
-      key = s_ent.key(i, d, obj);
-      dropped = (key & 65536u) != 0u;
+      key = s_ent.template key<IL>(i, d, obj);
+      dropped = !IL && (key & 65536u) != 0u;
     } else {
       const int32_t k = depth_key(d, dr.min_depth, dr.depth_inv);
       dropped = k < 0 || k > 65535;
       key = dropped ? kNoKey : (uint32_t)k;
     }
     if (dropped) ++drop; else ++in;
-    if (key != kNoKey) atomicAdd(&h[slab_bucket<SCENE>(key, bits)], 1u);
+    if (key != kNoKey) atomicAdd(&h[slab_bucket<SCENE, IL>(key, bits)], 1u);
     return key;
   };
   // four splats per thread and step: the loads of a step are independent, so a thread keeps 16 B in flight instead
@@ -260,7 +264,7 @@ __device__ __forceinline__ void load_keys8(const uint32_t *__restrict__ key32, u
 // fields of one 64-bit word (12 slabs x 4 bits, at most 8 per field), the warp adds each field with redux.
 // cnt[s * row + c] = entries of slab s in chunk c.  (A pass per slab read the 4 B keys of all N splats once more for
 // every slab that ran.)
-template <bool SCENE>
+template <bool SCENE, bool IL = false>
 __global__ void __launch_bounds__(kCompactThreads) k_compact_count_all(const uint32_t *__restrict__ key32,
                                                                        const FrameParams *__restrict__ fp,
                                                                        const SlabTable *__restrict__ tab,
@@ -288,7 +292,7 @@ __global__ void __launch_bounds__(kCompactThreads) k_compact_count_all(const uin
     unsigned long long m = 0ull;
 #pragma unroll
     for (int j = 0; j < 8; ++j)
-      if (k[j] != kNoKey) m += 1ull << (4u * s_slab[slab_bucket<SCENE>(k[j], bits)]);
+      if (k[j] != kNoKey) m += 1ull << (4u * s_slab[slab_bucket<SCENE, IL>(k[j], bits)]);
     for (int s = 0; s < n_slabs; ++s) {
       const uint32_t v = __reduce_add_sync(0xffffffffu, (uint32_t)(m >> (4 * s)) & 15u);
       if (lane == 0 && v) atomicAdd(&s_c[s], v);
@@ -341,7 +345,7 @@ __global__ void __launch_bounds__(1024) k_compact_scan_all(uint32_t *__restrict_
 
 // the slab's entries (buckets in [klo, khi) / 16) in index order: splat index and key (plain frames: the 16-bit key;
 // SCENE: the 24-bit key, whose quirk-Q5 entries pass SM1 the dropped splat's index)
-template <bool SCENE>
+template <bool SCENE, bool IL = false>
 __global__ void __launch_bounds__(kCompactThreads) k_compact_write(const uint32_t *__restrict__ key32,
                                                                    const FrameParams *__restrict__ fp,
                                                                    const FrameCounters *__restrict__ ctr,
@@ -356,7 +360,7 @@ __global__ void __launch_bounds__(kCompactThreads) k_compact_write(const uint32_
   const uint32_t n = fp->n_splats, lo = tab->klo[slab], hi = tab->khi[slab];
   auto in_slab = [&](uint32_t k) {  // plain keys compare directly (bounds are bucket * 16); kNoKey maps past every bucket
     if (!SCENE) return k >= lo && k < hi;
-    const uint32_t bk = slab_bucket<SCENE>(k, bits);
+    const uint32_t bk = slab_bucket<SCENE, IL>(k, bits);
     return bk >= (lo >> 4) && bk < (hi >> 4);
   };
   const uint32_t nchunks = (n + kCompactChunk - 1) / kCompactChunk;
@@ -402,10 +406,11 @@ static int grid_for(gs_context *c, uint64_t n, int per_cta, int per_sm) {
   return (int)(t < cap ? t : cap);
 }
 
-void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const ObjCounters *octr,
-                 int set, cudaStream_t st) {
+// interleave: the scene's interleaved instantiations (scene frames only)
+void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
+                 const ObjCounters *octr, int set, cudaStream_t st) {
   cudaMemsetAsync(c->slab_tab[set], 0, sizeof(SlabTable), st);
-  (scene ? k_keys<true> : k_keys<false>)<<<grid_for(c, c->cap, 256 * 8, 8), 256, 0, st>>>(c->depth, fp, ctr, c->key32[set],
+  (interleave ? k_keys<true, true> : scene ? k_keys<true> : k_keys<false>)<<<grid_for(c, c->cap, 256 * 8, 8), 256, 0, st>>>(c->depth, fp, ctr, c->key32[set],
                                                                                         c->slab_tab[set], scene, octr);
 }
 
@@ -421,21 +426,22 @@ void launch_slab_init(gs_context *c, const FrameParams *fp, FrameCounters *ctr, 
 }
 
 // stage A, after the plan: chunk offsets of every scheduled slab (the loop's k_compact_write reads row `slab`)
-void launch_compact_offsets(gs_context *c, const FrameParams *fp, const SceneTable *scene, int set, int n_slabs, cudaStream_t st) {
+void launch_compact_offsets(gs_context *c, const FrameParams *fp, const SceneTable *scene, bool interleave, int set, int n_slabs,
+                            cudaStream_t st) {
   const int grid = grid_for(c, c->cap, kCompactChunk, 8);
-  (scene ? k_compact_count_all<true> : k_compact_count_all<false>)<<<grid, kCompactThreads, 0, st>>>(
+  (interleave ? k_compact_count_all<true, true> : scene ? k_compact_count_all<true> : k_compact_count_all<false>)<<<grid, kCompactThreads, 0, st>>>(
       c->key32[set], fp, c->slab_tab[set], scene, n_slabs, c->chunk_cnt[set], c->chunk_row);
   k_compact_scan_all<<<n_slabs, 1024, 0, st>>>(c->chunk_cnt[set], fp, c->chunk_row);
 }
 
 // scene frames compact into scene_key (24-bit keys), which the one-pass scene sort alone uses otherwise
-void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, int set, int slab,
-                       cudaStream_t st) {
+void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave, int set,
+                       int slab, cudaStream_t st) {
   k_slab_begin<<<1, 32, 0, st>>>(c->slab_tab[set], ctr, slab, scene == nullptr);
   const int grid = grid_for(c, c->cap, kCompactChunk, 8);
   const uint32_t *cnt = c->chunk_cnt[set] + (size_t)slab * c->chunk_row;
   if (scene)
-    k_compact_write<true><<<grid, kCompactThreads, 0, st>>>(c->key32[set], fp, ctr, c->slab_tab[set], scene, slab, cnt, c->cidx,
+    (interleave ? k_compact_write<true, true> : k_compact_write<true>)<<<grid, kCompactThreads, 0, st>>>(c->key32[set], fp, ctr, c->slab_tab[set], scene, slab, cnt, c->cidx,
                                                             c->scene_key);
   else
     k_compact_write<false><<<grid, kCompactThreads, 0, st>>>(c->key32[set], fp, ctr, c->slab_tab[set], scene, slab, cnt, c->cidx,

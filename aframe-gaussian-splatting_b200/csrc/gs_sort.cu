@@ -20,6 +20,9 @@
 //                        stay 0, the entity-local splat 0, and come after all its in-range entries)
 //   k_radix_*<M1>, <M2>, <M3>: three stable 8-bit passes -> (rank, key, index) order = each entity's sortedIndexes + first,
 //                        concatenated in draw order
+// Interleaved scene frames (GS_RENDER_SCENE_INTERLEAVE): k_scene_keys<true> keys every entity in the frame's one range
+// (22-bit key16 << 6 | rank, out-of-range keys clamped, payload = the splat), and the same three passes give one
+// (key, rank, index) order over all entities.
 //
 // PLY ingest (gs_push_ply): k_radix_*<P<0>> .. <P<24>> sort the rows by a 32-bit importance key, four stable 8-bit passes
 // (the stable Array.prototype.sort of index.js:668).  Each pass reads the digit through the permutation (key[perm[i]]), so
@@ -205,6 +208,8 @@ __global__ void __launch_bounds__(256) k_depth_cull_scene(const float4 *__restri
 }
 
 // Scene frames: the 24-bit sort key of every splat (kNoKey = not sorted) and the payload of the first radix pass.
+// IL: the interleaved key (SceneKeyTable::key<true>), whose payload is always the splat itself.
+template <bool IL>
 __global__ void __launch_bounds__(256) k_scene_keys(const float *__restrict__ depth, const FrameParams *__restrict__ fp,
                                                     const SceneTable *__restrict__ scene, const ObjCounters *__restrict__ octr,
                                                     FrameCounters *ctr, uint32_t *__restrict__ key_out,
@@ -212,7 +217,7 @@ __global__ void __launch_bounds__(256) k_scene_keys(const float *__restrict__ de
   GS_PDL_ENTRY();
   __shared__ SceneKeyTable s_ent;
   __shared__ uint32_t s_in, s_drop;
-  s_ent.load(scene, octr);
+  s_ent.load<IL>(scene, octr, ctr);
   if (threadIdx.x == 0) { s_in = 0; s_drop = 0; }
   __syncthreads();
   const uint32_t n = ctr->sort.n_valid ? fp->n_splats : 0u;
@@ -222,8 +227,8 @@ __global__ void __launch_bounds__(256) k_scene_keys(const float *__restrict__ de
     uint32_t key = kNoKey;
     if (d != GS_DEPTH_REJECT) {
       int k;
-      key = s_ent.key(i, d, k);
-      if (key & 65536u) {  // quirk Q5: the entity's first splat
+      key = s_ent.key<IL>(i, d, k);
+      if (!IL && (key & 65536u)) {  // quirk Q5: the entity's first splat
         pay_out[i] = s_ent.first[k];
         ++drop;
       } else {
@@ -269,9 +274,10 @@ void launch_depth_cull_scene(gs_context *c, const FrameParams *fp, const SceneTa
 }
 
 void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *scene, const ObjCounters *octr, FrameCounters *ctr,
-                       cudaStream_t st) {
+                       bool interleave, cudaStream_t st) {
   const int grid = persistent_grid(c, c->cap, 256 * 4, 8);
-  launch_chain(c, k_scene_keys, grid, 256, st, (const float *)c->depth, fp, scene, octr, ctr, c->scene_key, c->scene_pay);
+  launch_chain(c, interleave ? k_scene_keys<true> : k_scene_keys<false>, grid, 256, st, (const float *)c->depth, fp, scene, octr,
+               ctr, c->scene_key, c->scene_pay);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -652,12 +658,24 @@ struct SM1 : RadixPass {
   __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const { idx_out[pos] = pay; hi_out[pos] = (uint16_t)carry; }
 };
 
+// SM1I: SM1 of an interleaved scene frame.  Bit 16 is a key bit there, not a Q5 drop: every payload is the entry's splat.
+struct SM1I : SM1 {
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) const {
+    const uint32_t k = key[i];
+    carry = k >> 8;
+    pay = idx[i];
+    return k & 255u;
+  }
+};
+
 // plain frames: S1, then D2 as in the depth sort (6 launches); scene frames: SM1, M2, M3 as in the scene sort (9 launches)
-void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, const FrameBufs &b,
-                      cudaStream_t st) {
+void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
+                      const FrameBufs &b, cudaStream_t st) {
   const RadixScratch s{c->table_n, c->totals, c->table_n_stride};
   if (scene) {
-    run_pass(c, SM1{{}, ctr, scene, c->scene_key, c->cidx, c->idx_a, c->scene_hi}, s, c->cap, st);
+    const SM1 p1{{}, ctr, scene, c->scene_key, c->cidx, c->idx_a, c->scene_hi};
+    if (interleave) run_pass(c, SM1I{p1}, s, c->cap, st);
+    else run_pass(c, p1, s, c->cap, st);
     run_pass(c, M2{{}, ctr, c->scene_hi, c->idx_a, c->scene_pay, c->dig_a}, s, c->cap, st);
     run_pass(c, M3{{}, ctr, c->dig_a, c->scene_pay, b.order}, s, c->cap, st);
     return;

@@ -69,8 +69,11 @@ enum {
                                      keeps culling closed tiles' lists, so it is slower than a plain frame)  */
   GS_RENDER_DEPTH_DEVICE = 1u << 5, /* gs_render_params.depth_in is a device pointer (default: host memory) */
   GS_RENDER_COLOR_DEVICE = 1u << 6, /* gs_render_scene*: color_in is a device pointer (default: host memory)   */
-  GS_RENDER_BLEND_UNORM8 = 1u << 7  /* RGBA8 frames whose bytes are those an RGBA8 framebuffer holds after the
+  GS_RENDER_BLEND_UNORM8 = 1u << 7, /* RGBA8 frames whose bytes are those an RGBA8 framebuffer holds after the
                                        reference's back-to-front blend, rounded after every fragment (below)    */
+  GS_RENDER_SCENE_INTERLEAVE = 1u << 8 /* scene frames and picks: one back-to-front order over every entity's splats,
+                                          so overlapping entities blend by depth (see "Interleaved scenes" below);
+                                          gs_render, gs_render_async and gs_render_stereo refuse it        */
 };
 
 /*
@@ -362,10 +365,39 @@ GS_API int gs_render_stereo(gs_context *ctx, const float view[4], const float *c
  *     entity-local splat 0 is drawn again - in a shared table, the entity's FIRST splat;
  *   - projection, viewport and focal are shared by the draw (index.js:184-195); gsModelViewMatrix is per entity;
  *   - each entity is drawn whole, back to front in its own order, over what the previous entities left: entities do
- *     not interleave by depth and, writing no depth, never occlude each other; each depth-tests against depth_in;
+ *     not interleave by depth unless GS_RENDER_SCENE_INTERLEAVE (below) and, writing no depth, never occlude each other;
+ *     each depth-tests against depth_in;
  *   - draw order: A-Frame 1.4's renderer system sets three.js sortObjects to false, so transparent meshes are drawn in
  *     scene-graph (DOM) order (recalled from the three.js / A-Frame sources, not verifiable in this image; see SURVEY.md
  *     A.1).  The library takes the order from the caller (objs[0] first, i.e. furthest back) and imposes none.
+ *
+ * Interleaved scenes (GS_RENDER_SCENE_INTERLEAVE in gs_render_params.flags; not the reference's behaviour, which stays the
+ * default): a scene frame draws every splat of every entity in ONE back-to-front order, so an object inside or behind
+ * another splat entity blends with it by depth instead of covering it or being covered whole.
+ *   - filter: unchanged, each entity's own worker test (its view row, its cutout, index.js:548) in fp64; splats outside
+ *     every range are not drawn;
+ *   - one key space: every entity's depth is camera-space z of the same camera.  min / max = the smallest / largest fp64
+ *     depth of any kept splat of any entity; with q = ((f64) f32(depth) - min) * (65535 / (max - min)) in the reference's
+ *     operations, k = ToInt32(q), key16 = k when 0 <= k <= 65535, otherwise 0 for q < 0 and 65535 else.  The key is the
+ *     reference's wherever the reference keeps the splat; a splat it would drop (quirk Q5) is clamped to the nearer end of
+ *     the range, never turned into a repeat of a first splat: an interleaved frame has no Q5 repeats and n_dropped is 0;
+ *   - order: (key16, draw rank, table index) ascending, draw rank = the entity's index in objs: at equal keys objs[0]
+ *     is drawn first (further back), as in the default mode;
+ *   - drawing: unchanged.  Each splat is projected with its own entity's modelview (its view modelview in stereo and views
+ *     frames); projection, viewport, depth test, colour target, stop rule and store are those of the scene frame;
+ *   - scope: gs_render_scene[_async], gs_render_scene_stereo[_async], gs_render_scene_views[_async], every *_target[_async]
+ *     entry point and gs_pick_scene, on the one-pass and the slab path, with GS_RENDER_STATS where accepted,
+ *     GS_RENDER_BLEND_UNORM8, GS_TARGET_DEPTH_WRITE, SH contexts and host or device buffers.  Stereo and views frames sort
+ *     once from the head camera.  One entity spanning the whole table takes the scene path, not the plain frame's, so the
+ *     clamp rule holds for every entity list.  gs_render, gs_render_async and gs_render_stereo return GS_ERR_INVALID for
+ *     the flag and change nothing;
+ *   - consequences: a pick reports the nearer entity where entities overlap; a depth-writing frame writes the median
+ *     surface of the merged stack; a far-off entity widens every entity's key bucket, (max - min) / 65535, readable from
+ *     gs_stats min_depth / max_depth.
+ * Two identities follow: an interleaved frame of one entity is byte-identical to the default scene frame of that entity
+ * (for a whole-table entity, the plain frame) when that frame has n_dropped == 0; and entities with one modelview, no
+ * cutout, ranges adjacent in table order and ranks in table order give the default frame of one entity spanning their
+ * union range, when that frame has n_dropped == 0.
  */
 #define GS_MAX_OBJECTS 64
 typedef struct gs_object {
@@ -401,6 +433,12 @@ GS_API int gs_render_scene(gs_context *ctx, const gs_render_params *frame, const
  * *out_count = its length.
  */
 GS_API int gs_sort_scene(gs_context *ctx, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx, uint32_t *out_count);
+/*
+ * Draw order of a GS_RENDER_SCENE_INTERLEAVE frame of these entities: every kept splat once, in (key16, draw rank, table
+ * index) order (see "Interleaved scenes" above).  Arguments and refusals as gs_sort_scene.
+ */
+GS_API int gs_sort_scene_interleaved(gs_context *ctx, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx,
+                                     uint32_t *out_count);
 
 /*
  * WebXR on a page of several entities: one scene sort per frame from the HEAD camera (each entity's tick(),
@@ -487,7 +525,9 @@ typedef struct gs_target {
  * after whose blend T < 0.5: the pixel's median surface.  A mono frame's value is bit for bit gs_pick_scene(...).depth at
  * that pixel with depth_in the rectangle's depth before the frame; stereo and views frames walk each view's pairs in the
  * head-sorted draw order.  A pixel whose T stays >= 0.5 keeps its depth.  Every written value passed the LEQUAL test, so
- * depth never increases.  The colour is byte-identical to the frame without the flag.
+ * depth never increases.  The colour is byte-identical to the frame without the flag.  Entities never interleave unless
+ * GS_RENDER_SCENE_INTERLEAVE: by default the written surface is that of the per-entity stack drawn in objs order, with the
+ * flag that of the merged back-to-front stack.
  *   - device targets: the depth is written in place; host targets: the rectangle staged at submission is written back by
  *     the frame's read-back, next to the colour;
  *   - an overflowed run stores no depth either, and its re-run starts from the depth as it was;
@@ -573,11 +613,14 @@ GS_API int gs_render_scene_views_target(gs_context *ctx, const gs_render_params 
  *   depth: the window depth z/w * 0.5 + 0.5 of the hit splat's quad, as the depth test compares it; 1 with no hit;
  *   alpha: 1 - T where the walk ends: bit-equal to the A channel of the GS_FORMAT_RGBA32F gs_render_scene frame of the same
  *          arguments with bg_rgba alpha 0 and no colour target.
- * Entities are drawn whole in objs order and never interleave by depth (see the scene rules above): a later entity covers
- * an earlier one whatever their depths, so the pick reports the entity that is visible, not the nearer one.
+ * Entities are drawn whole in objs order and never interleave by depth unless GS_RENDER_SCENE_INTERLEAVE (see the scene
+ * rules above): a later entity covers an earlier one whatever their depths, so the pick reports the entity that is
+ * visible, not the nearer one.  With GS_RENDER_SCENE_INTERLEAVE the pick walks the one merged order and reports the nearer
+ * entity where entities overlap.
  *
  * gs_pick_scene: n_points (x, y) pairs in xy (host), results in out (host, n_points entries), in the order of xy.
- *   - From frame it reads projection, width, height, focal, depth_in and GS_RENDER_DEPTH_DEVICE; objs as gs_render_scene.
+ *   - From frame it reads projection, width, height, focal, depth_in, GS_RENDER_DEPTH_DEVICE and
+ *     GS_RENDER_SCENE_INTERLEAVE; objs as gs_render_scene.
  *   - Synchronous: it runs in the four pipeline slots like a scene frame, waits only for the frame whose slot it takes (as
  *     a fifth gs_render_scene_async would) and returns when out is filled.  It is always one-pass, whatever GS_SLAB_MIN
  *     says (the slab path draws the same bytes), and leaves no order for GS_RENDER_REUSE_SORT.  Frames submitted before or
@@ -586,7 +629,7 @@ GS_API int gs_render_scene_views_target(gs_context *ctx, const gs_render_params 
  *     whole frame are counted, so a pick needs the instance buffers of the one-pass frame (82 B per candidate), also on
  *     a context whose frames take the slab path, and returns GS_ERR_CAPACITY where that frame would.
  *   - GS_ERR_INVALID, changing nothing, for: n_points 0 or above GS_MAX_PICKS, a point outside the frame, any flag other than
- *     GS_RENDER_DEPTH_DEVICE, a sharded context (gs_set_shard world > 1), and whatever gs_render_scene refuses.  An empty
+ *     GS_RENDER_DEPTH_DEVICE and GS_RENDER_SCENE_INTERLEAVE, a sharded context (gs_set_shard world > 1), and whatever gs_render_scene refuses.  An empty
  *     table returns GS_ERR_EMPTY.
  */
 typedef struct gs_pick {
