@@ -16,6 +16,7 @@ GS_RENDER_BLEND_UNORM8 = 128
 GS_RENDER_SCENE_INTERLEAVE = 256
 GS_MAX_OBJECTS = 64
 GS_MAX_VIEWS = 4
+GS_MAX_CAMERAS = 6
 GS_TARGET_DEVICE = 1
 GS_TARGET_DEPTH_WRITE = 2
 
@@ -67,6 +68,12 @@ class GsTarget(C.Structure):
     _fields_ = [
         ("color", C.c_void_p), ("depth", C.c_void_p), ("pitch", C.c_uint32), ("rows", C.c_uint32), ("flags", C.c_uint32),
     ]
+
+
+class GsCubeFace(C.Structure):
+    """gs_cube_face: one face of gs_cube_to_equirect (pixels, size, camera-to-world rotation, projection)."""
+    _fields_ = [("rgba", C.c_void_p), ("width", C.c_uint32), ("height", C.c_uint32), ("rotation", C.c_float * 9),
+                ("proj", C.c_float * 16)]
 
 
 # every symbol include/gsplat_b200.h declares: name -> (restype, argtypes)
@@ -124,6 +131,12 @@ SYMBOLS = {
     "gs_render_scene_views_target": (C.c_int, [_P, C.POINTER(GsRenderParams), C.c_uint32, C.POINTER(GsObject),
                                                C.POINTER(C.c_float), C.c_uint32, C.POINTER(GsTarget), C.POINTER(C.c_uint32),
                                                C.POINTER(GsStats)]),
+    "gs_render_scene_cameras_async": (C.c_int, [_P, C.POINTER(GsRenderParams), C.c_uint32, C.POINTER(GsObject),
+                                                C.POINTER(C.c_float), C.c_uint32, C.POINTER(_P), C.POINTER(_P),
+                                                C.POINTER(C.c_uint64)]),
+    "gs_render_scene_cameras": (C.c_int, [_P, C.POINTER(GsRenderParams), C.c_uint32, C.POINTER(GsObject), C.POINTER(C.c_float),
+                                          C.c_uint32, C.POINTER(_P), C.POINTER(_P), C.POINTER(GsStats)]),
+    "gs_cube_to_equirect": (C.c_int, [_P, C.POINTER(GsCubeFace), C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, _P]),
     "gs_pick_scene": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.c_uint32, C.POINTER(C.c_uint32),
                                 C.c_uint32, C.POINTER(GsPick)]),
     "gs_read_projected": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),

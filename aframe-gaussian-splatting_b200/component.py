@@ -22,9 +22,10 @@ import numpy as np
 from . import ply as _ply
 from .renderer import SceneObject, SplatContext
 from .scenes import FrameInputs
-from .three_math import (Matrix4, Object3D, PerspectiveCamera, focal_length, get_model_view_matrix,
+from .three_math import (Matrix4, Object3D, PerspectiveCamera, cube_cameras, focal_length, get_model_view_matrix,
                          get_projection_matrix, world_to_cutout)
 from ._lib import GS_FORMAT_RGBA8
+from . import three_math as _tm
 
 ROW_LENGTH = 3 * 4 + 3 * 4 + 4 + 4  # index.js:227
 
@@ -428,6 +429,43 @@ class SplatScene:
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out,
                                           blend_unorm8=blend_unorm8, interleave=self.interleave)
+
+    def render_cameras(self, cameras, sizes, color_in=None, depth_in=None, bg=(0.0, 0.0, 0.0, 0.0),
+                       fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
+        """One frame of every entity for each of 1..6 cameras that may look different ways (a cube camera's faces, a rear
+        view, a minimap), each sorted with its own matrices (gs_render_scene_cameras).  sizes[c] = (w, h) device pixels of
+        camera c; color_in[c] / depth_in[c] as render() at that size, or None.  Camera c's frame is render(w, h,
+        cameras[c], ...) byte for byte.  Returns one frame per camera, row 0 = bottom."""
+        if not self.entities:
+            raise ValueError("SplatScene.render_cameras: no entity added")
+        if len(cameras) != len(sizes):
+            raise ValueError("render_cameras: one size per camera")
+        cam_frames = [[e._frame_inputs_px(int(w), int(h), cam) for e in self.entities] for cam, (w, h) in zip(cameras, sizes)]
+        objs = [SceneObject(*self.range_of(e), fr.modelview, fr.cutout) for e, fr in zip(self.entities, cam_frames[0])]
+        return self.renderer.render_scene_cameras([fr[0] for fr in cam_frames], objs,
+                                                  [[f.modelview for f in fr] for fr in cam_frames], color_in=color_in,
+                                                  depth_in=depth_in, bg=bg, fmt=fmt, blend_unorm8=blend_unorm8,
+                                                  interleave=self.interleave)
+
+    def render_cube(self, position, size: int, near: float = 0.1, far: float = 1000.0, bg=(0.0, 0.0, 0.0, 0.0),
+                    fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
+        """The six size x size faces of a THREE.CubeCamera at `position` (three_math.cube_cameras: px, nx, py, ny, pz, nz),
+        as one cameras frame.  Returns (faces, cameras)."""
+        cams = cube_cameras(position, near, far)
+        faces = self.render_cameras(cams, [(size, size)] * 6, bg=bg, fmt=fmt, blend_unorm8=blend_unorm8)
+        return faces, cams
+
+    def render_panorama(self, position, width: int, height: int, face_size: Optional[int] = None, near: float = 0.1,
+                        far: float = 1000.0, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
+                        blend_unorm8: bool = False) -> np.ndarray:
+        """A width x height equirectangular panorama seen from `position`, centred on -Z, row 0 = bottom (A-Frame's
+        screenshot component's equirectangular capture): the six cube faces of render_cube, resampled on the GPU
+        (gs_cube_to_equirect).  face_size defaults to width / 4, the face resolution that matches the panorama's pixels
+        per degree at the equator (at most 4096)."""
+        size = int(face_size) if face_size else max(1, min(4096, int(width) // 4))
+        faces, cams = self.render_cube(position, size, near, far, bg=bg, fmt=fmt, blend_unorm8=blend_unorm8)
+        return self.renderer.cube_to_equirect(faces, [_tm.rotation3(c) for c in cams],
+                                              [c.projectionMatrix.elements for c in cams], width, height, fmt=fmt)
 
     def pick(self, points, width: int, height: int, camera=None, depth_in: Optional[np.ndarray] = None):
         """What lies under pixels of the frame render() draws with these arguments (gs_pick_scene): for each (x, y) of

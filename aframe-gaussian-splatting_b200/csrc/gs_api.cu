@@ -1175,21 +1175,32 @@ static void sync_graph_key(gs_context *c, const gs_context::Slot &sl, uint32_t n
   }
 }
 
+// a stage of the slot's frame: replayed from its cached graph, or launched directly for a camera's pass of a cameras frame
+// (those never capture a graph, so they leave every cached graph and graph key as they were)
+template <class F>
+static int run_stage(gs_context *c, const gs_context::Slot &sl, cudaGraphExec_t &ge, cudaStream_t stream, F enqueue) {
+  if (sl.cameras) {
+    GS_CUDA(c, enqueue(false));
+    return GS_OK;
+  }
+  return run_graph(c, ge, stream, enqueue);
+}
+
 // Three frames overlap: while frame k is rasterised (stream C), frame k+1 is binned (stream B) and frame k+2 is
 // sorted / projected (stream A).  A and B are high priority: their short latency-bound kernels slot in as the
 // long issue-bound raster's CTAs retire.  Stage hand-offs are events; buffers between stages are double-buffered.
 static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_t n_tiles, uint32_t n_bins) {
-  sync_graph_key(c, sl, n_tiles, n_bins);
+  if (!sl.cameras) sync_graph_key(c, sl, n_tiles, n_bins);
   const int set = sl.set;
   // A: order/proj_rec/rect[set] must no longer be read by the binning stage that used them last
   if (c->sort_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->sort_set_free[set], 0));
-  int rc = run_graph(c, stage_graph(sl, kSortStage, reuse), c->stream, [&](bool ext) { return enqueue_sort_stage(c, sl, reuse, ext); });
+  int rc = run_stage(c, sl, stage_graph(sl, kSortStage, reuse), c->stream, [&](bool ext) { return enqueue_sort_stage(c, sl, reuse, ext); });
   if (rc) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_sorted, c->stream));
   // B: needs A of this frame; inst_rec/bin_range[set] must no longer be read by the raster that used them last
   GS_CUDA(c, cudaStreamWaitEvent(c->bstream, sl.ev_sorted, 0));
   if (c->bin_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->bstream, c->bin_set_free[set], 0));
-  if ((rc = run_graph(c, stage_graph(sl, kBinStage, reuse), c->bstream, [&](bool ext) {
+  if ((rc = run_stage(c, sl, stage_graph(sl, kBinStage, reuse), c->bstream, [&](bool ext) {
          return sl.pick ? enqueue_pick_bin_stage(c, sl, n_bins, ext) : enqueue_bin_stage(c, sl, n_bins, ext);
        }))) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_binned, c->bstream));
@@ -1200,7 +1211,7 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
     if ((rc = run_graph(c, stage_graph(sl, kRasterStage, reuse), c->rstream,
                         [&](bool ext) { return enqueue_pick_stage(c, sl, ext); }))) return rc;
   } else if (sl.raster_flags == c->raster_base_flags) {
-    if ((rc = run_graph(c, stage_graph(sl, kRasterStage, reuse), c->rstream,
+    if ((rc = run_stage(c, sl, stage_graph(sl, kRasterStage, reuse), c->rstream,
                         [&](bool ext) { return enqueue_raster_stage(c, sl, n_tiles, ext); }))) return rc;
   } else {
     // depth-tested / statistics / GS_RENDER_BLEND_UNORM8 frames use other instantiations of the raster: plain launches, no
@@ -1592,8 +1603,52 @@ static int restore_host_target(gs_context *c, gs_context::Slot &sl) {
   return GS_OK;
 }
 
+// a camera's pass of a cameras frame has completed (c->stats holds its statistics): add them to the frame's sums, and once
+// every camera has been added, make the sums the statistics of the frame
+static void add_camera_stats(gs_context *c, const gs_context::Slot &sl) {
+  gs_context::CameraSum &cs = c->cam_sum[sl.group % gs_context::kSlots];
+  const gs_stats &s = c->stats;
+  if (cs.group != sl.group) {
+    cs.group = sl.group;
+    cs.s = s;
+    cs.done = 0;
+  } else {
+    cs.s.n_sorted += s.n_sorted;
+    cs.s.n_dropped += s.n_dropped;
+    cs.s.n_visible += s.n_visible;
+    cs.s.n_instances += s.n_instances;
+    cs.s.n_instances_kept += s.n_instances_kept;
+    cs.s.n_tiles += s.n_tiles;
+    cs.s.ms_sort += s.ms_sort;
+    cs.s.ms_project += s.ms_project;
+    cs.s.ms_bin += s.ms_bin;
+    cs.s.ms_raster += s.ms_raster;
+    cs.s.ms_total += s.ms_total;
+    cs.s.kernel_launches += s.kernel_launches;
+    cs.s.n_slabs_run += s.n_slabs_run;  // one-pass passes: 0
+  }
+  if (sl.ticket == sl.group) {  // camera 0's size and depth range
+    cs.s.width = s.width;
+    cs.s.height = s.height;
+    cs.s.min_depth = s.min_depth;
+    cs.s.max_depth = s.max_depth;
+  }
+  cs.s.n_slabs = 0;
+  if (++cs.done == sl.group_n) c->stats = cs.s;
+}
+
 static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   if (!sl.pending) return fail(c, GS_ERR_INVALID, "gs_wait: no frame in flight for this ticket");
+  if (sl.group != ~0ull && sl.ticket == sl.group + sl.group_n - 1) {
+    // the last camera of a cameras frame (its ticket is the frame's): every camera before it is collected first
+    for (uint64_t t = sl.group; t < sl.ticket; ++t) {
+      gs_context::Slot &o = c->slot[t % gs_context::kSlots];
+      if (o.pending && o.ticket == t) {
+        int rc_cam = wait_slot(c, o, nullptr);
+        if (rc_cam) return rc_cam;
+      }
+    }
+  }
   for (int attempt = 0;; ++attempt) {
     GS_CUDA(c, cudaEventSynchronize(sl.ev_copied));
     sl.pending = false;
@@ -1693,6 +1748,7 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   c->order_count = sl.ctr_host->sort.n_valid;
   c->last_sorted = sl.ctr_host->sort.n_valid;
   c->have_last_sorted = true;
+  if (sl.group != ~0ull) add_camera_stats(c, sl);
   if (stats) *stats = c->stats;
   return GS_OK;
 }
@@ -1757,9 +1813,11 @@ static int check_blend8(gs_context *c, const gs_render_params *p) {
 // color_in: the colour target or nullptr; stereo: the views of a views scene frame (nullptr otherwise; p is view 0);
 // target: the gs_target the frame is drawn into in place (nullptr otherwise; color_in is then nullptr and out_rgba the
 // target's colour buffer).
+// group: a camera's pass of a cameras frame, the ticket of the frame's first camera and the frame's camera count (~0 and 0
+// otherwise); such a pass is always one-pass.
 static int render_async(gs_context *c, const gs_render_params *p, const SceneTable *scene, size_t scene_bytes,
                         const void *color_in, void *out_rgba, uint64_t *out_ticket, const ViewsInput *stereo = nullptr,
-                        const TargetInput *target = nullptr) {
+                        const TargetInput *target = nullptr, uint64_t group = ~0ull, uint32_t group_n = 0) {
   if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
   if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
@@ -1802,7 +1860,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   const uint32_t expect_sorted = c->have_last_sorted ? c->last_sorted : sortable;
   // views frames by their own threshold (GS_SLAB_MIN_XR); they accept neither flag.  GS_RENDER_BLEND_UNORM8 frames are
   // always one-pass: the slab path stops at front-to-back saturation, which rounding after every blend does not have
-  const bool slab = expect_sorted >= (stereo ? c->slab_min_xr : c->slab_min) &&
+  const bool slab = group == ~0ull && expect_sorted >= (stereo ? c->slab_min_xr : c->slab_min) &&
                     !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS | GS_RENDER_BLEND_UNORM8));
   need.slab = slab;
   if ((int)slab != c->last_mode) {
@@ -1820,6 +1878,9 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   sl.n_sortable = sortable;
   sl.slab = slab;
   sl.pick = false;
+  sl.cameras = group != ~0ull;
+  sl.group = group;
+  sl.group_n = group_n;
   sl.color_in[0] = color_in;
   sl.color_device = (p->flags & GS_RENDER_COLOR_DEVICE) != 0;
   sl.target = target != nullptr;
@@ -1871,7 +1932,8 @@ extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *o
 
 // gs_render_scene_async, and gs_render_scene_target_async (target set: color_in is nullptr, out_rgba the target's colour)
 static int scene_async(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
-                       const void *color_in, void *out_rgba, uint64_t *out_ticket, const TargetInput *target) {
+                       const void *color_in, void *out_rgba, uint64_t *out_ticket, const TargetInput *target,
+                       uint64_t group = ~0ull, uint32_t group_n = 0) {
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render_scene before any push");
   if (frame->flags & GS_RENDER_REUSE_SORT) return fail(c, GS_ERR_INVALID, "scene frames always sort: GS_RENDER_REUSE_SORT is not accepted");
   size_t bytes = 0;
@@ -1885,9 +1947,9 @@ static int scene_async(gs_context *c, const gs_render_params *frame, const gs_ob
     memcpy(p.modelview, objs[0].modelview, sizeof(p.modelview));
     p.has_cutout = objs[0].has_cutout;
     memcpy(p.cutout16, objs[0].cutout16, sizeof(p.cutout16));
-    return render_async(c, &p, nullptr, 0, color_in, out_rgba, out_ticket, nullptr, target);
+    return render_async(c, &p, nullptr, 0, color_in, out_rgba, out_ticket, nullptr, target, group, group_n);
   }
-  return render_async(c, frame, c->scene_tmp, bytes, color_in, out_rgba, out_ticket, nullptr, target);
+  return render_async(c, frame, c->scene_tmp, bytes, color_in, out_rgba, out_ticket, nullptr, target, group, group_n);
 }
 
 extern "C" int gs_render_scene_async(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
@@ -2013,6 +2075,8 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   sl.n_sortable = c->n;
   sl.slab = false;
   sl.pick = true;
+  sl.cameras = false;
+  sl.group = ~0ull;
   sl.color_in[0] = nullptr;
   sl.color_device = false;
   sl.target = false;
@@ -2246,6 +2310,102 @@ extern "C" int gs_render_scene_views(gs_context *c, const gs_render_params *view
   int rc = gs_render_scene_views_async(c, views, n_views, objs, view_modelviews, n_objs, color_in, out_rgba, &t);
   if (rc) return rc;
   return gs_wait(c, t, stats);
+}
+
+// gs_render_scene_cameras_async: every rule is checked before the first camera is submitted, then each camera is one
+// gs_render_scene pass with its own modelviews (tickets group .. group + n_cams - 1; the last is the frame's)
+extern "C" int gs_render_scene_cameras_async(gs_context *c, const gs_render_params *cams, uint32_t n_cams,
+                                             const gs_object *objs, const float *cam_modelviews, uint32_t n_objs,
+                                             const void *const *color_in, void *const *out_rgba, uint64_t *out_ticket) {
+  if (!c) return GS_ERR_INVALID;
+  if (n_cams == 0 || n_cams > GS_MAX_CAMERAS) return fail(c, GS_ERR_INVALID, "cameras frame: between 1 and GS_MAX_CAMERAS cameras");
+  if (!cams || !cam_modelviews || !out_rgba) return fail(c, GS_ERR_INVALID, "cameras frame: missing cameras, modelviews or outputs");
+  for (uint32_t v = 0; v < n_cams; ++v)
+    if (!out_rgba[v]) return fail(c, GS_ERR_INVALID, "cameras frame: missing output");
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "cameras frame before any push");
+  if (cams[0].flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS | GS_RENDER_OUT_TILED | GS_RENDER_OUT_PEER))
+    return fail(c, GS_ERR_INVALID, "cameras frame: GS_RENDER_REUSE_SORT, _STATS, _OUT_TILED and _OUT_PEER are not accepted");
+  if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "cameras frame: not on a sharded context");
+  int rc;
+  for (uint32_t v = 0; v < n_cams; ++v) {
+    const gs_render_params &p = cams[v];
+    if (p.flags != cams[0].flags) return fail(c, GS_ERR_INVALID, "cameras frame: every camera must have the same flags");
+    if (p.out_format != cams[0].out_format) return fail(c, GS_ERR_INVALID, "cameras frame: every camera must have the same out_format");
+    if (p.width == 0 || p.height == 0 || p.width > 4096 || p.height > 4096)
+      return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
+    if (p.out_format != GS_FORMAT_RGBA8 && p.out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+    if ((rc = check_blend8(c, &p))) return rc;
+  }
+  size_t bytes = 0;
+  if ((rc = build_scene_table(c, objs, n_objs, (cams[0].flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes)))
+    return rc;
+  std::vector<gs_object> cam_objs(objs, objs + n_objs);
+  const uint64_t group = c->next_ticket;
+  uint64_t t = 0;
+  for (uint32_t v = 0; v < n_cams; ++v) {
+    for (uint32_t k = 0; k < n_objs; ++k)
+      memcpy(cam_objs[k].modelview, cam_modelviews + ((size_t)v * n_objs + k) * 16, sizeof(cam_objs[k].modelview));
+    if ((rc = scene_async(c, &cams[v], cam_objs.data(), n_objs, color_in ? color_in[v] : nullptr, out_rgba[v], &t, nullptr,
+                          group, n_cams)))
+      return rc;
+  }
+  if (out_ticket) *out_ticket = t;
+  return GS_OK;
+}
+
+extern "C" int gs_render_scene_cameras(gs_context *c, const gs_render_params *cams, uint32_t n_cams, const gs_object *objs,
+                                       const float *cam_modelviews, uint32_t n_objs, const void *const *color_in,
+                                       void *const *out_rgba, gs_stats *stats) {
+  uint64_t t = 0;
+  int rc = gs_render_scene_cameras_async(c, cams, n_cams, objs, cam_modelviews, n_objs, color_in, out_rgba, &t);
+  if (rc) return rc;
+  return gs_wait(c, t, stats);
+}
+
+extern "C" int gs_cube_to_equirect(gs_context *c, const gs_cube_face faces[6], int32_t out_format, uint32_t flags,
+                                   uint32_t width, uint32_t height, void *out_rgba) {
+  if (!c) return GS_ERR_INVALID;
+  if (!faces || !out_rgba) return fail(c, GS_ERR_INVALID, "cube_to_equirect: missing faces or output");
+  if (out_format != GS_FORMAT_RGBA8 && out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+  if (flags & ~(uint32_t)(GS_RENDER_COLOR_DEVICE | GS_RENDER_OUT_DEVICE))
+    return fail(c, GS_ERR_INVALID, "cube_to_equirect: only GS_RENDER_COLOR_DEVICE and GS_RENDER_OUT_DEVICE are accepted");
+  if (width == 0 || height == 0 || width > 8192 || height > 8192)
+    return fail(c, GS_ERR_INVALID, "cube_to_equirect: panorama size must be within 1..8192 per side");
+  for (int f = 0; f < 6; ++f)
+    if (!faces[f].rgba || faces[f].width == 0 || faces[f].height == 0 || faces[f].width > 4096 || faces[f].height > 4096)
+      return fail(c, GS_ERR_INVALID, "cube_to_equirect: every face needs pixels and a size within 1..4096 per side");
+  GS_CUDA(c, cudaSetDevice(c->device));
+  const cudaStream_t st = c->rstream;
+  const size_t px = out_format == GS_FORMAT_RGBA8 ? 4 : 16;
+  const bool faces_dev = (flags & GS_RENDER_COLOR_DEVICE) != 0, out_dev = (flags & GS_RENDER_OUT_DEVICE) != 0;
+  CubeFaces cf{};
+  void *staged[7] = {};  // host faces and a host output go through stream-ordered device copies
+  cudaError_t e = cudaSuccess;
+  for (int f = 0; f < 6 && e == cudaSuccess; ++f) {
+    cf.width[f] = faces[f].width;
+    cf.height[f] = faces[f].height;
+    memcpy(cf.rot[f], faces[f].rotation, sizeof(cf.rot[f]));
+    memcpy(cf.proj[f], faces[f].proj, sizeof(cf.proj[f]));
+    cf.rgba[f] = faces[f].rgba;
+    if (faces_dev) continue;
+    const size_t bytes = px * faces[f].width * faces[f].height;
+    if ((e = cudaMallocAsync(&staged[f], bytes, st)) == cudaSuccess &&
+        (e = cudaMemcpyAsync(staged[f], faces[f].rgba, bytes, cudaMemcpyHostToDevice, st)) == cudaSuccess)
+      cf.rgba[f] = staged[f];
+  }
+  void *dst = out_rgba;
+  const size_t out_bytes = px * width * height;
+  if (e == cudaSuccess && !out_dev && (e = cudaMallocAsync(&staged[6], out_bytes, st)) == cudaSuccess) dst = staged[6];
+  if (e == cudaSuccess) {
+    launch_cube_to_equirect(cf, out_format, width, height, dst, st);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess && !out_dev) e = cudaMemcpyAsync(out_rgba, dst, out_bytes, cudaMemcpyDeviceToHost, st);
+  for (void *p : staged)
+    if (p) cudaFreeAsync(p, st);
+  if (e == cudaSuccess && (!faces_dev || !out_dev)) e = cudaStreamSynchronize(st);
+  GS_CUDA(c, e);
+  return GS_OK;
 }
 
 extern "C" int gs_peer_export(gs_context *c, size_t frame_bytes, void *handle_out) {

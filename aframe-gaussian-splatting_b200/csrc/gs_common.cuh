@@ -444,6 +444,11 @@ struct gs_context {
     uint32_t n_sortable = 0;                 // splats the frame's sort considers (scene frames: in the entities' ranges)
     bool slab = false;                       // rendered by the front-to-back slab path
     bool pick = false;                       // a pick (gs_pick_scene): bin and pick stages instead of binning and raster
+    // one camera's pass of a cameras frame (gs_render_scene_cameras): stages launched without graphs.  group: the ticket of
+    // the frame's first camera (its cameras hold tickets group .. group + group_n - 1), ~0 for every other frame
+    bool cameras = false;
+    uint64_t group = ~0ull;
+    uint32_t group_n = 0;
     int n_slabs = 0;
     cudaEvent_t slab_ev[gs::kMaxSlabs][2] = {};  // raster of each slab (timing)
     cudaEvent_t ev[5]{};                     // stage boundaries (timing)
@@ -471,6 +476,12 @@ struct gs_context {
     int set = 0;                                    // which order/proj_rec/rect and inst_rec/bin_range copy it uses
   } slot[kSlots];
   uint64_t next_ticket = 0;
+  // statistics of a cameras frame summed over its cameras as they complete, at [group % kSlots]
+  struct CameraSum {
+    uint64_t group = ~0ull;
+    gs_stats s{};
+    uint32_t done = 0;  // cameras added
+  } cam_sum[kSlots];
   cudaStream_t bstream = nullptr;                   // binning stage (high priority, like the sort stage's `stream`)
   cudaEvent_t sort_set_free[2] = {nullptr, nullptr};  // last binning stage that read order/proj_rec/rect[i]
   cudaEvent_t bin_set_free[2] = {nullptr, nullptr};   // last raster that read inst_rec/bin_range[i]
@@ -597,6 +608,15 @@ void launch_emit_pick(gs_context *c, const FrameParams *fp, FrameCounters *ctr, 
 void launch_tile_radix_pick(gs_context *c, FrameCounters *ctr, const FrameBufs &b, uint32_t n_bins, uint32_t *pay, cudaStream_t st);
 // k_pick: one warp per point (scene: the slot's scene table, also filled when the pick takes the plain path of one entity
 // over the whole table)
+// gs_cube_to_equirect (gs_panorama.cu): the six faces and the output of one panorama
+struct CubeFaces {
+  const void *rgba[6];
+  uint32_t width[6], height[6];
+  float rot[6][9];
+  float proj[6][16];
+};
+void launch_cube_to_equirect(const CubeFaces &f, int32_t out_format, uint32_t width, uint32_t height, void *out,
+                             cudaStream_t st);
 void launch_pick(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameBufs &b, const uint32_t *pay,
                  const PickInput *in, gs_pick *out, cudaStream_t st);
 // views scene frames: one grid over every view's tiles (n_tiles: their sum), view v's frame at fp + v (flags: packed | depth,

@@ -11,7 +11,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F, GS_RENDER_BLEND_UNORM8, GS_RENDER_OUT_DEVICE, GS_RENDER_OUT_TILED,
-                   GS_RENDER_REUSE_SORT, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_STATS, GS_TARGET_DEPTH_WRITE, GS_TARGET_DEVICE, GsObject, GsRenderParams, GsStats, GsTarget)
+                   GS_RENDER_REUSE_SORT, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_STATS, GS_TARGET_DEPTH_WRITE, GS_TARGET_DEVICE, GsCubeFace, GsObject, GsRenderParams, GsStats, GsTarget)
 from .scenes import FrameInputs
 
 
@@ -416,6 +416,85 @@ class SplatContext:
                                                           mv.ctypes.data_as(C.POINTER(C.c_float)), len(objects), col, ptrs,
                                                           C.byref(t)))
         return t.value
+
+    def render_scene_cameras(self, cams: Sequence[FrameInputs], objects: Sequence[SceneObject], cam_mvs,
+                             color_in=None, depth_in=None, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
+                             blend_unorm8: bool = False, interleave: bool = False):
+        """gs_render_scene_cameras: 1..GS_MAX_CAMERAS cameras that may look different ways (cube faces, a rear view), each
+        at its own size and each sorted with its own matrices.  cam_mvs[c][k] is entity k's modelview of camera c (its sort
+        and its draw); `objects` give the ranges and cutouts (their modelviews are ignored).  color_in[c] / depth_in[c] as
+        in render_scene_views.  Camera c's frame equals render_scene(cams[c], objects with cam_mvs[c], color_in[c],
+        depth_in[c]) byte for byte.  Returns one frame per camera, row 0 = bottom."""
+        n = len(cams)
+        color_in = [None] * n if color_in is None else list(color_in)
+        depth_in = [None] * n if depth_in is None else list(depth_in)
+        dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
+        outs = [np.empty((v.height, v.width, 4), dtype) for v in cams]
+        cols = []
+        for v, c in zip(cams, color_in):
+            if c is not None:
+                c = np.ascontiguousarray(c, dtype=dtype)
+                if c.size != v.width * v.height * 4:
+                    raise ValueError("color_in must hold width*height RGBA pixels")
+            cols.append(c)
+        params = [self.make_params(v, bg, fmt, _blend8(blend_unorm8) | _interleave(interleave), depth_in=d)
+                  for v, d in zip(cams, depth_in)]
+        arr, objs, mv, col, ptrs = self._views_args(params, objects, cam_mvs,
+                                                    [None if c is None else c.ctypes.data for c in cols],
+                                                    [o.ctypes.data for o in outs])
+        st = GsStats()
+        self._check(self._lib.gs_render_scene_cameras(self._h, arr, n, objs, mv.ctypes.data_as(C.POINTER(C.c_float)),
+                                                      len(objects), col, ptrs, C.byref(st)))
+        self.last_stats = st
+        return outs
+
+    def render_scene_cameras_async(self, cams_params, objects: Sequence[SceneObject], cam_mvs, color_ptrs, out_ptrs) -> int:
+        """gs_render_scene_cameras_async: enqueue one cameras frame (collected with wait()).  Arguments as
+        render_scene_views_async, with cam_mvs[c][k] entity k's modelview of camera c."""
+        arr, objs, mv, col, ptrs = self._views_args(cams_params, objects, cam_mvs, color_ptrs, out_ptrs)
+        t = C.c_uint64()
+        self._check(self._lib.gs_render_scene_cameras_async(self._h, arr, len(cams_params), objs,
+                                                            mv.ctypes.data_as(C.POINTER(C.c_float)), len(objects), col,
+                                                            ptrs, C.byref(t)))
+        return t.value
+
+    def cube_to_equirect(self, faces, rotations, projections, width: int, height: int, fmt: int = GS_FORMAT_RGBA8,
+                         out=None):
+        """gs_cube_to_equirect: a width x height equirectangular panorama (row 0 = bottom, centred on -Z) resampled from
+        six faces.  faces[f]: a host (h, w, 4) array of the format's dtype, or a device face (ptr, w, h) (all six of one
+        kind); rotations[f]: the face camera's camera-to-world rotation, 9 floats column-major (its matrixWorld's 3x3);
+        projections[f]: its projection matrix, 16 floats column-major.  out: None (returns a new host array), a host
+        array, or a device pointer (int; returns it)."""
+        if len(faces) != 6 or len(rotations) != 6 or len(projections) != 6:
+            raise ValueError("cube_to_equirect: six faces, rotations and projections")
+        dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
+        arr = (GsCubeFace * 6)()
+        keep = []
+        device = [not isinstance(f, np.ndarray) for f in faces]
+        if any(device) != all(device):
+            raise ValueError("cube_to_equirect: the faces are all host arrays or all device pointers")
+        for i, f in enumerate(faces):
+            if device[i]:
+                arr[i].rgba, arr[i].width, arr[i].height = int(f[0]), int(f[1]), int(f[2])
+            else:
+                a = np.ascontiguousarray(f, dtype=dtype)
+                if a.ndim != 3 or a.shape[2] != 4:
+                    raise ValueError("cube_to_equirect: a host face is an (h, w, 4) array")
+                keep.append(a)
+                arr[i].rgba, arr[i].width, arr[i].height = a.ctypes.data, a.shape[1], a.shape[0]
+            arr[i].rotation[:] = [float(x) for x in np.asarray(rotations[i], np.float32).reshape(9)]
+            arr[i].proj[:] = [float(x) for x in np.asarray(projections[i], np.float32).reshape(16)]
+        flags = _lib.GS_RENDER_COLOR_DEVICE if all(device) else 0
+        if out is None:
+            out = np.empty((height, width, 4), dtype)
+        if isinstance(out, np.ndarray):
+            assert out.dtype == dtype and out.size == width * height * 4 and out.flags["C_CONTIGUOUS"]
+            ptr = out.ctypes.data
+        else:
+            flags |= GS_RENDER_OUT_DEVICE
+            ptr = int(out)
+        self._check(self._lib.gs_cube_to_equirect(self._h, arr, fmt, flags, width, height, C.c_void_p(ptr)))
+        return out
 
     # -- frames drawn into the caller's framebuffer in place (gs_render_scene*_target) --
     @staticmethod

@@ -205,3 +205,57 @@ def world_to_cutout(cutout: Object3D, obj: Object3D) -> Matrix4:
 def focal_length(height_px: float, gs_projection: Matrix4) -> float:
     """index.js:191: focal = (viewport.w / 2.0) * Math.abs(projectionMatrix.elements[5])."""
     return (height_px / 2.0) * abs(gs_projection.elements[5])
+
+
+def look_at_quaternion(eye: Sequence[float], target: Sequence[float], up: Sequence[float]):
+    """Quaternion (x, y, z, w) of Object3D.lookAt(target) for a camera at eye with the given up vector: Matrix4.lookAt
+    (z = normalize(eye - target), x = normalize(up x z), y = z x x) then Quaternion.setFromRotationMatrix."""
+    z = [eye[i] - target[i] for i in range(3)]
+    n = math.sqrt(z[0] * z[0] + z[1] * z[1] + z[2] * z[2])
+    z = [v / n for v in z]
+    x = [up[1] * z[2] - up[2] * z[1], up[2] * z[0] - up[0] * z[2], up[0] * z[1] - up[1] * z[0]]
+    n = math.sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2])
+    x = [v / n for v in x]
+    y = [z[1] * x[2] - z[2] * x[1], z[2] * x[0] - z[0] * x[2], z[0] * x[1] - z[1] * x[0]]
+    m11, m12, m13 = x[0], y[0], z[0]
+    m21, m22, m23 = x[1], y[1], z[1]
+    m31, m32, m33 = x[2], y[2], z[2]
+    trace = m11 + m22 + m33
+    if trace > 0:
+        s = 0.5 / math.sqrt(trace + 1.0)
+        return ((m32 - m23) * s, (m13 - m31) * s, (m21 - m12) * s, 0.25 / s)
+    if m11 > m22 and m11 > m33:
+        s = 2.0 * math.sqrt(1.0 + m11 - m22 - m33)
+        return (0.25 * s, (m12 + m21) / s, (m13 + m31) / s, (m32 - m23) / s)
+    if m22 > m33:
+        s = 2.0 * math.sqrt(1.0 + m22 - m11 - m33)
+        return ((m12 + m21) / s, 0.25 * s, (m23 + m32) / s, (m13 - m31) / s)
+    s = 2.0 * math.sqrt(1.0 + m33 - m11 - m22)
+    return ((m13 + m31) / s, (m23 + m32) / s, 0.25 * s, (m21 - m12) / s)
+
+
+# THREE.CubeCamera's faces: (look direction, up), in its order px, nx, py, ny, pz, nz
+CUBE_FACES = (((1.0, 0.0, 0.0), (0.0, -1.0, 0.0)), ((-1.0, 0.0, 0.0), (0.0, -1.0, 0.0)),
+              ((0.0, 1.0, 0.0), (0.0, 0.0, 1.0)), ((0.0, -1.0, 0.0), (0.0, 0.0, -1.0)),
+              ((0.0, 0.0, 1.0), (0.0, -1.0, 0.0)), ((0.0, 0.0, -1.0), (0.0, -1.0, 0.0)))
+
+
+def cube_cameras(position: Sequence[float], near: float = 0.1, far: float = 1000.0) -> List[PerspectiveCamera]:
+    """The six cameras of a THREE.CubeCamera at `position`: fov 90, aspect 1, in its face order (px, nx, py, ny, pz, nz),
+    each looking down its axis with CubeCamera's up vector (-Y for the four side faces, +Z for py, -Z for ny).
+
+    The orientations are recalled from the three.js source (CubeCamera.updateCoordinateSystem, WebGL coordinate system)
+    and cannot be checked against it offline, as SURVEY.md A.1 notes for the other three.js semantics restated here.  A
+    panorama does not depend on them: gs_cube_to_equirect resamples from whatever face rotations it is given."""
+    cams = []
+    for d, up in CUBE_FACES:
+        target = [position[i] + d[i] for i in range(3)]
+        q = look_at_quaternion(position, target, up)
+        cams.append(PerspectiveCamera(fov=90.0, aspect=1.0, near=near, far=far, position=position, quaternion=q))
+    return cams
+
+
+def rotation3(obj: Object3D) -> List[float]:
+    """The camera-to-world rotation of an unscaled Object3D: the 3x3 of its matrixWorld, 9 values column-major."""
+    e = obj.matrixWorld.elements
+    return [e[0], e[1], e[2], e[4], e[5], e[6], e[8], e[9], e[10]]

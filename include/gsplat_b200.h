@@ -643,6 +643,79 @@ typedef struct gs_pick {
 GS_API int gs_pick_scene(gs_context *ctx, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
                          const uint32_t *xy, uint32_t n_points, gs_pick *out);
 
+/*
+ * Cameras that look different ways: the six faces of a cube camera (A-Frame's equirectangular screenshot, a
+ * THREE.CubeCamera environment map), a rear view, a minimap.  A views frame shares one head sort across its views, which is
+ * right for eyes and insets but draws a camera facing elsewhere in the wrong order; a cameras frame sorts every camera
+ * with its own matrices.
+ *   - cams[c]: camera c's projection, its own width x height (1..4096 per side), focal, bg_rgba, out_format and depth_in;
+ *     its modelview and cutout are ignored.  Every camera has the same flags and out_format.
+ *   - cam_modelviews: n_cams * n_objs * 16 floats; entity k's getModelViewMatrix(camera c) starts at (c * n_objs + k) * 16.
+ *     Camera c sorts entity k by row 2 of that matrix and projects with it; objs[k].modelview is ignored, objs[k] gives
+ *     the range and the cutout, which acts in every camera's sort.
+ *   - color_in: NULL, or color_in[c] NULL or camera c's colour target; out_rgba[c]: camera c's frame.
+ * Camera c's frame is byte-identical to the one-pass gs_render_scene frame of cams[c], those modelviews, objs and
+ * color_in[c]: quirk Q5, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_BLEND_UNORM8, both formats, host or device colour and depth
+ * and SH colour (from camera c's own position) all behave as they do there.
+ * The frame takes one pass of the scene pipeline per camera, in camera order: each camera is sorted, projected, binned and
+ * rasterised by the scene frame's kernels while the next camera is sorted, so the cameras overlap as consecutive frames do.
+ * Those passes hold pipeline slots as frames do (a frame of more than four cameras waits for its own first cameras to finish
+ * before it returns), and the ticket returned is collected with gs_wait like any other; gs_wait collects every camera.
+ * Cameras frames launch their stages without CUDA graphs, so they never capture a graph nor make other frames re-capture
+ * theirs.
+ *   - Path: always one-pass, whatever GS_SLAB_MIN says (gs_stats.n_slabs is 0).  Each camera's pass needs the instance
+ *     buffers of that camera's one-pass frame and returns GS_ERR_CAPACITY where that frame would; an overflow is re-run as
+ *     a frame's is.
+ *   - gs_stats: n_sorted, n_dropped, n_visible, n_instances, n_instances_kept, n_tiles, the ms_* times and kernel_launches
+ *     summed over the cameras; min_depth, max_depth, width and height of camera 0.
+ *   - GS_ERR_INVALID, changing nothing, for: n_cams 0 or above GS_MAX_CAMERAS, GS_RENDER_REUSE_SORT, _STATS, _OUT_TILED or
+ *     _OUT_PEER, a sharded context, unequal flags or out_formats, and whatever gs_render_scene refuses.  An empty table
+ *     returns GS_ERR_EMPTY.
+ */
+#define GS_MAX_CAMERAS 6
+GS_API int gs_render_scene_cameras_async(gs_context *ctx, const gs_render_params *cams, uint32_t n_cams,
+                                         const gs_object *objs, const float *cam_modelviews, uint32_t n_objs,
+                                         const void *const *color_in, void *const *out_rgba, uint64_t *out_ticket);
+GS_API int gs_render_scene_cameras(gs_context *ctx, const gs_render_params *cams, uint32_t n_cams, const gs_object *objs,
+                                   const float *cam_modelviews, uint32_t n_objs, const void *const *color_in,
+                                   void *const *out_rgba, gs_stats *stats);
+
+/*
+ * An equirectangular panorama (2:1 for a full sphere) resampled from six cube faces, as A-Frame's screenshot component
+ * does with its cube camera.  faces[f]: face f's frame (width x height pixels of out_format, row 0 = bottom), the face
+ * camera's world rotation (camera to world, column-major 3x3: its columns are the camera's x, y and z axes in world) and its
+ * projection (column-major 4x4).  The faces may be in any order and orientation: only the rotations given are used.
+ * Output pixel (i, j) of width x height (row 0 = bottom, 1..8192 per side) is computed as follows; fp32 unless stated, no
+ * FMA, each sum left to right:
+ *   lon = ((i + 0.5) / width) * 2pi - pi,  lat = ((j + 0.5) / height) * pi - pi/2, both in fp64;
+ *   d = (sin lon * cos lat, sin lat, -cos lon * cos lat) in fp64, each rounded once to f32 (the centre, lon = lat = 0,
+ *       is the camera's -Z);
+ *   face = argmax over f of s_f = -((d.x * R_f[6] + d.y * R_f[7]) + d.z * R_f[8]) (the face's forward axis -z),
+ *          ties to the lower index;
+ *   v = R^T d: v.x = (d.x * R[0] + d.y * R[1]) + d.z * R[2], v.y with R[3..5], v.z with R[6..8];
+ *   cx = ((P[0] * v.x + P[4] * v.y) + P[8] * v.z) + P[12], cy with P[1], P[5], P[9], P[13], cw with P[3], P[7], P[11], P[15];
+ *   u = ((cx / cw + 1) * 0.5) * w_f - 0.5,  t = ((cy / cw + 1) * 0.5) * h_f - 0.5, each then clamped to [-1, w_f] (fmin /
+ *       fmax: NaN gives -1) and [-1, h_f];
+ *   x0 = floor(u), fx = u - x0, xa = clamp(x0, 0, w_f - 1), xb = clamp(x0 + 1, 0, w_f - 1) (y0, fy, ya, yb from t);
+ *   lerp(a, b, s) = a * (1 - s) + b * s per channel; out = lerp(lerp(T[ya][xa], T[ya][xb], fx), lerp(T[yb][xa], T[yb][xb], fx), fy).
+ * So sampling is bilinear within the chosen face and clamped to its edge texels, never filtered across faces.  RGBA8 texels
+ * are read as byte / 255 and the result is stored as q8 (GS_RENDER_BLEND_UNORM8 above).
+ *   - flags: GS_RENDER_COLOR_DEVICE when the faces are device memory, GS_RENDER_OUT_DEVICE when out_rgba is; no other.
+ *   - It runs on the context's stream (gs_stream), after every frame submitted before it; call it once the frame that drew
+ *     the faces has been collected with gs_wait, since gs_wait may re-run that frame.  It returns once the panorama is in
+ *     out_rgba when any buffer is host memory; with device faces and output it returns once the work is enqueued.
+ *   - GS_ERR_INVALID for a missing face or output, a face size outside 1..4096, a bad format, an output size outside
+ *     1..8192 or an unknown flag.
+ */
+typedef struct gs_cube_face {
+  const void *rgba;   /* width x height pixels, row 0 = bottom           */
+  uint32_t width, height;
+  float rotation[9];  /* camera to world, column-major                   */
+  float proj[16];     /* projection, column-major                        */
+} gs_cube_face;
+GS_API int gs_cube_to_equirect(gs_context *ctx, const gs_cube_face faces[6], int32_t out_format, uint32_t flags,
+                               uint32_t width, uint32_t height, void *out_rgba);
+
 /* Per-splat projected record of the last gs_render (testing the vertex-shader restatement):
  * 8 floats per resident splat {cx, cy, a1x, a1y, a2x, a2y, rgba8-as-bits, tile-rect-as-bits};
  * rect == 0xFFFFFFFF marks a splat that was not projected/visible. */
