@@ -4,12 +4,13 @@ walk's transmittance first falls below 0.5.
 The blended pairs are the oracle's (oracle.pairs: the kernels' fp32 coverage and depth test, bit for bit), entity by
 entity in draw order (scene_oracle.entity_order: each entity's own sort, quirk Q5 included).  Later entities are nearer
 in the walk, whatever their depths: entities are drawn whole and never interleave.  Only the transmittance is fp64:
-T_after = T_before * (1 - exp(-r^2) * alpha byte / 255).
+T_after = T_before * (1 - exp(-r^2) * alpha byte / 255), the segmented walk of composite_fp64.walk.
 """
 from __future__ import annotations
 
 import numpy as np
 
+import composite_fp64 as cf
 import scene_oracle as so
 
 NONE = 0xFFFFFFFF
@@ -44,17 +45,7 @@ def crossings(pairs, cc, n_pixels, threshold=THRESHOLD):
     pix, splat, r2 = pairs["pix"], pairs["splat"], pairs["r2"]
     a = (np.asarray(cc, np.uint32)[splat, 3] >> np.uint32(24)).astype(np.float64) / 255.0
     w = np.exp(-r2.astype(np.float64)) * a
-    om = 1.0 - w
-    opaque = om <= 0.0  # w = 1 (alpha byte 255 at r^2 = 0): T is exactly 0 from this pair on
-    lg = np.log(np.where(opaque, 1.0, om))
-    start = np.r_[0, np.flatnonzero(np.diff(pix)) + 1] if len(pix) else np.zeros(0, np.int64)
-    lengths = np.diff(np.r_[start, len(pix)])
-    cum, zeros = np.cumsum(lg), np.cumsum(opaque)
-    base = np.repeat(np.r_[0.0, cum][start], lengths)
-    zbase = np.repeat(np.r_[0, zeros][start], lengths)
-    t_after = np.where(zeros - zbase > 0, 0.0, np.exp(cum - base))
-    rank = np.arange(len(pix)) - np.repeat(start, lengths)
-    t_before = np.where(rank > 0, np.r_[1.0, t_after[:-1]], 1.0)
+    t_before, t_after, rank, start, lengths = cf.walk(pix, w)
     out = {"splat": np.full(n_pixels, NONE, np.uint32), "obj": np.full(n_pixels, -1, np.int64),
            "t_before": np.ones(n_pixels), "t_after": np.ones(n_pixels), "alpha": np.zeros(n_pixels),
            "rank": np.full(n_pixels, -1, np.int64)}

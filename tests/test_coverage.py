@@ -12,6 +12,8 @@ a = fp32(byte / 255).  B carries at most 4 u of relative error (a, expf within 1
 already in d is scaled by (1 - B) <= 1.  So a pixel blended n times is within 8 n u of the exact back-to-front blend of
 the same pairs, which composite_fp64 evaluates (its own error is ~1e-16 n).
 """
+import math
+
 import numpy as np
 import pytest
 
@@ -155,19 +157,189 @@ def test_fp64_compositor_check_rejects_mutants(orc, scenes):
 
 
 def test_layers_to_stop(orc):
-    """The stop depth of the stacks: the opaque layer K-th from the front ends every pixel there; the opaque stack ends
-    every pixel within its two front-most layers (the tile's corners lie at r^2 ~ 5e-4: alpha 0.9995 leaves T > 3e-4)."""
+    """The stop depth of the stacks (front_to_back's n): the opaque layer K-th from the front ends every pixel there; the
+    opaque stack ends every pixel within its two front-most layers (the tile's corners lie at r^2 ~ 5e-4: alpha 0.9995
+    leaves T > 3e-4)."""
     for regime, k in (("stop255", 256), ("stop256", 257), ("stop383", 384), ("stop384", 385), ("opaque10000", 2)):
         s = fp.stack(regime)
         order = np.arange(len(s.cs), dtype=np.uint32)
         pr = orc.pairs(s.cs, s.cc, order, s.proj, s.mv, 16, 16, s.focal)
         assert len(pr["pix"]) == 256 * len(s.cs)
-        n = cf.layers_to_stop(pr, s.cc[order, 3], 16, 16, 3e-4)
+        ref = cf.front_to_back(cf.nearest_first(pr, s.cc[order, 3]), 16, 16, t_stop=3e-4)
+        n = ref["n"]
         assert (n.max() == k and n.min() >= k - 1) if regime == "opaque10000" else np.all(n == k), regime
+        assert np.all(ref["stopped"])
     s = fp.stack("faint2000")
     pr = orc.pairs(s.cs, s.cc, np.arange(len(s.cs), dtype=np.uint32), s.proj, s.mv, s.width, s.height, s.focal)
-    n = cf.layers_to_stop(pr, s.cc[:, 3], s.width, s.height, 3e-4)
-    assert np.all(n[:, :16] == 2000) and np.all((n == 0) | (n == 2000))
+    ref = cf.front_to_back(cf.nearest_first(pr, s.cc[:, 3]), s.width, s.height, t_stop=3e-4)
+    n = ref["n"]
+    assert np.all(n[:, :16] == 2000) and np.all((n == 0) | (n == 2000)) and not ref["stopped"].any()
+
+
+# ---- the front-to-back reference with the stop rule (composite_fp64.front_to_back) ----
+def _scalar_front_to_back(pr, w, h, bg, color_in, t_stop):
+    """front_to_back's value and n, one pixel and one pair at a time, straight from the definition."""
+    dst = cf.destination(w, h, bg, color_in)
+    out, n = dst.copy(), np.zeros(w * h, np.int64)
+    pairs = {}
+    for i, p in enumerate(pr["pix"].tolist()):
+        pairs.setdefault(p, []).append(i)
+    for p, idx in pairs.items():
+        t, c = 1.0, np.zeros(3)
+        for i in idx:
+            if not t >= t_stop:
+                break
+            v = int(pr["rgba"][i])
+            a = math.exp(-float(pr["r2"][i])) * ((v >> 24) & 255) / 255.0
+            c += np.array([(v >> s) & 255 for s in (0, 8, 16)]) / 255.0 * a * t
+            t *= 1.0 - a
+            n[p] += 1
+        out[p, :3] = c + dst[p, :3] * t
+        out[p, 3] = 1.0 - t + dst[p, 3] * t
+    return out.reshape(h, w, 4), n.reshape(h, w)
+
+
+def _pixel_lists(rng, w, h, depth):
+    """Random nearest-first pairs: every third pixel empty, depths 1..depth, alpha bytes and r^2 over their range."""
+    pix, r2, rgba = [], [], []
+    for p in range(w * h):
+        if p % 3 == 0:
+            continue
+        k = int(rng.integers(1, depth + 1))
+        pix += [p] * k
+        r2 += list(rng.uniform(0.0, 4.0, k) * (rng.uniform(0, 1, k) > 0.3))
+        rgba += list(rng.integers(0, 1 << 32, k, dtype=np.int64))
+    return {"pix": np.array(pix, np.int64), "r2": np.array(r2, np.float32), "rgba": np.array(rgba, np.uint32)}
+
+
+def test_front_to_back_equals_scalar_loop():
+    rng = np.random.default_rng(12)
+    w, h = 9, 7
+    pr = _pixel_lists(rng, w, h, 60)
+    # pixel 1: an opaque pair at r^2 = 0 (T exactly 0) first; pixel 2: the T after its first pair is t_stop exactly,
+    # so the second pair is still blended (and crosses) and the third is not
+    pr["r2"][pr["pix"] == 1] = np.float32(0.0)
+    pr["rgba"][np.flatnonzero(pr["pix"] == 1)[0]] = np.uint32(0xFF336699)
+    i2 = np.flatnonzero(pr["pix"] == 2)
+    pr["r2"][i2] = np.float32(0.0)
+    pr["rgba"][i2[:3]] = np.uint32(0x80102030)
+    t_land = 1.0 - math.exp(-0.0) * 128 / 255.0
+    col8 = rng.integers(0, 256, (h, w, 4), dtype=np.uint8)
+    dests = [dict(bg=(0.25, 0.5, 0.75, 0.125)), dict(color_in=col8), dict(color_in=col8.astype(np.float32) / 255.0)]
+    for t_stop in (cf.T_STOP, 0.05, t_land):
+        for d in dests:
+            ref = cf.front_to_back(pr, w, h, t_stop=t_stop, **d)
+            val, n = _scalar_front_to_back(pr, w, h, d.get("bg", (0.0,) * 4), d.get("color_in"), t_stop)
+            assert np.array_equal(ref["n"], n), (t_stop, d.keys())
+            assert np.abs(ref["value"] - val).max() <= 1e-12, (t_stop, d.keys())
+            assert np.all(ref["value"].reshape(-1, 4)[0::3] == cf.destination(w, h, **d)[0::3])  # empty pixels
+    ref = cf.front_to_back(pr, w, h, t_stop=t_land)
+    assert ref["n"].ravel()[1] == 1 and ref["value"].reshape(-1, 4)[1, 3] == 1.0
+    assert ref["n"].ravel()[2] == 2 and ref["stopped"].ravel()[2] and ref["ambig"].ravel()[2]
+
+
+# numpy fp32 restatement of the raster's front-to-back pixel loop (gs_raster.cu k_raster, scalar loop, store_pixel), in
+# its operation order; libm exp2f stands in for ex2.approx (both within the 16 u alpha budget of composite_fp64)
+F = np.float32
+K_NEG_LOG2E = F(-1.4426950216293334961)
+MUTANTS = ("t_stop_9e-4", "stop_before_crossing", "no_dst_when_stopped", "alpha_without_dst", "r2_fp16", "alpha_fp16")
+
+
+def _fma(a, b, c):
+    return (a.astype(np.float64) * b.astype(np.float64) + c.astype(np.float64)).astype(F)
+
+
+def _kernel_fp32(pr, w, h, bg=(0.0,) * 4, color_in=None, mutant=None):
+    t_stop = F(9e-4) if mutant == "t_stop_9e-4" else F(cf.T_STOP)
+    pix = pr["pix"]
+    bytes_ = np.stack([(pr["rgba"] >> np.uint32(s)) & np.uint32(255) for s in (0, 8, 16, 24)], 1).astype(F) / F(255)
+    r2 = pr["r2"].astype(np.float16).astype(F) if mutant == "r2_fp16" else pr["r2"]
+    T, R = np.ones(w * h, F), np.zeros((w * h, 3), F)
+    live = np.ones(w * h, bool)
+    _, _, rank, _, _ = cf.walk(pix, np.zeros(len(pix)))
+    for s in [np.flatnonzero(rank == 0)] + cf._layers(rank):
+        s = s[live[pix[s]]]
+        if not len(s):
+            continue
+        p = pix[s]
+        alpha = (np.exp2((r2[s] * K_NEG_LOG2E).astype(F)).astype(F) * bytes_[s, 3]).astype(F)
+        if mutant == "alpha_fp16":
+            alpha = alpha.astype(np.float16).astype(F)
+        wt = (alpha * T[p]).astype(F)
+        tn = (T[p] - wt).astype(F)
+        if mutant == "stop_before_crossing":
+            go = tn >= t_stop
+            live[p[~go]] = False
+            s, p, wt, tn = s[go], p[go], wt[go], tn[go]
+        R[p] = _fma(bytes_[s, :3], wt[:, None], R[p])
+        T[p] = tn
+        live[p] &= tn >= t_stop
+    d = cf.destination(w, h, bg, color_in)
+    d = (np.asarray(color_in, F) / F(255) if color_in is not None and np.asarray(color_in).dtype == np.uint8
+         else d.astype(F)).reshape(-1, 4)
+    out = np.empty((w * h, 4), F)
+    out[:, :3] = _fma(d[:, :3], T[:, None], R)
+    out[:, 3] = _fma(d[:, 3], T, (F(1) - T).astype(F))
+    if mutant == "no_dst_when_stopped":
+        dead = T < t_stop
+        out[dead, :3] = R[dead]
+        out[dead, 3] = F(1) - T[dead]
+    if mutant == "alpha_without_dst":
+        out[:, 3] = F(1) - T
+    return out.reshape(h, w, 4)
+
+
+def _restatement_cases(orc, scenes):
+    """Every footprint family and every deep stack, over a random clear colour; with the oracle's fp32 frame."""
+    rng = np.random.default_rng(21)
+    cases = [(k, s) for k, s in scenes.items() if k[1:] == (400, 300)] + [((r,), fp.stack(r)) for r in fp.STACKS]
+    for key, s in cases:
+        order = np.arange(len(s.cs), dtype=np.uint32)
+        pr = orc.pairs(s.cs, s.cc, order, s.proj, s.mv, s.width, s.height, s.focal)
+        bg = tuple(float(v) for v in rng.uniform(0, 1, 4).astype(F))
+        frame, _ = orc.render(s.cs, s.cc, order, s.proj, s.mv, s.width, s.height, s.focal, bg=bg)
+        nf = cf.nearest_first(pr, s.cc[order, 3])
+        yield key, s, nf, bg, frame, cf.front_to_back(nf, s.width, s.height, bg=bg)
+
+
+def test_kernel_restatement_within_eps_and_mutants_caught(orc, scenes):
+    """The fp32 restatement of the pixel loop stays within eps(n) of front_to_back on every family and stack; each
+    mutant of it exceeds the bound on at least one of them, while at least three mutants stay within the 1e-3 frame
+    tolerance of the fp32 oracle (the gap this bound closes)."""
+    caught = {m: [] for m in MUTANTS}
+    oracle_err = {m: 0.0 for m in MUTANTS}
+    stopped = 0
+    for key, s, nf, bg, frame, ref in _restatement_cases(orc, scenes):
+        w, h = s.width, s.height
+        r = cf.check_float(_kernel_fp32(nf, w, h, bg), ref)
+        assert r["ok"], (key, r)
+        stopped += ref["stopped"].sum()
+        for m in MUTANTS:
+            got = _kernel_fp32(nf, w, h, bg, mutant=m)
+            if not cf.check_float(got, ref)["ok"]:
+                caught[m].append(key)
+            oracle_err[m] = max(oracle_err[m], float(np.abs(got - frame).max()))
+    assert stopped > 1000
+    assert all(caught.values()), caught
+    assert sum(e <= 1e-3 for e in oracle_err.values()) >= 3, oracle_err
+
+
+def test_kernel_restatement_over_colour_targets(orc):
+    """The restatement over RGBA8 and RGBA32F colour targets: within eps(n); its RGBA8 bytes pass check_u8."""
+    s = fp.family("needles", 400, 300)
+    order = np.arange(len(s.cs), dtype=np.uint32)
+    nf = cf.nearest_first(orc.pairs(s.cs, s.cc, order, s.proj, s.mv, 400, 300, s.focal), s.cc[order, 3])
+    col8 = np.random.default_rng(9).integers(0, 256, (300, 400, 4), dtype=np.uint8)
+    for col in (col8, col8.astype(F) / F(255)):
+        ref = cf.front_to_back(nf, 400, 300, color_in=col)
+        got = _kernel_fp32(nf, 400, 300, color_in=col)
+        assert cf.check_float(got, ref)["ok"]
+        u8 = (np.clip(got, 0, 1) * F(255) + F(0.5)).astype(F).astype(np.uint8)
+        r = cf.check_u8(u8, ref)
+        assert r["ok"], r
+        bad = u8.copy()
+        bad[5, 7, 1] ^= 1
+        assert not cf.check_u8(bad, ref)["ok"] or r["midpoint"] > 0
 
 
 def test_footprint_families(orc):
