@@ -14,6 +14,7 @@ GS_RENDER_OUT_DEVICE, GS_RENDER_REUSE_SORT, GS_RENDER_OUT_TILED, GS_RENDER_OUT_P
 GS_RENDER_STATS, GS_RENDER_DEPTH_DEVICE, GS_RENDER_COLOR_DEVICE = 16, 32, 64
 GS_RENDER_BLEND_UNORM8 = 128
 GS_RENDER_SCENE_INTERLEAVE = 256
+GS_RENDER_SORT_F32 = 512
 GS_MAX_OBJECTS = 64
 GS_MAX_VIEWS = 4
 GS_MAX_CAMERAS = 6
@@ -107,6 +108,7 @@ SYMBOLS = {
     "gs_render_scene": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.c_uint32, _P, _P, C.POINTER(GsStats)]),
     "gs_sort_scene": (C.c_int, [_P, C.POINTER(GsObject), C.c_uint32, _P, C.POINTER(C.c_uint32)]),
     "gs_sort_scene_interleaved": (C.c_int, [_P, C.POINTER(GsObject), C.c_uint32, _P, C.POINTER(C.c_uint32)]),
+    "gs_sort_scene_flags": (C.c_int, [_P, C.POINTER(GsObject), C.c_uint32, C.c_uint32, _P, C.POINTER(C.c_uint32)]),
     "gs_render_scene_stereo_async": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.POINTER(C.c_float),
                                                C.c_uint32, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_uint64)]),
     "gs_render_scene_stereo": (C.c_int, [_P, C.POINTER(GsRenderParams), C.POINTER(GsObject), C.POINTER(C.c_float), C.c_uint32,

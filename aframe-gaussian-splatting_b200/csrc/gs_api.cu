@@ -232,6 +232,7 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles) {
   if (slab_ready(c, n_tiles)) return GS_OK;
   if (!slab_keys_ready(c)) {
     dev_free(c->key32[0]); dev_free(c->key32[1]); dev_free(c->cidx); dev_free(c->ckey); dev_free(c->chunk_cnt[0]); dev_free(c->chunk_cnt[1]);
+    dev_free(c->zdepth[0]); dev_free(c->zdepth[1]);
     GS_CUDA(c, dev_alloc(&c->key32[0], (size_t)c->cap + 8));
     GS_CUDA(c, dev_alloc(&c->key32[1], (size_t)c->cap + 8));
     GS_CUDA(c, dev_alloc(&c->cidx, (size_t)c->cap));
@@ -263,13 +264,14 @@ static int ensure_slab(gs_context *c, uint32_t n_tiles) {
 // is idle).  A views frame (n_views views; every other frame: 1) bins every view's bins and keeps slab state for every
 // view's tiles; the tile statistics are view 0's.
 struct FrameNeeds {
-  bool slab, scene, depth_write;
+  bool slab, scene, depth_write, f32;  // f32: GS_RENDER_SORT_F32 (its passes ping-pong through scene_pay; slab frames: zdepth)
   uint32_t n_views, n_bins_all, n_tiles, n_tiles_all;
 };
 static bool frame_bufs_ready(const gs_context *c, const FrameNeeds &f) {
   return scratch_ready(c) && bins_ready(c, f.n_bins_all) && tile_stats_ready(c, f.n_tiles) &&
          (!f.slab || slab_ready(c, f.n_tiles_all)) && (!f.slab || !f.depth_write || c->pix_depth) &&
-         (!f.scene || scene_bufs_ready(c)) && stereo_bufs_ready(c, f.n_views) && c->cap_inst != 0;
+         ((!f.scene && !f.f32) || scene_bufs_ready(c)) && (!f.slab || !f.f32 || c->zdepth[0]) &&
+         stereo_bufs_ready(c, f.n_views) && c->cap_inst != 0;
 }
 static int ensure_frame_bufs(gs_context *c, const FrameNeeds &f) {
   int rc;
@@ -278,7 +280,10 @@ static int ensure_frame_bufs(gs_context *c, const FrameNeeds &f) {
   // the slab loop of a GS_TARGET_DEPTH_WRITE frame carries each pixel's crossing depth beside pix_state (no graph can bake it
   // before it exists, and ensure_slab frees it only together with pix_state, dropping the graphs)
   if (f.slab && f.depth_write && !c->pix_depth) GS_CUDA(c, dev_alloc(&c->pix_depth, (size_t)c->slab_tiles_cap * 256));
-  if (f.scene && (rc = ensure_scene_bufs(c))) return rc;
+  // a precise slab frame's loop reads its set's copy of the depths (allocated with the slab buffers' capacity, freed with them)
+  if (f.slab && f.f32 && !c->zdepth[0])
+    for (int i = 0; i < 2; ++i) GS_CUDA(c, dev_alloc(&c->zdepth[i], (size_t)c->slab_cap + 8));
+  if ((f.scene || f.f32) && (rc = ensure_scene_bufs(c))) return rc;
   if ((rc = ensure_stereo_bufs(c, f.n_views))) return rc;
   if (c->cap_inst == 0) {
     // first frame: room for two bin instances per resident splat (a typical scene needs ~1); GS_INST_CAP overrides
@@ -465,6 +470,7 @@ extern "C" int gs_destroy(gs_context *c) {
   dev_free(c->table_n); dev_free(c->table_d); dev_free(c->slice_total); dev_free(c->totals); dev_free(c->sort_hdr);
   dev_free(c->slice_prefix); dev_free(c->ent); dev_free(c->ent_off);
   dev_free(c->key32[0]); dev_free(c->key32[1]); dev_free(c->cidx); dev_free(c->ckey); dev_free(c->chunk_cnt[0]); dev_free(c->chunk_cnt[1]);
+  dev_free(c->zdepth[0]); dev_free(c->zdepth[1]);
   dev_free(c->slab_tab[0]); dev_free(c->slab_tab[1]);
   dev_free(c->pix_state); dev_free(c->tile_closed); dev_free(c->bin_open); dev_free(c->pix_depth);
   dev_free(c->scene_key); dev_free(c->scene_pay); dev_free(c->scene_hi);
@@ -907,10 +913,11 @@ static void stats_from_counters(gs_context *c, const FrameCounters &h, uint32_t 
   s.max_depth = h.sort.n_valid ? dec_f64(h.sort.max_enc) : -INFINITY;
 }
 
-// gs_sort and gs_sort_scene: one sort in slot 0 and buffer set 0 of an idle pipeline, its counters and order read back.
-// scene: the validated table of gs_sort_scene (nullptr: the one-entity sort of gs_sort, by view and cutout)
+// gs_sort and gs_sort_scene*: one sort in slot 0 and buffer set 0 of an idle pipeline, its counters and order read back.
+// scene: the validated table of gs_sort_scene* (nullptr: the one-entity sort of gs_sort, by view and cutout); f32: the
+// precise order of GS_RENDER_SORT_F32 (scene sorts only)
 static int sort_only(gs_context *c, const float *view, const float *cutout, const SceneTable *scene, size_t scene_bytes,
-                     uint32_t *out_idx, uint32_t *out_count) {
+                     uint32_t *out_idx, uint32_t *out_count, bool f32 = false) {
   int rc = idle(c);
   if (rc) return rc;
   if ((rc = ensure_scratch(c))) return rc;
@@ -930,8 +937,12 @@ static int sort_only(gs_context *c, const float *view, const float *cutout, cons
   GS_CUDA(c, cudaEventRecord(c->ev[0], c->stream));
   if (scene) {
     launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
-    launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, scene->interleave != 0, c->stream);
-    launch_scene_radix(c, sl.fp, sl.ctr, bufs, c->stream);
+    if (f32) {
+      launch_sort_f32(c, sl.fp, sl.ctr, sl.scene_dev, scene->interleave != 0, bufs, c->stream);
+    } else {
+      launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, scene->interleave != 0, c->stream);
+      launch_scene_radix(c, sl.fp, sl.ctr, bufs, c->stream);
+    }
   } else {
     launch_depth_cull(c, sl.fp, sl.ctr, c->stream);
     launch_depth_radix(c, sl.fp, sl.ctr, bufs, c->stream);
@@ -944,7 +955,7 @@ static int sort_only(gs_context *c, const float *view, const float *cutout, cons
   GS_CUDA(c, cudaStreamSynchronize(c->stream));
   memset(&c->stats, 0, sizeof(c->stats));
   stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
-  c->stats.kernel_launches = scene ? 11 : 7;
+  c->stats.kernel_launches = scene ? (f32 ? 16 : 11) : 7;
   float ms = 0;
   cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]);
   c->stats.ms_sort = ms;
@@ -1009,7 +1020,8 @@ static gs_context::GraphKey graph_key(const gs_context *c, const gs_context::Slo
   k.p3 = c->scene_key;
   k.psh = c->sh;
   k.sh_degree = c->sh_degree;
-  k.interleave = interleaved(sl) ? 1u : 0u;
+  k.sort_mode = (interleaved(sl) ? 1u : 0u) | (sl.f32 ? 2u : 0u);
+  k.pz = c->zdepth[0];
   if (sl.stereo) {
     k.n_views = sl.n_views;
     for (uint32_t v = 0; v < sl.n_views; ++v) k.view_size[v] = sl.view[v].width | sl.view[v].height << 16;
@@ -1052,11 +1064,14 @@ static cudaError_t enqueue_sort_stage(gs_context *c, gs_context::Slot &sl, bool 
   else launch_project(c, sl.fp, sl.ctr, b, x);
   if ((e = record(sl.evp[1], x, external_events))) return e;
   if ((e = cudaEventRecord(c->ev_join[0], x))) return e;
-  if (sl.scene) {
+  if (sl.scene && sl.f32) {
+    launch_sort_f32(c, sl.fp, sl.ctr, sl.scene_dev, interleaved(sl), b, m);
+  } else if (sl.scene) {
     launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, interleaved(sl), m);
     launch_scene_radix(c, sl.fp, sl.ctr, b, m);
   } else if (!reuse) {
-    launch_depth_radix(c, sl.fp, sl.ctr, b, m);
+    if (sl.f32) launch_sort_f32(c, sl.fp, sl.ctr, nullptr, false, b, m);
+    else launch_depth_radix(c, sl.fp, sl.ctr, b, m);
     if ((e = cudaMemcpyAsync(c->sort_hdr, sl.ctr, sizeof(SortHeader), cudaMemcpyDeviceToDevice, m))) return e;
   }
   if ((e = record(sl.ev[1], m, external_events))) return e;
@@ -1218,7 +1233,9 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
     // cached graph (so a frame of one blend mode never replays a raster graph captured for the other)
     GS_CUDA(c, enqueue_raster_stage(c, sl, n_tiles, false));
   }
-  sl.launches = (sl.scene ? 11u : (reuse ? 0u : 7u)) + 1u + (n_bins <= 256u ? 5u : 9u) + 1u;
+  // precise frames: a depth pass and four radix passes (scene frames: five, and no scene keys)
+  const uint32_t sort_launches = sl.f32 ? (sl.scene ? 16u : 13u) : (sl.scene ? 11u : 7u);
+  sl.launches = (reuse ? 0u : sort_launches) + 1u + (n_bins <= 256u ? 5u : 9u) + 1u;
   return GS_OK;
 }
 
@@ -1238,7 +1255,7 @@ static cudaError_t enqueue_slab_keys_stage(gs_context *c, gs_context::Slot &sl, 
   if ((e = record(sl.ev[0], st, external_events))) return e;
   if (scene) launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, st);
   else launch_depth_cull(c, sl.fp, sl.ctr, st);
-  launch_keys(c, sl.fp, sl.ctr, scene, interleaved(sl), sl.octr, sl.set, st);
+  launch_keys(c, sl.fp, sl.ctr, scene, interleaved(sl), sl.f32, sl.octr, sl.set, st);
   launch_slab_plan(c, sl.fp, sl.ctr, sl.set, c->slab_first, sl.n_slabs, st);
   launch_compact_offsets(c, sl.fp, scene, interleaved(sl), sl.set, sl.n_slabs, st);  // one pass over the keys for every slab's compaction offsets
   if ((e = record(sl.ev[1], st, external_events))) return e;
@@ -1259,7 +1276,8 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
   if ((e = record(sl.ev[2], st, external_events))) return e;
   for (int s = 0; s < sl.n_slabs; ++s) {
     launch_slab_begin(c, sl.fp, sl.ctr, scene, interleaved(sl), sl.set, s, st);  // entry count (0 once every bin is closed) + compaction
-    launch_slab_sort(c, sl.fp, sl.ctr, scene, interleaved(sl), b, st);           // draw order of the slab
+    if (sl.f32) launch_slab_sort_f32(c, sl.ctr, scene, interleaved(sl), c->zdepth[sl.set], b, st);  // precise order of the slab
+    else launch_slab_sort(c, sl.fp, sl.ctr, scene, interleaved(sl), b, st);           // draw order of the slab
     launch_project_entries(c, sl.fp, sl.ctr, scene, stereo, b, st);  // vertex shader for the slab's entries (of each view)
     if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, st))) return e;
     launch_emit(c, fp, sl.ctr, b, c->bin_open, st);
@@ -1311,8 +1329,10 @@ static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_ti
   }
   GS_CUDA(c, cudaEventRecord(sl.ev_binned, c->rstream));
   c->sort_set_free[set] = sl.ev_binned;
-  // scene frames: three radix passes per slab instead of two (views frames: the scene frame's launches, every view's bins)
-  sl.launches = 6u + 1u + (uint32_t)n_slabs * ((n_bins <= 256u ? 16u : 20u) + (sl.scene ? 3u : 0u)) + 2u;
+  // scene frames: three radix passes per slab instead of two (views frames: the scene frame's launches, every view's bins);
+  // precise frames: four (scene frames: five)
+  const uint32_t extra = sl.f32 ? (sl.scene ? 9u : 6u) : (sl.scene ? 3u : 0u);
+  sl.launches = 6u + 1u + (uint32_t)n_slabs * ((n_bins <= 256u ? 16u : 20u) + extra) + 2u;
   return GS_OK;
 }
 
@@ -1809,6 +1829,18 @@ static int check_blend8(gs_context *c, const gs_render_params *p) {
   return GS_OK;
 }
 
+// GS_RENDER_SORT_F32 sorts every frame it is set on: no GS_RENDER_REUSE_SORT, and (out of its scope) no tiled or peer
+// output and no sharded context
+static int check_sort_f32(gs_context *c, const gs_render_params *p) {
+  if (!(p->flags & GS_RENDER_SORT_F32)) return GS_OK;
+  if (p->flags & GS_RENDER_REUSE_SORT)
+    return fail(c, GS_ERR_INVALID, "GS_RENDER_SORT_F32 sorts the frame: GS_RENDER_REUSE_SORT is not accepted");
+  if (p->flags & (GS_RENDER_OUT_TILED | GS_RENDER_OUT_PEER))
+    return fail(c, GS_ERR_INVALID, "GS_RENDER_SORT_F32: GS_RENDER_OUT_TILED and _OUT_PEER are not accepted");
+  if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "GS_RENDER_SORT_F32: not on a sharded context");
+  return GS_OK;
+}
+
 // gs_render_async, scene and views scene frames.  scene: the table built by build_scene_table (nullptr = a plain frame);
 // color_in: the colour target or nullptr; stereo: the views of a views scene frame (nullptr otherwise; p is view 0);
 // target: the gs_target the frame is drawn into in place (nullptr otherwise; color_in is then nullptr and out_rgba the
@@ -1822,11 +1854,12 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
   if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
   int rcode;
-  if ((rcode = check_blend8(c, p))) return rcode;
+  if ((rcode = check_blend8(c, p)) || (rcode = check_sort_f32(c, p))) return rcode;
   // a views frame's bin table holds every view's bins (4 * 43 * 43 at most, still a 16-bit id), its slab state every
   // view's tiles
   FrameNeeds need{};
   need.scene = scene != nullptr;
+  need.f32 = (p->flags & GS_RENDER_SORT_F32) != 0;
   need.n_views = stereo ? stereo->n : 1u;
   need.depth_write = target && (target->t->flags & GS_TARGET_DEPTH_WRITE);
   for (uint32_t v = 0; v < need.n_views; ++v) {
@@ -1878,6 +1911,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   sl.n_sortable = sortable;
   sl.slab = slab;
   sl.pick = false;
+  sl.f32 = need.f32;
   sl.cameras = group != ~0ull;
   sl.group = group;
   sl.group_n = group_n;
@@ -2015,8 +2049,9 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   if (!c || !frame || !xy || !out) return GS_ERR_INVALID;
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_pick_scene before any push");
   if (n_points == 0 || n_points > GS_MAX_PICKS) return fail(c, GS_ERR_INVALID, "gs_pick_scene: between 1 and GS_MAX_PICKS points");
-  if (frame->flags & ~(uint32_t)(GS_RENDER_DEPTH_DEVICE | GS_RENDER_SCENE_INTERLEAVE))
-    return fail(c, GS_ERR_INVALID, "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE and GS_RENDER_SCENE_INTERLEAVE is accepted");
+  if (frame->flags & ~(uint32_t)(GS_RENDER_DEPTH_DEVICE | GS_RENDER_SCENE_INTERLEAVE | GS_RENDER_SORT_F32))
+    return fail(c, GS_ERR_INVALID,
+                "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE, GS_RENDER_SCENE_INTERLEAVE and GS_RENDER_SORT_F32 is accepted");
   if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "gs_pick_scene: not on a sharded context");
   if (frame->width == 0 || frame->height == 0 || frame->width > 4096 || frame->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
@@ -2047,6 +2082,7 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   }
   FrameNeeds need{};
   need.scene = !plain;
+  need.f32 = (frame->flags & GS_RENDER_SORT_F32) != 0;
   need.n_views = 1;
   {
     RenderConsts grid;
@@ -2075,6 +2111,7 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   sl.n_sortable = c->n;
   sl.slab = false;
   sl.pick = true;
+  sl.f32 = need.f32;
   sl.cameras = false;
   sl.group = ~0ull;
   sl.color_in[0] = nullptr;
@@ -2118,6 +2155,19 @@ extern "C" int gs_sort_scene_interleaved(gs_context *c, const gs_object *objs, u
   return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count);
 }
 
+extern "C" int gs_sort_scene_flags(gs_context *c, const gs_object *objs, uint32_t n_objs, uint32_t flags, uint32_t *out_idx,
+                                   uint32_t *out_count) {
+  if (!c) return GS_ERR_INVALID;
+  if (flags & ~(uint32_t)(GS_RENDER_SCENE_INTERLEAVE | GS_RENDER_SORT_F32))
+    return fail(c, GS_ERR_INVALID, "gs_sort_scene_flags: no flag other than GS_RENDER_SCENE_INTERLEAVE and GS_RENDER_SORT_F32 is accepted");
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_sort_scene_flags before any push");
+  GS_CUDA(c, cudaSetDevice(c->device));
+  size_t bytes = 0;
+  int rc = build_scene_table(c, objs, n_objs, (flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes);
+  if (rc) return rc;
+  return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count, (flags & GS_RENDER_SORT_F32) != 0);
+}
+
 extern "C" int gs_wait(gs_context *c, uint64_t ticket, gs_stats *stats) {
   if (!c) return GS_ERR_INVALID;
   if (ticket >= c->next_ticket) return fail(c, GS_ERR_INVALID, "gs_wait: unknown ticket");
@@ -2146,6 +2196,8 @@ extern "C" int gs_render_stereo(gs_context *c, const float view[4], const float 
   for (int e = 0; e < 2; ++e) {  // refused before the sort, so that a refusal changes nothing
     if (eyes[e].flags & GS_RENDER_SCENE_INTERLEAVE)
       return fail(c, GS_ERR_INVALID, "GS_RENDER_SCENE_INTERLEAVE is a scene frame flag: gs_render_stereo has no entities");
+    if (eyes[e].flags & GS_RENDER_SORT_F32)
+      return fail(c, GS_ERR_INVALID, "GS_RENDER_SORT_F32: gs_render_stereo draws the stored order of gs_sort (use gs_render_scene_stereo)");
     if ((rc = check_blend8(c, &eyes[e]))) return rc;
   }
   rc = gs_sort(c, view, cutout16_or_null, nullptr, nullptr);

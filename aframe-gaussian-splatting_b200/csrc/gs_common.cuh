@@ -355,6 +355,8 @@ struct gs_context {
   // ---- front-to-back slab path (gs_slab.cu): allocated when a scene first crosses the slab threshold ----
   uint32_t slab_cap = 0;           // splats the per-splat slab buffers are sized for
   uint32_t *key32[2] = {nullptr, nullptr};  // [cap] 16-bit depth key of every splat, kNoKey if not in the sort (one per set)
+  float *zdepth[2] = {nullptr, nullptr};    // [cap] GS_RENDER_SORT_F32 slab frames: the set's copy of depth, which the slab
+                                            // loop's passes read (allocated by the first such frame, freed with key32)
   uint32_t *cidx = nullptr;        // [cap] splat indices of the current slab, in index order
   uint16_t *ckey = nullptr;        // [cap] their keys (scene frames: 24-bit keys in scene_key)
   uint32_t *chunk_cnt[2] = {nullptr, nullptr};  // [kMaxSlabs][chunk_row] per-slab compaction offsets of every 2048-splat chunk (one per set)
@@ -444,6 +446,7 @@ struct gs_context {
     uint32_t n_sortable = 0;                 // splats the frame's sort considers (scene frames: in the entities' ranges)
     bool slab = false;                       // rendered by the front-to-back slab path
     bool pick = false;                       // a pick (gs_pick_scene): bin and pick stages instead of binning and raster
+    bool f32 = false;                        // GS_RENDER_SORT_F32: sorted by the f32 depth (gs_sort.cu Z passes)
     // one camera's pass of a cameras frame (gs_render_scene_cameras): stages launched without graphs.  group: the ticket of
     // the frame's first camera (its cameras hold tickets group .. group + group_n - 1), ~0 for every other frame
     bool cameras = false;
@@ -514,7 +517,9 @@ struct gs_context {
     uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr;
     uint32_t n_views = 0, view_size[gs::kMaxViews] = {}, pad2 = 0; const void *px = nullptr;
     const void *psh = nullptr; uint32_t sh_degree = 0;  // the projection's instantiation and SH table
-    uint32_t interleave = 0;  // scene keys and slab passes of GS_RENDER_SCENE_INTERLEAVE frames
+    uint32_t sort_mode = 0;  // bit 0: scene keys and slab passes of GS_RENDER_SCENE_INTERLEAVE frames; bit 1: the passes of
+                             // GS_RENDER_SORT_F32 frames
+    const void *pz = nullptr;  // zdepth[0] (GS_RENDER_SORT_F32 slab loops bake it)
   } gkey[gs::kGraphDomains];                     // [GraphDomain] (kept apart: a views frame or a pick re-captures only its own graphs)
 
   // ---- fused exchange: one shared allocation per rank = flag rows + a ring of 3 frames, opened by every peer ----
@@ -566,6 +571,10 @@ void launch_depth_cull_scene(gs_context *c, const FrameParams *fp, const SceneTa
 void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *scene, const ObjCounters *octr, FrameCounters *ctr,
                        bool interleave, cudaStream_t st);
 void launch_scene_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 9 launches
+// GS_RENDER_SORT_F32 one-pass frames, after the depth pass (scene NULL: a plain frame): the precise order -> b.order.
+// 12 launches (scene frames: 15, and no launch_scene_keys)
+void launch_sort_f32(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
+                     const FrameBufs &b, cudaStream_t st);
 void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, const FrameCounters *ctr,
                           const FrameBufs &b, cudaStream_t st);
 // views scene frames: every view's projection in one pass -> b.proj_rec / rect (view 0), b.proj_recx / rectx (views 1..)
@@ -630,7 +639,8 @@ void launch_peer_release(gs_context *c, const PeerRows &rows, uint32_t world, ui
 // ---- slab path launchers (gs_slab.cu / gs_raster.cu) ----
 // scene: the slot's scene table (device) of a scene frame, NULL for a plain frame; octr: its per-entity depth ranges;
 // interleave: the scene is keyed and cut as one interleaved order (GS_RENDER_SCENE_INTERLEAVE)
-void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
+// f32: the planning keys of a GS_RENDER_SORT_F32 frame (no Q5 drop), and its depths copied into zdepth[set]
+void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave, bool f32,
                  const ObjCounters *octr, int set, cudaStream_t st);  // keys + bucket histogram
 void launch_slab_plan(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, uint32_t first_target, int n_slabs, cudaStream_t st);
 // stereo: every view's pixel state, closed flags and bins (fp = &views->view[0])
@@ -641,6 +651,9 @@ void launch_slab_begin(gs_context *c, const FrameParams *fp, FrameCounters *ctr,
                        int slab, cudaStream_t st);  // + compaction: 2 launches
 void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
                       const FrameBufs &b, cudaStream_t st);  // 6 launches (scene frames: 9)
+// GS_RENDER_SORT_F32: the slab's precise order from its compacted entries and the set's zdepth (12 launches, scene 15)
+void launch_slab_sort_f32(gs_context *c, FrameCounters *ctr, const SceneTable *scene, bool interleave, const float *zdepth,
+                          const FrameBufs &b, cudaStream_t st);
 // views: the slot's view table of a views scene frame (view 0 into b.proj_rec / rect, views 1.. into b.proj_recx / rectx)
 void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene,
                             const ViewTable *views, const FrameBufs &b, cudaStream_t st);

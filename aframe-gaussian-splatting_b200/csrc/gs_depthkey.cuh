@@ -20,6 +20,13 @@ __device__ __forceinline__ int32_t depth_key(float depth_f32, double min_depth, 
   return js_to_int32(__dmul_rn(__dsub_rn((double)depth_f32, min_depth), depth_inv));
 }
 
+// Slab path of precise frames (GS_RENDER_SORT_F32): the reference key's q = (d - min) * inv truncated and clamped to
+// [0, 65535] (NaN: 0).  Inside the range it is the reference's key; outside it is the nearer end, so no splat is dropped.
+// It never decreases as d increases, which is what lets the slab plan cut the precise order into contiguous slabs.
+__device__ __forceinline__ uint32_t clamp_key16(double q) {
+  return q >= 65535.0 ? 65535u : (q > 0.0 ? (uint32_t)q : 0u);
+}
+
 struct DepthRange {
   double min_depth, depth_inv;
 };
@@ -82,6 +89,14 @@ struct SceneKeyTable {
       const int32_t q = depth_key(d, min[obj], inv[obj]);
       return tag[obj] | ((q >= 0 && q <= 65535) ? (uint32_t)q : 65536u);
     }
+  }
+  // Slab planning key of a precise frame (GS_RENDER_SORT_F32): key<IL>'s layout with key16 = clamp_key16(q), so no entry
+  // is a Q5 drop (IL: key16 << 6 | rank; else rank << 17 | key16).
+  template <bool IL>
+  __device__ uint32_t plan_key(uint32_t i, float d) const {
+    const int obj = scene_find(first, end, n, i);
+    const uint32_t k16 = clamp_key16(__dmul_rn(__dsub_rn((double)d, min[obj]), inv[obj]));
+    return IL ? (k16 << 6 | tag[obj]) : (tag[obj] | k16);
   }
 };
 

@@ -34,6 +34,18 @@
 // Interleaved scene frames (GS_RENDER_SCENE_INTERLEAVE, the IL instantiations) cut the axis of their 22-bit key
 // key16 << 6 | rank: the buckets are depth buckets shared by every entity, no entry is a Q5 drop, and the per-slab sort
 // is SM1I, M2, M3.
+// Precise frames (GS_RENDER_SORT_F32, the F32 instantiations of k_keys) are still planned on these 16-bit axes, but with
+// key16 = clamp_key16(q): the reference's key where it lies in [0, 65535], else the nearer end, so there are no Q5 entries
+// (n_dropped is 0 and plain frames give slab 0 no repeats of splat 0).  Each slab is sorted by the passes of the one-pass
+// precise sort (gs_sort.cu Z<...>) over its compacted entries, reading the f32 depths from the set's zdepth copy.  Why a
+// slab frame equals the one-pass frame: (1) key16 is a non-decreasing function of d within one key space (the plain
+// frame's range, an entity's range, or the interleaved union range), so the bucket of an entry never decreases along the
+// precise order: plain frames (d, index) -> key16 >> 4; default scene frames (rank, d, index) -> (rank, key16 >> (16 - bits));
+// interleaved frames (d, rank, index) -> key16 >> 4 of the one shared range, equal for equal d whatever the rank.  So every
+// slab, a run of buckets, is a contiguous run of the precise order, and the slabs are taken nearest run first.  (2) The
+// compaction keeps index order and the per-slab passes are the same stable LSD passes as the one-pass sort, so each run
+// comes out in exactly its one-pass order.  The raster then composites the same sequence front to back, and the saturation
+// argument above holds unchanged.
 //
 // Views scene frames (gs_render_scene_views, gs_render_scene_stereo) cut their slabs from the HEAD camera's scene order,
 // which is every view's draw order: stage A, the plan and the compaction offsets are those of the scene frame, shared by
@@ -55,11 +67,15 @@ constexpr int kCompactChunk = kCompactThreads * kCompactItems;  // 2048 splats p
 // keys of all splats + bucket histogram (index.js:557-563).  Plain frames: the 16-bit key, kNoKey for a quirk-Q5 drop.
 // SCENE: the 24-bit key of k_scene_keys (each entity's own range); a Q5 drop is a real entry at the top of its entity.
 // IL: the interleaved key of k_scene_keys<true> (the frame's one range), never dropped.
+// F32 (GS_RENDER_SORT_F32): the same layouts with key16 = clamp_key16 (plain frames: a 16-bit key in [0, 65535]), never
+// dropped; the f32 depths also go to zdepth, the set's copy that the slab loop's passes read (the next frame's stage A
+// overwrites depth while this frame's loop runs).
 // ---------------------------------------------------------------------------------------------
-template <bool SCENE, bool IL = false>
+template <bool SCENE, bool IL = false, bool F32 = false>
 __global__ void __launch_bounds__(256) k_keys(const float *__restrict__ depth, const FrameParams *__restrict__ fp,
                                               FrameCounters *ctr, uint32_t *__restrict__ key32, SlabTable *tab,
-                                              const SceneTable *__restrict__ scene, const ObjCounters *__restrict__ octr) {
+                                              const SceneTable *__restrict__ scene, const ObjCounters *__restrict__ octr,
+                                              float *__restrict__ zdepth) {
   __shared__ uint32_t h[kSlabBuckets];
   __shared__ uint32_t s_in, s_drop;
   __shared__ typename std::conditional<SCENE, SceneKeyTable, uint32_t>::type s_ent;
@@ -81,7 +97,13 @@ __global__ void __launch_bounds__(256) k_keys(const float *__restrict__ depth, c
     if (d == GS_DEPTH_REJECT) return kNoKey;
     uint32_t key;
     bool dropped;  // typed-array write out of range (quirk Q5)
-    if constexpr (SCENE) {
+    if constexpr (F32 && SCENE) {
+      key = s_ent.template plan_key<IL>(i, d);
+      dropped = false;
+    } else if constexpr (F32) {
+      key = clamp_key16(__dmul_rn(__dsub_rn((double)d, dr.min_depth), dr.depth_inv));
+      dropped = false;
+    } else if constexpr (SCENE) {
       int obj;
       key = s_ent.template key<IL>(i, d, obj);
       dropped = !IL && (key & 65536u) != 0u;
@@ -102,8 +124,13 @@ __global__ void __launch_bounds__(256) k_keys(const float *__restrict__ depth, c
     uint4 k;
     k.x = key_of(i, d.x); k.y = key_of(i + 1, d.y); k.z = key_of(i + 2, d.z); k.w = key_of(i + 3, d.w);
     *(uint4 *)(key32 + i) = k;
+    if constexpr (F32) *(float4 *)(zdepth + i) = d;
   }
-  if (blockIdx.x == 0 && tid < n - n4) key32[n4 + tid] = key_of(n4 + tid, __ldg(depth + n4 + tid));
+  if (blockIdx.x == 0 && tid < n - n4) {
+    const float d = __ldg(depth + n4 + tid);
+    key32[n4 + tid] = key_of(n4 + tid, d);
+    if constexpr (F32) zdepth[n4 + tid] = d;
+  }
   for (int o = 16; o > 0; o >>= 1) {
     in += __shfl_xor_sync(0xffffffffu, in, o);
     drop += __shfl_xor_sync(0xffffffffu, drop, o);
@@ -407,11 +434,14 @@ static int grid_for(gs_context *c, uint64_t n, int per_cta, int per_sm) {
 }
 
 // interleave: the scene's interleaved instantiations (scene frames only)
-void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
+// f32: a precise frame's planning keys, and its depths into the set's zdepth
+void launch_keys(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave, bool f32,
                  const ObjCounters *octr, int set, cudaStream_t st) {
   cudaMemsetAsync(c->slab_tab[set], 0, sizeof(SlabTable), st);
-  (interleave ? k_keys<true, true> : scene ? k_keys<true> : k_keys<false>)<<<grid_for(c, c->cap, 256 * 8, 8), 256, 0, st>>>(c->depth, fp, ctr, c->key32[set],
-                                                                                        c->slab_tab[set], scene, octr);
+  auto *k = f32 ? (interleave ? k_keys<true, true, true> : scene ? k_keys<true, false, true> : k_keys<false, false, true>)
+                : (interleave ? k_keys<true, true> : scene ? k_keys<true> : k_keys<false>);
+  k<<<grid_for(c, c->cap, 256 * 8, 8), 256, 0, st>>>(c->depth, fp, ctr, c->key32[set], c->slab_tab[set], scene, octr,
+                                                     f32 ? c->zdepth[set] : nullptr);
 }
 
 void launch_slab_plan(gs_context *c, const FrameParams *fp, FrameCounters *ctr, int set, uint32_t first_target, int n_slabs,

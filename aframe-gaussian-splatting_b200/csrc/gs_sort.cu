@@ -23,6 +23,9 @@
 // Interleaved scene frames (GS_RENDER_SCENE_INTERLEAVE): k_scene_keys<true> keys every entity in the frame's one range
 // (22-bit key16 << 6 | rank, out-of-range keys clamped, payload = the splat), and the same three passes give one
 // (key, rank, index) order over all entities.
+// Precise frames (GS_RENDER_SORT_F32): k_radix_*<Z<0..24, ...>> sort by the 31-bit f32 depth key ~bits(d) in four passes,
+// and scene frames add k_radix_*<Z<kRankDigit, ...>> over the draw rank (last: (rank, d, index); first when interleaved:
+// (d, rank, index)).  k_scene_keys is not run: no key16, no Q5.  The slab path runs the same passes over each slab.
 //
 // PLY ingest (gs_push_ply): k_radix_*<P<0>> .. <P<24>> sort the rows by a 32-bit importance key, four stable 8-bit passes
 // (the stable Array.prototype.sort of index.js:668).  Each pass reads the digit through the permutation (key[perm[i]]), so
@@ -682,6 +685,93 @@ void launch_slab_sort(gs_context *c, const FrameParams *fp, FrameCounters *ctr, 
   }
   run_pass(c, S1{{}, ctr, c->ckey, c->cidx, c->idx_a, c->dig_a}, s, c->cap, st);
   run_pass(c, D2{{}, ctr, c->dig_a, c->idx_a, b.order}, s, c->cap, st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Precise frames (GS_RENDER_SORT_F32): the order by the f32 depth d itself, no 16-bit bucket.  Every kept d is < 0, so
+// the 31-bit key ~bits(d) grows as the splat comes nearer: ascending key = farthest first.  Four stable 8-bit passes
+// over it give (d, index); scene frames add one pass over the draw rank, last for (rank, d, index) and first for the
+// interleaved (d, rank, index).  No range and no Q5: every kept splat is drawn once.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t f32_key(float d) { return ~__float_as_uint(d); }
+
+// draw rank of sorted splat `s`: the last entity whose range starts at or before it holds it
+__device__ __forceinline__ uint32_t scene_rank(const SceneTable *__restrict__ scene, uint32_t s) {
+  uint32_t lo = 0, hi = scene->n;
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (scene->obj[mid].first <= s) lo = mid; else hi = mid;
+  }
+  return scene->obj[lo].rank;
+}
+
+constexpr int kRankDigit = -1;
+// Z<kShift, kAll>: digit = bits kShift .. kShift+7 of the element's depth key, or its draw rank (kRankDigit).  The
+// payload is the splat and each pass reads the key through it (depth[splat], as P<kShift> does).  kAll: the elements are
+// the table's splats (the first pass of a one-pass frame: rejected splats are skipped, the kept ones counted into
+// n_inrange); otherwise idx[i], the previous pass's order or the slab's compacted entries.
+template <int kShift, bool kAll>
+struct Z : RadixPass {
+  FrameCounters *ctr;
+  const FrameParams *fp;
+  const SceneTable *scene;  // the rank pass
+  const float *depth;       // one-pass frames: c->depth; slab frames: their set's copy (k_keys)
+  const uint32_t *idx;
+  uint32_t *idx_out;
+  __device__ uint32_t count() const { return kAll ? (ctr->sort.n_valid ? fp->n_splats : 0u) : ctr->sort.n_valid; }
+  __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &) const {
+    const uint32_t s = kAll ? i : idx[i];
+    pay = s;
+    if constexpr (kShift == kRankDigit) {
+      if (kAll && __ldg(depth + s) == GS_DEPTH_REJECT) return kInvalidDigit;
+      return scene_rank(scene, s);
+    } else {
+      const float d = __ldg(depth + s);
+      if (kAll && d == GS_DEPTH_REJECT) return kInvalidDigit;
+      return (f32_key(d) >> kShift) & 255u;
+    }
+  }
+  __device__ void store(uint32_t pos, uint32_t pay, uint32_t) const { idx_out[pos] = pay; }
+  __device__ void scanned(uint32_t total) const {
+    if (kAll && total) atomicAdd(&ctr->sort.n_inrange, total);
+  }
+};
+
+// The passes of a precise order -> order, ping-ponging through idx_a and scene_pay.  kAll: a one-pass frame (the first
+// pass reads every splat); else a slab of the slab path (the first pass reads the slab's compacted entries, src).
+// Plain frames 12 launches, scene frames 15.
+template <bool kAll>
+static void sort_f32(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
+                     const float *depth, const uint32_t *src, uint32_t *order, cudaStream_t st) {
+  const RadixScratch s{c->table_n, c->totals, c->table_n_stride};
+  uint32_t *a = c->idx_a, *b = c->scene_pay;
+  if (scene && interleave) {  // (d, rank, index): the rank is the least significant part
+    run_pass(c, Z<kRankDigit, kAll>{{}, ctr, fp, scene, depth, src, a}, s, c->cap, st);
+    run_pass(c, Z<0, false>{{}, ctr, fp, scene, depth, a, b}, s, c->cap, st);
+    run_pass(c, Z<8, false>{{}, ctr, fp, scene, depth, b, a}, s, c->cap, st);
+    run_pass(c, Z<16, false>{{}, ctr, fp, scene, depth, a, b}, s, c->cap, st);
+    run_pass(c, Z<24, false>{{}, ctr, fp, scene, depth, b, order}, s, c->cap, st);
+    return;
+  }
+  run_pass(c, Z<0, kAll>{{}, ctr, fp, scene, depth, src, a}, s, c->cap, st);
+  run_pass(c, Z<8, false>{{}, ctr, fp, scene, depth, a, b}, s, c->cap, st);
+  run_pass(c, Z<16, false>{{}, ctr, fp, scene, depth, b, a}, s, c->cap, st);
+  if (!scene) {
+    run_pass(c, Z<24, false>{{}, ctr, fp, scene, depth, a, order}, s, c->cap, st);
+    return;
+  }
+  run_pass(c, Z<24, false>{{}, ctr, fp, scene, depth, a, b}, s, c->cap, st);
+  run_pass(c, Z<kRankDigit, false>{{}, ctr, fp, scene, depth, b, order}, s, c->cap, st);  // (rank, d, index)
+}
+
+void launch_sort_f32(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const SceneTable *scene, bool interleave,
+                     const FrameBufs &b, cudaStream_t st) {
+  sort_f32<true>(c, fp, ctr, scene, interleave, c->depth, nullptr, b.order, st);
+}
+
+void launch_slab_sort_f32(gs_context *c, FrameCounters *ctr, const SceneTable *scene, bool interleave, const float *zdepth,
+                          const FrameBufs &b, cudaStream_t st) {
+  sort_f32<false>(c, nullptr, ctr, scene, interleave, zdepth, c->cidx, b.order, st);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -71,9 +71,12 @@ enum {
   GS_RENDER_COLOR_DEVICE = 1u << 6, /* gs_render_scene*: color_in is a device pointer (default: host memory)   */
   GS_RENDER_BLEND_UNORM8 = 1u << 7, /* RGBA8 frames whose bytes are those an RGBA8 framebuffer holds after the
                                        reference's back-to-front blend, rounded after every fragment (below)    */
-  GS_RENDER_SCENE_INTERLEAVE = 1u << 8 /* scene frames and picks: one back-to-front order over every entity's splats,
+  GS_RENDER_SCENE_INTERLEAVE = 1u << 8, /* scene frames and picks: one back-to-front order over every entity's splats,
                                           so overlapping entities blend by depth (see "Interleaved scenes" below);
                                           gs_render, gs_render_async and gs_render_stereo refuse it        */
+  GS_RENDER_SORT_F32 = 1u << 9 /* order the frame by the full f32 depth instead of the reference's 16-bit buckets
+                                  (see "Precise order" below); gs_render_stereo, GS_RENDER_REUSE_SORT, _OUT_TILED,
+                                  _OUT_PEER and sharded contexts refuse it                             */
 };
 
 /*
@@ -398,6 +401,28 @@ GS_API int gs_render_stereo(gs_context *ctx, const float view[4], const float *c
  * (for a whole-table entity, the plain frame) when that frame has n_dropped == 0; and entities with one modelview, no
  * cutout, ranges adjacent in table order and ranks in table order give the default frame of one entity spanning their
  * union range, when that frame has n_dropped == 0.
+ *
+ * Precise order (GS_RENDER_SORT_F32 in gs_render_params.flags; not the reference's behaviour, which stays the default):
+ * the frame is ordered by each splat's f32 depth itself, not by the 16-bit bucket (max - min) / 65535 wide, so one distant
+ * splat no longer coarsens the order of the whole scene.
+ *   - filter: unchanged, each entity's own worker test (its view row, its cutout, index.js:548) in fp64;
+ *   - key: d = (float) depth, the Float32Array value of index.js:549.  Every kept d is < 0.  No range, no ToInt32, no
+ *     clamp and no quirk Q5: every kept splat is drawn once, n_dropped is 0 and every sorted splat is in range.
+ *     min_depth / max_depth are still reported;
+ *   - order, ascending (farthest first): plain frames (d, table index); default scene frames (draw rank, d, table index),
+ *     each entity still drawn whole in objs order; interleaved scene frames (d, draw rank, table index);
+ *   - drawing: unchanged.  Stereo and views frames sort once from the head camera, each camera of a cameras frame sorts on
+ *     its own, and a pick walks this order;
+ *   - scope: gs_render[_async], every gs_render_scene* entry point, every *_target[_async] entry point, the cameras frames
+ *     and gs_pick_scene, on the one-pass and the slab path, with GS_RENDER_STATS where accepted, GS_RENDER_BLEND_UNORM8,
+ *     GS_TARGET_DEPTH_WRITE, SH contexts and host or device buffers;
+ *   - refusals (GS_ERR_INVALID, nothing changed): gs_render_stereo (it draws gs_sort's stored order), together with
+ *     GS_RENDER_REUSE_SORT (which does not sort: a reuse frame draws whichever order is stored, a precise one included),
+ *     with GS_RENDER_OUT_TILED or GS_RENDER_OUT_PEER, and on a sharded context.
+ * Refinement: where the default frame has n_dropped == 0, the precise order refines the default one.  Along it the default
+ * bucket - (rank, key16) with each entity's range, or key16 over the union range when interleaved - never decreases, and
+ * each bucket's run, put back in (draw rank, table index) order, is the default order's.  So a scene whose kept splats
+ * each have a key16 of their own (per entity, or over the union) and no Q5 drop gives the default frame byte for byte.
  */
 #define GS_MAX_OBJECTS 64
 typedef struct gs_object {
@@ -439,6 +464,14 @@ GS_API int gs_sort_scene(gs_context *ctx, const gs_object *objs, uint32_t n_objs
  */
 GS_API int gs_sort_scene_interleaved(gs_context *ctx, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx,
                                      uint32_t *out_count);
+/*
+ * Draw order of a scene frame of these entities with `flags`: GS_RENDER_SCENE_INTERLEAVE and / or GS_RENDER_SORT_F32 (any
+ * other bit: GS_ERR_INVALID).  flags 0 is gs_sort_scene, GS_RENDER_SCENE_INTERLEAVE alone gs_sort_scene_interleaved, and
+ * with GS_RENDER_SORT_F32 the precise order above.  A plain frame's order is that of one whole-table entity with the
+ * frame's modelview.  Arguments and refusals as gs_sort_scene.
+ */
+GS_API int gs_sort_scene_flags(gs_context *ctx, const gs_object *objs, uint32_t n_objs, uint32_t flags, uint32_t *out_idx,
+                               uint32_t *out_count);
 
 /*
  * WebXR on a page of several entities: one scene sort per frame from the HEAD camera (each entity's tick(),
