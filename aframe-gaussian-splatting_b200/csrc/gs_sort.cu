@@ -77,7 +77,7 @@ __global__ void __launch_bounds__(256) k_depth_cull(const float4 *__restrict__ c
   double dmin = INFINITY, dmax = -INFINITY;
   uint32_t cnt = 0;
   const uint32_t stride = gridDim.x * blockDim.x;
-  auto process = [&](uint32_t i, const float4 c, const float s) {
+  auto process = [&](const float4 c, const float s) -> float {
     double depth;
     const bool keep = worker_keep(sc, c, s, depth);
     float out = GS_DEPTH_REJECT;
@@ -87,22 +87,24 @@ __global__ void __launch_bounds__(256) k_depth_cull(const float4 *__restrict__ c
       if (depth > dmax) dmax = depth;
       if (depth < dmin) dmin = depth;
     }
-    depth_out[i] = out;
+    return out;
   };
-  // two splats per thread and step, loads first: twice the bytes in flight per thread (the pass is a pure stream)
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += 2 * stride) {
-    const uint32_t j = i + stride;
-    const bool two = j < n;
-    const float4 c0 = __ldg(cs + i);
-    const float s0 = __ldg(sa + i);
-    float4 c1 = c0;
-    float s1 = s0;
-    if (two) {
-      c1 = __ldg(cs + j);
-      s1 = __ldg(sa + j);
-    }
-    process(i, c0, s0);
-    if (two) process(j, c1, s1);
+  // four splats per thread and step, loads first: four 16 B centres and one 16 B load of their sizes in flight per
+  // thread (the pass is a pure stream; one splat per load left it at under half the HBM rate at 1 M splats)
+  const uint32_t n4 = n & ~3u;
+  for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) * 4u; i < n4; i += stride * 4u) {
+    const float4 c0 = __ldg(cs + i), c1 = __ldg(cs + i + 1), c2 = __ldg(cs + i + 2), c3 = __ldg(cs + i + 3);
+    const float4 s = __ldg((const float4 *)(sa + i));
+    float4 out;
+    out.x = process(c0, s.x);
+    out.y = process(c1, s.y);
+    out.z = process(c2, s.z);
+    out.w = process(c3, s.w);
+    *(float4 *)(depth_out + i) = out;
+  }
+  if (blockIdx.x == 0 && threadIdx.x < n - n4) {  // the last n % 4 splats
+    const uint32_t i = n4 + threadIdx.x;
+    depth_out[i] = process(__ldg(cs + i), __ldg(sa + i));
   }
   // block reduction
   for (int o = 16; o > 0; o >>= 1) {
@@ -321,17 +323,28 @@ __global__ void __launch_bounds__(kRadixThreads) k_radix_hist(Pass p, const Radi
   p.hist_prologue(n);
   for (uint32_t c = blockIdx.x; c < num_chunks; c += gridDim.x) {
     h[tid] = 0;
-    __syncthreads();
+    // every digit of the thread's slice first: kRadixItems loads in flight, none waits behind a shared atomic
     const uint32_t base = c * kRadixTile + warp * (32 * kRadixItems) + lane;
+    uint32_t digit[kRadixItems];
+    auto load_slice = [&](auto tail) {  // tail: the chunk ends past n, every element is checked
 #pragma unroll
-    for (int k = 0; k < kRadixItems; ++k) {
-      const uint32_t i = base + k * 32;
-      if (i < n) {
-        uint32_t pay, carry;
-        const uint32_t digit = p.load(i, pay, carry);
-        if (digit != kInvalidDigit) atomicAdd(&h[digit], 1u);
+      for (int k = 0; k < kRadixItems; ++k) {
+        const uint32_t i = base + k * 32;
+        digit[k] = kInvalidDigit;
+        if (!decltype(tail)::value || i < n) {
+          uint32_t pay, carry;
+          digit[k] = p.load(i, pay, carry);
+        }
       }
-    }
+    };
+    if ((c + 1) * kRadixTile <= n) load_slice(std::false_type{});  // a whole chunk: one block of loads, no branch
+    else load_slice(std::true_type{});
+    __syncthreads();
+    // one shared atomic per element: on H100 this beats a warp-aggregated count (__match_any_sync per step), even for the
+    // concentrated digits of the depth sort's high byte and of the bin id
+#pragma unroll
+    for (int k = 0; k < kRadixItems; ++k)
+      if (digit[k] != kInvalidDigit) atomicAdd(&h[digit[k]], 1u);
     __syncthreads();
     s.table[(size_t)tid * s.stride + c] = h[tid];
     __syncthreads();
@@ -339,57 +352,64 @@ __global__ void __launch_bounds__(kRadixThreads) k_radix_hist(Pass p, const Radi
   p.hist_epilogue();
 }
 
-// grid = 256 CTAs (one per digit)
+// One warp per digit row, kScanRows rows per CTA: grid = 256 / kScanRows CTAs.  A lane takes kScanSpan consecutive
+// chunks of a 32 * kScanSpan block (one shuffle scan of the lanes' sums per block; 256 chunks = 1 M elements in one),
+// and no CTA barrier is needed.
+constexpr int kScanRows = 8;
+constexpr int kScanSpan = 8;
+
 template <class Pass>
-__global__ void __launch_bounds__(256) k_radix_scan(const Pass p, const RadixScratch s) {
+__global__ void __launch_bounds__(32 * kScanRows) k_radix_scan(const Pass p, const RadixScratch s) {
   GS_PDL_ENTRY();
-  __shared__ uint32_t s_warp[8];
-  __shared__ uint32_t s_carry;
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t lane = threadIdx.x & 31, digit = blockIdx.x * kScanRows + (threadIdx.x >> 5);
   const uint32_t n = p.count();
   const uint32_t num_chunks = (n + kRadixTile - 1) / kRadixTile;
-  uint32_t *row = s.table + (size_t)blockIdx.x * s.stride;
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
-  for (uint32_t b = 0; b < num_chunks; b += 256) {
-    const uint32_t i = b + tid;
-    const uint32_t v = (i < num_chunks) ? row[i] : 0u;
-    uint32_t incl = v;
+  uint32_t *row = s.table + (size_t)digit * s.stride;
+  uint32_t carry = 0;
+  for (uint32_t b = 0; b < num_chunks; b += 32 * kScanSpan) {
+    const uint32_t first = b + lane * kScanSpan;
+    uint32_t v[kScanSpan], sum = 0;
+#pragma unroll
+    for (int k = 0; k < kScanSpan; ++k) {
+      v[k] = first + k < num_chunks ? row[first + k] : 0u;
+      sum += v[k];
+    }
+    uint32_t incl = sum;
+#pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
       const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
       if (lane >= (uint32_t)o) incl += t;
     }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    uint32_t wbase = 0;
-    for (uint32_t k = 0; k < warp; ++k) wbase += s_warp[k];
-    const uint32_t carry = s_carry;
-    if (i < num_chunks) row[i] = carry + wbase + incl - v;
-    __syncthreads();
-    if (tid == 255) s_carry = carry + wbase + incl;
-    __syncthreads();
+    uint32_t run = carry + incl - sum;
+#pragma unroll
+    for (int k = 0; k < kScanSpan; ++k) {
+      if (first + k < num_chunks) row[first + k] = run;
+      run += v[k];
+    }
+    carry += __shfl_sync(0xffffffffu, incl, 31);
   }
-  if (tid == 0) {
-    s.totals[blockIdx.x] = s_carry;
-    p.scanned(s_carry);
+  if (lane == 0) {
+    s.totals[digit] = carry;
+    p.scanned(carry);
   }
 }
 
 // 512 threads x 8 elements per chunk: 16 warps rank their 256-element slices independently (an 8-step
-// dependent chain each), then one scan over the 16 warp counters per digit orders the slices.
+// dependent chain each), then a 16-lane shuffle scan over the 16 warp counters of each digit orders the slices.
 constexpr int kScatThreads = 512;
 constexpr int kScatItems = kRadixTile / kScatThreads;  // 8
 constexpr int kScatWarps = kScatThreads / 32;          // 16
+constexpr int kWcntPitch = 257;  // words per warp row of the counters: the 16 rows of a digit fall on 16 different banks
 
 template <class Pass>
 __global__ void __launch_bounds__(kScatThreads, 2) k_radix_scatter(Pass p, const RadixScratch s) {
   GS_PDL_ENTRY();
   constexpr bool kCarry = !std::is_void<typename Pass::Carry>::value;
   using carry_t = typename std::conditional<kCarry, typename Pass::Carry, uint8_t>::type;
-  __shared__ uint32_t wcnt[kScatWarps][256];
+  __shared__ uint32_t wcnt[kScatWarps * kWcntPitch];  // [warp][digit]: the warp's count, scanned into its first rank
   __shared__ uint32_t tile_off[256];  // global slot of the digit's first element MINUS its slot in the staged chunk
-  __shared__ uint32_t s_loc[256];     // slot of the digit's first element in the staged (locally sorted) chunk
-  __shared__ uint32_t s_warp_tot[8];
+  __shared__ uint32_t s_loc[256];     // the chunk's count of each digit, then the slot of its first staged element
+  __shared__ uint32_t s_warp_tot[2][8];
   __shared__ uint32_t s_pay[kRadixTile];
   __shared__ carry_t s_carry[kCarry ? kRadixTile : 1];
   __shared__ uint8_t s_dig[kRadixTile];
@@ -399,91 +419,123 @@ __global__ void __launch_bounds__(kScatThreads, 2) k_radix_scatter(Pass p, const
   const uint32_t num_chunks = (n + kRadixTile - 1) / kRadixTile;
   if (blockIdx.x >= num_chunks) return;
 
-  // block-wide exclusive scan over the 256 digit slots (threads >= 256 contribute 0)
-  auto scan256 = [&](uint32_t v) -> uint32_t {
-    uint32_t incl = v;
+  // block-wide exclusive scan of two values over the 256 digit slots (threads >= 256 contribute 0)
+  auto scan256x2 = [&](uint32_t &a, uint32_t &b) {
+    uint32_t ia = a, ib = b;
+#pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= (uint32_t)o) incl += t;
+      const uint32_t ta = __shfl_up_sync(0xffffffffu, ia, o), tb = __shfl_up_sync(0xffffffffu, ib, o);
+      if (lane >= (uint32_t)o) { ia += ta; ib += tb; }
     }
-    __syncthreads();  // previous users of s_warp_tot are done
-    if (lane == 31 && warp < 8) s_warp_tot[warp] = incl;
+    if (lane == 31 && warp < 8) { s_warp_tot[0][warp] = ia; s_warp_tot[1][warp] = ib; }
     __syncthreads();
-    uint32_t wbase = 0;
-    for (uint32_t k = 0; k < warp && k < 8; ++k) wbase += s_warp_tot[k];
-    return wbase + incl - v;
+    uint32_t wa = 0, wb = 0;
+    for (uint32_t k = 0; k < warp && k < 8; ++k) { wa += s_warp_tot[0][k]; wb += s_warp_tot[1][k]; }
+    a = wa + ia - a;
+    b = wb + ib - b;
   };
 
-  // first output slot of each digit
+  // the pass's digit totals: issued before the chunk, their scan (the first output slot of each digit) waits for the
+  // ranking and shares its block scan
   const uint32_t dtot = tid < 256 ? s.totals[tid] : 0u;
-  const uint32_t dbase = scan256(dtot);
-  if (blockIdx.x == 0 && tid < 256) p.digit_range(tid, dbase, dbase + dtot);
   p.prepare(n);
 
   for (uint32_t c = blockIdx.x; c < num_chunks; c += gridDim.x) {
     // this chunk's per-digit offset: issued first so its latency hides behind the ranking
     const uint32_t toff = tid < 256 ? __ldg(s.table + (size_t)tid * s.stride + c) : 0u;
-    for (uint32_t k = tid; k < kScatWarps * 256; k += kScatThreads) (&wcnt[0][0])[k] = 0u;
     // ---- load (warp-striped: consecutive lanes read consecutive elements) ----
     const uint32_t base = c * kRadixTile + warp * (32 * kScatItems) + lane;
-    uint32_t digit[kScatItems], pay[kScatItems], rank[kScatItems];
-    carry_t carry[kScatItems];
+    // key = digit | carry << 8 in one register (at most 24 bits), kInvalidDigit for a skipped element
+    uint32_t key[kScatItems], pay[kScatItems], rank[kScatItems];
+    auto load_slice = [&](auto tail) {  // as in k_radix_hist
 #pragma unroll
-    for (int k = 0; k < kScatItems; ++k) {
-      const uint32_t i = base + k * 32;
-      uint32_t cv = 0;
-      digit[k] = kInvalidDigit;
-      pay[k] = 0;
-      if (i < n) digit[k] = p.load(i, pay[k], cv);
-      carry[k] = (carry_t)cv;
-    }
+      for (int k = 0; k < kScatItems; ++k) {
+        const uint32_t i = base + k * 32;
+        uint32_t cv = 0;
+        key[k] = kInvalidDigit;
+        pay[k] = 0;
+        if (!decltype(tail)::value || i < n) {
+          const uint32_t d = p.load(i, pay[k], cv);
+          if (d != kInvalidDigit) key[k] = d | (kCarry ? (uint32_t)(carry_t)cv << 8 : 0u);
+        }
+      }
+    };
+    if ((c + 1) * kRadixTile <= n) load_slice(std::false_type{});
+    else load_slice(std::true_type{});
+    for (uint32_t k = tid; k < kScatWarps * kWcntPitch; k += kScatThreads) wcnt[k] = 0u;
     __syncthreads();
     // ---- stable rank inside the warp (input order = lane order within a step, steps in order) ----
+    uint32_t *const my_cnt = wcnt + warp * kWcntPitch;
 #pragma unroll
     for (int k = 0; k < kScatItems; ++k) {
-      const uint32_t d = digit[k];
+      const uint32_t d = key[k] == kInvalidDigit ? kInvalidDigit : key[k] & 255u;
       const uint32_t peers = __match_any_sync(0xffffffffu, d);
       const uint32_t lt = __popc(peers & ((1u << lane) - 1u));
       uint32_t prior = 0;
-      if (d != kInvalidDigit) prior = wcnt[warp][d];
+      if (d != kInvalidDigit) prior = my_cnt[d];
       __syncwarp();
-      if (d != kInvalidDigit && lt == 0) wcnt[warp][d] = prior + __popc(peers);
+      if (d != kInvalidDigit && lt == 0) my_cnt[d] = prior + __popc(peers);
       __syncwarp();
       rank[k] = prior + lt;
     }
     __syncthreads();
-    // ---- thread `tid` < 256 owns digit `tid`: exclusive scan over the warps, then over the digits ----
-    uint32_t total = 0;
-    if (tid < 256) {
+    // ---- exclusive scan of each digit's 16 warp counters: lane w of a half-warp holds warp w's count, a half-warp a
+    //      digit, a warp the digits d and d + 16 of its step (conflict-free with the padded rows) ----
+    {
+      const uint32_t w = lane & 15;
 #pragma unroll
-      for (int w = 0; w < kScatWarps; ++w) {
-        const uint32_t cnt = wcnt[w][tid];
-        wcnt[w][tid] = total;
-        total += cnt;
+      for (int r = 0; r < 8; ++r) {
+        const uint32_t d = 32 * (warp >> 1) + 8 * (warp & 1) + r + 16 * (lane >> 4);
+        const uint32_t v = wcnt[w * kWcntPitch + d];
+        uint32_t incl = v;
+#pragma unroll
+        for (int o = 1; o < 16; o <<= 1) {
+          const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o, 16);
+          if (w >= (uint32_t)o) incl += t;
+        }
+        wcnt[w * kWcntPitch + d] = incl - v;
+        if (w == 15) s_loc[d] = incl;
       }
     }
-    const uint32_t loc = scan256(total);
+    __syncthreads();
+    // ---- thread `tid` < 256 owns digit `tid`: its slot in the staged chunk and its first output slot ----
+    const uint32_t cnt = tid < 256 ? s_loc[tid] : 0u;
+    uint32_t loc = cnt, dbase = dtot;
+    scan256x2(loc, dbase);  // its barrier also ends every read of the counts in s_loc
     if (tid < 256) {
+      if (c == 0) p.digit_range(tid, dbase, dbase + dtot);
       s_loc[tid] = loc;
       tile_off[tid] = dbase + toff - loc;
-      if (tid == 255) s_total = loc + total;
+      if (tid == 255) s_total = loc + cnt;
     }
     __syncthreads();
     // ---- stage the chunk in shared memory in sorted order ----
 #pragma unroll
     for (int k = 0; k < kScatItems; ++k) {
-      const uint32_t d = digit[k];
-      if (d == kInvalidDigit) continue;
-      const uint32_t lp = s_loc[d] + wcnt[warp][d] + rank[k];
+      if (key[k] == kInvalidDigit) continue;
+      const uint32_t d = key[k] & 255u;
+      const uint32_t lp = s_loc[d] + my_cnt[d] + rank[k];
       s_pay[lp] = pay[k];
       s_dig[lp] = (uint8_t)d;
-      if (kCarry) s_carry[lp] = carry[k];
+      if (kCarry) s_carry[lp] = (carry_t)(key[k] >> 8);
     }
     __syncthreads();
-    // ---- write out: consecutive threads write consecutive slots of the same digit run (coalesced) ----
+    // ---- write out: consecutive threads write consecutive slots of the same digit run (coalesced); two slots per
+    //      thread and step, both read from shared memory before either store (a gathering store has two loads in flight) ----
     const uint32_t nvalid = s_total;
-    for (uint32_t i = tid; i < nvalid; i += kScatThreads)
-      p.store(tile_off[s_dig[i]] + i, s_pay[i], kCarry ? (uint32_t)s_carry[i] : 0u);
+    for (uint32_t i = tid; i < nvalid; i += 2 * kScatThreads) {
+      const uint32_t j = i + kScatThreads;
+      const bool two = j < nvalid;
+      const uint32_t pos0 = tile_off[s_dig[i]] + i, pay0 = s_pay[i], car0 = kCarry ? (uint32_t)s_carry[i] : 0u;
+      uint32_t pos1 = 0, pay1 = 0, car1 = 0;
+      if (two) {
+        pos1 = tile_off[s_dig[j]] + j;
+        pay1 = s_pay[j];
+        car1 = kCarry ? (uint32_t)s_carry[j] : 0u;
+      }
+      p.store(pos0, pay0, car0);
+      if (two) p.store(pos1, pay1, car1);
+    }
     __syncthreads();
   }
 }
@@ -492,13 +544,25 @@ template <class Pass>
 static void run_pass(gs_context *c, const Pass &p, const RadixScratch &s, uint64_t n_max, cudaStream_t st) {
   const int grid = persistent_grid(c, n_max, kRadixTile, 8);
   launch_chain(c, k_radix_hist<Pass>, grid, kRadixThreads, st, p, s);
-  launch_chain(c, k_radix_scan<Pass>, 256, 256, st, p, s);
+  launch_chain(c, k_radix_scan<Pass>, 256 / kScanRows, 32 * kScanRows, st, p, s);
   launch_chain(c, k_radix_scatter<Pass>, grid, kScatThreads, st, p, s);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Depth sort: index.js:557-567 as two stable 8-bit passes over the 16-bit key -> b.order (6 launches)
 // ---------------------------------------------------------------------------------------------
+// js_to_int32 (gs_depthkey.cuh) restated without branches, equal for every double: ToInt32 is the low 32 bits of trunc(q)
+// in two's complement, which shifting q's significand by its exponent gives directly (|q| < 1, inf and NaN: 0).  Its
+// straight-line code lets a radix pass issue the depth loads of all its elements before the first key is formed; the
+// fmod branch of js_to_int32 made each load wait for the previous element's key.
+__device__ __forceinline__ int32_t js_to_int32_flat(double q) {
+  const unsigned long long b = (unsigned long long)__double_as_longlong(q);
+  const int e = (int)((b >> 52) & 0x7FFu) - 1075;  // q = m * 2^e for a normal q; inf / NaN give e = 972
+  const unsigned long long m = (b & 0xFFFFFFFFFFFFFull) | 0x10000000000000ull;
+  const uint32_t lo = e >= 32 ? 0u : e >= 0 ? (uint32_t)(m << e) : e > -53 ? (uint32_t)(m >> -e) : 0u;
+  return (int32_t)((b >> 63) ? 0u - lo : lo);
+}
+
 // D1: low key byte of every splat the worker filter kept.  Counts the entries in range and those the reference's
 // typed-array store drops (quirk Q5).
 struct D1 : RadixPass {
@@ -512,14 +576,16 @@ struct D1 : RadixPass {
   __device__ uint32_t count() const { return ctr->sort.n_valid ? fp->n_splats : 0u; }
   __device__ void prepare(uint32_t n) { if (n) dr = load_depth_range(ctr); }
   __device__ uint32_t load(uint32_t i, uint32_t &pay, uint32_t &carry) {
+    // no branch on the loaded depth: the kernel's loads of its next elements need not wait for this one
     const float d = __ldg(depth + i);
-    if (d == GS_DEPTH_REJECT) return kInvalidDigit;
-    const int32_t key = depth_key(d, dr.min_depth, dr.depth_inv);
-    if (key < 0 || key > 65535) { ++n_drop; return kInvalidDigit; }  // typed-array store out of range: dropped (quirk Q5)
-    ++n_in;
+    const bool kept = d != GS_DEPTH_REJECT;
+    const int32_t key = js_to_int32_flat(__dmul_rn(__dsub_rn((double)d, dr.min_depth), dr.depth_inv));  // depth_key
+    const bool in = key >= 0 && key <= 65535;  // else the typed-array store drops it (quirk Q5)
+    n_drop += kept && !in;
+    n_in += kept && in;
     pay = i;
     carry = (uint32_t)key >> 8;
-    return key & 255;
+    return kept && in ? (uint32_t)key & 255u : kInvalidDigit;
   }
   __device__ void store(uint32_t pos, uint32_t pay, uint32_t carry) const { idx_out[pos] = pay; hi_out[pos] = (uint8_t)carry; }
   __device__ void hist_epilogue() {
