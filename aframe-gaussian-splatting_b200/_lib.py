@@ -20,6 +20,7 @@ GS_MAX_VIEWS = 4
 GS_MAX_CAMERAS = 6
 GS_TARGET_DEVICE = 1
 GS_TARGET_DEPTH_WRITE = 2
+GS_CROP_KEEP_INSIDE, GS_CROP_KEEP_OUTSIDE = 0, 1
 
 
 class GsStats(C.Structure):
@@ -53,6 +54,11 @@ class GsObject(C.Structure):
         ("first", C.c_uint32), ("count", C.c_uint32), ("modelview", C.c_float * 16),
         ("has_cutout", C.c_int32), ("cutout16", C.c_float * 16),
     ]
+
+
+class GsCropBox(C.Structure):
+    """gs_crop_box: one entity range of gs_crop, its mode and its box (the entity's worldToCutout)."""
+    _fields_ = [("first", C.c_uint32), ("count", C.c_uint32), ("mode", C.c_uint32), ("box16", C.c_float * 16)]
 
 
 GS_PICK_NONE = 0xFFFFFFFF
@@ -92,6 +98,7 @@ SYMBOLS = {
     "gs_insert_splats": (C.c_int, [_P, C.c_uint32, _P, C.c_uint32]),
     "gs_insert_ply": (C.c_int, [_P, C.c_uint32, _P, C.c_size_t, _P, C.POINTER(C.c_uint32)]),
     "gs_erase": (C.c_int, [_P, C.c_uint32, C.c_uint32]),
+    "gs_crop": (C.c_int, [_P, C.POINTER(GsCropBox), C.c_uint32, C.POINTER(C.c_uint32)]),
     "gs_push_packed": (C.c_int, [_P, _P, _P, _P, C.c_uint32]),
     "gs_num_splats": (C.c_int, [_P, C.POINTER(C.c_uint32)]),
     "gs_read_packed": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P]),

@@ -420,6 +420,23 @@ class SplatScene:
         self._order.append(component)
         self._range[id(component)] = [self.renderer.num_splats, 0]
 
+    def crop(self, component: GaussianSplattingComponent, inside: bool = True, box=None) -> int:
+        """Apply a box to the entity's splats once, on the device (gs_crop): inside=True keeps the splats inside the box,
+        inside=False erases them.  box: a worldToCutout matrix (16 floats, column-major); None takes the entity's current
+        cutout, the matrix its frames use (ValueError if it has none).  The entity keeps its place in the table: its range
+        shrinks, the entities behind it move down, and later pushes append at its new end.  Returns the splats it kept.
+        A cropped entity may keep its cutout attached: every splat left is inside it, so its frames are the same either
+        way (where a frame drops no splat, quirk Q5)."""
+        if box is None:
+            if component.cutout is None:
+                raise ValueError("SplatScene.crop: the entity has no cutout; pass box=")
+            box = world_to_cutout(component.cutout, component.object).elements
+        first, count = self._range[id(component)]
+        kept = int(self.renderer.crop([(first, count, np.asarray(box, np.float32), inside)])[0])
+        self._range[id(component)][1] = kept
+        self._shift_after(component, kept - count)
+        return kept
+
     def objects(self, width: int, height: int, camera=None):
         """(shared FrameInputs of the draw, [SceneObject per entity in draw order]) for a width x height viewport."""
         frames = [e.frame_inputs(width, height, camera) for e in self.entities]

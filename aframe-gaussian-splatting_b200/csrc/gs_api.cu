@@ -677,6 +677,95 @@ extern "C" int gs_erase(gs_context *c, uint32_t first, uint32_t count) {
   return GS_OK;
 }
 
+// gs_crop (gs_crop.cu): the ranges are validated and sorted first, so a refusal changes nothing.  Passes 1-2 count what
+// each range keeps; the counts come back to the host, which sizes the temporary (the failure point that leaves the table
+// unchanged) and stops there when nothing is removed; pass 3 compacts the rows behind the first removed one.
+extern "C" int gs_crop(gs_context *c, const gs_crop_box *boxes, uint32_t n_boxes, uint32_t *out_counts) {
+  if (!c) return GS_ERR_INVALID;
+  if (!boxes || n_boxes == 0 || n_boxes > (uint32_t)GS_MAX_OBJECTS)
+    return fail(c, GS_ERR_INVALID, "gs_crop: between 1 and GS_MAX_OBJECTS boxes");
+  std::vector<uint32_t> idx;  // non-empty boxes, by first row
+  for (uint32_t i = 0; i < n_boxes; ++i) {
+    if ((uint64_t)boxes[i].first + boxes[i].count > c->n) return fail(c, GS_ERR_INVALID, "gs_crop: a range runs past the resident splats");
+    if (boxes[i].mode != GS_CROP_KEEP_INSIDE && boxes[i].mode != GS_CROP_KEEP_OUTSIDE)
+      return fail(c, GS_ERR_INVALID, "gs_crop: mode is GS_CROP_KEEP_INSIDE or GS_CROP_KEEP_OUTSIDE");
+    if (boxes[i].count) idx.push_back(i);
+  }
+  std::sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return boxes[a].first < boxes[b].first; });
+  for (size_t j = 1; j < idx.size(); ++j)
+    if ((uint64_t)boxes[idx[j - 1]].first + boxes[idx[j - 1]].count > boxes[idx[j]].first)
+      return fail(c, GS_ERR_INVALID, "gs_crop: ranges overlap");
+  CropTable t;
+  memset(&t, 0, sizeof(t));
+  t.n = (uint32_t)idx.size();
+  for (size_t j = 0; j < idx.size(); ++j) {
+    const gs_crop_box &b = boxes[idx[j]];
+    for (int e = 0; e < 16; ++e) t.r[j].box[e] = (double)b.box16[e];
+    t.r[j].first = b.first;
+    t.r[j].end = b.first + b.count;
+    t.r[j].keep_inside = b.mode == GS_CROP_KEEP_INSIDE ? 1u : 0u;
+  }
+  GS_CUDA(c, cudaSetDevice(c->device));
+  int rc = drain(c);  // frames in flight read the table (as for gs_erase)
+  if (rc) return rc;
+  std::vector<uint32_t> kept(kMaxObjects, 0u);
+  uint32_t removed = 0, r0 = 0xFFFFFFFFu;
+  const uint32_t lo = t.n ? t.r[0].first : 0u, n = c->n;
+  cudaStream_t st = c->push_stream;
+  CropScratch s{};
+  void *tmp = nullptr;
+  auto release = [&]() {
+    if (s.tab) cudaFreeAsync(s.tab, st);
+    if (tmp) cudaFreeAsync(tmp, st);
+  };
+  if (t.n) {
+    const uint32_t chunks = crop_chunks(n - lo);
+    const size_t tab_bytes = (sizeof(CropTable) + 15) & ~(size_t)15;
+    cudaError_t e = cudaMallocAsync((void **)&s.tab, tab_bytes + sizeof(uint32_t) * ((size_t)chunks + 2 + kMaxObjects), st);
+    if (e) {
+      cudaGetLastError();  // an allocation failure is not sticky
+      s.tab = nullptr;
+      GS_CUDA(c, e);
+    }
+    s.kept = (uint32_t *)((char *)s.tab + tab_bytes);
+    s.first_drop = s.kept + kMaxObjects;
+    s.chunk_cnt = s.first_drop + 1;
+    if (!e) e = cudaMemcpyAsync(s.tab, &t, sizeof(CropTable), cudaMemcpyHostToDevice, st);
+    if (!e) e = cudaMemsetAsync(s.kept, 0, sizeof(uint32_t) * kMaxObjects, st);
+    if (!e) e = cudaMemsetAsync(s.first_drop, 0xFF, sizeof(uint32_t), st);
+    if (!e) {
+      launch_crop_count(c, s, lo, n, st);
+      e = cudaGetLastError();
+    }
+    if (!e) e = cudaMemcpyAsync(kept.data(), s.kept, sizeof(uint32_t) * t.n, cudaMemcpyDeviceToHost, st);
+    if (!e) e = cudaMemcpyAsync(&r0, s.first_drop, sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
+    if (!e) e = cudaStreamSynchronize(st);
+    for (uint32_t j = 0; j < t.n && !e; ++j) removed += (t.r[j].end - t.r[j].first) - kept[j];
+    if (!e && removed) {
+      const uint32_t moved = n - r0 - removed;  // the kept rows behind the first removed one
+      if (moved && (e = cudaMallocAsync(&tmp, crop_tmp_bytes(moved, c->sh ? c->sh_vecs : 0u), st))) {
+        cudaGetLastError();
+        tmp = nullptr;
+      }
+      if (!e) {
+        launch_crop_write(c, s, lo, r0, n, moved, tmp, st);
+        e = cudaGetLastError();
+      }
+    }
+    release();
+    GS_CUDA(c, e);
+  }
+  if (out_counts) {
+    for (uint32_t i = 0; i < n_boxes; ++i) out_counts[i] = 0;  // empty ranges keep 0
+    for (size_t j = 0; j < idx.size(); ++j) out_counts[idx[j]] = kept[j];
+  }
+  GS_CUDA(c, cudaEventRecord(c->push_done, st));
+  c->n -= removed;
+  c->pushed = true;
+  c->have_order = false;
+  return GS_OK;
+}
+
 // pinned staging of the PLY path, created on first use
 static int ensure_ply_staging(gs_context *c) {
   for (int i = 0; i < 2; ++i) {

@@ -99,6 +99,22 @@ struct SortConsts {
   int has_cutout;
 };
 
+// The worker's cutout test (index.js:533 -> mul(cutout, x, -y, z) of index.js:492-500, Q12: centre only, y negated), in
+// fp64 with every operation rounded: true when no coordinate of the mapped centre lies outside [-0.5, 0.5].  A NaN
+// compares false, so a NaN centre is inside.  The one definition of "inside" for frames (worker_keep) and gs_crop.
+__device__ __forceinline__ bool cutout_inside(const double *e, const double x, const double y, const double z) {
+  const double ny = -y;
+  const double w = __ddiv_rn(
+      1.0, __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[3], x), __dmul_rn(e[7], ny)), __dmul_rn(e[11], z)), e[15]));
+  const double c0 = __dmul_rn(
+      __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[0], x), __dmul_rn(e[4], ny)), __dmul_rn(e[8], z)), e[12]), w);
+  const double c1 = __dmul_rn(
+      __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[1], x), __dmul_rn(e[5], ny)), __dmul_rn(e[9], z)), e[13]), w);
+  const double c2 = __dmul_rn(
+      __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[2], x), __dmul_rn(e[6], ny)), __dmul_rn(e[10], z)), e[14]), w);
+  return !(c0 < -0.5 || c0 > 0.5 || c1 < -0.5 || c1 > 0.5 || c2 < -0.5 || c2 > 0.5);
+}
+
 // Per-frame inputs, resident in device memory (one copy per pipeline slot) so that the whole frame is a static
 // CUDA graph: a 400-byte host->device copy of this struct is the only per-frame input traffic.
 constexpr int kMaxPeers = 16;
@@ -590,6 +606,41 @@ void launch_pack_perm(gs_context *c, const uint8_t *rows_dev, const uint32_t *pe
 size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len, uint32_t sh_vecs);
 // k_move_rows: one launch for disjoint ranges, else two through tmp
 void launch_move_rows(gs_context *c, uint32_t from, uint32_t to, uint32_t len, void *tmp, cudaStream_t st);
+// one row span of the table arrays (or of a temporary laid out like them): centres, cov/colour, size_alpha, SH rows
+struct RowSpan {
+  float4 *cs;
+  uint4 *cc;
+  float *sa;
+  uint4 *sh;  // NULL on a degree-0 context
+};
+RowSpan table_span(gs_context *c, uint32_t row);
+// k_move_rows over n rows of two disjoint spans (size_alpha as float4 when both share their alignment mod 16 B)
+void launch_copy_rows(const RowSpan &src, const RowSpan &dst, uint32_t n, uint32_t sh_vecs, cudaStream_t st);
+// gs_crop (gs_crop.cu): the ranges of one crop, sorted by first, and the per-call device scratch of its passes
+struct CropRange {
+  double box[16];        // the entity's worldToCutout, widened as SortConsts.cutout is
+  uint32_t first, end;   // rows [first, end) of the table, non-empty
+  uint32_t keep_inside;  // GS_CROP_KEEP_INSIDE: keep the rows cutout_inside accepts; else keep the others
+  uint32_t pad;
+};
+struct CropTable {
+  uint32_t n, pad;
+  CropRange r[kMaxObjects];
+};
+struct CropScratch {
+  CropTable *tab;        // device copy of the table
+  uint32_t *chunk_cnt;   // kept rows per chunk of [lo, N), exclusive-scanned in place (chunks + 1 words)
+  uint32_t *kept;        // kept rows per range (kMaxObjects words; zeroed by the caller)
+  uint32_t *first_drop;  // first removed row (0xFFFFFFFF: none; set by the caller)
+};
+uint32_t crop_chunks(uint32_t rows);  // chunks of the compaction over `rows` rows
+// pass 1 and 2 over rows [lo, n): per-chunk and per-range kept counts, the first removed row, the chunk offsets
+void launch_crop_count(gs_context *c, const CropScratch &s, uint32_t lo, uint32_t n, cudaStream_t st);
+// bytes of the temporary that holds `kept` rows written behind row r0 (crop_write)
+size_t crop_tmp_bytes(uint32_t kept, uint32_t sh_vecs);
+// pass 3: the kept rows of [r0, n) (r0 = the first removed row) into tmp, in order, then back into the table at r0
+void launch_crop_write(gs_context *c, const CropScratch &s, uint32_t lo, uint32_t r0, uint32_t n, uint32_t kept, void *tmp,
+                       cudaStream_t st);
 // PLY push: decode `rows` whole rows of a staged body chunk into .splat rows + importance keys at [first_row, ...);
 // sh (SH contexts, else NULL): the rows' coefficients into sh_rows (sh->vecs words per row), in file order too
 void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,

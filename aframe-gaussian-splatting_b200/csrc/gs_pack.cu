@@ -3,7 +3,8 @@
 //   k_pack_perm : row perm[j] of the decoded PLY rows -> slot first + j, optionally also written out in that order
 //                 (gs_push_ply: the gather of processPlyBuffer's importance order fused with the pack; on an SH context
 //                 the row's coefficients are gathered with it)
-//   k_move_rows : rows [from, from+len) of the table -> [to, to+len) (gs_insert_* / gs_erase open or close a gap)
+//   k_move_rows : rows [from, from+len) of the table -> [to, to+len) (gs_insert_* / gs_erase open or close a gap; gs_crop
+//                 copies its compacted rows back with it)
 //
 // One thread per .splat row, all arithmetic in fp64 exactly as JavaScript evaluates it (Three.js r147
 // Matrix4.compose / transpose / scale / premultiply restated entry by entry, sums left to right, no FMA):
@@ -149,13 +150,7 @@ __global__ void __launch_bounds__(256) k_pack_perm(const uint4 *__restrict__ row
 // ranges never overlap within one launch (an overlapping move goes through a temporary, launch_move_rows), so the
 // accesses are restrict.  The 16 B records (and an SH context's sh_vecs words of coefficients) are copied as they are;
 // size_alpha goes as float4 when source and destination share their alignment mod 16 B (sa_vec), with up to 3 scalar
-// rows before the first aligned float4 (sa_head) and up to 3 after the last.
-struct RowSpan {
-  float4 *cs;
-  uint4 *cc;
-  float *sa;
-  uint4 *sh;  // NULL on a degree-0 context
-};
+// rows before the first aligned float4 (sa_head) and up to 3 after the last.  (RowSpan: gs_common.cuh.)
 
 __global__ void __launch_bounds__(256) k_move_rows(const RowSpan src, const RowSpan dst, uint32_t n, uint32_t sa_head,
                                                    uint32_t sa_vec, uint32_t sh_vecs) {
@@ -181,12 +176,12 @@ __global__ void __launch_bounds__(256) k_move_rows(const RowSpan src, const RowS
   }
 }
 
-static RowSpan table_span(gs_context *c, uint32_t row) {
+RowSpan table_span(gs_context *c, uint32_t row) {
   return RowSpan{c->center_scale + row, c->cov_color + row, c->size_alpha + row,
                  c->sh ? c->sh + (size_t)row * c->sh_vecs : nullptr};
 }
 
-static void launch_copy_rows(const RowSpan &src, const RowSpan &dst, uint32_t n, uint32_t sh_vecs, cudaStream_t st) {
+void launch_copy_rows(const RowSpan &src, const RowSpan &dst, uint32_t n, uint32_t sh_vecs, cudaStream_t st) {
   const uintptr_t s = (uintptr_t)src.sa, d = (uintptr_t)dst.sa;
   const uint32_t vec = ((s ^ d) & 15u) == 0, head = vec ? std::min<uint32_t>(n, (uint32_t)((16u - (d & 15u)) & 15u) / 4u) : 0;
   k_move_rows<<<(n + 255) / 256, 256, 0, st>>>(src, dst, n, head, vec, sh_vecs);

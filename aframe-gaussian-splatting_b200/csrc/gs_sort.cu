@@ -49,21 +49,8 @@ __device__ __forceinline__ bool worker_keep(const SortConsts &sc, const float4 c
   // index.js:519-523
   depth = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(sc.view[0], x), __dmul_rn(sc.view[1], y)), __dmul_rn(sc.view[2], z)),
                     sc.view[3]);
-  bool in_box = true;
-  if (sc.has_cutout) {
-    // index.js:533 -> mul(cutout, x, -y, z) of index.js:492-500 (Q12: centre only, y negated)
-    const double *e = sc.cutout;
-    const double ny = -y;
-    const double w = __ddiv_rn(
-        1.0, __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[3], x), __dmul_rn(e[7], ny)), __dmul_rn(e[11], z)), e[15]));
-    const double c0 = __dmul_rn(
-        __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[0], x), __dmul_rn(e[4], ny)), __dmul_rn(e[8], z)), e[12]), w);
-    const double c1 = __dmul_rn(
-        __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[1], x), __dmul_rn(e[5], ny)), __dmul_rn(e[9], z)), e[13]), w);
-    const double c2 = __dmul_rn(
-        __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[2], x), __dmul_rn(e[6], ny)), __dmul_rn(e[10], z)), e[14]), w);
-    if (c0 < -0.5 || c0 > 0.5 || c1 < -0.5 || c1 > 0.5 || c2 < -0.5 || c2 > 0.5) in_box = false;
-  }
+  // index.js:533 (cutout_inside: the same test gs_crop applies to the table)
+  const bool in_box = !sc.has_cutout || cutout_inside(sc.cutout, x, y, z);
   // index.js:548
   return (depth < 0.0) && ((double)s > __dmul_rn(-0.0001, depth)) && in_box;
 }

@@ -146,6 +146,22 @@ class SplatContext:
         """gs_erase: remove splats [first, first+count); the splats behind them move down by count."""
         self._check(self._lib.gs_erase(self._h, int(first), int(count)))
 
+    def crop(self, boxes) -> np.ndarray:
+        """gs_crop: crop table ranges to a box, or erase what lies inside it, on the device.  boxes: a sequence of
+        (first, count, box16, keep_inside=True), one per entity range, box16 its worldToCutout (16 floats, column-major).
+        keep_inside=True keeps the rows inside the box, False the rows outside it.  The rows behind the first removed
+        one move down in order.  Returns the rows each range kept (uint32)."""
+        arr = (_lib.GsCropBox * max(len(boxes), 1))()
+        for i, b in enumerate(boxes):
+            first, count, box16 = b[:3]
+            keep_inside = True if len(b) < 4 else bool(b[3])
+            arr[i].first, arr[i].count = int(first), int(count)
+            arr[i].mode = _lib.GS_CROP_KEEP_INSIDE if keep_inside else _lib.GS_CROP_KEEP_OUTSIDE
+            arr[i].box16[:] = [float(v) for v in np.asarray(box16, np.float32).reshape(16)]
+        counts = np.zeros(max(len(boxes), 1), np.uint32)
+        self._check(self._lib.gs_crop(self._h, arr, len(boxes), counts.ctypes.data_as(C.POINTER(C.c_uint32))))
+        return counts[:len(boxes)]
+
     def push_packed(self, center_scale: np.ndarray, cov_color: np.ndarray, size_alpha: np.ndarray) -> None:
         cs = np.ascontiguousarray(center_scale, dtype=np.float32).reshape(-1, 4)
         cc = np.ascontiguousarray(cov_color, dtype=np.uint32).reshape(-1, 4)

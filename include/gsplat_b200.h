@@ -247,6 +247,39 @@ GS_API int gs_insert_ply(gs_context *ctx, uint32_t at, const void *ply, size_t b
 GS_API int gs_erase(gs_context *ctx, uint32_t first, uint32_t count);
 
 /*
+ * gs_crop: crop entity ranges to a box, or erase what lies inside it, on the device.  A page's cutout box (cutoutEntity,
+ * index.js:443-448, 533) hides the splats outside it in every frame, at the cost of testing every resident splat per
+ * frame; when the box and the entity no longer move relative to each other, one gs_crop applies it to the table instead.
+ * It is also the first step of cleaning a capture: crop it to a box, or delete the floaters inside one.
+ *
+ * Box i covers rows [first, first+count) of the resident table (one entity's range).  A row of it is INSIDE exactly when
+ * the cutout branch of the frames' worker filter lets it through with box16 as the cutout: mul(box, x, -y, z) of the
+ * row's centre in fp64 (box16 widened to double, every operation rounded, index.js:492-500), each coordinate then within
+ * [-0.5, 0.5].  A NaN compares false, so a NaN centre is inside, as it is for the cutout.
+ *   - GS_CROP_KEEP_INSIDE keeps the rows inside (crop to the box); GS_CROP_KEEP_OUTSIDE keeps the others (erase inside).
+ *   - Each range keeps its rows in their relative order, and rows outside every range are kept.  Every row behind the
+ *     first removed row moves down, its SH row (gs_set_sh_degree) with it; N shrinks by the rows removed.
+ *   - out_counts (host, n_boxes entries, or NULL): the rows box i kept.
+ *   - Table-edit rules as gs_erase: the call waits for the frames in flight, runs behind any queued push, and after it the
+ *     draw order is stale.  A crop that removes nothing changes no byte of the table; one that removes every row leaves
+ *     N = 0, and the next sort or render returns GS_ERR_EMPTY.
+ *   - GS_ERR_INVALID, nothing changed: boxes NULL, n_boxes 0 or above GS_MAX_OBJECTS, a range past the resident splats,
+ *     overlapping ranges (they may come in any order; count 0 is allowed and keeps 0), a mode other than the two.
+ *   - Its stream-ordered temporary holds the rows that move, 36 B each plus the SH row of an SH context; it is allocated
+ *     before anything is written, so GS_ERR_OOM leaves the table unchanged.
+ * A frame of the cropped table equals the frame of the uncropped one with the box as the entity's cutout, byte for byte,
+ * wherever that frame drops no splat (n_dropped == 0: quirk Q5 repeats an entity's first splat, which the crop may
+ * change).  So a cropped entity may keep its cutout: every row left passes it.
+ */
+enum { GS_CROP_KEEP_INSIDE = 0, GS_CROP_KEEP_OUTSIDE = 1 };
+typedef struct gs_crop_box {
+  uint32_t first, count;   /* rows [first, first+count) of the resident table: one entity's range                    */
+  uint32_t mode;           /* GS_CROP_KEEP_INSIDE (crop to the box) or GS_CROP_KEEP_OUTSIDE (erase what is inside)   */
+  float box16[16];         /* the entity's worldToCutout (index.js:443-448), as gs_object.cutout16                   */
+} gs_crop_box;             /* 76 bytes */
+GS_API int gs_crop(gs_context *ctx, const gs_crop_box *boxes, uint32_t n_boxes, uint32_t *out_counts_or_null);
+
+/*
  * Append n already-packed splats: the two data-texture records the reference uploads
  * (centerAndScaleData float4, covAndColorData uint4, index.js:40-46,378-394) and the worker's
  * matrices[15] (max(scale)*alpha/255, index.js:397).  Host pointers.
