@@ -15,6 +15,7 @@ GS_RENDER_STATS, GS_RENDER_DEPTH_DEVICE, GS_RENDER_COLOR_DEVICE = 16, 32, 64
 GS_RENDER_BLEND_UNORM8 = 128
 GS_RENDER_SCENE_INTERLEAVE = 256
 GS_RENDER_SORT_F32 = 512
+GS_RENDER_SORT_RADIAL = 2048
 GS_MAX_OBJECTS = 64
 GS_MAX_VIEWS = 4
 GS_MAX_CAMERAS = 6

@@ -261,22 +261,25 @@ class GaussianSplattingComponent:
 
     def render(self, width: int, height: int, camera=None, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
                out: Optional[np.ndarray] = None, synchronous: bool = True, color_in: Optional[np.ndarray] = None,
-               sort_f32: bool = False) -> np.ndarray:
+               sort_f32: bool = False, sort_radial: bool = False) -> np.ndarray:
         """Draw the mesh into an RGBA frame (row 0 = bottom).  synchronous=True sorts with this frame's camera
         (the oracle's definition); synchronous=False draws with the order of the last tick(), which is what the
         reference does while a sort is in flight (index.js:206,439-440).
         color_in: the colour buffer the mesh is blended into ((H, W, 4) of the output dtype, row 0 = bottom), i.e. the
         rest of the scene drawn before it (index.js:177-181); None = the clear colour bg.  Such a frame, and any frame
         of an entity that shares a SplatScene, sorts with this frame's camera.
-        sort_f32 (GS_RENDER_SORT_F32): order by the f32 depth itself, not the reference's 16-bit buckets; such a frame
-        always sorts with its own camera."""
+        sort_f32 (GS_RENDER_SORT_F32): order by the f32 depth itself, not the reference's 16-bit buckets; sort_radial
+        (GS_RENDER_SORT_RADIAL): order by each splat's distance from the camera.  Such a frame always sorts with its own
+        camera."""
         fr = self.frame_inputs(width, height, camera)
         if color_in is None and self.scene is None:
-            reuse = (not synchronous) and self._have_order and not sort_f32
-            return self.renderer.render(fr, bg=bg, fmt=fmt, out=out, reuse_sort=reuse, sort_f32=sort_f32)
+            reuse = (not synchronous) and self._have_order and not (sort_f32 or sort_radial)
+            return self.renderer.render(fr, bg=bg, fmt=fmt, out=out, reuse_sort=reuse, sort_f32=sort_f32,
+                                        sort_radial=sort_radial)
         first, count = self.scene.range_of(self) if self.scene is not None else (0, self.renderer.num_splats)
         obj = SceneObject(first, count, fr.modelview, fr.cutout)
-        return self.renderer.render_scene(fr, [obj], bg=bg, fmt=fmt, color_in=color_in, out=out, sort_f32=sort_f32)
+        return self.renderer.render_scene(fr, [obj], bg=bg, fmt=fmt, color_in=color_in, out=out, sort_f32=sort_f32,
+                                          sort_radial=sort_radial)
 
     # ---- index.js:600-745 ----
     def processPlyBuffer(self, inputBuffer: bytes) -> bytes:
@@ -340,15 +343,21 @@ class SplatScene:
     sort_f32=True (GS_RENDER_SORT_F32) orders every frame by each splat's f32 depth instead of the reference's 16-bit
     buckets, in either mode, so one distant entity or backdrop no longer coarsens the order of the rest.  It applies to
     the same calls and to render_cameras.
+
+    sort_radial=True (GS_RENDER_SORT_RADIAL) orders every frame by each splat's distance from the sorting camera instead,
+    in either mode, so turning the camera (a head in a headset) without moving it does not reorder the splats.  It
+    applies to the calls sort_f32 applies to.
     """
 
     def __init__(self, renderer: Optional[SplatContext] = None, device: int = 0, sh_degree: int = 0,
-                 interleave: bool = False, sort_f32: bool = False):
+                 interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False):
         """sh_degree 1..3: .ply entities keep their spherical harmonics and draw their view-dependent colour (each view
         from its own camera); 0 draws the reference's flat colour.  A given renderer takes the degree while it is empty.
-        interleave: one depth order over every entity; sort_f32: the precise order (see the class)."""
+        interleave: one depth order over every entity; sort_f32: the precise order; sort_radial: the radial order (see
+        the class)."""
         self.interleave = bool(interleave)
         self.sort_f32 = bool(sort_f32)
+        self.sort_radial = bool(sort_radial)
         self.renderer = renderer or SplatContext(device, sh_degree=sh_degree)
         if renderer is not None and sh_degree:
             renderer.set_sh_degree(sh_degree)
@@ -453,7 +462,8 @@ class SplatScene:
             raise ValueError("SplatScene.render: no entity added")
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out,
-                                          blend_unorm8=blend_unorm8, interleave=self.interleave, sort_f32=self.sort_f32)
+                                          blend_unorm8=blend_unorm8, interleave=self.interleave, sort_f32=self.sort_f32,
+                                          sort_radial=self.sort_radial)
 
     def render_cameras(self, cameras, sizes, color_in=None, depth_in=None, bg=(0.0, 0.0, 0.0, 0.0),
                        fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
@@ -470,7 +480,8 @@ class SplatScene:
         return self.renderer.render_scene_cameras([fr[0] for fr in cam_frames], objs,
                                                   [[f.modelview for f in fr] for fr in cam_frames], color_in=color_in,
                                                   depth_in=depth_in, bg=bg, fmt=fmt, blend_unorm8=blend_unorm8,
-                                                  interleave=self.interleave, sort_f32=self.sort_f32)
+                                                  interleave=self.interleave, sort_f32=self.sort_f32,
+                                                  sort_radial=self.sort_radial)
 
     def render_cube(self, position, size: int, near: float = 0.1, far: float = 1000.0, bg=(0.0, 0.0, 0.0, 0.0),
                     fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
@@ -505,7 +516,8 @@ class SplatScene:
             raise ValueError("SplatScene.pick: no entity added")
         frame, objs = self.objects(width, height, camera)
         xy = np.ascontiguousarray(points, dtype=np.uint32).reshape(-1, 2)
-        splat, obj, depth, alpha = self.renderer.pick_scene(frame, objs, xy, depth_in=depth_in, interleave=self.interleave, sort_f32=self.sort_f32)
+        splat, obj, depth, alpha = self.renderer.pick_scene(frame, objs, xy, depth_in=depth_in, interleave=self.interleave, sort_f32=self.sort_f32,
+                                                            sort_radial=self.sort_radial)
         out = []
         for (x, y), s, k, d, a in zip(xy, splat, obj, depth, alpha):
             if k < 0:
@@ -555,7 +567,8 @@ class SplatScene:
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene_target(frame, objs, color, depth, viewport=(x, y), fmt=fmt,
                                                  blend_unorm8=blend_unorm8, write_depth=write_depth,
-                                                 interleave=self.interleave, sort_f32=self.sort_f32)
+                                                 interleave=self.interleave, sort_f32=self.sort_f32,
+                                                 sort_radial=self.sort_radial)
 
     def _xr_ratio(self) -> float:
         """The first entity's xrPixelRatio, 1 when it is not positive (the rule of render_xr)."""
@@ -608,7 +621,8 @@ class SplatScene:
         xy = [c for x, y, _, _ in rects for c in (x, y)]
         return self.renderer.render_scene_views_target(views, objs, view_mvs, color, xy, depth, fmt=fmt,
                                                        blend_unorm8=blend_unorm8, write_depth=write_depth,
-                                                       interleave=self.interleave, sort_f32=self.sort_f32)
+                                                       interleave=self.interleave, sort_f32=self.sort_f32,
+                                                       sort_radial=self.sort_radial)
 
     def render_xr_layer(self, eye_cameras, width: int, height: int, color: np.ndarray, depth: Optional[np.ndarray] = None,
                         fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False, write_depth: bool = False) -> np.ndarray:
@@ -626,7 +640,8 @@ class SplatScene:
             raise ValueError(f"render_xr_layer: the layer must hold two {w} x {h} eyes side by side")
         return self.renderer.render_scene_stereo_target(eyes, objs, eye_mvs, color, depth, eye_xy=(0, 0, w, 0), fmt=fmt,
                                                         blend_unorm8=blend_unorm8, write_depth=write_depth,
-                                                        interleave=self.interleave, sort_f32=self.sort_f32)
+                                                        interleave=self.interleave, sort_f32=self.sort_f32,
+                                                        sort_radial=self.sort_radial)
 
     def render_xr(self, eye_cameras, width: int, height: int, color_in=(None, None), depth_in=(None, None),
                   bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
@@ -642,4 +657,5 @@ class SplatScene:
             raise ValueError("SplatScene.render_xr: no entity added")
         _, objs, eyes, eye_mvs = self._xr_objects(eye_cameras, width, height)
         return self.renderer.render_scene_stereo(eyes, objs, eye_mvs, color_in=color_in, depth_in=depth_in, bg=bg, fmt=fmt,
-                                                 blend_unorm8=blend_unorm8, interleave=self.interleave, sort_f32=self.sort_f32)
+                                                 blend_unorm8=blend_unorm8, interleave=self.interleave, sort_f32=self.sort_f32,
+                                                 sort_radial=self.sort_radial)

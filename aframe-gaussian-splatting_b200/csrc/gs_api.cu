@@ -1004,9 +1004,9 @@ static void stats_from_counters(gs_context *c, const FrameCounters &h, uint32_t 
 
 // gs_sort and gs_sort_scene*: one sort in slot 0 and buffer set 0 of an idle pipeline, its counters and order read back.
 // scene: the validated table of gs_sort_scene* (nullptr: the one-entity sort of gs_sort, by view and cutout); f32: the
-// precise order of GS_RENDER_SORT_F32 (scene sorts only)
+// precise order of GS_RENDER_SORT_F32, radial: that of GS_RENDER_SORT_RADIAL (scene sorts only; radial implies f32)
 static int sort_only(gs_context *c, const float *view, const float *cutout, const SceneTable *scene, size_t scene_bytes,
-                     uint32_t *out_idx, uint32_t *out_count, bool f32 = false) {
+                     uint32_t *out_idx, uint32_t *out_count, bool f32 = false, bool radial = false) {
   int rc = idle(c);
   if (rc) return rc;
   if ((rc = ensure_scratch(c))) return rc;
@@ -1025,7 +1025,7 @@ static int sort_only(gs_context *c, const float *view, const float *cutout, cons
   if (scene) GS_CUDA(c, cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, c->stream));
   GS_CUDA(c, cudaEventRecord(c->ev[0], c->stream));
   if (scene) {
-    launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, c->stream);
+    launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, radial, c->stream);
     if (f32) {
       launch_sort_f32(c, sl.fp, sl.ctr, sl.scene_dev, scene->interleave != 0, bufs, c->stream);
     } else {
@@ -1033,7 +1033,7 @@ static int sort_only(gs_context *c, const float *view, const float *cutout, cons
       launch_scene_radix(c, sl.fp, sl.ctr, bufs, c->stream);
     }
   } else {
-    launch_depth_cull(c, sl.fp, sl.ctr, c->stream);
+    launch_depth_cull(c, sl.fp, sl.ctr, false, c->stream);
     launch_depth_radix(c, sl.fp, sl.ctr, bufs, c->stream);
   }
   GS_CUDA(c, cudaGetLastError());
@@ -1109,7 +1109,7 @@ static gs_context::GraphKey graph_key(const gs_context *c, const gs_context::Slo
   k.p3 = c->scene_key;
   k.psh = c->sh;
   k.sh_degree = c->sh_degree;
-  k.sort_mode = (interleaved(sl) ? 1u : 0u) | (sl.f32 ? 2u : 0u);
+  k.sort_mode = (interleaved(sl) ? 1u : 0u) | (sl.f32 ? 2u : 0u) | (sl.radial ? 4u : 0u);
   k.pz = c->zdepth[0];
   if (sl.stereo) {
     k.n_views = sl.n_views;
@@ -1138,11 +1138,11 @@ static cudaError_t enqueue_sort_stage(gs_context *c, gs_context::Slot &sl, bool 
   if (sl.scene && (e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, m))) return e;
   if ((e = record(sl.ev[0], m, external_events))) return e;
   if (sl.scene) {
-    launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, m);
+    launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, sl.radial, m);
   } else if (reuse) {
     if ((e = cudaMemcpyAsync(sl.ctr, c->sort_hdr, sizeof(SortHeader), cudaMemcpyDeviceToDevice, m))) return e;
   } else {
-    launch_depth_cull(c, sl.fp, sl.ctr, m);
+    launch_depth_cull(c, sl.fp, sl.ctr, sl.radial, m);
   }
   // fork: the vertex-shader kernel only needs the cull result, so it runs beside the depth radix passes
   if ((e = cudaEventRecord(c->ev_fork[0], m))) return e;
@@ -1342,8 +1342,8 @@ static cudaError_t enqueue_slab_keys_stage(gs_context *c, gs_context::Slot &sl, 
   if ((e = cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), st))) return e;
   if (scene && (e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, st))) return e;
   if ((e = record(sl.ev[0], st, external_events))) return e;
-  if (scene) launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, st);
-  else launch_depth_cull(c, sl.fp, sl.ctr, st);
+  if (scene) launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, sl.radial, st);
+  else launch_depth_cull(c, sl.fp, sl.ctr, sl.radial, st);
   launch_keys(c, sl.fp, sl.ctr, scene, interleaved(sl), sl.f32, sl.octr, sl.set, st);
   launch_slab_plan(c, sl.fp, sl.ctr, sl.set, c->slab_first, sl.n_slabs, st);
   launch_compact_offsets(c, sl.fp, scene, interleaved(sl), sl.set, sl.n_slabs, st);  // one pass over the keys for every slab's compaction offsets
@@ -1918,15 +1918,16 @@ static int check_blend8(gs_context *c, const gs_render_params *p) {
   return GS_OK;
 }
 
-// GS_RENDER_SORT_F32 sorts every frame it is set on: no GS_RENDER_REUSE_SORT, and (out of its scope) no tiled or peer
-// output and no sharded context
+// GS_RENDER_SORT_F32 and GS_RENDER_SORT_RADIAL sort every frame they are set on: no GS_RENDER_REUSE_SORT, and (out of
+// their scope) no tiled or peer output and no sharded context
 static int check_sort_f32(gs_context *c, const gs_render_params *p) {
-  if (!(p->flags & GS_RENDER_SORT_F32)) return GS_OK;
+  if (!(p->flags & (GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL))) return GS_OK;
+  const std::string flag = (p->flags & GS_RENDER_SORT_RADIAL) ? "GS_RENDER_SORT_RADIAL" : "GS_RENDER_SORT_F32";
   if (p->flags & GS_RENDER_REUSE_SORT)
-    return fail(c, GS_ERR_INVALID, "GS_RENDER_SORT_F32 sorts the frame: GS_RENDER_REUSE_SORT is not accepted");
+    return fail(c, GS_ERR_INVALID, (flag + " sorts the frame: GS_RENDER_REUSE_SORT is not accepted").c_str());
   if (p->flags & (GS_RENDER_OUT_TILED | GS_RENDER_OUT_PEER))
-    return fail(c, GS_ERR_INVALID, "GS_RENDER_SORT_F32: GS_RENDER_OUT_TILED and _OUT_PEER are not accepted");
-  if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "GS_RENDER_SORT_F32: not on a sharded context");
+    return fail(c, GS_ERR_INVALID, (flag + ": GS_RENDER_OUT_TILED and _OUT_PEER are not accepted").c_str());
+  if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, (flag + ": not on a sharded context").c_str());
   return GS_OK;
 }
 
@@ -1948,7 +1949,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   // view's tiles
   FrameNeeds need{};
   need.scene = scene != nullptr;
-  need.f32 = (p->flags & GS_RENDER_SORT_F32) != 0;
+  need.f32 = (p->flags & (GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL)) != 0;  // a radial frame takes the precise passes
   need.n_views = stereo ? stereo->n : 1u;
   need.depth_write = target && (target->t->flags & GS_TARGET_DEPTH_WRITE);
   for (uint32_t v = 0; v < need.n_views; ++v) {
@@ -2001,6 +2002,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   sl.slab = slab;
   sl.pick = false;
   sl.f32 = need.f32;
+  sl.radial = (p->flags & GS_RENDER_SORT_RADIAL) != 0;
   sl.cameras = group != ~0ull;
   sl.group = group;
   sl.group_n = group_n;
@@ -2138,9 +2140,10 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   if (!c || !frame || !xy || !out) return GS_ERR_INVALID;
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_pick_scene before any push");
   if (n_points == 0 || n_points > GS_MAX_PICKS) return fail(c, GS_ERR_INVALID, "gs_pick_scene: between 1 and GS_MAX_PICKS points");
-  if (frame->flags & ~(uint32_t)(GS_RENDER_DEPTH_DEVICE | GS_RENDER_SCENE_INTERLEAVE | GS_RENDER_SORT_F32))
+  if (frame->flags & ~(uint32_t)(GS_RENDER_DEPTH_DEVICE | GS_RENDER_SCENE_INTERLEAVE | GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL))
     return fail(c, GS_ERR_INVALID,
-                "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE, GS_RENDER_SCENE_INTERLEAVE and GS_RENDER_SORT_F32 is accepted");
+                "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32 and "
+                "GS_RENDER_SORT_RADIAL is accepted");
   if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "gs_pick_scene: not on a sharded context");
   if (frame->width == 0 || frame->height == 0 || frame->width > 4096 || frame->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
@@ -2171,7 +2174,7 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   }
   FrameNeeds need{};
   need.scene = !plain;
-  need.f32 = (frame->flags & GS_RENDER_SORT_F32) != 0;
+  need.f32 = (frame->flags & (GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL)) != 0;
   need.n_views = 1;
   {
     RenderConsts grid;
@@ -2201,6 +2204,7 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   sl.slab = false;
   sl.pick = true;
   sl.f32 = need.f32;
+  sl.radial = (frame->flags & GS_RENDER_SORT_RADIAL) != 0;
   sl.cameras = false;
   sl.group = ~0ull;
   sl.color_in[0] = nullptr;
@@ -2247,14 +2251,17 @@ extern "C" int gs_sort_scene_interleaved(gs_context *c, const gs_object *objs, u
 extern "C" int gs_sort_scene_flags(gs_context *c, const gs_object *objs, uint32_t n_objs, uint32_t flags, uint32_t *out_idx,
                                    uint32_t *out_count) {
   if (!c) return GS_ERR_INVALID;
-  if (flags & ~(uint32_t)(GS_RENDER_SCENE_INTERLEAVE | GS_RENDER_SORT_F32))
-    return fail(c, GS_ERR_INVALID, "gs_sort_scene_flags: no flag other than GS_RENDER_SCENE_INTERLEAVE and GS_RENDER_SORT_F32 is accepted");
+  if (flags & ~(uint32_t)(GS_RENDER_SCENE_INTERLEAVE | GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL))
+    return fail(c, GS_ERR_INVALID,
+                "gs_sort_scene_flags: no flag other than GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32 and GS_RENDER_SORT_RADIAL "
+                "is accepted");
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_sort_scene_flags before any push");
   GS_CUDA(c, cudaSetDevice(c->device));
   size_t bytes = 0;
   int rc = build_scene_table(c, objs, n_objs, (flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes);
   if (rc) return rc;
-  return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count, (flags & GS_RENDER_SORT_F32) != 0);
+  const bool radial = (flags & GS_RENDER_SORT_RADIAL) != 0;
+  return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count, radial || (flags & GS_RENDER_SORT_F32), radial);
 }
 
 extern "C" int gs_wait(gs_context *c, uint64_t ticket, gs_stats *stats) {
@@ -2285,8 +2292,10 @@ extern "C" int gs_render_stereo(gs_context *c, const float view[4], const float 
   for (int e = 0; e < 2; ++e) {  // refused before the sort, so that a refusal changes nothing
     if (eyes[e].flags & GS_RENDER_SCENE_INTERLEAVE)
       return fail(c, GS_ERR_INVALID, "GS_RENDER_SCENE_INTERLEAVE is a scene frame flag: gs_render_stereo has no entities");
-    if (eyes[e].flags & GS_RENDER_SORT_F32)
-      return fail(c, GS_ERR_INVALID, "GS_RENDER_SORT_F32: gs_render_stereo draws the stored order of gs_sort (use gs_render_scene_stereo)");
+    if (eyes[e].flags & (GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL))
+      return fail(c, GS_ERR_INVALID,
+                  "GS_RENDER_SORT_F32 and GS_RENDER_SORT_RADIAL: gs_render_stereo draws the stored order of gs_sort (use "
+                  "gs_render_scene_stereo)");
     if ((rc = check_blend8(c, &eyes[e]))) return rc;
   }
   rc = gs_sort(c, view, cutout16_or_null, nullptr, nullptr);

@@ -463,6 +463,7 @@ struct gs_context {
     bool slab = false;                       // rendered by the front-to-back slab path
     bool pick = false;                       // a pick (gs_pick_scene): bin and pick stages instead of binning and raster
     bool f32 = false;                        // GS_RENDER_SORT_F32: sorted by the f32 depth (gs_sort.cu Z passes)
+    bool radial = false;                     // GS_RENDER_SORT_RADIAL: f32 too, its depth pass writing -r (k_depth_cull<true>)
     // one camera's pass of a cameras frame (gs_render_scene_cameras): stages launched without graphs.  group: the ticket of
     // the frame's first camera (its cameras hold tickets group .. group + group_n - 1), ~0 for every other frame
     bool cameras = false;
@@ -534,7 +535,7 @@ struct gs_context {
     uint32_t n_views = 0, view_size[gs::kMaxViews] = {}, pad2 = 0; const void *px = nullptr;
     const void *psh = nullptr; uint32_t sh_degree = 0;  // the projection's instantiation and SH table
     uint32_t sort_mode = 0;  // bit 0: scene keys and slab passes of GS_RENDER_SCENE_INTERLEAVE frames; bit 1: the passes of
-                             // GS_RENDER_SORT_F32 frames
+                             // GS_RENDER_SORT_F32 frames; bit 2: the depth pass of GS_RENDER_SORT_RADIAL frames
     const void *pz = nullptr;  // zdepth[0] (GS_RENDER_SORT_F32 slab loops bake it)
   } gkey[gs::kGraphDomains];                     // [GraphDomain] (kept apart: a views frame or a pick re-captures only its own graphs)
 
@@ -578,11 +579,13 @@ struct FrameBufs {
 };
 
 // -- launchers (each .cu file owns its kernels); every per-frame input comes from device memory (fp, ctr) --
-void launch_depth_cull(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st);
+// radial (GS_RENDER_SORT_RADIAL): the depth pass writes f32(-r) and records the range of -r (fp->rc.mv, scene: each
+// entity's mv, holds the sorting modelview)
+void launch_depth_cull(gs_context *c, const FrameParams *fp, FrameCounters *ctr, bool radial, cudaStream_t st);
 void launch_depth_radix(gs_context *c, const FrameParams *fp, FrameCounters *ctr, const FrameBufs &b, cudaStream_t st);  // 6 launches -> b.order
 // scene frames: per-entity depth pass, per-entity keys, (rank, key, index) sort -> b.order, per-entity projection
 void launch_depth_cull_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, ObjCounters *octr, FrameCounters *ctr,
-                             cudaStream_t st);
+                             bool radial, cudaStream_t st);
 // interleave (GS_RENDER_SCENE_INTERLEAVE): one key space over every entity, in the same launches
 void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *scene, const ObjCounters *octr, FrameCounters *ctr,
                        bool interleave, cudaStream_t st);

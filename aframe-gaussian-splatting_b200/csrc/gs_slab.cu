@@ -46,6 +46,8 @@
 // compaction keeps index order and the per-slab passes are the same stable LSD passes as the one-pass sort, so each run
 // comes out in exactly its one-pass order.  The raster then composites the same sequence front to back, and the saturation
 // argument above holds unchanged.
+// Radial frames (GS_RENDER_SORT_RADIAL) are precise frames whose depth pass stored dr = f32(-r) and the ranges of -r: the
+// same instantiations plan and sort them, and (1) and (2) hold with dr for d.
 //
 // Views scene frames (gs_render_scene_views, gs_render_scene_stereo) cut their slabs from the HEAD camera's scene order,
 // which is every view's draw order: stage A, the plan and the compaction offsets are those of the scene frame, shared by

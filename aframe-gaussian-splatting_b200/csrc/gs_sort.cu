@@ -26,6 +26,9 @@
 // Precise frames (GS_RENDER_SORT_F32): k_radix_*<Z<0..24, ...>> sort by the 31-bit f32 depth key ~bits(d) in four passes,
 // and scene frames add k_radix_*<Z<kRankDigit, ...>> over the draw rank (last: (rank, d, index); first when interleaved:
 // (d, rank, index)).  k_scene_keys is not run: no key16, no Q5.  The slab path runs the same passes over each slab.
+// Radial frames (GS_RENDER_SORT_RADIAL): k_depth_cull<true> / k_depth_cull_scene<true> write f32(-r), r the fp64 distance
+// of the centre from the sorting camera, in place of the depth, and record the range of -r; the precise passes then sort
+// by it unchanged.
 //
 // PLY ingest (gs_push_ply): k_radix_*<P<0>> .. <P<24>> sort the rows by a 32-bit importance key, four stable 8-bit passes
 // (the stable Array.prototype.sort of index.js:668).  Each pass reads the digit through the permutation (key[perm[i]]), so
@@ -55,11 +58,37 @@ __device__ __forceinline__ bool worker_keep(const SortConsts &sc, const float4 c
   return (depth < 0.0) && ((double)s > __dmul_rn(-0.0001, depth)) && in_box;
 }
 
+// Radial frames (GS_RENDER_SORT_RADIAL): rows 0 and 1 of the sorting modelview (column-major, widened to fp64).  Row 2 is
+// the worker's view row, so the kept splat's depth zc is already the third camera-space coordinate.
+struct RadialRows {
+  double x[4], y[4];
+};
+__device__ __forceinline__ RadialRows radial_rows(const float *__restrict__ mv) {
+  RadialRows m;
+  for (int i = 0; i < 4; ++i) {
+    m.x[i] = (double)mv[4 * i];
+    m.y[i] = (double)mv[4 * i + 1];
+  }
+  return m;
+}
+// -r of a kept centre: r = sqrt((xc xc + yc yc) + zc zc) in fp64, every operation rounded, summed left to right as the
+// depth is.  zc < 0, so r > 0; the centre is finite (an infinite coordinate fails the filter), so r is finite.
+__device__ __forceinline__ double radial_depth(const RadialRows &m, const float4 c, const double zc) {
+  const double x = c.x, y = c.y, z = c.z;
+  const double xc = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(m.x[0], x), __dmul_rn(m.x[1], y)), __dmul_rn(m.x[2], z)), m.x[3]);
+  const double yc = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(m.y[0], x), __dmul_rn(m.y[1], y)), __dmul_rn(m.y[2], z)), m.y[3]);
+  return -__dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(xc, xc), __dmul_rn(yc, yc)), __dmul_rn(zc, zc)));
+}
+
+// RADIAL: the key and the range are those of -r (radial_depth) instead of the depth; filter and sentinel unchanged
+template <bool RADIAL>
 __global__ void __launch_bounds__(256) k_depth_cull(const float4 *__restrict__ cs, const float *__restrict__ sa,
                                                     const FrameParams *__restrict__ fp,
                                                     float *__restrict__ depth_out, FrameCounters *ctr) {
   GS_PDL_ENTRY();
   const SortConsts sc = fp->sc;
+  RadialRows rows;
+  if constexpr (RADIAL) rows = radial_rows(fp->rc.mv);
   const uint32_t n = fp->n_splats;  // resident splats when the frame was submitted (a push may be appending more)
   double dmin = INFINITY, dmax = -INFINITY;
   uint32_t cnt = 0;
@@ -69,6 +98,7 @@ __global__ void __launch_bounds__(256) k_depth_cull(const float4 *__restrict__ c
     const bool keep = worker_keep(sc, c, s, depth);
     float out = GS_DEPTH_REJECT;
     if (keep) {
+      if constexpr (RADIAL) depth = radial_depth(rows, c, depth);
       out = (float)depth;  // Float32Array store (index.js:549)
       ++cnt;
       if (depth > dmax) dmax = depth;
@@ -122,8 +152,10 @@ __global__ void __launch_bounds__(256) k_depth_cull(const float4 *__restrict__ c
 
 // ---------------------------------------------------------------------------------------------
 // Scene frames, K1: k_depth_cull with each splat's own entity; min/max/validCount per entity (and over the frame, for the
-// statistics).  Splats outside every entity's range are not sorted.
+// statistics).  Splats outside every entity's range are not sorted.  RADIAL: -r from each entity's own modelview, as
+// k_depth_cull<true>.
 // ---------------------------------------------------------------------------------------------
+template <bool RADIAL>
 __global__ void __launch_bounds__(256) k_depth_cull_scene(const float4 *__restrict__ cs, const float *__restrict__ sa,
                                                           const FrameParams *__restrict__ fp, const SceneTable *__restrict__ scene,
                                                           float *__restrict__ depth_out, FrameCounters *ctr, ObjCounters *octr) {
@@ -165,6 +197,7 @@ __global__ void __launch_bounds__(256) k_depth_cull_scene(const float4 *__restri
         flush();
         cur = k;
       }
+      if constexpr (RADIAL) depth = radial_depth(radial_rows(scene->obj[k].mv), c, depth);
       out = (float)depth;  // Float32Array store (index.js:549)
       ++cnt;
       if (depth > dmax) dmax = depth;
@@ -252,17 +285,19 @@ static int persistent_grid(gs_context *c, uint64_t n_elems, int per_cta, int cta
   return (int)(tiles < cap ? tiles : cap);
 }
 
-void launch_depth_cull(gs_context *c, const FrameParams *fp, FrameCounters *ctr, cudaStream_t st) {
+void launch_depth_cull(gs_context *c, const FrameParams *fp, FrameCounters *ctr, bool radial, cudaStream_t st) {
   // grids are sized by the table CAPACITY (stable across pushes) and the kernels read the splat count from fp, so a
   // captured frame graph stays valid while a scene is still loading
   const int grid = persistent_grid(c, c->cap, 256 * 4, 8);
-  launch_chain(c, k_depth_cull, grid, 256, st, c->center_scale, c->size_alpha, fp, c->depth, ctr);
+  launch_chain(c, radial ? k_depth_cull<true> : k_depth_cull<false>, grid, 256, st, c->center_scale, c->size_alpha, fp,
+               c->depth, ctr);
 }
 
 void launch_depth_cull_scene(gs_context *c, const FrameParams *fp, const SceneTable *scene, ObjCounters *octr, FrameCounters *ctr,
-                             cudaStream_t st) {
+                             bool radial, cudaStream_t st) {
   const int grid = persistent_grid(c, c->cap, 256 * 4, 8);
-  launch_chain(c, k_depth_cull_scene, grid, 256, st, c->center_scale, c->size_alpha, fp, scene, c->depth, ctr, octr);
+  launch_chain(c, radial ? k_depth_cull_scene<true> : k_depth_cull_scene<false>, grid, 256, st, c->center_scale,
+               c->size_alpha, fp, scene, c->depth, ctr, octr);
 }
 
 void launch_scene_keys(gs_context *c, const FrameParams *fp, const SceneTable *scene, const ObjCounters *octr, FrameCounters *ctr,

@@ -74,9 +74,13 @@ enum {
   GS_RENDER_SCENE_INTERLEAVE = 1u << 8, /* scene frames and picks: one back-to-front order over every entity's splats,
                                           so overlapping entities blend by depth (see "Interleaved scenes" below);
                                           gs_render, gs_render_async and gs_render_stereo refuse it        */
-  GS_RENDER_SORT_F32 = 1u << 9 /* order the frame by the full f32 depth instead of the reference's 16-bit buckets
+  GS_RENDER_SORT_F32 = 1u << 9, /* order the frame by the full f32 depth instead of the reference's 16-bit buckets
                                   (see "Precise order" below); gs_render_stereo, GS_RENDER_REUSE_SORT, _OUT_TILED,
                                   _OUT_PEER and sharded contexts refuse it                             */
+  /* bit 10 stays unassigned: gs_sort_scene_flags and gs_pick_scene refuse it as an unknown flag */
+  GS_RENDER_SORT_RADIAL = 1u << 11 /* order the frame by each splat's distance from the camera, which turning the
+                                      camera does not change (see "Radial order" below); refused where
+                                      GS_RENDER_SORT_F32 is                                              */
 };
 
 /*
@@ -456,6 +460,28 @@ GS_API int gs_render_stereo(gs_context *ctx, const float view[4], const float *c
  * bucket - (rank, key16) with each entity's range, or key16 over the union range when interleaved - never decreases, and
  * each bucket's run, put back in (draw rank, table index) order, is the default order's.  So a scene whose kept splats
  * each have a key16 of their own (per entity, or over the union) and no Q5 drop gives the default frame byte for byte.
+ *
+ * Radial order (GS_RENDER_SORT_RADIAL in gs_render_params.flags; opt-in, default and precise frames are unchanged): the
+ * frame is ordered by each splat's distance from the sorting camera instead of its camera-space z.  Turning the camera
+ * without moving it changes every z, and two overlapping splats whose difference is nearly perpendicular to the view axis
+ * swap ("popping"); their distances do not change.
+ *   - filter: unchanged, each entity's own worker test in fp64 (the kept set is that of default and precise frames);
+ *   - camera-space centre in fp64: mv is the modelview the frame sorts with (the frame's for a plain frame, objs[k].modelview
+ *     for scene frames, the head's for stereo and views frames, cam_modelviews[c][k] for camera c of a cameras frame), its
+ *     f32 entries widened, every operation rounded and nothing contracted: xc = ((mv[0] x + mv[4] y) + mv[8] z) + mv[12],
+ *     yc = ((mv[1] x + mv[5] y) + mv[9] z) + mv[13], zc = the worker's depth (row 2 is the view row);
+ *   - key: r = sqrt((xc xc + yc yc) + zc zc), correctly rounded, and dr = (float) -r.  Every kept zc is < 0, so r > 0, and
+ *     a kept centre is finite (an infinite coordinate makes the depth infinite or NaN, which the filter rejects), so r is
+ *     finite; dr may still round to -inf;
+ *   - order: the precise order's, with dr in place of d, ascending (farthest first): plain frames (dr, table index);
+ *     default scene frames (draw rank, dr, table index); interleaved scene frames (dr, draw rank, table index);
+ *   - counters: no range, no ToInt32 and no quirk Q5, so n_dropped is 0.  min_depth / max_depth report the fp64 range of
+ *     -r, not of the depth;
+ *   - GS_RENDER_SORT_F32 set as well is accepted and gives the same frame;
+ *   - scope and refusals: those of GS_RENDER_SORT_F32 above;
+ *   - consequences: the order depends on the camera's position, not on its rotation, up to the rounding of the rotated f32
+ *     matrix.  A stereo or views frame's head order no longer changes while the head only turns.  A splat can be nearer
+ *     than another by z and farther by distance, so where the two overlap the radial frame blends them the other way.
  */
 #define GS_MAX_OBJECTS 64
 typedef struct gs_object {
@@ -498,9 +524,10 @@ GS_API int gs_sort_scene(gs_context *ctx, const gs_object *objs, uint32_t n_objs
 GS_API int gs_sort_scene_interleaved(gs_context *ctx, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx,
                                      uint32_t *out_count);
 /*
- * Draw order of a scene frame of these entities with `flags`: GS_RENDER_SCENE_INTERLEAVE and / or GS_RENDER_SORT_F32 (any
- * other bit: GS_ERR_INVALID).  flags 0 is gs_sort_scene, GS_RENDER_SCENE_INTERLEAVE alone gs_sort_scene_interleaved, and
- * with GS_RENDER_SORT_F32 the precise order above.  A plain frame's order is that of one whole-table entity with the
+ * Draw order of a scene frame of these entities with `flags`: any combination of GS_RENDER_SCENE_INTERLEAVE,
+ * GS_RENDER_SORT_F32 and GS_RENDER_SORT_RADIAL (any other bit: GS_ERR_INVALID).  flags 0 is gs_sort_scene,
+ * GS_RENDER_SCENE_INTERLEAVE alone gs_sort_scene_interleaved, with GS_RENDER_SORT_F32 the precise order above and with
+ * GS_RENDER_SORT_RADIAL (F32 or not) the radial order.  A plain frame's order is that of one whole-table entity with the
  * frame's modelview.  Arguments and refusals as gs_sort_scene.
  */
 GS_API int gs_sort_scene_flags(gs_context *ctx, const gs_object *objs, uint32_t n_objs, uint32_t flags, uint32_t *out_idx,
@@ -685,8 +712,8 @@ GS_API int gs_render_scene_views_target(gs_context *ctx, const gs_render_params 
  * entity where entities overlap.
  *
  * gs_pick_scene: n_points (x, y) pairs in xy (host), results in out (host, n_points entries), in the order of xy.
- *   - From frame it reads projection, width, height, focal, depth_in, GS_RENDER_DEPTH_DEVICE and
- *     GS_RENDER_SCENE_INTERLEAVE; objs as gs_render_scene.
+ *   - From frame it reads projection, width, height, focal, depth_in, GS_RENDER_DEPTH_DEVICE, GS_RENDER_SCENE_INTERLEAVE,
+ *     GS_RENDER_SORT_F32 and GS_RENDER_SORT_RADIAL; objs as gs_render_scene.
  *   - Synchronous: it runs in the four pipeline slots like a scene frame, waits only for the frame whose slot it takes (as
  *     a fifth gs_render_scene_async would) and returns when out is filled.  It is always one-pass, whatever GS_SLAB_MIN
  *     says (the slab path draws the same bytes), and leaves no order for GS_RENDER_REUSE_SORT.  Frames submitted before or
@@ -695,7 +722,7 @@ GS_API int gs_render_scene_views_target(gs_context *ctx, const gs_render_params 
  *     whole frame are counted, so a pick needs the instance buffers of the one-pass frame (82 B per candidate), also on
  *     a context whose frames take the slab path, and returns GS_ERR_CAPACITY where that frame would.
  *   - GS_ERR_INVALID, changing nothing, for: n_points 0 or above GS_MAX_PICKS, a point outside the frame, any flag other than
- *     GS_RENDER_DEPTH_DEVICE and GS_RENDER_SCENE_INTERLEAVE, a sharded context (gs_set_shard world > 1), and whatever gs_render_scene refuses.  An empty
+ *     those four, a sharded context (gs_set_shard world > 1), and whatever gs_render_scene refuses.  An empty
  *     table returns GS_ERR_EMPTY.
  */
 typedef struct gs_pick {
