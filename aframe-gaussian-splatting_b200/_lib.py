@@ -22,6 +22,7 @@ GS_MAX_CAMERAS = 6
 GS_TARGET_DEVICE = 1
 GS_TARGET_DEPTH_WRITE = 2
 GS_CROP_KEEP_INSIDE, GS_CROP_KEEP_OUTSIDE = 0, 1
+GS_EXPORT_SPLAT, GS_EXPORT_PLY, GS_EXPORT_PLY_COMPRESSED = 0, 1, 2
 
 
 class GsStats(C.Structure):
@@ -105,6 +106,8 @@ SYMBOLS = {
     "gs_read_packed": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P]),
     "gs_set_sh_degree": (C.c_int, [_P, C.c_uint32]),
     "gs_read_sh": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
+    "gs_set_keep_rows": (C.c_int, [_P, C.c_uint32]),
+    "gs_export": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_uint32, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "gs_sort": (C.c_int, [_P, C.POINTER(C.c_float), C.POINTER(C.c_float), _P, C.POINTER(C.c_uint32)]),
     "gs_render": (C.c_int, [_P, C.POINTER(GsRenderParams), _P, C.POINTER(GsStats)]),
     "gs_render_async": (C.c_int, [_P, C.POINTER(GsRenderParams), _P, C.POINTER(C.c_uint64)]),

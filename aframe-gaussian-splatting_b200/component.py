@@ -350,17 +350,20 @@ class SplatScene:
     """
 
     def __init__(self, renderer: Optional[SplatContext] = None, device: int = 0, sh_degree: int = 0,
-                 interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False):
+                 interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, keep_rows: bool = False):
         """sh_degree 1..3: .ply entities keep their spherical harmonics and draw their view-dependent colour (each view
         from its own camera); 0 draws the reference's flat colour.  A given renderer takes the degree while it is empty.
         interleave: one depth order over every entity; sort_f32: the precise order; sort_radial: the radial order (see
-        the class)."""
+        the class).  keep_rows: keep every splat's .splat row so that save() can write an entity out (a given renderer
+        takes it while it is empty)."""
         self.interleave = bool(interleave)
         self.sort_f32 = bool(sort_f32)
         self.sort_radial = bool(sort_radial)
         self.renderer = renderer or SplatContext(device, sh_degree=sh_degree)
         if renderer is not None and sh_degree:
             renderer.set_sh_degree(sh_degree)
+        if keep_rows and not self.renderer.keep_rows:
+            self.renderer.set_keep_rows(True)
         self.entities: list = []   # components, in draw order
         self._order: list = []     # components, in table order (an empty range's place is its position here)
         self._range: dict = {}     # id(component) -> [first, count]
@@ -445,6 +448,16 @@ class SplatScene:
         self._range[id(component)][1] = kept
         self._shift_after(component, kept - count)
         return kept
+
+    def save(self, component: GaussianSplattingComponent, path=None, format: str = "splat") -> bytes:
+        """Write the entity's splats out as one file (gs_export of its range): format "splat", "ply" or
+        "compressed_ply".  Returns the bytes, and also writes them to `path` when given.  Needs keep_rows=True."""
+        first, count = self._range[id(component)]
+        blob = self.renderer.export(first, count, format)
+        if path is not None:
+            with open(path, "wb") as f:
+                f.write(blob)
+        return blob
 
     def objects(self, width: int, height: int, camera=None):
         """(shared FrameInputs of the draw, [SceneObject per entity in draw order]) for a width x height viewport."""

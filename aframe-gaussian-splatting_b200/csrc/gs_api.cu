@@ -63,27 +63,31 @@ static int ensure_table(gs_context *c, uint64_t need, bool exact = false) {
   float4 *cs = nullptr;
   uint4 *cc = nullptr;
   float *sa = nullptr;
-  uint4 *sh = nullptr;
+  uint4 *sh = nullptr, *keep = nullptr;
   GS_CUDA(c, dev_alloc(&cs, ncap));
   GS_CUDA(c, dev_alloc(&cc, ncap));
   GS_CUDA(c, dev_alloc(&sa, ncap));
   if (c->sh_vecs) GS_CUDA(c, dev_alloc(&sh, ncap * c->sh_vecs));  // SH contexts: the coefficients grow with the table
+  if (c->keep_rows) GS_CUDA(c, dev_alloc(&keep, ncap * 2));        // keep-rows contexts: so do the .splat rows
   if (c->n) {
     GS_CUDA(c, cudaMemcpyAsync(cs, c->center_scale, sizeof(float4) * c->n, cudaMemcpyDeviceToDevice, c->push_stream));
     GS_CUDA(c, cudaMemcpyAsync(cc, c->cov_color, sizeof(uint4) * c->n, cudaMemcpyDeviceToDevice, c->push_stream));
     GS_CUDA(c, cudaMemcpyAsync(sa, c->size_alpha, sizeof(float) * c->n, cudaMemcpyDeviceToDevice, c->push_stream));
     if (sh)
       GS_CUDA(c, cudaMemcpyAsync(sh, c->sh, sizeof(uint4) * c->sh_vecs * c->n, cudaMemcpyDeviceToDevice, c->push_stream));
+    if (keep) GS_CUDA(c, cudaMemcpyAsync(keep, c->keep, sizeof(uint4) * 2 * c->n, cudaMemcpyDeviceToDevice, c->push_stream));
   }
   GS_CUDA(c, cudaStreamSynchronize(c->push_stream));
   dev_free(c->center_scale);
   dev_free(c->cov_color);
   dev_free(c->size_alpha);
   dev_free(c->sh);
+  dev_free(c->keep);
   c->center_scale = cs;
   c->cov_color = cc;
   c->size_alpha = sa;
   c->sh = sh;
+  c->keep = keep;
   c->cap = (uint32_t)ncap;
   return GS_OK;
 }
@@ -440,7 +444,7 @@ extern "C" int gs_destroy(gs_context *c) {
   if (c->stream) cudaStreamSynchronize(c->stream);
   if (c->bstream) cudaStreamSynchronize(c->bstream);
   if (c->rstream) cudaStreamSynchronize(c->rstream);
-  dev_free(c->center_scale); dev_free(c->cov_color); dev_free(c->size_alpha); dev_free(c->sh);
+  dev_free(c->center_scale); dev_free(c->cov_color); dev_free(c->size_alpha); dev_free(c->sh); dev_free(c->keep);
   dev_free(c->depth); dev_free(c->idx_a); dev_free(c->dig_a);
   for (int i = 0; i < 2; ++i) { dev_free(c->order[i]); dev_free(c->proj_rec[i]); dev_free(c->rect[i]); }
   for (int i = 0; i < 2; ++i) { dev_free(c->proj_recx[i]); dev_free(c->rectx[i]); }
@@ -563,6 +567,22 @@ extern "C" int gs_read_sh(gs_context *c, uint32_t first, uint32_t n, uint16_t *o
   return GS_OK;
 }
 
+extern "C" int gs_set_keep_rows(gs_context *c, uint32_t on) {
+  if (!c) return GS_ERR_INVALID;
+  if (c->n) return fail(c, GS_ERR_INVALID, "gs_set_keep_rows: the table is not empty");
+  if ((on != 0) == c->keep_rows) return GS_OK;
+  GS_CUDA(c, cudaSetDevice(c->device));
+  int rc0 = drain(c);
+  if (rc0) return rc0;
+  GS_CUDA(c, cudaStreamSynchronize(c->push_stream));
+  uint4 *keep = nullptr;
+  if (on) GS_CUDA(c, dev_alloc(&keep, (size_t)c->cap * 2));
+  dev_free(c->keep);
+  c->keep = keep;
+  c->keep_rows = on != 0;
+  return GS_OK;
+}
+
 // SH contexts: rows [first, first + n) of the SH table become zeros (rows without coefficients: .splat and packed pushes)
 static int zero_sh(gs_context *c, uint32_t first, uint32_t n) {
   if (c->sh)
@@ -601,7 +621,7 @@ static int begin_move(gs_context *c, uint32_t from, uint32_t to, uint32_t len, v
   *tmp = nullptr;
   int rc = drain(c);
   if (rc) return rc;
-  const size_t bytes = move_tmp_bytes(from, to, len, c->sh ? c->sh_vecs : 0u);
+  const size_t bytes = move_tmp_bytes(from, to, len, c->sh ? c->sh_vecs : 0u, c->keep_rows);
   const cudaError_t e = bytes ? cudaMallocAsync(tmp, bytes, c->push_stream) : cudaSuccess;
   if (e) cudaGetLastError();  // an allocation failure is not sticky: do not leave it for the next launch check
   GS_CUDA(c, e);
@@ -636,6 +656,9 @@ static int insert_rows(gs_context *c, uint32_t at, const void *rows32, uint32_t 
     GS_CUDA(c, cudaEventSynchronize(c->push_ev[b]));  // this staging pair's previous chunk has been packed
     memcpy(c->push_pinned[b], src + (size_t)off * 32, (size_t)m * 32);
     GS_CUDA(c, cudaMemcpyAsync(c->push_dev[b], c->push_pinned[b], (size_t)m * 32, cudaMemcpyHostToDevice, c->push_stream));
+    if (c->keep_rows)
+      GS_CUDA(c, cudaMemcpyAsync(c->keep + 2 * ((size_t)at + off), c->push_dev[b], (size_t)m * 32, cudaMemcpyDeviceToDevice,
+                                 c->push_stream));
     launch_pack(c, c->push_dev[b], at + off, m, c->push_stream);
     GS_CUDA(c, cudaGetLastError());
     GS_CUDA(c, cudaEventRecord(c->push_ev[b], c->push_stream));
@@ -743,7 +766,7 @@ extern "C" int gs_crop(gs_context *c, const gs_crop_box *boxes, uint32_t n_boxes
     for (uint32_t j = 0; j < t.n && !e; ++j) removed += (t.r[j].end - t.r[j].first) - kept[j];
     if (!e && removed) {
       const uint32_t moved = n - r0 - removed;  // the kept rows behind the first removed one
-      if (moved && (e = cudaMallocAsync(&tmp, crop_tmp_bytes(moved, c->sh ? c->sh_vecs : 0u), st))) {
+      if (moved && (e = cudaMallocAsync(&tmp, crop_tmp_bytes(moved, c->sh ? c->sh_vecs : 0u, c->keep_rows), st))) {
         cudaGetLastError();
         tmp = nullptr;
       }
@@ -826,7 +849,9 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   if (!e && sort) e = cudaMallocAsync((void **)&perm_b, (size_t)n * 4, st);
   if (!e && sort) e = cudaMallocAsync((void **)&table, (size_t)256 * (chunks + 1) * 4, st);
   if (!e && sort) e = cudaMallocAsync((void **)&totals, (size_t)256 * 4, st);
-  if (!e && rows32_out_or_null) e = cudaMallocAsync((void **)&out_dev, (size_t)n * 32, st);
+  // a keep-rows context keeps the ordered rows in its table (rows_dst); rows32_out then copies them from there
+  if (!e && rows32_out_or_null && !c->keep_rows) e = cudaMallocAsync((void **)&out_dev, (size_t)n * 32, st);
+  uint8_t *rows_dst = c->keep_rows ? (uint8_t *)(c->keep + 2 * (size_t)at) : out_dev;
   if (!e && sh) e = cudaMallocAsync((void **)&sh_dev, (size_t)n * sizeof(uint4) * S.vecs, st);
   if (e) {
     release();
@@ -859,10 +884,10 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   }
   if (!e) {
     launch_move_rows(c, at, at + n, tail, move_tmp, st);  // opens the gap for the rows (nothing to move for an append)
-    launch_pack_perm(c, rows_dev, perm, at, n, out_dev, sh_dev, st);
+    launch_pack_perm(c, rows_dev, perm, at, n, rows_dst, sh_dev, st);
     e = cudaGetLastError();
   }
-  if (!e && rows32_out_or_null) e = cudaMemcpyAsync(rows32_out_or_null, out_dev, (size_t)n * 32, cudaMemcpyDeviceToHost, st);
+  if (!e && rows32_out_or_null) e = cudaMemcpyAsync(rows32_out_or_null, rows_dst, (size_t)n * 32, cudaMemcpyDeviceToHost, st);
   release();
   if (!e && rows32_out_or_null) e = cudaStreamSynchronize(st);
   GS_CUDA(c, e);
@@ -890,6 +915,7 @@ extern "C" int gs_insert_ply(gs_context *c, uint32_t at, const void *ply, size_t
 extern "C" int gs_push_packed(gs_context *c, const float *center_scale4, const uint32_t *cov_color4,
                               const float *size_alpha, uint32_t n) {
   if (!c || ((!center_scale4 || !cov_color4 || !size_alpha) && n)) return GS_ERR_INVALID;
+  if (c->keep_rows) return fail(c, GS_ERR_INVALID, "gs_push_packed: a keep-rows context needs each splat's .splat row");
   if (!n) return GS_OK;
   GS_CUDA(c, cudaSetDevice(c->device));
   int rc;
@@ -914,6 +940,82 @@ extern "C" int gs_read_packed(gs_context *c, uint32_t first, uint32_t n, float *
   if (center_scale4) GS_CUDA(c, cudaMemcpy(center_scale4, c->center_scale + first, sizeof(float4) * (size_t)n, cudaMemcpyDeviceToHost));
   if (cov_color4) GS_CUDA(c, cudaMemcpy(cov_color4, c->cov_color + first, sizeof(uint4) * (size_t)n, cudaMemcpyDeviceToHost));
   if (size_alpha) GS_CUDA(c, cudaMemcpy(size_alpha, c->size_alpha + first, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+  return GS_OK;
+}
+
+// gs_export: the header text is composed here, the body on the device in the file's layout (gs_export.cu), in one
+// stream-ordered temporary behind the queued pushes and edits on push_stream; frames in flight only read the table, so
+// they are not waited for.  The body crosses in one copy; the header is written only once the body is in place.
+static std::string export_header(uint32_t format, uint32_t n, uint32_t k) {
+  std::string h = "ply\nformat binary_little_endian 1.0\n";
+  if (format == GS_EXPORT_PLY) {
+    h += "element vertex " + std::to_string(n) + "\n";
+    for (const char *p : {"x", "y", "z", "f_dc_0", "f_dc_1", "f_dc_2"}) h += std::string("property float ") + p + "\n";
+    for (uint32_t i = 0; i < 3 * k; ++i) h += "property float f_rest_" + std::to_string(i) + "\n";
+    for (const char *p : {"opacity", "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3"})
+      h += std::string("property float ") + p + "\n";
+  } else {
+    static const char *const kBounds[18] = {"min_x", "min_y", "min_z", "max_x", "max_y", "max_z", "min_scale_x",
+                                            "min_scale_y", "min_scale_z", "max_scale_x", "max_scale_y", "max_scale_z",
+                                            "min_r", "min_g", "min_b", "max_r", "max_g", "max_b"};
+    h += "element chunk " + std::to_string(((uint64_t)n + 255) / 256) + "\n";
+    for (const char *p : kBounds) h += std::string("property float ") + p + "\n";
+    h += "element vertex " + std::to_string(n) + "\n";
+    for (const char *p : {"packed_position", "packed_rotation", "packed_scale", "packed_color"})
+      h += std::string("property uint ") + p + "\n";
+    if (k) {
+      h += "element sh " + std::to_string(n) + "\n";
+      for (uint32_t i = 0; i < 3 * k; ++i) h += "property uchar f_rest_" + std::to_string(i) + "\n";
+    }
+  }
+  return h + "end_header\n";
+}
+
+static size_t export_body_bytes(uint32_t format, uint32_t n, uint32_t k) {
+  if (format == GS_EXPORT_SPLAT) return (size_t)n * 32;
+  if (format == GS_EXPORT_PLY) return (size_t)n * 4 * (14 + 3 * (size_t)k);
+  return ((size_t)n + 255) / 256 * 72 + (size_t)n * (16 + 3 * (size_t)k);
+}
+
+extern "C" int gs_export(gs_context *c, uint32_t first, uint32_t count, uint32_t format, void *out, size_t cap,
+                         size_t *out_bytes) {
+  if (!c) return GS_ERR_INVALID;
+  if (!out_bytes) return fail(c, GS_ERR_INVALID, "gs_export: out_bytes is NULL");
+  *out_bytes = 0;
+  if (format != GS_EXPORT_SPLAT && format != GS_EXPORT_PLY && format != GS_EXPORT_PLY_COMPRESSED)
+    return fail(c, GS_ERR_INVALID, "gs_export: unknown format");
+  const uint32_t k = sh_coeffs(c->sh_degree);
+  const std::string head = format == GS_EXPORT_SPLAT ? std::string() : export_header(format, count, k);
+  const size_t body = export_body_bytes(format, count, k), total = head.size() + body;
+  *out_bytes = total;
+  if (!c->keep_rows) return fail(c, GS_ERR_INVALID, "gs_export: the context keeps no .splat rows (gs_set_keep_rows)");
+  if ((uint64_t)first + count > c->n) return fail(c, GS_ERR_INVALID, "gs_export: range past the resident splats");
+  if (!out) return GS_OK;
+  if (cap < total) return fail(c, GS_ERR_INVALID, "gs_export: cap is below the file size");
+  GS_CUDA(c, cudaSetDevice(c->device));
+  cudaStream_t st = c->push_stream;
+  uint8_t *dst = (uint8_t *)out + head.size();
+  if (count && format == GS_EXPORT_SPLAT) {  // the kept rows are the file's body as they are
+    GS_CUDA(c, cudaMemcpyAsync(dst, c->keep + 2 * (size_t)first, body, cudaMemcpyDeviceToHost, st));
+    GS_CUDA(c, cudaStreamSynchronize(st));
+  } else if (count) {
+    uint8_t *tmp = nullptr;
+    cudaError_t e = cudaMallocAsync((void **)&tmp, body, st);
+    if (e) {
+      cudaGetLastError();  // an allocation failure is not sticky
+      GS_CUDA(c, e);
+    }
+    if (format == GS_EXPORT_PLY)
+      launch_export_ply(c, first, count, tmp, st);
+    else
+      launch_export_compressed(c, first, count, tmp, st);
+    e = cudaGetLastError();
+    if (!e) e = cudaMemcpyAsync(dst, tmp, body, cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(tmp, st);
+    if (!e) e = cudaStreamSynchronize(st);
+    GS_CUDA(c, e);
+  }
+  memcpy(out, head.data(), head.size());
   return GS_OK;
 }
 

@@ -221,6 +221,7 @@ struct PlyLayout {
 // ---- spherical harmonics (gs_set_sh_degree): per splat 3 K fp16 coefficients, K = (d + 1)^2 - 1, channel-major (R's K,
 // then G's, then B's: INRIA's f_rest order), padded to whole 16 B words ----
 constexpr int kMaxShCoeffs = 15;  // K of degree 3
+constexpr double kShC0 = 0.28209479177387814;  // index.js:728: f_dc -> colour (gs_ply.cu, gs_export.cu)
 __host__ __device__ constexpr uint32_t sh_coeffs(uint32_t degree) { return (degree + 1) * (degree + 1) - 1; }
 __host__ __device__ constexpr uint32_t sh_vecs(uint32_t degree) { return (3 * sh_coeffs(degree) * 2 + 15) / 16; }  // 0, 2, 3, 6
 // f_rest_* fields of a PLY file (SH contexts): file_k = K of the file's degree (the largest d <= 3 whose 3 K f_rest_* all
@@ -329,6 +330,9 @@ struct gs_context {
   // spherical-harmonic coefficients (gs_set_sh_degree; none at degree 0): sh_vecs 16 B words per splat, row i = splat i
   uint32_t sh_degree = 0, sh_vecs = 0;
   uint4 *sh = nullptr;
+  // each splat's source .splat row (gs_set_keep_rows; none by default): 2 16 B words per splat, row i = splat i
+  bool keep_rows = false;
+  uint4 *keep = nullptr;
 
   // ---- per-splat scratch (sized to cap) ----
   uint32_t scratch_cap = 0;
@@ -605,8 +609,8 @@ void launch_pack(gs_context *c, const uint8_t *rows_dev, uint32_t first, uint32_
 void launch_pack_perm(gs_context *c, const uint8_t *rows_dev, const uint32_t *perm, uint32_t first, uint32_t n,
                       uint8_t *rows_out, const uint4 *sh_rows, cudaStream_t st);
 // table edits: bytes of the temporary a move of rows [from, from+len) to [to, to+len) needs (0: the ranges are disjoint);
-// sh_vecs: the SH words per row that move with them
-size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len, uint32_t sh_vecs);
+// sh_vecs: the SH words per row that move with them; rows: whether the kept .splat rows move too (gs_set_keep_rows)
+size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len, uint32_t sh_vecs, bool rows);
 // k_move_rows: one launch for disjoint ranges, else two through tmp
 void launch_move_rows(gs_context *c, uint32_t from, uint32_t to, uint32_t len, void *tmp, cudaStream_t st);
 // one row span of the table arrays (or of a temporary laid out like them): centres, cov/colour, size_alpha, SH rows
@@ -614,9 +618,14 @@ struct RowSpan {
   float4 *cs;
   uint4 *cc;
   float *sa;
-  uint4 *sh;  // NULL on a degree-0 context
+  uint4 *sh;    // NULL on a degree-0 context
+  uint4 *rows;  // the kept .splat rows, 2 words each; NULL without gs_set_keep_rows
 };
 RowSpan table_span(gs_context *c, uint32_t row);
+// a temporary laid out like the table for len rows: cs | cc | sh | kept rows | 3 floats of slack + sa, its sa starting
+// at row offset sa_mod4 (mod 4) so that copies to or from a table span of that alignment move size_alpha as float4
+size_t span_tmp_bytes(uint32_t len, uint32_t sh_vecs, bool rows);
+RowSpan tmp_span(void *tmp, uint32_t len, uint32_t sh_vecs, bool rows, uint32_t sa_mod4);
 // k_move_rows over n rows of two disjoint spans (size_alpha as float4 when both share their alignment mod 16 B)
 void launch_copy_rows(const RowSpan &src, const RowSpan &dst, uint32_t n, uint32_t sh_vecs, cudaStream_t st);
 // gs_crop (gs_crop.cu): the ranges of one crop, sorted by first, and the per-call device scratch of its passes
@@ -640,10 +649,15 @@ uint32_t crop_chunks(uint32_t rows);  // chunks of the compaction over `rows` ro
 // pass 1 and 2 over rows [lo, n): per-chunk and per-range kept counts, the first removed row, the chunk offsets
 void launch_crop_count(gs_context *c, const CropScratch &s, uint32_t lo, uint32_t n, cudaStream_t st);
 // bytes of the temporary that holds `kept` rows written behind row r0 (crop_write)
-size_t crop_tmp_bytes(uint32_t kept, uint32_t sh_vecs);
+size_t crop_tmp_bytes(uint32_t kept, uint32_t sh_vecs, bool rows);
 // pass 3: the kept rows of [r0, n) (r0 = the first removed row) into tmp, in order, then back into the table at r0
 void launch_crop_write(gs_context *c, const CropScratch &s, uint32_t lo, uint32_t r0, uint32_t n, uint32_t kept, void *tmp,
                        cudaStream_t st);
+// gs_export (gs_export.cu): rows [first, first + n) of the kept .splat rows (and their SH rows on an SH context, sh_k
+// coefficients per channel) restated as INRIA PLY vertices into body (n (14 + 3 sh_k) floats), or quantised as a
+// compressed PLY body: ceil(n / 256) chunk rows of 18 floats, n 16 B vertex words, n 3 sh_k SH bytes
+void launch_export_ply(gs_context *c, uint32_t first, uint32_t n, uint8_t *body, cudaStream_t st);
+void launch_export_compressed(gs_context *c, uint32_t first, uint32_t n, uint8_t *body, cudaStream_t st);
 // PLY push: decode `rows` whole rows of a staged body chunk into .splat rows + importance keys at [first_row, ...);
 // sh (SH contexts, else NULL): the rows' coefficients into sh_rows (sh->vecs words per row), in file order too
 void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,

@@ -4,7 +4,8 @@
 //                  chunk (warp ballots), kept rows per range and the first removed row
 //   k_crop_scan  : pass 2, one CTA: exclusive scan of the chunk counts
 //   k_crop_write : pass 3 over the chunks from the first removed row on: the kept rows behind it, in order, into a
-//                  temporary (16 B centre, 16 B cov/colour, 4 B size_alpha, 16 B per SH word); k_move_rows (gs_pack.cu)
+//                  temporary (16 B centre, 16 B cov/colour, 4 B size_alpha, 16 B per SH word, 32 B per kept .splat
+//                  row); k_move_rows (gs_pack.cu)
 //                  then copies them back to the table at the first removed row
 // Plain kernels with no inter-CTA waiting (DESIGN §5), the pattern of the slab path's k_compact_count_all /
 // k_compact_write.  The host reads the counts back between passes 2 and 3: they size the temporary, give out_counts and
@@ -180,6 +181,10 @@ __global__ void __launch_bounds__(kCropThreads) k_crop_write(const RowSpan src, 
       __stcs(dst.cc + p, __ldcs(cc_s + row));
       __stcs(dst.sa + p, __ldcs(sa_s + row));
       for (uint32_t v = 0; v < sh_vecs; ++v) __stcs(dst.sh + (size_t)p * sh_vecs + v, __ldcs(sh_s + (size_t)row * sh_vecs + v));
+      if (dst.rows) {
+        __stcs(dst.rows + 2 * (size_t)p, __ldcs(src.rows + 2 * (size_t)row));
+        __stcs(dst.rows + 2 * (size_t)p + 1, __ldcs(src.rows + 2 * (size_t)row + 1));
+      }
     }
   }
 }
@@ -195,17 +200,14 @@ void launch_crop_count(gs_context *c, const CropScratch &s, uint32_t lo, uint32_
   k_crop_scan<<<1, 1024, 0, st>>>(s.chunk_cnt, chunks);
 }
 
-size_t crop_tmp_bytes(uint32_t kept, uint32_t sh_vecs) {
-  return (size_t)kept * (36 + 16 * (size_t)sh_vecs) + 16;  // cs | cc | sh | 3 floats of alignment slack + sa
-}
+size_t crop_tmp_bytes(uint32_t kept, uint32_t sh_vecs, bool rows) { return span_tmp_bytes(kept, sh_vecs, rows); }
 
 void launch_crop_write(gs_context *c, const CropScratch &s, uint32_t lo, uint32_t r0, uint32_t n, uint32_t kept, void *tmp,
                        cudaStream_t st) {
   if (!kept) return;  // everything from r0 on was removed: nothing moves
   const uint32_t w = c->sh ? c->sh_vecs : 0u;
-  uint4 *sh_t = (uint4 *)tmp + 2 * (size_t)kept;
   // the temporary's size_alpha shares the destination's alignment mod 16 B, so the copy back moves it as float4
-  const RowSpan t{(float4 *)tmp, (uint4 *)tmp + kept, (float *)(sh_t + (size_t)w * kept) + (r0 & 3u), w ? sh_t : nullptr};
+  const RowSpan t = tmp_span(tmp, kept, w, c->keep_rows, r0);
   const uint32_t chunks = crop_chunks(n - lo) - (r0 - lo) / kCropChunk;
   k_crop_write<<<crop_grid(c, chunks), kCropThreads, 0, st>>>(table_span(c, 0), t, w, s.tab, lo, r0, n, s.chunk_cnt);
   launch_copy_rows(t, table_span(c, r0), kept, w, st);

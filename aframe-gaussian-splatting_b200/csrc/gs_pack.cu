@@ -4,7 +4,7 @@
 //                 (gs_push_ply: the gather of processPlyBuffer's importance order fused with the pack; on an SH context
 //                 the row's coefficients are gathered with it)
 //   k_move_rows : rows [from, from+len) of the table -> [to, to+len) (gs_insert_* / gs_erase open or close a gap; gs_crop
-//                 copies its compacted rows back with it)
+//                 copies its compacted rows back with it), with their SH rows and kept .splat rows
 //
 // One thread per .splat row, all arithmetic in fp64 exactly as JavaScript evaluates it (Three.js r147
 // Matrix4.compose / transpose / scale / premultiply restated entry by entry, sums left to right, no FMA):
@@ -148,7 +148,8 @@ __global__ void __launch_bounds__(256) k_pack_perm(const uint4 *__restrict__ row
 
 // Table edit (gs_insert_*, gs_erase): copy n rows of the table arrays from src to dst, one row per thread.  The two
 // ranges never overlap within one launch (an overlapping move goes through a temporary, launch_move_rows), so the
-// accesses are restrict.  The 16 B records (and an SH context's sh_vecs words of coefficients) are copied as they are;
+// accesses are restrict.  The 16 B records (and an SH context's sh_vecs words of coefficients, and the two words of a
+// kept .splat row when the spans have them) are copied as they are;
 // size_alpha goes as float4 when source and destination share their alignment mod 16 B (sa_vec), with up to 3 scalar
 // rows before the first aligned float4 (sa_head) and up to 3 after the last.  (RowSpan: gs_common.cuh.)
 
@@ -162,6 +163,10 @@ __global__ void __launch_bounds__(256) k_move_rows(const RowSpan src, const RowS
   __stcs(dst.cs + i, __ldcs(cs_s + i));
   __stcs(dst.cc + i, __ldcs(cc_s + i));
   for (uint32_t v = 0; v < sh_vecs; ++v) __stcs(dst.sh + (size_t)i * sh_vecs + v, __ldcs(src.sh + (size_t)i * sh_vecs + v));
+  if (dst.rows) {
+    __stcs(dst.rows + 2 * (size_t)i, __ldcs(src.rows + 2 * (size_t)i));
+    __stcs(dst.rows + 2 * (size_t)i + 1, __ldcs(src.rows + 2 * (size_t)i + 1));
+  }
   if (!sa_vec) {
     __stcs(dst.sa + i, __ldcs(sa_s + i));
     return;
@@ -178,7 +183,17 @@ __global__ void __launch_bounds__(256) k_move_rows(const RowSpan src, const RowS
 
 RowSpan table_span(gs_context *c, uint32_t row) {
   return RowSpan{c->center_scale + row, c->cov_color + row, c->size_alpha + row,
-                 c->sh ? c->sh + (size_t)row * c->sh_vecs : nullptr};
+                 c->sh ? c->sh + (size_t)row * c->sh_vecs : nullptr, c->keep ? c->keep + 2 * (size_t)row : nullptr};
+}
+
+size_t span_tmp_bytes(uint32_t len, uint32_t sh_vecs, bool rows) {
+  return (size_t)len * (36 + 16 * (size_t)(sh_vecs + (rows ? 2u : 0u))) + 16;
+}
+
+RowSpan tmp_span(void *tmp, uint32_t len, uint32_t sh_vecs, bool rows, uint32_t sa_mod4) {
+  uint4 *sh_t = (uint4 *)tmp + 2 * (size_t)len, *rows_t = sh_t + (size_t)sh_vecs * len;
+  float *sa_t = (float *)(rows_t + (rows ? 2 * (size_t)len : 0)) + (sa_mod4 & 3u);
+  return RowSpan{(float4 *)tmp, (uint4 *)tmp + len, sa_t, sh_vecs ? sh_t : nullptr, rows ? rows_t : nullptr};
 }
 
 void launch_copy_rows(const RowSpan &src, const RowSpan &dst, uint32_t n, uint32_t sh_vecs, cudaStream_t st) {
@@ -187,24 +202,22 @@ void launch_copy_rows(const RowSpan &src, const RowSpan &dst, uint32_t n, uint32
   k_move_rows<<<(n + 255) / 256, 256, 0, st>>>(src, dst, n, head, vec, sh_vecs);
 }
 
-size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len, uint32_t sh_vecs) {
+size_t move_tmp_bytes(uint32_t from, uint32_t to, uint32_t len, uint32_t sh_vecs, bool rows) {
   const uint32_t shift = from > to ? from - to : to - from;
-  // cs | cc | sh | 3 floats of alignment slack + sa
-  return shift >= len ? 0 : (size_t)len * (36 + 16 * (size_t)sh_vecs) + 16;
+  return shift >= len ? 0 : span_tmp_bytes(len, sh_vecs, rows);
 }
 
 // Rows [from, from + len) of the table move to [to, to + len).  Disjoint ranges: one launch.  Overlapping ones: two,
-// through `tmp` (move_tmp_bytes(from, to, len, c->sh_vecs) bytes, 16 B aligned), whose size_alpha starts at the source's
+// through `tmp` (move_tmp_bytes(from, to, len, c->sh_vecs, c->keep_rows) bytes, 16 B aligned), whose size_alpha starts at the source's
 // alignment so that the first copy is always vectorised.
 void launch_move_rows(gs_context *c, uint32_t from, uint32_t to, uint32_t len, void *tmp, cudaStream_t st) {
   if (!len || from == to) return;
   const uint32_t w = c->sh ? c->sh_vecs : 0u;
-  if (!move_tmp_bytes(from, to, len, w)) {
+  if (!move_tmp_bytes(from, to, len, w, c->keep_rows)) {
     launch_copy_rows(table_span(c, from), table_span(c, to), len, w, st);
     return;
   }
-  uint4 *sh_t = (uint4 *)tmp + 2 * (size_t)len;
-  const RowSpan t{(float4 *)tmp, (uint4 *)tmp + len, (float *)(sh_t + (size_t)w * len) + (from & 3u), w ? sh_t : nullptr};
+  const RowSpan t = tmp_span(tmp, len, w, c->keep_rows, from);
   launch_copy_rows(table_span(c, from), t, len, w, st);
   launch_copy_rows(t, table_span(c, to), len, w, st);
 }

@@ -374,7 +374,6 @@ __device__ __forceinline__ double ply_get(const uint8_t *row, const PlyField f) 
   }
 }
 
-constexpr double kShC0 = 0.28209479177387814;  // index.js:728
 
 // Float32Array store (round to nearest even; NaN as the host's quiet NaN)
 __device__ __forceinline__ uint32_t f32_bits(double v) {

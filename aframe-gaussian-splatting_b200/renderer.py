@@ -63,13 +63,17 @@ def make_objects(objects: Sequence[SceneObject]):
     return arr
 
 
+_EXPORT_FORMATS = {"splat": _lib.GS_EXPORT_SPLAT, "ply": _lib.GS_EXPORT_PLY, "compressed_ply": _lib.GS_EXPORT_PLY_COMPRESSED}
+
+
 class SplatContext:
     """Owner of one gs_context.  Mirrors the worker protocol (clear / push / sort, index.js:572-598) and
     the draw (index.js:184-207)."""
 
-    def __init__(self, device: int = 0, sh_degree: int = 0):
+    def __init__(self, device: int = 0, sh_degree: int = 0, keep_rows: bool = False):
         """sh_degree 1..3: keep the spherical-harmonic coefficients of .ply files and draw every splat in its
-        view-dependent colour (gs_set_sh_degree); 0 draws the reference's flat colour."""
+        view-dependent colour (gs_set_sh_degree); 0 draws the reference's flat colour.  keep_rows: keep each splat's
+        .splat row so that export() can save the table (gs_set_keep_rows)."""
         self._lib = _lib.load()
         h = C.c_void_p()
         rc = self._lib.gs_create(int(device), C.byref(h))
@@ -80,6 +84,9 @@ class SplatContext:
         self.sh_degree = 0
         if sh_degree:
             self.set_sh_degree(sh_degree)
+        self.keep_rows = False
+        if keep_rows:
+            self.set_keep_rows(True)
 
     # -- lifetime --
     def close(self) -> None:
@@ -192,6 +199,24 @@ class SplatContext:
         """gs_set_sh_degree: 0 (flat colour) .. 3; only while the table is empty (after creation or clear())."""
         self._check(self._lib.gs_set_sh_degree(self._h, int(degree)))
         self.sh_degree = int(degree)
+
+    def set_keep_rows(self, on: bool) -> None:
+        """gs_set_keep_rows: keep each splat's 32-byte .splat row beside the table (32 B per splat), which export()
+        needs; only while the table is empty.  push_packed is refused while it is on."""
+        self._check(self._lib.gs_set_keep_rows(self._h, int(bool(on))))
+        self.keep_rows = bool(on)
+
+    def export(self, first: int = 0, count: Optional[int] = None, format="splat") -> bytes:
+        """gs_export: rows [first, first+count) (count None: to the end) as one file: format "splat" (32-byte rows, as
+        pushed), "ply" (INRIA float PLY with the context's f_rest_*) or "compressed_ply" (SuperSplat's chunked layout),
+        or the GS_EXPORT_* value.  Needs keep_rows."""
+        fmt = _EXPORT_FORMATS.get(format, format)
+        count = self.num_splats - first if count is None else count
+        size = C.c_size_t()
+        self._check(self._lib.gs_export(self._h, int(first), int(count), int(fmt), None, 0, C.byref(size)))
+        out = np.empty(size.value, np.uint8)
+        self._check(self._lib.gs_export(self._h, int(first), int(count), int(fmt), _ptr(out), out.size, C.byref(size)))
+        return out.tobytes()
 
     def read_sh(self, first: int = 0, n: Optional[int] = None) -> np.ndarray:
         """gs_read_sh: the SH coefficients of splats [first, first+n) as (n, 3, K) float16, K = (degree+1)^2 - 1, in table

@@ -328,6 +328,62 @@ GS_API int gs_set_sh_degree(gs_context *ctx, uint32_t degree);
 GS_API int gs_read_sh(gs_context *ctx, uint32_t first, uint32_t n, uint16_t *out);
 
 /*
+ * Saving an edited scene: export a range of the table as a .splat, INRIA PLY or compressed PLY file.
+ *
+ * gs_set_keep_rows(ctx, 1): keep each splat's 32-byte .splat row beside the table (0, the default, keeps none and
+ *   allocates nothing).  Accepted only while the table is empty, as gs_set_sh_degree; a non-empty table returns
+ *   GS_ERR_INVALID and changes nothing.  The whole row is kept, 32 B per splat, not only the scale and rotation the packed
+ *   record cannot give back: the pack converts the centre through fp64 and negates z, which does not keep a NaN's sign
+ *   and payload, and the .splat export is the pushed rows byte for byte.
+ *     - gs_push_splats / gs_insert_splats keep the rows given; gs_push_ply / gs_insert_ply (float and compressed) keep the
+ *       rows they convert, those rows32_out returns.  gs_push_packed has no rows and returns GS_ERR_INVALID.
+ *     - The rows grow with the table (gs_reserve) and move with their splats in every edit (gs_insert_*, gs_erase,
+ *       gs_crop), as the SH rows do; the temporaries of those edits hold 32 B more per moved splat.
+ *     - Frames never read them: every frame of a keep-rows context equals the frame of a context without it.
+ *
+ * gs_export: rows [first, first+count) (one entity's range) as one complete file in host memory `out`.
+ *   - out == NULL only sets *out_bytes to the file's exact size.  GS_ERR_INVALID, nothing written: out_bytes NULL, an
+ *     unknown format, a context without keep-rows, a range past N, cap below the size (*out_bytes is set to the size
+ *     in the last three cases).  count == 0 gives an empty .splat file or a PLY of its header alone.
+ *   - The export runs behind the pushes and edits already queued and sees their rows.  It does not wait for frames in
+ *     flight (they and the export only read the table) and returns when the bytes are in `out`.  The body is built on
+ *     the device in a stream-ordered temporary (GS_ERR_OOM changes nothing) and crosses in one copy; the header text is
+ *     composed on the host.
+ *   GS_EXPORT_SPLAT: the kept rows, 32 B each: the rows that were pushed (gs_push_splats' input, gs_push_ply's rows32_out),
+ *     in table order, without the erased or cropped ones.
+ *   GS_EXPORT_PLY: binary_little_endian 1.0, `element vertex N` and the float properties x y z f_dc_0..2
+ *     f_rest_0..{3K-1} opacity scale_0..2 rot_0..3, K the context's SH coefficients per channel (none at degree 0).
+ *     Every value is computed in fp64 and rounded once to f32, and every NaN written is 0x7FC00000 except a position's:
+ *       - x y z: the row's f32 bits;  f_dc_k = (b_k / 255 - 0.5) / SH_C0 of colour byte b_k;
+ *       - opacity = -log(255 / a - 1) of alpha byte a (-inf at 0, +inf at 255);
+ *       - rot_0..3 = (byte - 128) / 128 of the rotation bytes (w, x, y, z), not normalised;
+ *       - f_rest_{cK+k-1}: the stored fp16 coefficient k of channel c, widened to f32;
+ *       - scale_k of the row's scale s: among x = f32(log s) and the 4 f32 values either side of it, the one nearest to
+ *         log s (the smaller on a tie) for which gs_push_ply's conversion f32(exp(x)) gives s; f32(log s) when none does.
+ *         s = 0 gives -inf, +inf gives +inf, a negative or NaN s gives NaN.
+ *     Loading the file with gs_push_ply gives back every position, colour byte, alpha byte and SH coefficient, the scales
+ *     of rows that came from a PLY, and for those rows rotation bytes within 1 of their own (the loader normalises the
+ *     quaternion, so other rotation bytes come back as those of the normalised one, and the zero quaternion, all four
+ *     bytes 128, as bytes 0).  The loader re-sorts the rows by importance.
+ *   GS_EXPORT_PLY_COMPRESSED: the layout gs_push_ply reads: `element chunk C` (C = ceil(N / 256)) with the 18 float
+ *     bounds min_x .. max_b, `element vertex N` with uint packed_position packed_rotation packed_scale packed_color, and
+ *     when K > 0 `element sh N` with 3K uchar f_rest_*.  Chunks are 256 rows counted from `first`.  Each value quantises
+ *     the GS_EXPORT_PLY restatement above, in fp64, as SuperSplat's exporter does:
+ *       - bounds: the chunk's min and max of x y z, of scale_0..2, and of the colours SH_C0 f_dc + 0.5, written as f32;
+ *         NaN values are skipped (a bound is NaN only when every value of the chunk is);
+ *       - t = (v - min) / (max - min), 0 when max == min; packUnorm(t, bits) = clamp(floor(t (2^bits - 1) + 0.5)), a NaN
+ *         giving 0; positions and scales take 11, 10, 11 bits, colours 8;  alpha = packUnorm(sigmoid(opacity), 8);
+ *       - rotation: rot_0..3 normalised in fp64 (sqrt(w w + x x + y y + z z)); the largest |component| (the first on
+ *         ties) is made positive and its index (x 0, y 1, z 2, w 3) goes in bits 30-31; the other three, in x y z w order,
+ *         take 10 bits each as packUnorm(q sqrt(2)/2 + 0.5, 10).  The zero quaternion is stored as the identity;
+ *       - sh byte: clamp(trunc((f / 8 + 0.5) 256), 0, 255), NaN giving 0.
+ */
+enum { GS_EXPORT_SPLAT = 0, GS_EXPORT_PLY = 1, GS_EXPORT_PLY_COMPRESSED = 2 };
+GS_API int gs_set_keep_rows(gs_context *ctx, uint32_t on);
+GS_API int gs_export(gs_context *ctx, uint32_t first, uint32_t count, uint32_t format, void *out_or_null, size_t cap,
+                     size_t *out_bytes);
+
+/*
  * {method:"sort", view, cutout} -> {sortedIndexes} (index.js:449-453, 507-570, 587-596).
  * out_idx (host, capacity gs_num_splats) receives the surviving splat indices back-to-front,
  * bit-identical to the reference's Uint32Array (16-bit bucket order, ties by index; tail zeros
