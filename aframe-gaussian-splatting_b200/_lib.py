@@ -16,6 +16,7 @@ GS_RENDER_BLEND_UNORM8 = 128
 GS_RENDER_SCENE_INTERLEAVE = 256
 GS_RENDER_SORT_F32 = 512
 GS_RENDER_SORT_RADIAL = 2048
+GS_RENDER_ANTIALIAS = 4096
 GS_MAX_OBJECTS = 64
 GS_MAX_VIEWS = 4
 GS_MAX_CAMERAS = 6

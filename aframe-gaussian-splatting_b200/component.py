@@ -261,7 +261,7 @@ class GaussianSplattingComponent:
 
     def render(self, width: int, height: int, camera=None, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
                out: Optional[np.ndarray] = None, synchronous: bool = True, color_in: Optional[np.ndarray] = None,
-               sort_f32: bool = False, sort_radial: bool = False) -> np.ndarray:
+               sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False) -> np.ndarray:
         """Draw the mesh into an RGBA frame (row 0 = bottom).  synchronous=True sorts with this frame's camera
         (the oracle's definition); synchronous=False draws with the order of the last tick(), which is what the
         reference does while a sort is in flight (index.js:206,439-440).
@@ -270,16 +270,17 @@ class GaussianSplattingComponent:
         of an entity that shares a SplatScene, sorts with this frame's camera.
         sort_f32 (GS_RENDER_SORT_F32): order by the f32 depth itself, not the reference's 16-bit buckets; sort_radial
         (GS_RENDER_SORT_RADIAL): order by each splat's distance from the camera.  Such a frame always sorts with its own
-        camera."""
+        camera.  antialias (GS_RENDER_ANTIALIAS): scale each splat's alpha back for the shader's 0.3 px^2 blur, as
+        captures trained with anti-aliased rasterisation expect."""
         fr = self.frame_inputs(width, height, camera)
         if color_in is None and self.scene is None:
             reuse = (not synchronous) and self._have_order and not (sort_f32 or sort_radial)
             return self.renderer.render(fr, bg=bg, fmt=fmt, out=out, reuse_sort=reuse, sort_f32=sort_f32,
-                                        sort_radial=sort_radial)
+                                        sort_radial=sort_radial, antialias=antialias)
         first, count = self.scene.range_of(self) if self.scene is not None else (0, self.renderer.num_splats)
         obj = SceneObject(first, count, fr.modelview, fr.cutout)
         return self.renderer.render_scene(fr, [obj], bg=bg, fmt=fmt, color_in=color_in, out=out, sort_f32=sort_f32,
-                                          sort_radial=sort_radial)
+                                          sort_radial=sort_radial, antialias=antialias)
 
     # ---- index.js:600-745 ----
     def processPlyBuffer(self, inputBuffer: bytes) -> bytes:
@@ -347,18 +348,25 @@ class SplatScene:
     sort_radial=True (GS_RENDER_SORT_RADIAL) orders every frame by each splat's distance from the sorting camera instead,
     in either mode, so turning the camera (a head in a headset) without moving it does not reorder the splats.  It
     applies to the calls sort_f32 applies to.
+
+    antialias=True (GS_RENDER_ANTIALIAS) scales each splat's alpha by the share of its footprint's energy that the
+    shader's 0.3 px^2 blur did not add, so sub-pixel splats (far detail, XR eyes at a low pixel ratio, small cube faces)
+    no longer thicken and brighten.  It is what captures trained with anti-aliased rasterisation expect.  It applies to
+    every draw, pick and raycast of the scene.
     """
 
     def __init__(self, renderer: Optional[SplatContext] = None, device: int = 0, sh_degree: int = 0,
-                 interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, keep_rows: bool = False):
+                 interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, keep_rows: bool = False,
+                 antialias: bool = False):
         """sh_degree 1..3: .ply entities keep their spherical harmonics and draw their view-dependent colour (each view
         from its own camera); 0 draws the reference's flat colour.  A given renderer takes the degree while it is empty.
         interleave: one depth order over every entity; sort_f32: the precise order; sort_radial: the radial order (see
         the class).  keep_rows: keep every splat's .splat row so that save() can write an entity out (a given renderer
-        takes it while it is empty)."""
+        takes it while it is empty).  antialias: the anti-aliased alpha (see the class)."""
         self.interleave = bool(interleave)
         self.sort_f32 = bool(sort_f32)
         self.sort_radial = bool(sort_radial)
+        self.antialias = bool(antialias)
         self.renderer = renderer or SplatContext(device, sh_degree=sh_degree)
         if renderer is not None and sh_degree:
             renderer.set_sh_degree(sh_degree)
@@ -476,7 +484,7 @@ class SplatScene:
         frame, objs = self.objects(width, height, camera)
         return self.renderer.render_scene(frame, objs, bg=bg, fmt=fmt, color_in=color_in, depth_in=depth_in, out=out,
                                           blend_unorm8=blend_unorm8, interleave=self.interleave, sort_f32=self.sort_f32,
-                                          sort_radial=self.sort_radial)
+                                          sort_radial=self.sort_radial, antialias=self.antialias)
 
     def render_cameras(self, cameras, sizes, color_in=None, depth_in=None, bg=(0.0, 0.0, 0.0, 0.0),
                        fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
@@ -494,7 +502,7 @@ class SplatScene:
                                                   [[f.modelview for f in fr] for fr in cam_frames], color_in=color_in,
                                                   depth_in=depth_in, bg=bg, fmt=fmt, blend_unorm8=blend_unorm8,
                                                   interleave=self.interleave, sort_f32=self.sort_f32,
-                                                  sort_radial=self.sort_radial)
+                                                  sort_radial=self.sort_radial, antialias=self.antialias)
 
     def render_cube(self, position, size: int, near: float = 0.1, far: float = 1000.0, bg=(0.0, 0.0, 0.0, 0.0),
                     fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
@@ -530,7 +538,7 @@ class SplatScene:
         frame, objs = self.objects(width, height, camera)
         xy = np.ascontiguousarray(points, dtype=np.uint32).reshape(-1, 2)
         splat, obj, depth, alpha = self.renderer.pick_scene(frame, objs, xy, depth_in=depth_in, interleave=self.interleave, sort_f32=self.sort_f32,
-                                                            sort_radial=self.sort_radial)
+                                                            sort_radial=self.sort_radial, antialias=self.antialias)
         out = []
         for (x, y), s, k, d, a in zip(xy, splat, obj, depth, alpha):
             if k < 0:
@@ -581,7 +589,7 @@ class SplatScene:
         return self.renderer.render_scene_target(frame, objs, color, depth, viewport=(x, y), fmt=fmt,
                                                  blend_unorm8=blend_unorm8, write_depth=write_depth,
                                                  interleave=self.interleave, sort_f32=self.sort_f32,
-                                                 sort_radial=self.sort_radial)
+                                                 sort_radial=self.sort_radial, antialias=self.antialias)
 
     def _xr_ratio(self) -> float:
         """The first entity's xrPixelRatio, 1 when it is not positive (the rule of render_xr)."""
@@ -635,7 +643,7 @@ class SplatScene:
         return self.renderer.render_scene_views_target(views, objs, view_mvs, color, xy, depth, fmt=fmt,
                                                        blend_unorm8=blend_unorm8, write_depth=write_depth,
                                                        interleave=self.interleave, sort_f32=self.sort_f32,
-                                                       sort_radial=self.sort_radial)
+                                                       sort_radial=self.sort_radial, antialias=self.antialias)
 
     def render_xr_layer(self, eye_cameras, width: int, height: int, color: np.ndarray, depth: Optional[np.ndarray] = None,
                         fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False, write_depth: bool = False) -> np.ndarray:
@@ -654,7 +662,7 @@ class SplatScene:
         return self.renderer.render_scene_stereo_target(eyes, objs, eye_mvs, color, depth, eye_xy=(0, 0, w, 0), fmt=fmt,
                                                         blend_unorm8=blend_unorm8, write_depth=write_depth,
                                                         interleave=self.interleave, sort_f32=self.sort_f32,
-                                                        sort_radial=self.sort_radial)
+                                                        sort_radial=self.sort_radial, antialias=self.antialias)
 
     def render_xr(self, eye_cameras, width: int, height: int, color_in=(None, None), depth_in=(None, None),
                   bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
@@ -671,4 +679,4 @@ class SplatScene:
         _, objs, eyes, eye_mvs = self._xr_objects(eye_cameras, width, height)
         return self.renderer.render_scene_stereo(eyes, objs, eye_mvs, color_in=color_in, depth_in=depth_in, bg=bg, fmt=fmt,
                                                  blend_unorm8=blend_unorm8, interleave=self.interleave, sort_f32=self.sort_f32,
-                                                 sort_radial=self.sort_radial)
+                                                 sort_radial=self.sort_radial, antialias=self.antialias)

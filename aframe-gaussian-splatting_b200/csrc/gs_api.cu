@@ -1185,6 +1185,7 @@ extern "C" uint32_t gs_owned_tiles(uint32_t width, uint32_t height, uint32_t ran
 static FrameBufs slot_bufs(gs_context *c, const gs_context::Slot &sl) {
   FrameBufs b{c->order[sl.set], c->proj_rec[sl.set], c->rect[sl.set], c->inst_rec[sl.set], c->bin_range[sl.set]};
   b.sh_cam = sl.sh_cam_dev;
+  b.antialias = sl.antialias;
   if (sl.stereo) {
     b.views = true;
     if (sl.n_views > 1) {
@@ -1211,6 +1212,7 @@ static gs_context::GraphKey graph_key(const gs_context *c, const gs_context::Slo
   k.p3 = c->scene_key;
   k.psh = c->sh;
   k.sh_degree = c->sh_degree;
+  k.antialias = sl.antialias ? 1u : 0u;
   k.sort_mode = (interleaved(sl) ? 1u : 0u) | (sl.f32 ? 2u : 0u) | (sl.radial ? 4u : 0u);
   k.pz = c->zdepth[0];
   if (sl.stereo) {
@@ -2105,6 +2107,7 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   sl.pick = false;
   sl.f32 = need.f32;
   sl.radial = (p->flags & GS_RENDER_SORT_RADIAL) != 0;
+  sl.antialias = (p->flags & GS_RENDER_ANTIALIAS) != 0;
   sl.cameras = group != ~0ull;
   sl.group = group;
   sl.group_n = group_n;
@@ -2242,10 +2245,11 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   if (!c || !frame || !xy || !out) return GS_ERR_INVALID;
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_pick_scene before any push");
   if (n_points == 0 || n_points > GS_MAX_PICKS) return fail(c, GS_ERR_INVALID, "gs_pick_scene: between 1 and GS_MAX_PICKS points");
-  if (frame->flags & ~(uint32_t)(GS_RENDER_DEPTH_DEVICE | GS_RENDER_SCENE_INTERLEAVE | GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL))
+  if (frame->flags & ~(uint32_t)(GS_RENDER_DEPTH_DEVICE | GS_RENDER_SCENE_INTERLEAVE | GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL |
+                                 GS_RENDER_ANTIALIAS))
     return fail(c, GS_ERR_INVALID,
-                "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32 and "
-                "GS_RENDER_SORT_RADIAL is accepted");
+                "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32, "
+                "GS_RENDER_SORT_RADIAL and GS_RENDER_ANTIALIAS is accepted");
   if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "gs_pick_scene: not on a sharded context");
   if (frame->width == 0 || frame->height == 0 || frame->width > 4096 || frame->height > 4096)
     return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
@@ -2307,6 +2311,7 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
   sl.pick = true;
   sl.f32 = need.f32;
   sl.radial = (frame->flags & GS_RENDER_SORT_RADIAL) != 0;
+  sl.antialias = (frame->flags & GS_RENDER_ANTIALIAS) != 0;
   sl.cameras = false;
   sl.group = ~0ull;
   sl.color_in[0] = nullptr;

@@ -468,6 +468,7 @@ struct gs_context {
     bool pick = false;                       // a pick (gs_pick_scene): bin and pick stages instead of binning and raster
     bool f32 = false;                        // GS_RENDER_SORT_F32: sorted by the f32 depth (gs_sort.cu Z passes)
     bool radial = false;                     // GS_RENDER_SORT_RADIAL: f32 too, its depth pass writing -r (k_depth_cull<true>)
+    bool antialias = false;                  // GS_RENDER_ANTIALIAS: projected with the anti-aliased alpha (k_project<.., AA>)
     // one camera's pass of a cameras frame (gs_render_scene_cameras): stages launched without graphs.  group: the ticket of
     // the frame's first camera (its cameras hold tickets group .. group + group_n - 1), ~0 for every other frame
     bool cameras = false;
@@ -537,9 +538,10 @@ struct gs_context {
   struct GraphKey {
     uint32_t cap = 0, n_tiles = 0, n_bins = 0, pad = 0; uint64_t cap_inst = 0; const void *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr;
     uint32_t n_views = 0, view_size[gs::kMaxViews] = {}, pad2 = 0; const void *px = nullptr;
-    const void *psh = nullptr; uint32_t sh_degree = 0;  // the projection's instantiation and SH table
-    uint32_t sort_mode = 0;  // bit 0: scene keys and slab passes of GS_RENDER_SCENE_INTERLEAVE frames; bit 1: the passes of
-                             // GS_RENDER_SORT_F32 frames; bit 2: the depth pass of GS_RENDER_SORT_RADIAL frames
+    const void *psh = nullptr; uint32_t sh_degree = 0, antialias = 0;  // the projection's instantiation and SH table
+    uint32_t sort_mode = 0, pad3 = 0;  // sort_mode bit 0: scene keys and slab passes of GS_RENDER_SCENE_INTERLEAVE frames;
+                                       // bit 1: the passes of GS_RENDER_SORT_F32 frames; bit 2: the depth pass of
+                                       // GS_RENDER_SORT_RADIAL frames
     const void *pz = nullptr;  // zdepth[0] (GS_RENDER_SORT_F32 slab loops bake it)
   } gkey[gs::kGraphDomains];                     // [GraphDomain] (kept apart: a views frame or a pick re-captures only its own graphs)
 
@@ -580,6 +582,7 @@ struct FrameBufs {
   uint32_t bin_base[kMaxViews] = {};
   bool views = false;
   const float4 *sh_cam = nullptr;  // SH contexts: the slot's camera table (gs_context::Slot::sh_cam_dev)
+  bool antialias = false;          // GS_RENDER_ANTIALIAS: the projection's records take the anti-aliased alpha
 };
 
 // -- launchers (each .cu file owns its kernels); every per-frame input comes from device memory (fp, ctr) --

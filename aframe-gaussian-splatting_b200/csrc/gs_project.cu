@@ -6,6 +6,8 @@
 //                gsModelViewMatrix; views scene frames: every view per splat, the table row loaded once).
 //                <.., SH = 1..3> (contexts with gs_set_sh_degree > 0): each record's colour is the splat's view-dependent
 //                colour (sh_color below), its SH row loaded once with its cov_color row.
+//                <.., AA = true> (GS_RENDER_ANTIALIAS frames): each record's alpha byte is compensated for the 0.3 px^2
+//                blur (aa_alpha below); everything else of the record and its rectangle are the default instantiation's.
 //   k_count    : per entry of the draw order (== reference sortedIndexes): instance offset inside its 256-entry slice;
 //                per slice: total; last CTA: prefix over the slices + frame total D.
 //                Sparse frames (fewer than half of the splats sorted): each chunk's survivors are compacted first.
@@ -96,6 +98,24 @@ __device__ __forceinline__ uint32_t sh_color(uint32_t rgba, const uint4 *sh, con
 }
 
 // ---------------------------------------------------------------------------------------------
+// Anti-aliased alpha of a record (GS_RENDER_ANTIALIAS; include/gsplat_b200.h "Anti-aliased splats", restated by
+// tests/antialias_oracle.py).  cov00, cov10, cov11: the screen covariance before the shader's blur; d1, d2: its diagonal
+// after it (cov00 + 0.3, cov11 + 0.3).
+//   det0 = cov00 cov11 - cov10 cov10, det1 = d1 d2 - cov10 cov10, r = sqrt(det0 / det1), each operation rounded once
+//   comp = min(1, r) when det0 > 0, det1 > 0 and r is not NaN, else 0
+//   a' = q8(a / 255 * comp) = floor(clamp(., 0, 1) * 255 + 0.5).  The RGB bytes are kept.
+// comp <= 1, so a' never exceeds a; a byte is kept whenever |a comp - a| < 0.5.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t aa_alpha(uint32_t rgba, float cov00, float cov10, float cov11, float d1, float d2) {
+  const float det0 = SUB(MUL(cov00, cov11), MUL(cov10, cov10));
+  const float det1 = SUB(MUL(d1, d2), MUL(cov10, cov10));
+  const float r = __fsqrt_rn(DIV(det0, det1));
+  const float comp = (det0 > 0.0f && det1 > 0.0f && r == r) ? (r < 1.0f ? r : 1.0f) : 0.0f;
+  const float a = fminf(fmaxf(MUL(DIV((float)(rgba >> 24), 255.0f), comp), 0.0f), 1.0f);
+  return (rgba & 0x00FFFFFFu) | ((uint32_t)ADD(MUL(a, 255.0f), 0.5f) << 24);
+}
+
+// ---------------------------------------------------------------------------------------------
 // K2: vertex shader restatement.  One thread per resident splat, index order (coalesced 16 B + 16 B
 // loads, 32 B + 4 B stores).  Splats rejected by the worker filter are skipped, except splat 0 which
 // the reference may draw through the zero tail of quirk Q5.
@@ -105,7 +125,8 @@ __device__ __forceinline__ uint32_t sh_color(uint32_t rgba, const uint4 *sh, con
 // mv: the splat's gsModelViewMatrix (rc.mv, or its entity's in a scene frame).  c: its center_scale row; q: its
 // cov_color row, loaded on the first call that needs it (have_q), so a views frame's views load each row once.
 // SH > 0: shr receives the splat's SH row (sh) with q, and the record takes sh_color from eye, mv's camera position.
-template <int SH = 0>
+// AA (GS_RENDER_ANTIALIAS): the record's alpha byte is aa_alpha of this view's covariance (after sh_color's RGB).
+template <int SH = 0, bool AA = false>
 __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const float *mv, const float4 c,
                                                 const uint4 *__restrict__ cc, uint32_t i, uint32_t j,
                                                 float4 *__restrict__ rec_out, uint4 &q, bool &have_q,
@@ -212,6 +233,7 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
         rec_out[2 * (size_t)j] = make_float4(cx, cy, a1x, a1y);
         uint32_t rgba = q.w;
         if constexpr (SH > 0) rgba = sh_color<SH>(q.w, shr, c, eye);
+        if constexpr (AA) rgba = aa_alpha(rgba, cov00, cov10, cov11, diagonal1, diagonal2);
         rec_out[2 * (size_t)j + 1] = make_float4(a2x, a2y, __uint_as_float(rgba), zndc);
       }
     }
@@ -231,7 +253,8 @@ __device__ __forceinline__ uint32_t project_one(const RenderConsts &rc, const fl
 // into rec_x / rect_x at (v - 1) * x_stride.
 // SH (1..3, SH contexts): records take the view-dependent colour of degree SH: sh holds the table's SH rows, sh_cam the
 // camera position of entity k's view v at k * kMaxViews + v (plain frames: entry 0).
-template <bool BY_ENTRY, bool SCENE = false, bool STEREO = false, int SH = 0>
+// AA (GS_RENDER_ANTIALIAS frames): every record of every view takes its anti-aliased alpha (project_one).
+template <bool BY_ENTRY, bool SCENE = false, bool STEREO = false, int SH = 0, bool AA = false>
 __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, const uint4 *__restrict__ cc,
                                                  const float *__restrict__ depth,
                                                  const FrameParams *__restrict__ fp, float4 *__restrict__ rec_out,
@@ -277,25 +300,25 @@ __global__ void __launch_bounds__(256) k_project(const float4 *__restrict__ cs, 
       const int k = SCENE ? scene_find(s_first, s_end, n_obj, i) : 0;
       const float4 *cam = sh_cam + (size_t)k * kMaxViews;
       const float4 c = __ldg(cs + i);
-      if (!STEREO) return project_one<SH>(rc, SCENE ? scene->obj[k].mv : rc.mv, c, cc, i, j, rec_out, q, have_q, sh, shr, cam[0]);
+      if (!STEREO) return project_one<SH, AA>(rc, SCENE ? scene->obj[k].mv : rc.mv, c, cc, i, j, rec_out, q, have_q, sh, shr, cam[0]);
       const float(*mv)[16] = views->mv[k];
-      const uint32_t r0 = project_one<SH>(rc, mv[0], c, cc, i, j, rec_out, q, have_q, sh, shr, cam[0]);
+      const uint32_t r0 = project_one<SH, AA>(rc, mv[0], c, cc, i, j, rec_out, q, have_q, sh, shr, cam[0]);
       for (uint32_t v = 1; v < n_views; ++v) {
         const size_t x = (size_t)(v - 1) * x_stride;
-        rect_x[x + j] = project_one<SH>(views->view[v].rc, mv[v], c, cc, i, j, rec_x + 2 * x, q, have_q, sh, shr, cam[v]);
+        rect_x[x + j] = project_one<SH, AA>(views->view[v].rc, mv[v], c, cc, i, j, rec_x + 2 * x, q, have_q, sh, shr, cam[v]);
       }
       return r0;
     }
     if (!STEREO) {
       const float *mv = modelview(i);
-      return project_one(rc, mv, __ldg(cs + i), cc, i, j, rec_out, q, have_q);
+      return project_one<0, AA>(rc, mv, __ldg(cs + i), cc, i, j, rec_out, q, have_q);
     }
     const float(*mv)[16] = views->mv[scene_find(s_first, s_end, n_obj, i)];
     const float4 c = __ldg(cs + i);
-    const uint32_t r0 = project_one(rc, mv[0], c, cc, i, j, rec_out, q, have_q);
+    const uint32_t r0 = project_one<0, AA>(rc, mv[0], c, cc, i, j, rec_out, q, have_q);
     for (uint32_t v = 1; v < n_views; ++v) {
       const size_t x = (size_t)(v - 1) * x_stride;
-      rect_x[x + j] = project_one(views->view[v].rc, mv[v], c, cc, i, j, rec_x + 2 * x, q, have_q);
+      rect_x[x + j] = project_one<0, AA>(views->view[v].rc, mv[v], c, cc, i, j, rec_x + 2 * x, q, have_q);
     }
     return r0;
   };
@@ -613,9 +636,18 @@ __global__ void __launch_bounds__(256) k_emit_entries(const uint2 *__restrict__ 
   }
 }
 
-// the instantiation of k_project<BY_ENTRY, SCENE, STEREO> for the context's SH degree (0: the flat colour)
+// the instantiation of k_project<BY_ENTRY, SCENE, STEREO> for the context's SH degree (0: the flat colour) and the frame's
+// alpha (antialias: GS_RENDER_ANTIALIAS)
 template <bool BY_ENTRY, bool SCENE = false, bool STEREO = false>
-static decltype(&k_project<BY_ENTRY, SCENE, STEREO>) project_kernel(uint32_t sh_degree) {
+static decltype(&k_project<BY_ENTRY, SCENE, STEREO>) project_kernel(uint32_t sh_degree, bool antialias) {
+  if (antialias) {
+    switch (sh_degree) {
+      case 1: return k_project<BY_ENTRY, SCENE, STEREO, 1, true>;
+      case 2: return k_project<BY_ENTRY, SCENE, STEREO, 2, true>;
+      case 3: return k_project<BY_ENTRY, SCENE, STEREO, 3, true>;
+      default: return k_project<BY_ENTRY, SCENE, STEREO, 0, true>;
+    }
+  }
   switch (sh_degree) {
     case 1: return k_project<BY_ENTRY, SCENE, STEREO, 1>;
     case 2: return k_project<BY_ENTRY, SCENE, STEREO, 2>;
@@ -629,7 +661,7 @@ void launch_project(gs_context *c, const FrameParams *fp, const FrameCounters *c
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  launch_chain(c, project_kernel<false>(c->sh_degree), (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
+  launch_chain(c, project_kernel<false>(c->sh_degree, b.antialias), (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
                (const uint32_t *)nullptr, ctr, (const SceneTable *)nullptr,  // ctr: the sorted count picks the sparse-frame path
                (const ViewTable *)nullptr, (float4 *)nullptr, (uint32_t *)nullptr, 0u, (const uint4 *)c->sh, b.sh_cam);
 }
@@ -640,7 +672,7 @@ void launch_project_stereo(gs_context *c, const ViewTable *views, const SceneTab
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  launch_chain(c, project_kernel<false, true, true>(c->sh_degree), (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
+  launch_chain(c, project_kernel<false, true, true>(c->sh_degree, b.antialias), (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
                (const float *)c->depth, &views->view[0], b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, views,
                b.proj_recx, b.rectx, b.x_stride, (const uint4 *)c->sh, b.sh_cam);
 }
@@ -651,7 +683,7 @@ void launch_project_scene(gs_context *c, const FrameParams *fp, const SceneTable
   const uint64_t cap = (uint64_t)c->sm_count * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  launch_chain(c, project_kernel<false, true>(c->sh_degree), (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
+  launch_chain(c, project_kernel<false, true>(c->sh_degree, b.antialias), (int)blocks, 256, stream, (const float4 *)c->center_scale, (const uint4 *)c->cov_color,
                (const float *)c->depth, fp, b.proj_rec, b.rect, (const uint32_t *)nullptr, ctr, scene, (const ViewTable *)nullptr,
                (float4 *)nullptr, (uint32_t *)nullptr, 0u, (const uint4 *)c->sh, b.sh_cam);
 }
@@ -665,13 +697,13 @@ void launch_project_entries(gs_context *c, const FrameParams *fp, FrameCounters 
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   if (views) {
-    launch_chain(c, project_kernel<true, true, true>(c->sh_degree), (int)blocks, 256, stream, (const float4 *)c->center_scale,
+    launch_chain(c, project_kernel<true, true, true>(c->sh_degree, b.antialias), (int)blocks, 256, stream, (const float4 *)c->center_scale,
                  (const uint4 *)c->cov_color, (const float *)c->depth, &views->view[0], b.proj_rec, b.rect,
                  (const uint32_t *)b.order, (const FrameCounters *)ctr, scene, views, b.proj_recx, b.rectx, b.x_stride,
                  (const uint4 *)c->sh, b.sh_cam);
     return;
   }
-  launch_chain(c, scene ? project_kernel<true, true>(c->sh_degree) : project_kernel<true>(c->sh_degree), (int)blocks, 256, stream,
+  launch_chain(c, scene ? project_kernel<true, true>(c->sh_degree, b.antialias) : project_kernel<true>(c->sh_degree, b.antialias), (int)blocks, 256, stream,
                (const float4 *)c->center_scale, (const uint4 *)c->cov_color, (const float *)c->depth, fp, b.proj_rec, b.rect,
                (const uint32_t *)b.order, (const FrameCounters *)ctr, scene, (const ViewTable *)nullptr, (float4 *)nullptr,
                (uint32_t *)nullptr, 0u, (const uint4 *)c->sh, b.sh_cam);

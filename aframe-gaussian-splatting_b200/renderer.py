@@ -11,7 +11,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F, GS_RENDER_BLEND_UNORM8, GS_RENDER_OUT_DEVICE, GS_RENDER_OUT_TILED,
-                   GS_RENDER_REUSE_SORT, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32, GS_RENDER_SORT_RADIAL, GS_RENDER_STATS, GS_TARGET_DEPTH_WRITE, GS_TARGET_DEVICE, GsCubeFace, GsObject, GsRenderParams, GsStats, GsTarget)
+                   GS_RENDER_REUSE_SORT, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32, GS_RENDER_SORT_RADIAL, GS_RENDER_ANTIALIAS, GS_RENDER_STATS, GS_TARGET_DEPTH_WRITE, GS_TARGET_DEVICE, GsCubeFace, GsObject, GsRenderParams, GsStats, GsTarget)
 from .scenes import FrameInputs
 
 
@@ -39,6 +39,10 @@ def _f32(on: bool) -> int:
 
 def _radial(on: bool) -> int:
     return GS_RENDER_SORT_RADIAL if on else 0
+
+
+def _aa(on: bool) -> int:
+    return GS_RENDER_ANTIALIAS if on else 0
 
 
 @dataclass
@@ -264,18 +268,20 @@ class SplatContext:
 
     def render(self, frame: FrameInputs, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8, out: Optional[np.ndarray] = None,
                reuse_sort: bool = False, depth_in: Optional[np.ndarray] = None, stats: bool = False,
-               blend_unorm8: bool = False, sort_f32: bool = False, sort_radial: bool = False) -> np.ndarray:
+               blend_unorm8: bool = False, sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False) -> np.ndarray:
         """One frame into host memory: (H, W, 4) uint8 or float32, row 0 = bottom (GL orientation).
         blend_unorm8: GS_RENDER_BLEND_UNORM8, the RGBA8 target's blend rounded after every fragment (RGBA8 only).
         sort_f32: GS_RENDER_SORT_F32, ordered by the f32 depth itself instead of the reference's 16-bit buckets.
         sort_radial: GS_RENDER_SORT_RADIAL, ordered by each splat's distance from the camera, which turning it does not
-        change (the precise order's passes over f32(-r) in place of the depth)."""
+        change (the precise order's passes over f32(-r) in place of the depth).
+        antialias: GS_RENDER_ANTIALIAS, each splat's alpha scaled by sqrt(det S / det(S + 0.3 I)) of its screen
+        covariance S, so the shader's 0.3 px^2 blur no longer adds coverage (every draw and pick below takes it)."""
         dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
         if out is None:
             out = np.empty((frame.height, frame.width, 4), dtype)
         assert out.dtype == dtype and out.size == frame.height * frame.width * 4 and out.flags["C_CONTIGUOUS"]
         p = self.make_params(frame, bg, fmt, (GS_RENDER_REUSE_SORT if reuse_sort else 0) | (GS_RENDER_STATS if stats else 0) |
-                             _blend8(blend_unorm8) | _f32(sort_f32) | _radial(sort_radial), depth_in=depth_in)
+                             _blend8(blend_unorm8) | _f32(sort_f32) | _radial(sort_radial) | _aa(antialias), depth_in=depth_in)
         st = GsStats()
         self._check(self._lib.gs_render(self._h, C.byref(p), _ptr(out), C.byref(st)))
         self.last_stats = st
@@ -284,14 +290,15 @@ class SplatContext:
     def render_scene(self, frame: FrameInputs, objects: Sequence[SceneObject], bg=(0.0, 0.0, 0.0, 0.0),
                      fmt: int = GS_FORMAT_RGBA8, color_in: Optional[np.ndarray] = None,
                      depth_in: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None, stats: bool = False,
-                     blend_unorm8: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False) -> np.ndarray:
+                     blend_unorm8: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False) -> np.ndarray:
         """gs_render_scene: several entities in one frame, drawn whole in the order given, over `color_in` (the scene's
         colour buffer, (H, W, 4) of the output dtype, row 0 = bottom; None = bg) and depth-tested against `depth_in`.
         `frame` supplies projection, size and focal; its modelview and cutout are ignored.  blend_unorm8 as render().
         interleave (GS_RENDER_SCENE_INTERLEAVE): every entity's splats in one back-to-front order, so overlapping
         entities blend by depth instead of being drawn whole one after another.  sort_f32 (GS_RENDER_SORT_F32): the
         order by each splat's f32 depth instead of the reference's 16-bit buckets, in either mode; sort_radial
-        (GS_RENDER_SORT_RADIAL): that order by each splat's distance from the camera in place of its depth."""
+        (GS_RENDER_SORT_RADIAL): that order by each splat's distance from the camera in place of its depth.  antialias
+        as render()."""
         dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
         if out is None:
             out = np.empty((frame.height, frame.width, 4), dtype)
@@ -302,7 +309,7 @@ class SplatContext:
             if col.size != frame.width * frame.height * 4:
                 raise ValueError("color_in must hold width*height RGBA pixels")
         p = self.make_params(frame, bg, fmt, (GS_RENDER_STATS if stats else 0) | _blend8(blend_unorm8) | _interleave(interleave) |
-                             _f32(sort_f32) | _radial(sort_radial), depth_in=depth_in)
+                             _f32(sort_f32) | _radial(sort_radial) | _aa(antialias), depth_in=depth_in)
         objs = make_objects(objects)
         st = GsStats()
         self._check(self._lib.gs_render_scene(self._h, C.byref(p), objs, len(objects), _ptr(col), _ptr(out), C.byref(st)))
@@ -320,13 +327,14 @@ class SplatContext:
         return t.value
 
     def pick_scene(self, frame: FrameInputs, objects: Sequence[SceneObject], points, depth_in: Optional[np.ndarray] = None,
-                   depth_device: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False):
+                   depth_device: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False):
         """gs_pick_scene: for each pixel (x, y) of `points` ((n, 2), row 0 = bottom) of the scene frame render_scene draws
         with these arguments, the splat where the pixel turns half opaque.  Returns (splat u32, object i32, depth f32,
         alpha f32) arrays of n entries: GS_PICK_NONE / -1 / 1 where the pixel never does.  depth_in as render_scene, or a
-        device pointer (int) with depth_device=True; interleave and sort_f32 as render_scene (the pick walks that order)."""
+        device pointer (int) with depth_device=True; interleave and sort_f32 as render_scene (the pick walks that order);
+        antialias as render() (the pick walks the anti-aliased alphas)."""
         xy = np.ascontiguousarray(points, dtype=np.uint32).reshape(-1, 2)
-        p = self.make_params(frame, flags=_interleave(interleave) | _f32(sort_f32) | _radial(sort_radial), depth_in=None if depth_device else depth_in)
+        p = self.make_params(frame, flags=_interleave(interleave) | _f32(sort_f32) | _radial(sort_radial) | _aa(antialias), depth_in=None if depth_device else depth_in)
         if depth_device:
             p.depth_in = int(depth_in)
             p.flags |= _lib.GS_RENDER_DEPTH_DEVICE
@@ -356,14 +364,14 @@ class SplatContext:
         return out[:cnt.value].copy()
 
     def render_stereo(self, view: np.ndarray, eyes, cutout: Optional[np.ndarray] = None, bg=(0.0, 0.0, 0.0, 0.0),
-                      fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False):
+                      fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False, antialias: bool = False):
         """gs_render_stereo: one sort with the head camera's `view` (+ cutout), one draw per eye (two FrameInputs).
-        Returns the two frames, row 0 = bottom.  blend_unorm8 as render()."""
+        Returns the two frames, row 0 = bottom.  blend_unorm8 and antialias as render()."""
         assert len(eyes) == 2
         dtype = np.uint8 if fmt == GS_FORMAT_RGBA8 else np.float32
         outs = [np.empty((e.height, e.width, 4), dtype) for e in eyes]
         arr = (GsRenderParams * 2)()
-        keep = [self.make_params(e, bg, fmt, _blend8(blend_unorm8)) for e in eyes]
+        keep = [self.make_params(e, bg, fmt, _blend8(blend_unorm8) | _aa(antialias)) for e in eyes]
         for i in range(2):
             C.memmove(C.addressof(arr[i]), C.addressof(keep[i]), C.sizeof(GsRenderParams))
         ptrs = (C.c_void_p * 2)(outs[0].ctypes.data, outs[1].ctypes.data)
@@ -400,7 +408,7 @@ class SplatContext:
 
     def render_scene_stereo(self, eyes: Sequence[FrameInputs], objects: Sequence[SceneObject], eye_modelviews,
                             color_in=(None, None), depth_in=(None, None), bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
-                            blend_unorm8: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False):
+                            blend_unorm8: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False):
         """gs_render_scene_stereo: one WebXR frame of a multi-entity page.  `objects` carry each entity's range, HEAD
         modelview (its sort) and cutout, in draw order; eyes[e] (FrameInputs) gives eye e's projection, size and focal;
         eye_modelviews[e][k] is entity k's modelview of eye e.  color_in[e] / depth_in[e]: eye e's colour target ((H, W, 4)
@@ -416,7 +424,7 @@ class SplatContext:
                 if c.size != e.width * e.height * 4:
                     raise ValueError("color_in must hold width*height RGBA pixels")
             cols.append(c)
-        params = [self.make_params(e, bg, fmt, _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial), depth_in=d)
+        params = [self.make_params(e, bg, fmt, _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial) | _aa(antialias), depth_in=d)
                   for e, d in zip(eyes, depth_in)]
         arr, objs, mv, col, ptrs = self._stereo_args(params, objects, eye_modelviews,
                                                      [None if c is None else c.ctypes.data for c in cols],
@@ -440,7 +448,7 @@ class SplatContext:
 
     def render_scene_views(self, views: Sequence[FrameInputs], objects: Sequence[SceneObject], view_mvs,
                            color_in=None, depth_in=None, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
-                           blend_unorm8: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False):
+                           blend_unorm8: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False):
         """gs_render_scene_views: every view of one WebXR frame (1..GS_MAX_VIEWS FrameInputs, each at its own size) from
         one head sort.  view_mvs[v][k] is entity k's modelview of view v; color_in[v] / depth_in[v] as in
         render_scene_stereo (None = none for every view).  Returns one frame per view, row 0 = bottom.  interleave as
@@ -457,7 +465,7 @@ class SplatContext:
                 if c.size != v.width * v.height * 4:
                     raise ValueError("color_in must hold width*height RGBA pixels")
             cols.append(c)
-        params = [self.make_params(v, bg, fmt, _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial), depth_in=d)
+        params = [self.make_params(v, bg, fmt, _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial) | _aa(antialias), depth_in=d)
                   for v, d in zip(views, depth_in)]
         arr, objs, mv, col, ptrs = self._views_args(params, objects, view_mvs,
                                                     [None if c is None else c.ctypes.data for c in cols],
@@ -481,7 +489,7 @@ class SplatContext:
 
     def render_scene_cameras(self, cams: Sequence[FrameInputs], objects: Sequence[SceneObject], cam_mvs,
                              color_in=None, depth_in=None, bg=(0.0, 0.0, 0.0, 0.0), fmt: int = GS_FORMAT_RGBA8,
-                             blend_unorm8: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False):
+                             blend_unorm8: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False):
         """gs_render_scene_cameras: 1..GS_MAX_CAMERAS cameras that may look different ways (cube faces, a rear view), each
         at its own size and each sorted with its own matrices.  cam_mvs[c][k] is entity k's modelview of camera c (its sort
         and its draw); `objects` give the ranges and cutouts (their modelviews are ignored).  color_in[c] / depth_in[c] as
@@ -499,7 +507,7 @@ class SplatContext:
                 if c.size != v.width * v.height * 4:
                     raise ValueError("color_in must hold width*height RGBA pixels")
             cols.append(c)
-        params = [self.make_params(v, bg, fmt, _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial), depth_in=d)
+        params = [self.make_params(v, bg, fmt, _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial) | _aa(antialias), depth_in=d)
                   for v, d in zip(cams, depth_in)]
         arr, objs, mv, col, ptrs = self._views_args(params, objects, cam_mvs,
                                                     [None if c is None else c.ctypes.data for c in cols],
@@ -609,7 +617,7 @@ class SplatContext:
     def render_scene_target(self, frame: FrameInputs, objects: Sequence[SceneObject], color: np.ndarray,
                             depth: Optional[np.ndarray] = None, viewport=(0, 0), fmt: int = GS_FORMAT_RGBA8,
                             stats: bool = False, blend_unorm8: bool = False, write_depth: bool = False,
-                            interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False) -> np.ndarray:
+                            interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False) -> np.ndarray:
         """gs_render_scene_target: the scene frame blended IN PLACE into the rectangle of frame.width x frame.height at
         viewport = (x, y) of `color` ((rows, pitch, 4), row 0 = bottom), depth-tested against `depth` ((rows, pitch) f32
         window-space depth, or None).  Nothing outside the rectangle is read or written.  Returns `color`.
@@ -620,7 +628,7 @@ class SplatContext:
         t = self._array_target(color, depth, fmt, write_depth)
         p = self.make_params(frame, fmt=fmt,
                              flags=(GS_RENDER_STATS if stats else 0) | _blend8(blend_unorm8) | _interleave(interleave) |
-                             _f32(sort_f32) | _radial(sort_radial))
+                             _f32(sort_f32) | _radial(sort_radial) | _aa(antialias))
         st = GsStats()
         self._check(self._lib.gs_render_scene_target(self._h, C.byref(p), make_objects(objects), len(objects), C.byref(t),
                                                      int(viewport[0]), int(viewport[1]), C.byref(st)))
@@ -639,14 +647,14 @@ class SplatContext:
     def render_scene_stereo_target(self, eyes: Sequence[FrameInputs], objects: Sequence[SceneObject], eye_modelviews,
                                    color: np.ndarray, depth: Optional[np.ndarray] = None, eye_xy=None,
                                    fmt: int = GS_FORMAT_RGBA8, blend_unorm8: bool = False,
-                                   write_depth: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False) -> np.ndarray:
+                                   write_depth: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False) -> np.ndarray:
         """gs_render_scene_stereo_target: one WebXR frame drawn IN PLACE into one layer ((rows, pitch, 4) colour, optional
         (rows, pitch) f32 depth): eye e at (eye_xy[2e], eye_xy[2e+1]); eye_xy None = side by side, (0, 0, w, 0).
         Arguments as render_scene_stereo; buffers and write_depth as render_scene_target.  Returns `color`."""
         t = self._array_target(color, depth, fmt, write_depth)
         st = GsStats()
         args = self._stereo_target_args(eyes, fmt, objects, eye_modelviews, eye_xy,
-                                        _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial))
+                                        _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial) | _aa(antialias))
         self._check(self._lib.gs_render_scene_stereo_target(self._h, args[0], args[1], args[2], len(objects), C.byref(t),
                                                             args[3], C.byref(st)))
         self.last_stats = st
@@ -666,14 +674,14 @@ class SplatContext:
 
     def render_scene_views_target(self, views: Sequence[FrameInputs], objects: Sequence[SceneObject], view_mvs,
                                   color: np.ndarray, view_xy, depth: Optional[np.ndarray] = None, fmt: int = GS_FORMAT_RGBA8,
-                                  blend_unorm8: bool = False, write_depth: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False) -> np.ndarray:
+                                  blend_unorm8: bool = False, write_depth: bool = False, interleave: bool = False, sort_f32: bool = False, sort_radial: bool = False, antialias: bool = False) -> np.ndarray:
         """gs_render_scene_views_target: one WebXR frame of every view drawn IN PLACE into one layer ((rows, pitch, 4)
         colour, optional (rows, pitch) f32 depth): view v at (view_xy[2v], view_xy[2v+1]).  Arguments as
         render_scene_views; buffers and write_depth as render_scene_target.  Returns `color`."""
         t = self._array_target(color, depth, fmt, write_depth)
         st = GsStats()
         args = self._views_target_args(views, fmt, objects, view_mvs, view_xy,
-                                       _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial))
+                                       _blend8(blend_unorm8) | _interleave(interleave) | _f32(sort_f32) | _radial(sort_radial) | _aa(antialias))
         self._check(self._lib.gs_render_scene_views_target(self._h, args[0], len(views), args[1], args[2], len(objects),
                                                            C.byref(t), args[3], C.byref(st)))
         self.last_stats = st

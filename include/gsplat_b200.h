@@ -78,9 +78,12 @@ enum {
                                   (see "Precise order" below); gs_render_stereo, GS_RENDER_REUSE_SORT, _OUT_TILED,
                                   _OUT_PEER and sharded contexts refuse it                             */
   /* bit 10 stays unassigned: gs_sort_scene_flags and gs_pick_scene refuse it as an unknown flag */
-  GS_RENDER_SORT_RADIAL = 1u << 11 /* order the frame by each splat's distance from the camera, which turning the
+  GS_RENDER_SORT_RADIAL = 1u << 11, /* order the frame by each splat's distance from the camera, which turning the
                                       camera does not change (see "Radial order" below); refused where
                                       GS_RENDER_SORT_F32 is                                              */
+  GS_RENDER_ANTIALIAS = 1u << 12 /* scale each drawn splat's alpha by the share of its footprint's energy that the
+                                    shader's 0.3 px^2 blur did not add (see "Anti-aliased splats" below); accepted
+                                    by every draw and by gs_pick_scene, refused by gs_sort_scene_flags      */
 };
 
 /*
@@ -538,6 +541,28 @@ GS_API int gs_render_stereo(gs_context *ctx, const float view[4], const float *c
  *   - consequences: the order depends on the camera's position, not on its rotation, up to the rounding of the rotated f32
  *     matrix.  A stereo or views frame's head order no longer changes while the head only turns.  A splat can be nearer
  *     than another by z and farther by distance, so where the two overlap the radial frame blends them the other way.
+ *
+ * Anti-aliased splats (GS_RENDER_ANTIALIAS in gs_render_params.flags; opt-in, default frames are unchanged): the vertex
+ * shader adds 0.3 px^2 to both diagonal terms of every splat's screen covariance (index.js:139-141), which keeps a splat
+ * at least about half a pixel wide, and the footprint's alpha energy a 2 pi sqrt(det) grows by sqrt(det(S + 0.3 I) / det S).
+ * With this flag each record's alpha is scaled back by that factor, the compensation of trainers that rasterise
+ * anti-aliased (gsplat's rasterize_mode="antialiased", Mip-Splatting's 2D filter):
+ *   - in the projection, fp32, every operation rounded once and nothing contracted; cov00, cov10, cov11 are the screen
+ *     covariance of the shader, diagonal1 = cov00 + 0.3, diagonal2 = cov11 + 0.3 (each view, eye and camera with its own):
+ *       det0 = cov00 cov11 - cov10 cov10, det1 = diagonal1 diagonal2 - cov10 cov10, r = sqrt(det0 / det1) (correctly rounded)
+ *       comp = min(1, r) if det0 > 0, det1 > 0 and r is not NaN, else 0
+ *       a' = q8(a / 255 * comp), q8(x) = floor(clamp(x, 0, 1) * 255 + 0.5), a the record's alpha byte;
+ *   - the record keeps everything else: RGB bytes (the SH colour on SH contexts), centre, axes, z/w and rectangle.  A
+ *     rank-1 covariance (det0 <= 0, a needle) gets alpha 0 and is still binned and drawn with zero weight;
+ *   - a' flows unchanged through binning, the raster and its stop rule, GS_RENDER_BLEND_UNORM8, picks, GS_TARGET_DEPTH_WRITE,
+ *     the slab path and sharded output;
+ *   - consequences: n_visible, n_instances and n_instances_kept of a one-pass frame are those of the default frame; a
+ *     record keeps its byte whenever |a comp - a| < 0.5, so a scene whose splats all project large gives the default
+ *     frame byte for byte.  Without the r^2 <= 4 cut and the 0.1 clamp on lambda2 a footprint's alpha energy would be
+ *     a 2 pi sqrt(det0) (1 - e^-4), which does not depend on the blur;
+ *   - scope: every draw (gs_render[_async] with or without GS_RENDER_REUSE_SORT, gs_render_stereo, every gs_render_scene*,
+ *     views, target and cameras call) and gs_pick_scene, with any other flag they accept and on sharded contexts.
+ *     gs_sort_scene_flags refuses it: it is a drawing flag and changes no order.
  */
 #define GS_MAX_OBJECTS 64
 typedef struct gs_object {
