@@ -64,6 +64,11 @@ class GsCropBox(C.Structure):
     _fields_ = [("first", C.c_uint32), ("count", C.c_uint32), ("mode", C.c_uint32), ("box16", C.c_float * 16)]
 
 
+class GsExportPart(C.Structure):
+    """gs_export_part: one table range of gs_export_parts and the affine map of its .splat row frame (column-major)."""
+    _fields_ = [("first", C.c_uint32), ("count", C.c_uint32), ("pad", C.c_uint32 * 2), ("m", C.c_double * 16)]
+
+
 GS_PICK_NONE = 0xFFFFFFFF
 GS_MAX_PICKS = 4096
 
@@ -109,6 +114,9 @@ SYMBOLS = {
     "gs_read_sh": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
     "gs_set_keep_rows": (C.c_int, [_P, C.c_uint32]),
     "gs_export": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_uint32, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "gs_export_parts": (C.c_int, [_P, C.POINTER(GsExportPart), C.c_uint32, C.c_uint32, _P, C.c_size_t,
+                                  C.POINTER(C.c_size_t)]),
+    "gs_sh_rotation": (C.c_int, [C.POINTER(C.c_double), C.c_uint32, C.POINTER(C.c_double)]),
     "gs_sort": (C.c_int, [_P, C.POINTER(C.c_float), C.POINTER(C.c_float), _P, C.POINTER(C.c_uint32)]),
     "gs_render": (C.c_int, [_P, C.POINTER(GsRenderParams), _P, C.POINTER(GsStats)]),
     "gs_render_async": (C.c_int, [_P, C.POINTER(GsRenderParams), _P, C.POINTER(C.c_uint64)]),

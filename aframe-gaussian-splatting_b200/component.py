@@ -110,6 +110,31 @@ class SortWorker:
         return self.ctx.push_ply(blob)
 
 
+_ROW_TO_LOCAL = np.diag([1.0, -1.0, -1.0, 1.0])  # G: the .splat row frame (x, y, z) -> the entity's local frame
+
+
+def _affine_inverse(w: np.ndarray) -> np.ndarray:
+    inv = np.eye(4)
+    inv[:3, :3] = np.linalg.inv(w[:3, :3])
+    inv[:3, 3] = -(inv[:3, :3] @ w[:3, 3])
+    return inv
+
+
+def export_part_matrix(root_world, world):
+    """gs_export_parts' matrix (16 doubles, column-major) of an entity with matrixWorld `world` saved into a file loaded
+    under an entity with matrixWorld `root_world` (None: the identity): G W_root^-1 W G in fp64, G = diag(1, -1, -1, 1).
+    The table holds a row's (x, y, -z) (gs_push_splats) and the modelview conjugates the local frame by diag(1, -1, 1, 1)
+    (getModelViewMatrix), so G takes a row to the entity's local frame.  None (the exact identity) when the two matrices
+    are equal bit for bit."""
+    w = np.asarray(world, np.float64).reshape(4, 4).T
+    r = np.eye(4) if root_world is None else np.asarray(root_world, np.float64).reshape(4, 4).T
+    if np.array_equal(w.view(np.uint64), r.view(np.uint64)):
+        return None
+    a = _ROW_TO_LOCAL @ (w if root_world is None else _affine_inverse(r) @ w) @ _ROW_TO_LOCAL
+    a[3] = (0.0, 0.0, 0.0, 1.0)  # affine by construction: the product's bottom row is exact in exact arithmetic
+    return a.T.reshape(16)
+
+
 class GaussianSplattingComponent:
     """`gaussian_splatting` (index.js:1-746) for the sort + draw path."""
 
@@ -462,6 +487,23 @@ class SplatScene:
         "compressed_ply".  Returns the bytes, and also writes them to `path` when given.  Needs keep_rows=True."""
         first, count = self._range[id(component)]
         blob = self.renderer.export(first, count, format)
+        if path is not None:
+            with open(path, "wb") as f:
+                f.write(blob)
+        return blob
+
+    def save_all(self, path=None, format: str = "splat", root: Optional[Object3D] = None, entities=None) -> bytes:
+        """Write every entity (or those in `entities`), in draw order, as one file with each entity's placement baked
+        in (gs_export_parts): an entity whose object3D.matrixWorld is root's (None: the identity, the world frame) draws
+        each splat where this scene draws it once the file is loaded into it.  Rotations, mirrors and uniform scales are
+        baked into the centres, scales, rotations and SH coefficients; a non-uniform scale between root and an entity
+        raises GsError.  Cutouts are not applied: crop() an entity first to save only what its cutout shows.  format as
+        save(); returns the bytes, and also writes them to `path` when given.  Needs keep_rows=True."""
+        keep = None if entities is None else {id(e) for e in entities}
+        w_root = None if root is None else root.matrixWorld.elements
+        parts = [(*self._range[id(e)], export_part_matrix(w_root, e.object.matrixWorld.elements))
+                 for e in self.entities if keep is None or id(e) in keep]
+        blob = self.renderer.export_parts(parts, format)
         if path is not None:
             with open(path, "wb") as f:
                 f.write(blob)

@@ -1019,6 +1019,89 @@ extern "C" int gs_export(gs_context *c, uint32_t first, uint32_t count, uint32_t
   return GS_OK;
 }
 
+// gs_export_parts: every part's rows transformed (gs_transform.cu) into one stream-ordered temporary laid out as the
+// kept rows and SH rows, then the file built from it as gs_export builds it from the table
+extern "C" int gs_export_parts(gs_context *c, const gs_export_part *parts, uint32_t n_parts, uint32_t format, void *out,
+                               size_t cap, size_t *out_bytes) {
+  if (!c) return GS_ERR_INVALID;
+  if (!out_bytes) return fail(c, GS_ERR_INVALID, "gs_export_parts: out_bytes is NULL");
+  *out_bytes = 0;
+  if (!parts) return fail(c, GS_ERR_INVALID, "gs_export_parts: parts is NULL");
+  if (n_parts == 0 || n_parts > (uint32_t)GS_MAX_OBJECTS)
+    return fail(c, GS_ERR_INVALID, "gs_export_parts: between 1 and GS_MAX_OBJECTS parts");
+  std::vector<TransformConsts> tcs(n_parts);
+  uint64_t total_rows = 0;
+  for (uint32_t p = 0; p < n_parts; ++p) {
+    if ((uint64_t)parts[p].first + parts[p].count > c->n)
+      return fail(c, GS_ERR_INVALID, "gs_export_parts: range past the resident splats");
+    if (!transform_consts(parts[p].m, c->sh_degree, tcs[p]))
+      return fail(c, GS_ERR_INVALID, "gs_export_parts: a matrix that is not finite, affine and a similarity");
+    total_rows += parts[p].count;
+  }
+  if (total_rows > 0xFFFFFFFFull) return fail(c, GS_ERR_INVALID, "gs_export_parts: more than 2^32 - 1 rows");
+  const uint32_t n = (uint32_t)total_rows;
+  if (format != GS_EXPORT_SPLAT && format != GS_EXPORT_PLY && format != GS_EXPORT_PLY_COMPRESSED)
+    return fail(c, GS_ERR_INVALID, "gs_export_parts: unknown format");
+  const uint32_t k = sh_coeffs(c->sh_degree);
+  const std::string head = format == GS_EXPORT_SPLAT ? std::string() : export_header(format, n, k);
+  const size_t body = export_body_bytes(format, n, k), total = head.size() + body;
+  *out_bytes = total;
+  if (!c->keep_rows) return fail(c, GS_ERR_INVALID, "gs_export_parts: the context keeps no .splat rows (gs_set_keep_rows)");
+  if (!out) return GS_OK;
+  if (cap < total) return fail(c, GS_ERR_INVALID, "gs_export_parts: cap is below the file size");
+  GS_CUDA(c, cudaSetDevice(c->device));
+  cudaStream_t st = c->push_stream;
+  uint8_t *dst = (uint8_t *)out + head.size();
+  if (n) {
+    const size_t row_bytes = (size_t)n * 32, sh_bytes = (size_t)n * 16 * c->sh_vecs;
+    uint8_t *tmp = nullptr;
+    cudaError_t e = cudaMallocAsync((void **)&tmp, row_bytes + sh_bytes + (format == GS_EXPORT_SPLAT ? 0 : body), st);
+    if (e) {
+      cudaGetLastError();  // an allocation failure is not sticky
+      GS_CUDA(c, e);
+    }
+    uint4 *rows = (uint4 *)tmp, *sh = c->sh ? (uint4 *)(tmp + row_bytes) : nullptr;
+    uint32_t at = 0;
+    for (uint32_t p = 0; p < n_parts && !e; ++p) {
+      const gs_export_part &pt = parts[p];
+      if (!pt.count) continue;
+      const TransformConsts &tc = tcs[p];
+      const uint4 *src_sh = c->sh ? c->sh + (size_t)pt.first * c->sh_vecs : nullptr;
+      if (tc.copy_pos && tc.copy_scale && tc.copy_rot) {  // the identity: the rows as they are
+        e = cudaMemcpyAsync(rows + 2 * (size_t)at, c->keep + 2 * (size_t)pt.first, (size_t)pt.count * 32,
+                            cudaMemcpyDeviceToDevice, st);
+        if (!e && sh)
+          e = cudaMemcpyAsync(sh + (size_t)at * c->sh_vecs, src_sh, (size_t)pt.count * 16 * c->sh_vecs,
+                              cudaMemcpyDeviceToDevice, st);
+      } else {
+        launch_transform_rows(c->keep + 2 * (size_t)pt.first, src_sh, c->sh_degree, pt.count, tc, rows + 2 * (size_t)at,
+                              sh ? sh + (size_t)at * c->sh_vecs : nullptr, st);
+        e = cudaGetLastError();
+      }
+      at += pt.count;
+    }
+    uint8_t *src = tmp;  // .splat: the transformed rows are the body
+    if (!e && format != GS_EXPORT_SPLAT) {
+      src = tmp + row_bytes + sh_bytes;
+      if (format == GS_EXPORT_PLY)
+        launch_export_ply_rows(rows, sh, c->sh_degree, n, src, st);
+      else
+        launch_export_compressed_rows(rows, sh, c->sh_degree, n, src, st);
+      e = cudaGetLastError();
+    }
+    if (!e) e = cudaMemcpyAsync(dst, src, body, cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(tmp, st);
+    if (!e) e = cudaStreamSynchronize(st);
+    GS_CUDA(c, e);
+  }
+  memcpy(out, head.data(), head.size());
+  return GS_OK;
+}
+
+extern "C" int gs_sh_rotation(const double q9[9], uint32_t degree, double *out) {
+  return sh_rotation(q9, degree, out) ? GS_OK : GS_ERR_INVALID;
+}
+
 static void fill_sort_consts(SortConsts &sc, const float view[4], const float *cutout) {
   memset(&sc, 0, sizeof(sc));
   for (int i = 0; i < 4; ++i) sc.view[i] = (double)view[i];

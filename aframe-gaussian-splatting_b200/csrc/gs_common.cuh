@@ -661,6 +661,30 @@ void launch_crop_write(gs_context *c, const CropScratch &s, uint32_t lo, uint32_
 // compressed PLY body: ceil(n / 256) chunk rows of 18 floats, n 16 B vertex words, n 3 sh_k SH bytes
 void launch_export_ply(gs_context *c, uint32_t first, uint32_t n, uint8_t *body, cudaStream_t st);
 void launch_export_compressed(gs_context *c, uint32_t first, uint32_t n, uint8_t *body, cudaStream_t st);
+// the same kernels over n rows laid out as the kept rows (2 words each) and SH rows (sh_vecs words each) of a degree
+// `degree` context: gs_export_parts runs them on its transformed rows
+void launch_export_ply_rows(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, uint8_t *body, cudaStream_t st);
+void launch_export_compressed_rows(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, uint8_t *body,
+                                   cudaStream_t st);
+// gs_export_parts (gs_transform.cu): one part's transform, as k_transform_rows takes it (include/gsplat_b200.h)
+struct TransformConsts {
+  double L[9];        // the upper 3x3, row-major
+  double t[3];
+  double s;           // the scale, after the snap to 1
+  double q[4];        // qQ: w, x, y, z
+  double R[83];       // R_1^T (9), R_2^T (25), R_3^T (49), row-major (the first 9, 34 or 83 used)
+  uint32_t copy_pos;  // L == I and t == 0: the centre is copied
+  uint32_t copy_scale;  // s == 1: the scales are copied
+  uint32_t copy_rot;    // Q == I: the rotation bytes and SH coefficients are copied
+  uint32_t pad;
+};
+// the part constants of matrix m (16 doubles, column-major) on a degree `degree` context; false: the matrix is refused
+bool transform_consts(const double m[16], uint32_t degree, TransformConsts &tc);
+// R_l^T of q9 (row-major) for l = 1..degree into out (gs_sh_rotation); false: refused
+bool sh_rotation(const double q9[9], uint32_t degree, double *out);
+// k_transform_rows over n rows (2 words each) and their SH rows (sh_vecs(degree) words each) into out_rows / out_sh
+void launch_transform_rows(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, const TransformConsts &tc,
+                           uint4 *out_rows, uint4 *out_sh, cudaStream_t st);
 // PLY push: decode `rows` whole rows of a staged body chunk into .splat rows + importance keys at [first_row, ...);
 // sh (SH contexts, else NULL): the rows' coefficients into sh_rows (sh->vecs words per row), in file order too
 void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,

@@ -227,18 +227,26 @@ __global__ void __launch_bounds__(256) k_export_compressed(const uint4 *__restri
 static const uint4 *kept_rows(gs_context *c, uint32_t first) { return c->keep + 2 * (size_t)first; }
 static const uint4 *sh_rows(gs_context *c, uint32_t first) { return c->sh ? c->sh + (size_t)first * c->sh_vecs : nullptr; }
 
-void launch_export_ply(gs_context *c, uint32_t first, uint32_t n, uint8_t *body, cudaStream_t st) {
+void launch_export_ply_rows(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, uint8_t *body, cudaStream_t st) {
   const uint32_t grid = (n + 255) / 256;
-  auto kernel = c->sh_degree == 0 ? k_export_ply<0> : c->sh_degree == 1 ? k_export_ply<3>
-              : c->sh_degree == 2 ? k_export_ply<8> : k_export_ply<15>;
-  kernel<<<grid, 256, 0, st>>>(kept_rows(c, first), sh_rows(c, first), c->sh_vecs, n, (uint32_t *)body);
+  auto kernel = degree == 0 ? k_export_ply<0> : degree == 1 ? k_export_ply<3> : degree == 2 ? k_export_ply<8> : k_export_ply<15>;
+  kernel<<<grid, 256, 0, st>>>(rows, sh, sh_vecs(degree), n, (uint32_t *)body);
+}
+
+void launch_export_compressed_rows(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, uint8_t *body,
+                                   cudaStream_t st) {
+  const uint32_t grid = (n + 255) / 256;
+  auto kernel = degree == 0 ? k_export_compressed<0> : degree == 1 ? k_export_compressed<3>
+              : degree == 2 ? k_export_compressed<8> : k_export_compressed<15>;
+  kernel<<<grid, 256, 0, st>>>(rows, sh, sh_vecs(degree), n, body);
+}
+
+void launch_export_ply(gs_context *c, uint32_t first, uint32_t n, uint8_t *body, cudaStream_t st) {
+  launch_export_ply_rows(kept_rows(c, first), sh_rows(c, first), c->sh_degree, n, body, st);
 }
 
 void launch_export_compressed(gs_context *c, uint32_t first, uint32_t n, uint8_t *body, cudaStream_t st) {
-  const uint32_t grid = (n + 255) / 256;
-  auto kernel = c->sh_degree == 0 ? k_export_compressed<0> : c->sh_degree == 1 ? k_export_compressed<3>
-              : c->sh_degree == 2 ? k_export_compressed<8> : k_export_compressed<15>;
-  kernel<<<grid, 256, 0, st>>>(kept_rows(c, first), sh_rows(c, first), c->sh_vecs, n, body);
+  launch_export_compressed_rows(kept_rows(c, first), sh_rows(c, first), c->sh_degree, n, body, st);
 }
 
 }  // namespace gs

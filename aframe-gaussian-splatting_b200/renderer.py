@@ -222,6 +222,23 @@ class SplatContext:
         self._check(self._lib.gs_export(self._h, int(first), int(count), int(fmt), _ptr(out), out.size, C.byref(size)))
         return out.tobytes()
 
+    def export_parts(self, parts, format="splat") -> bytes:
+        """gs_export_parts: several table ranges as one file, in the order given, each row first transformed by its
+        range's affine map of the .splat row frame.  parts: a sequence of (first, count, m16), m16 16 numbers in
+        column-major order (a similarity: rotation, mirror, uniform scale, translation) or None for the identity.  The SH
+        coefficients of an SH context are rotated with the rows.  format as export().  Needs keep_rows."""
+        fmt = _EXPORT_FORMATS.get(format, format)
+        arr = (_lib.GsExportPart * max(len(parts), 1))()
+        for i, (first, count, m16) in enumerate(parts):
+            arr[i].first, arr[i].count = int(first), int(count)
+            m = np.eye(4) if m16 is None else np.asarray(m16, np.float64).reshape(16)
+            arr[i].m[:] = [float(v) for v in np.asarray(m, np.float64).reshape(16)]
+        size = C.c_size_t()
+        self._check(self._lib.gs_export_parts(self._h, arr, len(parts), int(fmt), None, 0, C.byref(size)))
+        out = np.empty(size.value, np.uint8)
+        self._check(self._lib.gs_export_parts(self._h, arr, len(parts), int(fmt), _ptr(out), out.size, C.byref(size)))
+        return out.tobytes()
+
     def read_sh(self, first: int = 0, n: Optional[int] = None) -> np.ndarray:
         """gs_read_sh: the SH coefficients of splats [first, first+n) as (n, 3, K) float16, K = (degree+1)^2 - 1, in table
         order (channel-major per splat, INRIA's f_rest order)."""

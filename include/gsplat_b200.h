@@ -387,6 +387,62 @@ GS_API int gs_export(gs_context *ctx, uint32_t first, uint32_t count, uint32_t f
                      size_t *out_bytes);
 
 /*
+ * Saving a whole scene: several entity ranges as one file, each with its placement baked in.
+ *
+ * gs_export_parts: the rows of parts[0], parts[1], ... in that order (parts may overlap, repeat a range, or be empty) as
+ *   one file of `format`.  Each row is first transformed by its part's matrix; every rule of gs_export then applies
+ *   unchanged to the transformed rows and SH coefficients.  Compressed chunks are 256 rows counted from the file's first
+ *   row, across part boundaries.  out == NULL only sets *out_bytes.  It needs keep-rows, runs behind the pushes and edits
+ *   already queued, does not wait for frames in flight and returns when the bytes are in `out`.
+ *   GS_ERR_INVALID, nothing written: out_bytes NULL, parts NULL, n_parts 0 or above GS_MAX_OBJECTS, a range past N, a
+ *   refused matrix (below), 2^32 rows or more in all, an unknown format, a context without keep-rows, cap below the size
+ *   (*out_bytes is 0 but in the last two cases, where it is set to the size, as gs_export does).  The transformed rows are built in one stream-ordered
+ *   temporary of 32 + 16 sh_vecs B per exported row (sh_vecs = 0, 2, 3, 6 at degrees 0..3), and the PLY formats' body
+ *   behind them, allocated before anything is written: GS_ERR_OOM changes nothing.  A part whose matrix copies
+ *   everything (below) is copied without a kernel.
+ *
+ * The transform.  m: the affine map of the .splat row frame (the frame of the row's x y z; the table holds x, y, -z and
+ *   an entity's local frame is x, -y, -z), column-major.  A = m, L its upper 3x3, t = (m[12], m[13], m[14]).  fp64, one
+ *   rounding per operation, left to right.
+ *   - Refused: a non-finite entry, a bottom row other than (0, 0, 0, 1) exactly, det L == 0 (det L = L00 (L11 L22 -
+ *     L12 L21) - L01 (L10 L22 - L12 L20) + L02 (L10 L21 - L11 L20)), or L not a similarity: s = cbrt(|det L|), set to 1
+ *     when |s - 1| <= 1e-6 (so an unscaled entity keeps its scale bytes), and any entry of L^T L / s^2 - I above 1e-5
+ *     in magnitude refuses it.  Q = L / s may be a mirror (det Q < 0).
+ *   - Centre: p'_i = ((L_i0 x + L_i1 y) + L_i2 z) + t_i, rounded once to f32; a NaN is written 0x7FC00000.
+ *   - Scales: f32(|s| scale_k), a NaN written 0x7FC00000.
+ *   - Rotation bytes (w, x, y, z): Qp = Q when det Q > 0, else -Q; qQ = three.js Quaternion.setFromRotationMatrix(Qp)
+ *     (its four branches, in fp64), normalised as Quaternion.normalize does (times 1 / sqrt(((x x + y y) + z z) + w w)).
+ *     q^ = (bytes - 128) / 128 normalised (sqrt(((w w + x x) + y y) + z z));
+ *     q' = qQ (x) q^ (Hamilton product: R(q') = Qp R(q^)); byte_k = js_store_u8_clamped(q'_k 128 + 128) (round half to
+ *     even, NaN and <= 0 to 0, >= 255 to 255), gs_push_ply's own quantisation.  The zero quaternion (all bytes 128) is
+ *     copied.
+ *   - SH (degree d > 0): y_l(v) is the vector of eval_sh's band-l terms, with their signs, in the renderer's order
+ *     (-C1 y, C1 z, -C1 x, ...), of a direction v of the row frame (the renderer evaluates at (d.x, d.y, -d.z) of table
+ *     coordinates).  R_l is the (2l+1)^2 matrix with y_l(Q^T v) = R_l y_l(v), and each channel's band becomes
+ *     c'_l = R_l^T c_l: c'_i = sum_j R_l^T[i][j] c_j from j = 0, in fp64, rounded once to fp16 (round to nearest even);
+ *     a NaN is stored 0x7FFF as the loaders store it.  R_l is orthogonal, so a band's norm is kept, but a coefficient
+ *     near 65504 may still round to +-inf.  A mirror needs no special case: the parity (-1)^l is in y_l(Q^T v).
+ *   - Copies, so that identity parts are byte-exact: the centre when L == I and t == 0 exactly, the scales when s == 1
+ *     after the snap, the rotation bytes and the SH coefficients when Q == I exactly.  Colour and alpha bytes are always
+ *     copied.
+ *
+ * gs_sh_rotation: the matrices the export applies for Q = q9 (row-major 3x3), degree 1..3: R_1^T, R_2^T, R_3^T up to
+ *   `degree`, each row-major, concatenated in `out` (9, 34 or 83 doubles).  Host only (no context, no device): R_l is
+ *   solved in fp64 from y_l at 2l+1 fixed directions and at those directions taken by Q^T; when q9 is a signed
+ *   permutation (every entry 0 or +-1), entries within 1e-12 of -1, 0 or 1 are set to them, so quarter turns, half turns
+ *   and mirrors about the axes move and negate coefficients exactly.  GS_ERR_INVALID: q9 or out NULL, degree 0 or above
+ *   3, a non-finite entry.
+ */
+typedef struct gs_export_part {
+  uint32_t first, count; /* rows [first, first+count) of the resident table (one entity's range); count 0 allowed */
+  uint32_t pad[2];
+  double m[16];          /* affine transform of the .splat row frame, column-major (m[3], m[7], m[11], m[15] = 0, 0, 0, 1) */
+} gs_export_part;        /* 144 bytes */
+GS_API int gs_export_parts(gs_context *ctx, const gs_export_part *parts, uint32_t n_parts, uint32_t format,
+                           void *out_or_null, size_t cap, size_t *out_bytes);
+GS_API int gs_sh_rotation(const double q9[9], uint32_t degree, double *out);
+
+/*
  * {method:"sort", view, cutout} -> {sortedIndexes} (index.js:449-453, 507-570, 587-596).
  * out_idx (host, capacity gs_num_splats) receives the surviving splat indices back-to-front,
  * bit-identical to the reference's Uint32Array (16-bit bucket order, ties by index; tail zeros
