@@ -140,6 +140,14 @@ static int ensure_slot_scene(gs_context *c, gs_context::Slot &sl) {
   return GS_OK;
 }
 
+// SH contexts: a slot's camera table (device + pinned staging), fixed size, allocated once
+static int ensure_slot_sh(gs_context *c, gs_context::Slot &sl) {
+  if (!sl.sh_cam_dev) GS_CUDA(c, cudaMalloc((void **)&sl.sh_cam_dev, sizeof(float4) * kMaxObjects * kMaxViews));
+  if (!sl.sh_cam_host)
+    GS_CUDA(c, cudaHostAlloc((void **)&sl.sh_cam_host, sizeof(float4) * kMaxObjects * kMaxViews, cudaHostAllocDefault));
+  return GS_OK;
+}
+
 // records and rectangles of views 1.. of views scene frames, each view's sized like the per-splat scratch (rounded up to
 // 4 splats: the projection clears 4 rectangles per store); allocated by the first views frame and grown to the largest
 // view count drawn since (the pipeline is idle)
@@ -1187,6 +1195,10 @@ static void stats_from_counters(gs_context *c, const FrameCounters &h, uint32_t 
   s.max_depth = h.sort.n_valid ? dec_f64(h.sort.max_enc) : -INFINITY;
 }
 
+// kernel launches of a sort (the sort stage of a frame): depth pass, keys and radix passes; precise sorts take a depth pass
+// and four radix passes (scene sorts: five, and no scene keys)
+static uint32_t sort_launches(bool scene, bool f32) { return f32 ? (scene ? 16u : 13u) : (scene ? 11u : 7u); }
+
 // gs_sort and gs_sort_scene*: one sort in slot 0 and buffer set 0 of an idle pipeline, its counters and order read back.
 // scene: the validated table of gs_sort_scene* (nullptr: the one-entity sort of gs_sort, by view and cutout); f32: the
 // precise order of GS_RENDER_SORT_F32, radial: that of GS_RENDER_SORT_RADIAL (scene sorts only; radial implies f32)
@@ -1229,7 +1241,7 @@ static int sort_only(gs_context *c, const float *view, const float *cutout, cons
   GS_CUDA(c, cudaStreamSynchronize(c->stream));
   memset(&c->stats, 0, sizeof(c->stats));
   stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
-  c->stats.kernel_launches = scene ? (f32 ? 16 : 11) : 7;
+  c->stats.kernel_launches = sort_launches(scene != nullptr, f32);
   float ms = 0;
   cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]);
   c->stats.ms_sort = ms;
@@ -1268,10 +1280,10 @@ extern "C" uint32_t gs_owned_tiles(uint32_t width, uint32_t height, uint32_t ran
 static FrameBufs slot_bufs(gs_context *c, const gs_context::Slot &sl) {
   FrameBufs b{c->order[sl.set], c->proj_rec[sl.set], c->rect[sl.set], c->inst_rec[sl.set], c->bin_range[sl.set]};
   b.sh_cam = sl.sh_cam_dev;
-  b.antialias = sl.antialias;
-  if (sl.stereo) {
+  b.antialias = sl.frame.antialias;
+  if (sl.frame.stereo) {
     b.views = true;
-    if (sl.n_views > 1) {
+    if (sl.frame.n_views > 1) {
       b.proj_recx = c->proj_recx[sl.set];
       b.rectx = c->rectx[sl.set];
       b.x_stride = c->stereo_cap;
@@ -1282,10 +1294,10 @@ static FrameBufs slot_bufs(gs_context *c, const gs_context::Slot &sl) {
 }
 
 // per-frame parameters the kernels read: a views frame's views (view v at +v), else the slot's own
-static const FrameParams *slot_fp(const gs_context::Slot &sl) { return sl.stereo ? &sl.stereo_dev->view[0] : sl.fp; }
+static const FrameParams *slot_fp(const gs_context::Slot &sl) { return sl.frame.stereo ? &sl.stereo_dev->view[0] : sl.fp; }
 
 // a scene frame (or pick) of GS_RENDER_SCENE_INTERLEAVE: its scene keys and slab passes are the interleaved instantiations
-static bool interleaved(const gs_context::Slot &sl) { return sl.scene && sl.scene_host->interleave; }
+static bool interleaved(const gs_context::Slot &sl) { return sl.frame.scene && sl.scene_host->interleave; }
 
 // graph key of a frame: anything baked into its captured launches (views frames: also the view shape and the extra views'
 // buffers, which only their bin sort takes as kernel arguments)
@@ -1295,13 +1307,13 @@ static gs_context::GraphKey graph_key(const gs_context *c, const gs_context::Slo
   k.p3 = c->scene_key;
   k.psh = c->sh;
   k.sh_degree = c->sh_degree;
-  k.antialias = sl.antialias ? 1u : 0u;
-  k.sort_mode = (interleaved(sl) ? 1u : 0u) | (sl.f32 ? 2u : 0u) | (sl.radial ? 4u : 0u);
+  k.antialias = sl.frame.antialias ? 1u : 0u;
+  k.sort_mode = (interleaved(sl) ? 1u : 0u) | (sl.frame.f32 ? 2u : 0u) | (sl.frame.radial ? 4u : 0u);
   k.pz = c->zdepth[0];
-  if (sl.stereo) {
-    k.n_views = sl.n_views;
-    for (uint32_t v = 0; v < sl.n_views; ++v) k.view_size[v] = sl.view[v].width | sl.view[v].height << 16;
-    k.px = sl.n_views > 1 ? c->proj_recx[0] : nullptr;
+  if (sl.frame.stereo) {
+    k.n_views = sl.frame.n_views;
+    for (uint32_t v = 0; v < sl.frame.n_views; ++v) k.view_size[v] = sl.frame.view[v].width | sl.frame.view[v].height << 16;
+    k.px = sl.frame.n_views > 1 ? c->proj_recx[0] : nullptr;
   }
   return k;
 }
@@ -1322,31 +1334,31 @@ static cudaError_t enqueue_sort_stage(gs_context *c, gs_context::Slot &sl, bool 
   cudaError_t e;
   if ((e = cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, m))) return e;
   if ((e = cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), m))) return e;
-  if (sl.scene && (e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, m))) return e;
+  if (sl.frame.scene && (e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, m))) return e;
   if ((e = record(sl.ev[0], m, external_events))) return e;
-  if (sl.scene) {
-    launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, sl.radial, m);
+  if (sl.frame.scene) {
+    launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, sl.frame.radial, m);
   } else if (reuse) {
     if ((e = cudaMemcpyAsync(sl.ctr, c->sort_hdr, sizeof(SortHeader), cudaMemcpyDeviceToDevice, m))) return e;
   } else {
-    launch_depth_cull(c, sl.fp, sl.ctr, sl.radial, m);
+    launch_depth_cull(c, sl.fp, sl.ctr, sl.frame.radial, m);
   }
   // fork: the vertex-shader kernel only needs the cull result, so it runs beside the depth radix passes
   if ((e = cudaEventRecord(c->ev_fork[0], m))) return e;
   if ((e = cudaStreamWaitEvent(x, c->ev_fork[0], 0))) return e;
   if ((e = record(sl.evp[0], x, external_events))) return e;
-  if (sl.stereo) launch_project_stereo(c, sl.stereo_dev, sl.scene_dev, sl.ctr, b, x);
-  else if (sl.scene) launch_project_scene(c, sl.fp, sl.scene_dev, sl.ctr, b, x);
+  if (sl.frame.stereo) launch_project_stereo(c, sl.stereo_dev, sl.scene_dev, sl.ctr, b, x);
+  else if (sl.frame.scene) launch_project_scene(c, sl.fp, sl.scene_dev, sl.ctr, b, x);
   else launch_project(c, sl.fp, sl.ctr, b, x);
   if ((e = record(sl.evp[1], x, external_events))) return e;
   if ((e = cudaEventRecord(c->ev_join[0], x))) return e;
-  if (sl.scene && sl.f32) {
+  if (sl.frame.scene && sl.frame.f32) {
     launch_sort_f32(c, sl.fp, sl.ctr, sl.scene_dev, interleaved(sl), b, m);
-  } else if (sl.scene) {
+  } else if (sl.frame.scene) {
     launch_scene_keys(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, interleaved(sl), m);
     launch_scene_radix(c, sl.fp, sl.ctr, b, m);
   } else if (!reuse) {
-    if (sl.f32) launch_sort_f32(c, sl.fp, sl.ctr, nullptr, false, b, m);
+    if (sl.frame.f32) launch_sort_f32(c, sl.fp, sl.ctr, nullptr, false, b, m);
     else launch_depth_radix(c, sl.fp, sl.ctr, b, m);
     if ((e = cudaMemcpyAsync(c->sort_hdr, sl.ctr, sizeof(SortHeader), cudaMemcpyDeviceToDevice, m))) return e;
   }
@@ -1396,7 +1408,7 @@ static cudaError_t enqueue_raster_stage(gs_context *c, gs_context::Slot &sl, uin
   cudaError_t e;
   if (sl.peer) launch_peer_acquire(c, sl.fp, sl.ctr, c->rstream);
   if ((e = record(sl.ev_r0, c->rstream, external_events))) return e;
-  if (sl.stereo) launch_raster_stereo(c, slot_fp(sl), n_tiles, slot_bufs(c, sl), sl.raster_flags, c->rstream);
+  if (sl.frame.stereo) launch_raster_stereo(c, slot_fp(sl), n_tiles, slot_bufs(c, sl), sl.raster_flags, c->rstream);
   else launch_raster(c, sl.fp, n_tiles, slot_bufs(c, sl), sl.raster_flags, c->rstream);
   if ((e = record(sl.ev[4], c->rstream, external_events))) return e;
   if (sl.peer) launch_peer_signal_wait(c, sl.fp, sl.ctr, c->rstream);
@@ -1434,21 +1446,22 @@ static int run_graph(gs_context *c, cudaGraphExec_t &ge, cudaStream_t stream, F 
 // stage is kSortStage, its slab loop kRasterStage.  Plain and scene frames differ in their sort stage only.
 enum FrameStage { kSortStage, kBinStage, kRasterStage };
 static int slab_graph_base(const gs_context::Slot &sl) {
-  return sl.stereo ? kGraphSlabViews : (sl.scene ? kGraphSlabScene : kGraphSlabPlain);
+  return sl.frame.stereo ? kGraphSlabViews : (sl.frame.scene ? kGraphSlabScene : kGraphSlabPlain);
 }
 static cudaGraphExec_t &stage_graph(gs_context::Slot &sl, FrameStage stage, bool reuse) {
   int id;
-  if (sl.pick) {
-    id = stage == kSortStage ? (sl.scene ? kGraphPickSortScene : kGraphPickSortPlain)
+  if (sl.frame.pick) {
+    id = stage == kSortStage ? (sl.frame.scene ? kGraphPickSortScene : kGraphPickSortPlain)
                              : (stage == kBinStage ? kGraphPickBin : kGraphPick);
-  } else if (sl.slab) {
+  } else if (sl.frame.slab) {
     id = slab_graph_base(sl);
     // loop: plain, depth-tested, fused peer exchange, depth-tested with depth write (views: no peer id, depth write at 3)
-    if (stage != kSortStage) id += sl.depth_write ? (sl.stereo ? 3 : 4) : (sl.peer ? 3 : ((sl.raster_flags & 2u) ? 2 : 1));
-  } else if (sl.stereo) {
+    if (stage != kSortStage)
+      id += sl.frame.depth_write ? (sl.frame.stereo ? 3 : 4) : (sl.peer ? 3 : ((sl.raster_flags & 2u) ? 2 : 1));
+  } else if (sl.frame.stereo) {
     id = kGraphViewsSort + (int)stage;
   } else if (stage == kSortStage) {
-    id = sl.scene ? kGraphSortScene : (reuse ? kGraphSortReuse : kGraphSort);
+    id = sl.frame.scene ? kGraphSortScene : (reuse ? kGraphSortReuse : kGraphSort);
   } else {
     id = stage == kBinStage ? kGraphBin : (sl.peer ? kGraphRasterPeer : kGraphRaster);
   }
@@ -1459,7 +1472,7 @@ static cudaGraphExec_t &stage_graph(gs_context::Slot &sl, FrameStage stage, bool
 // every view's), so neither kind re-captures the other's
 static void sync_graph_key(gs_context *c, const gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
   const gs_context::GraphKey k = graph_key(c, sl, n_tiles, n_bins);
-  const GraphDomain domain = sl.pick ? kGraphsPick : (sl.stereo ? kGraphsViews : kGraphsMono);
+  const GraphDomain domain = sl.frame.pick ? kGraphsPick : (sl.frame.stereo ? kGraphsViews : kGraphsMono);
   if (memcmp(&k, &c->gkey[domain], sizeof(k)) != 0) {
     drop_graphs(c, domain);
     c->gkey[domain] = k;
@@ -1470,7 +1483,7 @@ static void sync_graph_key(gs_context *c, const gs_context::Slot &sl, uint32_t n
 // (those never capture a graph, so they leave every cached graph and graph key as they were)
 template <class F>
 static int run_stage(gs_context *c, const gs_context::Slot &sl, cudaGraphExec_t &ge, cudaStream_t stream, F enqueue) {
-  if (sl.cameras) {
+  if (sl.frame.group != ~0ull) {
     GS_CUDA(c, enqueue(false));
     return GS_OK;
   }
@@ -1481,7 +1494,7 @@ static int run_stage(gs_context *c, const gs_context::Slot &sl, cudaGraphExec_t 
 // sorted / projected (stream A).  A and B are high priority: their short latency-bound kernels slot in as the
 // long issue-bound raster's CTAs retire.  Stage hand-offs are events; buffers between stages are double-buffered.
 static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_t n_tiles, uint32_t n_bins) {
-  if (!sl.cameras) sync_graph_key(c, sl, n_tiles, n_bins);
+  if (sl.frame.group == ~0ull) sync_graph_key(c, sl, n_tiles, n_bins);
   const int set = sl.set;
   // A: order/proj_rec/rect[set] must no longer be read by the binning stage that used them last
   if (c->sort_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->sort_set_free[set], 0));
@@ -1492,13 +1505,13 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
   GS_CUDA(c, cudaStreamWaitEvent(c->bstream, sl.ev_sorted, 0));
   if (c->bin_set_free[set]) GS_CUDA(c, cudaStreamWaitEvent(c->bstream, c->bin_set_free[set], 0));
   if ((rc = run_stage(c, sl, stage_graph(sl, kBinStage, reuse), c->bstream, [&](bool ext) {
-         return sl.pick ? enqueue_pick_bin_stage(c, sl, n_bins, ext) : enqueue_bin_stage(c, sl, n_bins, ext);
+         return sl.frame.pick ? enqueue_pick_bin_stage(c, sl, n_bins, ext) : enqueue_bin_stage(c, sl, n_bins, ext);
        }))) return rc;
   GS_CUDA(c, cudaEventRecord(sl.ev_binned, c->bstream));
   c->sort_set_free[set] = sl.ev_binned;
   // C
   GS_CUDA(c, cudaStreamWaitEvent(c->rstream, sl.ev_binned, 0));
-  if (sl.pick) {
+  if (sl.frame.pick) {
     if ((rc = run_graph(c, stage_graph(sl, kRasterStage, reuse), c->rstream,
                         [&](bool ext) { return enqueue_pick_stage(c, sl, ext); }))) return rc;
   } else if (sl.raster_flags == c->raster_base_flags) {
@@ -1509,9 +1522,7 @@ static int launch_frame(gs_context *c, gs_context::Slot &sl, bool reuse, uint32_
     // cached graph (so a frame of one blend mode never replays a raster graph captured for the other)
     GS_CUDA(c, enqueue_raster_stage(c, sl, n_tiles, false));
   }
-  // precise frames: a depth pass and four radix passes (scene frames: five, and no scene keys)
-  const uint32_t sort_launches = sl.f32 ? (sl.scene ? 16u : 13u) : (sl.scene ? 11u : 7u);
-  sl.launches = (reuse ? 0u : sort_launches) + 1u + (n_bins <= 256u ? 5u : 9u) + 1u;
+  sl.launches = (reuse ? 0u : sort_launches(sl.frame.scene, sl.frame.f32)) + 1u + (n_bins <= 256u ? 5u : 9u) + 1u;
   return GS_OK;
 }
 
@@ -1523,15 +1534,15 @@ static uint64_t slab_cumulative(uint32_t first, int k) { return (uint64_t)first 
 // A scene frame takes the per-entity depth pass and 24-bit keys (the scene table was copied to sl.scene_dev ahead of it).
 static cudaError_t enqueue_slab_keys_stage(gs_context *c, gs_context::Slot &sl, bool external_events) {
   cudaStream_t st = c->stream;
-  const SceneTable *scene = sl.scene ? sl.scene_dev : nullptr;
+  const SceneTable *scene = sl.frame.scene ? sl.scene_dev : nullptr;
   cudaError_t e;
   if ((e = cudaMemcpyAsync(sl.fp, sl.fp_host, sizeof(FrameParams), cudaMemcpyHostToDevice, st))) return e;
   if ((e = cudaMemsetAsync(sl.ctr, 0, sizeof(FrameCounters), st))) return e;
   if (scene && (e = cudaMemsetAsync(sl.octr, 0, sizeof(ObjCounters) * kMaxObjects, st))) return e;
   if ((e = record(sl.ev[0], st, external_events))) return e;
-  if (scene) launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, sl.radial, st);
-  else launch_depth_cull(c, sl.fp, sl.ctr, sl.radial, st);
-  launch_keys(c, sl.fp, sl.ctr, scene, interleaved(sl), sl.f32, sl.octr, sl.set, st);
+  if (scene) launch_depth_cull_scene(c, sl.fp, sl.scene_dev, sl.octr, sl.ctr, sl.frame.radial, st);
+  else launch_depth_cull(c, sl.fp, sl.ctr, sl.frame.radial, st);
+  launch_keys(c, sl.fp, sl.ctr, scene, interleaved(sl), sl.frame.f32, sl.octr, sl.set, st);
   launch_slab_plan(c, sl.fp, sl.ctr, sl.set, c->slab_first, sl.n_slabs, st);
   launch_compact_offsets(c, sl.fp, scene, interleaved(sl), sl.set, sl.n_slabs, st);  // one pass over the keys for every slab's compaction offsets
   if ((e = record(sl.ev[1], st, external_events))) return e;
@@ -1544,29 +1555,29 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
                                            bool external_events) {
   cudaStream_t st = c->rstream;
   const FrameBufs b = slot_bufs(c, sl);
-  const SceneTable *scene = sl.scene ? sl.scene_dev : nullptr;
-  const ViewTable *stereo = sl.stereo ? sl.stereo_dev : nullptr;
+  const SceneTable *scene = sl.frame.scene ? sl.scene_dev : nullptr;
+  const ViewTable *stereo = sl.frame.stereo ? sl.stereo_dev : nullptr;
   const FrameParams *fp = slot_fp(sl);  // the frame's (a stereo frame's pair) for the projection, binning and raster
   cudaError_t e;
-  launch_slab_init(c, fp, sl.ctr, sl.stereo, st);
+  launch_slab_init(c, fp, sl.ctr, sl.frame.stereo, st);
   if ((e = record(sl.ev[2], st, external_events))) return e;
   for (int s = 0; s < sl.n_slabs; ++s) {
     launch_slab_begin(c, sl.fp, sl.ctr, scene, interleaved(sl), sl.set, s, st);  // entry count (0 once every bin is closed) + compaction
-    if (sl.f32) launch_slab_sort_f32(c, sl.ctr, scene, interleaved(sl), c->zdepth[sl.set], b, st);  // precise order of the slab
+    if (sl.frame.f32) launch_slab_sort_f32(c, sl.ctr, scene, interleaved(sl), c->zdepth[sl.set], b, st);  // precise order
     else launch_slab_sort(c, sl.fp, sl.ctr, scene, interleaved(sl), b, st);           // draw order of the slab
     launch_project_entries(c, sl.fp, sl.ctr, scene, stereo, b, st);  // vertex shader for the slab's entries (of each view)
     if ((e = cudaMemsetAsync(b.bin_range, 0, sizeof(uint2) * (size_t)n_bins, st))) return e;
     launch_emit(c, fp, sl.ctr, b, c->bin_open, st);
     launch_tile_radix(c, sl.ctr, b, n_bins, st);
     if ((e = record(sl.slab_ev[s][0], st, external_events))) return e;
-    launch_raster_slab(c, fp, sl.ctr, n_tiles, b, (sl.raster_flags & 2u) != 0, sl.stereo, sl.depth_write, st);
+    launch_raster_slab(c, fp, sl.ctr, n_tiles, b, (sl.raster_flags & 2u) != 0, sl.frame.stereo, sl.frame.depth_write, st);
     if ((e = record(sl.slab_ev[s][1], st, external_events))) return e;
   }
   launch_slab_end(c, sl.ctr, st);
   if ((e = record(sl.ev[3], st, external_events))) return e;
   if (sl.peer) launch_peer_acquire(c, sl.fp, sl.ctr, st);
   if ((e = record(sl.ev_r0, st, external_events))) return e;
-  launch_resolve(c, fp, n_tiles, sl.stereo, sl.depth_write, st);
+  launch_resolve(c, fp, n_tiles, sl.frame.stereo, sl.frame.depth_write, st);
   if ((e = record(sl.ev[4], st, external_events))) return e;
   if (sl.peer) launch_peer_signal_wait(c, sl.fp, sl.ctr, st);
   return cudaGetLastError();
@@ -1577,12 +1588,13 @@ static cudaError_t enqueue_slab_loop_stage(gs_context *c, gs_context::Slot &sl, 
 // A views frame passes n_tiles and n_bins of every view and keeps its graphs under the views key, as on the one-pass path.
 static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_tiles, uint32_t n_bins) {
   sync_graph_key(c, sl, n_tiles, n_bins);
-  const int set = sl.set, kind = sl.stereo ? 2 : (sl.scene ? 1 : 0);  // plain, scene and views frames keep their own graphs
+  // plain, scene and views frames keep their own graphs
+  const int set = sl.set, kind = sl.frame.stereo ? 2 : (sl.frame.scene ? 1 : 0);
   // slabs of slab_first, 2x, 4x ... entries: enough of them to cover every splat the sort considers
   int n_slabs = 1;
-  while (n_slabs < kMaxSlabs && slab_cumulative(c->slab_first, n_slabs) < sl.n_sortable) ++n_slabs;
+  while (n_slabs < kMaxSlabs && slab_cumulative(c->slab_first, n_slabs) < sl.frame.n_sortable) ++n_slabs;
   if (n_slabs != sl.graph_slabs[set][kind]) {  // the captured stages bake the slab count
-    const int base = slab_graph_base(sl), n_ids = sl.stereo ? 4 : 5;  // this set's and kind's keys graph and loop graphs
+    const int base = slab_graph_base(sl), n_ids = sl.frame.stereo ? 4 : 5;  // this set's and kind's keys graph and loop graphs
     for (int id = base; id < base + n_ids; ++id) kill_graph(sl.graph[set][id]);
     sl.graph_slabs[set][kind] = n_slabs;
   }
@@ -1607,7 +1619,7 @@ static int launch_frame_slabs(gs_context *c, gs_context::Slot &sl, uint32_t n_ti
   c->sort_set_free[set] = sl.ev_binned;
   // scene frames: three radix passes per slab instead of two (views frames: the scene frame's launches, every view's bins);
   // precise frames: four (scene frames: five)
-  const uint32_t extra = sl.f32 ? (sl.scene ? 9u : 6u) : (sl.scene ? 3u : 0u);
+  const uint32_t extra = sl.frame.f32 ? (sl.frame.scene ? 9u : 6u) : (sl.frame.scene ? 3u : 0u);
   sl.launches = 6u + 1u + (uint32_t)n_slabs * ((n_bins <= 256u ? 16u : 20u) + extra) + 2u;
   return GS_OK;
 }
@@ -1619,24 +1631,26 @@ static int enqueue_readback(gs_context *c, gs_context::Slot &sl) {
   c->bin_set_free[sl.set] = sl.ev_done;
   GS_CUDA(c, cudaStreamWaitEvent(c->copy_stream, sl.ev_done, 0));
   GS_CUDA(c, cudaMemcpyAsync(sl.ctr_host, sl.ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, c->copy_stream));
-  if (sl.pick)
+  if (sl.frame.pick)
     GS_CUDA(c, cudaMemcpyAsync(c->pick_out_host, c->pick_out, sizeof(gs_pick) * c->pick_in_host->n, cudaMemcpyDeviceToHost,
                                c->copy_stream));
   if (sl.host_out)
-    for (uint32_t e = 0; e < sl.n_views; ++e) {
-      if (sl.target) {  // a host gs_target: 2-D copies into the rectangles only
-        const gs_render_params &vp = sl.view[e];
+    for (uint32_t e = 0; e < sl.frame.n_views; ++e) {
+      if (sl.frame.target) {  // a host gs_target: 2-D copies into the rectangles only
+        const gs_render_params &vp = sl.frame.view[e];
         const size_t px_bytes = vp.out_format == GS_FORMAT_RGBA8 ? 4 : 16, row = px_bytes * vp.width;
-        char *dst = (char *)sl.tcolor + ((size_t)sl.torg[e][1] * sl.tpitch + sl.torg[e][0]) * px_bytes;
-        GS_CUDA(c, cudaMemcpy2DAsync(dst, px_bytes * sl.tpitch, sl.frame_src[e], row, row, vp.height,
+        const uint32_t ox = sl.frame.torg[e][0], oy = sl.frame.torg[e][1];
+        char *dst = (char *)sl.frame.tcolor + ((size_t)oy * sl.frame.tpitch + ox) * px_bytes;
+        GS_CUDA(c, cudaMemcpy2DAsync(dst, px_bytes * sl.frame.tpitch, sl.frame_src[e], row, row, vp.height,
                                      cudaMemcpyDeviceToHost, c->copy_stream));
-        if (sl.depth_write) {  // and the depth the frame wrote into its staged rectangle
-          float *ddst = const_cast<float *>(sl.tdepth) + (size_t)sl.torg[e][1] * sl.tpitch + sl.torg[e][0];
-          GS_CUDA(c, cudaMemcpy2DAsync(ddst, sizeof(float) * sl.tpitch, sl.depth_dev[e], sizeof(float) * vp.width,
+        if (sl.frame.depth_write) {  // and the depth the frame wrote into its staged rectangle
+          float *ddst = const_cast<float *>(sl.frame.tdepth) + (size_t)oy * sl.frame.tpitch + ox;
+          GS_CUDA(c, cudaMemcpy2DAsync(ddst, sizeof(float) * sl.frame.tpitch, sl.depth_dev[e], sizeof(float) * vp.width,
                                        sizeof(float) * vp.width, vp.height, cudaMemcpyDeviceToHost, c->copy_stream));
         }
       } else {
-        GS_CUDA(c, cudaMemcpyAsync(sl.out_user[e], sl.frame_src[e], sl.out_bytes[e], cudaMemcpyDeviceToHost, c->copy_stream));
+        GS_CUDA(c, cudaMemcpyAsync(sl.frame.out_user[e], sl.frame_src[e], sl.out_bytes[e], cudaMemcpyDeviceToHost,
+                                   c->copy_stream));
       }
     }
   if (sl.raster_flags & 4u)
@@ -1700,7 +1714,7 @@ static void fill_render_consts(gs_context *c, const gs_render_params *p, RenderC
 // device frame that the readback copies to the caller's host buffer
 static int stage_out(gs_context *c, gs_context::Slot &sl, int e, FrameParams &fp) {
   if (!sl.host_out) {
-    fp.out = sl.out_user[e];
+    fp.out = sl.frame.out_user[e];
     sl.frame_src[e] = nullptr;
     return GS_OK;
   }
@@ -1717,36 +1731,38 @@ static int stage_inputs(gs_context *c, gs_context::Slot &sl, int e, const gs_ren
   int rcode;
   const size_t px_bytes = p->out_format == GS_FORMAT_RGBA8 ? 4 : 16;
   const size_t pixels = (size_t)p->width * p->height;
-  if (sl.target) {
+  if (sl.frame.target) {
     // colour and depth of view e's rectangle of a gs_target.  A run that overflows stores nothing (fp.overflow), and its
     // re-run reuses the staged rectangles: the host buffers already hold the overflowed run's read-back by then
     fp.overflow = &sl.ctr->overflow;
-    const uint32_t ox = sl.torg[e][0], oy = sl.torg[e][1];
-    if (sl.target_device) {  // in place: the buffers at the rectangle's origin, rows of the target's pitch
-      const size_t origin = (size_t)oy * sl.tpitch + ox;
-      fp.out = (char *)sl.tcolor + origin * px_bytes;
+    const uint32_t ox = sl.frame.torg[e][0], oy = sl.frame.torg[e][1];
+    if (sl.frame.target_device) {  // in place: the buffers at the rectangle's origin, rows of the target's pitch
+      const size_t origin = (size_t)oy * sl.frame.tpitch + ox;
+      fp.out = (char *)sl.frame.tcolor + origin * px_bytes;
       fp.color_in = fp.out;
-      fp.depth_in = sl.tdepth ? sl.tdepth + origin : nullptr;
+      fp.depth_in = sl.frame.tdepth ? sl.frame.tdepth + origin : nullptr;
       // GS_TARGET_DEPTH_WRITE: the depth is written where it is read (gs_target::depth is const for the frames that only
       // test against it)
-      if (sl.depth_write) fp.depth_out = const_cast<float *>(sl.tdepth) + origin;
-      fp.rc.pitch = sl.tpitch;
+      if (sl.frame.depth_write) fp.depth_out = const_cast<float *>(sl.frame.tdepth) + origin;
+      fp.rc.pitch = sl.frame.tpitch;
       return GS_OK;
     }
     const size_t row = px_bytes * p->width;
     if ((rcode = ensure_dev(c, sl.color_dev[e], sl.color_bytes[e], px_bytes * pixels))) return rcode;
-    if (sl.restage)
-      GS_CUDA(c, cudaMemcpy2DAsync(sl.color_dev[e], row, (const char *)sl.tcolor + ((size_t)oy * sl.tpitch + ox) * px_bytes,
-                                   px_bytes * sl.tpitch, row, p->height, cudaMemcpyHostToDevice, c->stream));
+    if (sl.frame.restage)
+      GS_CUDA(c, cudaMemcpy2DAsync(sl.color_dev[e], row,
+                                   (const char *)sl.frame.tcolor + ((size_t)oy * sl.frame.tpitch + ox) * px_bytes,
+                                   px_bytes * sl.frame.tpitch, row, p->height, cudaMemcpyHostToDevice, c->stream));
     fp.color_in = sl.color_dev[e];
-    if (sl.tdepth) {
+    if (sl.frame.tdepth) {
       if ((rcode = ensure_dev(c, sl.depth_dev[e], sl.depth_bytes[e], sizeof(float) * pixels))) return rcode;
-      if (sl.restage)
-        GS_CUDA(c, cudaMemcpy2DAsync(sl.depth_dev[e], sizeof(float) * p->width, sl.tdepth + (size_t)oy * sl.tpitch + ox,
-                                     sizeof(float) * sl.tpitch, sizeof(float) * p->width, p->height, cudaMemcpyHostToDevice,
-                                     c->stream));
+      if (sl.frame.restage)
+        GS_CUDA(c, cudaMemcpy2DAsync(sl.depth_dev[e], sizeof(float) * p->width,
+                                     sl.frame.tdepth + (size_t)oy * sl.frame.tpitch + ox, sizeof(float) * sl.frame.tpitch,
+                                     sizeof(float) * p->width, p->height, cudaMemcpyHostToDevice, c->stream));
       fp.depth_in = sl.depth_dev[e];
-      if (sl.depth_write) fp.depth_out = (float *)sl.depth_dev[e];  // written in the staging copy, read back with the colour
+      // written in the staging copy, read back with the colour
+      if (sl.frame.depth_write) fp.depth_out = (float *)sl.depth_dev[e];
     }
     return GS_OK;
   }
@@ -1759,12 +1775,13 @@ static int stage_inputs(gs_context *c, gs_context::Slot &sl, int e, const gs_ren
       fp.depth_in = sl.depth_dev[e];
     }
   }
-  if (sl.color_in[e]) {
-    if (sl.color_device) {
-      fp.color_in = sl.color_in[e];
+  if (sl.frame.color_in[e]) {
+    if (sl.frame.color_device) {
+      fp.color_in = sl.frame.color_in[e];
     } else {  // host colour target: staged like a host depth_in
       if ((rcode = ensure_dev(c, sl.color_dev[e], sl.color_bytes[e], px_bytes * pixels))) return rcode;
-      GS_CUDA(c, cudaMemcpyAsync(sl.color_dev[e], sl.color_in[e], px_bytes * pixels, cudaMemcpyHostToDevice, c->stream));
+      GS_CUDA(c, cudaMemcpyAsync(sl.color_dev[e], sl.frame.color_in[e], px_bytes * pixels, cudaMemcpyHostToDevice,
+                                 c->stream));
       fp.color_in = sl.color_dev[e];
     }
   }
@@ -1772,11 +1789,11 @@ static int stage_inputs(gs_context *c, gs_context::Slot &sl, int e, const gs_ren
 }
 
 static int submit(gs_context *c, gs_context::Slot &sl) {
-  const gs_render_params *p = &sl.params;
+  const gs_render_params *p = &sl.frame.view[0];
   FrameParams &fp = *sl.fp_host;
   RenderConsts &rc = fp.rc;
   memset(&fp, 0, sizeof(fp));
-  fp.n_splats = sl.n_splats;  // what was resident when the frame was submitted; later pushes append behind it
+  fp.n_splats = sl.frame.n_splats;  // what was resident when the frame was submitted; later pushes append behind it
   if (c->pushed) GS_CUDA(c, cudaStreamWaitEvent(c->stream, c->push_done, 0));
   fill_render_consts(c, p, rc);
   const float view[4] = {p->modelview[2], p->modelview[6], p->modelview[10], p->modelview[14]};  // index.js:442
@@ -1787,9 +1804,9 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   size_t out_pixels = (size_t)p->width * p->height;
   if (rc.out_tiled) out_pixels = (size_t)gs_owned_tiles(p->width, p->height, c->shard_rank, c->shard_world) * 256;
   sl.out_bytes[0] = out_pixels * px_bytes;
-  sl.host_out = sl.target ? !sl.target_device : !(p->flags & GS_RENDER_OUT_DEVICE);
+  sl.host_out = sl.frame.target ? !sl.frame.target_device : !(p->flags & GS_RENDER_OUT_DEVICE);
   sl.peer = (p->flags & GS_RENDER_OUT_PEER) != 0;
-  if (sl.pick) {  // no frame: the results go to pick_out (a re-run after an overflow may have grown pick_pay's demand)
+  if (sl.frame.pick) {  // no frame: the results go to pick_out (a re-run after an overflow may have grown pick_pay's demand)
     sl.host_out = false;
     if ((rcode = ensure_pick_bufs(c))) return rcode;
   } else if (sl.peer) {
@@ -1821,27 +1838,27 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   if ((rcode = stage_inputs(c, sl, 0, p, fp))) return rcode;
   // raster instantiation: pixel loop (two pixels per lane by default), depth test, statistics; GS_RENDER_BLEND_UNORM8
   // frames always take the two-pixel loop of that mode (bit 3), whatever GS_RASTER says
-  const bool depth = p->depth_in || (sl.target && sl.tdepth);  // a target's depth is that of every view
+  const bool depth = p->depth_in || (sl.frame.target && sl.frame.tdepth);  // a target's depth is that of every view
   const bool blend8 = (p->flags & GS_RENDER_BLEND_UNORM8) != 0;
   sl.raster_flags = (blend8 ? 9u : c->raster_base_flags) | (depth ? 2u : 0u) | ((p->flags & GS_RENDER_STATS) ? 4u : 0u) |
-                    (sl.depth_write ? 16u : 0u);
+                    (sl.frame.depth_write ? 16u : 0u);
   // a views frame bins every view (ids bin_base[v] + bin) and rasters every view's tiles in one grid, on either path
   uint32_t n_tiles_all = rc.n_tiles, n_bins_all = rc.n_bins;
-  if (sl.stereo) {
+  if (sl.frame.stereo) {
     // the view frames the views kernels read: view 0 as above, the others from their own parameters (same flags)
     ViewTable &vt = *sl.stereo_host;
-    vt.n_views = sl.n_views;
+    vt.n_views = sl.frame.n_views;
     vt.view[0] = fp;
     n_tiles_all = n_bins_all = 0;
     for (uint32_t v = 0; v < (uint32_t)kMaxViews; ++v) {
-      vt.tile_base[v] = v < sl.n_views ? n_tiles_all : 0xFFFFFFFFu;
-      vt.bin_base[v] = v < sl.n_views ? n_bins_all : 0xFFFFFFFFu;
-      if (v >= sl.n_views) continue;
+      vt.tile_base[v] = v < sl.frame.n_views ? n_tiles_all : 0xFFFFFFFFu;
+      vt.bin_base[v] = v < sl.frame.n_views ? n_bins_all : 0xFFFFFFFFu;
+      if (v >= sl.frame.n_views) continue;
       FrameParams &fv = vt.view[v];
       if (v > 0) {
-        const gs_render_params &pv = sl.view[v];
+        const gs_render_params &pv = sl.frame.view[v];
         memset(&fv, 0, sizeof(fv));
-        fv.n_splats = sl.n_splats;
+        fv.n_splats = sl.frame.n_splats;
         fill_render_consts(c, &pv, fv.rc);
         sl.out_bytes[v] = (size_t)pv.width * pv.height * (pv.out_format == GS_FORMAT_RGBA8 ? 4 : 16);
         if ((rcode = stage_out(c, sl, (int)v, fv)) || (rcode = stage_inputs(c, sl, (int)v, &pv, fv))) return rcode;
@@ -1854,22 +1871,23 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   }
   // the scene table goes ahead of the sort stage on its stream (only the entities in use are copied; a pick on the plain
   // path also maps its hits through it)
-  if (sl.scene || sl.pick) GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, sl.scene_bytes, cudaMemcpyHostToDevice, c->stream));
+  if (sl.frame.scene || sl.frame.pick)
+    GS_CUDA(c, cudaMemcpyAsync(sl.scene_dev, sl.scene_host, sl.scene_bytes, cudaMemcpyHostToDevice, c->stream));
   if (c->sh_degree) {
     // SH contexts: the camera position of every modelview the projection uses, entity k's view v at k * kMaxViews + v
-    const uint32_t n_ent = sl.scene ? sl.scene_host->n : 1u;
+    const uint32_t n_ent = sl.frame.scene ? sl.scene_host->n : 1u;
     for (uint32_t k = 0; k < n_ent; ++k)
-      for (uint32_t v = 0; v < sl.n_views; ++v)
-        sh_camera(sl.stereo ? sl.stereo_host->mv[k][v] : (sl.scene ? sl.scene_host->obj[k].mv : p->modelview),
+      for (uint32_t v = 0; v < sl.frame.n_views; ++v)
+        sh_camera(sl.frame.stereo ? sl.stereo_host->mv[k][v] : (sl.frame.scene ? sl.scene_host->obj[k].mv : p->modelview),
                   sl.sh_cam_host[k * kMaxViews + v]);
     GS_CUDA(c, cudaMemcpyAsync(sl.sh_cam_dev, sl.sh_cam_host, sizeof(float4) * kMaxViews * std::max(n_ent, 1u),
                                cudaMemcpyHostToDevice, c->stream));
   }
-  const bool reuse = !sl.scene && (p->flags & GS_RENDER_REUSE_SORT) && c->have_order;
+  const bool reuse = !sl.frame.scene && (p->flags & GS_RENDER_REUSE_SORT) && c->have_order;
   // a frame normally takes the buffer set the previous frame did not; a frame that reuses the last sort must read
   // that sort's set, so it runs in it
   sl.set = reuse ? c->last_set : (c->last_set ^ 1);
-  if (sl.slab) {
+  if (sl.frame.slab) {
     if ((rcode = launch_frame_slabs(c, sl, n_tiles_all, n_bins_all))) return rcode;
   } else {
     if ((rcode = launch_frame(c, sl, reuse, n_tiles_all, n_bins_all))) return rcode;
@@ -1879,7 +1897,7 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
   sl.pending = true;
   // a slab frame leaves no complete draw order behind (GS_RENDER_REUSE_SORT then sorts again), nor does a scene frame or a
   // pick
-  c->have_order = !sl.slab && !sl.scene && !sl.pick;
+  c->have_order = !sl.frame.slab && !sl.frame.scene && !sl.frame.pick;
   return GS_OK;
 }
 
@@ -1887,13 +1905,13 @@ static int submit(gs_context *c, gs_context::Slot &sl) {
 // frame buffer into the rectangles, so the colour staged at submission is copied back.  (A device target is drawn in
 // place, and an overflowed run leaves it untouched.)
 static int restore_host_target(gs_context *c, gs_context::Slot &sl) {
-  if (!sl.target || sl.target_device) return GS_OK;
-  for (uint32_t e = 0; e < sl.n_views; ++e) {
-    const gs_render_params &vp = sl.view[e];
+  if (!sl.frame.target || sl.frame.target_device) return GS_OK;
+  for (uint32_t e = 0; e < sl.frame.n_views; ++e) {
+    const gs_render_params &vp = sl.frame.view[e];
     const size_t px_bytes = vp.out_format == GS_FORMAT_RGBA8 ? 4 : 16, row = px_bytes * vp.width;
-    char *dst = (char *)sl.tcolor + ((size_t)sl.torg[e][1] * sl.tpitch + sl.torg[e][0]) * px_bytes;
-    GS_CUDA(c, cudaMemcpy2DAsync(dst, px_bytes * sl.tpitch, sl.color_dev[e], row, row, vp.height, cudaMemcpyDeviceToHost,
-                                 c->copy_stream));
+    char *dst = (char *)sl.frame.tcolor + ((size_t)sl.frame.torg[e][1] * sl.frame.tpitch + sl.frame.torg[e][0]) * px_bytes;
+    GS_CUDA(c, cudaMemcpy2DAsync(dst, px_bytes * sl.frame.tpitch, sl.color_dev[e], row, row, vp.height,
+                                 cudaMemcpyDeviceToHost, c->copy_stream));
   }
   GS_CUDA(c, cudaStreamSynchronize(c->copy_stream));
   return GS_OK;
@@ -1902,10 +1920,10 @@ static int restore_host_target(gs_context *c, gs_context::Slot &sl) {
 // a camera's pass of a cameras frame has completed (c->stats holds its statistics): add them to the frame's sums, and once
 // every camera has been added, make the sums the statistics of the frame
 static void add_camera_stats(gs_context *c, const gs_context::Slot &sl) {
-  gs_context::CameraSum &cs = c->cam_sum[sl.group % gs_context::kSlots];
+  gs_context::CameraSum &cs = c->cam_sum[sl.frame.group % gs_context::kSlots];
   const gs_stats &s = c->stats;
-  if (cs.group != sl.group) {
-    cs.group = sl.group;
+  if (cs.group != sl.frame.group) {
+    cs.group = sl.frame.group;
     cs.s = s;
     cs.done = 0;
   } else {
@@ -1923,21 +1941,21 @@ static void add_camera_stats(gs_context *c, const gs_context::Slot &sl) {
     cs.s.kernel_launches += s.kernel_launches;
     cs.s.n_slabs_run += s.n_slabs_run;  // one-pass passes: 0
   }
-  if (sl.ticket == sl.group) {  // camera 0's size and depth range
+  if (sl.ticket == sl.frame.group) {  // camera 0's size and depth range
     cs.s.width = s.width;
     cs.s.height = s.height;
     cs.s.min_depth = s.min_depth;
     cs.s.max_depth = s.max_depth;
   }
   cs.s.n_slabs = 0;
-  if (++cs.done == sl.group_n) c->stats = cs.s;
+  if (++cs.done == sl.frame.group_n) c->stats = cs.s;
 }
 
 static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   if (!sl.pending) return fail(c, GS_ERR_INVALID, "gs_wait: no frame in flight for this ticket");
-  if (sl.group != ~0ull && sl.ticket == sl.group + sl.group_n - 1) {
+  if (sl.frame.group != ~0ull && sl.ticket == sl.frame.group + sl.frame.group_n - 1) {
     // the last camera of a cameras frame (its ticket is the frame's): every camera before it is collected first
-    for (uint64_t t = sl.group; t < sl.ticket; ++t) {
+    for (uint64_t t = sl.frame.group; t < sl.ticket; ++t) {
       gs_context::Slot &o = c->slot[t % gs_context::kSlots];
       if (o.pending && o.ticket == t) {
         int rc_cam = wait_slot(c, o, nullptr);
@@ -1980,7 +1998,7 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
     if (rcode) return rcode;
     // grow once to the measured demand (+12.5 %); a frame whose overflow flag is stale (an earlier frame's regrow
     // already made room) is simply run again
-    const uint64_t demand = sl.slab ? sl.ctr_host->n_inst_slab_max : sl.ctr_host->n_inst;
+    const uint64_t demand = sl.frame.slab ? sl.ctr_host->n_inst_slab_max : sl.ctr_host->n_inst;
     if (demand > c->cap_inst) {
       const uint64_t need = std::max<uint64_t>(demand + demand / 8, c->cap_inst + c->cap_inst / 2);
       rcode = ensure_instances(c, need);
@@ -1992,15 +2010,15 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
         return rc_t ? rc_t : rcode;
       }
     }
-    sl.restage = false;  // a target frame blends over the rectangles staged at its first submission
+    sl.frame.restage = false;  // a target frame blends over the rectangles staged at its first submission
     if ((rcode = submit(c, sl))) return rcode;
   }
-  if (sl.pick) return GS_OK;  // a pick leaves the statistics and the sorted count of the frames as they were
+  if (sl.frame.pick) return GS_OK;  // a pick leaves the statistics and the sorted count of the frames as they were
   memset(&c->stats, 0, sizeof(c->stats));
   stats_from_counters(c, *sl.ctr_host, sl.fp_host->n_splats);
   c->stats.kernel_launches = sl.launches;
   c->stats.n_tiles = sl.fp_host->rc.n_tiles;
-  if (sl.stereo) {  // every view's
+  if (sl.frame.stereo) {  // every view's
     const ViewTable &vt = *sl.stereo_host;
     c->stats.n_tiles = vt.tile_base[vt.n_views - 1] + vt.view[vt.n_views - 1].rc.n_tiles;
   }
@@ -2015,10 +2033,10 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
       c->stats.n_pair_hits += v.w;
     }
   }
-  c->stats.width = sl.params.width;
-  c->stats.height = sl.params.height;
+  c->stats.width = sl.frame.view[0].width;
+  c->stats.height = sl.frame.view[0].height;
   cudaEventElapsedTime(&c->stats.ms_sort, sl.ev[0], sl.ev[1]);
-  if (sl.slab) {
+  if (sl.frame.slab) {
     // slab path: ms_sort = depth/cull + keys + plan; ms_raster = the slabs' rasters + the resolve; ms_bin = the rest of
     // the slab loop (compaction, per-slab sort, projection, binning)
     float loop = 0.f, res = 0.f, rs = 0.f;
@@ -2044,7 +2062,7 @@ static int wait_slot(gs_context *c, gs_context::Slot &sl, gs_stats *stats) {
   c->order_count = sl.ctr_host->sort.n_valid;
   c->last_sorted = sl.ctr_host->sort.n_valid;
   c->have_last_sorted = true;
-  if (sl.group != ~0ull) add_camera_stats(c, sl);
+  if (sl.frame.group != ~0ull) add_camera_stats(c, sl);
   if (stats) *stats = c->stats;
   return GS_OK;
 }
@@ -2081,13 +2099,14 @@ static int wait_overlapping(gs_context *c, const TargetInput &t, const gs_render
   for (;;) {
     gs_context::Slot *hit = nullptr;
     for (auto &o : c->slot) {
-      const bool shared = o.tcolor == t.t->color || ((dw || o.depth_write) && t.t->depth && o.tdepth == t.t->depth);
-      if (!o.pending || !o.target || !shared || (hit && o.ticket > hit->ticket)) continue;
+      const gs_context::FrameDesc &of = o.frame;
+      const bool shared = of.tcolor == t.t->color || ((dw || of.depth_write) && t.t->depth && of.tdepth == t.t->depth);
+      if (!o.pending || !of.target || !shared || (hit && o.ticket > hit->ticket)) continue;
       bool meet = false;
       for (uint32_t a = 0; a < n_views; ++a)
-        for (uint32_t b = 0; b < o.n_views; ++b)
-          meet = meet || rects_overlap(t.xy[a][0], t.xy[a][1], views[a].width, views[a].height, o.torg[b][0], o.torg[b][1],
-                                       o.view[b].width, o.view[b].height);
+        for (uint32_t b = 0; b < of.n_views; ++b)
+          meet = meet || rects_overlap(t.xy[a][0], t.xy[a][1], views[a].width, views[a].height, of.torg[b][0], of.torg[b][1],
+                                       of.view[b].width, of.view[b].height);
       if (meet) hit = &o;
     }
     if (!hit) return GS_OK;
@@ -2118,24 +2137,47 @@ static int check_sort_f32(gs_context *c, const gs_render_params *p) {
   return GS_OK;
 }
 
-// gs_render_async, scene and views scene frames.  scene: the table built by build_scene_table (nullptr = a plain frame);
+// the size rule of every view (a gs_target frame checks it among the target's rules, ahead of the table's emptiness)
+static int check_size(gs_context *c, const gs_render_params *p) {
+  if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
+    return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
+  return GS_OK;
+}
+
+// the rules of one view of any frame: its size, its format and those of GS_RENDER_BLEND_UNORM8
+static int check_view(gs_context *c, const gs_render_params *p) {
+  int rc = check_size(c, p);
+  if (rc) return rc;
+  if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+  return check_blend8(c, p);
+}
+
+// a pick's validated query points and where their results go
+struct PickQuery {
+  const uint32_t *xy;
+  uint32_t n;
+  gs_pick *out;
+};
+
+// Every frame: gs_render_async, scene and views scene frames, a camera's pass and a pick.  scene: the frame draws the
+// entities of the table build_scene_table left in c->scene_tmp, scene_bytes long (false: the plain frame of p's matrices);
 // color_in: the colour target or nullptr; stereo: the views of a views scene frame (nullptr otherwise; p is view 0);
 // target: the gs_target the frame is drawn into in place (nullptr otherwise; color_in is then nullptr and out_rgba the
 // target's colour buffer).
 // group: a camera's pass of a cameras frame, the ticket of the frame's first camera and the frame's camera count (~0 and 0
 // otherwise); such a pass is always one-pass.
-static int render_async(gs_context *c, const gs_render_params *p, const SceneTable *scene, size_t scene_bytes,
-                        const void *color_in, void *out_rgba, uint64_t *out_ticket, const ViewsInput *stereo = nullptr,
-                        const TargetInput *target = nullptr, uint64_t group = ~0ull, uint32_t group_n = 0) {
-  if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
-    return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
-  if (p->out_format != GS_FORMAT_RGBA8 && p->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+// pick: the points of a pick (nullptr otherwise).  A pick is always one-pass, stages the scene table on the plain path
+// too (k_pick maps its hits through it), and is waited for at once.
+static int render_async(gs_context *c, const gs_render_params *p, bool scene, size_t scene_bytes, const void *color_in,
+                        void *out_rgba, uint64_t *out_ticket, const ViewsInput *stereo = nullptr,
+                        const TargetInput *target = nullptr, uint64_t group = ~0ull, uint32_t group_n = 0,
+                        const PickQuery *pick = nullptr) {
   int rcode;
-  if ((rcode = check_blend8(c, p)) || (rcode = check_sort_f32(c, p))) return rcode;
+  if ((rcode = check_view(c, p)) || (rcode = check_sort_f32(c, p))) return rcode;
   // a views frame's bin table holds every view's bins (4 * 43 * 43 at most, still a 16-bit id), its slab state every
   // view's tiles
   FrameNeeds need{};
-  need.scene = scene != nullptr;
+  need.scene = scene;
   need.f32 = (p->flags & (GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL)) != 0;  // a radial frame takes the precise passes
   need.n_views = stereo ? stereo->n : 1u;
   need.depth_write = target && (target->t->flags & GS_TARGET_DEPTH_WRITE);
@@ -2162,15 +2204,16 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   // large scenes render front to back in depth slabs, plain, scene and stereo frames alike; the one-pass and slab paths share
   // scratch buffers, so a change drains (the criterion is the number of SORTED splats: the last frame's count when there
   // is one, else the splats the sort considers - the resident ones, or those in the scene's entity ranges)
+  const SceneTable &table = *c->scene_tmp;
   uint32_t sortable = c->n;
   if (scene) {
     sortable = 0;
-    for (uint32_t k = 0; k < scene->n; ++k) sortable += scene->obj[k].end - scene->obj[k].first;
+    for (uint32_t k = 0; k < table.n; ++k) sortable += table.obj[k].end - table.obj[k].first;
   }
   const uint32_t expect_sorted = c->have_last_sorted ? c->last_sorted : sortable;
   // views frames by their own threshold (GS_SLAB_MIN_XR); they accept neither flag.  GS_RENDER_BLEND_UNORM8 frames are
   // always one-pass: the slab path stops at front-to-back saturation, which rounding after every blend does not have
-  const bool slab = group == ~0ull && expect_sorted >= (stereo ? c->slab_min_xr : c->slab_min) &&
+  const bool slab = !pick && group == ~0ull && expect_sorted >= (stereo ? c->slab_min_xr : c->slab_min) &&
                     !(p->flags & (GS_RENDER_REUSE_SORT | GS_RENDER_STATS | GS_RENDER_BLEND_UNORM8));
   need.slab = slab;
   if ((int)slab != c->last_mode) {
@@ -2179,60 +2222,82 @@ static int render_async(gs_context *c, const gs_render_params *p, const SceneTab
   }
   // growing any shared buffer needs an idle pipeline
   if (!frame_bufs_ready(c, need) && ((rcode = idle(c)) || (rcode = ensure_frame_bufs(c, need)))) return rcode;
-  sl.params = *p;
-  sl.n_views = need.n_views;
-  sl.view[0] = *p;
-  sl.out_user[0] = out_rgba;
-  sl.ticket = ticket;
-  sl.n_splats = c->n;
-  sl.n_sortable = sortable;
-  sl.slab = slab;
-  sl.pick = false;
-  sl.f32 = need.f32;
-  sl.radial = (p->flags & GS_RENDER_SORT_RADIAL) != 0;
-  sl.antialias = (p->flags & GS_RENDER_ANTIALIAS) != 0;
-  sl.cameras = group != ~0ull;
-  sl.group = group;
-  sl.group_n = group_n;
-  sl.color_in[0] = color_in;
-  sl.color_device = (p->flags & GS_RENDER_COLOR_DEVICE) != 0;
-  sl.target = target != nullptr;
-  sl.depth_write = need.depth_write;
-  sl.restage = true;
+  if (pick) {
+    // the points and their bins, ahead of the frame's stages on the sort stream
+    if ((rcode = ensure_pick_bufs(c))) return rcode;
+    PickInput &in = *c->pick_in_host;
+    in.n = pick->n;
+    memset(in.open, 0, sizeof(in.open));
+    const uint32_t bins_x = (p->width + kBin - 1) / kBin;
+    for (uint32_t i = 0; i < pick->n; ++i) {
+      const uint32_t x = pick->xy[2 * i], y = pick->xy[2 * i + 1];
+      in.xy[i] = make_uint2(x, y);
+      in.open[(y / kBin) * bins_x + x / kBin] = 1u;
+    }
+    GS_CUDA(c, cudaMemcpyAsync(c->pick_in, c->pick_in_host, sizeof(PickInput), cudaMemcpyHostToDevice, c->stream));
+  }
+  gs_context::FrameDesc f;
+  f.n_views = need.n_views;
+  f.view[0] = *p;
+  f.out_user[0] = out_rgba;
+  f.color_in[0] = color_in;
+  f.color_device = (p->flags & GS_RENDER_COLOR_DEVICE) != 0;
+  f.n_splats = c->n;
+  f.n_sortable = sortable;
+  f.scene = scene;
+  f.stereo = stereo != nullptr;
+  f.slab = slab;
+  f.pick = pick != nullptr;
+  f.f32 = need.f32;
+  f.radial = (p->flags & GS_RENDER_SORT_RADIAL) != 0;
+  f.antialias = (p->flags & GS_RENDER_ANTIALIAS) != 0;
+  f.group = group;
+  f.group_n = group_n;
+  if (stereo)
+    for (uint32_t v = 1; v < stereo->n; ++v) {
+      f.view[v] = stereo->views[v];
+      f.out_user[v] = stereo->out[v];
+      f.color_in[v] = stereo->color_in ? stereo->color_in[v] : nullptr;
+    }
   if (target) {
-    sl.target_device = (target->t->flags & GS_TARGET_DEVICE) != 0;
-    sl.tcolor = target->t->color;
-    sl.tdepth = target->t->depth;
-    sl.tpitch = target->t->pitch;
-    memcpy(sl.torg, target->xy, sizeof(sl.torg));
+    f.target = true;
+    f.target_device = (target->t->flags & GS_TARGET_DEVICE) != 0;
+    f.tcolor = target->t->color;
+    f.tdepth = target->t->depth;
+    f.tpitch = target->t->pitch;
+    memcpy(f.torg, target->xy, sizeof(f.torg));
+    f.depth_write = need.depth_write;
   }
-  if (c->sh_degree && !sl.sh_cam_dev) {  // SH contexts: the slot's camera table, fixed size, allocated once
-    GS_CUDA(c, cudaMalloc((void **)&sl.sh_cam_dev, sizeof(float4) * kMaxObjects * kMaxViews));
-    GS_CUDA(c, cudaHostAlloc((void **)&sl.sh_cam_host, sizeof(float4) * kMaxObjects * kMaxViews, cudaHostAllocDefault));
-  }
-  sl.scene = scene != nullptr;
-  if (scene) {
+  sl.frame = f;
+  sl.ticket = ticket;
+  if (c->sh_degree && (rcode = ensure_slot_sh(c, sl))) return rcode;
+  if (scene || pick) {
     if ((rcode = ensure_slot_scene(c, sl))) return rcode;
-    memcpy(sl.scene_host, scene, scene_bytes);
+    memcpy(sl.scene_host, &table, scene_bytes);
     sl.scene_bytes = scene_bytes;
   }
-  sl.stereo = stereo != nullptr;
   if (stereo) {
     if ((rcode = ensure_slot_stereo(c, sl))) return rcode;
-    for (uint32_t v = 1; v < stereo->n; ++v) {
-      sl.view[v] = stereo->views[v];
-      sl.out_user[v] = stereo->out[v];
-      sl.color_in[v] = stereo->color_in ? stereo->color_in[v] : nullptr;
-    }
-    memcpy(sl.stereo_host->mv, stereo->mv, sizeof(stereo->mv[0]) * scene->n);
+    memcpy(sl.stereo_host->mv, stereo->mv, sizeof(stereo->mv[0]) * table.n);
     // one copy: header, the frames, and the entities in use (up to the last view in use of the last one)
     sl.stereo_bytes = offsetof(ViewTable, mv);
-    if (scene->n) sl.stereo_bytes += sizeof(stereo->mv[0]) * (scene->n - 1) + sizeof(float) * 16 * stereo->n;
+    if (table.n) sl.stereo_bytes += sizeof(stereo->mv[0]) * (table.n - 1) + sizeof(float) * 16 * stereo->n;
   }
   if ((rcode = submit(c, sl))) return rcode;
   c->next_ticket = ticket + 1;
   if (out_ticket) *out_ticket = ticket;
+  if (!pick) return GS_OK;
+  if ((rcode = wait_slot(c, sl, nullptr))) return rcode;
+  memcpy(pick->out, c->pick_out_host, sizeof(gs_pick) * pick->n);
   return GS_OK;
+}
+
+// the synchronous form of an _async entry point: async(c, args..., &ticket), then its frame waited for if it was submitted
+template <class F, class... A>
+static int submit_and_wait(F async, gs_context *c, gs_stats *stats, A... args) {
+  uint64_t t = 0;
+  const int rc = async(c, args..., &t);
+  return rc ? rc : gs_wait(c, t, stats);
 }
 
 extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *out_rgba, uint64_t *out_ticket) {
@@ -2240,7 +2305,18 @@ extern "C" int gs_render_async(gs_context *c, const gs_render_params *p, void *o
   if (p->flags & GS_RENDER_SCENE_INTERLEAVE)
     return fail(c, GS_ERR_INVALID, "GS_RENDER_SCENE_INTERLEAVE is a scene frame flag: gs_render has no entities");
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render before any push");
-  return render_async(c, p, nullptr, 0, nullptr, out_rgba, out_ticket);
+  return render_async(c, p, false, 0, nullptr, out_rgba, out_ticket);
+}
+
+// A scene frame of one entity over the whole table, not interleaved, is drawn as the plain frame with that entity's
+// matrices (an interleaved frame keeps the scene path, whose keys clamp where the plain sort drops).  Whether the frame p
+// of the validated entities objs takes that path; if it does, p gets the entity's modelview and cutout.
+static bool plain_path(const gs_context *c, const gs_object *objs, uint32_t n_objs, gs_render_params &p) {
+  if ((p.flags & GS_RENDER_SCENE_INTERLEAVE) || n_objs != 1 || objs[0].first != 0 || objs[0].count != c->n) return false;
+  memcpy(p.modelview, objs[0].modelview, sizeof(p.modelview));
+  p.has_cutout = objs[0].has_cutout;
+  memcpy(p.cutout16, objs[0].cutout16, sizeof(p.cutout16));
+  return true;
 }
 
 // gs_render_scene_async, and gs_render_scene_target_async (target set: color_in is nullptr, out_rgba the target's colour)
@@ -2250,19 +2326,11 @@ static int scene_async(gs_context *c, const gs_render_params *frame, const gs_ob
   if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_render_scene before any push");
   if (frame->flags & GS_RENDER_REUSE_SORT) return fail(c, GS_ERR_INVALID, "scene frames always sort: GS_RENDER_REUSE_SORT is not accepted");
   size_t bytes = 0;
-  const bool interleave = (frame->flags & GS_RENDER_SCENE_INTERLEAVE) != 0;
-  int rc = build_scene_table(c, objs, n_objs, interleave, *c->scene_tmp, &bytes);
+  int rc = build_scene_table(c, objs, n_objs, (frame->flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes);
   if (rc) return rc;
-  if (!interleave && n_objs == 1 && objs[0].first == 0 && objs[0].count == c->n) {
-    // one entity over the whole table: the plain frame with this entity's matrices, plus the colour target (an interleaved
-    // frame keeps the scene path, whose keys clamp where the plain sort drops)
-    gs_render_params p = *frame;
-    memcpy(p.modelview, objs[0].modelview, sizeof(p.modelview));
-    p.has_cutout = objs[0].has_cutout;
-    memcpy(p.cutout16, objs[0].cutout16, sizeof(p.cutout16));
-    return render_async(c, &p, nullptr, 0, color_in, out_rgba, out_ticket, nullptr, target, group, group_n);
-  }
-  return render_async(c, frame, c->scene_tmp, bytes, color_in, out_rgba, out_ticket, nullptr, target, group, group_n);
+  gs_render_params p = *frame;
+  const bool plain = plain_path(c, objs, n_objs, p);
+  return render_async(c, &p, !plain, bytes, color_in, out_rgba, out_ticket, nullptr, target, group, group_n);
 }
 
 extern "C" int gs_render_scene_async(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
@@ -2288,8 +2356,8 @@ static int check_target(gs_context *c, const gs_render_params *p, const gs_targe
     return fail(c, GS_ERR_INVALID,
                 "target frame: GS_RENDER_OUT_DEVICE, _COLOR_DEVICE, _DEPTH_DEVICE (use GS_TARGET_DEVICE), _OUT_TILED, "
                 "_OUT_PEER and _REUSE_SORT are not accepted");
-  if (p->width == 0 || p->height == 0 || p->width > 4096 || p->height > 4096)
-    return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
+  int rc = check_size(c, p);
+  if (rc) return rc;
   if ((uint64_t)x + p->width > t->pitch || (uint64_t)y + p->height > t->rows)
     return fail(c, GS_ERR_INVALID, "target frame: the viewport rectangle is not inside the target");
   return GS_OK;
@@ -2307,18 +2375,12 @@ extern "C" int gs_render_scene_target_async(gs_context *c, const gs_render_param
 
 extern "C" int gs_render_scene_target(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
                                       const gs_target *target, uint32_t x, uint32_t y, gs_stats *stats) {
-  uint64_t t = 0;
-  int rc = gs_render_scene_target_async(c, frame, objs, n_objs, target, x, y, &t);
-  if (rc) return rc;
-  return gs_wait(c, t, stats);
+  return submit_and_wait(gs_render_scene_target_async, c, stats, frame, objs, n_objs, target, x, y);
 }
 
 extern "C" int gs_render_scene(gs_context *c, const gs_render_params *frame, const gs_object *objs, uint32_t n_objs,
                                const void *color_in, void *out_rgba, gs_stats *stats) {
-  uint64_t t = 0;
-  int rc = gs_render_scene_async(c, frame, objs, n_objs, color_in, out_rgba, &t);
-  if (rc) return rc;
-  return gs_wait(c, t, stats);
+  return submit_and_wait(gs_render_scene_async, c, stats, frame, objs, n_objs, color_in, out_rgba);
 }
 
 // gs_pick_scene: the scene frame's sort and projection stage, then a bin stage that bins only the bins of the query points
@@ -2334,108 +2396,42 @@ extern "C" int gs_pick_scene(gs_context *c, const gs_render_params *frame, const
                 "gs_pick_scene: no flag other than GS_RENDER_DEPTH_DEVICE, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32, "
                 "GS_RENDER_SORT_RADIAL and GS_RENDER_ANTIALIAS is accepted");
   if (c->shard_world > 1) return fail(c, GS_ERR_INVALID, "gs_pick_scene: not on a sharded context");
-  if (frame->width == 0 || frame->height == 0 || frame->width > 4096 || frame->height > 4096)
-    return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
-  if (frame->out_format != GS_FORMAT_RGBA8 && frame->out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
+  int rc = check_view(c, frame);
+  if (rc) return rc;
   for (uint32_t i = 0; i < n_points; ++i)
     if (xy[2 * i] >= frame->width || xy[2 * i + 1] >= frame->height)
       return fail(c, GS_ERR_INVALID, "gs_pick_scene: a point lies outside the frame");
   size_t bytes = 0;
-  const bool interleave = (frame->flags & GS_RENDER_SCENE_INTERLEAVE) != 0;
-  int rc = build_scene_table(c, objs, n_objs, interleave, *c->scene_tmp, &bytes);
-  if (rc) return rc;
-  // the frame gs_render_scene draws: one entity over the whole table takes the plain path with its matrices (not when
-  // interleaved)
-  gs_render_params p = *frame;
-  const bool plain = !interleave && n_objs == 1 && objs[0].first == 0 && objs[0].count == c->n;
-  if (plain) {
-    memcpy(p.modelview, objs[0].modelview, sizeof(p.modelview));
-    p.has_cutout = objs[0].has_cutout;
-    memcpy(p.cutout16, objs[0].cutout16, sizeof(p.cutout16));
-  }
+  if ((rc = build_scene_table(c, objs, n_objs, (frame->flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes)))
+    return rc;
+  gs_render_params p = *frame;  // the frame gs_render_scene draws
+  const bool plain = plain_path(c, objs, n_objs, p);
+  const PickQuery q{xy, n_points, out};
+  return render_async(c, &p, !plain, bytes, nullptr, nullptr, nullptr, nullptr, nullptr, ~0ull, 0, &q);
+}
+
+// gs_sort_scene_flags and the two sorts it generalises, each with its own message for an empty table
+static int sort_scene(gs_context *c, const gs_object *objs, uint32_t n_objs, uint32_t flags, uint32_t *out_idx,
+                      uint32_t *out_count, const char *empty) {
+  if (c->n == 0) return fail(c, GS_ERR_EMPTY, empty);
   GS_CUDA(c, cudaSetDevice(c->device));
-  const uint64_t ticket = c->next_ticket;
-  gs_context::Slot &sl = c->slot[ticket % gs_context::kSlots];
-  if (sl.pending && (rc = wait_slot(c, sl, nullptr))) return rc;
-  if (c->last_mode != 0) {  // always one-pass: the one-pass and slab paths share scratch buffers
-    if ((rc = idle(c))) return rc;
-    c->last_mode = 0;
-  }
-  FrameNeeds need{};
-  need.scene = !plain;
-  need.f32 = (frame->flags & (GS_RENDER_SORT_F32 | GS_RENDER_SORT_RADIAL)) != 0;
-  need.n_views = 1;
-  {
-    RenderConsts grid;
-    fill_grid(p.width, p.height, grid);
-    need.n_tiles = need.n_tiles_all = grid.n_tiles;
-    need.n_bins_all = grid.n_bins;
-  }
-  if (!frame_bufs_ready(c, need) && ((rc = idle(c)) || (rc = ensure_frame_bufs(c, need)))) return rc;
-  if ((rc = ensure_pick_bufs(c)) || (rc = ensure_slot_scene(c, sl))) return rc;
-  // the points and their bins, ahead of the frame's stages on the sort stream
-  PickInput &in = *c->pick_in_host;
-  in.n = n_points;
-  memset(in.open, 0, sizeof(in.open));
-  const uint32_t bins_x = (p.width + kBin - 1) / kBin;
-  for (uint32_t i = 0; i < n_points; ++i) {
-    in.xy[i] = make_uint2(xy[2 * i], xy[2 * i + 1]);
-    in.open[(xy[2 * i + 1] / kBin) * bins_x + xy[2 * i] / kBin] = 1u;
-  }
-  GS_CUDA(c, cudaMemcpyAsync(c->pick_in, c->pick_in_host, sizeof(PickInput), cudaMemcpyHostToDevice, c->stream));
-  sl.params = p;
-  sl.n_views = 1;
-  sl.view[0] = p;
-  sl.out_user[0] = nullptr;
-  sl.ticket = ticket;
-  sl.n_splats = c->n;
-  sl.n_sortable = c->n;
-  sl.slab = false;
-  sl.pick = true;
-  sl.f32 = need.f32;
-  sl.radial = (frame->flags & GS_RENDER_SORT_RADIAL) != 0;
-  sl.antialias = (frame->flags & GS_RENDER_ANTIALIAS) != 0;
-  sl.cameras = false;
-  sl.group = ~0ull;
-  sl.color_in[0] = nullptr;
-  sl.color_device = false;
-  sl.target = false;
-  sl.depth_write = false;
-  sl.restage = true;
-  if (c->sh_degree && !sl.sh_cam_dev) {
-    GS_CUDA(c, cudaMalloc((void **)&sl.sh_cam_dev, sizeof(float4) * kMaxObjects * kMaxViews));
-    GS_CUDA(c, cudaHostAlloc((void **)&sl.sh_cam_host, sizeof(float4) * kMaxObjects * kMaxViews, cudaHostAllocDefault));
-  }
-  sl.scene = !plain;
-  memcpy(sl.scene_host, c->scene_tmp, bytes);
-  sl.scene_bytes = bytes;
-  sl.stereo = false;
-  if ((rc = submit(c, sl))) return rc;
-  c->next_ticket = ticket + 1;
-  if ((rc = wait_slot(c, sl, nullptr))) return rc;
-  memcpy(out, c->pick_out_host, sizeof(gs_pick) * n_points);
-  return GS_OK;
+  size_t bytes = 0;
+  int rc = build_scene_table(c, objs, n_objs, (flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes);
+  if (rc) return rc;
+  const bool radial = (flags & GS_RENDER_SORT_RADIAL) != 0;
+  return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count, radial || (flags & GS_RENDER_SORT_F32), radial);
 }
 
 extern "C" int gs_sort_scene(gs_context *c, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx, uint32_t *out_count) {
   if (!c) return GS_ERR_INVALID;
-  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_sort_scene before any push");
-  GS_CUDA(c, cudaSetDevice(c->device));
-  size_t bytes = 0;
-  int rc = build_scene_table(c, objs, n_objs, false, *c->scene_tmp, &bytes);
-  if (rc) return rc;
-  return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count);
+  return sort_scene(c, objs, n_objs, 0, out_idx, out_count, "gs_sort_scene before any push");
 }
 
 extern "C" int gs_sort_scene_interleaved(gs_context *c, const gs_object *objs, uint32_t n_objs, uint32_t *out_idx,
                                          uint32_t *out_count) {
   if (!c) return GS_ERR_INVALID;
-  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_sort_scene_interleaved before any push");
-  GS_CUDA(c, cudaSetDevice(c->device));
-  size_t bytes = 0;
-  int rc = build_scene_table(c, objs, n_objs, true, *c->scene_tmp, &bytes);
-  if (rc) return rc;
-  return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count);
+  return sort_scene(c, objs, n_objs, GS_RENDER_SCENE_INTERLEAVE, out_idx, out_count,
+                    "gs_sort_scene_interleaved before any push");
 }
 
 extern "C" int gs_sort_scene_flags(gs_context *c, const gs_object *objs, uint32_t n_objs, uint32_t flags, uint32_t *out_idx,
@@ -2445,13 +2441,7 @@ extern "C" int gs_sort_scene_flags(gs_context *c, const gs_object *objs, uint32_
     return fail(c, GS_ERR_INVALID,
                 "gs_sort_scene_flags: no flag other than GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32 and GS_RENDER_SORT_RADIAL "
                 "is accepted");
-  if (c->n == 0) return fail(c, GS_ERR_EMPTY, "gs_sort_scene_flags before any push");
-  GS_CUDA(c, cudaSetDevice(c->device));
-  size_t bytes = 0;
-  int rc = build_scene_table(c, objs, n_objs, (flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes);
-  if (rc) return rc;
-  const bool radial = (flags & GS_RENDER_SORT_RADIAL) != 0;
-  return sort_only(c, nullptr, nullptr, c->scene_tmp, bytes, out_idx, out_count, radial || (flags & GS_RENDER_SORT_F32), radial);
+  return sort_scene(c, objs, n_objs, flags, out_idx, out_count, "gs_sort_scene_flags before any push");
 }
 
 extern "C" int gs_wait(gs_context *c, uint64_t ticket, gs_stats *stats) {
@@ -2467,10 +2457,7 @@ extern "C" int gs_wait(gs_context *c, uint64_t ticket, gs_stats *stats) {
 }
 
 extern "C" int gs_render(gs_context *c, const gs_render_params *p, void *out_rgba, gs_stats *stats) {
-  uint64_t t = 0;
-  int rc = gs_render_async(c, p, out_rgba, &t);
-  if (rc) return rc;
-  return gs_wait(c, t, stats);
+  return submit_and_wait(gs_render_async, c, stats, p, out_rgba);
 }
 
 // XR: one sort request per frame from the head camera (tick(), index.js:438-455), one draw per eye with that eye's
@@ -2523,10 +2510,7 @@ static int scene_views_async(gs_context *c, const gs_render_params *views, uint3
   for (uint32_t v = 1; v < n_views; ++v) {  // view 0 is checked by render_async
     const gs_render_params &p = views[v];
     if (p.flags != views[0].flags) return fail(c, GS_ERR_INVALID, "views frame: every view must have the same flags");
-    if (p.width == 0 || p.height == 0 || p.width > 4096 || p.height > 4096)
-      return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
-    if (p.out_format != GS_FORMAT_RGBA8 && p.out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
-    if ((rc = check_blend8(c, &p))) return rc;
+    if ((rc = check_view(c, &p))) return rc;
   }
   size_t bytes = 0;
   rc = build_scene_table(c, objs, n_objs, (views[0].flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes);
@@ -2538,7 +2522,7 @@ static int scene_views_async(gs_context *c, const gs_render_params *views, uint3
     for (uint32_t v = 0; v < n_views; ++v)
       memcpy(mv[j][v], view_modelviews + ((size_t)v * n_objs + t.obj[j].rank) * 16, sizeof(mv[j][v]));
   const ViewsInput in{n_views, views, color_in, out_rgba, mv};
-  return render_async(c, &views[0], c->scene_tmp, bytes, color_in ? color_in[0] : nullptr, out_rgba[0], out_ticket, &in, target);
+  return render_async(c, &views[0], true, bytes, color_in ? color_in[0] : nullptr, out_rgba[0], out_ticket, &in, target);
 }
 
 // the stereo calls are the two-view case, with equal eye sizes (a WebXR projection layer's two eyes)
@@ -2619,37 +2603,29 @@ extern "C" int gs_render_scene_views_target_async(gs_context *c, const gs_render
 extern "C" int gs_render_scene_stereo_target(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
                                              const float *eye_modelviews, uint32_t n_objs, const gs_target *layer,
                                              const uint32_t eye_xy[4], gs_stats *stats) {
-  uint64_t t = 0;
-  int rc = gs_render_scene_stereo_target_async(c, eyes, objs, eye_modelviews, n_objs, layer, eye_xy, &t);
-  if (rc) return rc;
-  return gs_wait(c, t, stats);
+  return submit_and_wait(gs_render_scene_stereo_target_async, c, stats, eyes, objs, eye_modelviews, n_objs, layer,
+                         eye_xy);
 }
 
 extern "C" int gs_render_scene_views_target(gs_context *c, const gs_render_params *views, uint32_t n_views,
                                             const gs_object *objs, const float *view_modelviews, uint32_t n_objs,
                                             const gs_target *layer, const uint32_t *view_xy, gs_stats *stats) {
-  uint64_t t = 0;
-  int rc = gs_render_scene_views_target_async(c, views, n_views, objs, view_modelviews, n_objs, layer, view_xy, &t);
-  if (rc) return rc;
-  return gs_wait(c, t, stats);
+  return submit_and_wait(gs_render_scene_views_target_async, c, stats, views, n_views, objs, view_modelviews, n_objs,
+                         layer, view_xy);
 }
 
 extern "C" int gs_render_scene_stereo(gs_context *c, const gs_render_params eyes[2], const gs_object *objs,
                                       const float *eye_modelviews, uint32_t n_objs, const void *const color_in[2],
                                       void *const out_rgba[2], gs_stats *stats) {
-  uint64_t t = 0;
-  int rc = gs_render_scene_stereo_async(c, eyes, objs, eye_modelviews, n_objs, color_in, out_rgba, &t);
-  if (rc) return rc;
-  return gs_wait(c, t, stats);
+  return submit_and_wait(gs_render_scene_stereo_async, c, stats, eyes, objs, eye_modelviews, n_objs, color_in,
+                         out_rgba);
 }
 
 extern "C" int gs_render_scene_views(gs_context *c, const gs_render_params *views, uint32_t n_views, const gs_object *objs,
                                      const float *view_modelviews, uint32_t n_objs, const void *const *color_in,
                                      void *const *out_rgba, gs_stats *stats) {
-  uint64_t t = 0;
-  int rc = gs_render_scene_views_async(c, views, n_views, objs, view_modelviews, n_objs, color_in, out_rgba, &t);
-  if (rc) return rc;
-  return gs_wait(c, t, stats);
+  return submit_and_wait(gs_render_scene_views_async, c, stats, views, n_views, objs, view_modelviews, n_objs,
+                         color_in, out_rgba);
 }
 
 // gs_render_scene_cameras_async: every rule is checked before the first camera is submitted, then each camera is one
@@ -2671,10 +2647,7 @@ extern "C" int gs_render_scene_cameras_async(gs_context *c, const gs_render_para
     const gs_render_params &p = cams[v];
     if (p.flags != cams[0].flags) return fail(c, GS_ERR_INVALID, "cameras frame: every camera must have the same flags");
     if (p.out_format != cams[0].out_format) return fail(c, GS_ERR_INVALID, "cameras frame: every camera must have the same out_format");
-    if (p.width == 0 || p.height == 0 || p.width > 4096 || p.height > 4096)
-      return fail(c, GS_ERR_INVALID, "frame size must be within 1..4096 per side");
-    if (p.out_format != GS_FORMAT_RGBA8 && p.out_format != GS_FORMAT_RGBA32F) return fail(c, GS_ERR_INVALID, "bad out_format");
-    if ((rc = check_blend8(c, &p))) return rc;
+    if ((rc = check_view(c, &p))) return rc;
   }
   size_t bytes = 0;
   if ((rc = build_scene_table(c, objs, n_objs, (cams[0].flags & GS_RENDER_SCENE_INTERLEAVE) != 0, *c->scene_tmp, &bytes)))
@@ -2696,10 +2669,8 @@ extern "C" int gs_render_scene_cameras_async(gs_context *c, const gs_render_para
 extern "C" int gs_render_scene_cameras(gs_context *c, const gs_render_params *cams, uint32_t n_cams, const gs_object *objs,
                                        const float *cam_modelviews, uint32_t n_objs, const void *const *color_in,
                                        void *const *out_rgba, gs_stats *stats) {
-  uint64_t t = 0;
-  int rc = gs_render_scene_cameras_async(c, cams, n_cams, objs, cam_modelviews, n_objs, color_in, out_rgba, &t);
-  if (rc) return rc;
-  return gs_wait(c, t, stats);
+  return submit_and_wait(gs_render_scene_cameras_async, c, stats, cams, n_cams, objs, cam_modelviews, n_objs,
+                         color_in, out_rgba);
 }
 
 extern "C" int gs_cube_to_equirect(gs_context *c, const gs_cube_face faces[6], int32_t out_format, uint32_t flags,

@@ -423,7 +423,39 @@ struct gs_context {
   // (With three slots a caller that receives frames in host memory had to collect frame k-1's copy before it could
   // submit frame k+2, and the sort stage idled for the length of the copy.) ----
   static constexpr int kSlots = 4;
+  // What the caller decided about one frame: render_async builds it and a slot holds it whole, so a field a frame kind
+  // does not set holds its default here, never an earlier frame's value
+  struct FrameDesc {
+    uint32_t n_views = 1;                    // views of a views scene frame (every other frame: 1)
+    gs_render_params view[gs::kMaxViews]{};  // each view's parameters ([0]: the frame's)
+    void *out_user[gs::kMaxViews] = {};      // each view's output
+    const void *color_in[gs::kMaxViews] = {};  // caller's colour target (scene frames), host unless color_device
+    bool color_device = false;
+    uint32_t n_splats = 0;                   // resident splats when the frame was submitted
+    uint32_t n_sortable = 0;                 // splats the frame's sort considers (scene frames: in the entities' ranges)
+    bool scene = false;                      // multi-entity frame (gs_render_scene): the slot's scene table
+    bool stereo = false;                     // views scene frame (gs_render_scene_views / _stereo): the slot's view table
+    bool slab = false;                       // rendered by the front-to-back slab path
+    bool pick = false;                       // a pick (gs_pick_scene): bin and pick stages instead of binning and raster
+    bool f32 = false;                        // GS_RENDER_SORT_F32: sorted by the f32 depth (gs_sort.cu Z passes)
+    bool radial = false;                     // GS_RENDER_SORT_RADIAL: f32 too, its depth pass writing -r (k_depth_cull<true>)
+    bool antialias = false;                  // GS_RENDER_ANTIALIAS: projected with the anti-aliased alpha (k_project<.., AA>)
+    // one camera's pass of a cameras frame (gs_render_scene_cameras), whose stages are launched without graphs: the ticket
+    // of the frame's first camera (its cameras hold tickets group .. group + group_n - 1); ~0 for every other frame
+    uint64_t group = ~0ull;
+    uint32_t group_n = 0;
+    // frames into a gs_target (gs_render_scene*_target): each view drawn in place at its rectangle of the caller's buffers
+    bool target = false;
+    bool target_device = false;              // GS_TARGET_DEVICE: read and written where they are; else staged per view
+    void *tcolor = nullptr;
+    const float *tdepth = nullptr;
+    uint32_t tpitch = 0;
+    uint32_t torg[gs::kMaxViews][2] = {};    // rectangle origin (x, y) of each view
+    bool restage = true;                     // false while gs_wait re-runs the frame: the staged rectangles are reused
+    bool depth_write = false;                // GS_TARGET_DEPTH_WRITE: the frame also stores the target's depth
+  };
   struct Slot {
+    FrameDesc frame;                         // the slot's frame; what follows is derived by submit or owned by the slot
     gs::FrameCounters *ctr = nullptr;        // device
     gs::FrameCounters *ctr_host = nullptr;   // pinned
     gs::FrameParams *fp = nullptr;           // device
@@ -433,14 +465,8 @@ struct gs_context {
     size_t frame_bytes[gs::kMaxViews] = {};
     void *depth_dev[gs::kMaxViews] = {};     // staging of a host depth_in
     size_t depth_bytes[gs::kMaxViews] = {};
-    const void *color_in[gs::kMaxViews] = {};  // caller's colour target (scene frames), host unless color_device
-    bool color_device = false;
     void *color_dev[gs::kMaxViews] = {};     // staging of a host color_in
     size_t color_bytes[gs::kMaxViews] = {};
-    bool scene = false;                      // multi-entity frame (gs_render_scene): scene table below
-    bool stereo = false;                     // views scene frame (gs_render_scene_views / _stereo): view table below
-    uint32_t n_views = 1;                    // its views (every other frame: 1)
-    gs_render_params view[gs::kMaxViews]{};  // each view's parameters ([0] = params)
     gs::ViewTable *stereo_dev = nullptr;     // device copy, fixed size (captured graphs bake the pointer)
     gs::ViewTable *stereo_host = nullptr;    // pinned staging
     size_t stereo_bytes = 0;                 // bytes in use (header, frames, and the entities in use)
@@ -452,28 +478,7 @@ struct gs_context {
     // order; 0 for a plain frame) and view v at k * kMaxViews + v.  Fixed size (captured graphs bake the pointer)
     float4 *sh_cam_dev = nullptr;
     float4 *sh_cam_host = nullptr;           // pinned staging
-    // frames into a gs_target (gs_render_scene*_target): each view drawn in place at its rectangle of the caller's buffers
-    bool target = false;
-    bool target_device = false;              // GS_TARGET_DEVICE: read and written where they are; else staged per view
-    void *tcolor = nullptr;
-    const float *tdepth = nullptr;
-    uint32_t tpitch = 0;
-    uint32_t torg[gs::kMaxViews][2] = {};    // rectangle origin (x, y) of each view
-    bool restage = true;                     // false while gs_wait re-runs the frame: the staged rectangles are reused
-    bool depth_write = false;                // GS_TARGET_DEPTH_WRITE: the frame also stores the target's depth
     uint32_t raster_flags = 0;               // k_raster instantiation of this frame (packed | depth | stats | blend8 | depth write)
-    uint32_t n_splats = 0;                   // resident splats when the frame was submitted
-    uint32_t n_sortable = 0;                 // splats the frame's sort considers (scene frames: in the entities' ranges)
-    bool slab = false;                       // rendered by the front-to-back slab path
-    bool pick = false;                       // a pick (gs_pick_scene): bin and pick stages instead of binning and raster
-    bool f32 = false;                        // GS_RENDER_SORT_F32: sorted by the f32 depth (gs_sort.cu Z passes)
-    bool radial = false;                     // GS_RENDER_SORT_RADIAL: f32 too, its depth pass writing -r (k_depth_cull<true>)
-    bool antialias = false;                  // GS_RENDER_ANTIALIAS: projected with the anti-aliased alpha (k_project<.., AA>)
-    // one camera's pass of a cameras frame (gs_render_scene_cameras): stages launched without graphs.  group: the ticket of
-    // the frame's first camera (its cameras hold tickets group .. group + group_n - 1), ~0 for every other frame
-    bool cameras = false;
-    uint64_t group = ~0ull;
-    uint32_t group_n = 0;
     int n_slabs = 0;
     cudaEvent_t slab_ev[gs::kMaxSlabs][2] = {};  // raster of each slab (timing)
     cudaEvent_t ev[5]{};                     // stage boundaries (timing)
@@ -494,9 +499,7 @@ struct gs_context {
     int index = 0;
     bool pending = false;
     bool host_out = false;
-    void *out_user[gs::kMaxViews] = {};
     size_t out_bytes[gs::kMaxViews] = {};
-    gs_render_params params{};
     uint32_t launches = 0;
     int set = 0;                                    // which order/proj_rec/rect and inst_rec/bin_range copy it uses
   } slot[kSlots];
