@@ -24,6 +24,7 @@ GS_TARGET_DEVICE = 1
 GS_TARGET_DEPTH_WRITE = 2
 GS_CROP_KEEP_INSIDE, GS_CROP_KEEP_OUTSIDE = 0, 1
 GS_EXPORT_SPLAT, GS_EXPORT_PLY, GS_EXPORT_PLY_COMPRESSED = 0, 1, 2
+GS_EXPORT_SPZ = 4
 
 
 class GsStats(C.Structure):

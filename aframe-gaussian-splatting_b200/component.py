@@ -197,6 +197,8 @@ class GaussianSplattingComponent:
             is_ply = str(src).endswith(".ply")  # index.js:257
             with open(os.fspath(src), "rb") as f:
                 buf = np.frombuffer(f.read(), dtype=np.uint8)
+            if str(src).endswith(".spz"):  # gunzipped on the host, then decoded on the device like a PLY (gs_push_ply)
+                buf, is_ply = np.frombuffer(_ply.read_spz(buf), dtype=np.uint8), True
         if is_ply:
             # index.js:315-324: the whole file is converted (processPlyBuffer) and its rows pushed at once.  The device
             # decodes, importance-sorts and packs it (gs_push_ply); the table is sized from the header's vertex count,
@@ -483,8 +485,8 @@ class SplatScene:
         return kept
 
     def save(self, component: GaussianSplattingComponent, path=None, format: str = "splat") -> bytes:
-        """Write the entity's splats out as one file (gs_export of its range): format "splat", "ply" or
-        "compressed_ply".  Returns the bytes, and also writes them to `path` when given.  Needs keep_rows=True."""
+        """Write the entity's splats out as one file (gs_export of its range): format "splat", "ply", "compressed_ply"
+        or "spz" (gzipped, as an .spz file is stored).  Returns the bytes, and also writes them to `path` when given.  Needs keep_rows=True."""
         first, count = self._range[id(component)]
         blob = self.renderer.export(first, count, format)
         if path is not None:

@@ -814,16 +814,19 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   if (out_n) *out_n = 0;
   PlyLayout L{};
   PlyCompressedLayout Z{};  // a compressed PLY (ply_is_compressed): decoded by k_ply_decode_compressed
+  PlySpzLayout P{};         // an .spz stream (ply_is_spz): decoded by k_ply_decode_spz
   PlyShLayout S{};
   S.ctx_k = sh_coeffs(c->sh_degree);
   S.vecs = c->sh_vecs;
   PlyShLayout *sh = c->sh_degree ? &S : nullptr;
   uint32_t n = 0;
   size_t data_off = 0;
-  const bool compressed = ply_is_compressed((const uint8_t *)ply, bytes);
-  if (compressed ? ply_parse_compressed((const uint8_t *)ply, bytes, Z, n, c->err)
-                 : ply_parse((const uint8_t *)ply, bytes, L, n, data_off, c->err, sh))
-    return GS_ERR_INVALID;  // nothing changed yet
+  const bool spz = ply_is_spz((const uint8_t *)ply, bytes);
+  const bool compressed = !spz && ply_is_compressed((const uint8_t *)ply, bytes);
+  const int parsed = spz          ? ply_parse_spz((const uint8_t *)ply, bytes, P, n, c->err)
+                     : compressed ? ply_parse_compressed((const uint8_t *)ply, bytes, Z, n, c->err)
+                                  : ply_parse((const uint8_t *)ply, bytes, L, n, data_off, c->err, sh);
+  if (parsed) return parsed;  // nothing changed yet
   if (!n) return GS_OK;
   GS_CUDA(c, cudaSetDevice(c->device));
   int rc;
@@ -835,11 +838,14 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   cudaStream_t st = c->push_stream;
   // temporaries, stream-ordered: decoded rows (32 B) + key per row, two permutations, radix tables, ordered rows
   const uint32_t chunks = (n + kRadixTile - 1) / kRadixTile;
-  // a compressed piece: whole chunks of rows (ply_stage_compressed); sh_k: its SH bytes per splat / 3
-  const uint32_t sh_k = sh ? Z.file_k : 0u;
+  // a compressed piece: whole chunks of rows (ply_stage_compressed); an .spz piece: each section's slice of its rows
+  // (ply_stage_spz); sh_k: their SH bytes per splat / 3
+  const uint32_t sh_k = sh ? (spz ? P.file_k : Z.file_k) : 0u;
   const size_t stride = L.stride;
-  const size_t rows_per_chunk = compressed ? ply_compressed_piece_rows(sh_k) : gs_context::kPlyChunkBytes / stride;
-  const size_t body_bytes = compressed ? gs_context::kPlyChunkBytes : rows_per_chunk * stride;
+  const size_t rows_per_chunk = spz          ? ply_spz_piece_rows(P, sh_k)
+                                : compressed ? ply_compressed_piece_rows(sh_k)
+                                             : gs_context::kPlyChunkBytes / stride;
+  const size_t body_bytes = compressed || spz ? gs_context::kPlyChunkBytes : rows_per_chunk * stride;
   uint8_t *rows_dev = nullptr, *out_dev = nullptr, *body[2] = {nullptr, nullptr};
   uint32_t *key = nullptr, *perm_a = nullptr, *perm_b = nullptr, *table = nullptr, *totals = nullptr;
   uint4 *sh_dev = nullptr;  // SH contexts: the decoded coefficients, in file order
@@ -849,7 +855,7 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
       if (p) cudaFreeAsync(p, st);
   };
   cudaError_t e = cudaSuccess;
-  const bool sort = (compressed || L.has_scale) && n > 1;  // without scale_0 every key is 0: the stable sort is the identity
+  const bool sort = (compressed || spz || L.has_scale) && n > 1;  // without scale_0 every key is 0: the stable sort is the identity
   e = cudaMallocAsync((void **)&rows_dev, (size_t)n * 32, st);
   if (!e) e = cudaMallocAsync((void **)&key, (size_t)n * 4, st);
   for (int i = 0; i < 2 && !e; ++i) e = cudaMallocAsync((void **)&body[i], body_bytes, st);
@@ -871,15 +877,21 @@ static int insert_ply(gs_context *c, uint32_t at, const void *ply, size_t bytes,
   for (uint32_t r0 = 0, k = 0; r0 < n && !e; r0 += (uint32_t)rows_per_chunk, ++k) {
     const uint32_t m = (uint32_t)std::min<size_t>(rows_per_chunk, n - r0);
     const int b = (int)(k & 1u);
-    const size_t piece = compressed ? ply_compressed_piece_bytes(m, sh_k) : (size_t)m * stride;
+    const size_t piece = spz          ? ply_spz_piece_bytes(P, m, sh_k)
+                         : compressed ? ply_compressed_piece_bytes(m, sh_k)
+                                      : (size_t)m * stride;
     if ((e = cudaEventSynchronize(c->ply_ev[b]))) break;  // this pinned buffer's previous chunk is on the device
-    if (compressed)
+    if (spz)
+      ply_stage_spz((const uint8_t *)ply, P, sh_k, r0, m, (uint8_t *)c->ply_pinned[b]);
+    else if (compressed)
       ply_stage_compressed((const uint8_t *)ply, Z, sh_k, r0, m, (uint8_t *)c->ply_pinned[b]);
     else
       memcpy(c->ply_pinned[b], src + (size_t)r0 * stride, piece);
     if ((e = cudaMemcpyAsync(body[b], c->ply_pinned[b], piece, cudaMemcpyHostToDevice, st))) break;
     if ((e = cudaEventRecord(c->ply_ev[b], st))) break;
-    if (compressed)
+    if (spz)
+      launch_ply_decode_spz(body[b], m, P, r0, rows_dev, key, sh, sh_dev, st);
+    else if (compressed)
       launch_ply_decode_compressed(body[b], m, Z, r0, rows_dev, key, sh, sh_dev, st);
     else
       launch_ply_decode(body[b], m, L, r0, rows_dev, key, sh, sh_dev, st);
@@ -981,19 +993,54 @@ static std::string export_header(uint32_t format, uint32_t n, uint32_t k) {
 
 static size_t export_body_bytes(uint32_t format, uint32_t n, uint32_t k) {
   if (format == GS_EXPORT_SPLAT) return (size_t)n * 32;
+  if (format == GS_EXPORT_SPZ) return (size_t)n * (20 + 3 * (size_t)k);
   if (format == GS_EXPORT_PLY) return (size_t)n * 4 * (14 + 3 * (size_t)k);
   return ((size_t)n + 255) / 256 * 72 + (size_t)n * (16 + 3 * (size_t)k);
 }
+
+static bool export_format_known(uint32_t format) {
+  return format == GS_EXPORT_SPLAT || format == GS_EXPORT_PLY || format == GS_EXPORT_PLY_COMPRESSED || format == GS_EXPORT_SPZ;
+}
+
+// GS_EXPORT_SPZ's 16 B header (the bytes ahead of the body)
+static std::string spz_header(uint32_t n, uint32_t degree, uint32_t fb) {
+  uint8_t h[16] = {'N', 'G', 'S', 'P', 3, 0, 0, 0, 0, 0, 0, 0, (uint8_t)degree, (uint8_t)fb, 0, 0};
+  memcpy(h + 8, &n, 4);
+  return std::string((const char *)h, 16);
+}
+
+// GS_EXPORT_SPZ's body of n rows laid out as the kept rows and SH rows: the device max-reduction of the finite
+// coordinates (into bound, 4 B of device memory) fixes fb, then k_export_spz writes the body.  fb = -1: a position is too
+// large for 24-bit fixed point, and nothing was written.
+static cudaError_t export_spz(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, uint32_t *bound, uint8_t *body,
+                              int &fb, cudaStream_t st) {
+  uint32_t host_bound = 0;
+  cudaError_t e = cudaMemsetAsync(bound, 0, 4, st);
+  if (!e) {
+    launch_export_spz_bound(rows, n, bound, st);
+    e = cudaGetLastError();
+  }
+  if (!e) e = cudaMemcpyAsync(&host_bound, bound, 4, cudaMemcpyDeviceToHost, st);
+  if (!e) e = cudaStreamSynchronize(st);
+  fb = e ? -1 : spz_fraction_bits(host_bound);
+  if (e || fb < 0) return e;
+  launch_export_spz_rows(rows, sh, degree, n, (uint32_t)fb, body, st);
+  return cudaGetLastError();
+}
+
+static const char *const kSpzTooLarge = "spz: a position too large for 24-bit fixed point";
 
 extern "C" int gs_export(gs_context *c, uint32_t first, uint32_t count, uint32_t format, void *out, size_t cap,
                          size_t *out_bytes) {
   if (!c) return GS_ERR_INVALID;
   if (!out_bytes) return fail(c, GS_ERR_INVALID, "gs_export: out_bytes is NULL");
   *out_bytes = 0;
-  if (format != GS_EXPORT_SPLAT && format != GS_EXPORT_PLY && format != GS_EXPORT_PLY_COMPRESSED)
-    return fail(c, GS_ERR_INVALID, "gs_export: unknown format");
+  if (!export_format_known(format)) return fail(c, GS_ERR_INVALID, "gs_export: unknown format");
   const uint32_t k = sh_coeffs(c->sh_degree);
-  const std::string head = format == GS_EXPORT_SPLAT ? std::string() : export_header(format, count, k);
+  // the .spz header's fb is known once the body is; an empty range takes 12
+  std::string head = format == GS_EXPORT_SPLAT ? std::string()
+                     : format == GS_EXPORT_SPZ ? spz_header(count, c->sh_degree, 12)
+                                               : export_header(format, count, k);
   const size_t body = export_body_bytes(format, count, k), total = head.size() + body;
   *out_bytes = total;
   if (!c->keep_rows) return fail(c, GS_ERR_INVALID, "gs_export: the context keeps no .splat rows (gs_set_keep_rows)");
@@ -1008,17 +1055,30 @@ extern "C" int gs_export(gs_context *c, uint32_t first, uint32_t count, uint32_t
     GS_CUDA(c, cudaStreamSynchronize(st));
   } else if (count) {
     uint8_t *tmp = nullptr;
-    cudaError_t e = cudaMallocAsync((void **)&tmp, body, st);
+    cudaError_t e = cudaMallocAsync((void **)&tmp, body + (format == GS_EXPORT_SPZ ? 16 : 0), st);
     if (e) {
       cudaGetLastError();  // an allocation failure is not sticky
       GS_CUDA(c, e);
     }
-    if (format == GS_EXPORT_PLY)
-      launch_export_ply(c, first, count, tmp, st);
-    else
-      launch_export_compressed(c, first, count, tmp, st);
-    e = cudaGetLastError();
-    if (!e) e = cudaMemcpyAsync(dst, tmp, body, cudaMemcpyDeviceToHost, st);
+    uint8_t *src = tmp;
+    if (format == GS_EXPORT_SPZ) {  // the bound word first, the body behind it
+      int fb = -1;
+      src = tmp + 16;
+      e = export_spz(c->keep + 2 * (size_t)first, c->sh ? c->sh + (size_t)first * c->sh_vecs : nullptr, c->sh_degree,
+                     count, (uint32_t *)tmp, src, fb, st);
+      if (!e && fb < 0) {
+        cudaFreeAsync(tmp, st);
+        return fail(c, GS_ERR_INVALID, kSpzTooLarge);
+      }
+      head = spz_header(count, c->sh_degree, (uint32_t)fb);
+    } else {
+      if (format == GS_EXPORT_PLY)
+        launch_export_ply(c, first, count, tmp, st);
+      else
+        launch_export_compressed(c, first, count, tmp, st);
+      e = cudaGetLastError();
+    }
+    if (!e) e = cudaMemcpyAsync(dst, src, body, cudaMemcpyDeviceToHost, st);
     cudaFreeAsync(tmp, st);
     if (!e) e = cudaStreamSynchronize(st);
     GS_CUDA(c, e);
@@ -1048,10 +1108,11 @@ extern "C" int gs_export_parts(gs_context *c, const gs_export_part *parts, uint3
   }
   if (total_rows > 0xFFFFFFFFull) return fail(c, GS_ERR_INVALID, "gs_export_parts: more than 2^32 - 1 rows");
   const uint32_t n = (uint32_t)total_rows;
-  if (format != GS_EXPORT_SPLAT && format != GS_EXPORT_PLY && format != GS_EXPORT_PLY_COMPRESSED)
-    return fail(c, GS_ERR_INVALID, "gs_export_parts: unknown format");
+  if (!export_format_known(format)) return fail(c, GS_ERR_INVALID, "gs_export_parts: unknown format");
   const uint32_t k = sh_coeffs(c->sh_degree);
-  const std::string head = format == GS_EXPORT_SPLAT ? std::string() : export_header(format, n, k);
+  std::string head = format == GS_EXPORT_SPLAT ? std::string()
+                     : format == GS_EXPORT_SPZ ? spz_header(n, c->sh_degree, 12)
+                                               : export_header(format, n, k);
   const size_t body = export_body_bytes(format, n, k), total = head.size() + body;
   *out_bytes = total;
   if (!c->keep_rows) return fail(c, GS_ERR_INVALID, "gs_export_parts: the context keeps no .splat rows (gs_set_keep_rows)");
@@ -1063,7 +1124,8 @@ extern "C" int gs_export_parts(gs_context *c, const gs_export_part *parts, uint3
   if (n) {
     const size_t row_bytes = (size_t)n * 32, sh_bytes = (size_t)n * 16 * c->sh_vecs;
     uint8_t *tmp = nullptr;
-    cudaError_t e = cudaMallocAsync((void **)&tmp, row_bytes + sh_bytes + (format == GS_EXPORT_SPLAT ? 0 : body), st);
+    const size_t extra = format == GS_EXPORT_SPLAT ? 0 : format == GS_EXPORT_SPZ ? 16 + body : body;  // .spz: bound word, body
+    cudaError_t e = cudaMallocAsync((void **)&tmp, row_bytes + sh_bytes + extra, st);
     if (e) {
       cudaGetLastError();  // an allocation failure is not sticky
       GS_CUDA(c, e);
@@ -1089,7 +1151,16 @@ extern "C" int gs_export_parts(gs_context *c, const gs_export_part *parts, uint3
       at += pt.count;
     }
     uint8_t *src = tmp;  // .splat: the transformed rows are the body
-    if (!e && format != GS_EXPORT_SPLAT) {
+    if (!e && format == GS_EXPORT_SPZ) {  // positions after the part transforms fix fb
+      int fb = -1;
+      src = tmp + row_bytes + sh_bytes + 16;
+      e = export_spz(rows, sh, c->sh_degree, n, (uint32_t *)(tmp + row_bytes + sh_bytes), src, fb, st);
+      if (!e && fb < 0) {
+        cudaFreeAsync(tmp, st);
+        return fail(c, GS_ERR_INVALID, kSpzTooLarge);
+      }
+      head = spz_header(n, c->sh_degree, (uint32_t)fb);
+    } else if (!e && format != GS_EXPORT_SPLAT) {
       src = tmp + row_bytes + sh_bytes;
       if (format == GS_EXPORT_PLY)
         launch_export_ply_rows(rows, sh, c->sh_degree, n, src, st);

@@ -259,6 +259,26 @@ size_t ply_compressed_piece_bytes(uint32_t m, uint32_t sh_k);
 // Stages rows [r0, r0 + m) of the file (r0 a multiple of 256) as one piece at dst
 void ply_stage_compressed(const uint8_t *ply, const PlyCompressedLayout &Z, uint32_t sh_k, uint32_t r0, uint32_t m,
                           uint8_t *dst);
+// ---- .spz stream (inflated; include/gsplat_b200.h, ".spz streams"): a 16 B header, then six column sections of N
+// splats: positions (9 B), alphas (1 B), colours (3 B), scales (3 B), rotations (3 B in version 2, 4 B in version 3), SH
+// (3 K B).  A piece of rows [r0, r0 + m) is staged as each section's slice back to back, each padded to 16 B ----
+constexpr int kSpzSections = 6;
+struct PlySpzLayout {
+  uint64_t sec[kSpzSections];   // stream offsets of the sections
+  uint32_t width[kSpzSections];  // their bytes per splat
+  uint32_t version, file_k, fb;  // version 2 or 3; K of the file's SH degree; fractional bits of the positions
+};
+// Whether the buffer is an .spz stream: it starts with "NGSP" and its 10 KB window holds no "end_header\n" (so no buffer
+// ply_parse or ply_parse_compressed accepts is one)
+bool ply_is_spz(const uint8_t *ply, size_t bytes);
+// Parses the header of a stream ply_is_spz accepted.  Returns GS_OK with the layout and splat count, GS_ERR_CAPACITY above
+// 2^31 - 1 splats, or GS_ERR_INVALID with `err` ("spz: ...").
+int ply_parse_spz(const uint8_t *ply, size_t bytes, PlySpzLayout &P, uint32_t &n, std::string &err);
+// Rows per staged piece and the bytes of a piece of m rows; sh_k: SH bytes per splat / 3 staged (0 = none)
+uint32_t ply_spz_piece_rows(const PlySpzLayout &P, uint32_t sh_k);
+size_t ply_spz_piece_bytes(const PlySpzLayout &P, uint32_t m, uint32_t sh_k);
+// Stages rows [r0, r0 + m) of the stream as one piece at dst: one memcpy per section
+void ply_stage_spz(const uint8_t *ply, const PlySpzLayout &P, uint32_t sh_k, uint32_t r0, uint32_t m, uint8_t *dst);
 
 // ---- front-to-back slab path ----
 constexpr int kMaxSlabs = 12;         // geometric slab sizes: 1 M, 2 M, 4 M ... entries (nearest first)
@@ -669,6 +689,13 @@ void launch_export_compressed(gs_context *c, uint32_t first, uint32_t n, uint8_t
 void launch_export_ply_rows(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, uint8_t *body, cudaStream_t st);
 void launch_export_compressed_rows(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, uint8_t *body,
                                    cudaStream_t st);
+// GS_EXPORT_SPZ over such rows: k_export_spz_bound atomically raises *bound (zeroed by the caller) to the largest f32 bit
+// pattern of a finite |coordinate|; spz_fraction_bits turns it into the stream's fractional bits (-1: refused); then
+// k_export_spz writes the six sections of an .spz body (n (20 + 3 K) bytes, version 3)
+void launch_export_spz_bound(const uint4 *rows, uint32_t n, uint32_t *bound, cudaStream_t st);
+int spz_fraction_bits(uint32_t bound);
+void launch_export_spz_rows(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, uint32_t fb, uint8_t *body,
+                            cudaStream_t st);
 // gs_export_parts (gs_transform.cu): one part's transform, as k_transform_rows takes it (include/gsplat_b200.h)
 struct TransformConsts {
   double L[9];        // the upper 3x3, row-major
@@ -695,6 +722,9 @@ void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, 
 // compressed PLY push: the same for a staged piece of `rows` rows (ply_stage_compressed with sh_k = sh ? file_k : 0)
 void launch_ply_decode_compressed(const uint8_t *piece, uint32_t rows, const PlyCompressedLayout &Z, uint32_t first_row,
                                   uint8_t *rows32, uint32_t *key, const PlyShLayout *sh, uint4 *sh_rows, cudaStream_t st);
+// .spz push: the same for a staged piece of `rows` rows (ply_stage_spz with sh_k = sh ? file_k : 0)
+void launch_ply_decode_spz(const uint8_t *piece, uint32_t rows, const PlySpzLayout &P, uint32_t first_row, uint8_t *rows32,
+                           uint32_t *key, const PlyShLayout *sh, uint4 *sh_rows, cudaStream_t st);
 // PLY push: stable ascending sort of n 32-bit keys as four 8-bit passes (12 launches); returns the buffer holding the
 // permutation (perm_b).  table: 256 * (ceil(n / kRadixTile) + 1) words, totals: 256 words.
 uint32_t *launch_ply_sort(gs_context *c, const uint32_t *key, uint32_t *perm_a, uint32_t *perm_b, uint32_t *table,

@@ -3,9 +3,16 @@
 //   k_export_compressed : one CTA per 256-row chunk counted from the range's first row: each thread restates its row in
 //                         registers, block reductions give the chunk's nine fp64 (min, max) pairs, then the chunk row, the
 //                         four 16 B vertex words and the SH bytes are stored (the SH bytes staged in shared memory)
+//   k_export_spz_bound  : the largest finite |coordinate| of the rows (one atomic max per warp), which fixes the .spz
+//                         stream's fractional bits on the host (spz_fraction_bits)
+//   k_export_spz        : one row per thread: the row's bytes in the six column sections of an .spz body (version 3)
 // A .splat export needs no kernel: the kept rows are its body.  The rules are gs_export's (include/gsplat_b200.h); every
 // fp64 operation is written out and the library builds with --fmad=false, so nothing is contracted.
 #include <cuda_fp16.h>
+#include <string.h>
+
+#include <algorithm>
+#include <cmath>
 
 #include "gs_common.cuh"
 
@@ -222,6 +229,132 @@ __global__ void __launch_bounds__(256) k_export_compressed(const uint4 *__restri
     uint8_t *dst = body + (size_t)nch * 72 + (size_t)n * 16 + (size_t)blockIdx.x * 256 * 3 * K;
     for (uint32_t b = tid; b < nb; b += 256) dst[b] = s_sh[b];
   }
+}
+
+// ---- GS_EXPORT_SPZ (include/gsplat_b200.h, ".spz streams"): the spz writer's quantisation of the restated row ----
+// The largest f32 bit pattern of a finite |coordinate| (order-preserving for non-negative floats); 0 without one
+__global__ void __launch_bounds__(256) k_export_spz_bound(const uint4 *__restrict__ rows, uint32_t n,
+                                                          uint32_t *__restrict__ bound) {
+  uint32_t m = 0u;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint4 a = __ldg(rows + 2 * (size_t)i);
+    const uint32_t x = a.x & 0x7FFFFFFFu, y = a.y & 0x7FFFFFFFu, z = a.z & 0x7FFFFFFFu;
+    m = max(m, x < 0x7F800000u ? x : 0u);
+    m = max(m, y < 0x7F800000u ? y : 0u);
+    m = max(m, z < 0x7F800000u ? z : 0u);
+  }
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31u) == 0u && m) atomicMax(bound, m);
+}
+
+// q8(v) = clamp(floor(v + 0.5), 0, 255), NaN -> 0
+__device__ __forceinline__ uint32_t spz_q8(double v) {
+  const double f = floor(v + 0.5);
+  if (!(f > 0.0)) return 0u;  // NaN, <= 0
+  return f >= 255.0 ? 255u : (uint32_t)f;
+}
+
+// a position: the 24-bit two's complement of lround(x 2^fb) (half away from zero); a coordinate that is not finite is 0
+__device__ __forceinline__ uint32_t spz_fixed(uint32_t bits, double unit) {
+  const float x = __uint_as_float(bits);
+  if (!isfinite(x)) return 0u;
+  return (uint32_t)(int32_t)round((double)x * unit) & 0xFFFFFFu;
+}
+
+// smallest three of the restated rot_0..3 (w, x, y, z), normalised in fp64; the zero quaternion is the identity
+__device__ __forceinline__ uint32_t spz_rotation_word(const uint32_t rot[4]) {
+  const double w = __uint_as_float(rot[0]);
+  double q[4] = {__uint_as_float(rot[1]), __uint_as_float(rot[2]), __uint_as_float(rot[3]), w};  // x, y, z, w
+  const double nrm = sqrt(((w * w + q[0] * q[0]) + q[1] * q[1]) + q[2] * q[2]);
+  if (nrm == 0.0) return 3u << 30;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) q[k] = q[k] / nrm;
+  uint32_t big = 0;
+  double qb = q[0];
+#pragma unroll
+  for (uint32_t k = 1; k < 4; ++k)
+    if (fabs(q[k]) > fabs(qb)) {  // the first one on ties
+      big = k;
+      qb = q[k];
+    }
+  const double sign = qb < 0.0 ? -1.0 : 1.0;  // the largest is made positive
+  uint32_t word = big << 30, shift = 20;
+#pragma unroll
+  for (uint32_t k = 0; k < 4; ++k) {
+    if (k == big) continue;
+    const double v = sign * q[k];
+    const double m = floor(511.0 * fabs(v) / sqrt(0.5) + 0.5);
+    word |= ((v < 0.0 ? 512u : 0u) | (m >= 511.0 ? 511u : (uint32_t)m)) << shift;
+    shift -= 10;
+  }
+  return word;
+}
+
+// an SH byte: lround(f 128) + 128 in the writer's buckets (8 for a channel's first three coefficients, else 16), clamped
+// to [0, 255]; NaN -> 128
+__device__ __forceinline__ uint32_t spz_sh_byte(uint32_t bits, uint32_t j) {
+  const double f = (double)__uint_as_float(bits);
+  if (isnan(f)) return 128u;
+  const double b = j < 3 ? 8.0 : 16.0;
+  const double q = floor((round(f * 128.0) + 128.0 + b / 2.0) / b) * b;
+  return q <= 0.0 ? 0u : q >= 255.0 ? 255u : (uint32_t)q;
+}
+
+template <uint32_t K>
+__global__ void __launch_bounds__(256) k_export_spz(const uint4 *__restrict__ rows, const uint4 *__restrict__ sh,
+                                                    uint32_t sh_vecs, uint32_t n, uint32_t fb, uint8_t *__restrict__ body) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const ExportRow r = export_row(__ldg(rows + 2 * (size_t)i), __ldg(rows + 2 * (size_t)i + 1));
+  const double unit = ldexp(1.0, (int)fb);
+  uint8_t *pos = body + (size_t)i * 9, *alpha = body + (size_t)n * 9 + i, *col = body + (size_t)n * 10 + (size_t)i * 3;
+  uint8_t *scale = body + (size_t)n * 13 + (size_t)i * 3, *rot = body + (size_t)n * 16 + (size_t)i * 4;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const uint32_t p = spz_fixed(r.pos[k], unit);
+    pos[3 * k] = (uint8_t)p;
+    pos[3 * k + 1] = (uint8_t)(p >> 8);
+    pos[3 * k + 2] = (uint8_t)(p >> 16);
+    col[k] = (uint8_t)spz_q8((double)__uint_as_float(r.dc[k]) * 0.15 * 255.0 + 127.5);
+    scale[k] = (uint8_t)spz_q8(((double)__uint_as_float(r.scale[k]) + 10.0) * 16.0);
+  }
+  alpha[0] = (uint8_t)spz_q8(1.0 / (1.0 + exp(-(double)__uint_as_float(r.opacity))) * 255.0);
+  const uint32_t word = spz_rotation_word(r.rot);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) rot[k] = (uint8_t)(word >> (8 * k));
+  if constexpr (K > 0) {
+    const uint32_t *halves = (const uint32_t *)(sh + (size_t)i * sh_vecs);
+    uint8_t *o = body + (size_t)n * 20 + (size_t)i * 3 * K;
+#pragma unroll
+    for (uint32_t j = 0; j < K; ++j)
+#pragma unroll
+      for (uint32_t ch = 0; ch < 3; ++ch) o[3 * j + ch] = (uint8_t)spz_sh_byte(export_rest(halves, ch * K + j), j);
+  }
+}
+
+int spz_fraction_bits(uint32_t bound) {
+  double m;
+  {
+    float f;
+    memcpy(&f, &bound, 4);
+    m = (double)f;
+  }
+  for (int f = 12; f >= 0; --f)
+    if (m * std::ldexp(1.0, f) < 8388607.5) return f;  // lround(m 2^f) <= 2^23 - 1
+  return -1;
+}
+
+void launch_export_spz_bound(const uint4 *rows, uint32_t n, uint32_t *bound, cudaStream_t st) {
+  const uint32_t grid = std::min<uint32_t>((n + 255) / 256, 1024u);
+  if (grid) k_export_spz_bound<<<grid, 256, 0, st>>>(rows, n, bound);
+}
+
+void launch_export_spz_rows(const uint4 *rows, const uint4 *sh, uint32_t degree, uint32_t n, uint32_t fb, uint8_t *body,
+                            cudaStream_t st) {
+  const uint32_t grid = (n + 255) / 256;
+  if (!grid) return;
+  auto kernel = degree == 0 ? k_export_spz<0> : degree == 1 ? k_export_spz<3> : degree == 2 ? k_export_spz<8> : k_export_spz<15>;
+  kernel<<<grid, 256, 0, st>>>(rows, sh, sh_vecs(degree), n, fb, body);
 }
 
 static const uint4 *kept_rows(gs_context *c, uint32_t first) { return c->keep + 2 * (size_t)first; }

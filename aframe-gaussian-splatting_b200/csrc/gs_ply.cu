@@ -13,6 +13,9 @@
 //   ply_stage_compressed stages whole chunks of rows as [chunk bounds | 16 B packed words | SH bytes], and
 //   k_ply_decode_compressed<kSH> (one CTA of 256 threads per chunk) forms each property in fp64, rounds it once to f32
 //   and runs the row conversion k_ply_decode runs (ply_convert_row): the rows of the file's float restatement.
+//   .spz streams (inflated; ply_is_spz): ply_parse_spz checks the 16 B header, ply_stage_spz stages each of the six
+//   column sections' slice of a piece (padded to 16 B), and k_ply_decode_spz<kSH, kV3> (one CTA per 256 rows) forms each
+//   property in fp64 from its bytes, rounds it once to f32 and runs ply_convert_row likewise.
 //
 // Numerics: fp64 as JavaScript evaluates it, no contraction (the library is built with --fmad=false).  The importance
 // product runs left to right and is rounded to f32 (Float32Array store); the key is the complement of the order-preserving
@@ -349,6 +352,66 @@ void ply_stage_compressed(const uint8_t *ply, const PlyCompressedLayout &Z, uint
   }
 }
 
+// ---- .spz stream (inflated): a 16 B header and six column sections ----
+bool ply_is_spz(const uint8_t *ply, size_t bytes) {
+  if (bytes < 4 || memcmp(ply, "NGSP", 4) != 0) return false;
+  const std::string head((const char *)ply, bytes < 10240 ? bytes : 10240);
+  return head.find("end_header\n") == std::string::npos;  // such a buffer is a PLY to ply_parse's rules
+}
+
+int ply_parse_spz(const uint8_t *ply, size_t bytes, PlySpzLayout &P, uint32_t &n, std::string &err) {
+  memset(&P, 0, sizeof(P));
+  n = 0;
+  auto refuse = [&](const std::string &m) { err = "spz: " + m; return GS_ERR_INVALID; };
+  if (bytes < 16) return refuse("stream shorter than its header");
+  uint32_t h[3];
+  memcpy(h, ply, 12);  // magic, version, N (little-endian)
+  const uint32_t degree = ply[12], fb = ply[13];  // ply[14] (flags) and ply[15] (reserved) are not read
+  if (h[1] != 2 && h[1] != 3) return refuse("version " + std::to_string(h[1]) + " is not 2 or 3");
+  if (degree > 3) return refuse("sh_degree " + std::to_string(degree) + " is above 3");
+  if (fb > 31) return refuse("fractional_bits " + std::to_string(fb) + " is above 31");
+  if (h[2] > 0x7FFFFFFFu) { err = "more than 2^31-1 splats"; return GS_ERR_CAPACITY; }
+  P.version = h[1];
+  P.file_k = sh_coeffs(degree);
+  P.fb = fb;
+  const uint32_t width[kSpzSections] = {9, 1, 3, 3, P.version == 3 ? 4u : 3u, 3 * P.file_k};
+  uint64_t off = 16;
+  for (int s = 0; s < kSpzSections; ++s) {
+    P.sec[s] = off;
+    P.width[s] = width[s];
+    off += (uint64_t)h[2] * width[s];
+  }
+  if (off > bytes) return refuse("body shorter than its N splats");  // trailing bytes are ignored
+  n = h[2];
+  return GS_OK;
+}
+
+// the bytes per splat of staged section s (the SH section only as far as the context reads it)
+static uint32_t spz_staged_width(const PlySpzLayout &P, int s, uint32_t sh_k) {
+  return s == kSpzSections - 1 ? 3 * sh_k : P.width[s];
+}
+
+uint32_t ply_spz_piece_rows(const PlySpzLayout &P, uint32_t sh_k) {
+  size_t per_row = 0;
+  for (int s = 0; s < kSpzSections; ++s) per_row += spz_staged_width(P, s, sh_k);
+  return (uint32_t)((gs_context::kPlyChunkBytes - 16 * kSpzSections) / per_row) & ~255u;  // 16 B of padding per section
+}
+
+size_t ply_spz_piece_bytes(const PlySpzLayout &P, uint32_t m, uint32_t sh_k) {
+  size_t b = 0;
+  for (int s = 0; s < kSpzSections; ++s) b += ((size_t)m * spz_staged_width(P, s, sh_k) + 15) & ~(size_t)15;
+  return b;
+}
+
+void ply_stage_spz(const uint8_t *ply, const PlySpzLayout &P, uint32_t sh_k, uint32_t r0, uint32_t m, uint8_t *dst) {
+  for (int s = 0; s < kSpzSections; ++s) {
+    const uint32_t w = spz_staged_width(P, s, sh_k);
+    const size_t b = (size_t)m * w;
+    memcpy(dst, ply + P.sec[s] + (size_t)r0 * P.width[s], b);
+    dst += (b + 15) & ~(size_t)15;
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // decode (device)
 // ---------------------------------------------------------------------------------------------
@@ -558,6 +621,92 @@ __global__ void __launch_bounds__(256) k_ply_decode_compressed(const uint8_t *__
   ply_convert_row([&](int k) { return v[k]; }, pos[0], pos[1], pos[2], true, true, true, first_row + i, rows32, key_out);
 }
 
+// ---- .spz: each property in fp64 from its bytes, rounded once to f32, then the conversion above (include/gsplat_b200.h,
+// ".spz streams") ----
+// One CTA per 256 rows of a staged piece.  The byte columns are 9-, 3- and 4-byte strided, so the CTA first copies its
+// slice of every section into shared memory with 16 B loads (each slice starts 16 B aligned: 256 w is a multiple of 16,
+// and the piece pads every section to 16 B).
+template <bool kSH, bool kV3>
+__global__ void __launch_bounds__(256) k_ply_decode_spz(const uint8_t *__restrict__ piece, uint32_t rows, uint32_t file_k,
+                                                        uint32_t fb, uint32_t first_row, uint4 *__restrict__ rows32,
+                                                        uint32_t *__restrict__ key_out, const PlyShLayout S,
+                                                        uint4 *__restrict__ sh_rows) {
+  constexpr uint32_t kRot = kV3 ? 4 : 3;
+  constexpr uint32_t kWidth[kSpzSections - 1] = {9, 1, 3, 3, kRot};
+  constexpr uint32_t kFixed = 9 + 1 + 3 + 3 + kRot;
+  __shared__ uint4 s_buf[256 * (kFixed + (kSH ? 3 * kMaxShCoeffs : 0)) / 16];
+  const uint32_t base = blockIdx.x * 256, i = base + threadIdx.x, here = min(256u, rows - base);
+  const uint32_t nb = kSH ? 3 * file_k : 0u;
+  const uint8_t *src = piece;
+  uint8_t *const s = (uint8_t *)s_buf;
+  uint32_t s_off = 0;
+#pragma unroll
+  for (int k = 0; k < kSpzSections; ++k) {
+    const uint32_t w = k < kSpzSections - 1 ? kWidth[k] : nb;
+    const uint4 *from = (const uint4 *)(src + (size_t)base * w);
+    uint4 *to = (uint4 *)(s + s_off);
+    const uint32_t nvec = (here * w + 15) / 16;
+    for (uint32_t v = threadIdx.x; v < nvec; v += 256) to[v] = __ldg(from + v);
+    src += ((size_t)rows * w + 15) & ~(size_t)15;
+    s_off += 256 * w;
+  }
+  __syncthreads();
+  if (i >= rows) return;
+  const uint32_t t = threadIdx.x;
+  const uint8_t *p = s + t * 9, *a = s + 256 * 9 + t, *c = s + 256 * 10 + t * 3, *sc = s + 256 * 13 + t * 3;
+  const uint8_t *r = s + 256 * 16 + t * kRot;
+  if (kSH) {
+    const uint8_t *u = s + 256 * kFixed + t * nb;  // coefficient j of channel ch at byte 3 j + ch
+    ply_store_sh([&](uint32_t h) {
+      const uint32_t ch = h / S.ctx_k, j = h - ch * S.ctx_k;
+      if (j >= file_k) return 0u;
+      return (uint32_t)__half_as_ushort(__float2half_rn(__double2float_rn(((double)u[3 * j + ch] - 128.0) / 128.0)));
+    }, S, first_row + i, sh_rows);
+  }
+  // positions: 24-bit two's complement, times 2^-fb (exact in f32)
+  const double unit = ldexp(1.0, -(int)fb);
+  uint32_t pos[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const int32_t q = (int32_t)(((uint32_t)p[3 * k] | ((uint32_t)p[3 * k + 1] << 8) | ((uint32_t)p[3 * k + 2] << 16)) << 8) >> 8;
+    pos[k] = f32_bits((double)q * unit);
+  }
+  double v[PF_COUNT];
+  v[PF_OP] = ply_f32(-log(1.0 / ((double)a[0] / 255.0) - 1.0));
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    v[PF_DC0 + k] = ply_f32(((double)c[k] / 255.0 - 0.5) / 0.15);
+    v[PF_S0 + k] = ply_f32((double)sc[k] / 16.0 - 10.0);
+  }
+  double q[4];  // x, y, z, w
+  if (kV3) {  // smallest three: the top 2 bits name the largest; the others, highest index first from the low bits
+    uint32_t word = (uint32_t)r[0] | ((uint32_t)r[1] << 8) | ((uint32_t)r[2] << 16) | ((uint32_t)r[3] << 24);
+    const uint32_t big = word >> 30;
+#pragma unroll
+    for (int k = 3; k >= 0; --k) {  // q[big] is replaced below, and takes no bits
+      const double m = sqrt(0.5) * (double)(word & 511u) / 511.0;
+      q[k] = (word & 512u) ? -m : m;
+      if ((uint32_t)k != big) word >>= 10;
+    }
+    double sum = 0.0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)  // the sum in ascending index order (adding +0 for the largest changes nothing)
+      sum = sum + ((uint32_t)k != big ? q[k] * q[k] : 0.0);
+    const double qm = sqrt(fmax(0.0, 1.0 - sum));
+#pragma unroll
+    for (int k = 0; k < 4; ++k) q[k] = (uint32_t)k == big ? qm : q[k];
+  } else {  // x, y, z in bytes; w >= 0 from the unit norm
+#pragma unroll
+    for (int k = 0; k < 3; ++k) q[k] = (double)r[k] / 127.5 - 1.0;
+    q[3] = sqrt(fmax(0.0, 1.0 - ((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2])));
+  }
+  v[PF_R0] = ply_f32(q[3]);
+  v[PF_R1] = ply_f32(q[0]);
+  v[PF_R2] = ply_f32(q[1]);
+  v[PF_R3] = ply_f32(q[2]);
+  ply_convert_row([&](int k) { return v[k]; }, pos[0], pos[1], pos[2], true, true, true, first_row + i, rows32, key_out);
+}
+
 void launch_ply_decode(const uint8_t *chunk, uint32_t rows, const PlyLayout &L, uint32_t first_row, uint8_t *rows32,
                        uint32_t *key, const PlyShLayout *sh, uint4 *sh_rows, cudaStream_t st) {
   if (!rows) return;
@@ -579,6 +728,17 @@ void launch_ply_decode_compressed(const uint8_t *piece, uint32_t rows, const Ply
   else
     k_ply_decode_compressed<false><<<grid, 256, 0, st>>>(piece, rows, Z.has_color, 0u, first_row, (uint4 *)rows32, key,
                                                           PlyShLayout{}, nullptr);
+}
+
+void launch_ply_decode_spz(const uint8_t *piece, uint32_t rows, const PlySpzLayout &P, uint32_t first_row, uint8_t *rows32,
+                           uint32_t *key, const PlyShLayout *sh, uint4 *sh_rows, cudaStream_t st) {
+  if (!rows) return;
+  const uint32_t grid = (rows + 255) / 256;
+  const bool v3 = P.version == 3;
+  auto kernel = sh ? (v3 ? k_ply_decode_spz<true, true> : k_ply_decode_spz<true, false>)
+                   : (v3 ? k_ply_decode_spz<false, true> : k_ply_decode_spz<false, false>);
+  kernel<<<grid, 256, 0, st>>>(piece, rows, sh ? P.file_k : 0u, P.fb, first_row, (uint4 *)rows32, key,
+                               sh ? *sh : PlyShLayout{}, sh_rows);
 }
 
 }  // namespace gs

@@ -10,6 +10,8 @@ from __future__ import annotations
 
 import math
 import re
+import struct
+import zlib
 
 import numpy as np
 
@@ -324,6 +326,110 @@ def decompress_ply(blob) -> bytes:
         f_rest = np.stack([_f32(sh_byte_value(_column(blob, els["sh"], f"f_rest_{k}", "u1")))
                            for k in range(3 * file_k)], axis=1)
     return write_inria_ply(None, xyz, f_dc, opacity, scale, rot, n_rest=3 * file_k, f_rest=f_rest)
+
+
+_SPZ_MAGIC = b"NGSP"
+_SPZ_K = (0, 3, 8, 15)
+
+
+def is_spz(blob) -> bool:
+    """Whether gs_push_ply decodes `blob` as an inflated .spz stream: it starts with "NGSP" and its 10 KB window holds no
+    "end_header\\n" (include/gsplat_b200.h, ".spz streams")."""
+    head = bytes(memoryview(blob)[:1024 * 10])
+    return head[:4] == _SPZ_MAGIC and head.find(b"end_header\n") < 0
+
+
+def read_spz(blob) -> bytes:
+    """An .spz file as stored (a gzip stream, 1f 8b) -> the inflated stream gs_push_ply reads; any other blob is returned
+    unchanged."""
+    blob = bytes(blob)
+    if blob[:2] == b"\x1f\x8b":
+        return zlib.decompress(blob, 16 + zlib.MAX_WBITS)
+    return blob
+
+
+def spz_header(blob) -> dict:
+    """The 16-byte header of an inflated .spz stream, checked with gs_push_ply's rules and messages (ValueError):
+    version, n, sh_degree, fractional_bits, flags, antialiased (flags bit 0, reported, not acted on: such a file is
+    meant to be drawn with antialias=True), and the section offsets (positions, alphas, colours, scales, rotations, sh)."""
+    blob = bytes(blob)
+
+    def refuse(m):
+        raise ValueError("spz: " + m)
+
+    if len(blob) < 16:
+        refuse("stream shorter than its header")
+    magic, version, n = struct.unpack_from("<4sII", blob)
+    degree, fb, flags = blob[12], blob[13], blob[14]
+    if version not in (2, 3):
+        refuse(f"version {version} is not 2 or 3")
+    if degree > 3:
+        refuse(f"sh_degree {degree} is above 3")
+    if fb > 31:
+        refuse(f"fractional_bits {fb} is above 31")
+    if n > 0x7FFFFFFF:
+        raise ValueError("more than 2^31-1 splats")
+    k = _SPZ_K[degree]
+    widths = (9, 1, 3, 3, 4 if version == 3 else 3, 3 * k)
+    offs, off = [], 16
+    for w in widths:
+        offs.append(off)
+        off += n * w
+    if off > len(blob):
+        refuse("body shorter than its N splats")
+    return {"magic": magic, "version": version, "n": n, "sh_degree": degree, "fractional_bits": fb, "flags": flags,
+            "antialiased": bool(flags & 1), "k": k, "sections": tuple(offs), "widths": widths}
+
+
+def decompress_spz(blob) -> bytes:
+    """An inflated .spz stream (is_spz) -> the INRIA float PLY gs_push_ply decodes it to: x y z, f_dc_*, f_rest_* when
+    the stream has SH, opacity, scale_*, rot_* (rot_0 = w), each computed in fp64 from the bytes and rounded once to f32
+    by the rules of include/gsplat_b200.h (".spz streams").  No coordinate conversion is applied.  Raises ValueError
+    with gs_push_ply's message for a malformed stream.  Also a converter: write the result out as a .ply."""
+    blob = bytes(blob)
+    if not is_spz(blob):
+        raise ValueError("not an .spz stream")
+    h = spz_header(blob)
+    n, k, fb = h["n"], h["k"], h["fractional_bits"]
+
+    def section(s):
+        w = h["widths"][s]
+        return np.frombuffer(blob, np.uint8, count=n * w, offset=h["sections"][s]).reshape(n, w)
+
+    p = section(0).reshape(n, 3, 3).astype(np.int64)
+    q = p[:, :, 0] | (p[:, :, 1] << 8) | (p[:, :, 2] << 16)
+    q = np.where(q >= 1 << 23, q - (1 << 24), q)
+    xyz = _f32(q.astype(np.float64) * math.ldexp(1.0, -fb))
+    a = section(1)[:, 0].astype(np.float64)
+    with np.errstate(divide="ignore"):
+        opacity = _f32(-np.log(1.0 / (a / 255.0) - 1.0))
+    f_dc = _f32((section(2).astype(np.float64) / 255.0 - 0.5) / 0.15)
+    scale = _f32(section(3).astype(np.float64) / 16.0 - 10.0)
+    r = section(4)
+    if h["version"] == 2:
+        x, y, z = [r[:, i].astype(np.float64) / 127.5 - 1.0 for i in range(3)]
+        w = np.sqrt(np.maximum(0.0, 1.0 - ((x * x + y * y) + z * z)))
+        quat = [x, y, z, w]
+    else:
+        word = r.copy().view("<u4").reshape(n).astype(np.int64)
+        big = word >> 30
+        quat = [np.zeros(n) for _ in range(4)]
+        for i in (3, 2, 1, 0):
+            take = big != i
+            m = math.sqrt(0.5) * (word & 511).astype(np.float64) / 511.0
+            quat[i] = np.where(take, np.where(word & 512 != 0, -m, m), 0.0)
+            word = np.where(take, word >> 10, word)
+        s = np.zeros(n)
+        for i in range(4):  # ascending index order; the largest adds +0
+            s = s + np.where(big != i, quat[i] * quat[i], 0.0)
+        qm = np.sqrt(np.maximum(0.0, 1.0 - s))
+        quat = [np.where(big == i, qm, quat[i]) for i in range(4)]
+    rot = np.stack([_f32(quat[3]), _f32(quat[0]), _f32(quat[1]), _f32(quat[2])], axis=1)
+    f_rest = None
+    if k:
+        u = section(5).reshape(n, k, 3).astype(np.float64)  # byte (i K + j) 3 + c
+        f_rest = _f32(((u - 128.0) / 128.0).transpose(0, 2, 1).reshape(n, 3 * k))  # f_rest_{c K + j}
+    return write_inria_ply(None, xyz.reshape(n, 3), f_dc, opacity, scale, rot, n_rest=3 * k, f_rest=f_rest)
 
 
 def write_inria_ply(path_or_none, xyz, f_dc, opacity, scale_log, rot, n_rest: int = 45, f_rest=None) -> bytes:

@@ -3,13 +3,14 @@ one GPU.  No computation happens here: numpy arrays are only the host buffers th
 from __future__ import annotations
 
 import ctypes as C
+import gzip
 import re
 from dataclasses import dataclass
 from typing import Optional, Sequence
 
 import numpy as np
 
-from . import _lib
+from . import _lib, ply
 from ._lib import (GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F, GS_RENDER_BLEND_UNORM8, GS_RENDER_OUT_DEVICE, GS_RENDER_OUT_TILED,
                    GS_RENDER_REUSE_SORT, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32, GS_RENDER_SORT_RADIAL, GS_RENDER_ANTIALIAS, GS_RENDER_STATS, GS_TARGET_DEPTH_WRITE, GS_TARGET_DEVICE, GsCubeFace, GsObject, GsRenderParams, GsStats, GsTarget)
 from .scenes import FrameInputs
@@ -67,7 +68,14 @@ def make_objects(objects: Sequence[SceneObject]):
     return arr
 
 
-_EXPORT_FORMATS = {"splat": _lib.GS_EXPORT_SPLAT, "ply": _lib.GS_EXPORT_PLY, "compressed_ply": _lib.GS_EXPORT_PLY_COMPRESSED}
+_EXPORT_FORMATS = {"splat": _lib.GS_EXPORT_SPLAT, "ply": _lib.GS_EXPORT_PLY, "compressed_ply": _lib.GS_EXPORT_PLY_COMPRESSED,
+                   "spz": _lib.GS_EXPORT_SPZ}
+
+
+def _as_file(blob: bytes, format) -> bytes:
+    """format "spz": the inflated stream the library writes, gzipped as an .spz file is stored (mtime 0, so the bytes
+    are deterministic); every other format as written."""
+    return gzip.compress(blob, mtime=0) if format == "spz" else blob
 
 
 class SplatContext:
@@ -145,8 +153,12 @@ class SplatContext:
         if return_rows:
             # the header's `element vertex N` (index.js:608) sizes the output; a file the call refuses writes nothing, and
             # every row takes at least one byte of the file, so a count above the file size is refused
-            m = re.search(rb"element vertex (\d+)\n", buf[:10240].tobytes())
-            rows = np.empty((min(int(m.group(1)), buf.size) if m else 0, 32), np.uint8)
+            if ply.is_spz(buf):  # an .spz stream: the header's N
+                count = int.from_bytes(buf[8:12].tobytes(), "little") if buf.size >= 12 else 0
+            else:
+                m = re.search(rb"element vertex (\d+)\n", buf[:10240].tobytes())
+                count = int(m.group(1)) if m else 0
+            rows = np.empty((min(count, buf.size), 32), np.uint8)
         n = C.c_uint32()
         src = buf.ctypes.data_as(C.c_void_p)
         if at is None:
@@ -212,15 +224,16 @@ class SplatContext:
 
     def export(self, first: int = 0, count: Optional[int] = None, format="splat") -> bytes:
         """gs_export: rows [first, first+count) (count None: to the end) as one file: format "splat" (32-byte rows, as
-        pushed), "ply" (INRIA float PLY with the context's f_rest_*) or "compressed_ply" (SuperSplat's chunked layout),
-        or the GS_EXPORT_* value.  Needs keep_rows."""
+        pushed), "ply" (INRIA float PLY with the context's f_rest_*), "compressed_ply" (SuperSplat's chunked layout) or
+        "spz" (an .spz file: the library's version 3 stream, gzipped), or the GS_EXPORT_* value (GS_EXPORT_SPZ gives the
+        inflated stream).  Needs keep_rows."""
         fmt = _EXPORT_FORMATS.get(format, format)
         count = self.num_splats - first if count is None else count
         size = C.c_size_t()
         self._check(self._lib.gs_export(self._h, int(first), int(count), int(fmt), None, 0, C.byref(size)))
         out = np.empty(size.value, np.uint8)
         self._check(self._lib.gs_export(self._h, int(first), int(count), int(fmt), _ptr(out), out.size, C.byref(size)))
-        return out.tobytes()
+        return _as_file(out.tobytes(), format)
 
     def export_parts(self, parts, format="splat") -> bytes:
         """gs_export_parts: several table ranges as one file, in the order given, each row first transformed by its
@@ -237,7 +250,7 @@ class SplatContext:
         self._check(self._lib.gs_export_parts(self._h, arr, len(parts), int(fmt), None, 0, C.byref(size)))
         out = np.empty(size.value, np.uint8)
         self._check(self._lib.gs_export_parts(self._h, arr, len(parts), int(fmt), _ptr(out), out.size, C.byref(size)))
-        return out.tobytes()
+        return _as_file(out.tobytes(), format)
 
     def read_sh(self, first: int = 0, n: Optional[int] = None) -> np.ndarray:
         """gs_read_sh: the SH coefficients of splats [first, first+n) as (n, 3, K) float16, K = (degree+1)^2 - 1, in table

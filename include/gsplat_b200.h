@@ -206,6 +206,40 @@ GS_API int gs_push_splats(gs_context *ctx, const void *rows32, uint32_t n);
  *       and likewise g, b (never alpha); f_dc_k = (c_k - 0.5) / SH_C0; opacity = -log(1 / alpha - 1) (+-inf at 1 and 0);
  *     - sh byte u: f_rest = ((u + 0.5) / 256 - 0.5) 8, the centre of the exporter's bucket trunc((f / 8 + 0.5) 256)
  *       clamped to [0, 255].  No published file pins this rule down; it is this library's definition.
+ *
+ * .spz streams (".spz streams"; the packed-gaussian format of Niantic's open-source spz library) take a third path.  An
+ * .spz file is a gzip stream; this library reads and writes it inflated (the Python layer gunzips and gzips: ply.read_spz,
+ * SplatContext.export).  A buffer is an .spz stream when its first four bytes are "NGSP" and its 10 KB window holds no
+ * "end_header\n".  The reference refuses every such buffer, so every file it reads decodes as before.  A gzip buffer
+ * (1f 8b) is not inflated and keeps the refusal "Unable to read .ply file header".
+ *   Layout, little-endian: a 16 B header, then six column sections of N splats in this order (K = 0, 3, 8, 15 for SH
+ *   degree 0..3):
+ *     - header: u32 magic 0x5053474e ("NGSP"), u32 version, u32 N, u8 sh_degree, u8 fractional_bits fb, u8 flags (bit 0:
+ *       trained antialiased), u8 reserved;
+ *     - positions, 9 N B: x, y, z of each splat as 24-bit two's-complement fixed point;  alphas, N B;  colours, 3 N B;
+ *       scales, 3 N B;  rotations, 3 N B (version 2) or 4 N B (version 3);  SH, 3 K N B: per splat, per coefficient j
+ *       (0..K-1), per channel c (R, G, B innermost), byte u at (i K + j) 3 + c.
+ *   Header rules (GS_ERR_INVALID, the message prefixed "spz: ", the table unchanged): fewer than 16 bytes ("stream shorter
+ *   than its header"); a version other than 2 or 3 ("version V is not 2 or 3"); sh_degree above 3 ("sh_degree D is above
+ *   3"); fb above 31 ("fractional_bits F is above 31"); fewer than 16 + N (20 + 3 K) bytes in version 3 or 16 + N (19 + 3 K)
+ *   in version 2 ("body shorter than its N splats").  N above 2^31 - 1 returns GS_ERR_CAPACITY.  Trailing bytes, flags and
+ *   reserved are ignored; N == 0 inserts nothing.
+ *   Decode: the rows, table and SH coefficients are exactly those of the INRIA float PLY (rot_0 = w, rot_1..3 = x, y, z)
+ *   whose every property is computed in fp64 from the bytes and rounded once to f32 (ply.decompress_spz writes it):
+ *     - x = int24 2^-fb (exact in f32), likewise y, z;
+ *     - alpha byte a: opacity = -log(1 / (a / 255) - 1) (+inf at 255, -inf at 0);
+ *     - colour byte c: f_dc = (c / 255 - 0.5) / 0.15;  scale byte s: scale_k = s / 16 - 10 (a log scale);
+ *     - version 2 rotation bytes b (x, y, z): q = b / 127.5 - 1, w = sqrt(max(0, 1 - ((x x + y y) + z z)));
+ *     - version 3 rotation word v (u32, "smallest three"): v >> 30 is the index i_L of the largest component (x 0, y 1,
+ *       z 2, w 3).  Walking the indices 3, 2, 1, 0 and skipping i_L, each takes the low 10 bits of v, then v >>= 10: sign
+ *       bit 9, magnitude m in bits 0-8, q_i = +-(sqrt(0.5) m) / 511.  Then q_iL = sqrt(max(0, 1 - S)), S the sum of the
+ *       other three q_i^2 in ascending index order;
+ *     - SH byte u: f_rest_{c K + j} = (u - 128) / 128 (exact in fp16).
+ *   No coordinate conversion is applied: the numbers are used as stored, as a PLY's are.  A file stored in a y-up, z-back
+ *   frame (y and z negated relative to this library's .splat frame) is placed by turning its entity 180 degrees about x;
+ *   the SH evaluation follows the modelview with no special case.  The flags are not acted on: a file flagged
+ *   antialiased is meant to be drawn with GS_RENDER_ANTIALIAS.  These rules restate the public spz library from its
+ *   description; they are kept here, in one place, so that a correction is one edit.
  */
 GS_API int gs_push_ply(gs_context *ctx, const void *ply, size_t bytes, void *rows32_out_or_null, uint32_t *out_n);
 /*
@@ -380,8 +414,28 @@ GS_API int gs_read_sh(gs_context *ctx, uint32_t first, uint32_t n, uint16_t *out
  *         ties) is made positive and its index (x 0, y 1, z 2, w 3) goes in bits 30-31; the other three, in x y z w order,
  *         take 10 bits each as packUnorm(q sqrt(2)/2 + 0.5, 10).  The zero quaternion is stored as the identity;
  *       - sh byte: clamp(trunc((f / 8 + 0.5) 256), 0, 255), NaN giving 0.
+ *   GS_EXPORT_SPZ: the inflated .spz stream gs_push_ply reads (".spz streams" above), version 3: 16 + N (20 + 3 K) bytes,
+ *     the header magic, 3, N, the context's SH degree, fb, flags 0, reserved 0.  A size query needs no device work.  Each
+ *     value quantises the GS_EXPORT_PLY restatement above, in fp64, following the spz writer's rules, with
+ *     q8(v) = clamp(floor(v + 0.5), 0, 255) and NaN giving 0:
+ *       - fb: the largest f in 0..12 for which every finite coordinate x of the file has lround(|x| 2^f) <= 2^23 - 1 (one
+ *         device max-reduction over the rows written); N == 0 gives 12.  When even f = 0 fails (|x| >= 2^23 - 0.5) the
+ *         call returns GS_ERR_INVALID ("spz: a position too large for 24-bit fixed point") and writes nothing;
+ *       - position: the 24-bit two's complement of lround(x 2^fb), half away from zero; a coordinate that is not finite
+ *         is written as 0;
+ *       - alpha = q8(sigmoid(opacity) 255), which gives back the row's alpha byte;  colour = q8(f_dc 0.15 255 + 127.5);
+ *         scale = q8((scale_k + 10) 16);
+ *       - rotation word: rot_0..3 normalised in fp64 (sqrt(((w w + x x) + y y) + z z)); the zero quaternion is the
+ *         identity (0xC0000000).  The largest |component| in x y z w order (the first on ties) gives i_L, and all four are
+ *         negated when it is negative.  Each other component, in ascending index, takes 10 bits, the first in the highest:
+ *         sign bit 9 (q < 0), m = min(511, floor(511 |q| / sqrt(0.5) + 0.5)) in bits 0-8;
+ *       - SH byte of coefficient j of a channel, value f: q = lround(f 128) + 128 (half away from zero), bucketed with
+ *         b = 8 for j < 3 and 16 above as floor((q + b / 2) / b) b, clamped to [0, 255]; NaN gives 128.
+ *     Loading the file gives back every alpha byte, positions within 2^-(fb+1), and the other values within the steps
+ *     above.  The Python layer (SplatContext.export(format="spz")) returns the stream gzipped.
+ * The value 3 is not assigned: gs_export and gs_export_parts refuse it as an unknown format.
  */
-enum { GS_EXPORT_SPLAT = 0, GS_EXPORT_PLY = 1, GS_EXPORT_PLY_COMPRESSED = 2 };
+enum { GS_EXPORT_SPLAT = 0, GS_EXPORT_PLY = 1, GS_EXPORT_PLY_COMPRESSED = 2, GS_EXPORT_SPZ = 4 };
 GS_API int gs_set_keep_rows(gs_context *ctx, uint32_t on);
 GS_API int gs_export(gs_context *ctx, uint32_t first, uint32_t count, uint32_t format, void *out_or_null, size_t cap,
                      size_t *out_bytes);
