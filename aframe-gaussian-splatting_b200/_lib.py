@@ -65,6 +65,18 @@ class GsCropBox(C.Structure):
     _fields_ = [("first", C.c_uint32), ("count", C.c_uint32), ("mode", C.c_uint32), ("box16", C.c_float * 16)]
 
 
+GS_MAX_OUTLIER_K = 32
+
+
+class GsOutlierStats(C.Structure):
+    """gs_outlier_stats: one range's scored rows, its kept rows and the score statistics (NaN when scored <= k)."""
+    _fields_ = [("scored", C.c_uint32), ("kept", C.c_uint32), ("mean", C.c_double), ("stddev", C.c_double),
+                ("threshold", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class GsExportPart(C.Structure):
     """gs_export_part: one table range of gs_export_parts and the affine map of its .splat row frame (column-major)."""
     _fields_ = [("first", C.c_uint32), ("count", C.c_uint32), ("pad", C.c_uint32 * 2), ("m", C.c_double * 16)]
@@ -108,6 +120,9 @@ SYMBOLS = {
     "gs_insert_ply": (C.c_int, [_P, C.c_uint32, _P, C.c_size_t, _P, C.POINTER(C.c_uint32)]),
     "gs_erase": (C.c_int, [_P, C.c_uint32, C.c_uint32]),
     "gs_crop": (C.c_int, [_P, C.POINTER(GsCropBox), C.c_uint32, C.POINTER(C.c_uint32)]),
+    "gs_outlier_scores": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_uint32, C.c_double, _P, C.POINTER(GsOutlierStats)]),
+    "gs_remove_outliers": (C.c_int, [_P, C.POINTER(C.c_uint32), C.c_uint32, C.c_uint32, C.c_double,
+                                     C.POINTER(GsOutlierStats)]),
     "gs_push_packed": (C.c_int, [_P, _P, _P, _P, C.c_uint32]),
     "gs_num_splats": (C.c_int, [_P, C.POINTER(C.c_uint32)]),
     "gs_read_packed": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P]),

@@ -484,6 +484,25 @@ class SplatScene:
         self._shift_after(component, kept - count)
         return kept
 
+    def remove_floaters(self, component: GaussianSplattingComponent, k: int = 20, std_ratio: float = 2.0) -> int:
+        """Remove the entity's floaters once, on the device (gs_remove_outliers): the splats whose mean distance to
+        their k nearest neighbours in the entity lies more than std_ratio standard deviations above the entity's mean.
+        The entity keeps its place in the table as with crop(): its range shrinks and the entities behind it move down.
+        Returns the splats it kept."""
+        first, count = self._range[id(component)]
+        kept = int(self.renderer.remove_outliers([(first, count)], k, std_ratio)[0]["kept"])
+        self._range[id(component)][1] = kept
+        self._shift_after(component, kept - count)
+        return kept
+
+    def floaters(self, component: GaussianSplattingComponent, k: int = 20, std_ratio: float = 2.0) -> np.ndarray:
+        """A bool mask over the entity's splats: True where remove_floaters with the same arguments would remove the
+        splat (gs_outlier_scores; nothing changes).  For previewing the edit."""
+        first, count = self._range[id(component)]
+        scores, st = self.renderer.outlier_scores(first, count, k, std_ratio)
+        with np.errstate(invalid="ignore"):
+            return scores > st["threshold"]
+
     def save(self, component: GaussianSplattingComponent, path=None, format: str = "splat") -> bytes:
         """Write the entity's splats out as one file (gs_export of its range): format "splat", "ply", "compressed_ply"
         or "spz" (gzipped, as an .spz file is stored).  Returns the bytes, and also writes them to `path` when given.  Needs keep_rows=True."""

@@ -7,6 +7,8 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <cmath>
+#include <limits>
 #include <new>
 #include <vector>
 
@@ -708,9 +710,64 @@ extern "C" int gs_erase(gs_context *c, uint32_t first, uint32_t count) {
   return GS_OK;
 }
 
-// gs_crop (gs_crop.cu): the ranges are validated and sorted first, so a refusal changes nothing.  Passes 1-2 count what
-// each range keeps; the counts come back to the host, which sizes the temporary (the failure point that leaves the table
-// unchanged) and stops there when nothing is removed; pass 3 compacts the rows behind the first removed one.
+// The compaction of gs_crop and gs_remove_outliers (gs_crop.cu) over the non-empty ranges of t, sorted by first, on
+// push_stream after the drain.  drop: the removed-row bits (NULL: t's boxes decide).  Passes 1-2 count what each range
+// keeps; the counts come back to the host, which sizes the temporary (the failure point that leaves the table unchanged)
+// and stops there when nothing is removed; pass 3 compacts the rows behind the first removed one.  kept[j]: the rows
+// range j kept; removed: the rows removed.  The caller shrinks c->n.
+static cudaError_t compact_ranges(gs_context *c, const CropTable &t, const uint32_t *drop, std::vector<uint32_t> &kept,
+                                  uint32_t &removed) {
+  uint32_t r0 = 0xFFFFFFFFu;
+  removed = 0;
+  const uint32_t lo = t.n ? t.r[0].first : 0u, n = c->n;
+  cudaStream_t st = c->push_stream;
+  CropScratch s{};
+  s.drop = drop;
+  void *tmp = nullptr;
+  auto release = [&]() {
+    if (s.tab) cudaFreeAsync(s.tab, st);
+    if (tmp) cudaFreeAsync(tmp, st);
+  };
+  if (t.n) {
+    const uint32_t chunks = crop_chunks(n - lo);
+    const size_t tab_bytes = (sizeof(CropTable) + 15) & ~(size_t)15;
+    cudaError_t e = cudaMallocAsync((void **)&s.tab, tab_bytes + sizeof(uint32_t) * ((size_t)chunks + 2 + kMaxObjects), st);
+    if (e) {
+      cudaGetLastError();  // an allocation failure is not sticky
+      return e;
+    }
+    s.kept = (uint32_t *)((char *)s.tab + tab_bytes);
+    s.first_drop = s.kept + kMaxObjects;
+    s.chunk_cnt = s.first_drop + 1;
+    if (!e) e = cudaMemcpyAsync(s.tab, &t, sizeof(CropTable), cudaMemcpyHostToDevice, st);
+    if (!e) e = cudaMemsetAsync(s.kept, 0, sizeof(uint32_t) * kMaxObjects, st);
+    if (!e) e = cudaMemsetAsync(s.first_drop, 0xFF, sizeof(uint32_t), st);
+    if (!e) {
+      launch_crop_count(c, s, lo, n, st);
+      e = cudaGetLastError();
+    }
+    if (!e) e = cudaMemcpyAsync(kept.data(), s.kept, sizeof(uint32_t) * t.n, cudaMemcpyDeviceToHost, st);
+    if (!e) e = cudaMemcpyAsync(&r0, s.first_drop, sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
+    if (!e) e = cudaStreamSynchronize(st);
+    for (uint32_t j = 0; j < t.n && !e; ++j) removed += (t.r[j].end - t.r[j].first) - kept[j];
+    if (!e && removed) {
+      const uint32_t moved = n - r0 - removed;  // the kept rows behind the first removed one
+      if (moved && (e = cudaMallocAsync(&tmp, crop_tmp_bytes(moved, c->sh ? c->sh_vecs : 0u, c->keep_rows), st))) {
+        cudaGetLastError();
+        tmp = nullptr;
+      }
+      if (!e) {
+        launch_crop_write(c, s, lo, r0, n, moved, tmp, st);
+        e = cudaGetLastError();
+      }
+    }
+    release();
+    return e;
+  }
+  return cudaSuccess;
+}
+
+// gs_crop (gs_crop.cu): the ranges are validated and sorted first, so a refusal changes nothing; then compact_ranges.
 extern "C" int gs_crop(gs_context *c, const gs_crop_box *boxes, uint32_t n_boxes, uint32_t *out_counts) {
   if (!c) return GS_ERR_INVALID;
   if (!boxes || n_boxes == 0 || n_boxes > (uint32_t)GS_MAX_OBJECTS)
@@ -740,56 +797,129 @@ extern "C" int gs_crop(gs_context *c, const gs_crop_box *boxes, uint32_t n_boxes
   int rc = drain(c);  // frames in flight read the table (as for gs_erase)
   if (rc) return rc;
   std::vector<uint32_t> kept(kMaxObjects, 0u);
-  uint32_t removed = 0, r0 = 0xFFFFFFFFu;
-  const uint32_t lo = t.n ? t.r[0].first : 0u, n = c->n;
-  cudaStream_t st = c->push_stream;
-  CropScratch s{};
-  void *tmp = nullptr;
-  auto release = [&]() {
-    if (s.tab) cudaFreeAsync(s.tab, st);
-    if (tmp) cudaFreeAsync(tmp, st);
-  };
-  if (t.n) {
-    const uint32_t chunks = crop_chunks(n - lo);
-    const size_t tab_bytes = (sizeof(CropTable) + 15) & ~(size_t)15;
-    cudaError_t e = cudaMallocAsync((void **)&s.tab, tab_bytes + sizeof(uint32_t) * ((size_t)chunks + 2 + kMaxObjects), st);
-    if (e) {
-      cudaGetLastError();  // an allocation failure is not sticky
-      s.tab = nullptr;
-      GS_CUDA(c, e);
-    }
-    s.kept = (uint32_t *)((char *)s.tab + tab_bytes);
-    s.first_drop = s.kept + kMaxObjects;
-    s.chunk_cnt = s.first_drop + 1;
-    if (!e) e = cudaMemcpyAsync(s.tab, &t, sizeof(CropTable), cudaMemcpyHostToDevice, st);
-    if (!e) e = cudaMemsetAsync(s.kept, 0, sizeof(uint32_t) * kMaxObjects, st);
-    if (!e) e = cudaMemsetAsync(s.first_drop, 0xFF, sizeof(uint32_t), st);
-    if (!e) {
-      launch_crop_count(c, s, lo, n, st);
-      e = cudaGetLastError();
-    }
-    if (!e) e = cudaMemcpyAsync(kept.data(), s.kept, sizeof(uint32_t) * t.n, cudaMemcpyDeviceToHost, st);
-    if (!e) e = cudaMemcpyAsync(&r0, s.first_drop, sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
-    if (!e) e = cudaStreamSynchronize(st);
-    for (uint32_t j = 0; j < t.n && !e; ++j) removed += (t.r[j].end - t.r[j].first) - kept[j];
-    if (!e && removed) {
-      const uint32_t moved = n - r0 - removed;  // the kept rows behind the first removed one
-      if (moved && (e = cudaMallocAsync(&tmp, crop_tmp_bytes(moved, c->sh ? c->sh_vecs : 0u, c->keep_rows), st))) {
-        cudaGetLastError();
-        tmp = nullptr;
-      }
-      if (!e) {
-        launch_crop_write(c, s, lo, r0, n, moved, tmp, st);
-        e = cudaGetLastError();
-      }
-    }
-    release();
-    GS_CUDA(c, e);
-  }
+  uint32_t removed = 0;
+  const cudaError_t e = compact_ranges(c, t, nullptr, kept, removed);
+  GS_CUDA(c, e);
   if (out_counts) {
     for (uint32_t i = 0; i < n_boxes; ++i) out_counts[i] = 0;  // empty ranges keep 0
     for (size_t j = 0; j < idx.size(); ++j) out_counts[idx[j]] = kept[j];
   }
+  GS_CUDA(c, cudaEventRecord(c->push_done, c->push_stream));
+  c->n -= removed;
+  c->pushed = true;
+  c->have_order = false;
+  return GS_OK;
+}
+
+// gs_outlier_scores / gs_remove_outliers (gs_outlier.cu): the arguments are checked and the non-empty ranges sorted by
+// first row before anything runs, so a refusal changes nothing.  idx: the caller's index of each range of t.
+static int outlier_table(gs_context *c, const char *who, const uint32_t *ranges, uint32_t n_ranges, uint32_t k,
+                         double std_ratio, OutlierTable &t, std::vector<uint32_t> &idx) {
+  auto refuse = [&](const char *why) { return fail(c, GS_ERR_INVALID, (std::string(who) + ": " + why).c_str()); };
+  if (k == 0 || k > GS_MAX_OUTLIER_K) return refuse("k is 1 .. GS_MAX_OUTLIER_K");
+  if (!std::isfinite(std_ratio)) return refuse("std_ratio is not finite");
+  if (!ranges || n_ranges == 0 || n_ranges > (uint32_t)GS_MAX_OBJECTS) return refuse("between 1 and GS_MAX_OBJECTS ranges");
+  for (uint32_t i = 0; i < n_ranges; ++i) {
+    if ((uint64_t)ranges[2 * i] + ranges[2 * i + 1] > c->n) return refuse("a range runs past the resident splats");
+    if (ranges[2 * i + 1]) idx.push_back(i);
+  }
+  std::sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return ranges[2 * a] < ranges[2 * b]; });
+  for (size_t j = 1; j < idx.size(); ++j)
+    if ((uint64_t)ranges[2 * idx[j - 1]] + ranges[2 * idx[j - 1] + 1] > ranges[2 * idx[j]]) return refuse("ranges overlap");
+  memset(&t, 0, sizeof(t));
+  t.n = (uint32_t)idx.size();
+  t.k = k;
+  t.std_ratio = std_ratio;
+  for (size_t j = 0; j < idx.size(); ++j) {
+    t.r[j].first = ranges[2 * idx[j]];
+    t.r[j].count = ranges[2 * idx[j] + 1];
+    t.r[j].pos = t.rows;
+    t.rows += t.r[j].count;
+  }
+  return GS_OK;
+}
+
+static void outlier_stats_of(const OutlierRange *g, uint32_t count, gs_outlier_stats &o) {
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  o.scored = g ? g->m : 0u;
+  o.kept = count - (g ? g->removed : 0u);
+  o.mean = g && g->judged ? g->mean : nan;
+  o.stddev = g && g->judged ? g->stddev : nan;
+  o.threshold = g && g->judged ? g->threshold : nan;
+}
+
+// the scores of one range, read only: behind the queued pushes and edits on push_stream, without waiting for frames in
+// flight (they and this call only read the table), as gs_export
+extern "C" int gs_outlier_scores(gs_context *c, uint32_t first, uint32_t count, uint32_t k, double std_ratio, double *scores_out,
+                                 gs_outlier_stats *stats_out) {
+  if (!c) return GS_ERR_INVALID;
+  const uint32_t range[2] = {first, count};
+  OutlierTable t;
+  std::vector<uint32_t> idx;
+  int rc = outlier_table(c, "gs_outlier_scores", range, 1, k, std_ratio, t, idx);
+  if (rc) return rc;
+  if (!stats_out) return fail(c, GS_ERR_INVALID, "gs_outlier_scores: stats_out is NULL");
+  if (t.n) {
+    GS_CUDA(c, cudaSetDevice(c->device));
+    cudaStream_t st = c->push_stream;
+    void *tmp = nullptr;
+    cudaError_t e = cudaMallocAsync(&tmp, outlier_tmp_bytes(t, c->n, false, scores_out != nullptr), st);
+    if (e) {
+      cudaGetLastError();  // an allocation failure is not sticky
+      GS_CUDA(c, e);
+    }
+    const OutlierScratch s = outlier_scratch(tmp, t, c->n, false, scores_out != nullptr);
+    e = outlier_run(c, t, s, st);
+    if (!e && scores_out) e = cudaMemcpyAsync(scores_out, s.out, sizeof(double) * count, cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(tmp, st);
+    if (!e) e = cudaStreamSynchronize(st);
+    GS_CUDA(c, e);
+  }
+  outlier_stats_of(t.n ? &t.r[0] : nullptr, count, *stats_out);
+  return GS_OK;
+}
+
+// every range scored, then one compaction (compact_ranges) with the removed-row bits as its verdict.  The outlier
+// temporary is allocated after the drain and before any pass; the compaction's own before it writes the table.
+extern "C" int gs_remove_outliers(gs_context *c, const uint32_t *ranges, uint32_t n_ranges, uint32_t k, double std_ratio,
+                                  gs_outlier_stats *out) {
+  if (!c) return GS_ERR_INVALID;
+  OutlierTable t;
+  std::vector<uint32_t> idx;
+  int rc = outlier_table(c, "gs_remove_outliers", ranges, n_ranges, k, std_ratio, t, idx);
+  if (rc) return rc;
+  GS_CUDA(c, cudaSetDevice(c->device));
+  if ((rc = drain(c))) return rc;  // frames in flight read the table (as for gs_crop)
+  cudaStream_t st = c->push_stream;
+  uint32_t removed = 0;
+  if (t.n) {
+    void *tmp = nullptr;
+    cudaError_t e = cudaMallocAsync(&tmp, outlier_tmp_bytes(t, c->n, true, false), st);
+    if (e) {
+      cudaGetLastError();
+      GS_CUDA(c, e);
+    }
+    const OutlierScratch s = outlier_scratch(tmp, t, c->n, true, false);
+    e = outlier_run(c, t, s, st);
+    for (uint32_t j = 0; j < t.n && !e; ++j) removed += t.r[j].removed;
+    if (!e && removed) {
+      CropTable ct;
+      memset(&ct, 0, sizeof(ct));
+      ct.n = t.n;
+      for (uint32_t j = 0; j < t.n; ++j) {
+        ct.r[j].first = t.r[j].first;
+        ct.r[j].end = t.r[j].first + t.r[j].count;
+      }
+      std::vector<uint32_t> kept(kMaxObjects, 0u);
+      uint32_t compacted = 0;
+      e = compact_ranges(c, ct, s.drop, kept, compacted);
+    }
+    cudaFreeAsync(tmp, st);
+    GS_CUDA(c, e);
+  }
+  if (out)
+    for (uint32_t i = 0; i < n_ranges; ++i) outlier_stats_of(nullptr, 0, out[i]);  // empty ranges: 0 rows, NaN stats
+  for (size_t j = 0; j < idx.size() && out; ++j) outlier_stats_of(&t.r[j], t.r[j].count, out[idx[j]]);
   GS_CUDA(c, cudaEventRecord(c->push_done, st));
   c->n -= removed;
   c->pushed = true;

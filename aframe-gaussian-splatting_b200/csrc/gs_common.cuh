@@ -670,6 +670,7 @@ struct CropScratch {
   uint32_t *chunk_cnt;   // kept rows per chunk of [lo, N), exclusive-scanned in place (chunks + 1 words)
   uint32_t *kept;        // kept rows per range (kMaxObjects words; zeroed by the caller)
   uint32_t *first_drop;  // first removed row (0xFFFFFFFF: none; set by the caller)
+  const uint32_t *drop = nullptr;  // gs_remove_outliers: bit `row` set = row removed (NULL: gs_crop's boxes decide)
 };
 uint32_t crop_chunks(uint32_t rows);  // chunks of the compaction over `rows` rows
 // pass 1 and 2 over rows [lo, n): per-chunk and per-range kept counts, the first removed row, the chunk offsets
@@ -679,6 +680,45 @@ size_t crop_tmp_bytes(uint32_t kept, uint32_t sh_vecs, bool rows);
 // pass 3: the kept rows of [r0, n) (r0 = the first removed row) into tmp, in order, then back into the table at r0
 void launch_crop_write(gs_context *c, const CropScratch &s, uint32_t lo, uint32_t r0, uint32_t n, uint32_t kept, void *tmp,
                        cudaStream_t st);
+// gs_outlier_scores / gs_remove_outliers (gs_outlier.cu): the ranges of one call, sorted by first, and its layout
+constexpr int kOutlierMaxLevels = 8;  // levels of a range's hierarchy: 2^32 rows make 7 (leaves of 32, nodes of 32)
+struct OutlierRange {
+  uint32_t first, count;  // table rows [first, first + count), count > 0
+  uint32_t pos;           // its first row's place among the call's range rows (the counts before it)
+  uint32_t m;             // its scored rows (finite centres), from the bounds pass
+  uint32_t sorted;        // the sorted place of its first scored row (the m before it)
+  uint32_t judged;        // m > k: its rows are scored; else every score is NaN and every row kept
+  uint32_t leaf, root;    // its first leaf and the root of its hierarchy (judged ranges)
+  uint32_t removed, pad;  // results: rows whose score exceeds the threshold
+  double mean, stddev, threshold;
+};
+struct OutlierTable {
+  uint32_t n, k;          // ranges, neighbours
+  uint32_t rows, scored;  // the ranges' rows R, their scored rows M (sorted places [0, M), then the others)
+  uint32_t n_leaves, pad;
+  double std_ratio;
+  OutlierRange r[kMaxObjects];
+};
+struct OutlierScratch {
+  OutlierTable *tab;
+  uint32_t *bound;    // per range: 6 ordered box words, then (at kMaxObjects * 6) scored rows, then (* 7) removed rows
+  double *stats;      // per range: mean, stddev, threshold
+  uint32_t *key;      // 2R words: the key halves; then R doubles: the scores in sorted order (scores)
+  uint32_t *perm;     // 3R words: the radix permutations; then R doubles: the scores by range row (out)
+  float4 *pts;        // R: the centres in sorted order, the table row in w
+  float4 *node;       // 2 per node: box lo | first child, box hi | children
+  uint2 *child;       // inner nodes: first child, children
+  uint32_t *radix_table, *radix_totals;
+  uint32_t *drop;     // removed-row bits by table row (gs_remove_outliers), else NULL
+  uint32_t n_drop_words;
+  double *scores, *out;
+};
+// one stream-ordered temporary for a call over the ranges of t (rows set) on a table of n_table rows: drop: with the
+// removed-row bits; out: with the scores by range row
+size_t outlier_tmp_bytes(const OutlierTable &t, uint32_t n_table, bool drop, bool out);
+OutlierScratch outlier_scratch(void *tmp, const OutlierTable &t, uint32_t n_table, bool drop, bool out);
+// scores, stats and verdict of every range of t on st; t's layout fields and results are filled in
+cudaError_t outlier_run(gs_context *c, OutlierTable &t, const OutlierScratch &s, cudaStream_t st);
 // gs_export (gs_export.cu): rows [first, first + n) of the kept .splat rows (and their SH rows on an SH context, sh_k
 // coefficients per channel) restated as INRIA PLY vertices into body (n (14 + 3 sh_k) floats), or quantised as a
 // compressed PLY body: ceil(n / 256) chunk rows of 18 floats, n 16 B vertex words, n 3 sh_k SH bytes

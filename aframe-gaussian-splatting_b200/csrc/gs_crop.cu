@@ -1,5 +1,6 @@
 // gs_crop.cu — gs_crop: keep (or erase) the splats of entity ranges inside a cutout box, compacting the table in place.
-//   k_crop_count : pass 1 over rows [lo, N) (lo = the first range's first row): the crop's verdict per row (cutout_inside,
+// gs_remove_outliers (gs_outlier.cu) compacts through the same passes with its own verdict (BitVerdict).
+//   k_crop_count : pass 1 over rows [lo, N) (lo = the first range's first row): the verdict per row (gs_crop: cutout_inside,
 //                  the frames' own test, with each range's box and mode; rows outside every range are kept), kept rows per
 //                  chunk (warp ballots), kept rows per range and the first removed row
 //   k_crop_scan  : pass 2, one CTA: exclusive scan of the chunk counts
@@ -22,9 +23,26 @@ constexpr int kCropWarps = kCropThreads / 32;
 __host__ __device__ __forceinline__ uint32_t chunks_of(uint32_t rows) { return (rows + kCropChunk - 1) / kCropChunk; }
 uint32_t crop_chunks(uint32_t rows) { return chunks_of(rows); }
 
+// The verdict policies of the compaction (the kernels' last parameter): whether row `row` (centre c) of range k
+// (tab->r[k]) is kept.  gs_crop: the range's cutout box and mode.
+struct BoxVerdict {
+  __device__ __forceinline__ bool keep(const CropTable *__restrict__ tab, int k, uint32_t, const float4 &c) const {
+    const CropRange &r = tab->r[k];
+    return cutout_inside(r.box, c.x, c.y, c.z) == (r.keep_inside != 0u);
+  }
+};
+// gs_remove_outliers (gs_outlier.cu): bit `row` of drop set = removed; the table holds only the ranges.
+struct BitVerdict {
+  const uint32_t *drop;
+  __device__ __forceinline__ bool keep(const CropTable *__restrict__, int, uint32_t row, const float4 &) const {
+    return !((drop[row >> 5] >> (row & 31u)) & 1u);
+  }
+};
+
 // The verdict on a thread's rows base + 256 j (j < kCropItems) of one chunk: bit j set = kept.  Rows at or past n are
 // not kept and have range -1, as do rows outside every range, which are kept.  The centres are returned for the write.
-__device__ __forceinline__ uint32_t crop_keep(const float4 *__restrict__ cs, const CropTable *__restrict__ tab,
+template <class V>
+__device__ __forceinline__ uint32_t crop_keep(const float4 *__restrict__ cs, const CropTable *__restrict__ tab, const V &v,
                                               const uint32_t *s_first, const uint32_t *s_end, uint32_t n_r, uint32_t base,
                                               uint32_t n, float4 (&c)[kCropItems], int (&k)[kCropItems]) {
 #pragma unroll
@@ -38,10 +56,7 @@ __device__ __forceinline__ uint32_t crop_keep(const float4 *__restrict__ cs, con
     const uint32_t row = base + j * kCropThreads;
     k[j] = row < n ? scene_find(s_first, s_end, n_r, row) : -1;
     bool kj = row < n;
-    if (k[j] >= 0) {
-      const CropRange &r = tab->r[k[j]];
-      kj = cutout_inside(r.box, c[j].x, c[j].y, c[j].z) == (r.keep_inside != 0u);
-    }
+    if (k[j] >= 0) kj = v.keep(tab, k[j], row, c[j]);
     keep |= (kj ? 1u : 0u) << j;
   }
   return keep;
@@ -54,9 +69,11 @@ __device__ __forceinline__ void crop_load_ranges(const CropTable *__restrict__ t
   }
 }
 
+template <class V>
 __global__ void __launch_bounds__(kCropThreads) k_crop_count(const float4 *__restrict__ cs, const CropTable *__restrict__ tab,
                                                              uint32_t lo, uint32_t n, uint32_t *__restrict__ chunk_cnt,
-                                                             uint32_t *__restrict__ kept, uint32_t *__restrict__ first_drop) {
+                                                             uint32_t *__restrict__ kept, uint32_t *__restrict__ first_drop,
+                                                             const V v) {
   __shared__ uint32_t s_first[kMaxObjects], s_end[kMaxObjects], s_kept[kMaxObjects];
   __shared__ uint32_t s_cnt;
   const uint32_t n_r = tab->n, tid = threadIdx.x, lane = tid & 31u;
@@ -70,7 +87,7 @@ __global__ void __launch_bounds__(kCropThreads) k_crop_count(const float4 *__res
     const uint32_t base = lo + ch * kCropChunk + tid;
     float4 c[kCropItems];
     int k[kCropItems];
-    const uint32_t keep = crop_keep(cs, tab, s_first, s_end, n_r, base, n, c, k);
+    const uint32_t keep = crop_keep(cs, tab, v, s_first, s_end, n_r, base, n, c, k);
     uint32_t total = 0;
 #pragma unroll
     for (int j = 0; j < kCropItems; ++j) {
@@ -135,9 +152,10 @@ __global__ void __launch_bounds__(1024) k_crop_scan(uint32_t *__restrict__ cnt, 
 
 // The kept rows of [r0, n) into dst, in table order: row i goes to (kept rows of [lo, i)) - (r0 - lo), since every row of
 // [lo, r0) is kept.  Within a chunk the order is (j, warp, lane), the row order.
+template <class V>
 __global__ void __launch_bounds__(kCropThreads) k_crop_write(const RowSpan src, const RowSpan dst, uint32_t sh_vecs,
                                                              const CropTable *__restrict__ tab, uint32_t lo, uint32_t r0,
-                                                             uint32_t n, const uint32_t *__restrict__ chunk_off) {
+                                                             uint32_t n, const uint32_t *__restrict__ chunk_off, const V v) {
   __shared__ uint32_t s_first[kMaxObjects], s_end[kMaxObjects];
   __shared__ uint32_t s_pre[kCropItems * kCropWarps];  // kept rows of the chunk before (j, warp), j-major
   const uint32_t n_r = tab->n, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
@@ -151,7 +169,7 @@ __global__ void __launch_bounds__(kCropThreads) k_crop_write(const RowSpan src, 
     const uint32_t base = lo + ch * kCropChunk + tid;
     float4 c[kCropItems];
     int k[kCropItems];
-    const uint32_t keep = crop_keep(src.cs, tab, s_first, s_end, n_r, base, n, c, k);
+    const uint32_t keep = crop_keep(src.cs, tab, v, s_first, s_end, n_r, base, n, c, k);
     uint32_t bal[kCropItems];
 #pragma unroll
     for (int j = 0; j < kCropItems; ++j) {
@@ -196,7 +214,12 @@ static int crop_grid(gs_context *c, uint32_t chunks) {
 
 void launch_crop_count(gs_context *c, const CropScratch &s, uint32_t lo, uint32_t n, cudaStream_t st) {
   const uint32_t chunks = crop_chunks(n - lo);
-  k_crop_count<<<crop_grid(c, chunks), kCropThreads, 0, st>>>(c->center_scale, s.tab, lo, n, s.chunk_cnt, s.kept, s.first_drop);
+  if (s.drop)
+    k_crop_count<<<crop_grid(c, chunks), kCropThreads, 0, st>>>(c->center_scale, s.tab, lo, n, s.chunk_cnt, s.kept, s.first_drop,
+                                                                BitVerdict{s.drop});
+  else
+    k_crop_count<<<crop_grid(c, chunks), kCropThreads, 0, st>>>(c->center_scale, s.tab, lo, n, s.chunk_cnt, s.kept, s.first_drop,
+                                                                BoxVerdict{});
   k_crop_scan<<<1, 1024, 0, st>>>(s.chunk_cnt, chunks);
 }
 
@@ -209,7 +232,11 @@ void launch_crop_write(gs_context *c, const CropScratch &s, uint32_t lo, uint32_
   // the temporary's size_alpha shares the destination's alignment mod 16 B, so the copy back moves it as float4
   const RowSpan t = tmp_span(tmp, kept, w, c->keep_rows, r0);
   const uint32_t chunks = crop_chunks(n - lo) - (r0 - lo) / kCropChunk;
-  k_crop_write<<<crop_grid(c, chunks), kCropThreads, 0, st>>>(table_span(c, 0), t, w, s.tab, lo, r0, n, s.chunk_cnt);
+  if (s.drop)
+    k_crop_write<<<crop_grid(c, chunks), kCropThreads, 0, st>>>(table_span(c, 0), t, w, s.tab, lo, r0, n, s.chunk_cnt,
+                                                                BitVerdict{s.drop});
+  else
+    k_crop_write<<<crop_grid(c, chunks), kCropThreads, 0, st>>>(table_span(c, 0), t, w, s.tab, lo, r0, n, s.chunk_cnt, BoxVerdict{});
   launch_copy_rows(t, table_span(c, r0), kept, w, st);
 }
 

@@ -189,6 +189,31 @@ class SplatContext:
         self._check(self._lib.gs_crop(self._h, arr, len(boxes), counts.ctypes.data_as(C.POINTER(C.c_uint32))))
         return counts[:len(boxes)]
 
+    def outlier_scores(self, first: int = 0, count: Optional[int] = None, k: int = 20, std_ratio: float = 2.0):
+        """gs_outlier_scores: each row of [first, first+count) (count None: to the end of the table) scored by its mean
+        distance to its k nearest scored rows of the range, read only.  Returns (scores, stats): the scores as float64
+        in table order (NaN for a non-finite centre, and for every row when the range has k or fewer scored rows) and a
+        dict of scored, kept (the rows remove_outliers would keep), mean, stddev and threshold (mean + std_ratio
+        stddev).  The defaults are Open3D's remove_statistical_outlier example values."""
+        if count is None:
+            count = self.num_splats - int(first)
+        scores = np.empty(max(int(count), 1), np.float64)
+        st = _lib.GsOutlierStats()
+        self._check(self._lib.gs_outlier_scores(self._h, int(first), int(count), int(k), float(std_ratio), _ptr(scores),
+                                                C.byref(st)))
+        return scores[:int(count)], st.as_dict()
+
+    def remove_outliers(self, ranges, k: int = 20, std_ratio: float = 2.0) -> list:
+        """gs_remove_outliers: remove from each (first, count) range the rows whose score (outlier_scores) exceeds
+        mean + std_ratio stddev of the range's scores, compacting the table in place as crop() does.  Returns one stats
+        dict per range, its kept the rows it kept."""
+        arr = (C.c_uint32 * max(2 * len(ranges), 2))()
+        for i, (first, count) in enumerate(ranges):
+            arr[2 * i], arr[2 * i + 1] = int(first), int(count)
+        out = (_lib.GsOutlierStats * max(len(ranges), 1))()
+        self._check(self._lib.gs_remove_outliers(self._h, arr, len(ranges), int(k), float(std_ratio), out))
+        return [out[i].as_dict() for i in range(len(ranges))]
+
     def push_packed(self, center_scale: np.ndarray, cov_color: np.ndarray, size_alpha: np.ndarray) -> None:
         cs = np.ascontiguousarray(center_scale, dtype=np.float32).reshape(-1, 4)
         cc = np.ascontiguousarray(cov_color, dtype=np.uint32).reshape(-1, 4)

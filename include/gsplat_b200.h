@@ -321,6 +321,58 @@ typedef struct gs_crop_box {
 GS_API int gs_crop(gs_context *ctx, const gs_crop_box *boxes, uint32_t n_boxes, uint32_t *out_counts_or_null);
 
 /*
+ * Removing floaters: statistical outlier removal over entity ranges, on the device (the filter PCL, Open3D and
+ * CloudCompare provide).  The second step of cleaning a capture after gs_crop: a floater hangs inside the box, next to
+ * the real surfaces, but far from its own nearest neighbours.  The definition, exact to the bit:
+ *   - Points.  Each range (one entity's rows [first, first+count)) is scored on its own.  A row's point is the f32 centre
+ *     of its packed record (center_scale.xyz, as gs_read_packed returns it; the sign of z does not change a distance).  A
+ *     row with a non-finite coordinate is not scored, is nobody's neighbour, has score NaN and is always kept.  Rows
+ *     outside every range are not scored, not neighbours, and kept.
+ *   - Distance.  For rows a and b, dx = (double)a.x - (double)b.x (dy, dz the same) and s = (dx*dx + dy*dy) + dz*dz,
+ *     every operation rounded in fp64 (__dsub_rn / __dmul_rn / __dadd_rn, nothing contracted): f32 centres up to
+ *     +-3.4e38 cannot overflow.
+ *   - Neighbours.  The k nearest neighbours of a row are the k other scored rows of its range with the smallest s.  The
+ *     row itself is excluded by index, not by distance, so a duplicate centre is a neighbour at distance 0.  Ties at the
+ *     k-th place do not matter: the multiset of the k smallest s is unique.
+ *   - Score.  d_i = sqrt(s_i) correctly rounded (__dsqrt_rn), d_1 <= d_2 <= ...; score = ((d_1 + d_2) + ... + d_k) / k,
+ *     summed from the nearest neighbour outward (__dadd_rn, then __ddiv_rn).
+ *   - Statistics over the m scored rows of the range: mean = (sum of scores) / m; stddev = sqrt(sum((score - mean)^2) /
+ *     (m - 1)) (two passes, sample deviation); threshold = mean + std_ratio * stddev (__dmul_rn, then __dadd_rn).  The
+ *     sums run in a fixed reduction tree (no floating-point atomics): every run gives the same bits.
+ *   - Too few rows.  When m <= k nothing in the range is judged: every score and statistic is NaN, and every row is kept.
+ *   - Verdict.  A row is removed iff its score is a number and score > threshold (fp64).  So a range whose centres all
+ *     equal their neighbours' removes nothing: stddev is 0, and 0 > 0 is false.  A negative std_ratio is allowed.
+ * gs_outlier_scores: reads only.  scores_out (host, count doubles in table order, or NULL) receives the scores of rows
+ *   [first, first+count); stats_out its statistics, with kept = the rows gs_remove_outliers would keep with the same
+ *   arguments.  It runs behind the queued pushes and edits and sees their rows, and does not wait for frames in flight,
+ *   as gs_export.
+ * gs_remove_outliers: scores each range of `ranges` ((first, count) pairs, any order, count 0 allowed), then compacts the
+ *   table in place, as gs_crop: each range keeps its surviving rows in their relative order, every row behind the first
+ *   removed one moves down with its SH row and kept .splat row, N shrinks by the rows removed.  out (n_ranges entries, or
+ *   NULL): range i's statistics, kept = the rows it kept.  Table-edit rules as gs_crop: the call waits for the frames in
+ *   flight and runs behind queued pushes; the draw order is stale after it; a call that removes nothing writes no byte of
+ *   the table; removing every row leaves N = 0.
+ * GS_ERR_INVALID, nothing changed: k of 0 or above GS_MAX_OUTLIER_K, a std_ratio that is not finite, a range past N,
+ *   ranges NULL, n_ranges of 0 or above GS_MAX_OBJECTS, overlapping ranges, stats_out NULL (gs_outlier_scores).
+ * Memory: one stream-ordered temporary of about 37.5 B per row of the ranges (key halves and then the scores 8 B, three
+ *   sort permutations 12 B, the centres in sorted order 16 B, the index nodes 1.3 B, radix tables) plus N / 8 bytes of
+ *   removed-row bits (gs_remove_outliers), and gs_crop's temporary for the rows that move.  Each is allocated before the
+ *   table is written, so GS_ERR_OOM changes nothing.
+ */
+#define GS_MAX_OUTLIER_K 32
+typedef struct gs_outlier_stats {
+  uint32_t scored;   /* m: rows of the range whose centre is finite                                         */
+  uint32_t kept;     /* rows of the range kept (gs_remove_outliers) or that would be kept (gs_outlier_scores) */
+  double mean;       /* mean of the m scores; NaN when m <= k                                               */
+  double stddev;     /* sample standard deviation (divisor m - 1) of the scores; NaN when m <= k            */
+  double threshold;  /* mean + std_ratio * stddev (one rounding each, no FMA); NaN when m <= k              */
+} gs_outlier_stats;  /* 32 bytes */
+GS_API int gs_outlier_scores(gs_context *ctx, uint32_t first, uint32_t count, uint32_t k, double std_ratio,
+                             double *scores_out_or_null, gs_outlier_stats *stats_out);
+GS_API int gs_remove_outliers(gs_context *ctx, const uint32_t *ranges /* (first, count) pairs */, uint32_t n_ranges,
+                              uint32_t k, double std_ratio, gs_outlier_stats *out_or_null /* n_ranges entries */);
+
+/*
  * Append n already-packed splats: the two data-texture records the reference uploads
  * (centerAndScaleData float4, covAndColorData uint4, index.js:40-46,378-394) and the worker's
  * matrices[15] (max(scale)*alpha/255, index.js:397).  Host pointers.
