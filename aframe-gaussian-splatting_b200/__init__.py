@@ -13,7 +13,7 @@ from ._lib import (GS_FORMAT_RGBA8, GS_FORMAT_RGBA32F, GS_RENDER_OUT_DEVICE, GS_
                    GS_RENDER_COLOR_DEVICE, GS_RENDER_BLEND_UNORM8, GS_RENDER_SCENE_INTERLEAVE, GS_RENDER_SORT_F32, GS_RENDER_SORT_RADIAL, GS_RENDER_ANTIALIAS, GS_MAX_OBJECTS, GS_MAX_CAMERAS, GS_TARGET_DEVICE,
                    GS_TARGET_DEPTH_WRITE, GS_CROP_KEEP_INSIDE, GS_CROP_KEEP_OUTSIDE, GS_EXPORT_SPLAT, GS_EXPORT_PLY,
                    GS_EXPORT_PLY_COMPRESSED, GS_EXPORT_SPZ, GS_MAX_OUTLIER_K, GsCropBox, GsCubeFace, GsExportPart, GsObject,
-                   GsOutlierStats, GsRenderParams, GsStats, GsTarget)
+                   GsOutlierStats, GsRenderParams, GsSimplifyRange, GsSimplifyStats, GsStats, GsTarget)
 from .renderer import GsError, SceneObject, SplatContext  # noqa: F401
 from .scenes import FrameInputs, make_frame, synth_splats  # noqa: F401
 from .component import GaussianSplattingComponent, SortWorker, SplatScene  # noqa: F401

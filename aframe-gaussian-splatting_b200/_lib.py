@@ -77,6 +77,23 @@ class GsOutlierStats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class GsSimplifyRange(C.Structure):
+    """gs_simplify_range: one entity range of gs_simplify / gs_simplify_cells and its cell size (local units)."""
+    _fields_ = [("first", C.c_uint32), ("count", C.c_uint32), ("cell", C.c_double)]
+
+
+class GsSimplifyStats(C.Structure):
+    """gs_simplify_stats: one range's rows before and after (cells), its mergeable rows, merged cells, largest cell and
+    the box of its finite centres."""
+    _fields_ = [("rows", C.c_uint32), ("mergeable", C.c_uint32), ("cells", C.c_uint32), ("merged", C.c_uint32),
+                ("largest", C.c_uint32), ("pad", C.c_uint32), ("lo", C.c_float * 3), ("hi", C.c_float * 3)]
+
+    def as_dict(self):
+        d = {k: getattr(self, k) for k in ("rows", "mergeable", "cells", "merged", "largest")}
+        d["lo"], d["hi"] = tuple(self.lo), tuple(self.hi)
+        return d
+
+
 class GsExportPart(C.Structure):
     """gs_export_part: one table range of gs_export_parts and the affine map of its .splat row frame (column-major)."""
     _fields_ = [("first", C.c_uint32), ("count", C.c_uint32), ("pad", C.c_uint32 * 2), ("m", C.c_double * 16)]
@@ -123,6 +140,8 @@ SYMBOLS = {
     "gs_outlier_scores": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_uint32, C.c_double, _P, C.POINTER(GsOutlierStats)]),
     "gs_remove_outliers": (C.c_int, [_P, C.POINTER(C.c_uint32), C.c_uint32, C.c_uint32, C.c_double,
                                      C.POINTER(GsOutlierStats)]),
+    "gs_simplify_cells": (C.c_int, [_P, C.POINTER(GsSimplifyRange), C.c_uint32, C.POINTER(GsSimplifyStats)]),
+    "gs_simplify": (C.c_int, [_P, C.POINTER(GsSimplifyRange), C.c_uint32, C.POINTER(GsSimplifyStats)]),
     "gs_push_packed": (C.c_int, [_P, _P, _P, _P, C.c_uint32]),
     "gs_num_splats": (C.c_int, [_P, C.POINTER(C.c_uint32)]),
     "gs_read_packed": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P]),

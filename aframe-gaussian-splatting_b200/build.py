@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgsplat_b200.so")
-SOURCES = ["gs_api.cu", "gs_sort.cu", "gs_slab.cu", "gs_pack.cu", "gs_ply.cu", "gs_project.cu", "gs_raster.cu", "gs_pick.cu", "gs_panorama.cu", "gs_crop.cu", "gs_export.cu", "gs_transform.cu", "gs_outlier.cu"]
+SOURCES = ["gs_api.cu", "gs_sort.cu", "gs_slab.cu", "gs_pack.cu", "gs_ply.cu", "gs_project.cu", "gs_raster.cu", "gs_pick.cu", "gs_panorama.cu", "gs_crop.cu", "gs_export.cu", "gs_transform.cu", "gs_outlier.cu", "gs_simplify.cu"]
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17",

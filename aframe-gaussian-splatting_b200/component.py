@@ -349,6 +349,29 @@ class _EntityWorker(SortWorker):
         return self.scene._push_ply(self.component, blob)
 
 
+def simplify_cell_for(ctx: SplatContext, first: int, count: int, target: int) -> Optional[float]:
+    """The cell SplatScene.simplify(target=) takes for rows [first, first+count) of ctx: a geometric bisection of 30
+    gs_simplify_cells probes between the smallest cell the range's box allows and twice its largest extent, keeping the
+    smallest probed cell whose count is at most target (the largest cell when none is).  None: no mergeable row."""
+    if not count:
+        return None
+    st = ctx.simplify_cells(first, count, 1.0e30)
+    ext = max(float(np.float64(h) - np.float64(lo)) for lo, h in zip(st["lo"], st["hi"]))
+    if not st["mergeable"] or not math.isfinite(ext):
+        return None
+    if ext == 0.0:
+        return 1.0   # every mergeable splat in one cell, whatever its size
+    lo, hi = math.nextafter(ext / 524288.0, math.inf), 2.0 * ext   # ext / lo < 2^19: the smallest allowed cell
+    best = hi
+    for _ in range(30):
+        mid = math.sqrt(lo * hi)
+        if ctx.simplify_cells(first, count, mid)["cells"] <= target:
+            best = hi = mid
+        else:
+            lo = mid
+    return best
+
+
 class SplatScene:
     """Several `gaussian_splatting` entities of one page drawn into one frame from one GPU context.
 
@@ -491,6 +514,28 @@ class SplatScene:
         Returns the splats it kept."""
         first, count = self._range[id(component)]
         kept = int(self.renderer.remove_outliers([(first, count)], k, std_ratio)[0]["kept"])
+        self._range[id(component)][1] = kept
+        self._shift_after(component, kept - count)
+        return kept
+
+    def simplify(self, component: GaussianSplattingComponent, cell: Optional[float] = None,
+                 target: Optional[int] = None) -> int:
+        """Merge the entity's splats cell by cell once, on the device (gs_simplify): each cubic cell of size `cell`
+        (the entity's local units) becomes one moment-matched splat.  Pass exactly one of cell and target.  target: the
+        cell is searched on the host with gs_simplify_cells (a geometric bisection of 30 probes between the smallest
+        cell the entity's box allows and twice its largest extent), and the smallest probed cell whose splat count is at
+        most target is taken.  The count is not monotone in the cell size on a fixed grid, so the result is at most
+        target, not the nearest count to it (when no probe reaches target, the largest cell is taken).  The entity keeps
+        its place in the table as with crop(): its range shrinks and the entities behind it move down.  Returns the
+        splats it kept."""
+        if (cell is None) == (target is None):
+            raise ValueError("SplatScene.simplify: pass exactly one of cell= and target=")
+        first, count = self._range[id(component)]
+        if cell is None:
+            cell = simplify_cell_for(self.renderer, first, count, int(target))
+            if cell is None:
+                return count
+        kept = int(self.renderer.simplify([(first, count, float(cell))])[0]["cells"])
         self._range[id(component)][1] = kept
         self._shift_after(component, kept - count)
         return kept

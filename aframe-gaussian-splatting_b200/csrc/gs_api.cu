@@ -714,9 +714,15 @@ extern "C" int gs_erase(gs_context *c, uint32_t first, uint32_t count) {
 // push_stream after the drain.  drop: the removed-row bits (NULL: t's boxes decide).  Passes 1-2 count what each range
 // keeps; the counts come back to the host, which sizes the temporary (the failure point that leaves the table unchanged)
 // and stops there when nothing is removed; pass 3 compacts the rows behind the first removed one.  kept[j]: the rows
-// range j kept; removed: the rows removed.  The caller shrinks c->n.
+// range j kept; removed: the rows removed.  The caller shrinks c->n.  merge (gs_simplify, else NULL): its merged rows,
+// packed into their head rows once the compaction's temporary is allocated, before pass 3 moves them.
+struct MergedRows {
+  const uint4 *rows, *sh;
+  const uint32_t *head;
+  uint32_t n;
+};
 static cudaError_t compact_ranges(gs_context *c, const CropTable &t, const uint32_t *drop, std::vector<uint32_t> &kept,
-                                  uint32_t &removed) {
+                                  uint32_t &removed, const MergedRows *merge = nullptr) {
   uint32_t r0 = 0xFFFFFFFFu;
   removed = 0;
   const uint32_t lo = t.n ? t.r[0].first : 0u, n = c->n;
@@ -757,6 +763,7 @@ static cudaError_t compact_ranges(gs_context *c, const CropTable &t, const uint3
         tmp = nullptr;
       }
       if (!e) {
+        if (merge) launch_pack_at(c, merge->rows, merge->sh, merge->head, merge->n, st);
         launch_crop_write(c, s, lo, r0, n, moved, tmp, st);
         e = cudaGetLastError();
       }
@@ -921,6 +928,117 @@ extern "C" int gs_remove_outliers(gs_context *c, const uint32_t *ranges, uint32_
     for (uint32_t i = 0; i < n_ranges; ++i) outlier_stats_of(nullptr, 0, out[i]);  // empty ranges: 0 rows, NaN stats
   for (size_t j = 0; j < idx.size() && out; ++j) outlier_stats_of(&t.r[j], t.r[j].count, out[idx[j]]);
   GS_CUDA(c, cudaEventRecord(c->push_done, st));
+  c->n -= removed;
+  c->pushed = true;
+  c->have_order = false;
+  return GS_OK;
+}
+
+// gs_simplify_cells / gs_simplify (gs_simplify.cu): the arguments are checked and the non-empty ranges sorted by first
+// row before anything runs, so a refusal changes nothing.  idx: the caller's index of each range of t.
+static int simplify_table(gs_context *c, const char *who, const gs_simplify_range *ranges, uint32_t n_ranges, SimplifyTable &t,
+                          std::vector<uint32_t> &idx) {
+  auto refuse = [&](const char *why) { return fail(c, GS_ERR_INVALID, (std::string(who) + ": " + why).c_str()); };
+  if (!ranges || n_ranges == 0 || n_ranges > (uint32_t)GS_MAX_OBJECTS) return refuse("between 1 and GS_MAX_OBJECTS ranges");
+  for (uint32_t i = 0; i < n_ranges; ++i) {
+    if ((uint64_t)ranges[i].first + ranges[i].count > c->n) return refuse("a range runs past the resident splats");
+    if (!std::isfinite(ranges[i].cell) || !(ranges[i].cell > 0.0)) return refuse("a cell size is not finite and > 0");
+    if (ranges[i].count) idx.push_back(i);
+  }
+  std::sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return ranges[a].first < ranges[b].first; });
+  for (size_t j = 1; j < idx.size(); ++j)
+    if ((uint64_t)ranges[idx[j - 1]].first + ranges[idx[j - 1]].count > ranges[idx[j]].first) return refuse("ranges overlap");
+  memset(&t, 0, sizeof(t));
+  t.ot.n = (uint32_t)idx.size();
+  for (size_t j = 0; j < idx.size(); ++j) {
+    t.ot.r[j].first = ranges[idx[j]].first;
+    t.ot.r[j].count = ranges[idx[j]].count;
+    t.ot.r[j].pos = t.ot.rows;
+    t.ot.rows += t.ot.r[j].count;
+    t.cell[j] = ranges[idx[j]].cell;
+  }
+  return GS_OK;
+}
+
+// Runs the call's passes in one temporary (edit: with the merged rows and removed-row bits, then the compaction), and
+// fills out (n_ranges entries).  *removed: the rows the compaction removed.
+static int simplify_call(gs_context *c, const char *who, const gs_simplify_range *ranges, uint32_t n_ranges, bool edit,
+                         gs_simplify_stats *out, uint32_t &removed) {
+  SimplifyTable t;
+  std::vector<uint32_t> idx;
+  int rc = simplify_table(c, who, ranges, n_ranges, t, idx);
+  if (rc) return rc;
+  if (!edit && !out) return fail(c, GS_ERR_INVALID, "gs_simplify_cells: out is NULL");
+  GS_CUDA(c, cudaSetDevice(c->device));
+  if (edit && (rc = drain(c))) return rc;  // frames in flight read the table (as for gs_crop)
+  cudaStream_t st = c->push_stream;
+  removed = 0;
+  std::vector<float> lo_hi(6 * kMaxObjects, std::numeric_limits<float>::quiet_NaN());
+  std::vector<uint32_t> count(4 * kMaxObjects, 0u);
+  int refused = -1;
+  if (t.ot.n) {
+    const uint32_t w = c->sh ? c->sh_vecs : 0u;
+    void *tmp = nullptr;
+    cudaError_t e = cudaMallocAsync(&tmp, simplify_tmp_bytes(t, c->n, w, edit), st);
+    if (e) {
+      cudaGetLastError();  // an allocation failure is not sticky
+      GS_CUDA(c, e);
+    }
+    const SimplifyScratch s = simplify_scratch(tmp, t, c->n, w, edit);
+    uint32_t merged = 0;
+    e = simplify_run(c, t, s, edit, st, &refused, lo_hi.data(), count.data(), &merged);
+    if (edit && !e && refused < 0 && merged) {
+      CropTable ct;
+      memset(&ct, 0, sizeof(ct));
+      ct.n = t.ot.n;
+      for (uint32_t j = 0; j < t.ot.n; ++j) {
+        ct.r[j].first = t.ot.r[j].first;
+        ct.r[j].end = t.ot.r[j].first + t.ot.r[j].count;
+      }
+      std::vector<uint32_t> kept(kMaxObjects, 0u);
+      const MergedRows m{s.mrows, s.msh, s.mhead, merged};
+      e = compact_ranges(c, ct, s.drop, kept, removed, &m);
+    }
+    cudaFreeAsync(tmp, st);
+    GS_CUDA(c, e);
+  }
+  if (refused >= 0) return fail(c, GS_ERR_INVALID, (std::string(who) + ": a cell is too small for its range's box").c_str());
+  if (out) {
+    for (uint32_t i = 0; i < n_ranges; ++i) {  // empty ranges: no rows, an empty box
+      memset(&out[i], 0, sizeof(gs_simplify_stats));
+      for (int a = 0; a < 3; ++a) out[i].lo[a] = out[i].hi[a] = std::numeric_limits<float>::quiet_NaN();
+    }
+    for (size_t j = 0; j < idx.size(); ++j) {
+      gs_simplify_stats &o = out[idx[j]];
+      o.rows = t.ot.r[j].count;
+      o.mergeable = count[kSpMergeable * kMaxObjects + j];
+      o.cells = (o.rows - o.mergeable) + count[kSpCells * kMaxObjects + j];
+      o.merged = count[kSpMerged * kMaxObjects + j];
+      o.largest = count[kSpLargest * kMaxObjects + j];
+      for (int a = 0; a < 3; ++a) {
+        o.lo[a] = lo_hi[6 * j + a];
+        o.hi[a] = lo_hi[6 * j + 3 + a];
+      }
+    }
+  }
+  return GS_OK;
+}
+
+// read only: behind the queued pushes and edits on push_stream, without waiting for frames in flight, as gs_export
+extern "C" int gs_simplify_cells(gs_context *c, const gs_simplify_range *ranges, uint32_t n_ranges, gs_simplify_stats *out) {
+  if (!c) return GS_ERR_INVALID;
+  uint32_t removed = 0;
+  return simplify_call(c, "gs_simplify_cells", ranges, n_ranges, false, out, removed);
+}
+
+// the cells of every range, the merged rows, then one compaction (compact_ranges) with the removed-row bits as its
+// verdict; the merged rows are packed into their heads between its allocation and its write
+extern "C" int gs_simplify(gs_context *c, const gs_simplify_range *ranges, uint32_t n_ranges, gs_simplify_stats *out) {
+  if (!c) return GS_ERR_INVALID;
+  uint32_t removed = 0;
+  const int rc = simplify_call(c, "gs_simplify", ranges, n_ranges, true, out, removed);
+  if (rc) return rc;
+  GS_CUDA(c, cudaEventRecord(c->push_done, c->push_stream));
   c->n -= removed;
   c->pushed = true;
   c->have_order = false;

@@ -6,6 +6,7 @@
 // (__fmaf_rn) where the parity definition calls for them or where they are rounding-neutral
 // accumulations inside the stated tolerance.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
@@ -719,6 +720,120 @@ size_t outlier_tmp_bytes(const OutlierTable &t, uint32_t n_table, bool drop, boo
 OutlierScratch outlier_scratch(void *tmp, const OutlierTable &t, uint32_t n_table, bool drop, bool out);
 // scores, stats and verdict of every range of t on st; t's layout fields and results are filled in
 cudaError_t outlier_run(gs_context *c, OutlierTable &t, const OutlierScratch &s, cudaStream_t st);
+// k_outlier_bounds over the ranges of tab (device; n, rows, first, pos set) into bound, initialised here: per range 6
+// ordered box words (ol_dec), then at kMaxObjects * 6 its finite centres; kMaxObjects * 8 words in all
+cudaError_t outlier_bounds(gs_context *c, const OutlierTable *tab, uint32_t rows, uint32_t *bound, cudaStream_t st);
+// the stable ascending order of n 64-bit keys (klo | khi << 32): launch_ply_sort of the low words, the high words gathered
+// through that order into klo (clobbered), launch_ply_sort again.  perm: 3n words; the order is j -> (*p_lo)[p_hi[j]]
+// with p_hi returned.  table, totals as launch_ply_sort's.
+uint32_t *launch_key64_sort(gs_context *c, uint32_t *klo, const uint32_t *khi, uint32_t *perm, uint32_t *table,
+                            uint32_t *totals, uint32_t n, cudaStream_t st, uint32_t **p_lo);
+// the range keys' helpers (gs_outlier.cu, gs_simplify.cu)
+__device__ __forceinline__ float ol_dec(uint32_t e) { return __uint_as_float((e & 0x80000000u) ? (e & 0x7FFFFFFFu) : ~e); }
+__device__ __forceinline__ bool ol_finite(const float4 &c) { return isfinite(c.x) && isfinite(c.y) && isfinite(c.z); }
+// last i < n with a[i] <= v (a ascending, a[0] <= v)
+__device__ __forceinline__ uint32_t ol_find(const uint32_t *a, uint32_t n, uint32_t v) {
+  uint32_t lo = 0, hi = n;  // first i with a[i] > v
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (a[mid] <= v) lo = mid + 1; else hi = mid;
+  }
+  return lo - 1;
+}
+// 19 low bits of v spread to every third bit
+__device__ __forceinline__ uint64_t ol_spread(uint64_t v) {
+  v &= 0x7FFFFull;
+  v = (v | (v << 32)) & 0x001F00000000FFFFull;
+  v = (v | (v << 16)) & 0x001F0000FF0000FFull;
+  v = (v | (v << 8)) & 0x100F00F00F00F00Full;
+  v = (v | (v << 4)) & 0x10C30C30C30C30C3ull;
+  v = (v | (v << 2)) & 0x1249249249249249ull;
+  return v;
+}
+// (rank << 57) | Morton code: ranks below 64 leave bit 63 clear, so no key of a range row equals ~0
+static_assert(kMaxObjects <= 64, "range ranks take 6 bits of the 64-bit keys");
+// Uint8ClampedArray's store (gs_ply.cu js_store_u8_clamped): NaN and <= 0 to 0, >= 255 to 255, else round half to even
+__device__ __forceinline__ uint32_t u8_clamped(double v) {
+  if (!(v > 0.0)) return 0u;
+  if (v >= 255.0) return 255u;
+  return (uint32_t)rint(v);
+}
+// fp16 bits of v, rounded to nearest even; NaN as 0x7FFF (the loader's)
+__device__ __forceinline__ uint32_t half_bits(double v) {
+  return isnan(v) ? 0x7FFFu : (uint32_t)__half_as_ushort(__double2half(v));
+}
+// three.js Quaternion.setFromRotationMatrix of row-major m (w, x, y, z), then Quaternion.normalize (gs_export_parts'
+// placement, gs_simplify's merged axes)
+__host__ __device__ inline void quat_from_matrix(const double m[9], double q[4]) {
+  const double m11 = m[0], m12 = m[1], m13 = m[2], m21 = m[3], m22 = m[4], m23 = m[5], m31 = m[6], m32 = m[7], m33 = m[8];
+  const double trace = (m11 + m22) + m33;
+  double w, x, y, z;
+  if (trace > 0.0) {
+    const double s = 0.5 / sqrt(trace + 1.0);
+    w = 0.25 / s;
+    x = (m32 - m23) * s;
+    y = (m13 - m31) * s;
+    z = (m21 - m12) * s;
+  } else if (m11 > m22 && m11 > m33) {
+    const double s = 2.0 * sqrt(((1.0 + m11) - m22) - m33);
+    w = (m32 - m23) / s;
+    x = 0.25 * s;
+    y = (m12 + m21) / s;
+    z = (m13 + m31) / s;
+  } else if (m22 > m33) {
+    const double s = 2.0 * sqrt(((1.0 + m22) - m11) - m33);
+    w = (m13 - m31) / s;
+    x = (m12 + m21) / s;
+    y = 0.25 * s;
+    z = (m23 + m32) / s;
+  } else {
+    const double s = 2.0 * sqrt(((1.0 + m33) - m11) - m22);
+    w = (m21 - m12) / s;
+    x = (m13 + m31) / s;
+    y = (m23 + m32) / s;
+    z = 0.25 * s;
+  }
+  const double len = sqrt(((x * x + y * y) + z * z) + w * w);
+  if (len == 0.0) {
+    q[0] = 1.0;
+    q[1] = q[2] = q[3] = 0.0;
+    return;
+  }
+  const double inv = 1.0 / len;
+  q[0] = w * inv;
+  q[1] = x * inv;
+  q[2] = y * inv;
+  q[3] = z * inv;
+}
+// gs_simplify_cells / gs_simplify (gs_simplify.cu): the ranges of one call, sorted by first, and its scratch
+struct SimplifyTable {
+  OutlierTable ot;           // n, rows and each range's first, count, pos (the bounds pass reads them)
+  double cell[kMaxObjects];  // each range's cell size h
+};
+enum { kSpMergeable = 0, kSpCells = 1, kSpMerged = 2, kSpLargest = 3 };  // per-range counts, kMaxObjects words each
+struct SimplifyScratch {
+  SimplifyTable *tab;
+  uint32_t *bound;          // outlier_bounds' words
+  uint32_t *count;          // 4 kMaxObjects per-range counts (kSp*), then the merged cells' counter
+  unsigned long long *key;  // R: each range row's key ((rank << 57) | Morton of its cell; ~0: not mergeable)
+  uint32_t *klo, *khi;      // R each: the key halves; after the sort klo holds the range row at each sorted place
+  uint32_t *perm;           // 3R: the sort's permutations
+  uint2 *cells;             // R / 2: each merged cell's first sorted place and members (in no fixed order)
+  uint4 *mrows, *msh;       // R / 2 merged .splat rows (2 words each) and SH rows (sh_vecs words each): gs_simplify
+  uint32_t *mhead;          // R / 2: each merged row's head (its table row)
+  uint32_t *radix_table, *radix_totals;
+  uint32_t *drop;           // removed-row bits by table row (gs_simplify), else NULL
+  uint32_t n_drop_words;
+};
+size_t simplify_tmp_bytes(const SimplifyTable &t, uint32_t n_table, uint32_t sh_vecs, bool edit);
+SimplifyScratch simplify_scratch(void *tmp, const SimplifyTable &t, uint32_t n_table, uint32_t sh_vecs, bool edit);
+// The bounds pass, then (when every range passes the 2^19 rule; else *refused = its rank and nothing more runs) keys,
+// sort, cell heads and counts, and for an edit the merged rows.  lo_hi: 6 floats per range; count: 4 words per range
+// (kSp*); *merged_cells: the cells of two members or more.
+cudaError_t simplify_run(gs_context *c, const SimplifyTable &t, const SimplifyScratch &s, bool edit, cudaStream_t st,
+                         int *refused, float *lo_hi, uint32_t *count, uint32_t *merged_cells);
+// gs_simplify: pack_row of n merged .splat rows into the table rows head[i], with their SH rows and kept rows
+void launch_pack_at(gs_context *c, const uint4 *rows, const uint4 *sh, const uint32_t *head, uint32_t n, cudaStream_t st);
 // gs_export (gs_export.cu): rows [first, first + n) of the kept .splat rows (and their SH rows on an SH context, sh_k
 // coefficients per channel) restated as INRIA PLY vertices into body (n (14 + 3 sh_k) floats), or quantised as a
 // compressed PLY body: ceil(n / 256) chunk rows of 18 floats, n 16 B vertex words, n 3 sh_k SH bytes

@@ -3,8 +3,9 @@
 //   k_outlier_bounds : per range, the box of its finite centres (exact f32 min / max as ordered words) and their count m
 //   k_outlier_keys   : per range row, a 63-bit key: the range's rank above a 57-bit Morton code (19 bits per axis) within
 //                      the range's box; a non-finite centre takes ~0, behind every range
-//   launch_ply_sort  : the low 32 key bits, stably (gs_sort.cu); k_outlier_hi gathers the high words through that
-//                      permutation; launch_ply_sort again: the composed order is the 64-bit key order
+//   launch_key64_sort: launch_ply_sort of the low 32 key bits, stably (gs_sort.cu); k_outlier_hi gathers the high words
+//                      through that permutation; launch_ply_sort again: the composed order is the 64-bit key order
+//                      (gs_simplify.cu sorts its cell keys with it too, and reuses k_outlier_bounds through outlier_bounds)
 //   k_outlier_gather : the centres in that order (16 B: x, y, z, table row), each range's scored rows contiguous
 //   k_outlier_leaves : one warp per leaf of 32 sorted rows (each range starts a fresh leaf): the tight f32 box
 //   k_outlier_nodes  : one thread per node of the next level: the box of its (up to 32) children, one launch per level
@@ -34,19 +35,6 @@ constexpr int kOlStack = 32 * kOutlierMaxLevels;  // a walk holds at most 31 sib
 __device__ __forceinline__ uint32_t ol_enc(float f) {
   const uint32_t u = __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float ol_dec(uint32_t e) { return __uint_as_float((e & 0x80000000u) ? (e & 0x7FFFFFFFu) : ~e); }
-
-__device__ __forceinline__ bool ol_finite(const float4 &c) { return isfinite(c.x) && isfinite(c.y) && isfinite(c.z); }
-
-// last i < n with a[i] <= v (a ascending, a[0] <= v)
-__device__ __forceinline__ uint32_t ol_find(const uint32_t *a, uint32_t n, uint32_t v) {
-  uint32_t lo = 0, hi = n;  // first i with a[i] > v
-  while (lo < hi) {
-    const uint32_t mid = (lo + hi) >> 1;
-    if (a[mid] <= v) lo = mid + 1; else hi = mid;
-  }
-  return lo - 1;
 }
 
 // s of the header's distance rule: every operation rounded in fp64, (dx dx + dy dy) + dz dz
@@ -90,16 +78,6 @@ __global__ void __launch_bounds__(kOlThreads) k_outlier_bounds(const float4 *__r
   }
 }
 
-// 19 low bits of v spread to every third bit
-__device__ __forceinline__ uint64_t ol_spread(uint64_t v) {
-  v &= 0x7FFFFull;
-  v = (v | (v << 32)) & 0x001F00000000FFFFull;
-  v = (v | (v << 16)) & 0x001F0000FF0000FFull;
-  v = (v | (v << 8)) & 0x100F00F00F00F00Full;
-  v = (v | (v << 4)) & 0x10C30C30C30C30C3ull;
-  v = (v | (v << 2)) & 0x1249249249249249ull;
-  return v;
-}
 // the cell of x in [lo, lo + ext] (19 bits); only the order of the rows depends on it, never a score
 __device__ __forceinline__ uint64_t ol_cell(float x, double lo, double scale) {
   const double t = __dmul_rn(__dsub_rn((double)x, lo), scale);
@@ -449,22 +427,35 @@ static int ol_grid(gs_context *c, size_t items, int per_block) {
   return (int)std::max<size_t>(1, std::min(b, cap));
 }
 
+cudaError_t outlier_bounds(gs_context *c, const OutlierTable *tab, uint32_t rows, uint32_t *bound, cudaStream_t st) {
+  // each range's box words (min 0xFFFFFFFF, max 0), then its finite centres, then 64 words the callers count in (0)
+  std::vector<uint32_t> init(kMaxObjects * 8, 0u);
+  for (int r = 0; r < kMaxObjects; ++r)
+    for (int a = 0; a < 3; ++a) init[r * 6 + a] = 0xFFFFFFFFu;
+  cudaError_t e = cudaMemcpyAsync(bound, init.data(), sizeof(uint32_t) * init.size(), cudaMemcpyHostToDevice, st);
+  if (e) return e;
+  k_outlier_bounds<<<ol_grid(c, rows, kOlThreads * 4), kOlThreads, 0, st>>>(c->center_scale, tab, bound);
+  return cudaGetLastError();  // a copy from pageable memory has staged init before it returns
+}
+
+uint32_t *launch_key64_sort(gs_context *c, uint32_t *klo, const uint32_t *khi, uint32_t *perm, uint32_t *table,
+                            uint32_t *totals, uint32_t n, cudaStream_t st, uint32_t **p_lo) {
+  uint32_t *t1 = perm, *t2 = perm + n, *t3 = perm + 2 * (size_t)n;
+  *p_lo = launch_ply_sort(c, klo, t1, t2, table, totals, n, st);  // == t2
+  k_outlier_hi<<<ol_grid(c, n, kOlThreads * 4), kOlThreads, 0, st>>>(khi, *p_lo, klo, n);
+  return launch_ply_sort(c, klo, t1, t3, table, totals, n, st);  // == t3
+}
+
 // Scores every range of t (ranges by first row, count > 0; n, k, std_ratio, first, count, pos, rows set) on st, then the
 // verdict.  Reads m back after the bounds pass (the layout of the sorted rows and of the hierarchy is planned on the
 // host), and at the end the stats and removed counts into t.  s.out (if any) then holds the scores by range row position.
 cudaError_t outlier_run(gs_context *c, OutlierTable &t, const OutlierScratch &s, cudaStream_t st) {
   const uint32_t R = t.rows;
-  // bound: each range's box words (min 0xFFFFFFFF, max 0), then its scored rows, then its removed rows (0)
-  std::vector<uint32_t> init(kMaxObjects * 8, 0u);
-  for (int r = 0; r < kMaxObjects; ++r)
-    for (int a = 0; a < 3; ++a) init[r * 6 + a] = 0xFFFFFFFFu;
   cudaError_t e = cudaMemcpyAsync(s.tab, &t, sizeof(OutlierTable), cudaMemcpyHostToDevice, st);
-  if (!e) e = cudaMemcpyAsync(s.bound, init.data(), sizeof(uint32_t) * init.size(), cudaMemcpyHostToDevice, st);
   if (s.drop && !e) e = cudaMemsetAsync(s.drop, 0, sizeof(uint32_t) * (size_t)s.n_drop_words, st);
-  if (e) return e;
-  k_outlier_bounds<<<ol_grid(c, R, kOlThreads * 4), kOlThreads, 0, st>>>(c->center_scale, s.tab, s.bound);
+  if (!e) e = outlier_bounds(c, s.tab, R, s.bound, st);
   uint32_t m[kMaxObjects];
-  if (!(e = cudaGetLastError())) e = cudaMemcpyAsync(m, s.bound + kMaxObjects * 6, sizeof(m), cudaMemcpyDeviceToHost, st);
+  if (!e) e = cudaMemcpyAsync(m, s.bound + kMaxObjects * 6, sizeof(m), cudaMemcpyDeviceToHost, st);
   if (!e) e = cudaStreamSynchronize(st);
   if (e) return e;
   // the sorted layout: each range's scored rows from `sorted` on; leaves and inner nodes of the judged ranges
@@ -510,11 +501,9 @@ cudaError_t outlier_run(gs_context *c, OutlierTable &t, const OutlierScratch &s,
   e = cudaMemcpyAsync(s.tab, &t, sizeof(OutlierTable), cudaMemcpyHostToDevice, st);
   if (!e && !child.empty()) e = cudaMemcpyAsync(s.child, child.data(), sizeof(uint2) * child.size(), cudaMemcpyHostToDevice, st);
   if (e) return e;
-  uint32_t *klo = s.key, *khi = s.key + R, *t1 = s.perm, *t2 = s.perm + R, *t3 = s.perm + 2 * (size_t)R;
+  uint32_t *klo = s.key, *khi = s.key + R, *p_lo = nullptr;
   k_outlier_keys<<<ol_grid(c, R, kOlThreads * 4), kOlThreads, 0, st>>>(c->center_scale, s.tab, s.bound, klo, khi);
-  uint32_t *p_lo = launch_ply_sort(c, klo, t1, t2, s.radix_table, s.radix_totals, R, st);  // == t2
-  k_outlier_hi<<<ol_grid(c, R, kOlThreads * 4), kOlThreads, 0, st>>>(khi, p_lo, klo, R);
-  uint32_t *p_hi = launch_ply_sort(c, klo, t1, t3, s.radix_table, s.radix_totals, R, st);  // == t3
+  uint32_t *p_hi = launch_key64_sort(c, klo, khi, s.perm, s.radix_table, s.radix_totals, R, st, &p_lo);
   k_outlier_gather<<<ol_grid(c, R, kOlThreads * 4), kOlThreads, 0, st>>>(c->center_scale, s.tab, p_lo, p_hi, s.pts);
   if (leaves) {
     k_outlier_leaves<<<ol_grid(c, (size_t)leaves * 32, kOlThreads), kOlThreads, 0, st>>>(s.tab, s.pts, s.node);

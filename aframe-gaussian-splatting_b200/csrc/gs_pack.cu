@@ -146,6 +146,30 @@ __global__ void __launch_bounds__(256) k_pack_perm(const uint4 *__restrict__ row
   pack_row(a, b, (size_t)first + j, cs, cc, sa, tab, nt);
 }
 
+// gs_simplify: merged row i (a .splat row, and its SH row) into table row head[i], packed as any loaded row; on a
+// keep-rows context the row is kept there too
+__global__ void __launch_bounds__(256) k_pack_at(const uint4 *__restrict__ rows, const uint4 *__restrict__ sh_rows,
+                                                 const uint32_t *__restrict__ head, uint32_t n, float4 *__restrict__ cs,
+                                                 uint4 *__restrict__ cc, float *__restrict__ sa, const double *__restrict__ tab,
+                                                 int nt, uint4 *__restrict__ keep, uint4 *__restrict__ sh, uint32_t sh_vecs) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const size_t o = __ldg(head + i);
+  const uint4 a = __ldg(rows + 2 * (size_t)i), b = __ldg(rows + 2 * (size_t)i + 1);
+  for (uint32_t v = 0; v < sh_vecs; ++v) sh[o * sh_vecs + v] = __ldg(sh_rows + (size_t)i * sh_vecs + v);
+  if (keep) {
+    keep[2 * o] = a;
+    keep[2 * o + 1] = b;
+  }
+  pack_row(a, b, o, cs, cc, sa, tab, nt);
+}
+
+void launch_pack_at(gs_context *c, const uint4 *rows, const uint4 *sh, const uint32_t *head, uint32_t n, cudaStream_t st) {
+  if (!n) return;
+  k_pack_at<<<(n + 255) / 256, 256, 0, st>>>(rows, sh, head, n, c->center_scale, c->cov_color, c->size_alpha, c->quirk_table,
+                                             c->quirk_n, c->keep, c->sh, c->sh ? c->sh_vecs : 0u);
+}
+
 // Table edit (gs_insert_*, gs_erase): copy n rows of the table arrays from src to dst, one row per thread.  The two
 // ranges never overlap within one launch (an overlapping move goes through a temporary, launch_move_rows), so the
 // accesses are restrict.  The 16 B records (and an SH context's sh_vecs words of coefficients, and the two words of a

@@ -105,49 +105,6 @@ bool sh_rotation(const double q9[9], uint32_t degree, double *out) {
   return true;
 }
 
-// three.js Quaternion.setFromRotationMatrix of row-major m (w, x, y, z), then Quaternion.normalize
-static void quat_from_matrix(const double m[9], double q[4]) {
-  const double m11 = m[0], m12 = m[1], m13 = m[2], m21 = m[3], m22 = m[4], m23 = m[5], m31 = m[6], m32 = m[7], m33 = m[8];
-  const double trace = (m11 + m22) + m33;
-  double w, x, y, z;
-  if (trace > 0.0) {
-    const double s = 0.5 / std::sqrt(trace + 1.0);
-    w = 0.25 / s;
-    x = (m32 - m23) * s;
-    y = (m13 - m31) * s;
-    z = (m21 - m12) * s;
-  } else if (m11 > m22 && m11 > m33) {
-    const double s = 2.0 * std::sqrt(((1.0 + m11) - m22) - m33);
-    w = (m32 - m23) / s;
-    x = 0.25 * s;
-    y = (m12 + m21) / s;
-    z = (m13 + m31) / s;
-  } else if (m22 > m33) {
-    const double s = 2.0 * std::sqrt(((1.0 + m22) - m11) - m33);
-    w = (m13 - m31) / s;
-    x = (m12 + m21) / s;
-    y = 0.25 * s;
-    z = (m23 + m32) / s;
-  } else {
-    const double s = 2.0 * std::sqrt(((1.0 + m33) - m11) - m22);
-    w = (m21 - m12) / s;
-    x = (m13 + m31) / s;
-    y = (m23 + m32) / s;
-    z = 0.25 * s;
-  }
-  const double len = std::sqrt(((x * x + y * y) + z * z) + w * w);
-  if (len == 0.0) {
-    q[0] = 1.0;
-    q[1] = q[2] = q[3] = 0.0;
-    return;
-  }
-  const double inv = 1.0 / len;
-  q[0] = w * inv;
-  q[1] = x * inv;
-  q[2] = y * inv;
-  q[3] = z * inv;
-}
-
 static double det3(const double a[9]) {
   return (a[0] * (a[4] * a[8] - a[5] * a[7]) - a[1] * (a[3] * a[8] - a[5] * a[6])) + a[2] * (a[3] * a[7] - a[4] * a[6]);
 }
@@ -197,13 +154,6 @@ __device__ __forceinline__ uint32_t f32_bits_or_nan(double v) {
   return isnan(v) ? kNaN32t : __float_as_uint(__double2float_rn(v));
 }
 
-// Uint8ClampedArray's store (gs_ply.cu js_store_u8_clamped): NaN and <= 0 to 0, >= 255 to 255, else round half to even
-__device__ __forceinline__ uint32_t u8_clamped(double v) {
-  if (!(v > 0.0)) return 0u;
-  if (v >= 255.0) return 255u;
-  return (uint32_t)rint(v);
-}
-
 // rotation bytes (w, x, y, z) of qQ (x) q^, q^ the row's normalised quaternion
 __device__ __forceinline__ uint32_t rotate_bytes(uint32_t rot, const double q[4]) {
   double w = ((double)(rot & 255u) - 128.0) / 128.0, x = ((double)((rot >> 8) & 255u) - 128.0) / 128.0;
@@ -219,10 +169,6 @@ __device__ __forceinline__ uint32_t rotate_bytes(uint32_t rot, const double q[4]
   const double rz = ((q[0] * z + q[1] * y) - q[2] * x) + q[3] * w;
   return u8_clamped(rw * 128.0 + 128.0) | (u8_clamped(rx * 128.0 + 128.0) << 8) | (u8_clamped(ry * 128.0 + 128.0) << 16) |
          (u8_clamped(rz * 128.0 + 128.0) << 24);
-}
-
-__device__ __forceinline__ uint32_t half_bits(double v) {
-  return isnan(v) ? 0x7FFFu : (uint32_t)__half_as_ushort(__double2half(v));
 }
 
 template <uint32_t K>

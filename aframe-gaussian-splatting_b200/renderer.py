@@ -214,6 +214,26 @@ class SplatContext:
         self._check(self._lib.gs_remove_outliers(self._h, arr, len(ranges), int(k), float(std_ratio), out))
         return [out[i].as_dict() for i in range(len(ranges))]
 
+    def _simplify(self, fn, ranges) -> list:
+        arr = (_lib.GsSimplifyRange * max(len(ranges), 1))()
+        for i, (first, count, cell) in enumerate(ranges):
+            arr[i].first, arr[i].count, arr[i].cell = int(first), int(count), float(cell)
+        out = (_lib.GsSimplifyStats * max(len(ranges), 1))()
+        self._check(fn(self._h, arr, len(ranges), out))
+        return [out[i].as_dict() for i in range(len(ranges))]
+
+    def simplify_cells(self, first: int, count: int, cell: float) -> dict:
+        """gs_simplify_cells: what simplify([(first, count, cell)]) would do, read only: a dict of rows, mergeable,
+        cells (the rows after), merged (cells of two rows or more), largest (rows of the largest cell) and the box
+        (lo, hi) of the range's finite centres."""
+        return self._simplify(self._lib.gs_simplify_cells, [(first, count, cell)])[0]
+
+    def simplify(self, ranges) -> list:
+        """gs_simplify: merge the rows of each grid cell of every (first, count, cell) range into one moment-matched
+        row (include/gsplat_b200.h, "Simplifying entities"), compacting the table in place as crop() does.  Returns one
+        stats dict per range (simplify_cells' keys)."""
+        return self._simplify(self._lib.gs_simplify, ranges)
+
     def push_packed(self, center_scale: np.ndarray, cov_color: np.ndarray, size_alpha: np.ndarray) -> None:
         cs = np.ascontiguousarray(center_scale, dtype=np.float32).reshape(-1, 4)
         cc = np.ascontiguousarray(cov_color, dtype=np.uint32).reshape(-1, 4)

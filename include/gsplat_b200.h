@@ -373,6 +373,78 @@ GS_API int gs_remove_outliers(gs_context *ctx, const uint32_t *ranges /* (first,
                               uint32_t k, double std_ratio, gs_outlier_stats *out_or_null /* n_ranges entries */);
 
 /*
+ * Simplifying entities: merge the splats of each grid cell of an entity range into one moment-matched splat, on the
+ * device.  A level of detail for far entities, phones or XR eyes, or a lighter file to save: merging keeps the coverage
+ * where erasing splats leaves holes.  The definition, exact to the bit (every operation one fp64 +, -, *, / or sqrt,
+ * rounded once: __dadd_rn / __dsub_rn / __dmul_rn / __ddiv_rn / __dsqrt_rn, nothing contracted):
+ *   - Input.  Each range (rows [first, first+count), its own cell size h > 0 in the entity's local units) is simplified
+ *     on its own.  Row i's input is its packed record, what frames draw: c = center_scale.xyz; the table-frame
+ *     covariance S^T = each int16 word of cov_color.xyz times center_scale.w (fp64); colour and alpha bytes from
+ *     cov_color.w; its SH coefficients (fp16 -> fp64) on an SH context.  The merge runs in the .splat row frame:
+ *     p_i = (c.x, c.y, -c.z), S_i = F S^T F with F = diag(1, 1, -1) (pack_row's Sigma is R diag(s^2) R^T there).
+ *   - Mergeable rows: centre and center_scale.w finite.  Every other row stays exactly as it is.
+ *   - Cells.  lo_a / hi_a: the range's f32 min / max of c_a over its rows with a finite centre (gs_remove_outliers'
+ *     box).  cell_a = floor((c_a - lo_a) / h) (fp64 subtraction, then division).  Refused (GS_ERR_INVALID) when
+ *     floor((hi_a - lo_a) / h) >= 2^19 on any axis.  A cell's members are taken in table order; its head is the first.
+ *   - A cell of one member is left byte for byte as it is (packed record, SH row, kept row): an h smaller than every
+ *     spacing changes nothing and writes no byte.  The members after the head of each cell are removed: each range
+ *     keeps one row per cell, at its head's place, and its rows that are not mergeable, all in table order; rows outside
+ *     every range are unchanged; rows behind the first removed row move down with their SH and kept rows, as gs_crop.
+ *   - A cell of n >= 2 members.  Member i: d_i = p_i - p_head; t_i = (S00 + S11) + S22; a_i = alpha byte / 255;
+ *     w_i = a_i t_i; W = sum w_i.  omega_i = w_i if W > 0, else 1.  Omega = sum omega_i; S1 = sum omega_i d_i;
+ *     S2_ab = sum omega_i (S_i,ab + d_a d_b) (six entries); Sc = sum omega_i (rgb_i / 255); Ssh = sum omega_i sh_i.
+ *   - Summation order of every sum above: lane l (0..31) sums members l, l+32, l+64, ... in table order, from 0; then
+ *     for o = 16, 8, 4, 2, 1: v_l = v_l + v_(l xor o).  Every lane ends with the same bits.
+ *   - Moments.  m = S1 / Omega; mu = p_head + m, stored as the f32 row position.  Sigma_ab = S2_ab / Omega - m_a m_b;
+ *     t_m = (Sigma00 + Sigma11) + Sigma22.
+ *   - Alpha.  W > 0: alpha = min(1, W / t_m), 1 when t_m <= 0 (alpha x trace "coverage" is conserved: a densely tiled
+ *     opaque surface stays opaque, a sparse cell turns translucent).  W = 0: alpha = 0.  Known bias: n coincident copies
+ *     of alpha a give min(1, n a) where compositing them gives 1 - (1 - a)^n.
+ *   - Bytes.  Colour and alpha bytes: js_store_u8_clamped(x * 255) with x = Sc / Omega and alpha (NaN and <= 0 to 0,
+ *     >= 255 to 255, else round half to even).  SH coefficient: the fp16 round-to-nearest-even of Ssh / Omega (NaN
+ *     stored as 0x7FFF, as the loader does).
+ *   - Axes.  Cyclic Jacobi on Sigma from V = I: exactly 8 sweeps over the pairs (0,1), (0,2), (1,2), a pair skipped when
+ *     a_pq == 0.  Rotation (Numerical Recipes): theta = (a_qq - a_pp) / (2 a_pq); t = sign(theta) / (|theta| +
+ *     sqrt(theta^2 + 1)) (sign(0) = 1); c = 1 / sqrt(t^2 + 1); s = t c; tau = s / (1 + c); a_pp -= t a_pq;
+ *     a_qq += t a_pq; a_pq = 0; the other index r: g = a_rp, h = a_rq, a_rp = g - s (h + g tau), a_rq = h + s (g - h
+ *     tau); each row k of V the same with g = V_kp, h = V_kq.  det V = (V00 (V11 V22 - V12 V21) - V01 (V10 V22 - V12
+ *     V20)) + V02 (V10 V21 - V11 V20); when < 0, column 2 of V is negated.  scale_k = f32(sqrt(max(a_kk, 0))) in
+ *     Jacobi's diagonal order (no sort).  q = three.js setFromRotationMatrix(V) then normalize (w, x, y, z); rotation
+ *     bytes 28..31 (w, x, y, z) = js_store_u8_clamped((q_k / |q|) 128 + 128), |q| = sqrt(((w^2 + x^2) + y^2) + z^2),
+ *     as the loader stores a PLY rotation.
+ *   - The merged .splat row (mu, scales, colour and alpha bytes, rotation bytes) is packed with pack_row, so every
+ *     record is still pack_row of a row; on a keep-rows context the row is kept, on an SH context its SH row stored.
+ *   - The order the device visits cells in (a Morton sort) decides only the speed, never membership or output.
+ * gs_simplify_cells: reads only.  out: the stats gs_simplify would return for the one range.  Runs behind the queued
+ *   pushes and edits, and does not wait for frames in flight, as gs_outlier_scores.
+ * gs_simplify: merges each range of `ranges` (any order, count 0 allowed).  out (n_ranges entries, or NULL): each
+ *   range's stats.  Table-edit rules as gs_crop: the call waits for the frames in flight and runs behind queued pushes;
+ *   the draw order is stale after it; a call that merges nothing writes no byte of the table.
+ * GS_ERR_INVALID, nothing changed: ranges NULL, n_ranges 0 or above GS_MAX_OBJECTS, a range past N, overlapping ranges, a
+ *   cell that is not finite or <= 0, a cell too small for its range's box (the 2^19 rule, checked after the bounds pass
+ *   and before any write), out NULL (gs_simplify_cells).
+ * Memory: one stream-ordered temporary of about 32 B per row of the ranges (keys and their halves, sort permutations, the
+ *   merged-cell list); gs_simplify adds (36 + 16 sh_vecs) / 2 B per row for the merged rows and their heads, N / 8 bytes
+ *   of removed-row bits, and gs_crop's temporary for the rows that move.  Each is allocated before the table is written,
+ *   so GS_ERR_OOM changes nothing.
+ */
+typedef struct gs_simplify_range {
+  uint32_t first, count;  /* table rows [first, first + count)                                     */
+  double cell;            /* the cell size h, in the entity's local units: finite and > 0          */
+} gs_simplify_range;      /* 16 bytes */
+typedef struct gs_simplify_stats {
+  uint32_t rows;       /* rows of the range before the call                                           */
+  uint32_t mergeable;  /* rows with a finite centre and center_scale.w                                */
+  uint32_t cells;      /* rows of the range after the call: its cells plus its rows not mergeable     */
+  uint32_t merged;     /* cells of two members or more                                                */
+  uint32_t largest;    /* members of the largest cell (0: no mergeable row)                           */
+  uint32_t pad;
+  float lo[3], hi[3];  /* the box of the range's finite centres (NaN when there is none)              */
+} gs_simplify_stats;   /* 48 bytes */
+GS_API int gs_simplify_cells(gs_context *ctx, const gs_simplify_range *ranges, uint32_t n_ranges, gs_simplify_stats *out);
+GS_API int gs_simplify(gs_context *ctx, const gs_simplify_range *ranges, uint32_t n_ranges, gs_simplify_stats *out_or_null);
+
+/*
  * Append n already-packed splats: the two data-texture records the reference uploads
  * (centerAndScaleData float4, covAndColorData uint4, index.js:40-46,378-394) and the worker's
  * matrices[15] (max(scale)*alpha/255, index.js:397).  Host pointers.
